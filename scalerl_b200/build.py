@@ -3,6 +3,7 @@ for the wgmma building blocks; never loaded by the product path) in-tree with nv
 Usage: python -m scalerl_b200.build [--force] [-v]"""
 import concurrent.futures as cf
 import os
+import re
 import subprocess
 import sys
 
@@ -65,6 +66,38 @@ def build(force=False, verbose=False):
     if verbose:
         print('\n'.join(log))
     return OUT
+
+
+def ptxas_report(path=os.path.join(HERE, 'build', 'ptxas.log')):
+    """What ptxas -v said about every kernel of the last build: {source: {mangled kernel: {'regs', 'spill_stores',
+    'spill_loads', 'serialized'}}}.  'serialized' lists the ptxas notes that the kernel's wgmma instructions were
+    serialized (not enough registers to keep them in flight, or a wgmma on a path ptxas considers divergent)."""
+    report, src, cur = {}, None, None
+    with open(path) as f:
+        for line in f:
+            m = re.match(r'== (\S+)', line)
+            if m:
+                src = m.group(1)
+                report[src] = {}
+                continue
+            entry = lambda name: report[src].setdefault(name, {'regs': None, 'spill_stores': 0, 'spill_loads': 0, 'serialized': []})
+            m = re.search(r"\((C\d+)\)[^']*wgmma\.mma_async instructions are serialized[^']*function '(\w+)'", line)
+            if m:
+                entry(m.group(2))['serialized'].append(m.group(1))
+                continue
+            m = re.search(r'Function properties for (\w+)', line)
+            if m:
+                cur = entry(m.group(1))
+                continue
+            m = re.search(r'(\d+) bytes spill stores, (\d+) bytes spill loads', line)
+            if m and cur is not None:
+                cur['spill_stores'], cur['spill_loads'] = int(m.group(1)), int(m.group(2))
+                continue
+            m = re.search(r'Used (\d+) registers', line)
+            if m and cur is not None:
+                cur['regs'] = int(m.group(1))
+                cur = None
+    return report
 
 
 if __name__ == '__main__':

@@ -108,6 +108,13 @@ SRL_DEVINL uint32_t elect_one_sync() {
 SRL_DEVINL void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 SRL_DEVINL void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 SRL_DEVINL void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// every committed group but the newest has completed: the MMAs of the next k-block can be issued while the last one retires
+SRL_DEVINL void wg_wait_prev() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// Per-warpgroup register budgets (setmaxnreg, .sync.aligned: every warp of the warpgroup executes it).  A CTA's warps are dealt
+// round-robin to the four SM sub-partitions of 16384 registers each, so per-thread counts summed over one warp of every role
+// must stay <= 512.  The TMA producer gives registers back, the warpgroups holding wgmma accumulators take them.
+template <int N> SRL_DEVINL void reg_release() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> SRL_DEVINL void reg_claim() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 // keeps the compiler from moving accumulator reads / writes across wgmma.wait_group
 template <int N>
 SRL_DEVINL void wg_fence_regs(float (&d)[N]) {
@@ -136,8 +143,9 @@ constexpr int fit_stages(int want, int fixed, int per) {
 }
 constexpr int WG_IMG_STRIDE = 20;                        // 16 columns + 4: conflict-free 16-byte row reads
 constexpr int WG_IMG_BYTES = 2 * 128 * WG_IMG_STRIDE * 4;
+// wg_acc_rows16: the same for two separate 64 x N accumulators d0 (rows 0..63) and d1 (rows 64..127).
 template <int N, bool ONE_BUF = false>
-SRL_DEVINL void wg_acc_row16(const float (&d)[2][N / 2], int c, float* img, int wt, int bar, float (&v)[16]) {
+SRL_DEVINL void wg_acc_rows16(const float (&d0)[N / 2], const float (&d1)[N / 2], int c, float* img, int wt, int bar, float (&v)[16]) {
   float* buf = ONE_BUF ? img : img + (c & 1) * 128 * WG_IMG_STRIDE;
   if (ONE_BUF) named_bar(bar, 128);                      // the previous chunk has been read by every thread
   const int w = wt >> 5, l = wt & 31;
@@ -148,12 +156,17 @@ SRL_DEVINL void wg_acc_row16(const float (&d)[2][N / 2], int c, float* img, int 
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const int row = 64 * h + 16 * w + (l >> 2) + 8 * rr, i = 4 * (2 * c + jj) + 2 * rr;
-        *reinterpret_cast<float2*>(buf + row * WG_IMG_STRIDE + 8 * jj + 2 * (l & 3)) = make_float2(d[h][i], d[h][i + 1]);
+        const float (&d)[N / 2] = h ? d1 : d0;
+        *reinterpret_cast<float2*>(buf + row * WG_IMG_STRIDE + 8 * jj + 2 * (l & 3)) = make_float2(d[i], d[i + 1]);
       }
   named_bar(bar, 128);
   const float4* q = reinterpret_cast<const float4*>(buf + wt * WG_IMG_STRIDE);
 #pragma unroll
   for (int j = 0; j < 4; ++j) { const float4 x = q[j]; v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w; }
+}
+template <int N, bool ONE_BUF = false>
+SRL_DEVINL void wg_acc_row16(const float (&d)[2][N / 2], int c, float* img, int wt, int bar, float (&v)[16]) {
+  wg_acc_rows16<N, ONE_BUF>(d[0], d[1], c, img, wt, bar, v);
 }
 
 // ------------------------------------------------------------------------------------------

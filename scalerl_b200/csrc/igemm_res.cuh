@@ -12,20 +12,25 @@
 //
 //   res_fwd_kernel<P>   K-major, persistent: forward convs and dgrads (dgrad = negative shifts over dY stored on the
 //                       grid of the conv input with zeros outside the valid outputs, which doubles as padding).
-//                       warp 8 = TMA producer (weights once, then one window per 128-position tile, S-deep ring),
+//                       warps 8-11 = producer warpgroup: warp 8 issues the TMA loads (weights once, then one window per
+//                       128-position tile, S-deep ring), warps 9-11 only give their registers back;
 //                       warps 0-7 = two consumer warpgroups taking alternate tiles: each issues NT taps x 4 K-steps of
 //                       wgmma into its register accumulator and runs that tile's epilogue while the other warpgroup
 //                       multiplies the next tile.
 //   res_wgrad_kernel<P> MN-major: dW[tap] = sum over positions X[pos + shift_tap]^T dY[pos].  One CTA owns a contiguous
 //                       range of positions, streams (window, dY) chunks of 128 positions through a ring and keeps ALL
-//                       taps' accumulators in registers, one consumer warpgroup per accumulator (tap pairs form M = 128;
-//                       an all-ones block yields the bias gradient).
+//                       taps' accumulators in registers: each 64-row tap block is one m64 accumulator, the blocks are
+//                       spread over two or three consumer warpgroups.  A producer warpgroup issues the TMA loads and sums
+//                       the staged dY columns (bias gradient) on a small register budget (setmaxnreg); the consumers keep
+//                       one chunk's MMAs in flight while they issue the next.
 #pragma once
 #include "igemm_tma.cuh"
 
 namespace srl {
 
-constexpr int RES_THREADS = 288;      // res_fwd_kernel: two consumer warpgroups + the producer warp
+constexpr int RES_THREADS = 384;      // res_fwd_kernel: two consumer warpgroups + the producer warpgroup
+// register budgets (per thread, setmaxnreg) of res_fwd_kernel: one warp of each warpgroup per sub-partition, 40 + 2 x 232 <= 512
+constexpr int RES_PRODUCER_REGS = 40, RES_CONSUMER_REGS = 232;
 constexpr int RES_MAX_TAPS = 10;
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -85,9 +90,10 @@ __global__ void __launch_bounds__(RES_THREADS, 1) res_fwd_kernel(const __grid_co
     P::prefetch(p);
   }
   __syncthreads();
-  if (warp != 8) pdl_wait(P::KID);
 
-  if (warp == 8) {
+  if (warp >= 8) {
+    reg_release<RES_PRODUCER_REGS>();
+    if (warp != 8) return;                 // warps 9-11 only give their registers back
     const uint32_t leader = elect_one_sync();      // converged warp, one elected issuing lane: no vote loop around every TMA instruction
     // the packed weights were complete before the first kernel of the chain started: their load overlaps the previous
     // kernel's tail; the activations are only touched after pdl_wait().  (W_AFTER_WAIT: the weights come from the stream predecessor.)
@@ -115,6 +121,8 @@ __global__ void __launch_bounds__(RES_THREADS, 1) res_fwd_kernel(const __grid_co
       __syncwarp();
     }
   } else {
+    reg_claim<RES_CONSUMER_REGS>();
+    pdl_wait(P::KID);
     // consumer warpgroup g takes this CTA's tiles it = g, g + 2, ...: its epilogue overlaps the other warpgroup's MMAs.  With a
     // single input stage warpgroup 0 takes every tile: tile it + 2 would be awaited on the same barrier with the parity of the
     // phase that just completed (tile it), before tile it + 1 was even loaded.
@@ -180,40 +188,118 @@ cudaError_t res_fwd_launch(const typename P::Params& p, int ntiles, int max_ctas
 
 // ------------------------------------------------------------------------------------------------------------------
 // wgrad
-//   P: NACC accumulators (each M = 128 = two 64-row blocks, N = DY_CH), NWIN, WROWS (= 128 + max shift), STAGES,
-//      acc_win(a), acc_shift0(a), acc_shift1(a) (block 1 = -1 -> the all-ones block: bias gradient),
-//      Params{ in[NWIN] maps, dy map, P (positions), chunks_per_cta }, epilogue16(p, acc, row, c0, v)
+//   P: NBLK tap blocks (each M = 64 rows of dW = 64 window rows, N = DY_CH), CWG consumer warpgroups, NWIN, WROWS
+//      (= 128 + max shift), STAGES, blk_win(b), blk_shift(b), PART (floats per CTA slice: tap blocks [b][row][co], then
+//      BIAS_CH bias sums), Params{ in[NWIN] maps, dy map, ws, P (positions), chunks_per_cta }
 // ------------------------------------------------------------------------------------------------------------------
 template <class P, int SPLIT>
 struct ResWgradCfg {
   static constexpr int ALO = (SPLIT && P::A_LO) ? 1 : 0;          // the input window has a low tensor (not conv1: exact u8 frames)
-  static constexpr bool BIAS_SMEM = P::SMEM_BIAS || SPLIT;        // split mode: bias gradient always from the staged dY tiles
   static constexpr int WIN_BYTES = ((P::WROWS * 128 + 1023) / 1024) * 1024;
   static constexpr int DY_BYTES = 128 * P::DY_CH * 2;             // 128 positions x DY_CH channels (64: SWIZZLE_128B rows, 32: SWIZZLE_64B rows)
   static constexpr int X_HI_BYTES = P::NWIN * WIN_BYTES;
   static constexpr int X_BYTES = X_HI_BYTES * (1 + ALO);
   static constexpr int STAGE_BYTES = X_BYTES + DY_BYTES * (1 + SPLIT);     // [windows hi][windows lo][dY hi][dY lo]
-  static constexpr int ONES_BYTES = 128 * 128;
-  static constexpr int STAGES = fit_stages(SPLIT ? P::SPLIT_STAGES : P::STAGES, ONES_BYTES + P::NACC * WG_IMG_BYTES + 1024 + 256, STAGE_BYTES);
-  static constexpr int SMEM_BYTES = ONES_BYTES + STAGES * STAGE_BYTES + P::NACC * WG_IMG_BYTES + 1024 + 256;
+  // warps: [CWG consumer warpgroups] [producer warpgroup: warp 0 also issues the TMA loads; the four warps produce the bias gradient]
+  // bias gradient: column sums of the staged dY tiles, or (BIAS_MMA: conv3 in the bf16 mode) a wgmma of an all-ones block with the
+  // dY tile -- the tensor cores' sum, the bits conv3's bias gradient has always had
+  static constexpr bool BIAS_MMA = !P::SMEM_BIAS && !SPLIT;
+  static constexpr int ONES_BYTES = BIAS_MMA ? 128 * 128 : 0;
+  // consumer warpgroup w holds tap blocks w * BPW .. w * BPW + BPW - 1 (fewer in the last one)
+  static constexpr int CWG = P::CWG, BPW = (P::NBLK + CWG - 1) / CWG;
+  static constexpr int PRODUCER_WARP = 4 * CWG;
+  static constexpr int THREADS = 32 * (PRODUCER_WARP + 4);
+  // ptxas keeps wgmma accumulators within the kernel's launch register count (65536 / THREADS), not within the setmaxnreg
+  // budget: a warpgroup's accumulators must leave room there for descriptors and loop state, or every wgmma is serialized
+  static_assert(BPW * P::DY_CH / 2 + 32 <= (65536 / THREADS & ~7), "wgmma accumulators exceed the launch register count");
+  // per-thread register budgets: one warp of every warpgroup shares a sub-partition, PRODUCER + CWG x CONSUMER <= 512
+  static constexpr int PRODUCER_REGS = BIAS_MMA ? 96 : 56;      // BIAS_MMA: one m64 accumulator (32 registers) on top
+  static constexpr int CONSUMER_REGS = ((512 - PRODUCER_REGS) / CWG & ~7) < 232 ? ((512 - PRODUCER_REGS) / CWG & ~7) : 232;
+  static constexpr int BIAS_BYTES = 2048;                          // bias partial sums of the four warps + the release-ordering slots
+  static constexpr int FIXED_BYTES = ONES_BYTES + CWG * WG_IMG_BYTES + BIAS_BYTES + 1024 + 256;
+  static constexpr int STAGES = fit_stages(SPLIT ? P::SPLIT_STAGES : P::STAGES, FIXED_BYTES, STAGE_BYTES);
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;
   static_assert(SMEM_BYTES <= 232448, "shared memory budget (227 KB)");
-  // warps: [4 bias-sum warps (BIAS_SMEM)] [one consumer warpgroup per accumulator] [TMA producer warp]
-  static constexpr int BW = BIAS_SMEM ? 4 : 0;
-  static constexpr int PRODUCER_WARP = BW + 4 * P::NACC;
-  static constexpr int THREADS = 32 * (PRODUCER_WARP + 1);
 };
+
+SRL_DEVINL void store16(float* dst, const float (&v)[16]) {
+#pragma unroll
+  for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+}
+
+// consumer warpgroup W of res_wgrad_kernel: its tap blocks are a compile-time set, so no wgmma sits behind a branch
+template <class P, int SPLIT, int W>
+SRL_DEVINL void res_wgrad_consumer(const typename P::Params& p, uint8_t* sSt, float* img, uint64_t* full, uint64_t* empty, int nch, int tid) {
+  using C = ResWgradCfg<P, SPLIT>;
+  constexpr int STAGES = C::STAGES, B0 = W * C::BPW, NB = P::NBLK - B0 < C::BPW ? P::NBLK - B0 : C::BPW;
+  constexpr uint32_t DYK = P::DY_CH * 2;           // descriptor address units per K = 16 step of the dY tile (16 rows x row bytes / 16)
+  const int wt = tid & 127;
+  float acc[NB][P::DY_CH / 2];
+#pragma unroll
+  for (int b = 0; b < NB; ++b)
+#pragma unroll
+    for (int j = 0; j < P::DY_CH / 2; ++j) acc[b][j] = 0.f;
+  for (int i = 0; i < nch; ++i) {
+    const int s = i % STAGES;
+    mbar_wait(&full[s], (i / STAGES) & 1);
+    const uint32_t st = smem_u32(sSt + s * C::STAGE_BYTES);
+    const uint64_t dyd = P::DY_CH == 64 ? make_smem_desc(st + C::X_BYTES, 8192, 1024) : make_smem_desc_sw64(st + C::X_BYTES, 4096, 512);
+    wg_fence();
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      const uint64_t xd = make_smem_desc(st + P::blk_win(B0 + b) * C::WIN_BYTES + P::blk_shift(B0 + b) * 128, 8192, 1024);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {          // 128 positions = 8 x (K = 16): +2048 B per step
+        Wgmma<P::DY_CH, 1, 1>::mma(acc[b], xd + 128 * k, dyd + DYK * k, 1);
+        if constexpr (SPLIT)         // hi(x) * lo(dy)
+          Wgmma<P::DY_CH, 1, 1>::mma(acc[b], xd + 128 * k, dyd + (uint64_t)(C::DY_BYTES / 16 + DYK * k), 1);
+        if constexpr (C::ALO)        // lo(x) * hi(dy)
+          Wgmma<P::DY_CH, 1, 1>::mma(acc[b], xd + (uint64_t)(C::X_HI_BYTES / 16 + 128 * k), dyd + DYK * k, 1);
+      }
+    }
+    wg_commit();
+    if constexpr (STAGES > 1) {
+      // chunk i stays in flight while chunk i + 1 is awaited and issued; chunk i - 1's stage is released as soon as it retired
+      wg_wait_prev();
+      __syncwarp();
+      if (i > 0 && (tid & 31) == 0) mbar_arrive(&empty[(i - 1) % STAGES]);
+    } else {     // one stage: the next chunk can only be loaded once this one retired
+      wg_wait_all();
+      __syncwarp();
+      if ((tid & 31) == 0) mbar_arrive(&empty[s]);
+    }
+  }
+  wg_wait_all();
+#pragma unroll
+  for (int b = 0; b < NB; ++b) wg_fence_regs(acc[b]);
+  if (nch > 0) {
+    // tap blocks leave in pairs (thread wt: row wt & 63 of block b + wt / 64); an odd last block is paired with itself
+    float* my_img = img + W * (WG_IMG_BYTES / 4);
+    float* ws = p.ws + (size_t)blockIdx.x * P::PART;
+#pragma unroll
+    for (int b = 0; b < NB; b += 2) {
+      const int b1 = b + 1 < NB ? b + 1 : b;
+#pragma unroll
+      for (int c = 0; c < P::DY_CH / 16; ++c) {       // an even number of 16-column chunks: the hand-off buffers keep alternating
+        float v[16];
+        wg_acc_rows16<P::DY_CH>(acc[b], acc[b1], c, my_img, wt, 2 + W, v);
+        if (wt < 64 || b1 != b) store16(ws + ((size_t)(B0 + b) * 64 + wt) * P::DY_CH + c * 16, v);
+      }
+    }
+  }
+}
 
 template <class P, int SPLIT>
 __global__ void __launch_bounds__(ResWgradCfg<P, SPLIT>::THREADS, 1) res_wgrad_kernel(const __grid_constant__ typename P::Params p) {
   using C = ResWgradCfg<P, SPLIT>;
   constexpr int STAGES = C::STAGES;
-  constexpr bool BIAS_SMEM = C::BIAS_SMEM;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sSt = smem;
-  uint8_t* sOnes = smem + STAGES * C::STAGE_BYTES;     // after the stages: block-1 - block-0 distances stay positive
+  uint8_t* sOnes = smem + STAGES * C::STAGE_BYTES;              // 1024-aligned: every stage is a multiple of 1024 bytes
   float* img = reinterpret_cast<float*>(sOnes + C::ONES_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sOnes + C::ONES_BYTES + P::NACC * WG_IMG_BYTES);
+  uint8_t* sBias = sOnes + C::ONES_BYTES + C::CWG * WG_IMG_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + C::BIAS_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
   const int tid = threadIdx.x, warp = tid >> 5;
@@ -222,14 +308,14 @@ __global__ void __launch_bounds__(ResWgradCfg<P, SPLIT>::THREADS, 1) res_wgrad_k
   const int c_end = min(nchunks_total, c_begin + p.chunks_per_cta);
   const int nch = max(0, c_end - c_begin);
 
-  if constexpr (!BIAS_SMEM) {  // all-ones block (bf16 1.0) for the bias-gradient accumulator
+  if constexpr (C::BIAS_MMA) {  // all-ones block (bf16 1.0): 128 positions x 64 rows
     uint4* q = reinterpret_cast<uint4*>(sOnes);
     for (int i = tid; i < C::ONES_BYTES / 16; i += C::THREADS) q[i] = make_uint4(0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
     fence_proxy_async_smem();
   }
   if (warp == C::PRODUCER_WARP && (tid & 31) == 0) {
-    // a stage is free after every consumer warp passed its wgmma wait (and, SMEM_BIAS, the four bias warps read the dy tile)
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4 * P::NACC + (BIAS_SMEM ? 4 : 0)); }
+    // a stage is free after every consumer warp passed its wgmma wait and the four producer warps used its dY tile
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4 * C::CWG + 4); }
     mbar_fence_init();
     P::prefetch(p);
   }
@@ -237,9 +323,22 @@ __global__ void __launch_bounds__(ResWgradCfg<P, SPLIT>::THREADS, 1) res_wgrad_k
   pdl_wait(P::KID);
   if (warp == C::PRODUCER_WARP && (tid & 31) == 0) pdl_launch();
 
-  if (warp == C::PRODUCER_WARP) {
+  // each role sets its register budget inside its own branch: ptxas ignores a setmaxnreg that is followed by shared code
+  // the warpgroup index through a shuffle: ptxas then knows it is warp-uniform and does not serialize the wgmma behind the branches
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
+  if (wg < C::CWG) {
+    static_assert(C::CWG == 2 || C::CWG == 3, "two or three consumer warpgroups");
+    reg_claim<C::CONSUMER_REGS>();
+    if (wg == 0) res_wgrad_consumer<P, SPLIT, 0>(p, sSt, img, full, empty, nch, tid);
+    else if (C::CWG == 2 || wg == 1) res_wgrad_consumer<P, SPLIT, 1>(p, sSt, img, full, empty, nch, tid);
+    else if constexpr (C::CWG == 3) res_wgrad_consumer<P, SPLIT, 2>(p, sSt, img, full, empty, nch, tid);
+  } else {
+    reg_release<C::PRODUCER_REGS>();
+    // warp 0 of this warpgroup keeps the ring full: chunks 0 .. STAGES-1 up front, chunk i + STAGES once chunk i is summed
+    // (its stage is free as soon as the consumers retired chunk i too)
+    const bool issuer = warp == C::PRODUCER_WARP;
     const uint32_t leader = elect_one_sync();
-    for (int i = 0; i < nch; ++i) {
+    auto load = [&](int i) {
       const int s = i % STAGES;
       mbar_wait(&empty[s], ((i / STAGES) & 1) ^ 1);
       if (leader) {
@@ -251,58 +350,51 @@ __global__ void __launch_bounds__(ResWgradCfg<P, SPLIT>::THREADS, 1) res_wgrad_k
         if constexpr (SPLIT) tma_load_2d(st + C::X_BYTES + C::DY_BYTES, &p.dy_lo, &full[s], 0, (c_begin + i) * 128);
       }
       __syncwarp();
-    }
-  } else if (warp >= C::BW) {
-    // consumer warpgroup of accumulator a: M = 128 rows (two 64-row blocks of the window, or block 0 + the all-ones block), N = DY_CH
-    const int a = (warp - C::BW) >> 2, wt = tid & 127;
-    constexpr uint32_t DYK = P::DY_CH * 2;           // descriptor address units per K = 16 step of the dY tile (16 rows x row bytes / 16)
-    const uint32_t ones = smem_u32(sOnes);
-    float acc[2][P::DY_CH / 2];
+    };
+    if (issuer)
+      for (int i = 0; i < STAGES && i < nch; ++i) load(i);
+    if constexpr (C::BIAS_MMA) {
+      // bias gradient = ones^T dY: every row of the m64 accumulator holds the column sums; row 0 sits in lanes 0-3 of warp 0
+      constexpr uint32_t DYK = P::DY_CH * 2;
+      float bacc[P::DY_CH / 2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+      for (int j = 0; j < P::DY_CH / 2; ++j) bacc[j] = 0.f;
+      const uint64_t od = make_smem_desc(smem_u32(sOnes), 8192, 1024);
+      for (int i = 0; i < nch; ++i) {
+        const int s = i % STAGES;
+        mbar_wait(&full[s], (i / STAGES) & 1);
+        const uint64_t dyd = make_smem_desc(smem_u32(sSt + s * C::STAGE_BYTES + C::X_BYTES), 8192, 1024);
+        wg_fence();
 #pragma unroll
-      for (int j = 0; j < P::DY_CH / 2; ++j) acc[h][j] = 0.f;
-    for (int i = 0; i < nch; ++i) {
-      const int s = i % STAGES;
-      mbar_wait(&full[s], (i / STAGES) & 1);
-      const uint32_t st = smem_u32(sSt + s * C::STAGE_BYTES);
-      const uint64_t dyd = P::DY_CH == 64 ? make_smem_desc(st + C::X_BYTES, 8192, 1024) : make_smem_desc_sw64(st + C::X_BYTES, 4096, 512);
-      const uint32_t blk0 = st + P::acc_win(a) * C::WIN_BYTES + P::acc_shift0(a) * 128;
-      // a half-empty accumulator (conv3's tenth "tap"): the all-ones block (bias gradient) in the bf16 mode; in the split
-      // mode the bias comes from the staged dY tiles and the spare half just re-reads the window one row further (ignored)
-      const uint32_t blk1 = P::acc_shift1(a) >= 0 ? st + P::acc_win1(a) * C::WIN_BYTES + P::acc_shift1(a) * 128
-                                                  : (BIAS_SMEM ? blk0 + 128 : ones);
-      const uint32_t a_hi = (blk1 - blk0) / 16;      // descriptor distance between the two 64-row M blocks
-      const uint64_t xd = make_smem_desc(blk0, 8192, 1024);
-      wg_fence();
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {          // 128 positions = 8 x (K = 16): +2048 B per step
-        wg_mma128<P::DY_CH, 1, 1>(acc, xd + 128 * k, a_hi, dyd + DYK * k, 1);
-        if constexpr (SPLIT)         // hi(x) * lo(dy)
-          wg_mma128<P::DY_CH, 1, 1>(acc, xd + 128 * k, a_hi, dyd + (uint64_t)(C::DY_BYTES / 16 + DYK * k), 1);
-        if constexpr (C::ALO)        // lo(x) * hi(dy)
-          wg_mma128<P::DY_CH, 1, 1>(acc, xd + (uint64_t)(C::X_HI_BYTES / 16 + 128 * k), a_hi, dyd + DYK * k, 1);
+        for (int k = 0; k < 8; ++k) Wgmma<P::DY_CH, 1, 1>::mma(bacc, od + 128 * k, dyd + DYK * k, 1);
+        wg_commit();
+        if constexpr (STAGES > 1) {        // as in the consumers: chunk i - 1's stage is released (and refilled) once it retired
+          wg_wait_prev();
+          __syncwarp();
+          if (i > 0 && (tid & 31) == 0) mbar_arrive(&empty[(i - 1) % STAGES]);
+          if (issuer && i > 0 && i - 1 + STAGES < nch) load(i - 1 + STAGES);
+        } else {
+          wg_wait_all();
+          __syncwarp();
+          if ((tid & 31) == 0) mbar_arrive(&empty[s]);
+          if (issuer && i + 1 < nch) load(i + 1);
+        }
       }
-      wg_commit();
       wg_wait_all();
-      wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
-      __syncwarp();
-      if ((tid & 31) == 0) mbar_arrive(&empty[s]);
-    }
-    if (nch > 0) {
-      float* my_img = img + a * (WG_IMG_BYTES / 4);
+      wg_fence_regs(bacc);
+      const int bt = tid & 127;
+      if (bt < 4 && nch > 0) {
+        float* db = p.ws + (size_t)blockIdx.x * P::PART + P::PART - P::BIAS_CH;
 #pragma unroll
-      for (int c = 0; c < P::DY_CH / 16; ++c) {
-        float v[16];
-        wg_acc_row16<P::DY_CH>(acc, c, my_img, wt, 2 + a, v);
-        P::template epilogue16<SPLIT>(p, a, wt, c * 16, v);
+        for (int j = 0; j < P::DY_CH / 8; ++j) { db[8 * j + 2 * bt] = bacc[4 * j]; db[8 * j + 2 * bt + 1] = bacc[4 * j + 1]; }
       }
+      return;
     }
-  } else if constexpr (BIAS_SMEM) {
-    // bias gradient = column sums of dy, taken from the staged dy tiles while the MMAs run (no all-ones accumulator).
+    // bias gradient = column sums of dy, taken from the staged dy tiles while the MMAs run.
     // dy tile rows: DY_CH channels = NG 16-byte groups; thread -> group g, rows q + RP k (RP rows per pass, NG passes)
     constexpr int NG = P::DY_CH / 8, RP = 128 / NG;
-    const int g = tid & (NG - 1), q = tid / NG;
+    const int bt = tid & 127, bw = bt >> 5;
+    const int g = bt & (NG - 1), q = bt / NG;
     float bs[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) bs[j] = 0.f;
@@ -311,7 +403,7 @@ __global__ void __launch_bounds__(ResWgradCfg<P, SPLIT>::THREADS, 1) res_wgrad_k
     // summed).  So the tile is read with ld.shared (same pipe as the mbarrier op), and every lane stores a value that
     // depends on all of its loads before the warp arrives: the store cannot issue until the loads returned, and the
     // arrive (release) is ordered after the store.
-    const uint32_t dep_slot = smem_u32(sOnes) + 4096 + tid * 4;
+    const uint32_t dep_slot = smem_u32(sBias) + 1024 + bt * 4;
     for (int i = 0; i < nch; ++i) {
       const int s = i % STAGES;
       mbar_wait(&full[s], (i / STAGES) & 1);
@@ -330,8 +422,9 @@ __global__ void __launch_bounds__(ResWgradCfg<P, SPLIT>::THREADS, 1) res_wgrad_k
       sts_volatile_f32(dep_slot, dep);
       __syncwarp();
       if ((tid & 31) == 0) mbar_arrive(&empty[s]);
+      if (issuer && i + STAGES < nch) load(i + STAGES);
     }
-    float* red = reinterpret_cast<float*>(sOnes);          // the all-ones block is not used by these problems
+    float* red = reinterpret_cast<float*>(sBias);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       if (NG == 4) bs[j] += __shfl_xor_sync(0xffffffffu, bs[j], 4);
@@ -340,10 +433,10 @@ __global__ void __launch_bounds__(ResWgradCfg<P, SPLIT>::THREADS, 1) res_wgrad_k
     }
     if ((tid & 31) < NG) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) red[warp * 64 + g * 8 + j] = bs[j];
+      for (int j = 0; j < 8; ++j) red[bw * 64 + g * 8 + j] = bs[j];
     }
-    asm volatile("bar.sync 1, 128;" ::: "memory");        // bias warps only
-    if (tid < P::BIAS_CH && nch > 0) p.ws[(size_t)blockIdx.x * P::PART + P::NACC * 128 * P::DY_CH + tid] = red[tid] + red[64 + tid] + red[128 + tid] + red[192 + tid];
+    asm volatile("bar.sync 1, 128;" ::: "memory");        // this warpgroup only
+    if (bt < P::BIAS_CH && nch > 0) p.ws[(size_t)blockIdx.x * P::PART + P::PART - P::BIAS_CH + bt] = red[bt] + red[64 + bt] + red[128 + bt] + red[192 + bt];
   }
 }
 
@@ -351,7 +444,7 @@ __global__ void __launch_bounds__(ResWgradCfg<P, SPLIT>::THREADS, 1) res_wgrad_k
 template <class P, int SPLIT>
 cudaError_t res_wgrad_launch_t(typename P::Params p, int target_ctas, cudaStream_t stream, int* ctas) {
   using C = ResWgradCfg<P, SPLIT>;
-  static_assert(P::PART == P::NACC * 128 * P::DY_CH + P::BIAS_CH, "partial slice layout");
+  static_assert(P::PART >= P::NBLK * 64 * P::DY_CH + P::BIAS_CH, "partial slice layout");
   const int nchunks = (p.P + 127) >> 7;
   *ctas = 0;
   if (nchunks <= 0) return cudaSuccess;

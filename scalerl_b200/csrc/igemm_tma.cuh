@@ -7,7 +7,8 @@
 //                   the wgmma (two m64 halves per K = 16 step), keeps the accumulator in registers and runs the epilogue
 //                   (registers -> shared-memory row hand-off -> global)
 //   full[s]  : mbarrier, 1 arrival (producer's arrive.expect_tx) + TMA complete_tx bytes
-//   empty[s] : mbarrier, 8 arrivals (one per consumer warp, after wgmma.wait_group)
+//   empty[s] : mbarrier, 8 arrivals (one per consumer warp, once the wgmma group reading the stage retired: the consumers keep one
+//              k-block's MMAs in flight and release its stage after issuing the next one)
 //
 // Shared-memory tiles are SWIZZLE_128B (the tensor maps are encoded with CU_TENSOR_MAP_SWIZZLE_128B, so the bytes
 // land exactly where the wgmma descriptors of igemm.cuh expect them).
@@ -161,11 +162,19 @@ __global__ void __launch_bounds__(IGT_THREADS) igemm_tma_kernel(const __grid_con
         }
       }
       wg_commit();
-      wg_wait_all();
-      wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
-      __syncwarp();
-      if ((tid & 31) == 0) mbar_arrive(&empty[s]);
+      if constexpr (C::STAGES > 1) {
+        // k-block kb stays in flight while kb + 1 is awaited and issued; kb - 1's stage is released as soon as it retired
+        wg_wait_prev();
+        __syncwarp();
+        if (kb > 0 && (tid & 31) == 0) mbar_arrive(&empty[(kb - 1) % C::STAGES]);
+      } else {
+        wg_wait_all();
+        __syncwarp();
+        if ((tid & 31) == 0) mbar_arrive(&empty[s]);
+      }
     }
+    wg_wait_all();
+    wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
     float* my_img = img + g * (WG_IMG_BYTES / 4);
 #pragma unroll
     for (int c = 0; c < NB / 16; ++c) {

@@ -157,64 +157,41 @@ struct RConv2Dgrad {   // the 4 stride-parity classes share A (da2g at (i'-kh', 
 // (encoder.cu) adds the slices in CTA order into the workspace and the bias gradients, and conv_wgrad_finalize_kernel then
 // writes the PyTorch-layout gradient tensors.  Workspace offsets (floats):
 // (WS_W3 / WS_W2 / WS_W1 / WS_TOTAL are defined in kernels.h: the optimizer kernel reads the workspace too)
-SRL_DEVINL void store16(float* dst, const float (&v)[16]) {
-#pragma unroll
-  for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-}
-
-struct RConv3Wgrad {   // acc a = taps (2a, 2a+1); acc 4 = (tap 8, ones -> db3).  ws: [10 taps][64 c][64 co] fp32 (co contiguous)
+// Tap block b = 64 rows of dW (one m64 wgmma accumulator) = window rows starting blk_shift(b) in window blk_win(b).
+struct RConv3Wgrad {   // block b = tap b.  ws: [10 taps][64 c][64 co] fp32 (co contiguous; the tenth block is not written), db3
   static constexpr int KID = 21;        // diagnostics timeline id
-  static constexpr int NACC = 5, NWIN = 1, WROWS = 128 + 20, STAGES = 3, SPLIT_STAGES = 2;
+  static constexpr int NBLK = 9, CWG = 3, NWIN = 1, WROWS = 128 + 20, STAGES = 3, SPLIT_STAGES = 2;
   static constexpr bool A_LO = true;
-  static constexpr bool SMEM_BIAS = false;     // the ninth tap leaves half an accumulator free: the all-ones block rides along
+  static constexpr bool SMEM_BIAS = false;     // db3 from an all-ones wgmma (bf16 mode; the split mode sums the dY columns)
   static constexpr int BIAS_CH = 64, DY_CH = 64;
   static constexpr int PART = WSP_W3;
   struct Params { SRL_TMAP in0; SRL_TMAP dy; SRL_TMAP in0_lo; SRL_TMAP dy_lo; float* ws; int P; int chunks_per_cta; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.dy); }
-  SRL_DEVINL static constexpr int sh(int tap) { return (tap / 3) * 9 + tap % 3; }
-  SRL_DEVINL static constexpr int acc_win(int) { return 0; }
-  SRL_DEVINL static constexpr int acc_win1(int) { return 0; }
-  SRL_DEVINL static constexpr int acc_shift0(int a) { return sh(2 * a); }
-  SRL_DEVINL static constexpr int acc_shift1(int a) { return a < 4 ? sh(2 * a + 1) : -1; }
+  SRL_DEVINL static constexpr int blk_win(int) { return 0; }
+  SRL_DEVINL static constexpr int blk_shift(int b) { return (b / 3) * 9 + b % 3; }
   SRL_DEVINL static void load_windows(const Params& p, int chunk, uint8_t* dst, int, uint64_t* bar, bool lo) { tma_load_2d(dst, lo ? &p.in0_lo : &p.in0, bar, 0, chunk * 128); }
-  template <int SPLIT>
-  SRL_DEVINL static void epilogue16(const Params& p, int a, int row, int c0, float (&v)[16]) {
-    const int tap = 2 * a + (row >> 6), c = row & 63;
-    float* ws = p.ws + (size_t)blockIdx.x * PART;
-    if (tap < 9) {
-      store16(ws + ((size_t)(a * 128 + row)) * 64 + c0, v);
-    } else if (!SPLIT && c == 0) {          // split mode: db3 comes from the staged dY tiles (igemm_res.cuh)
-      store16(ws + NACC * 128 * 64 + c0, v);
-    }
-  }
 };
 
-struct RConv2Wgrad {   // acc a = kh (blocks kww = 0,1: rows = (kw = 2kww + wp, c)); db2 = column sums of the staged dy tiles
+struct RConv2Wgrad {   // block b = (kh = b >> 1, kww = b & 1): rows = (kw = 2kww + wp, c), row-parity plane kh & 1
   static constexpr int KID = 22;        // diagnostics timeline id
-  static constexpr int NACC = 4, NWIN = 2, WROWS = 128 + 11, STAGES = 3, SPLIT_STAGES = 1;
+  static constexpr int NBLK = 8, CWG = 2, NWIN = 2, WROWS = 128 + 11, STAGES = 3, SPLIT_STAGES = 1;
   static constexpr bool A_LO = true;
   static constexpr bool SMEM_BIAS = true;
   static constexpr int BIAS_CH = 64, DY_CH = 64;
   static constexpr int PART = WSP_W2;
   struct Params { SRL_TMAP in0; SRL_TMAP in1; SRL_TMAP dy; SRL_TMAP in0_lo; SRL_TMAP in1_lo; SRL_TMAP dy_lo; float* ws; int P; int chunks_per_cta; };   // ws: [4 kh][128 (kw,c)][64 co]
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.in1); tma_prefetch_desc(&p.dy); }
-  SRL_DEVINL static constexpr int acc_win(int a) { return a & 1; }
-  SRL_DEVINL static constexpr int acc_win1(int a) { return a & 1; }
-  SRL_DEVINL static constexpr int acc_shift0(int a) { return (a >> 1) * 10; }
-  SRL_DEVINL static constexpr int acc_shift1(int a) { return (a >> 1) * 10 + 1; }
+  SRL_DEVINL static constexpr int blk_win(int b) { return (b >> 1) & 1; }
+  SRL_DEVINL static constexpr int blk_shift(int b) { return (b >> 2) * 10 + (b & 1); }
   SRL_DEVINL static void load_windows(const Params& p, int chunk, uint8_t* dst, int win_bytes, uint64_t* bar, bool lo) {
     tma_load_2d(dst, lo ? &p.in0_lo : &p.in0, bar, 0, chunk * 128);
     tma_load_2d(dst + win_bytes, lo ? &p.in1_lo : &p.in1, bar, 0, chunk * 128);
   }
-  template <int SPLIT>
-  SRL_DEVINL static void epilogue16(const Params& p, int a, int row, int c0, float (&v)[16]) {
-    store16(p.ws + (size_t)blockIdx.x * PART + ((size_t)(a * 128 + row)) * 64 + c0, v);
-  }
 };
 
-struct RConv1Wgrad {   // acc a = kh2 (blocks kw2 = 0,1: rows = (kw2, c, dy, dx)); db1 = column sums of the staged dy tiles
+struct RConv1Wgrad {   // block b = (kh2 = b >> 1, kw2 = b & 1): rows = (c, dy, dx)
   static constexpr int KID = 23;        // diagnostics timeline id
-  static constexpr int NACC = 2, NWIN = 1, WROWS = 128 + 22, STAGES = 5, SPLIT_STAGES = 3;
+  static constexpr int NBLK = 4, CWG = 2, NWIN = 1, WROWS = 128 + 22, STAGES = 5, SPLIT_STAGES = 3;
   static constexpr bool A_LO = false;          // the frames are exact in bf16
   static constexpr bool SMEM_BIAS = true;
   static constexpr int BIAS_CH = 32;
@@ -222,16 +199,9 @@ struct RConv1Wgrad {   // acc a = kh2 (blocks kw2 = 0,1: rows = (kw2, c, dy, dx)
   static constexpr int PART = WSP_W1;
   struct Params { SRL_TMAP in0; SRL_TMAP dy; SRL_TMAP dy_lo; float* ws; int P; int chunks_per_cta; };   // ws: [2 kh2][128 (kw2,c,dy,dx)][32 co]
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.dy); }
-  SRL_DEVINL static constexpr int acc_win(int) { return 0; }
-  SRL_DEVINL static constexpr int acc_win1(int) { return 0; }
-  SRL_DEVINL static constexpr int acc_shift0(int a) { return a * 21; }
-  SRL_DEVINL static constexpr int acc_shift1(int a) { return a * 21 + 1; }
+  SRL_DEVINL static constexpr int blk_win(int) { return 0; }
+  SRL_DEVINL static constexpr int blk_shift(int b) { return (b >> 1) * 21 + (b & 1); }
   SRL_DEVINL static void load_windows(const Params& p, int chunk, uint8_t* dst, int, uint64_t* bar, bool) { tma_load_2d(dst, &p.in0, bar, 0, chunk * 128); }
-  template <int SPLIT>
-  SRL_DEVINL static void epilogue16(const Params& p, int a, int row, int c0, float (&v)[16]) {
-    if (c0 >= 32) return;                    // N = 32: accumulator columns 32..63 are not written by the MMAs
-    store16(p.ws + (size_t)blockIdx.x * PART + ((size_t)(a * 128 + row)) * 32 + c0, v);
-  }
 };
 
 }  // namespace srl
