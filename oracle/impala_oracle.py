@@ -114,7 +114,7 @@ def atari_forward(params: Dict[str, torch.Tensor], obs: torch.Tensor, reward: to
     T1, B = obs.shape[:2]
     N = T1 * B
     rd = _bf16 if emulate_bf16 else (lambda t: t)
-    x = obs.reshape(N, *obs.shape[2:]).float()
+    x = obs.reshape(N, *obs.shape[2:]).to(params['conv1.weight'].dtype)      # float32, or float64 for fp64 references
     if emulate_bf16:
         a1 = F.conv2d(x, rd(params['conv1.weight']), None, stride=4) * (1.0 / 255.0) + params['conv1.bias'].view(1, -1, 1, 1)
     else:

@@ -18,6 +18,7 @@ import pytest
 import torch
 
 from oracle import impala_oracle as O
+from tests import layer_ref as R
 from tests.conftest import GOLDEN
 from tests.helpers import assert_close, rel_l2, strided_sample
 from tests.test_gpu_fullsize import _record
@@ -41,9 +42,9 @@ def _mask_flips(L, params, batch, T, B):
     z2 = F.conv2d(F.relu(z1), params['conv2.weight'], params['conv2.bias'], stride=2)
     z3 = F.conv2d(F.relu(z2), params['conv3.weight'], params['conv3.bias'], stride=1)
     zh = F.linear(F.relu(z3).reshape(NF, -1), params['fc.weight'], params['fc.bias'])
-    g1 = L.debug_buffer('a1').float().view(2, NF, 10, 10, 2, 32).permute(1, 5, 2, 0, 3, 4).reshape(NF, 32, 20, 20).cpu()
-    g2 = L.debug_buffer('a2').float().view(NF, 9, 9, 64).permute(0, 3, 1, 2).cpu()
-    g3 = L.debug_buffer('a3').float().view(NF, 7, 7, 64).permute(0, 3, 1, 2).cpu()
+    g1 = R.a1_planes_to_nchw(L.debug_buffer('a1').float().cpu(), NF)
+    g2 = R.nhwc_to_nchw(L.debug_buffer('a2').float().cpu(), NF, 9)
+    g3 = R.nhwc_to_nchw(L.debug_buffer('a3').float().cpu(), NF, 7)
     gh = L.debug_buffer('h').view(NF, 512).cpu()
     flips, units, worst = 0, 0, 0.0
     for z, g in ((z1, g1), (z2, g2), (z3, g3), (zh, gh)):
