@@ -15,7 +15,7 @@ SOURCES = ['api.cu', 'encoder.cu', 'vtrace.cu', 'heads_optim.cu', 'lstm.cu', 'pe
 HOOK_SOURCES = ['testhooks.cu', 'test_shift.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xptxas', '-v', '--expt-relaxed-constexpr'] + \
-             [f'-D{d}' for d in os.environ.get('SRL_DEFINES', '').split(',') if d]       # e.g. SRL_DEFINES=SRL_DEBUG_BIAS_REREAD (debug builds)
+             [f'-D{d}' for d in os.environ.get('SRL_DEFINES', '').split(',') if d]       # e.g. SRL_DEFINES=SRL_KSTAMP (diagnostics build)
 
 
 def _nvcc():

@@ -235,8 +235,7 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
   L->G = make_ptrs(grads, cfg->A);
   L->step = 0; L->have_fwd = false;
   { const char* nf = getenv("SRL_NO_COLUMN_FUSION"); L->column_fusion = !(nf && atoi(nf) != 0); }   // read once, at creation
-  // measured (profiles/r02_fused_front_timeline.md): one CTA per SM with ONE MMA-issuing thread paces the fused front at ~10 us per
-  // frame -- 52 us against 47 us for the three kernels it replaces -- so it is opt-in until it issues from two warps
+  // opt-in: the fused front has not been measured on H100 against the three kernels it replaces
   { const char* ff = getenv("SRL_FUSED_FWD"); L->fused_front = ff && atoi(ff) != 0; }
   for (int i = 0; i < 2 * PS_COUNT; ++i) L->events[i] = nullptr;
   for (int i = 0; i < PS_COUNT; ++i) L->slot_used[i] = false;
@@ -438,35 +437,20 @@ bool pdl_active() {
   return env_on && g_pdl_on;
 }
 void pdl_set_active(bool on) { g_pdl_on = on; }
-int pdl_skip_mask() {
-  static const int m = [] { const char* e = getenv("SRL_PDL_MASK"); return e ? atoi(e) : 0; }();
-  return m;
-}
 }  // namespace srl
 
 // the re-pack stream sits one level BELOW the greatest priority (which the learner's capture stream uses for the main chain) and above the wgrad
-// streams (default = least): its short blocks fill the slots the frame conversion leaves free without delaying it.  SRL_PACK_PRIORITY overrides.
+// streams (default = least): its short blocks fill the slots the frame conversion leaves free without delaying it
 static int pack_priority(int least, int greatest) {
-  const char* e = getenv("SRL_PACK_PRIORITY");
-  int v = e ? atoi(e) : greatest + 1;
-  if (v < greatest) v = greatest;
-  if (v > least) v = least;
-  return v;
+  return greatest + 1 > least ? least : greatest + 1;
 }
 
 static int encode_impl(srl_learner* L, const uint8_t* obs, int frames, cudaStream_t st, bool zero_small_grads = false) {
-  const bool zero_small_grads_in = zero_small_grads;      // true = called from the learner step (forward + backward)
   L->pf.st = st;
   pdl_set_active(!L->pf.on);
   // The bf16 operand copies are re-derived from the fp32 master weights at the START of every forward (not at the end
   // of the optimizer step): the pack kernel runs on the side stream underneath the frame conversion.
   cudaEvent_t packed = nullptr;
-  if (zero_small_grads && (side_mode() & 4)) {
-    int64_t off[12], cnt[12];
-    layout(L->cfg.A, off, cnt);
-    CU(cudaMemsetAsync(L->grads, 0, off[6] * sizeof(float), st), "zero small grads");
-    zero_small_grads = false;
-  }
   if (L->ss.side && !L->pf.on) {
     CU(cudaEventRecord(L->ss.ev[5], st), "fork pack");
     CU(cudaStreamWaitEvent(L->ss.pack, L->ss.ev[5], 0), "fork pack");
@@ -494,7 +478,7 @@ static int encode_impl(srl_learner* L, const uint8_t* obs, int frames, cudaStrea
   // learner step (bf16 mode): a3 -> fc.weight column order for the fc weight-gradient GEMM, on the wgrad side stream right after the fc forward,
   // i.e. under the column kernel (32 CTAs, the GPU is otherwise idle) instead of in the crowded backward phase
   L->buf.a3t_ready = false;
-  if (zero_small_grads_in && L->ss.side && !L->pf.on && L->cfg.precision == 0 && L->buf.a3t && !L->cfg.use_lstm) {
+  if (zero_small_grads && L->ss.side && !L->pf.on && L->cfg.precision == 0 && L->buf.a3t && !L->cfg.use_lstm) {
     CU(cudaEventRecord(L->ss.ev[10], st), "fork a3 transpose");
     CU(cudaStreamWaitEvent(L->ss.side, L->ss.ev[10], 0), "fork a3 transpose");
     CU(launch_a3_transpose(L->buf.a3, L->buf.a3t, L->cfg.T * L->cfg.B, L->ss.side), "a3_transpose");
@@ -551,7 +535,7 @@ static int fb_begin(srl_learner* L, const uint8_t* obs, const float* reward, con
   }
   L->pf.b(PS_HEAD_BWD);
   {
-    const bool fork = L->ss.side != nullptr && !L->pf.on && !(side_mode() & 2);
+    const bool fork = L->ss.side != nullptr && !L->pf.on;
     cudaStream_t sw = fork ? L->ss.side : st;
     if (fork) { CU(cudaEventRecord(L->ss.ev[8], st), "fork head wgrad"); CU(cudaStreamWaitEvent(sw, L->ss.ev[8], 0), "fork head wgrad"); }
     CU(launch_head_bwd(L->dlogits, L->dbaseline, L->buf.h, reward, action, L->P.wp, L->P.wb, NB, c.A, L->buf.dh, L->G.wp, L->G.bp, L->G.wb,
@@ -755,7 +739,6 @@ extern "C" int srl_learner_debug_buffer(srl_learner_t* L, const char* name, void
       {"logits", L->logits, NF * A}, {"baseline", L->baseline, NF}, {"dlogits", L->dlogits, NB * A}, {"dbaseline", L->dbaseline, NB},
       {"dh", L->buf.dh, NB * 512}, {"da3", L->buf.da3, NB * 81 * 64}, {"da2", L->buf.da2, NB * 100 * 64},
       {"da1", L->buf.da1, NB * 441 * 32}, {"wpack", L->buf.wpack, WPack::TOTAL},
-      {"fused_dbg", g_fused_dbg, 5 * 8 * 8 * 4},        // u64 stamps, counted in bf16 units by the Python helper (x4)
       {"a1_lo", L->buf.a1_lo, NF * 400 * 32}, {"a2_lo", L->buf.a2_lo, NF * 81 * 64}, {"a3_lo", L->buf.a3_lo, NF * 49 * 64},
       {"dh_lo", L->buf.dh_lo, NB * 512}, {"da3_lo", L->buf.da3_lo, NB * 81 * 64}, {"da2_lo", L->buf.da2_lo, NB * 100 * 64},
       {"da1_lo", L->buf.da1_lo, NB * 441 * 32}, {"wpack_lo", L->buf.wpack_lo, WPack::TOTAL}};

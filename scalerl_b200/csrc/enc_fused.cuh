@@ -55,17 +55,7 @@ struct EncFusedParams {
   bf16* a2;                  // [frames*81][64]
   int frames;
   int NFS;                   // frame capacity of the a1 planes (plane stride)
-  int exp_flags;             // diagnostics only (SRL_FUSED_EXP, results invalid): 1 converters skip the X-tile stores, 2 skip xs global stores, 4 conv1 epilogue skips its stores, 8 conv2 epilogue skips its stores
-  unsigned long long* dbg;   // diagnostics (SRL_FUSED_DEBUG): CTA 0 stamps %globaltimer at [role][frame][event]; nullptr = off
 };
-constexpr int FF_DBG_EVENTS = 8, FF_DBG_FRAMES = 8;       // per role: 8 frames x 8 events
-SRL_DEVINL void ff_stamp(const EncFusedParams& p, int role, int it, int ev) {
-  if (p.dbg && blockIdx.x == 0 && it < FF_DBG_FRAMES) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    p.dbg[(role * FF_DBG_FRAMES + it) * FF_DBG_EVENTS + ev] = t;
-  }
-}
 
 // mbarrier wait for the roles that are not on the critical issue path: back off between polls so the spinning warps do not
 // take issue slots from the converter / epilogue warps sharing their schedulers
@@ -99,7 +89,6 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
   float* img = reinterpret_cast<float*>(smem + FF_OFF_IMG);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nmine = p.frames > (int)blockIdx.x ? (p.frames - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-  if (tid == 0) ff_stamp(p, 0, 0, 0);
 
   float* s_b1 = reinterpret_cast<float*>(smem + FF_OFF_BAR + 256);      // [32]
   float* s_b2 = s_b1 + 32;                                               // [64]
@@ -116,7 +105,6 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
     reinterpret_cast<uint4*>(sA1 + 2 * FF_A1_PLANE)[i] = make_uint4(0, 0, 0, 0);
   pdl_wait(54);                          // the parameters below were written by the previous step's optimizer kernel
   pdl_launch();
-  if (tid == 0) ff_stamp(p, 0, 0, 1);
   // ---- conv weights: fp32 master -> bf16 K-major SWIZZLE_128B operand tiles (what pack_weights_kernel + TMA would deliver).
   //      Read in memory order as float4 (coalesced), several loads in flight per thread, scattered into the tiles.
   //  w1 tile j (= tap (kh2,kw2)): row co (32), k = c*16 + dy*4 + dx  <- W1[co][c][4kh2+dy][4kw2+dx]; a float4 = the 4 dx of one (co,c,kh,kw2)
@@ -159,7 +147,6 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
   }
   fence_proxy_async_smem();
   __syncthreads();
-  if (tid == 0) ff_stamp(p, 0, 0, 2);
 
   if (warp == 16) {
     // ------------------------------------------------------------------------------------------------ producer
@@ -169,7 +156,6 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
         mbar_wait(&u8_empty[ub], ((it >> 1) & 1) ^ 1);
         mbar_arrive_expect_tx(&u8_full[ub], 28224);
         bulk_load_1d(sU8 + ub * FF_U8_BYTES, p.obs + (size_t)f * 28224, 28224, &u8_full[ub]);
-        ff_stamp(p, 1, it, 0);
       }
     }
   } else if (warp >= 8) {
@@ -180,7 +166,6 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
     for (int it = 0; it < nmine; ++it) {
       const int f = blockIdx.x + it * gridDim.x, ub = it & 1;
       mbar_wait_relaxed(&u8_full[ub], (it >> 1) & 1);
-      if (t == 0) ff_stamp(p, 3, it, 0);
       const uint8_t* u8 = sU8 + ub * FF_U8_BYTES + src_g;
       bf16* xs_f = p.xs + (size_t)f * 441 * 64 + gp * 8;
       for (int j = 0; j < 4; ++j) {
@@ -210,15 +195,14 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
             uint4 v = make_uint4(0u, 0u, 0u, 0u);
             if (Qs[k] < 441) {
               v = u8x8_to_bf16x8(w0[k], w1[k]);
-              if (row < 128 && !(p.exp_flags & 2)) *reinterpret_cast<uint4*>(xs_f + (size_t)Qs[k] * 64) = v;     // conv1 wgrad's operand
+              if (row < 128) *reinterpret_cast<uint4*>(xs_f + (size_t)Qs[k] * 64) = v;     // conv1 wgrad's operand
             }
-            if (!(p.exp_flags & 1)) *reinterpret_cast<uint4*>(x + swz128(row, gp)) = v;
+            *reinterpret_cast<uint4*>(x + swz128(row, gp)) = v;
           }
         }
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) mbar_arrive(&x_full[s]);
-        if (t == 0) ff_stamp(p, 3, it, 1 + j);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&u8_empty[ub]);
@@ -246,13 +230,12 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
         wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
         __syncwarp();
         if (lane == 0) mbar_arrive(&x_empty[s]);
-        if (tid == 0) ff_stamp(p, 4, it, j);
         float r0[16], r1[16];
         wg_acc_row16<32, true>(acc, 0, img, tid, 2, r0);
         wg_acc_row16<32, true>(acc, 1, img, tid, 2, r1);
         if (j == 0) mbar_wait_relaxed(a1_empty, (it & 1) ^ 1);   // conv2 of the previous frame has finished reading the planes
         const int Q = j * 128 + tid, oh = Q / 21, ow = Q - oh * 21;
-        if (Q < 441 && oh < 20 && ow < 20 && !(p.exp_flags & 4)) {
+        if (Q < 441 && oh < 20 && ow < 20) {
           float v[32];
 #pragma unroll
           for (int c = 0; c < 16; ++c) {
@@ -277,7 +260,6 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
       fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) mbar_arrive(a1_full);
-      if (tid == 0) ff_stamp(p, 4, it, 4);
     }
   } else {
     // ------------------------------------------------------------------------------------------------ conv2 warpgroup (warps 4-7)
@@ -288,7 +270,6 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
     for (int it = 0; it < nmine; ++it) {
       const int f = blockIdx.x + it * gridDim.x;
       mbar_wait_relaxed(a1_full, it & 1);
-      if (row == 0) ff_stamp(p, 2, it, 4);
       float acc[2][32];
       wg_fence();
 #pragma unroll
@@ -302,21 +283,18 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
       wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
       __syncwarp();
       if (lane == 0) mbar_arrive(a1_empty);
-      if (row == 0) ff_stamp(p, 4, it, 5);
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         float v[16];
         wg_acc_row16<64, true>(acc, q, img + WG_IMG_BYTES / 8, row, 3, v);
-        if (ok && !(p.exp_flags & 8)) {
+        if (ok) {
 #pragma unroll
           for (int c = 0; c < 16; ++c) v[c] = fmaxf(v[c] + s_b2[q * 16 + c], 0.f);
           store_bf16x16(p.a2 + ((size_t)f * 81 + oh2 * 9 + ow2) * 64 + q * 16, v);
         }
       }
-      if (row == 0) ff_stamp(p, 4, it, 6);
     }
   }
-  if (tid == 0) ff_stamp(p, 0, 0, 3);
 }
 
 inline cudaError_t enc_fused_fwd_launch(const EncFusedParams& p, int max_ctas, cudaStream_t stream) {
@@ -327,7 +305,7 @@ inline cudaError_t enc_fused_fwd_launch(const EncFusedParams& p, int max_ctas, c
   // the weight re-pack kernel (needed only by conv3 / fc) undisturbed
   const int per = (p.frames + max_ctas - 1) / max_ctas;
   const int grid = (p.frames + per - 1) / per;
-  return launch_chain<PDL_RESFWD>(enc_fused_fwd_kernel, dim3(grid), dim3(FF_THREADS), FF_SMEM_BYTES, stream, p);
+  return launch_chain(enc_fused_fwd_kernel, dim3(grid), dim3(FF_THREADS), FF_SMEM_BYTES, stream, p);
 }
 
 }  // namespace srl

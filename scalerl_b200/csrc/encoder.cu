@@ -95,10 +95,8 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(ParamPtrs p, bf16* __
 }
 
 // u8 NCHW frames -> space-to-depth bf16 NHWC: xs[n][Y][X][c*16+dy*4+dx] = obs[n][c][4Y+dy][4X+dx]  (exact: u8 fits bf16).
-// One block per (frame, S2D_Y consecutive Y): the 16 S2D_Y source rows (c,dy) are read coalesced (21 u32 each, all loads of a
-// thread in flight together) into shared memory, then each thread converts u32 (4 x dx) -> 4 bf16 and the block writes
-// S2D_Y x 21 x 128 B contiguously.  S2D_Y = 21 (a whole frame per block, 84 B of loads in flight per thread) by default.
-template <int S2D_Y>
+// One block per frame: the 16 x 21 source rows (c,dy) are read coalesced (21 u32 each, 84 B of loads in flight per thread) into
+// shared memory, then each thread converts u32 (4 x dx) -> 4 bf16 and the block writes 21 x 21 x 128 B contiguously.
 __global__ void __launch_bounds__(352) obs_s2d_kernel(const uint8_t* __restrict__ obs, bf16* __restrict__ xs, int frame_blocks,
                                                       const float* __restrict__ w1, bf16* __restrict__ w1k, bf16* __restrict__ w1k_lo) {
   pdl_wait(1);     // launched with programmatic stream serialization: see common.cuh
@@ -114,26 +112,26 @@ __global__ void __launch_bounds__(352) obs_s2d_kernel(const uint8_t* __restrict_
     }
     return;
   }
-  __shared__ uint32_t tile[S2D_Y][16][21];
-  const int n = blockIdx.x / (21 / S2D_Y), Y0 = (blockIdx.x - n * (21 / S2D_Y)) * S2D_Y;
+  __shared__ uint32_t tile[21][16][21];
+  const int n = blockIdx.x;
   const int t = threadIdx.x;
   if (t < 336) {
     const int g = t / 21, X = t - g * 21;      // g = (c, dy)
     const uint8_t* src = obs + (size_t)n * 28224 + (g >> 2) * 7056 + (g & 3) * 84;
 #pragma unroll
-    for (int y = 0; y < S2D_Y; ++y) tile[y][g][X] = __ldg(reinterpret_cast<const uint32_t*>(src + (Y0 + y) * 336) + X);
+    for (int y = 0; y < 21; ++y) tile[y][g][X] = __ldg(reinterpret_cast<const uint32_t*>(src + y * 336) + X);
   }
   __syncthreads();
   if (t < 336) {
     const int X = t >> 4, g = t & 15;
 #pragma unroll
-    for (int y = 0; y < S2D_Y; ++y) {
+    for (int y = 0; y < 21; ++y) {
       const uint32_t w = tile[y][g][X];
       const float f0 = __uint_as_float(__byte_perm(w, 0x4B000000u, 0x7540)) - 8388608.f;
       const float f1 = __uint_as_float(__byte_perm(w, 0x4B000000u, 0x7541)) - 8388608.f;
       const float f2 = __uint_as_float(__byte_perm(w, 0x4B000000u, 0x7542)) - 8388608.f;
       const float f3 = __uint_as_float(__byte_perm(w, 0x4B000000u, 0x7543)) - 8388608.f;
-      *reinterpret_cast<uint2*>(xs + (((size_t)n * 21 + Y0 + y) * 21 + X) * 64 + g * 4) = make_uint2(pack_bf16x2(f0, f1), pack_bf16x2(f2, f3));
+      *reinterpret_cast<uint2*>(xs + (((size_t)n * 21 + y) * 21 + X) * 64 + g * 4) = make_uint2(pack_bf16x2(f0, f1), pack_bf16x2(f2, f3));
     }
   }
 }
@@ -290,13 +288,9 @@ cudaError_t build_tma_maps_lo(const EncoderBuffers& b, int NF, int NB, TmaMapsLo
   return ok ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-unsigned long long* g_fused_dbg = nullptr;
 static cudaError_t launch_s2d(const uint8_t* obs, int frames, bf16* xs, cudaStream_t st, const float* w1, bf16* w1k, bf16* w1k_lo) {
-  static const int ygroup = [] { const char* e = getenv("SRL_S2D_Y"); const int v = e ? atoi(e) : 21; return (v == 3 || v == 7) ? v : 21; }();
   constexpr int WB = (32 * 256 + 351) / 352;      // extra blocks that write conv1's weight copy
-  if (ygroup == 3) SRL_TRY(launch_chain<PDL_SIMT>(obs_s2d_kernel<3>, dim3(frames * 7 + WB), dim3(352), 0, st, obs, xs, frames * 7, w1, w1k, w1k_lo));
-  else if (ygroup == 7) SRL_TRY(launch_chain<PDL_SIMT>(obs_s2d_kernel<7>, dim3(frames * 3 + WB), dim3(352), 0, st, obs, xs, frames * 3, w1, w1k, w1k_lo));
-  else SRL_TRY(launch_chain<PDL_SIMT>(obs_s2d_kernel<21>, dim3(frames + WB), dim3(352), 0, st, obs, xs, frames, w1, w1k, w1k_lo));
+  SRL_TRY(launch_chain(obs_s2d_kernel, dim3(frames + WB), dim3(352), 0, st, obs, xs, frames, w1, w1k, w1k_lo));
   return cudaGetLastError();
 }
 
@@ -393,15 +387,7 @@ cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, 
   // bf16 mode: frame conversion + conv1 + conv2 as ONE persistent kernel (enc_fused.cuh); SRL_FUSED_FWD=0 or the fp32-accurate
   // operand mode use the three separate kernels
   if (fused_front && !sp && (reinterpret_cast<uintptr_t>(obs) & 15) == 0) {
-    static unsigned long long* dbg_buf = [] {       // SRL_FUSED_DEBUG=1: CTA 0 stamps its phases (tests/diag/diag_fused.py prints them)
-      const char* e = getenv("SRL_FUSED_DEBUG");
-      unsigned long long* q = nullptr;
-      if (e && atoi(e) != 0 && cudaMalloc(&q, 5 * FF_DBG_FRAMES * FF_DBG_EVENTS * 8) == cudaSuccess) cudaMemset(q, 0, 5 * FF_DBG_FRAMES * FF_DBG_EVENTS * 8);
-      return q;
-    }();
-    static const int exp_flags = [] { const char* e = getenv("SRL_FUSED_EXP"); return e ? atoi(e) : 0; }();
-    EncFusedParams q{obs, p.w1, p.b1, p.w2, p.b2, buf.xs, buf.a1, buf.a2, frames, buf.NF, exp_flags, dbg_buf};
-    g_fused_dbg = dbg_buf;
+    EncFusedParams q{obs, p.w1, p.b1, p.w2, p.b2, buf.xs, buf.a1, buf.a2, frames, buf.NF};
     pf.b(PS_ENC_FUSED); SRL_TRY(enc_fused_fwd_launch(q, kPersistentCtas, st)); pf.e(PS_ENC_FUSED);
     if (wait_before_conv1) SRL_TRY(cudaStreamWaitEvent(st, wait_before_conv1, 0));      // conv3 / fc read the packed weights
   } else {
@@ -423,11 +409,6 @@ cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, 
   return cudaSuccess;
 }
 
-int side_mode() {
-  static const int m = [] { const char* e = getenv("SRL_SIDE_MODE"); return e ? atoi(e) : 0; }();
-  return m;
-}
-
 cudaError_t encoder_backward(const uint8_t* obs, int frames, const EncoderBuffers& buf, const ParamPtrs& g, const TmaMaps& maps, int mode,
                              cudaStream_t st, const Profiler& pf, const SideStream& ss, int phase, const TmaMapsLo* lo) {
   (void)obs;
@@ -441,8 +422,7 @@ cudaError_t encoder_backward(const uint8_t* obs, int frames, const EncoderBuffer
   // The wgrad GEMMs only feed the optimizer: each runs on its own side stream beside the dgrad chain
   // (dh -> da3 -> da2 -> da1) and beside each other.  With per-kernel profiling on everything stays on `st`.
   const bool fork = ss.side != nullptr && !pf.on;
-  const bool one_side = (side_mode() & 1) != 0;      // diagnostic: all wgrads serial on one side stream
-  cudaStream_t s1 = fork ? ss.side : st, s2 = fork ? (one_side ? ss.side : ss.side2) : st, s3 = fork ? (one_side ? ss.side : ss.side3) : st;
+  cudaStream_t s1 = fork ? ss.side : st, s2 = fork ? ss.side2 : st, s3 = fork ? ss.side3 : st;
   Profiler p1 = pf, p2 = pf, p3 = pf; p1.st = s1; p2.st = s2; p3.st = s3;
   if (do_fc) {
     if (fork) { SRL_TRY(cudaEventRecord(ss.ev[0], st)); SRL_TRY(cudaStreamWaitEvent(s1, ss.ev[0], 0)); }
@@ -488,9 +468,9 @@ cudaError_t encoder_backward(const uint8_t* obs, int frames, const EncoderBuffer
     SRL_TRY(cudaEventRecord(ss.ev[7], s3)); SRL_TRY(cudaStreamWaitEvent(st, ss.ev[7], 0));
   }
   pf.b(PS_WGRAD_FINALIZE);
-  SRL_TRY(launch_chain<PDL_SIMT>(conv_wgrad_reduce_kernel, dim3((WS_TOTAL / 4 + 160 + 255) / 256), dim3(256), 0, st, (const float*)part3, n3,
-                                 (const float*)part2, n2, (const float*)part1, n1, buf.wgrad_ws, g.b3, g.b2, g.b1));
-  SRL_TRY(launch_chain<PDL_SIMT>(conv_wgrad_finalize_kernel, dim3((36864 + 32768 + 8192 + 255) / 256), dim3(256), 0, st, buf.wgrad_ws, g.w1, g.w2, g.w3));
+  SRL_TRY(launch_chain(conv_wgrad_reduce_kernel, dim3((WS_TOTAL / 4 + 160 + 255) / 256), dim3(256), 0, st, (const float*)part3, n3,
+                       (const float*)part2, n2, (const float*)part1, n1, buf.wgrad_ws, g.b3, g.b2, g.b1));
+  SRL_TRY(launch_chain(conv_wgrad_finalize_kernel, dim3((36864 + 32768 + 8192 + 255) / 256), dim3(256), 0, st, buf.wgrad_ws, g.w1, g.w2, g.w3));
   SRL_TRY(cudaGetLastError());
   pf.e(PS_WGRAD_FINALIZE);
   return cudaSuccess;

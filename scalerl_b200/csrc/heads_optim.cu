@@ -2,8 +2,6 @@
 //   * policy / baseline heads forward + backward (atari_model.py:104-107,126-127 and their autograd)
 //   * bias-gradient column sums over bf16 dY
 //   * clip_grad_norm_ (impala_atari.py:344-345) + RMSprop (impala_atari.py:99-105,346) / Adam update
-#include <stdio.h>
-#include <stdlib.h>
 #include "common.cuh"
 #include "kernels.h"
 #include <cooperative_groups.h>
@@ -376,14 +374,14 @@ cudaError_t launch_head_fwd(const float* hpart, int nsplit, const float* bfc, fl
                             const float* Wp, const float* bp, const float* Wb, const float* bb, int N, int A, float* logits,
                             float* baseline, cudaStream_t st) {
   if (N <= 0) return cudaSuccess;
-  return launch_chain<PDL_SIMT>(head_fwd_kernel, dim3((N + 1) / 2), dim3(256), 0, st, hpart, nsplit, bfc, h, reward, action, Wp, bp, Wb, bb, N, A, logits, baseline);
+  return launch_chain(head_fwd_kernel, dim3((N + 1) / 2), dim3(256), 0, st, hpart, nsplit, bfc, h, reward, action, Wp, bp, Wb, bb, N, A, logits, baseline);
   return cudaGetLastError();
 }
 cudaError_t launch_head_bwd(const float* dlogits, const float* dbaseline, const float* h, const float* reward, const int64_t* action,
                             const float* Wp, const float* Wb, int N, int A, __nv_bfloat16* dh, float* gWp, float* gbp, float* gWb,
                             float* gbb, float* part, cudaStream_t st, cudaStream_t st_wgrad, bool do_dh, __nv_bfloat16* dh_lo) {
   if (N <= 0) return cudaSuccess;
-  if (do_dh) SRL_TRY(launch_chain<PDL_SIMT>(head_bwd_dh_kernel, dim3(N, 4), dim3(128), 0, st, dlogits, dbaseline, h, Wp, Wb, N, A, dh, dh_lo));
+  if (do_dh) SRL_TRY(launch_chain(head_bwd_dh_kernel, dim3(N, 4), dim3(128), 0, st, dlogits, dbaseline, h, Wp, Wb, N, A, dh, dh_lo));
   const int CORE = 513 + A;
   // the head weight gradients only feed the optimizer: they may run on a side stream (st_wgrad) beside the fc backward
   const int nslab = (N + HEAD_SLAB - 1) / HEAD_SLAB, spg = (nslab + HEAD_GROUPS - 1) / HEAD_GROUPS, groups = (nslab + spg - 1) / spg;
@@ -645,19 +643,16 @@ SRL_DEVINL void dp_wait(const DpPeers& P, unsigned epoch) {        // all thread
 template <int OPT, bool NVLS>
 __global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ p, float* g, float* __restrict__ s0, float* __restrict__ s1,
                                                             int64_t n, float max_norm, float* coef, float* scratch, float lr, float a,
-                                                            float b, float eps, int step, int* dstep, const DpPeers P, int dbg) {
+                                                            float b, float eps, int step, int* dstep, const DpPeers P) {
   cg::grid_group grid = cg::this_grid();
   const int64_t n4 = n >> 2, stride = (int64_t)gridDim.x * blockDim.x, i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int W = P.world, R = P.rank;
-  unsigned long long ts[8];
-  ts[0] = dbg ? global_ns() : 0;
   const int64_t chunk = (n4 + W - 1) / W, lo = R * chunk, hi = min(n4, lo + chunk);
   const int t = dstep ? *reinterpret_cast<volatile int*>(dstep) + 1 : step;
   const unsigned e0 = reinterpret_cast<volatile unsigned*>(P.ctl[R])[32];     // epoch base (rewritten after the grid barrier)
   // ---- barrier 1: every rank's backward is complete
   if (blockIdx.x == 0) dp_signal(P, e0 + 1, false);      // the gradients were written by earlier kernels: already at L2
   dp_wait(P, e0 + 1);
-  if (dbg) ts[1] = global_ns();
   // ---- phase 1: reduce my slice over all ranks (rank order); the result goes to my exchange buffer rs (read by the peers
   //      in phase 2) and, in place, to my gradient buffer
   float s = 0.f;
@@ -715,12 +710,9 @@ __global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ 
     float tsum = 0.f;
     for (int w = 0; w < 16; ++w) tsum += red[w];
     scratch[4 + blockIdx.x] = tsum;
-    if (dbg) ts[2] = global_ns();
     // the slice stores are local: the grid barrier makes them visible at L2, which is where the peers' NVLink loads land
-    if (dbg) ts[3] = global_ns();
   }
   grid.sync();
-  if (dbg) ts[4] = global_ns();
   // ---- barrier 2: all slices pushed everywhere, per-slice sums of squares published
   if (blockIdx.x == 0) {
     if (threadIdx.x < 32) {
@@ -738,7 +730,6 @@ __global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ 
     dp_signal(P, e0 + 2, true);
   }
   dp_wait(P, e0 + 2);
-  if (dbg) ts[5] = global_ns();
   if (threadIdx.x == 0) {
     double tot = 0.0;
     for (int q = 0; q < W; ++q) tot += (double)__uint_as_float(reinterpret_cast<volatile unsigned*>(P.ctl[R])[8 + q]);
@@ -817,9 +808,6 @@ __global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ 
     }
   }
   // no closing barrier: after barrier 2 no rank touches another rank's memory until the next step's barrier 1
-  if (dbg && threadIdx.x == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1))
-    printf("dp_apply rank %d blk %d ns: wait1 %llu  phase1 %llu  fence %llu  gridsync %llu  sum+signal+wait2 %llu  phase2 %llu\n", R, blockIdx.x,
-           ts[1] - ts[0], ts[2] - ts[1], ts[3] - ts[2], ts[4] - ts[3], ts[5] - ts[4], global_ns() - ts[5]);
 }
 
 template <int OPT, bool NVLS>
@@ -841,8 +829,7 @@ static cudaError_t launch_dp_clip_optim_t(float* p, float* g, float* s0, float* 
   int blocks = (int)(need < 1 ? 1 : need);
   int cap = per_sm * sms; if (cap > 592) cap = 592;
   if (blocks > cap) blocks = cap;
-  static int dbg = [] { const char* e = getenv("SRL_DP_DEBUG"); return e ? atoi(e) : 0; }();
-  void* args[] = {&p, &g, &s0, &s1, &n, &max_norm, &coef, &scratch, &lr, &a, &b, &eps, &step, &dstep, &P, &dbg};
+  void* args[] = {&p, &g, &s0, &s1, &n, &max_norm, &coef, &scratch, &lr, &a, &b, &eps, &step, &dstep, &P};
   return cudaLaunchCooperativeKernel((const void*)dp_clip_optim_kernel<OPT, NVLS>, dim3(blocks), dim3(512), args, 0, st);
 }
 // Weight-publish snapshot (impala_atari.py:348): dst = src when the step's total loss is finite, else dst keeps the last good

@@ -179,7 +179,7 @@ cudaError_t res_fwd_launch_t(const typename P::Params& p, int ntiles, int max_ct
   static PerDeviceOnce once;
   { cudaError_t e = ensure_max_dynamic_smem(once, res_fwd_kernel<P, SPLIT>, C::SMEM_BYTES); if (e != cudaSuccess) return e; }
   const int grid = ntiles < max_ctas ? ntiles : max_ctas;
-  return launch_chain<PDL_RESFWD>(res_fwd_kernel<P, SPLIT>, dim3(grid), dim3(RES_THREADS), C::SMEM_BYTES, stream, p);
+  return launch_chain(res_fwd_kernel<P, SPLIT>, dim3(grid), dim3(RES_THREADS), C::SMEM_BYTES, stream, p);
 }
 template <class P>
 cudaError_t res_fwd_launch(const typename P::Params& p, int ntiles, int max_ctas, cudaStream_t stream, int split = 0) {
@@ -454,7 +454,7 @@ cudaError_t res_wgrad_launch_t(typename P::Params p, int target_ctas, cudaStream
   p.chunks_per_cta = (nchunks + target_ctas - 1) / target_ctas;
   const int grid = (nchunks + p.chunks_per_cta - 1) / p.chunks_per_cta;
   *ctas = grid;
-  return launch_chain<PDL_RESWGRAD>(res_wgrad_kernel<P, SPLIT>, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, stream, p);
+  return launch_chain(res_wgrad_kernel<P, SPLIT>, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, stream, p);
 }
 template <class P>
 cudaError_t res_wgrad_launch(const typename P::Params& p, int target_ctas, cudaStream_t stream, int* ctas, int split = 0) {

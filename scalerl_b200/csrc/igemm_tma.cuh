@@ -192,7 +192,7 @@ cudaError_t igemm_tma_launch(const typename P::Params& p, dim3 grid, cudaStream_
   if (grid.x == 0 || grid.y == 0) return cudaSuccess;
   static PerDeviceOnce once;      // set once per device (outside any stream capture: the first step always runs eagerly)
   { cudaError_t e = ensure_max_dynamic_smem(once, igemm_tma_kernel<P, SPLIT>, C::SMEM_BYTES); if (e != cudaSuccess) return e; }
-  return launch_chain<PDL_IGEMM>(igemm_tma_kernel<P, SPLIT>, grid, dim3(IGT_THREADS), C::SMEM_BYTES, stream, p);
+  return launch_chain(igemm_tma_kernel<P, SPLIT>, grid, dim3(IGT_THREADS), C::SMEM_BYTES, stream, p);
 }
 
 }  // namespace srl

@@ -24,16 +24,14 @@ struct Profiler {
 // the kernels, which would serialise them anyway).
 bool pdl_active();
 void pdl_set_active(bool on);      // per calling thread: every C-ABI entry point sets it for the launches it makes
-int pdl_skip_mask();      // SRL_PDL_MASK diagnostic: bit t set = kernels of class t launch without the attribute
-enum { PDL_SIMT = 0, PDL_IGEMM = 1, PDL_RESFWD = 2, PDL_RESWGRAD = 3 };
-template <int TAG, class... KA, class... A>
+template <class... KA, class... A>
 inline cudaError_t launch_chain(void (*kernel)(KA...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = (pdl_active() && !((pdl_skip_mask() >> TAG) & 1)) ? 1 : 0;
+  cfg.attrs = attr; cfg.numAttrs = pdl_active() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 
@@ -60,13 +58,12 @@ inline cudaError_t ensure_max_dynamic_smem(PerDeviceOnce& once, K kernel, int by
 }
 
 void kstamp_set_encoder(unsigned long long*); void kstamp_set_vtrace(unsigned long long*); void kstamp_set_heads(unsigned long long*);   // diagnostics build (common.cuh)
-int side_mode();   // SRL_SIDE_MODE diagnostic bitmask: 1 = one wgrad side stream, 2 = head wgrad on the main stream, 4 = grad memset on the main stream
 
 struct SideStream {
   cudaStream_t side = nullptr;      // fc wgrad, weight re-pack
   cudaStream_t side2 = nullptr;     // conv3 wgrad
   cudaStream_t side3 = nullptr;     // conv2 wgrad
-  cudaStream_t pack = nullptr;      // weight re-pack + gradient memset at the start of a step: HIGHEST priority (conv2 waits for it), unlike the wgrad streams
+  cudaStream_t pack = nullptr;      // weight re-pack + gradient memset at the start of a step: above the wgrad streams' priority (conv2 waits for it; api.cu pack_priority)
   cudaEvent_t ev[12] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
 };
 
@@ -190,7 +187,6 @@ bool make_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, 
 cudaError_t build_tma_maps(const EncoderBuffers& buf, int NF, int NB, TmaMaps* maps, const char** why);
 cudaError_t build_tma_maps_lo(const EncoderBuffers& buf, int NF, int NB, TmaMapsLo* maps, const char** why);
 // wpack_lo != nullptr: also the low copies bf16(w - bf16(w)) in the same layouts
-extern unsigned long long* g_fused_dbg;          // SRL_FUSED_DEBUG stamp buffer of the fused encoder front (device memory; 5 x 8 x 8 u64)
 cudaError_t launch_a3_transpose(const __nv_bfloat16* a3, __nv_bfloat16* a3t, int frames, cudaStream_t st);
 cudaError_t launch_pack_weights(const ParamPtrs& p, __nv_bfloat16* wpack, cudaStream_t st, __nv_bfloat16* wpack_lo = nullptr, bool skip_w1k = false);
 // wait_before_conv1: optional event (weight re-pack running on the side stream) that conv1 must wait for

@@ -34,8 +34,8 @@ struct RConv1Fwd {   // 2x2 s1 over xs (== 8x8 s4 over the frame): taps (kh2,kw2
   static constexpr bool A_LO = false;        // the frames are exact in bf16: only the weights have a low tensor
   struct Params { SRL_TMAP in0; SRL_TMAP w; SRL_TMAP w_lo; const float* bias; bf16* out; bf16* out_lo; int NF; int NFS; };   // NF frames now, NFS = frames the a1 planes are strided for
   // conv1's K-major weight copy (w1k) is written by the frame-conversion kernel's extra blocks (obs_s2d_kernel, encoder.cu), not by
-  // pack_weights_kernel: conv1 then depends only on its stream predecessor and never waits for the re-pack (profiles/r02_timeline.md);
-  // the weight tiles are therefore loaded AFTER griddepcontrol.wait
+  // pack_weights_kernel: conv1 then depends only on its stream predecessor and never waits for the re-pack (encoder_forward joins the
+  // re-pack stream only before conv2); the weight tiles are therefore loaded AFTER griddepcontrol.wait
   static constexpr bool W_AFTER_WAIT = true;
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.w); }
   SRL_DEVINL static int num_tiles(const Params& p) { return (p.NF * 441 + 127) >> 7; }

@@ -36,7 +36,6 @@ bool pdl_active() {
   return env_on;
 }
 void pdl_set_active(bool) {}
-int pdl_skip_mask() { return 0; }
 
 static inline int cdiv_(int a, int b) { return (a + b - 1) / b; }
 cudaError_t test_gemm(const void* A, const void* B, float* D, int M, int N, int K, bool mn_major, bool simt, cudaStream_t st) {

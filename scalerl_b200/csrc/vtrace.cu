@@ -7,7 +7,6 @@
 //   vtrace_logits_kernel       from_logits (log-softmax gather for both policies, then the recursion)
 //   impala_tail_kernel         one pass over the [T+1,B] batch rows: shifts, reward clip, discounts, V-trace,
 //                              pg/baseline/entropy losses (deterministic two-level reduction), dlogits, dbaseline
-#include <stdio.h>
 #include "common.cuh"
 #include "kernels.h"
 
@@ -532,7 +531,7 @@ cudaError_t launch_vtrace_logits(const float* bl, const float* tl, const int64_t
 // ------------------------------------------------------------------------------------------------
 constexpr int COL_THREADS = 1024, COL_MAX_A = 31;      // lane a == A computes the baseline: A + 1 <= 32 lanes
 //      // 32 warps: every frame of a T <= 31 column in one pass of phase A
-template <int NSPLIT, int AMAX, bool DBG>
+template <int NSPLIT, int AMAX>
 __global__ void __launch_bounds__(COL_THREADS) column_step_kernel(
     const float* __restrict__ hpart, const float* __restrict__ bfc, float* __restrict__ h, const float* __restrict__ reward,
     const int64_t* __restrict__ action, const uint8_t* __restrict__ done, const float* __restrict__ bl, const float* __restrict__ Wp,
@@ -550,9 +549,6 @@ __global__ void __launch_bounds__(COL_THREADS) column_step_kernel(
   float* s_dl = s_base + (T + 1);                     // [T][A+1]: dlogits..., dbaseline
   __shared__ bool is_last;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, b = blockIdx.x;
-  unsigned long long tstamp[6];
-  auto stamp = [&](int i) { if (DBG) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); tstamp[i] = t; } };
-  stamp(0);
   // the head weights were final before the step started: loaded before griddepcontrol.wait (overlaps the fc GEMM's tail)
   for (int j = tid; j < CORE; j += COL_THREADS) {       // a thread copies column j of every row: A + 1 independent loads in flight
     float wv[AMAX + 1];
@@ -566,7 +562,6 @@ __global__ void __launch_bounds__(COL_THREADS) column_step_kernel(
   pdl_wait(41);
   pdl_launch();
   __syncthreads();
-  stamp(1);
   // ---- A: frames t = warp, warp + 32, ...; a lane owns features j = 128 i + 4 lane .. +3 (i < 4)
   for (int t = warp; t <= T; t += COL_THREADS / 32) {
     const size_t n = (size_t)t * B + b;
@@ -627,7 +622,6 @@ __global__ void __launch_bounds__(COL_THREADS) column_step_kernel(
     }
   }
   __syncthreads();
-  stamp(2);
   // ---- B: V-trace, losses and head gradients of this column (one warp)
   if (warp == 0) {
     float l_pg = 0.f, l_bl = 0.f, l_ent = 0.f;
@@ -653,7 +647,6 @@ __global__ void __launch_bounds__(COL_THREADS) column_step_kernel(
       *reinterpret_cast<unsigned*>(scratch) = 0u;
     }
   }
-  stamp(3);
   // ---- C: dh[n][j] for the T learning frames of the column; thread = (feature j, parity of t)
   {
     const int j = tid & 511;
@@ -671,12 +664,6 @@ __global__ void __launch_bounds__(COL_THREADS) column_step_kernel(
       dh[((size_t)t * B + b) * 512 + j] = hi;
       if (dh_lo) dh_lo[((size_t)t * B + b) * 512 + j] = __float2bfloat16_rn(dv - __bfloat162float(hi));   // fp32-accurate operand mode
     }
-  }
-  if (DBG) {
-    stamp(4);
-    if (tid == 0 && (b == 0 || b == gridDim.x - 1))
-      printf("column_step b=%d ns: stage_w %llu  A %llu  B+losses %llu  C %llu\n", b, tstamp[1] - tstamp[0], tstamp[2] - tstamp[1],
-             tstamp[3] - tstamp[2], tstamp[4] - tstamp[3]);
   }
 }
 
@@ -701,20 +688,17 @@ cudaError_t launch_column_step(const float* hpart, int nsplit, const float* bfc,
     bool first;
     const int dev = once.device(&first);
     if (first) {
-      cudaError_t e = cudaFuncSetAttribute(column_step_kernel<4, 8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(column_step_kernel<4, 32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(column_step_kernel<4, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+      cudaError_t e = cudaFuncSetAttribute(column_step_kernel<4, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(column_step_kernel<4, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
       if (e != cudaSuccess) return e;
       once.mark(dev);
     }
   }
-  static const bool dbg = [] { const char* e = getenv("SRL_COLUMN_DEBUG"); return e && atoi(e) != 0; }();   // prints phase times
 #define SRL_COL_ARGS dim3(B), dim3(COL_THREADS), column_smem_bytes(T, A), st, hpart, bfc, h, reward, action, done, bl, Wp, bp, Wb, bb, T, B, A, \
                      discounting, clip_reward, clip_rho, clip_pg, baseline_cost, entropy_cost, logits, baseline, vs, pg, dlogits, dbaseline, dh, \
                      losses, scratch, dh_lo
-  if (A <= 8) return dbg ? launch_chain<PDL_SIMT>(column_step_kernel<4, 8, true>, SRL_COL_ARGS)
-                         : launch_chain<PDL_SIMT>(column_step_kernel<4, 8, false>, SRL_COL_ARGS);
-  return launch_chain<PDL_SIMT>(column_step_kernel<4, 32, false>, SRL_COL_ARGS);
+  if (A <= 8) return launch_chain(column_step_kernel<4, 8>, SRL_COL_ARGS);
+  return launch_chain(column_step_kernel<4, 32>, SRL_COL_ARGS);
 #undef SRL_COL_ARGS
 }
 
@@ -723,10 +707,10 @@ cudaError_t launch_impala_tail(const float* bl, const float* tl, const float* ba
                                float clip_pg, float baseline_cost, float entropy_cost, float* vs, float* pg, float* dlogits,
                                float* dbaseline, float* losses, float* scratch, cudaStream_t st) {
   if (B <= 2048) {   // latency-bound sizes: one warp per column, shuffle scan over T (block partials: 3*ceil(B/4) <= 1536 floats)
-    return launch_chain<PDL_SIMT>(impala_tail_warp_kernel, dim3((B + 3) / 4), dim3(128), 0, st, bl, tl, baseline, action, reward, done, T, B, A, discounting,
+    return launch_chain(impala_tail_warp_kernel, dim3((B + 3) / 4), dim3(128), 0, st, bl, tl, baseline, action, reward, done, T, B, A, discounting,
                         clip_reward, clip_rho, clip_pg, baseline_cost, entropy_cost, vs, pg, dlogits, dbaseline, losses, scratch);
   } else {
-    return launch_chain<PDL_SIMT>(impala_tail_kernel, dim3((B + 127) / 128), dim3(128), 0, st, bl, tl, baseline, action, reward, done, T, B, A, discounting,
+    return launch_chain(impala_tail_kernel, dim3((B + 127) / 128), dim3(128), 0, st, bl, tl, baseline, action, reward, done, T, B, A, discounting,
                         clip_reward, clip_rho, clip_pg, baseline_cost, entropy_cost, vs, pg, dlogits, dbaseline, losses, scratch);
   }
   return cudaGetLastError();

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """profiles/ncu_traffic.json from the summary table written by tools/ncu_summary.py:
-   python tools/ncu_traffic.py profiles/r01_ncu_full_v11.md 'source text' > profiles/ncu_traffic.json
+   python tools/ncu_summary.py ncu_out/prof.ncu-rep ncu_out/prof.md
+   python tools/ncu_traffic.py ncu_out/prof.md 'source text' > profiles/ncu_traffic.json
 Per bench.py profile slot: mean DRAM read+write bytes per launch, ncu duration, tensor-pipe activity."""
 import json
 import re
