@@ -8,11 +8,6 @@
 extern "C" {
 #endif
 const char* srl_test_last_error(void);
-/* wgmma mainloop unit GEMMs (bf16 in, f32 out)
- * kmajor : D[M,N] = A[M,K] . B[N,K]^T   (K%64==0, N%64==0)
- * mnmajor: D[M,N] = At[K,M]^T . Bt[K,N] (M%128==0, N%64==0) */
-int srl_test_gemm_kmajor(const void* A, const void* B, float* D, int M, int N, int K, int simt, void* stream);
-int srl_test_gemm_mnmajor(const void* At, const void* Bt, float* D, int M, int N, int K, int simt, void* stream);
 /* descriptor experiment: operand windows that start at an arbitrary 128-byte row of a SWIZZLE_128B tile.
  * kmajor (mn_major=0): A bf16 [160,64], B bf16 [64,64]  -> D[128,64] = A[shift:shift+128] . B^T
  * mnmajor (=1)       : A bf16 [96,128], B bf16 [96,64]  -> D[128,64] = A[shift:shift+64]^T . B[shift:shift+64]   (shift <= 32) */

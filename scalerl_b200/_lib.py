@@ -80,8 +80,6 @@ _SIGS = {
 }
 # libscalerl_b200_testhooks.so (include/scalerl_b200_testhooks.h): unit-test entry points, loaded by tests only
 _HOOK_SIGS = {
-    'srl_test_gemm_kmajor': [_P, _P, _P, _I, _I, _I, _I, _P],
-    'srl_test_gemm_mnmajor': [_P, _P, _P, _I, _I, _I, _I, _P],
     'srl_test_shifted_operand': [_P, _P, _P, _I, _I, _I, _P],
     'srl_test_poison_smem': [_P],
     'srl_test_pdl': [_P, _P, _I, C.c_uint, _P],

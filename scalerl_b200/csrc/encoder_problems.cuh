@@ -1,15 +1,13 @@
-// Shared epilogue helpers (bf16 packing, ReLU masks) and the plain-GEMM problems with which the unit tests validate
-// the register-gather wgmma mainloop of igemm.cuh (K-major and MN-major descriptors) in isolation.
-// The encoder itself runs on the TMA kernels: res_problems.cuh (convs) and tma_problems.cuh (fc layer).
+// Helpers shared by the TMA GEMM problems (res_problems.cuh, tma_problems.cuh) and the fused encoder front (enc_fused.cuh):
+// bf16 packing, the u8 -> bf16 frame conversion and ReLU masks.
 #pragma once
-#include "igemm.cuh"
+#include "common.cuh"
 
 namespace srl {
 
 typedef __nv_bfloat16 bf16;
 
 SRL_DEVINL uint4 ldg16(const void* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
-SRL_DEVINL uint4 zero16() { return make_uint4(0, 0, 0, 0); }
 
 // 8 consecutive u8 (two aligned u32 words) -> 8 bf16 (exact: 0..255 fit the 8-bit significand)
 SRL_DEVINL uint4 u8x8_to_bf16x8(uint32_t w0, uint32_t w1) {
@@ -52,53 +50,5 @@ SRL_DEVINL void relu_mask16_pre(const uint4 (&m)[2], float (&v)[16]) {
   }
 }
 SRL_DEVINL void ld_mask16(const bf16* mask, uint4 (&m)[2]) { m[0] = ldg16(mask); m[1] = ldg16(mask + 8); }
-
-// ============================================================================================
-// plain GEMM problems used by the unit tests to validate descriptors / pipeline in isolation
-// ============================================================================================
-struct TestGemmK {    // D[M][N] = A[M][K] * B[N][K]^T, K % 64 == 0, N % 64 == 0; grid = (ceil(M/128), N/64)
-  static constexpr int BN = 64, STAGES = 3;
-  static constexpr bool A_MN = false, B_MN = false;
-  static constexpr int BIAS = 0, BIAS_N = 0;
-  struct Params { const bf16* A; const bf16* B; float* D; int M, N, K; };
-  typedef int RowA;
-  typedef int RowB;
-  SRL_DEVINL static int num_kblocks(const Params& p, int, int) { return p.K / 64; }
-  SRL_DEVINL static RowA make_rowA(const Params& p, int tm, int, int srow) { const int m = tm * 128 + srow; return m < p.M ? m : -1; }
-  SRL_DEVINL static RowB make_rowB(const Params&, int, int ty, int srow) { return ty * 64 + srow; }
-  SRL_DEVINL static uint4 load_A(const Params& p, RowA m, int kb, int chunk) {
-    return m < 0 ? zero16() : ldg16(p.A + (size_t)m * p.K + kb * 64 + chunk * 8);
-  }
-  SRL_DEVINL static uint4 load_B(const Params& p, RowB n, int kb, int chunk) { return ldg16(p.B + (size_t)n * p.K + kb * 64 + chunk * 8); }
-  SRL_DEVINL static void epilogue16(const Params& p, int tm, int ty, int row, int c0, float (&v)[16]) {
-    const int m = tm * 128 + row;
-    if (m >= p.M) return;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) p.D[(size_t)m * p.N + ty * 64 + c0 + j] = v[j];
-  }
-};
-struct TestGemmMN {   // D[M][N] = At[K][M]^T * Bt[K][N], M % 128 == 0, N % 64 == 0, any K; grid = (M/128, N/64)
-  static constexpr int BN = 64, STAGES = 3;
-  static constexpr bool A_MN = true, B_MN = true;
-  static constexpr int BIAS = 0, BIAS_N = 0;
-  struct Params { const bf16* At; const bf16* Bt; float* D; int M, N, K; };
-  typedef int RowA;
-  typedef int RowB;
-  SRL_DEVINL static int num_kblocks(const Params& p, int, int) { return (p.K + 63) / 64; }
-  SRL_DEVINL static RowA make_rowA(const Params&, int, int, int srow) { return srow; }
-  SRL_DEVINL static RowB make_rowB(const Params&, int, int, int srow) { return srow; }
-  SRL_DEVINL static uint4 load_A(const Params& p, RowA srow, int kb, int chunk) {
-    const int k = kb * 64 + (srow & 63);
-    return k < p.K ? ldg16(p.At + (size_t)k * p.M + blockIdx.x * 128 + (srow >> 6) * 64 + chunk * 8) : zero16();
-  }
-  SRL_DEVINL static uint4 load_B(const Params& p, RowB srow, int kb, int chunk) {
-    const int k = kb * 64 + srow;
-    return k < p.K ? ldg16(p.Bt + (size_t)k * p.N + blockIdx.y * 64 + chunk * 8) : zero16();
-  }
-  SRL_DEVINL static void epilogue16(const Params& p, int tm, int ty, int row, int c0, float (&v)[16]) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) p.D[(size_t)(tm * 128 + row) * p.N + ty * 64 + c0 + j] = v[j];
-  }
-};
 
 }  // namespace srl

@@ -11,7 +11,7 @@
 //              k-block's MMAs in flight and release its stage after issuing the next one)
 //
 // Shared-memory tiles are SWIZZLE_128B (the tensor maps are encoded with CU_TENSOR_MAP_SWIZZLE_128B, so the bytes
-// land exactly where the wgmma descriptors of igemm.cuh expect them).
+// land exactly where the wgmma descriptors of common.cuh's make_smem_desc expect them).
 //   K-major problems : A = 128 rows x 128 B (one row per output pixel, 64 contraction elements), 4 MMAs (K=16) per stage
 //   MN-major problems: A = 2 blocks x KROWS rows x 128 B, B = KROWS rows x 128 B (row = one contraction index = one
 //                      pixel/frame, 64 channels); KROWS/16 MMAs per stage.  Rows a box does not write stay zero

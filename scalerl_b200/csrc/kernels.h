@@ -202,6 +202,5 @@ cudaError_t encoder_backward(const uint8_t* obs, int frames, const EncoderBuffer
 cudaError_t test_shift(const void* A, const void* B, float* D, int shift, int mn_major, int bo_mode, cudaStream_t st);
 cudaError_t test_poison_smem(cudaStream_t st);
 cudaError_t test_pdl(int* flag, int* out, int nblk, unsigned delay_ns, cudaStream_t st);
-cudaError_t test_gemm(const void* A, const void* B, float* D, int M, int N, int K, bool mn_major, bool simt, cudaStream_t st);
 
 }  // namespace srl

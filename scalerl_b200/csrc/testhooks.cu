@@ -1,13 +1,12 @@
 // Test-only entry points (include/scalerl_b200_testhooks.h), built into libscalerl_b200_testhooks.so -- NOT part of the
-// product library.  They exercise the building blocks the product kernels rely on, in isolation: the wgmma mainloop
-// with K-major / MN-major SWIZZLE_128B descriptors, operand descriptors that start at an arbitrary 128-byte row of a
-// swizzled tile (the "resident window" trick of igemm_res.cuh), programmatic dependent launch, and a shared-memory
-// poisoner (kernels must never depend on stale shared memory).
+// product library.  They exercise the building blocks the product kernels rely on, in isolation: K-major / MN-major
+// SWIZZLE_128B wgmma operand descriptors that start at an arbitrary 128-byte row of a swizzled tile (the "resident
+// window" trick of igemm_res.cuh), programmatic dependent launch, and a shared-memory poisoner (kernels must never
+// depend on stale shared memory).
 #include <stdio.h>
 #include <stdarg.h>
 #include <stdlib.h>
 #include "../../include/scalerl_b200_testhooks.h"
-#include "encoder_problems.cuh"
 #include "kernels.h"
 
 using namespace srl;
@@ -36,23 +35,8 @@ bool pdl_active() {
   return env_on;
 }
 void pdl_set_active(bool) {}
-
-static inline int cdiv_(int a, int b) { return (a + b - 1) / b; }
-cudaError_t test_gemm(const void* A, const void* B, float* D, int M, int N, int K, bool mn_major, bool simt, cudaStream_t st) {
-  if (mn_major) {
-    TestGemmMN::Params q{(const bf16*)A, (const bf16*)B, D, M, N, K};
-    return igemm_launch<TestGemmMN>(q, dim3(M / 128, N / 64), st, simt);
-  }
-  TestGemmK::Params q{(const bf16*)A, (const bf16*)B, D, M, N, K};
-  return igemm_launch<TestGemmK>(q, dim3(cdiv_(M, 128), N / 64), st, simt);
-}
 }  // namespace srl
 
-extern "C" int srl_test_gemm_kmajor(const void* A, const void* B, float* D, int M, int N, int K, int simt, void* stream) {
-  REQ(A && B && D && M > 0 && N > 0 && K > 0 && K % 64 == 0 && N % 64 == 0, "test_gemm_kmajor: need K%%64==0, N%%64==0");
-  CU(test_gemm(A, B, D, M, N, K, false, simt != 0, (cudaStream_t)stream), "test_gemm_kmajor");
-  return 0;
-}
 extern "C" int srl_test_shifted_operand(const void* A, const void* B, float* D, int shift, int mn_major, int base_offset_mode, void* stream) {
   REQ(A && B && D && shift >= 0 && shift <= 32, "test_shifted_operand: bad argument");
   CU(test_shift(A, B, D, shift, mn_major, base_offset_mode, (cudaStream_t)stream), "test_shifted_operand");
@@ -65,11 +49,6 @@ extern "C" int srl_test_pdl(int* flag, int* out, int nblk, unsigned delay_ns, vo
 }
 extern "C" int srl_test_poison_smem(void* stream) {
   CU(test_poison_smem((cudaStream_t)stream), "test_poison_smem");
-  return 0;
-}
-extern "C" int srl_test_gemm_mnmajor(const void* At, const void* Bt, float* D, int M, int N, int K, int simt, void* stream) {
-  REQ(At && Bt && D && M > 0 && N > 0 && K > 0 && M % 128 == 0 && N % 64 == 0, "test_gemm_mnmajor: need M%%128==0, N%%64==0");
-  CU(test_gemm(At, Bt, D, M, N, K, true, simt != 0, (cudaStream_t)stream), "test_gemm_mnmajor");
   return 0;
 }
 

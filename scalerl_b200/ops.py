@@ -270,21 +270,3 @@ def impala_loss_and_head_grads(behavior_logits, target_logits, baseline, action,
         float(baseline_cost), float(entropy_cost), vs.data_ptr(), pg.data_ptr(), dlogits.data_ptr(), dbaseline.data_ptr(),
         losses.data_ptr(), scratch.data_ptr(), _stream()), 'impala_loss_and_head_grads')
     return dict(vs=vs, pg_advantages=pg, dlogits=dlogits, dbaseline=dbaseline, losses=losses)
-
-
-@torch.no_grad()
-def test_gemm(a, b, mn_major=False, simt=False):
-    """unit-test hook for the wgmma mainloop. kmajor: a [M,K], b [N,K]; mnmajor: a [K,M], b [K,N]. bf16 in, f32 out."""
-    a = a.contiguous()
-    b = b.contiguous()
-    if mn_major:
-        K, M = a.shape
-        N = b.shape[1]
-        fn = _lib.hooks().srl_test_gemm_mnmajor
-    else:
-        M, K = a.shape
-        N = b.shape[0]
-        fn = _lib.hooks().srl_test_gemm_kmajor
-    d = torch.empty(M, N, device=a.device, dtype=torch.float32)
-    _lib.check_hook(fn(a.data_ptr(), b.data_ptr(), d.data_ptr(), M, N, K, 1 if simt else 0, _stream()), 'test_gemm')
-    return d

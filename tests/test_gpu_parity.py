@@ -32,31 +32,6 @@ def dev(t):
 
 
 # ------------------------------------------------------------------------------------------------
-# wgmma mainloop in isolation
-# ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize('simt', [True, False])
-@pytest.mark.parametrize('M,N,K', [(128, 64, 64), (128, 64, 256), (300, 128, 576), (1000, 192, 3136)])
-def test_gemm_kmajor(ops, M, N, K, simt):
-    g = torch.Generator().manual_seed(M + N + K)
-    a = torch.randn(M, K, generator=g).bfloat16()
-    b = torch.randn(N, K, generator=g).bfloat16()
-    ref = a.float() @ b.float().t()
-    d = ops.test_gemm(dev(a), dev(b), mn_major=False, simt=simt)
-    assert_close(d, ref, 1e-5, f'gemm_k {M}x{N}x{K} simt={simt}')
-
-
-@pytest.mark.parametrize('simt', [True, False])
-@pytest.mark.parametrize('M,N,K', [(128, 64, 64), (128, 64, 100), (256, 128, 1000), (512, 192, 640)])
-def test_gemm_mnmajor(ops, M, N, K, simt):
-    g = torch.Generator().manual_seed(M + N + K + 1)
-    at = torch.randn(K, M, generator=g).bfloat16()
-    bt = torch.randn(K, N, generator=g).bfloat16()
-    ref = at.float().t() @ bt.float()
-    d = ops.test_gemm(dev(at), dev(bt), mn_major=True, simt=simt)
-    assert_close(d, ref, 1e-5, f'gemm_mn {M}x{N}x{K} simt={simt}')
-
-
-# ------------------------------------------------------------------------------------------------
 # V-trace
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize('variant', [0, 1])
