@@ -127,7 +127,8 @@ int srl_learner_set_config(srl_learner_t* L, const srl_config_t* cfg);
 
 /* run-time switches of one learner context: "column_fusion" (default 1; 0 = three kernels head_fwd / impala_tail / head_bwd
  * instead of the fused column kernel -- the environment variable SRL_NO_COLUMN_FUSION is read once, at creation);
- * "fused_fwd" (default 0, SRL_FUSED_FWD=1): u8 frame conversion + conv1 + conv2 as ONE persistent kernel (bf16 mode) instead of three. */
+ * "fused_fwd" (default 0, SRL_FUSED_FWD=1): u8 frame conversion + conv1 + conv2 as ONE persistent kernel (bf16 mode) instead of three;
+ * "lstm_step_ksplit" (1, 2, 3 or 6; default 3): thread-block cluster size over which srl_learner_forward_lstm_step splits K. */
 int srl_learner_set_option(srl_learner_t* L, const char* name, int value);
 
 /* optimizer step count (Adam's bias-correction t; torch.optim state['step']): restore it when resuming from a checkpoint
@@ -135,7 +136,8 @@ int srl_learner_set_option(srl_learner_t* L, const char* name, int value);
 int srl_learner_set_step(srl_learner_t* L, int64_t step, void* stream);
 int64_t srl_learner_get_step(srl_learner_t* L, void* stream);
 
-/* re-derive the packed bf16 operand copies from the fp32 master parameters now (optional: every forward does it) */
+/* re-derive the packed bf16 operand copies from the fp32 master parameters now (optional: every forward does it).  With
+ * use_lstm it also packs the [W_ih | W_hh] copy that srl_learner_forward_lstm_step reads, which only this call writes. */
 int srl_learner_pack_weights(srl_learner_t* L, void* stream);
 
 /* AtariNet.forward for n_rows*B frames: obs u8 [rows,B,4,84,84], reward f32 [rows,B], action i64 [rows,B]
@@ -156,6 +158,16 @@ int srl_learner_forward_lstm(srl_learner_t* L, const uint8_t* obs, const float* 
 int srl_learner_forward_backward_lstm(srl_learner_t* L, const uint8_t* obs, const float* reward, const uint8_t* done,
                                       const int64_t* action, const float* behavior_logits, const float* h0, const float* c0,
                                       float* losses, float* vs, float* pg_advantages, void* stream);
+
+/* One actor step of AtariNet(use_lstm=True) for the context's B environments (atari_model.py:91-143 with T = 1):
+ * obs u8 [B,4,84,84], reward f32 [B], done u8 [B], action i64 [B], h_in/c_in f32 [2,B,H] -> policy_logits f32 [B,A],
+ * baseline f32 [B], h_out/c_out f32 [2,B,H] (must not alias h_in/c_in).  The state is reset by done before the step.
+ * H = 513 + A.  The LSTM weights are those of the last srl_learner_pack_weights (load them, then pack: the step reads a
+ * packed bf16 copy that no forward re-derives); the biases are read from the fp32 parameters at call time.  Bad pointers are
+ * rejected (SRL_EINVAL) before the context is used; a context without use_lstm is rejected too.  bf16 operands only. */
+int srl_learner_forward_lstm_step(srl_learner_t* L, const uint8_t* obs, const float* reward, const uint8_t* done,
+                                  const int64_t* action, const float* h_in, const float* c_in, float* policy_logits,
+                                  float* baseline, float* h_out, float* c_out, void* stream);
 
 /* The same step in two halves, for overlapping the gradient all-reduce with the backward pass:
  *   _begin : forward + V-trace/loss + head backward + the fc layer's backward.  On return (in stream order) the
@@ -193,7 +205,9 @@ int srl_learner_apply_gradients_dp(srl_learner_t* L, const srl_dp_peers_t* peers
 int srl_learner_snapshot_params(srl_learner_t* L, float* dst, const float* losses, void* stream);
 
 /* borrow internal activations / operand copies for tests: name in {"a1","a2","a3","h","logits","baseline",
- * "dlogits","dbaseline","dh","da3","da2","da1","wpack"}; returns device pointer + element count. */
+ * "dlogits","dbaseline","dh","da3","da2","da1","wpack"}; returns device pointer + element count.  use_lstm contexts add the
+ * actor step's bf16 operands: "lstm_step_xh" [2][B][2Hp] (per layer [x | m.h] of the last step, Hp = 576) and "lstm_step_w"
+ * [2][4Hp][2Hp] (per layer [W_ih | W_hh], rows interleaved so one 128-row tile holds the 4 gates of 32 units; csrc/lstm.cu). */
 int srl_learner_debug_buffer(srl_learner_t* L, const char* name, void** ptr, int64_t* count);
 
 /* per-kernel timing of one learner step: when enabled every kernel launch of forward_backward /

@@ -50,6 +50,7 @@ _SIGS = {
     'srl_learner_backward_finish': [_P, _P, _P],
     'srl_learner_forward_lstm': [_P] * 12,
     'srl_learner_forward_backward_lstm': [_P] * 12,
+    'srl_learner_forward_lstm_step': [_P] * 12,
     'srl_learner_apply_gradients': [_P, _P, _P],
     'srl_learner_apply_gradients_dp': [_P, _P, _P, _P],
     'srl_learner_debug_buffer': [_P, C.c_char_p, C.POINTER(_P), C.POINTER(_L)],

@@ -250,12 +250,15 @@ class ImpalaTrainer:
                 indices = [free_queue.get() for _ in range(num_envs)]
                 if any(i is None for i in indices):
                     break
+                state = agent_state
+                if len(state) and state[0].is_cuda:       # a device-resident state (GPU actor): one D2H per rollout, not one per environment
+                    state = torch.stack(state).cpu().unbind(0)
                 for e, index in enumerate(indices):
                     for key in env_output:
                         buffers[key][index][0, ...] = env_output[key][0, e]
                     for key in agent_output:
                         buffers[key][index][0, ...] = agent_output[key][0, e]
-                    for i, tensor in enumerate(agent_state):
+                    for i, tensor in enumerate(state):
                         rnn_state_buffers[index][i][...] = tensor[:, e:e + 1]
                 for t in range(T):
                     with torch.no_grad():

@@ -194,6 +194,8 @@ struct srl_learner {
   float *core, *lstm_out, *dout, *dcore;   // [NF][H], [NF][H], [NB][H], [NB][H]
   char* lstm_arena;
   int64_t lstm_off0, lstm_len;    // LSTM gradient range inside the flat buffer
+  LstmStep* lstm_step;            // use_lstm: the one-row actor step (packed weights + operands; csrc/lstm.cu)
+  int lstm_step_ksplit;           // K split of its GEMM (cluster size; srl_learner_set_option "lstm_step_ksplit")
   bool fused_front;               // frame conversion + conv1 + conv2 as one kernel (SRL_FUSED_FWD / srl_learner_set_option "fused_fwd")
   bool column_fusion;             // heads + V-trace/loss + dh in one column kernel (SRL_NO_COLUMN_FUSION / srl_learner_set_option)
   Profiler pf;                    // per-kernel event bracketing (off by default)
@@ -231,6 +233,7 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
   L->nparams = layout_ex(cfg->A, cfg->use_lstm, nullptr, nullptr);
   L->lo_arena = nullptr;
   L->lstm = nullptr; L->lstm_arena = nullptr; L->core = L->lstm_out = L->dout = L->dcore = nullptr; L->lstm_off0 = L->lstm_len = 0;
+  L->lstm_step = nullptr; L->lstm_step_ksplit = LSTM_STEP_KSPLIT;
   L->P = make_ptrs(params, cfg->A);
   L->G = make_ptrs(grads, cfg->A);
   L->step = 0; L->have_fwd = false;
@@ -352,11 +355,14 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
       L->core = q2; q2 += NF * H; L->lstm_out = q2; q2 += NF * H; L->dout = q2; q2 += NB * H; L->dcore = q2;
       ok = srl_lstm_create(cfg->T + 1, cfg->B, H, wp, gp, &L->lstm) == 0;
     }
+    const char* why = srl_lstm_last_error();
+    if (ok && lstm_step_create(cfg->B, H, wp, &L->lstm_step, &why) != cudaSuccess) ok = false;
     if (!ok) {
+      if (L->lstm) srl_lstm_destroy(L->lstm);
       if (L->lstm_arena) cudaFree(L->lstm_arena);
       cudaFree(L->arena);
       delete L;
-      return fail(SRL_ESTATE, "learner_create: LSTM core allocation failed: %s", srl_lstm_last_error());
+      return fail(SRL_ESTATE, "learner_create: LSTM core allocation failed: %s", why);
     }
   }
   *out = L;
@@ -372,6 +378,7 @@ extern "C" int srl_learner_destroy(srl_learner_t* L) {
   if (L->ss.side3) cudaStreamDestroy(L->ss.side3);
   if (L->ss.pack) cudaStreamDestroy(L->ss.pack);
   if (L->lstm) srl_lstm_destroy(L->lstm);
+  lstm_step_destroy(L->lstm_step);
   if (L->lstm_arena) cudaFree(L->lstm_arena);
   if (L->lo_arena) cudaFree(L->lo_arena);
   cudaFree(L->arena);
@@ -405,6 +412,11 @@ extern "C" int srl_learner_set_option(srl_learner_t* L, const char* name, int va
   REQ(L && name, "set_option: NULL argument");
   if (strcmp(name, "column_fusion") == 0) { L->column_fusion = value != 0; return 0; }
   if (strcmp(name, "fused_fwd") == 0) { L->fused_front = value != 0; return 0; }
+  if (strcmp(name, "lstm_step_ksplit") == 0) {
+    REQ(lstm_step_ksplit_supported(value), "set_option: lstm_step_ksplit=%d must be 1, 2, 3 or 6", value);
+    L->lstm_step_ksplit = value;
+    return 0;
+  }
   return fail(SRL_EINVAL, "set_option: unknown option '%s'", name);
 }
 
@@ -427,6 +439,8 @@ extern "C" int64_t srl_learner_get_step(srl_learner_t* L, void* stream) {
 extern "C" int srl_learner_pack_weights(srl_learner_t* L, void* stream) {
   REQ(L, "learner is NULL");
   CU(launch_pack_weights(L->P, L->buf.wpack, (cudaStream_t)stream, L->buf.wpack_lo), "pack_weights");
+  // the actor step's [W_ih | W_hh] copy: packed here, once per weight version, and never by the learner's own forward
+  if (L->lstm_step) CU(lstm_step_pack(L->lstm_step, (cudaStream_t)stream), "lstm_step_pack");
   return 0;
 }
 
@@ -594,6 +608,36 @@ extern "C" int srl_learner_forward_lstm(srl_learner_t* L, const uint8_t* obs, co
   return forward_lstm_impl(L, obs, reward, done, action, h0, c0, policy_logits, baseline, hT, cT, (cudaStream_t)stream);
 }
 
+static bool overlaps(const void* a, const void* b, int64_t bytes) {
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return x < y + (uintptr_t)bytes && y < x + (uintptr_t)bytes;
+}
+
+extern "C" int srl_learner_forward_lstm_step(srl_learner_t* L, const uint8_t* obs, const float* reward, const uint8_t* done,
+                                             const int64_t* action, const float* h_in, const float* c_in, float* policy_logits,
+                                             float* baseline, float* h_out, float* c_out, void* stream) {
+  // the pointer checks come before any use of the context
+  REQ(obs && reward && done && action && h_in && c_in && policy_logits && baseline && h_out && c_out, "learner_forward_lstm_step: NULL pointer");
+  REQ(h_out != h_in && h_out != c_in && c_out != h_in && c_out != c_in && h_out != c_out,
+      "learner_forward_lstm_step: h_out / c_out must not alias h_in, c_in or each other");
+  REQ(L, "learner_forward_lstm_step: learner is NULL");
+  REQ(L->cfg.use_lstm && L->lstm_step, "learner_forward_lstm_step: this learner was created with use_lstm=0");
+  REQ(L->cfg.precision == 0, "learner_forward_lstm_step: the step runs bf16 operands only (precision = 0)");
+  const srl_config_t& c = L->cfg;
+  const int B = c.B, H = 513 + c.A;
+  const int64_t sb = (int64_t)2 * B * H * 4;
+  REQ(!overlaps(h_out, h_in, sb) && !overlaps(h_out, c_in, sb) && !overlaps(c_out, h_in, sb) && !overlaps(c_out, c_in, sb) &&
+      !overlaps(h_out, c_out, sb), "learner_forward_lstm_step: h_out / c_out must not alias h_in, c_in or each other");
+  REQ((reinterpret_cast<uintptr_t>(obs) & 3) == 0, "learner_forward_lstm_step: obs must be 4-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = encode_impl(L, obs, B, st);
+  if (rc) return rc;
+  CU(launch_core_build(L->buf.hpart, FC_SPLITS, L->P.bf, reward, action, B, c.A, L->buf.h, L->core, st), "core_build");
+  CU(lstm_step_forward(L->lstm_step, L->core, done, h_in, c_in, h_out, c_out, L->lstm_step_ksplit, st), "lstm_step");
+  CU(launch_head_dense_fwd(h_out + (size_t)B * H, L->P.wp, L->P.bp, L->P.wb, L->P.bb, B, c.A, policy_logits, baseline, st), "head_dense_fwd");
+  return 0;
+}
+
 extern "C" int srl_learner_forward_backward_lstm(srl_learner_t* L, const uint8_t* obs, const float* reward, const uint8_t* done,
                                                  const int64_t* action, const float* behavior_logits, const float* h0, const float* c0,
                                                  float* losses, float* vs, float* pg_advantages, void* stream) {
@@ -734,6 +778,14 @@ extern "C" int srl_memcpy_d2d(void* dst, const void* src, int64_t bytes, void* s
 extern "C" int srl_learner_debug_buffer(srl_learner_t* L, const char* name, void** ptr, int64_t* count) {
   REQ(L && name && ptr && count, "debug_buffer: NULL argument");
   const int64_t NF = (int64_t)(L->cfg.T + 1) * L->cfg.B, NB = (int64_t)L->cfg.T * L->cfg.B, A = L->cfg.A;
+  if (strncmp(name, "lstm_step_", 10) == 0) {     // the actor step's bf16 operands: xh [2][B][2Hp] = [x | m.h], w [2][4Hp][2Hp]
+    REQ(L->lstm_step, "debug_buffer: '%s' exists only with use_lstm = 1", name);
+    void *xh, *w;
+    int64_t nxh, nw;
+    lstm_step_buffers(L->lstm_step, &xh, &nxh, &w, &nw);
+    if (strcmp(name, "lstm_step_xh") == 0) { *ptr = xh; *count = nxh; return 0; }
+    if (strcmp(name, "lstm_step_w") == 0) { *ptr = w; *count = nw; return 0; }
+  }
   struct { const char* n; void* p; int64_t c; } tab[] = {
       {"xs", L->buf.xs, NF * 441 * 64}, {"a1", L->buf.a1, NF * 400 * 32}, {"a2", L->buf.a2, NF * 81 * 64}, {"a3", L->buf.a3, NF * 49 * 64}, {"a3t", L->buf.a3t, NF * 49 * 64}, {"h", L->buf.h, NF * 512},
       {"logits", L->logits, NF * A}, {"baseline", L->baseline, NF}, {"dlogits", L->dlogits, NB * A}, {"dbaseline", L->dbaseline, NB},

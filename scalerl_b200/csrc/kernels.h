@@ -199,6 +199,18 @@ cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, 
 //        bytes, ready for an early all-reduce), 1 = conv layers only, 2 = both
 cudaError_t encoder_backward(const uint8_t* obs, int frames, const EncoderBuffers& buf, const ParamPtrs& g, const TmaMaps& maps, int mode,
                              cudaStream_t st, const Profiler& pf, const SideStream& ss, int phase, const TmaMapsLo* maps_lo = nullptr);
+// ---- lstm.cu: the actor step of the 2-layer LSTM core (one row of B environments, no BPTT)
+struct LstmStep;
+// weights8: the 8 nn.LSTM tensors of the flat parameter buffer (srl_lstm_create order); H = 513 + A
+cudaError_t lstm_step_create(int B, int H, const float* const* weights8, LstmStep** out, const char** why);
+void lstm_step_destroy(LstmStep* S);
+cudaError_t lstm_step_pack(LstmStep* S, cudaStream_t st);           // packed [W_ih | W_hh] bf16 copy of both layers from the fp32 parameters
+bool lstm_step_ksplit_supported(int ks);                            // K split (cluster size) of the step GEMM: 1, 2, 3 or 6
+constexpr int LSTM_STEP_KSPLIT = 3;                                 // default split (DESIGN.md §4: measured per N on H100)
+// core f32 [B][H], done u8 [B], h_in/c_in f32 [2][B][H] -> h_out/c_out f32 [2][B][H]; uses the weights of the last lstm_step_pack
+cudaError_t lstm_step_forward(LstmStep* S, const float* core, const uint8_t* done, const float* h_in, const float* c_in, float* h_out,
+                              float* c_out, int ksplit, cudaStream_t st);
+void lstm_step_buffers(const LstmStep* S, void** xh, int64_t* nxh, void** w, int64_t* nw);   // debug views of the bf16 operands
 cudaError_t test_shift(const void* A, const void* B, float* D, int shift, int mn_major, int bo_mode, cudaStream_t st);
 cudaError_t test_poison_smem(cudaStream_t st);
 cudaError_t test_pdl(int* flag, int* out, int nblk, unsigned delay_ns, cudaStream_t st);

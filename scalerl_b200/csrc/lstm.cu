@@ -10,6 +10,7 @@
 //   * after the scan: dX (one GEMM), dWih / dWhh (two MN-major GEMMs over all T*B rows), bias gradients (column sums)
 // H = 513 + A is padded to Hp (multiple of 64); the gate dimension is laid out [4][Hp] so every GEMM has K = Hp or 4Hp.
 // All GEMM operands are bf16 (fp32 accumulate); cell state, gate activations and gradients are fp32.
+// The actor's single step (one row of B environments, no BPTT) has its own fused kernel further down (lstm_step_kernel).
 #include <stdio.h>
 #include <new>
 #include "tma_problems.cuh"
@@ -178,6 +179,207 @@ __global__ void lstm_unpad_rows_kernel(const float* __restrict__ src, int rows, 
   dst[i] = src[(size_t)r * Hp + j];
 }
 
+// ------------------------------------------------------------------------------------------------ actor step (one row, no BPTT)
+// One environment step of both layers for the N environments of an actor call.  Per layer, ONE swap-AB wgmma GEMM
+//   gates^T [4Hp x N] = Wl [4Hp x 2Hp] . [x | m.h]^T [2Hp x N]      (Wl = [W_ih | W_hh], bf16; fp32 accumulate)
+// with the LSTM cell in the epilogue: the gate pre-activations never leave the CTA.
+//   * M = the 4Hp = 2304 gate rows of the packed weights (operand A, TMA); N = environments (operand B, TMA; rows past N are
+//     zero-filled by the TMA unit); K = 2Hp = 1152.
+//   * Row interleave of the packed weights: a 128-row M tile holds the 4 gates of 32 hidden units, placed so that the
+//     wgmma accumulator fragment gives every thread all 4 gates of ONE unit for each of its columns (common.cuh fragment:
+//     thread (w, l) of the warpgroup holds rows 16w + l/4 + 8rr of both m64 halves h):
+//         tile row R(u, q) = 64 (q >> 1) + 16 (u >> 3) + 8 (q & 1) + (u & 7),   unit j = 32 tm + u,  gate q = 2h + rr.
+//   * K split over a thread-block cluster of KS CTAs (grid.z): CTA rank r multiplies k-blocks [r, r+1) * 18/KS, stores its
+//     partial accumulators in its own shared memory, and after a cluster barrier every rank reduces a 1/KS share of the
+//     columns over distributed shared memory, always adding the ranks in order 0..KS-1 (the result does not depend on
+//     which CTA reduces), then runs the cell for that share.
+// bf16 rounding points are those of the rollout path: x = bf16(core) / bf16(h of layer 0), m.h = bf16(m * h) (lstm_pad_bf16_kernel,
+// lstm_init_hm_kernel, lstm_cell_fwd_kernel), so an actor step and the learner's row differ only in summation order.
+constexpr int LS_HP = 576;                       // Hp for every A in [1, 31]: H = 513 + A in [514, 544]
+constexpr int LS_G = 4 * LS_HP, LS_K = 2 * LS_HP, LS_KB = LS_K / 64;      // 2304 gate rows, K = 1152, 18 k-blocks
+constexpr int LS_BN = 128;                       // environments per CTA: two consumer warpgroups x 64 columns
+constexpr int LS_STAGES = 4, LS_TILE = 128 * 128, LS_STAGE = 2 * LS_TILE;
+constexpr int LS_PART = 64 * 256 * 4;            // K-split partials: 64 accumulators x 256 consumer threads
+constexpr int LS_THREADS = 288;
+constexpr int LS_SMEM = LS_STAGES * LS_STAGE + LS_PART + 256 + 1024;
+
+struct LstmStepParams {
+  SRL_TMAP w;                  // packed weights of both layers [2 * 4Hp][2Hp] bf16, box 64 x 128
+  SRL_TMAP xh;                 // this layer's operand [N][2Hp] bf16 = [x | m.h], box 64 x 128
+  const float *b_ih, *b_hh;    // this layer's biases, PyTorch layout [4H]
+  const float* c_in;           // [N][H] (this layer's slice of c_in [2][N][H])
+  const uint8_t* done;         // [N]
+  float *c_out, *h_out;        // [N][H]
+  __nv_bfloat16* x_next;       // layer 0: the x part of layer 1's operand (row stride 2Hp); layer 1: nullptr
+  int N, H, w_row0;            // w_row0: first packed row of this layer
+};
+
+SRL_DEVINL uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+SRL_DEVINL void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+SRL_DEVINL float ld_dsmem_f32(uint32_t saddr, uint32_t rank) {
+  uint32_t remote;
+  float v;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(saddr), "r"(rank));
+  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
+  return v;
+}
+
+// the cell for environment n, hidden unit j: acc = the 4 gate products (i, f, g, o) without biases; bias = {b_ih, b_hh} per gate
+SRL_DEVINL void lstm_step_cell(const LstmStepParams& p, int n, int j, const float (&acc)[4], const float (&bias)[8]) {
+  if (n >= p.N || j >= p.H) return;
+  float pre[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) pre[q] = acc[q] + bias[2 * q] + bias[2 * q + 1];
+  const float a0 = sigmoidf_(pre[0]), a1 = sigmoidf_(pre[1]), a2 = tanhf(pre[2]), a3 = sigmoidf_(pre[3]);
+  const size_t o = (size_t)n * p.H + j;
+  const float cp = p.done[n] ? 0.f : p.c_in[o];
+  const float cv = a1 * cp + a0 * a2;
+  const float hv = a3 * tanhf(cv);
+  p.c_out[o] = cv;
+  p.h_out[o] = hv;
+  if (p.x_next) p.x_next[(size_t)n * LS_K + j] = __float2bfloat16_rn(hv);
+}
+
+template <int KS>
+__global__ void __cluster_dims__(1, 1, KS) __launch_bounds__(LS_THREADS) lstm_step_kernel(const __grid_constant__ LstmStepParams p) {
+  static_assert(LS_KB % KS == 0, "the K split must divide the 18 k-blocks");
+  constexpr int NKB = LS_KB / KS;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  float* part = reinterpret_cast<float*>(smem + LS_STAGES * LS_STAGE);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + LS_STAGES * LS_STAGE + LS_PART);
+  uint64_t* empty = full + LS_STAGES;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tm = blockIdx.x, tn = blockIdx.y;
+  const uint32_t rank = KS > 1 ? cluster_ctarank() : 0;
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < LS_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    mbar_fence_init();
+    tma_prefetch_desc(&p.w); tma_prefetch_desc(&p.xh);
+  }
+  __syncthreads();
+  pdl_wait();                          // the operands (previous layer / prep kernel) and the state are complete from here on
+  if (tid == 256) pdl_launch();
+  const int kb0 = (int)rank * NKB;
+  const int g = warp >> 2, wt = tid & 127, w = wt >> 5;
+  const int j = tm * 32 + 8 * w + (lane >> 2);            // this thread's hidden unit
+  const int col0 = tn * LS_BN + g * 64 + 2 * (lane & 3);    // its first environment; + 8 j8 + e
+  if (warp == 8) {
+    const uint32_t leader = elect_one_sync();
+    for (int kb = 0; kb < NKB; ++kb) {
+      const int s = kb % LS_STAGES;
+      mbar_wait(&empty[s], ((kb / LS_STAGES) & 1) ^ 1);
+      if (leader) {
+        uint8_t* sA = smem + s * LS_STAGE;
+        mbar_arrive_expect_tx(&full[s], LS_STAGE);
+        tma_load_2d(sA, &p.w, &full[s], (kb0 + kb) * 64, p.w_row0 + tm * 128);
+        tma_load_2d(sA + LS_TILE, &p.xh, &full[s], (kb0 + kb) * 64, tn * LS_BN);
+      }
+      __syncwarp();
+    }
+  } else {
+    float acc[2][32];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+    for (int kb = 0; kb < NKB; ++kb) {
+      const int s = kb % LS_STAGES;
+      mbar_wait(&full[s], (kb / LS_STAGES) & 1);
+      const uint32_t a0 = smem_u32(smem + s * LS_STAGE);
+      const uint64_t ad0 = make_smem_desc(a0, 16, 1024), bd0 = make_smem_desc(a0 + LS_TILE + g * 64 * 128, 16, 1024);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wg_mma128<64, 0, 0>(acc, ad0 + (uint64_t)(2 * k), 64 * 128 / 16, bd0 + (uint64_t)(2 * k), (kb | k) != 0);
+      wg_commit();
+      wg_wait_prev();
+      __syncwarp();
+      if (kb > 0 && lane == 0) mbar_arrive(&empty[(kb - 1) % LS_STAGES]);
+    }
+    wg_wait_all();
+    wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
+    if constexpr (KS == 1) {
+      float bias[8];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        bias[2 * q] = j < p.H ? __ldg(p.b_ih + q * p.H + j) : 0.f;
+        bias[2 * q + 1] = j < p.H ? __ldg(p.b_hh + q * p.H + j) : 0.f;
+      }
+#pragma unroll
+      for (int j8 = 0; j8 < 8; ++j8)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float a4[4] = {acc[0][4 * j8 + e], acc[0][4 * j8 + 2 + e], acc[1][4 * j8 + e], acc[1][4 * j8 + 2 + e]};
+          lstm_step_cell(p, col0 + 8 * j8 + e, j, a4, bias);
+        }
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) part[(h * 32 + i) * 256 + g * 128 + wt] = acc[h][i];
+    }
+  }
+  if constexpr (KS > 1) {
+    cluster_sync_all();                  // every rank's partials are in its shared memory
+    if (warp < 8) {
+      float bias[8];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        bias[2 * q] = j < p.H ? __ldg(p.b_ih + q * p.H + j) : 0.f;
+        bias[2 * q + 1] = j < p.H ? __ldg(p.b_hh + q * p.H + j) : 0.f;
+      }
+      const uint32_t base = smem_u32(part) + (uint32_t)(g * 128 + wt) * 4;
+#pragma unroll
+      for (int j8 = 0; j8 < 8; ++j8) {
+        if (j8 % KS != (int)rank) continue;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float a4[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const uint32_t addr = base + (uint32_t)(((q >> 1) * 32 + 4 * j8 + 2 * (q & 1) + e) * 256) * 4;
+            float s = ld_dsmem_f32(addr, 0);
+#pragma unroll
+            for (int r = 1; r < KS; ++r) s += ld_dsmem_f32(addr, r);
+            a4[q] = s;
+          }
+          lstm_step_cell(p, col0 + 8 * j8 + e, j, a4, bias);
+        }
+      }
+    }
+    cluster_sync_all();                  // no CTA leaves while a peer still reads its partials
+  }
+}
+
+// step operands of layer 0 and the recurrent halves of both layers: xh[l][n] = [x | bf16(m_n h_l[n])], x = bf16(core[n]) (layer 0)
+__global__ void lstm_step_prep_kernel(const float* __restrict__ core, const uint8_t* __restrict__ done, const float* __restrict__ h_in, int N, int H,
+                                      __nv_bfloat16* __restrict__ xh) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N * LS_HP) return;
+  const int n = i / LS_HP, j = i - n * LS_HP;
+  const float m = done[n] ? 0.f : 1.f;
+  __nv_bfloat16* r0 = xh + (size_t)n * LS_K;
+  __nv_bfloat16* r1 = xh + ((size_t)N + n) * LS_K;
+  r0[j] = __float2bfloat16_rn(j < H ? core[(size_t)n * H + j] : 0.f);
+  r0[LS_HP + j] = __float2bfloat16_rn(j < H ? m * h_in[(size_t)n * H + j] : 0.f);
+  r1[LS_HP + j] = __float2bfloat16_rn(j < H ? m * h_in[((size_t)N + n) * H + j] : 0.f);
+}
+
+// packed step weights [2][4Hp][2Hp] bf16: row (layer, tile, R) = [W_ih | W_hh] row q H + j of that layer (interleave above), zero padded
+__global__ void lstm_step_pack_kernel(const float* __restrict__ wih0, const float* __restrict__ whh0, const float* __restrict__ wih1,
+                                      const float* __restrict__ whh1, int H, __nv_bfloat16* __restrict__ wp) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)2 * LS_G * LS_K) return;
+  const int row = (int)(i / LS_K), k = (int)(i - (int64_t)row * LS_K);
+  const int l = row / LS_G, R = row - l * LS_G, tile = R >> 7, r = R & 127;
+  const int u = 8 * ((r >> 4) & 3) + (r & 7), q = 2 * (r >> 6) + ((r >> 3) & 1), j = 32 * tile + u;
+  const int kk = k < LS_HP ? k : k - LS_HP;
+  const float* src = k < LS_HP ? (l ? wih1 : wih0) : (l ? whh1 : whh0);
+  wp[i] = __float2bfloat16_rn(j < H && kk < H ? src[(size_t)(q * H + j) * H + kk] : 0.f);
+}
+
 }  // namespace srl
 
 using namespace srl;
@@ -338,3 +540,84 @@ extern "C" int srl_lstm_backward(srl_lstm_t* L, const float* dout, const uint8_t
   LCU(cudaGetLastError(), "lstm backward");
   return 0;
 }
+
+// ------------------------------------------------------------------------------------------------ actor step: host side
+namespace srl {
+struct LstmStep {
+  int B, H;
+  const float* w[2][4];               // weight_ih, weight_hh, bias_ih, bias_hh per layer (fp32, caller-owned)
+  __nv_bfloat16 *wp, *xh;             // packed weights [2][4Hp][2Hp]; operands [2][B][2Hp]
+  alignas(64) CUtensorMap m_w, m_xh[2];
+};
+
+cudaError_t lstm_step_create(int B, int H, const float* const* weights8, LstmStep** out, const char** why) {
+  *out = nullptr;
+  if (B < 1 || H < 1 || (H + 63) / 64 * 64 != LS_HP) { *why = "lstm_step: H must be 513 + A with A in [1, 31]"; return cudaErrorInvalidValue; }
+  LstmStep* S = new (std::nothrow) LstmStep();
+  if (!S) { *why = "out of host memory"; return cudaErrorMemoryAllocation; }
+  S->B = B; S->H = H;
+  for (int l = 0; l < 2; ++l) for (int k = 0; k < 4; ++k) S->w[l][k] = weights8[4 * l + k];
+  const size_t wbytes = (size_t)2 * LS_G * LS_K * 2, xbytes = (size_t)2 * B * LS_K * 2;
+  char* a = nullptr;
+  cudaError_t e = cudaMalloc(&a, wbytes + xbytes);
+  if (e == cudaSuccess) e = cudaMemset(a, 0, wbytes + xbytes);      // the operands' padding columns stay zero from here on
+  if (e != cudaSuccess) { if (a) cudaFree(a); delete S; *why = "lstm_step: cudaMalloc failed"; return e; }
+  S->wp = (__nv_bfloat16*)a; S->xh = (__nv_bfloat16*)(a + wbytes);
+  const uint64_t dw[2] = {LS_K, 2 * LS_G}, dx[2] = {LS_K, (uint64_t)B}, st[1] = {LS_K};
+  const uint32_t box[2] = {64, 128};
+  if (!make_map(&S->m_w, S->wp, 2, dw, st, box) || !make_map(&S->m_xh[0], S->xh, 2, dx, st, box) ||
+      !make_map(&S->m_xh[1], S->xh + (size_t)B * LS_K, 2, dx, st, box)) {
+    cudaFree(a); delete S; *why = "lstm_step: tensor map creation failed"; return cudaErrorInvalidValue;
+  }
+  *out = S;
+  return cudaSuccess;
+}
+void lstm_step_destroy(LstmStep* S) { if (S) { cudaFree(S->wp); delete S; } }
+
+cudaError_t lstm_step_pack(LstmStep* S, cudaStream_t st) {
+  lstm_step_pack_kernel<<<cdiv_((int64_t)2 * LS_G * LS_K, 256), 256, 0, st>>>(S->w[0][0], S->w[0][1], S->w[1][0], S->w[1][1], S->H, S->wp);
+  return cudaGetLastError();
+}
+
+template <int KS>
+static cudaError_t launch_step_layer(const LstmStepParams& p, int ntiles, cudaStream_t st) {
+  static PerDeviceOnce once;
+  cudaError_t e = ensure_max_dynamic_smem(once, lstm_step_kernel<KS>, LS_SMEM);
+  if (e != cudaSuccess) return e;
+  return launch_chain(lstm_step_kernel<KS>, dim3(LS_G / 128, ntiles, KS), dim3(LS_THREADS), LS_SMEM, st, p);
+}
+
+bool lstm_step_ksplit_supported(int ks) { return ks == 1 || ks == 2 || ks == 3 || ks == 6; }
+
+cudaError_t lstm_step_forward(LstmStep* S, const float* core, const uint8_t* done, const float* h_in, const float* c_in, float* h_out,
+                              float* c_out, int ksplit, cudaStream_t st) {
+  const int B = S->B, H = S->H;
+  lstm_step_prep_kernel<<<cdiv_((int64_t)B * LS_HP, 256), 256, 0, st>>>(core, done, h_in, B, H, S->xh);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  for (int l = 0; l < 2; ++l) {
+    LstmStepParams p;
+    p.w = S->m_w; p.xh = S->m_xh[l];
+    p.b_ih = S->w[l][2]; p.b_hh = S->w[l][3];
+    p.c_in = c_in + (size_t)l * B * H; p.done = done;
+    p.c_out = c_out + (size_t)l * B * H; p.h_out = h_out + (size_t)l * B * H;
+    p.x_next = l == 0 ? S->xh + (size_t)B * LS_K : nullptr;
+    p.N = B; p.H = H; p.w_row0 = l * LS_G;
+    const int nt = cdiv_(B, LS_BN);
+    switch (ksplit) {
+      case 1: e = launch_step_layer<1>(p, nt, st); break;
+      case 2: e = launch_step_layer<2>(p, nt, st); break;
+      case 3: e = launch_step_layer<3>(p, nt, st); break;
+      case 6: e = launch_step_layer<6>(p, nt, st); break;
+      default: e = cudaErrorInvalidValue;
+    }
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+
+void lstm_step_buffers(const LstmStep* S, void** xh, int64_t* nxh, void** w, int64_t* nw) {
+  *xh = S ? S->xh : nullptr; *nxh = S ? (int64_t)2 * S->B * LS_K : 0;
+  *w = S ? S->wp : nullptr; *nw = (int64_t)2 * LS_G * LS_K;
+}
+}  // namespace srl
