@@ -204,8 +204,10 @@ int srl_learner_apply_gradients_dp(srl_learner_t* L, const srl_dp_peers_t* peers
  * `dst` to the actors' host memory asynchronously while the next step already updates the live parameters. */
 int srl_learner_snapshot_params(srl_learner_t* L, float* dst, const float* losses, void* stream);
 
-/* borrow internal activations / operand copies for tests: name in {"a1","a2","a3","h","logits","baseline",
- * "dlogits","dbaseline","dh","da3","da2","da1","wpack"}; returns device pointer + element count.  use_lstm contexts add the
+/* borrow internal activations / operand copies for tests: name in {"xs","a1","a2","a3","a3t","h","logits","baseline",
+ * "dlogits","dbaseline","dh","da3","da2","da1","wpack"}; returns device pointer + element count.  The fp32-accurate operand mode
+ * (precision = 1) adds the low twins "a1_lo","a2_lo","a3_lo","dh_lo","da3_lo","da2_lo","da1_lo","wpack_lo" (SRL_ESTATE in the
+ * bf16 mode).  h, logits, baseline, dlogits and dbaseline are f32, the rest bf16.  use_lstm contexts add the
  * actor step's bf16 operands: "lstm_step_xh" [2][B][2Hp] (per layer [x | m.h] of the last step, Hp = 576) and "lstm_step_w"
  * [2][4Hp][2Hp] (per layer [W_ih | W_hh], rows interleaved so one 128-row tile holds the 4 gates of 32 units; csrc/lstm.cu). */
 int srl_learner_debug_buffer(srl_learner_t* L, const char* name, void** ptr, int64_t* count);

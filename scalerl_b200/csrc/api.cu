@@ -181,18 +181,16 @@ struct srl_learner {
   float *scratch;                 // reductions (tail + grad norm)
   float* head_part;               // [HEAD_GROUPS][A+1][514+A] partial head weight gradients
   float *coef;                    // {norm, clip coef}
-  char* arena;
+  char* arena;                    // every workspace tensor (workspace_table)
   int64_t arena_bytes;
+  int64_t small_len;              // floats before fc.weight in the flat buffer: the small gradients cleared at the start of a step
   int step;                       // optimizer step count (Adam bias correction)
   bool have_fwd;
   TmaMaps maps;                   // tensor maps of the TMA mainloop
-  TmaMapsLo maps_lo;              // ... over the low operand tensors (precision = 1 only)
-  char* lo_arena;
   SideStream ss;                  // wgrad side stream + fork/join events
   int* dstep;                     // device-side optimizer step count (graph-replay safe Adam bias correction)
   srl_lstm_t* lstm;               // use_lstm: the 2-layer LSTM core (csrc/lstm.cu) working on views of params/grads
   float *core, *lstm_out, *dout, *dcore;   // [NF][H], [NF][H], [NB][H], [NB][H]
-  char* lstm_arena;
   int64_t lstm_off0, lstm_len;    // LSTM gradient range inside the flat buffer
   LstmStep* lstm_step;            // use_lstm: the one-row actor step (packed weights + operands; csrc/lstm.cu)
   int lstm_step_ksplit;           // K split of its GEMM (cluster size; srl_learner_set_option "lstm_step_ksplit")
@@ -200,7 +198,6 @@ struct srl_learner {
   bool column_fusion;             // heads + V-trace/loss + dh in one column kernel (SRL_NO_COLUMN_FUSION / srl_learner_set_option)
   Profiler pf;                    // per-kernel event bracketing (off by default)
   cudaEvent_t events[2 * PS_COUNT];
-  bool slot_used[PS_COUNT];
 };
 
 static const char* kSlotNames[PS_COUNT] = {"obs_s2d", "conv1_fwd", "conv2_fwd", "conv3_fwd", "fc_fwd", "head_fwd", "vtrace_loss_tail",
@@ -219,6 +216,60 @@ static int check_cfg(const srl_config_t* c) {
   return 0;
 }
 
+// The device workspace of a learner context, one row per tensor in carving order.  Every tensor is 256-byte aligned and zero-filled
+// at creation (the zeros of the da*g grids are the padding of the transposed convolutions).  In the fp32-accurate operand mode a row
+// with a low twin is followed by the twin, which srl_learner_debug_buffer calls "<name>_lo".  Rows without a name are internal.
+struct WsRow {
+  const char* name;
+  int elem;                       // bytes per element
+  int64_t count;                  // elements
+  void** hi;                      // receives the tensor's address (null: zeros only)
+  void** lo;                      // receives the low twin's address (null: no twin)
+};
+template <class T>
+static WsRow ws_row(const char* name, int64_t count, T** hi, T** lo = nullptr) {
+  return {name, (int)sizeof(T), count, reinterpret_cast<void**>(hi), reinterpret_cast<void**>(lo)};
+}
+constexpr int WS_MAX_ROWS = 32;
+static int workspace_table(srl_learner* L, WsRow* t) {
+  const srl_config_t& c = L->cfg;
+  const int64_t NF = (int64_t)(c.T + 1) * c.B, NB = (int64_t)c.T * c.B, A = c.A, H = 513 + A;
+  EncoderBuffers& b = L->buf;
+  OperandTensors &hi = b.hi, &lo = b.lo;
+  int n = 0;
+  t[n++] = ws_row("xs", NF * 441 * 64, &b.xs);
+  t[n++] = ws_row(nullptr, FC_SPLITS * NF * 512, &b.hpart);
+  t[n++] = ws_row("a1", NF * 400 * 32, &hi.a1, &lo.a1);
+  t[n++] = ws_row("a2", NF * 81 * 64, &hi.a2, &lo.a2);
+  t[n++] = ws_row("a3", NF * 49 * 64, &hi.a3, &lo.a3);
+  t[n++] = ws_row("h", NF * 512, &b.h);
+  t[n++] = ws_row("dh", NB * 512, &hi.dh, &lo.dh);
+  t[n++] = ws_row("da3", NB * 81 * 64, &hi.da3, &lo.da3);      // da3g (9x9 grid)
+  t[n++] = ws_row("da2", NB * 100 * 64, &hi.da2, &lo.da2);     // da2g (10x10 grid)
+  t[n++] = ws_row("da1", NB * 441 * 32, &hi.da1, &lo.da1);     // da1g (21x21 grid, 32 channels)
+  t[n++] = ws_row("wpack", WPack::TOTAL, &hi.wpack, &lo.wpack);
+  t[n++] = ws_row("logits", NF * A, &L->logits);
+  t[n++] = ws_row("baseline", NF, &L->baseline);
+  t[n++] = ws_row("dlogits", NB * A, &L->dlogits);
+  t[n++] = ws_row("dbaseline", NB, &L->dbaseline);
+  t[n++] = ws_row(nullptr, 4096, &L->scratch);
+  t[n++] = ws_row(nullptr, 4, &L->coef);
+  t[n++] = ws_row(nullptr, 4, &L->dstep);
+  t[n++] = ws_row(nullptr, WS_TOTAL, &b.wgrad_ws);
+  t[n++] = ws_row(nullptr, WSP_TOTAL, &b.wgrad_part);
+  t[n++] = ws_row(nullptr, HEAD_GROUPS * (A + 1) * (514 + A), &L->head_part);
+  t[n++] = ws_row("a3t", NF * 49 * 64, &b.a3t);
+  if (c.use_lstm) {
+    t[n++] = ws_row(nullptr, NF * H, &L->core);
+    t[n++] = ws_row(nullptr, NF * H, &L->lstm_out);
+    t[n++] = ws_row(nullptr, NB * H, &L->dout);
+    t[n++] = ws_row(nullptr, NB * H, &L->dcore);
+    t[n++] = ws_row<char>(nullptr, 1024, nullptr);      // 1 KiB of zeros behind dcore
+  }
+  return n;
+}
+static int64_t ws_bytes(const WsRow& r) { return ((int64_t)r.elem * r.count + 255) & ~int64_t(255); }
+
 static int pack_priority(int least, int greatest);
 extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float* grads, float* opt0, float* opt1, srl_learner_t** out) {
   int rc = check_cfg(cfg);
@@ -227,78 +278,37 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
   REQ(cfg->optimizer == 0 || opt1, "learner_create: Adam needs opt_state1");
   REQ(((reinterpret_cast<uintptr_t>(params) | reinterpret_cast<uintptr_t>(grads) | reinterpret_cast<uintptr_t>(opt0) |
         reinterpret_cast<uintptr_t>(opt1)) & 15) == 0, "learner_create: flat buffers must be 16-byte aligned");
-  srl_learner* L = new (std::nothrow) srl_learner();
+  srl_learner* L = new (std::nothrow) srl_learner();      // value-initialised: srl_learner_destroy can release any partial context
   REQ(L, "out of host memory");
+  auto undo = [L](int code) { srl_learner_destroy(L); return code; };      // the error message is written before the release
   L->cfg = *cfg; L->params = params; L->grads = grads; L->opt0 = opt0; L->opt1 = opt1;
-  L->nparams = layout_ex(cfg->A, cfg->use_lstm, nullptr, nullptr);
-  L->lo_arena = nullptr;
-  L->lstm = nullptr; L->lstm_arena = nullptr; L->core = L->lstm_out = L->dout = L->dcore = nullptr; L->lstm_off0 = L->lstm_len = 0;
-  L->lstm_step = nullptr; L->lstm_step_ksplit = LSTM_STEP_KSPLIT;
+  int64_t off[20];
+  L->nparams = layout_ex(cfg->A, cfg->use_lstm, off, nullptr);
+  L->small_len = off[6];
+  L->lstm_step_ksplit = LSTM_STEP_KSPLIT;
   L->P = make_ptrs(params, cfg->A);
   L->G = make_ptrs(grads, cfg->A);
-  L->step = 0; L->have_fwd = false;
   { const char* nf = getenv("SRL_NO_COLUMN_FUSION"); L->column_fusion = !(nf && atoi(nf) != 0); }   // read once, at creation
   // opt-in: the fused front has not been measured on H100 against the three kernels it replaces
   { const char* ff = getenv("SRL_FUSED_FWD"); L->fused_front = ff && atoi(ff) != 0; }
-  for (int i = 0; i < 2 * PS_COUNT; ++i) L->events[i] = nullptr;
-  for (int i = 0; i < PS_COUNT; ++i) L->slot_used[i] = false;
-  const int64_t NF = (int64_t)(cfg->T + 1) * cfg->B, NB = (int64_t)cfg->T * cfg->B, A = cfg->A;
-  // carve one arena (256-byte aligned pieces)
-  int64_t sizes[24]; int k = 0;
-  auto al = [](int64_t b) { return (b + 255) & ~int64_t(255); };
-  sizes[k++] = al(NF * 441 * 64 * 2);   // xs
-  sizes[k++] = al((int64_t)FC_SPLITS * NF * 512 * 4);   // hpart
-  sizes[k++] = al(NF * 400 * 32 * 2);   // a1
-  sizes[k++] = al(NF * 81 * 64 * 2);    // a2
-  sizes[k++] = al(NF * 49 * 64 * 2);    // a3
-  sizes[k++] = al(NF * 512 * 4);        // h
-  sizes[k++] = al(NB * 512 * 2);        // dh
-  sizes[k++] = al(NB * 81 * 64 * 2);    // da3g (9x9 grid)
-  sizes[k++] = al(NB * 100 * 64 * 2);   // da2g (10x10 grid)
-  sizes[k++] = al(NB * 441 * 32 * 2);   // da1g (21x21 grid, 32 channels)
-  sizes[k++] = al(WPack::TOTAL * 2);    // wpack
-  sizes[k++] = al(NF * A * 4);          // logits
-  sizes[k++] = al(NF * 4);              // baseline
-  sizes[k++] = al(NB * A * 4);          // dlogits
-  sizes[k++] = al(NB * 4);              // dbaseline
-  sizes[k++] = al(4096 * 4);            // scratch
-  sizes[k++] = al(16);                  // coef
-  sizes[k++] = al(16);                  // dstep
-  sizes[k++] = al(81920 * 4);           // conv wgrad workspace (res_problems.cuh WS_TOTAL = 81920 floats)
-  sizes[k++] = al(WSP_TOTAL * 4);       // conv wgrad per-CTA partials
-  sizes[k++] = al((int64_t)HEAD_GROUPS * (A + 1) * (514 + A) * 4);     // head wgrad partials
-  sizes[k++] = al(NF * 3136 * 2);       // a3t
+  const int64_t NF = (int64_t)(cfg->T + 1) * cfg->B, NB = (int64_t)cfg->T * cfg->B;
+  WsRow t[WS_MAX_ROWS];
+  const int n = workspace_table(L, t);
+  const bool split = cfg->precision == 1;
   int64_t total = 0;
-  for (int i = 0; i < k; ++i) total += sizes[i];
+  for (int i = 0; i < n; ++i) total += ws_bytes(t[i]) * (split && t[i].lo ? 2 : 1);
   cudaError_t e = cudaMalloc(&L->arena, total);
-  if (e != cudaSuccess) { delete L; return cuda_fail(e, "learner_create: cudaMalloc workspace"); }
+  if (e != cudaSuccess) return undo(cuda_fail(e, "learner_create: cudaMalloc workspace"));
   e = cudaMemset(L->arena, 0, total);
-  if (e != cudaSuccess) { cudaFree(L->arena); delete L; return cuda_fail(e, "learner_create: cudaMemset"); }
+  if (e != cudaSuccess) return undo(cuda_fail(e, "learner_create: cudaMemset"));
   L->arena_bytes = total;
-  char* q = L->arena; int i = 0;
-  L->buf.xs = (__nv_bfloat16*)q; q += sizes[i++];
-  L->buf.hpart = (float*)q; q += sizes[i++];
-  L->buf.a1 = (__nv_bfloat16*)q; q += sizes[i++];
-  L->buf.a2 = (__nv_bfloat16*)q; q += sizes[i++];
-  L->buf.a3 = (__nv_bfloat16*)q; q += sizes[i++];
-  L->buf.h = (float*)q; q += sizes[i++];
-  L->buf.dh = (__nv_bfloat16*)q; q += sizes[i++];
-  L->buf.da3 = (__nv_bfloat16*)q; q += sizes[i++];
-  L->buf.da2 = (__nv_bfloat16*)q; q += sizes[i++];
-  L->buf.da1 = (__nv_bfloat16*)q; q += sizes[i++];
-  L->buf.wpack = (__nv_bfloat16*)q; q += sizes[i++];
+  char* q = L->arena;
+  for (int i = 0; i < n; ++i) {
+    if (t[i].hi) *t[i].hi = q;
+    q += ws_bytes(t[i]);
+    if (split && t[i].lo) { *t[i].lo = q; q += ws_bytes(t[i]); }
+  }
   L->buf.NF = (int)NF;
-  L->logits = (float*)q; q += sizes[i++];
-  L->baseline = (float*)q; q += sizes[i++];
-  L->dlogits = (float*)q; q += sizes[i++];
-  L->dbaseline = (float*)q; q += sizes[i++];
-  L->scratch = (float*)q; q += sizes[i++];
-  L->coef = (float*)q; q += sizes[i++];
-  L->dstep = (int*)q; q += sizes[i++];
-  L->buf.wgrad_ws = (float*)q; q += sizes[i++];
-  L->buf.wgrad_part = (float*)q; q += sizes[i++];
-  L->head_part = (float*)q; q += sizes[i++];
-  L->buf.a3t = (__nv_bfloat16*)q; q += sizes[i++];
   if (cudaStreamCreateWithFlags(&L->ss.side, cudaStreamNonBlocking) != cudaSuccess ||
       cudaStreamCreateWithFlags(&L->ss.side2, cudaStreamNonBlocking) != cudaSuccess ||
       cudaStreamCreateWithFlags(&L->ss.side3, cudaStreamNonBlocking) != cudaSuccess) L->ss.side = nullptr;
@@ -310,60 +320,17 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
   for (int e2 = 0; e2 < 12 && L->ss.side; ++e2)
     if (cudaEventCreateWithFlags(&L->ss.ev[e2], cudaEventDisableTiming) != cudaSuccess) { L->ss.side = nullptr; }
   cudaGetLastError();
-  if (cfg->precision == 1) {      // low twins of every bf16 operand tensor (same layouts), zero-initialised like the originals
-    const int64_t lo_sizes[8] = {al(NF * 400 * 32 * 2), al(NF * 81 * 64 * 2), al(NF * 49 * 64 * 2), al(NB * 512 * 2), al(NB * 81 * 64 * 2),
-                                 al(NB * 100 * 64 * 2), al(NB * 441 * 32 * 2), al(WPack::TOTAL * 2)};
-    int64_t lo_total = 0;
-    for (int j = 0; j < 8; ++j) lo_total += lo_sizes[j];
-    if (cudaMalloc(&L->lo_arena, lo_total) != cudaSuccess || cudaMemset(L->lo_arena, 0, lo_total) != cudaSuccess) {
-      if (L->lo_arena) cudaFree(L->lo_arena);
-      cudaFree(L->arena); delete L;
-      return fail(SRL_ESTATE, "learner_create: cudaMalloc of the low operand tensors failed");
-    }
-    L->arena_bytes += lo_total;
-    char* ql = L->lo_arena; int j = 0;
-    L->buf.a1_lo = (__nv_bfloat16*)ql; ql += lo_sizes[j++];
-    L->buf.a2_lo = (__nv_bfloat16*)ql; ql += lo_sizes[j++];
-    L->buf.a3_lo = (__nv_bfloat16*)ql; ql += lo_sizes[j++];
-    L->buf.dh_lo = (__nv_bfloat16*)ql; ql += lo_sizes[j++];
-    L->buf.da3_lo = (__nv_bfloat16*)ql; ql += lo_sizes[j++];
-    L->buf.da2_lo = (__nv_bfloat16*)ql; ql += lo_sizes[j++];
-    L->buf.da1_lo = (__nv_bfloat16*)ql; ql += lo_sizes[j++];
-    L->buf.wpack_lo = (__nv_bfloat16*)ql; ql += lo_sizes[j++];
-  }
-  {
-    const char* why = nullptr;
-    if (build_tma_maps(L->buf, (int)NF, (int)NB, &L->maps, &why) != cudaSuccess ||
-        (cfg->precision == 1 && build_tma_maps_lo(L->buf, (int)NF, (int)NB, &L->maps_lo, &why) != cudaSuccess)) {
-      if (L->lo_arena) cudaFree(L->lo_arena);
-      cudaFree(L->arena);
-      delete L;
-      return fail(SRL_ESTATE, "learner_create: building TMA tensor map '%s' failed (driver without cuTensorMapEncodeTiled?)", why ? why : "?");
-    }
-  }
+  const char* why = nullptr;
+  if (build_tma_maps(L->buf, (int)NF, (int)NB, &L->maps, &why) != cudaSuccess)
+    return undo(fail(SRL_ESTATE, "learner_create: building TMA tensor map '%s' failed (driver without cuTensorMapEncodeTiled?)", why ? why : "?"));
   if (cfg->use_lstm) {
-    int64_t off[20], cnt[20];
-    const int64_t total_p = layout_ex(cfg->A, 1, off, cnt);
     const int H = 513 + cfg->A;
     const float* wp[8]; float* gp[8];
     for (int i = 0; i < 8; ++i) { wp[i] = params + off[12 + i]; gp[i] = grads + off[12 + i]; }
-    L->lstm_off0 = off[12]; L->lstm_len = total_p - off[12];
-    const int64_t bytes = ((NF + NF + NB + NB) * (int64_t)H * 4 + 1024);
-    bool ok = cudaMalloc(&L->lstm_arena, bytes) == cudaSuccess && cudaMemset(L->lstm_arena, 0, bytes) == cudaSuccess;
-    if (ok) {
-      float* q2 = (float*)L->lstm_arena;
-      L->core = q2; q2 += NF * H; L->lstm_out = q2; q2 += NF * H; L->dout = q2; q2 += NB * H; L->dcore = q2;
-      ok = srl_lstm_create(cfg->T + 1, cfg->B, H, wp, gp, &L->lstm) == 0;
-    }
-    const char* why = srl_lstm_last_error();
-    if (ok && lstm_step_create(cfg->B, H, wp, &L->lstm_step, &why) != cudaSuccess) ok = false;
-    if (!ok) {
-      if (L->lstm) srl_lstm_destroy(L->lstm);
-      if (L->lstm_arena) cudaFree(L->lstm_arena);
-      cudaFree(L->arena);
-      delete L;
-      return fail(SRL_ESTATE, "learner_create: LSTM core allocation failed: %s", why);
-    }
+    L->lstm_off0 = off[12]; L->lstm_len = L->nparams - off[12];
+    why = srl_lstm_last_error();
+    if (srl_lstm_create(cfg->T + 1, cfg->B, H, wp, gp, &L->lstm) != 0 || lstm_step_create(cfg->B, H, wp, &L->lstm_step, &why) != cudaSuccess)
+      return undo(fail(SRL_ESTATE, "learner_create: LSTM core allocation failed: %s", why));
   }
   *out = L;
   return 0;
@@ -379,8 +346,6 @@ extern "C" int srl_learner_destroy(srl_learner_t* L) {
   if (L->ss.pack) cudaStreamDestroy(L->ss.pack);
   if (L->lstm) srl_lstm_destroy(L->lstm);
   lstm_step_destroy(L->lstm_step);
-  if (L->lstm_arena) cudaFree(L->lstm_arena);
-  if (L->lo_arena) cudaFree(L->lo_arena);
   cudaFree(L->arena);
   delete L;
   return 0;
@@ -438,7 +403,7 @@ extern "C" int64_t srl_learner_get_step(srl_learner_t* L, void* stream) {
 
 extern "C" int srl_learner_pack_weights(srl_learner_t* L, void* stream) {
   REQ(L, "learner is NULL");
-  CU(launch_pack_weights(L->P, L->buf.wpack, (cudaStream_t)stream, L->buf.wpack_lo), "pack_weights");
+  CU(launch_pack_weights(L->P, L->buf.hi.wpack, (cudaStream_t)stream, L->buf.lo.wpack), "pack_weights");
   // the actor step's [W_ih | W_hh] copy: packed here, once per weight version, and never by the learner's own forward
   if (L->lstm_step) CU(lstm_step_pack(L->lstm_step, (cudaStream_t)stream), "lstm_step_pack");
   return 0;
@@ -464,38 +429,34 @@ static int encode_impl(srl_learner* L, const uint8_t* obs, int frames, cudaStrea
   pdl_set_active(!L->pf.on);
   // The bf16 operand copies are re-derived from the fp32 master weights at the START of every forward (not at the end
   // of the optimizer step): the pack kernel runs on the side stream underneath the frame conversion.
-  cudaEvent_t packed = nullptr;
-  if (L->ss.side && !L->pf.on) {
+  // Without side streams, or with per-kernel profiling on, both run on `st` (the profiler brackets are no-ops otherwise).
+  const bool fork = L->ss.side && !L->pf.on;
+  cudaStream_t pack_st = fork ? L->ss.pack : st;
+  if (fork) {
     CU(cudaEventRecord(L->ss.ev[5], st), "fork pack");
-    CU(cudaStreamWaitEvent(L->ss.pack, L->ss.ev[5], 0), "fork pack");
-    if (zero_small_grads) {   // the accumulated gradient segments (everything before fc.weight) are cleared under the frame conversion
-      int64_t off[12], cnt[12];
-      layout(L->cfg.A, off, cnt);
-      CU(cudaMemsetAsync(L->grads, 0, off[6] * sizeof(float), L->ss.pack), "zero small grads");
-    }
-    CU(launch_pack_weights(L->P, L->buf.wpack, L->ss.pack, L->buf.wpack_lo, true), "pack_weights");
-    CU(cudaEventRecord(L->ss.ev[6], L->ss.pack), "join pack");
-    packed = L->ss.ev[6];
-  } else {
-    if (zero_small_grads) {
-      int64_t off[12], cnt[12];
-      layout(L->cfg.A, off, cnt);
-      L->pf.b(PS_ZERO_GRADS);
-      CU(cudaMemsetAsync(L->grads, 0, off[6] * sizeof(float), st), "zero small grads");
-      L->pf.e(PS_ZERO_GRADS);
-    }
-    L->pf.b(PS_PACK);
-    CU(launch_pack_weights(L->P, L->buf.wpack, st, L->buf.wpack_lo, true), "pack_weights");
-    L->pf.e(PS_PACK);
+    CU(cudaStreamWaitEvent(pack_st, L->ss.ev[5], 0), "fork pack");
   }
-  CU(encoder_forward(obs, frames, L->P, L->buf, L->maps, L->cfg.precision, st, L->pf, packed, &L->maps_lo, L->fused_front), "encoder_forward");
+  if (zero_small_grads) {     // the accumulated gradient segments (everything before fc.weight) are cleared under the frame conversion
+    L->pf.b(PS_ZERO_GRADS);
+    CU(cudaMemsetAsync(L->grads, 0, L->small_len * sizeof(float), pack_st), "zero small grads");
+    L->pf.e(PS_ZERO_GRADS);
+  }
+  L->pf.b(PS_PACK);
+  CU(launch_pack_weights(L->P, L->buf.hi.wpack, pack_st, L->buf.lo.wpack, true), "pack_weights");
+  L->pf.e(PS_PACK);
+  cudaEvent_t packed = nullptr;
+  if (fork) {
+    CU(cudaEventRecord(L->ss.ev[6], pack_st), "join pack");
+    packed = L->ss.ev[6];
+  }
+  CU(encoder_forward(obs, frames, L->P, L->buf, L->maps, L->cfg.precision, st, L->pf, packed, L->fused_front), "encoder_forward");
   // learner step (bf16 mode): a3 -> fc.weight column order for the fc weight-gradient GEMM, on the wgrad side stream right after the fc forward,
   // i.e. under the column kernel (32 CTAs, the GPU is otherwise idle) instead of in the crowded backward phase
   L->buf.a3t_ready = false;
-  if (zero_small_grads && L->ss.side && !L->pf.on && L->cfg.precision == 0 && L->buf.a3t && !L->cfg.use_lstm) {
+  if (zero_small_grads && fork && L->cfg.precision == 0 && L->buf.a3t && !L->cfg.use_lstm) {
     CU(cudaEventRecord(L->ss.ev[10], st), "fork a3 transpose");
     CU(cudaStreamWaitEvent(L->ss.side, L->ss.ev[10], 0), "fork a3 transpose");
-    CU(launch_a3_transpose(L->buf.a3, L->buf.a3t, L->cfg.T * L->cfg.B, L->ss.side), "a3_transpose");
+    CU(launch_a3_transpose(L->buf.hi.a3, L->buf.a3t, L->cfg.T * L->cfg.B, L->ss.side), "a3_transpose");
     L->buf.a3t_ready = true;
   }
   return 0;
@@ -535,8 +496,8 @@ static int fb_begin(srl_learner* L, const uint8_t* obs, const float* reward, con
     L->pf.b(PS_TAIL);
     CU(launch_column_step(L->buf.hpart, FC_SPLITS, L->P.bf, L->buf.h, reward, action, done, behavior_logits, L->P.wp, L->P.bp, L->P.wb,
                           L->P.bb, c.T, c.B, c.A, c.discounting, c.reward_clip_abs_one, c.clip_rho_threshold, c.clip_pg_rho_threshold,
-                          c.baseline_cost, c.entropy_cost, L->logits, L->baseline, vs, pg_advantages, L->dlogits, L->dbaseline, L->buf.dh,
-                          losses, L->scratch, st, L->buf.dh_lo), "column_step");
+                          c.baseline_cost, c.entropy_cost, L->logits, L->baseline, vs, pg_advantages, L->dlogits, L->dbaseline, L->buf.hi.dh,
+                          losses, L->scratch, st, L->buf.lo.dh), "column_step");
     L->pf.e(PS_TAIL);
   } else {
     rc = forward_impl(L, obs, reward, action, NF, L->logits, L->baseline, st, true);
@@ -552,11 +513,11 @@ static int fb_begin(srl_learner* L, const uint8_t* obs, const float* reward, con
     const bool fork = L->ss.side != nullptr && !L->pf.on;
     cudaStream_t sw = fork ? L->ss.side : st;
     if (fork) { CU(cudaEventRecord(L->ss.ev[8], st), "fork head wgrad"); CU(cudaStreamWaitEvent(sw, L->ss.ev[8], 0), "fork head wgrad"); }
-    CU(launch_head_bwd(L->dlogits, L->dbaseline, L->buf.h, reward, action, L->P.wp, L->P.wb, NB, c.A, L->buf.dh, L->G.wp, L->G.bp, L->G.wb,
-                       L->G.bb, L->head_part, st, sw, !fused, L->buf.dh_lo), "head_bwd");      // side stream `side` is joined by encoder_backward (after the fc wgrad)
+    CU(launch_head_bwd(L->dlogits, L->dbaseline, L->buf.h, reward, action, L->P.wp, L->P.wb, NB, c.A, L->buf.hi.dh, L->G.wp, L->G.bp, L->G.wb,
+                       L->G.bb, L->head_part, st, sw, !fused, L->buf.lo.dh), "head_bwd");      // side stream `side` is joined by encoder_backward (after the fc wgrad)
   }
   L->pf.e(PS_HEAD_BWD);
-  CU(encoder_backward(obs, NB, L->buf, L->G, L->maps, c.precision, st, L->pf, L->ss, phase, &L->maps_lo), "encoder_backward");
+  CU(encoder_backward(NB, L->buf, L->G, L->maps, c.precision, st, L->pf, L->ss, phase), "encoder_backward");
   L->have_fwd = true;
   return 0;
 }
@@ -583,7 +544,7 @@ extern "C" int srl_learner_backward_finish(srl_learner_t* L, const uint8_t* obs,
   const srl_config_t& c = L->cfg;
   L->pf.st = (cudaStream_t)stream;
   pdl_set_active(!L->pf.on);
-  CU(encoder_backward(obs, c.T * c.B, L->buf, L->G, L->maps, c.precision, (cudaStream_t)stream, L->pf, L->ss, 1, &L->maps_lo), "encoder_backward");
+  CU(encoder_backward(c.T * c.B, L->buf, L->G, L->maps, c.precision, (cudaStream_t)stream, L->pf, L->ss, 1), "encoder_backward");
   return 0;
 }
 
@@ -650,18 +611,14 @@ extern "C" int srl_learner_forward_backward_lstm(srl_learner_t* L, const uint8_t
   CU(launch_impala_tail(behavior_logits, L->logits, L->baseline, action, reward, done, c.T, c.B, c.A, c.discounting, c.reward_clip_abs_one,
                         c.clip_rho_threshold, c.clip_pg_rho_threshold, c.baseline_cost, c.entropy_cost, vs, pg_advantages, L->dlogits,
                         L->dbaseline, losses, L->scratch, st), "impala_tail");
-  {
-    int64_t off[12], cnt[12];
-    layout(c.A, off, cnt);
-    CU(cudaMemsetAsync(L->grads, 0, off[6] * sizeof(float), st), "zero small grads");
-    CU(cudaMemsetAsync(L->grads + L->lstm_off0, 0, L->lstm_len * sizeof(float), st), "zero lstm grads");
-  }
+  CU(cudaMemsetAsync(L->grads, 0, L->small_len * sizeof(float), st), "zero small grads");
+  CU(cudaMemsetAsync(L->grads + L->lstm_off0, 0, L->lstm_len * sizeof(float), st), "zero lstm grads");
   CU(launch_head_dense_bwd(L->lstm_out, L->dlogits, L->dbaseline, L->P.wp, L->P.wb, NB, c.A, L->dout, L->G.wp, L->G.bp, L->G.wb, L->G.bb, st),
      "head_dense_bwd");
   rc = srl_lstm_backward(L->lstm, L->dout, done, L->dcore, st);
   if (rc) return fail(rc, "lstm_backward: %s", srl_lstm_last_error());
-  CU(launch_dcore_to_dh(L->dcore, L->buf.h, NB, c.A, L->buf.dh, st), "dcore_to_dh");
-  CU(encoder_backward(obs, NB, L->buf, L->G, L->maps, c.precision, st, L->pf, L->ss, 2, &L->maps_lo), "encoder_backward");
+  CU(launch_dcore_to_dh(L->dcore, L->buf.h, NB, c.A, L->buf.hi.dh, st), "dcore_to_dh");
+  CU(encoder_backward(NB, L->buf, L->G, L->maps, c.precision, st, L->pf, L->ss, 2), "encoder_backward");
   L->have_fwd = true;
   return 0;
 }
@@ -777,7 +734,6 @@ extern "C" int srl_memcpy_d2d(void* dst, const void* src, int64_t bytes, void* s
 
 extern "C" int srl_learner_debug_buffer(srl_learner_t* L, const char* name, void** ptr, int64_t* count) {
   REQ(L && name && ptr && count, "debug_buffer: NULL argument");
-  const int64_t NF = (int64_t)(L->cfg.T + 1) * L->cfg.B, NB = (int64_t)L->cfg.T * L->cfg.B, A = L->cfg.A;
   if (strncmp(name, "lstm_step_", 10) == 0) {     // the actor step's bf16 operands: xh [2][B][2Hp] = [x | m.h], w [2][4Hp][2Hp]
     REQ(L->lstm_step, "debug_buffer: '%s' exists only with use_lstm = 1", name);
     void *xh, *w;
@@ -786,18 +742,18 @@ extern "C" int srl_learner_debug_buffer(srl_learner_t* L, const char* name, void
     if (strcmp(name, "lstm_step_xh") == 0) { *ptr = xh; *count = nxh; return 0; }
     if (strcmp(name, "lstm_step_w") == 0) { *ptr = w; *count = nw; return 0; }
   }
-  struct { const char* n; void* p; int64_t c; } tab[] = {
-      {"xs", L->buf.xs, NF * 441 * 64}, {"a1", L->buf.a1, NF * 400 * 32}, {"a2", L->buf.a2, NF * 81 * 64}, {"a3", L->buf.a3, NF * 49 * 64}, {"a3t", L->buf.a3t, NF * 49 * 64}, {"h", L->buf.h, NF * 512},
-      {"logits", L->logits, NF * A}, {"baseline", L->baseline, NF}, {"dlogits", L->dlogits, NB * A}, {"dbaseline", L->dbaseline, NB},
-      {"dh", L->buf.dh, NB * 512}, {"da3", L->buf.da3, NB * 81 * 64}, {"da2", L->buf.da2, NB * 100 * 64},
-      {"da1", L->buf.da1, NB * 441 * 32}, {"wpack", L->buf.wpack, WPack::TOTAL},
-      {"a1_lo", L->buf.a1_lo, NF * 400 * 32}, {"a2_lo", L->buf.a2_lo, NF * 81 * 64}, {"a3_lo", L->buf.a3_lo, NF * 49 * 64},
-      {"dh_lo", L->buf.dh_lo, NB * 512}, {"da3_lo", L->buf.da3_lo, NB * 81 * 64}, {"da2_lo", L->buf.da2_lo, NB * 100 * 64},
-      {"da1_lo", L->buf.da1_lo, NB * 441 * 32}, {"wpack_lo", L->buf.wpack_lo, WPack::TOTAL}};
-  for (auto& t : tab)
-    if (strcmp(t.n, name) == 0) {
-      if (!t.p) return fail(SRL_ESTATE, "debug_buffer: '%s' exists only in the fp32-accurate operand mode (precision = 1)", name);
-      *ptr = t.p; *count = t.c; return 0;
+  WsRow t[WS_MAX_ROWS];
+  const int n = workspace_table(L, t);
+  const size_t len = strlen(name);
+  const bool twin = len > 3 && strcmp(name + len - 3, "_lo") == 0;
+  for (int i = 0; i < n; ++i) {
+    const WsRow& r = t[i];
+    if (!r.name) continue;
+    if (strcmp(r.name, name) == 0) { *ptr = *r.hi; *count = r.count; return 0; }
+    if (twin && r.lo && strlen(r.name) == len - 3 && strncmp(r.name, name, len - 3) == 0) {
+      if (!*r.lo) return fail(SRL_ESTATE, "debug_buffer: '%s' exists only in the fp32-accurate operand mode (precision = 1)", name);
+      *ptr = *r.lo; *count = r.count; return 0;
     }
+  }
   return fail(SRL_EINVAL, "debug_buffer: unknown buffer '%s'", name);
 }

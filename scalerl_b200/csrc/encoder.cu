@@ -4,7 +4,7 @@
 #include "res_problems.cuh"
 #include "enc_fused.cuh"
 #include "kernels.h"
-#include <initializer_list>
+#include <stdio.h>
 #include <stdlib.h>
 
 namespace srl {
@@ -205,87 +205,59 @@ bool make_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, 
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-cudaError_t build_tma_maps(const EncoderBuffers& b, int NF, int NB, TmaMaps* M, const char** why) {
-  const uint64_t nf = NF, nb = NB;
-  bool ok = true;
-  auto mk = [&](CUtensorMap* m, const void* base, int rank, std::initializer_list<uint64_t> dims, std::initializer_list<uint64_t> strides,
-                std::initializer_list<uint32_t> box, const char* name) {
-    if (!ok) return;
-    uint64_t d[5], s[4]; uint32_t bx[5];
-    int i = 0; for (auto v : dims) d[i++] = v;
-    i = 0; for (auto v : strides) s[i++] = v;
-    i = 0; for (auto v : box) bx[i++] = v;
-    if (!make_map(m, base, rank, d, s, bx)) { ok = false; if (why) *why = name; }
-  };
-  auto rows = [&](CUtensorMap* m, const void* base, uint64_t nrows, uint32_t boxrows, const char* name) {
-    mk(m, base, 2, {64, nrows}, {64}, {64, boxrows}, name);
-  };
-  rows(&M->xs_w, b.xs, nf * 441, RConv1Fwd::WROWS, "xs_w");
-  rows(&M->a1p0_w, b.a1, nf * 100, RConv2Fwd::WROWS, "a1p0_w");
-  rows(&M->a1p1_w, b.a1 + (size_t)nf * 100 * 64, nf * 100, RConv2Fwd::WROWS, "a1p1_w");
-  rows(&M->a2_w, b.a2, nf * 81, RConv3Fwd::WROWS, "a2_w");
-  rows(&M->da3g_w, b.da3, nb * 81, RConv3Dgrad::WROWS, "da3g_w");
-  rows(&M->da3g_b, b.da3, nb * 81, 128, "da3g_b");
-  rows(&M->da2g_w, b.da2, nb * 100, RConv2Dgrad::WROWS, "da2g_w");
-  rows(&M->da2g_b, b.da2, nb * 100, 128, "da2g_b");
-  { const uint64_t d[2] = {32, nb * 441}, st_[1] = {32}; const uint32_t bx[2] = {32, 128};      // da1g: 32-channel rows (64 B), SWIZZLE_64B
-    if (ok && !make_map(&M->da1g_b, b.da1, 2, d, st_, bx, true)) { ok = false; if (why) *why = "da1g_b"; } }
-  static_assert(RConv1Wgrad::WROWS == RConv1Fwd::WROWS && RConv2Wgrad::WROWS == RConv2Fwd::WROWS && RConv3Wgrad::WROWS == RConv3Fwd::WROWS,
-                "forward and wgrad share the window maps");
-  mk(&M->a3m128, b.a3, 2, {3136, nf}, {3136}, {64, 128}, "a3m128");
-  mk(&M->a3m64, b.a3, 2, {3136, nf}, {3136}, {64, 64}, "a3m64");
-  if (b.a3t) mk(&M->a3tm64, b.a3t, 2, {3136, nf}, {3136}, {64, 64}, "a3tm64");
-  mk(&M->dhm128, b.dh, 2, {512, nb}, {512}, {64, 128}, "dhm128");
-  mk(&M->dhm64, b.dh, 2, {512, nb}, {512}, {64, 64}, "dhm64");
+// Every map is 2-D over dense rows of `inner` elements (box = box_inner x box_rows).  The first map that cannot be built is
+// remembered by name (with "_lo" for the low operand set) and every later one is skipped.
+struct MapBuilder {
+  const char* failed = nullptr;
+  bool lo = false, failed_lo = false;
+  void operator()(CUtensorMap* m, const void* base, uint64_t inner, uint64_t rows, uint32_t box_inner, uint32_t box_rows, const char* name,
+                  bool swizzle64 = false) {
+    const uint64_t d[2] = {inner, rows}, s[1] = {inner};
+    const uint32_t bx[2] = {box_inner, box_rows};
+    if (!failed && !make_map(m, base, 2, d, s, bx, swizzle64)) { failed = name; failed_lo = lo; }
+  }
+};
+
+static void build_operand_maps(MapBuilder& mk, const OperandTensors& b, uint64_t nf, uint64_t nb, OperandMaps* M) {
+  mk(&M->a1p0_w, b.a1, 64, nf * 100, 64, RConv2Fwd::WROWS, "a1p0_w");
+  mk(&M->a1p1_w, b.a1 + (size_t)nf * 100 * 64, 64, nf * 100, 64, RConv2Fwd::WROWS, "a1p1_w");
+  mk(&M->a2_w, b.a2, 64, nf * 81, 64, RConv3Fwd::WROWS, "a2_w");
+  mk(&M->da3g_w, b.da3, 64, nb * 81, 64, RConv3Dgrad::WROWS, "da3g_w");
+  mk(&M->da3g_b, b.da3, 64, nb * 81, 64, 128, "da3g_b");
+  mk(&M->da2g_w, b.da2, 64, nb * 100, 64, RConv2Dgrad::WROWS, "da2g_w");
+  mk(&M->da2g_b, b.da2, 64, nb * 100, 64, 128, "da2g_b");
+  mk(&M->da1g_b, b.da1, 32, nb * 441, 32, 128, "da1g_b", true);      // da1g: 32-channel rows (64 B), SWIZZLE_64B
+  mk(&M->a3m128, b.a3, 3136, nf, 64, 128, "a3m128");
+  mk(&M->a3m64, b.a3, 3136, nf, 64, 64, "a3m64");
+  mk(&M->dhm128, b.dh, 512, nb, 64, 128, "dhm128");
+  mk(&M->dhm64, b.dh, 512, nb, 64, 64, "dhm64");
   const bf16* w = b.wpack;
-  mk(&M->w1k, w + WPack::W1K, 2, {256, 32}, {256}, {64, 32}, "w1k");
-  mk(&M->w2k, w + WPack::W2K, 2, {512, 64}, {512}, {64, 64}, "w2k");
-  mk(&M->w3k, w + WPack::W3K, 2, {576, 64}, {576}, {64, 64}, "w3k");
-  mk(&M->wfk, w + WPack::WFK, 2, {3136, 512}, {3136}, {64, 64}, "wfk");
-  mk(&M->wfd, w + WPack::WFD, 2, {512, 3136}, {512}, {64, 64}, "wfd");
-  mk(&M->w3d, w + WPack::W3D, 2, {576, 64}, {576}, {64, 64}, "w3d");
-  mk(&M->w2d, w + WPack::W2D, 2, {256, 128}, {256}, {64, 128}, "w2d");
-  M->valid = ok;
-  if (!ok && why && !*why) *why = "cuTensorMapEncodeTiled unavailable";
-  return ok ? cudaSuccess : cudaErrorInvalidValue;
+  mk(&M->w1k, w + WPack::W1K, 256, 32, 64, 32, "w1k");
+  mk(&M->w2k, w + WPack::W2K, 512, 64, 64, 64, "w2k");
+  mk(&M->w3k, w + WPack::W3K, 576, 64, 64, 64, "w3k");
+  mk(&M->wfk, w + WPack::WFK, 3136, 512, 64, 64, "wfk");
+  mk(&M->wfd, w + WPack::WFD, 512, 3136, 64, 64, "wfd");
+  mk(&M->w3d, w + WPack::W3D, 576, 64, 64, 64, "w3d");
+  mk(&M->w2d, w + WPack::W2D, 256, 128, 64, 128, "w2d");
 }
 
-cudaError_t build_tma_maps_lo(const EncoderBuffers& b, int NF, int NB, TmaMapsLo* M, const char** why) {
+cudaError_t build_tma_maps(const EncoderBuffers& b, int NF, int NB, TmaMaps* M, const char** why) {
+  static_assert(RConv1Wgrad::WROWS == RConv1Fwd::WROWS && RConv2Wgrad::WROWS == RConv2Fwd::WROWS && RConv3Wgrad::WROWS == RConv3Fwd::WROWS,
+                "forward and wgrad share the window maps");
   const uint64_t nf = NF, nb = NB;
-  bool ok = true;
-  auto mk = [&](CUtensorMap* m, const void* base, std::initializer_list<uint64_t> dims, std::initializer_list<uint64_t> strides,
-                std::initializer_list<uint32_t> box, const char* name) {
-    if (!ok) return;
-    uint64_t d[5], s[4]; uint32_t bx[5];
-    int i = 0; for (auto v : dims) d[i++] = v;
-    i = 0; for (auto v : strides) s[i++] = v;
-    i = 0; for (auto v : box) bx[i++] = v;
-    if (!make_map(m, base, 2, d, s, bx)) { ok = false; if (why) *why = name; }
-  };
-  auto rows = [&](CUtensorMap* m, const void* base, uint64_t nrows, uint32_t boxrows, const char* name) { mk(m, base, {64, nrows}, {64}, {64, boxrows}, name); };
-  rows(&M->a1p0_w, b.a1_lo, nf * 100, RConv2Fwd::WROWS, "a1p0_w_lo");
-  rows(&M->a1p1_w, b.a1_lo + (size_t)nf * 100 * 64, nf * 100, RConv2Fwd::WROWS, "a1p1_w_lo");
-  rows(&M->a2_w, b.a2_lo, nf * 81, RConv3Fwd::WROWS, "a2_w_lo");
-  rows(&M->da3g_w, b.da3_lo, nb * 81, RConv3Dgrad::WROWS, "da3g_w_lo");
-  rows(&M->da3g_b, b.da3_lo, nb * 81, 128, "da3g_b_lo");
-  rows(&M->da2g_w, b.da2_lo, nb * 100, RConv2Dgrad::WROWS, "da2g_w_lo");
-  rows(&M->da2g_b, b.da2_lo, nb * 100, 128, "da2g_b_lo");
-  { const uint64_t d[2] = {32, nb * 441}, st_[1] = {32}; const uint32_t bx[2] = {32, 128};
-    if (ok && !make_map(&M->da1g_b, b.da1_lo, 2, d, st_, bx, true)) { ok = false; if (why) *why = "da1g_b_lo"; } }
-  mk(&M->a3m128, b.a3_lo, {3136, nf}, {3136}, {64, 128}, "a3m128_lo");
-  mk(&M->a3m64, b.a3_lo, {3136, nf}, {3136}, {64, 64}, "a3m64_lo");
-  mk(&M->dhm128, b.dh_lo, {512, nb}, {512}, {64, 128}, "dhm128_lo");
-  mk(&M->dhm64, b.dh_lo, {512, nb}, {512}, {64, 64}, "dhm64_lo");
-  const bf16* w = b.wpack_lo;
-  mk(&M->w1k, w + WPack::W1K, {256, 32}, {256}, {64, 32}, "w1k_lo");
-  mk(&M->w2k, w + WPack::W2K, {512, 64}, {512}, {64, 64}, "w2k_lo");
-  mk(&M->w3k, w + WPack::W3K, {576, 64}, {576}, {64, 64}, "w3k_lo");
-  mk(&M->wfk, w + WPack::WFK, {3136, 512}, {3136}, {64, 64}, "wfk_lo");
-  mk(&M->wfd, w + WPack::WFD, {512, 3136}, {512}, {64, 64}, "wfd_lo");
-  mk(&M->w3d, w + WPack::W3D, {576, 64}, {576}, {64, 64}, "w3d_lo");
-  mk(&M->w2d, w + WPack::W2D, {256, 128}, {256}, {64, 128}, "w2d_lo");
-  M->valid = ok;
-  return ok ? cudaSuccess : cudaErrorInvalidValue;
+  MapBuilder mk;
+  mk(&M->xs_w, b.xs, 64, nf * 441, 64, RConv1Fwd::WROWS, "xs_w");
+  mk(&M->a3tm64, b.a3t, 3136, nf, 64, 64, "a3tm64");
+  build_operand_maps(mk, b.hi, nf, nb, &M->hi);
+  mk.lo = true;
+  if (b.lo.wpack) build_operand_maps(mk, b.lo, nf, nb, &M->lo);
+  M->valid = !mk.failed;
+  if (mk.failed && why) {
+    static thread_local char name[32];
+    snprintf(name, sizeof(name), "%s%s", mk.failed, mk.failed_lo ? "_lo" : "");
+    *why = name;
+  }
+  return mk.failed ? cudaErrorInvalidValue : cudaSuccess;
 }
 
 static cudaError_t launch_s2d(const uint8_t* obs, int frames, bf16* xs, cudaStream_t st, const float* w1, bf16* w1k, bf16* w1k_lo) {
@@ -377,30 +349,28 @@ __global__ void __launch_bounds__(256) conv_wgrad_finalize_kernel(float* __restr
 }
 
 cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, const EncoderBuffers& buf, const TmaMaps& maps, int mode,
-                            cudaStream_t st, const Profiler& pf, cudaEvent_t wait_before_conv1, const TmaMapsLo* lo, bool fused_front) {
+                            cudaStream_t st, const Profiler& pf, cudaEvent_t wait_before_conv1, bool fused_front) {
   if (frames <= 0) return cudaSuccess;
   if ((mode != 0 && mode != 1) || !maps.valid) return cudaErrorInvalidValue;
   const int sp = mode;                                    // 1: fp32-accurate split operands
-  TmaMapsLo dummy;                                        // bf16 mode: the low maps are never touched by the kernels
-  if (sp && (!lo || !lo->valid)) return cudaErrorInvalidValue;
-  const TmaMapsLo& L = sp ? *lo : dummy;
+  if (sp && !buf.lo.wpack) return cudaErrorInvalidValue;  // bf16 mode: the kernels never touch the low tensors and maps
   // bf16 mode: frame conversion + conv1 + conv2 as ONE persistent kernel (enc_fused.cuh); SRL_FUSED_FWD=0 or the fp32-accurate
   // operand mode use the three separate kernels
   if (fused_front && !sp && (reinterpret_cast<uintptr_t>(obs) & 15) == 0) {
-    EncFusedParams q{obs, p.w1, p.b1, p.w2, p.b2, buf.xs, buf.a1, buf.a2, frames, buf.NF};
+    EncFusedParams q{obs, p.w1, p.b1, p.w2, p.b2, buf.xs, buf.hi.a1, buf.hi.a2, frames, buf.NF};
     pf.b(PS_ENC_FUSED); SRL_TRY(enc_fused_fwd_launch(q, kPersistentCtas, st)); pf.e(PS_ENC_FUSED);
     if (wait_before_conv1) SRL_TRY(cudaStreamWaitEvent(st, wait_before_conv1, 0));      // conv3 / fc read the packed weights
   } else {
-  pf.b(PS_S2D); SRL_TRY(launch_s2d(obs, frames, buf.xs, st, p.w1, buf.wpack + WPack::W1K, sp ? buf.wpack_lo + WPack::W1K : nullptr)); pf.e(PS_S2D);
-  { RConv1Fwd::Params q{maps.xs_w, maps.w1k, L.w1k, p.b1, buf.a1, buf.a1_lo, frames, buf.NF};
+  pf.b(PS_S2D); SRL_TRY(launch_s2d(obs, frames, buf.xs, st, p.w1, buf.hi.wpack + WPack::W1K, sp ? buf.lo.wpack + WPack::W1K : nullptr)); pf.e(PS_S2D);
+  { RConv1Fwd::Params q{maps.xs_w, maps.hi.w1k, maps.lo.w1k, p.b1, buf.hi.a1, buf.lo.a1, frames, buf.NF};
     pf.b(PS_CONV1_FWD); SRL_TRY(res_fwd_launch<RConv1Fwd>(q, cdiv(frames * 441, 128), 2 * kPersistentCtas, st, sp)); pf.e(PS_CONV1_FWD); }
   if (wait_before_conv1) SRL_TRY(cudaStreamWaitEvent(st, wait_before_conv1, 0));      // conv1's weight copy comes from the frame-conversion kernel; conv2 is the first reader of the re-packed copies
-  { RConv2Fwd::Params q{maps.a1p0_w, maps.a1p1_w, maps.w2k, L.a1p0_w, L.a1p1_w, L.w2k, p.b2, buf.a2, buf.a2_lo, frames};
+  { RConv2Fwd::Params q{maps.hi.a1p0_w, maps.hi.a1p1_w, maps.hi.w2k, maps.lo.a1p0_w, maps.lo.a1p1_w, maps.lo.w2k, p.b2, buf.hi.a2, buf.lo.a2, frames};
     pf.b(PS_CONV2_FWD); SRL_TRY(res_fwd_launch<RConv2Fwd>(q, cdiv(frames * 100, 128), kPersistentCtas, st, sp)); pf.e(PS_CONV2_FWD); }
   }
-  { RConv3Fwd::Params q{maps.a2_w, maps.w3k, L.a2_w, L.w3k, p.b3, buf.a3, buf.a3_lo, frames};
+  { RConv3Fwd::Params q{maps.hi.a2_w, maps.hi.w3k, maps.lo.a2_w, maps.lo.w3k, p.b3, buf.hi.a3, buf.lo.a3, frames};
     pf.b(PS_CONV3_FWD); SRL_TRY(res_fwd_launch<RConv3Fwd>(q, cdiv(frames * 81, 128), kPersistentCtas, st, sp)); pf.e(PS_CONV3_FWD); }
-  { TFcFwd::Params q{maps.a3m128, maps.wfk, L.a3m128, L.wfk, buf.hpart, frames};
+  { TFcFwd::Params q{maps.hi.a3m128, maps.hi.wfk, maps.lo.a3m128, maps.lo.wfk, buf.hpart, frames};
     static_assert(TFcFwd::SPLITS == FC_SPLITS, "split count");
     pf.b(PS_FC_FWD);
     if (sp) SRL_TRY((igemm_tma_launch<TFcFwd, 1>(q, dim3(cdiv(frames, 128), 8 * FC_SPLITS), st)));
@@ -409,15 +379,12 @@ cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, 
   return cudaSuccess;
 }
 
-cudaError_t encoder_backward(const uint8_t* obs, int frames, const EncoderBuffers& buf, const ParamPtrs& g, const TmaMaps& maps, int mode,
-                             cudaStream_t st, const Profiler& pf, const SideStream& ss, int phase, const TmaMapsLo* lo) {
-  (void)obs;
+cudaError_t encoder_backward(int frames, const EncoderBuffers& buf, const ParamPtrs& g, const TmaMaps& maps, int mode,
+                             cudaStream_t st, const Profiler& pf, const SideStream& ss, int phase) {
   if (frames <= 0) return cudaSuccess;
   if ((mode != 0 && mode != 1) || !maps.valid) return cudaErrorInvalidValue;
   const int sp = mode;
-  TmaMapsLo dummy;
-  if (sp && (!lo || !lo->valid)) return cudaErrorInvalidValue;
-  const TmaMapsLo& L = sp ? *lo : dummy;
+  if (sp && !buf.lo.wpack) return cudaErrorInvalidValue;
   const bool do_fc = phase != 1, do_conv = phase != 0;
   // The wgrad GEMMs only feed the optimizer: each runs on its own side stream beside the dgrad chain
   // (dh -> da3 -> da2 -> da1) and beside each other.  With per-kernel profiling on everything stays on `st`.
@@ -429,16 +396,16 @@ cudaError_t encoder_backward(const uint8_t* obs, int frames, const EncoderBuffer
     { const bool native = !sp && buf.a3t != nullptr;          // bf16 mode: B operand = a3 transposed into fc.weight's column order, 256-column tiles
       p1.b(PS_FC_WGRAD);
       if (native) {
-        if (!buf.a3t_ready) SRL_TRY(launch_a3_transpose(buf.a3, buf.a3t, frames, s1));
-        TFcWgradN::Params q{maps.dhm64, maps.a3tm64, g.wf, g.bf, frames};
+        if (!buf.a3t_ready) SRL_TRY(launch_a3_transpose(buf.hi.a3, buf.a3t, frames, s1));
+        TFcWgradN::Params q{maps.hi.dhm64, maps.a3tm64, g.wf, g.bf, frames};
         SRL_TRY((igemm_tma_launch<TFcWgradN, 0>(q, dim3(1, 4 * (TFcWgradN::NCT + 1)), s1)));
       } else {
-        TFcWgrad::Params q{maps.dhm64, maps.a3m64, L.dhm64, L.a3m64, g.wf, g.bf, frames};
+        TFcWgrad::Params q{maps.hi.dhm64, maps.hi.a3m64, maps.lo.dhm64, maps.lo.a3m64, g.wf, g.bf, frames};
         if (sp) SRL_TRY((igemm_tma_launch<TFcWgrad, 1>(q, dim3(1, 4 * 50), s1))); else SRL_TRY((igemm_tma_launch<TFcWgrad, 0>(q, dim3(1, 4 * 50), s1)));
       }
       buf.a3t_ready = false;
       p1.e(PS_FC_WGRAD); }
-    { TFcDgrad::Params q{maps.dhm128, maps.wfd, L.dhm128, L.wfd, buf.a3, buf.da3, buf.da3_lo, frames};
+    { TFcDgrad::Params q{maps.hi.dhm128, maps.hi.wfd, maps.lo.dhm128, maps.lo.wfd, buf.hi.a3, buf.hi.da3, buf.lo.da3, frames};
       pf.b(PS_FC_DGRAD);
       if (sp) SRL_TRY((igemm_tma_launch<TFcDgrad, 1>(q, dim3(cdiv(frames, 128), 49), st))); else SRL_TRY((igemm_tma_launch<TFcDgrad, 0>(q, dim3(cdiv(frames, 128), 49), st)));
       pf.e(PS_FC_DGRAD); }
@@ -451,16 +418,16 @@ cudaError_t encoder_backward(const uint8_t* obs, int frames, const EncoderBuffer
   float* part2 = part3 + (size_t)WG_PART_CTAS * WSP_W3;
   float* part1 = part2 + (size_t)WG_PART_CTAS * WSP_W2;
   int n3 = 0, n2 = 0, n1 = 0;       // CTAs (partial slices) of the three wgrad launches
-  { RConv3Wgrad::Params q{maps.a2_w, maps.da3g_b, L.a2_w, L.da3g_b, part3, frames * 81, 0};
+  { RConv3Wgrad::Params q{maps.hi.a2_w, maps.hi.da3g_b, maps.lo.a2_w, maps.lo.da3g_b, part3, frames * 81, 0};
     p2.b(PS_CONV3_WGRAD); SRL_TRY(res_wgrad_launch<RConv3Wgrad>(q, side_wgrad_ctas(), s2, &n3, sp)); p2.e(PS_CONV3_WGRAD); }
-  { RConv3Dgrad::Params q{maps.da3g_w, maps.w3d, L.da3g_w, L.w3d, buf.a2, buf.da2, buf.da2_lo, frames};
+  { RConv3Dgrad::Params q{maps.hi.da3g_w, maps.hi.w3d, maps.lo.da3g_w, maps.lo.w3d, buf.hi.a2, buf.hi.da2, buf.lo.da2, frames};
     pf.b(PS_CONV3_DGRAD); SRL_TRY(res_fwd_launch<RConv3Dgrad>(q, cdiv(frames * 81, 128), bwd_ctas(), st, sp)); pf.e(PS_CONV3_DGRAD); }
   if (fork) { SRL_TRY(cudaEventRecord(ss.ev[2], st)); SRL_TRY(cudaStreamWaitEvent(s3, ss.ev[2], 0)); }
-  { RConv2Wgrad::Params q{maps.a1p0_w, maps.a1p1_w, maps.da2g_b, L.a1p0_w, L.a1p1_w, L.da2g_b, part2, frames * 100, 0};
+  { RConv2Wgrad::Params q{maps.hi.a1p0_w, maps.hi.a1p1_w, maps.hi.da2g_b, maps.lo.a1p0_w, maps.lo.a1p1_w, maps.lo.da2g_b, part2, frames * 100, 0};
     p3.b(PS_CONV2_WGRAD); SRL_TRY(res_wgrad_launch<RConv2Wgrad>(q, side_wgrad_ctas(), s3, &n2, sp)); p3.e(PS_CONV2_WGRAD); }
-  { RConv2Dgrad::Params q{maps.da2g_w, maps.w2d, L.da2g_w, L.w2d, buf.a1, buf.da1, buf.da1_lo, frames, buf.NF};
+  { RConv2Dgrad::Params q{maps.hi.da2g_w, maps.hi.w2d, maps.lo.da2g_w, maps.lo.w2d, buf.hi.a1, buf.hi.da1, buf.lo.da1, frames, buf.NF};
     pf.b(PS_CONV2_DGRAD); SRL_TRY(res_fwd_launch<RConv2Dgrad>(q, cdiv(frames * 100, 128), bwd_ctas(), st, sp)); pf.e(PS_CONV2_DGRAD); }
-  { RConv1Wgrad::Params q{maps.xs_w, maps.da1g_b, L.da1g_b, part1, frames * 441, 0};
+  { RConv1Wgrad::Params q{maps.xs_w, maps.hi.da1g_b, maps.lo.da1g_b, part1, frames * 441, 0};
     pf.b(PS_CONV1_WGRAD); SRL_TRY(res_wgrad_launch<RConv1Wgrad>(q, bwd_ctas(), st, &n1, sp)); pf.e(PS_CONV1_WGRAD); }
   if (fork) {      // join: fc wgrad (phase 2 only: phase 1 was joined by the caller of phase 0), conv3 wgrad, conv2 wgrad
     if (do_fc) { SRL_TRY(cudaStreamWaitEvent(st, ss.ev[4], 0)); }

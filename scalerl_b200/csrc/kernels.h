@@ -150,55 +150,54 @@ struct ParamPtrs {
   float *w1, *b1, *w2, *b2, *w3, *b3, *wf, *bf, *wp, *bp, *wb, *bb;
 };
 constexpr int FC_SPLITS = 4;
+// The bf16 operand tensors of the GEMMs.  The fp32-accurate operand mode (srl_config_t.precision = 1) holds a second set, the "low"
+// twins bf16(v - bf16(v)) in the same layouts.  xs has none: u8 frames are exact in bf16.
+struct OperandTensors {
+  __nv_bfloat16 *a1, *a2, *a3;          // a1 [2 planes][NF*100][64], a2 [NF*81][64], a3 [NF*49][64]
+  __nv_bfloat16 *dh, *da3, *da2, *da1;  // dh [NB][512]; da3g [NB*81][64], da2g [NB*100][64], da1g [NB*441][32] (grid layouts, zero-padded)
+  __nv_bfloat16* wpack;
+};
 struct EncoderBuffers {   // row layouts: see res_problems.cuh
   __nv_bfloat16* xs;                    // space-to-depth bf16 copy of the u8 frames [NF*441][64], 64 = (c,dy,dx)
-  __nv_bfloat16 *a1, *a2, *a3;          // a1 [2 planes][NF*100][64], a2 [NF*81][64], a3 [NF*49][64]
+  OperandTensors hi, lo = {};           // lo: all null in the bf16 mode
   mutable bool a3t_ready = false;       // the transpose below was already launched for this step (early, under the column kernel: api.cu encode_impl)
   __nv_bfloat16* a3t = nullptr;         // [NF][64*49]: a3 of the learning frames in fc.weight's own column order (c,h,w) -- fc wgrad's B operand (bf16 mode)
   float* hpart;                         // [FC_SPLITS][NF][512] split-K partials of the fc layer
   float* h;                             // [NF][512] fc output (post-ReLU), fp32
-  __nv_bfloat16 *dh, *da3, *da2, *da1;  // dh [NB][512]; da3g [NB*81][64], da2g [NB*100][64], da1g [NB*441][32] (grid layouts, zero-padded)
-  __nv_bfloat16* wpack;
   float* wgrad_ws;                      // conv weight-gradient accumulation workspace (res_problems.cuh: WS_TOTAL floats)
   float* wgrad_part;                    // per-CTA partials of the conv wgrad kernels (WSP_TOTAL floats)
   int NF;                               // frames the forward buffers were sized for (plane stride of a1)
-  // fp32-accurate operand mode (srl_config_t.precision = 1): the "low" twin bf16(v - bf16(v)) of every operand tensor above
-  // (same layouts; nullptr in the bf16 mode).  xs has none: u8 frames are exact in bf16.
-  __nv_bfloat16 *a1_lo = nullptr, *a2_lo = nullptr, *a3_lo = nullptr, *dh_lo = nullptr, *da3_lo = nullptr, *da2_lo = nullptr, *da1_lo = nullptr,
-                *wpack_lo = nullptr;
 };
 // tensor maps of the TMA kernels (built once per learner context: every operand buffer is fixed).
 // Activations are [rows][64] bf16; "w" = window box (128 + max tap shift rows), "b" = 128-row box.
-struct TmaMaps {
-  alignas(64) CUtensorMap xs_w, a1p0_w, a1p1_w, a2_w, da3g_w, da3g_b, da2g_w, da2g_b, da1g_b;      // conv layers (res_problems.cuh)
-  alignas(64) CUtensorMap a3m128, a3m64, dhm128, dhm64;                                            // fc layer (tma_problems.cuh)
-  alignas(64) CUtensorMap a3tm64;                                                                  // a3 in fc.weight's native column order (c,h,w): fc wgrad's B operand
+struct OperandMaps {      // the maps over one OperandTensors set
+  alignas(64) CUtensorMap a1p0_w, a1p1_w, a2_w, da3g_w, da3g_b, da2g_w, da2g_b, da1g_b;      // conv layers (res_problems.cuh)
+  alignas(64) CUtensorMap a3m128, a3m64, dhm128, dhm64;                                      // fc layer (tma_problems.cuh)
   alignas(64) CUtensorMap w1k, w2k, w3k, wfk, wfd, w3d, w2d;
-  bool valid = false;
 };
-struct TmaMapsLo {      // the same maps over the low tensors (built only in the fp32-accurate mode)
-  alignas(64) CUtensorMap a1p0_w, a1p1_w, a2_w, da3g_w, da3g_b, da2g_w, da2g_b, da1g_b, a3m128, a3m64, dhm128, dhm64;
-  alignas(64) CUtensorMap w1k, w2k, w3k, wfk, wfd, w3d, w2d;
+struct TmaMaps {
+  alignas(64) CUtensorMap xs_w;
+  alignas(64) CUtensorMap a3tm64;       // a3 in fc.weight's native column order (c,h,w): fc wgrad's B operand
+  OperandMaps hi, lo = {};              // lo: built only in the fp32-accurate mode
   bool valid = false;
 };
 // bf16 tensor map, dims innermost-first, strides in ELEMENTS for dims 1..rank-1, SWIZZLE_128B, zero OOB fill (encoder.cu)
 bool make_map(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems, const uint32_t* box, bool swizzle64 = false);
-// returns cudaSuccess or an error; `why` gets a message on failure
+// the maps of buf.hi, and of buf.lo when it is allocated.  Returns cudaSuccess or an error; `why` gets the name of the map that failed
 cudaError_t build_tma_maps(const EncoderBuffers& buf, int NF, int NB, TmaMaps* maps, const char** why);
-cudaError_t build_tma_maps_lo(const EncoderBuffers& buf, int NF, int NB, TmaMapsLo* maps, const char** why);
 // wpack_lo != nullptr: also the low copies bf16(w - bf16(w)) in the same layouts
 cudaError_t launch_a3_transpose(const __nv_bfloat16* a3, __nv_bfloat16* a3t, int frames, cudaStream_t st);
 cudaError_t launch_pack_weights(const ParamPtrs& p, __nv_bfloat16* wpack, cudaStream_t st, __nv_bfloat16* wpack_lo = nullptr, bool skip_w1k = false);
 // wait_before_conv1: optional event (weight re-pack running on the side stream) that conv1 must wait for
-// mode: 0 = bf16 operands, 1 = fp32-accurate split operands (maps_lo must be valid)
+// mode: 0 = bf16 operands, 1 = fp32-accurate split operands (buf.lo and maps.lo must be built)
 cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, const EncoderBuffers& buf, const TmaMaps& maps, int mode,
-                            cudaStream_t st, const Profiler& pf, cudaEvent_t wait_before_conv1, const TmaMapsLo* maps_lo = nullptr,
+                            cudaStream_t st, const Profiler& pf, cudaEvent_t wait_before_conv1,
                             bool fused_front = true);      // fused_front: frame conversion + conv1 + conv2 in one kernel (enc_fused.cuh; bf16 mode)
-// backward for the first `frames` frames given buf.dh; accumulates into the (pre-zeroed) gradient tensors in `g`
+// backward for the first `frames` frames given buf.hi.dh; accumulates into the (pre-zeroed) gradient tensors in `g`
 // phase: 0 = fc layer only (fc.weight / fc.bias gradients complete and joined to `st` on return: 95 % of the gradient
 //        bytes, ready for an early all-reduce), 1 = conv layers only, 2 = both
-cudaError_t encoder_backward(const uint8_t* obs, int frames, const EncoderBuffers& buf, const ParamPtrs& g, const TmaMaps& maps, int mode,
-                             cudaStream_t st, const Profiler& pf, const SideStream& ss, int phase, const TmaMapsLo* maps_lo = nullptr);
+cudaError_t encoder_backward(int frames, const EncoderBuffers& buf, const ParamPtrs& g, const TmaMaps& maps, int mode,
+                             cudaStream_t st, const Profiler& pf, const SideStream& ss, int phase);
 // ---- lstm.cu: the actor step of the 2-layer LSTM core (one row of B environments, no BPTT)
 struct LstmStep;
 // weights8: the 8 nn.LSTM tensors of the flat parameter buffer (srl_lstm_create order); H = 513 + A
