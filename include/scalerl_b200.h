@@ -125,6 +125,28 @@ int64_t srl_learner_workspace_bytes(const srl_learner_t* L);
 /* update a hyper-parameter that does not change buffer sizes (lr, costs, clip...) */
 int srl_learner_set_config(srl_learner_t* L, const srl_config_t* cfg);
 
+/* Learning-rate schedule of the optimizer step.  The lr of the 1-based optimizer step t (the device step count, so a replayed
+ * CUDA graph follows the schedule and a restored step count resumes it):
+ *   SRL_LR_CONSTANT: cfg.learning_rate (the default; frames_per_step and total_frames are not read)
+ *   SRL_LR_LINEAR  : max(lr * (1 - min((t-1) * frames_per_step, total_frames) / total_frames), lr_end), evaluated in double and
+ *                    rounded once to float.  lr_end = 0 is torchbeast's LambdaLR(1 - min(epoch*T*B, total)/total) stepped after each
+ *                    optimizer step; lr_end > 0 is the floor of ScaleRL's LinearDecayScheduler (scalerl/utils/lr_scheduler.py:50-88).
+ * frames_per_step: frames of one optimizer step over all ranks (T * B * world); total_frames: the frame budget of the run.
+ * SRL_EINVAL: unknown kind, lr_end < 0, or (linear) frames_per_step <= 0 / total_frames <= 0.
+ * After this call srl_learner_apply_gradients[_dp] write THREE floats to grad_norm_out: {norm, clip coefficient, lr of the step}.
+ * Synchronous (writes the configured lr into the context's coefficient block).  The call affects launches issued after it: a
+ * CUDA graph captured before it keeps the schedule it was captured with. */
+#define SRL_LR_CONSTANT 0
+#define SRL_LR_LINEAR 1
+int srl_learner_set_lr_schedule(srl_learner_t* L, int kind, float lr_end, double frames_per_step, double total_frames);
+/* RMSprop momentum (torch.optim.RMSprop(momentum=..., centered=False); reference impala_atari.py:99-105, rl_args.py:116):
+ * v = alpha v + (1 - alpha) g^2;  buf = momentum buf + g / (sqrt(v) + eps);  p -= lr buf  (g: the clipped gradient).
+ * momentum_buf: caller-owned flat f32 device buffer of the parameter layout (torch's 'momentum_buffer'), 16-byte aligned; zero it
+ * before the first step.  momentum = 0 (buffer NULL or ignored) turns momentum off.  SRL_EINVAL: momentum < 0, momentum > 0
+ * without a buffer or with Adam, a misaligned buffer.  Affects launches issued after the call; graphs captured before keep the
+ * old setting. */
+int srl_learner_set_momentum(srl_learner_t* L, float momentum, float* momentum_buf);
+
 /* run-time switches of one learner context: "column_fusion" (default 1; 0 = three kernels head_fwd / impala_tail / head_bwd
  * instead of the fused column kernel -- the environment variable SRL_NO_COLUMN_FUSION is read once, at creation);
  * "fused_fwd" (default 0, SRL_FUSED_FWD=1): u8 frame conversion + conv1 + conv2 as ONE persistent kernel (bf16 mode) instead of three;
@@ -180,7 +202,8 @@ int srl_learner_forward_backward_begin(srl_learner_t* L, const uint8_t* obs, con
 int srl_learner_backward_finish(srl_learner_t* L, const uint8_t* obs, void* stream);
 
 /* clip_grad_norm_(max_grad_norm) over `grads` (after the caller's all-reduce, if any) + optimizer step.
- * grad_norm_out: f32 [2] = {total L2 norm, clip coefficient} (may be NULL).  The bf16 operand copies of the weights
+ * grad_norm_out: f32 [2] = {total L2 norm, clip coefficient} (may be NULL); f32 [3] = {..., lr of the step} once
+ * srl_learner_set_lr_schedule has been called.  The bf16 operand copies of the weights
  * are re-derived at the start of the next srl_learner_forward* call. */
 int srl_learner_apply_gradients(srl_learner_t* L, float* grad_norm_out, void* stream);
 

@@ -71,6 +71,8 @@ _SIGS = {
     'srl_learner_set_option': [_P, C.c_char_p, _I],
     'srl_learner_snapshot_params': [_P, _P, _P, _P],
     'srl_learner_set_step': [_P, _L, _P],
+    'srl_learner_set_lr_schedule': [_P, _I, _F, C.c_double, C.c_double],
+    'srl_learner_set_momentum': [_P, _F, _P],
     'srl_memcpy_d2d': [_P, _P, _L, _P],
     'srl_host_register': [_P, _L],
     'srl_host_unregister': [_P],

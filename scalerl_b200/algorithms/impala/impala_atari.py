@@ -68,6 +68,8 @@ class ImpalaArguments:
     momentum: float = 0.0
     epsilon: float = 1e-5
     optimizer: str = 'rmsprop'
+    lr_schedule: str = 'constant'  # 'linear': decay to min_learning_rate over total_steps frames (torchbeast's LambdaLR; rl_args.py:233-252)
+    min_learning_rate: float = 0.0
     disable_checkpoint: bool = False
     num_actions: int = 6
     obs_shape: Tuple[int, int, int] = (4, 84, 84)
@@ -177,7 +179,9 @@ class ImpalaTrainer:
         return ImpalaHParams(rollout_length=a.rollout_length, batch_size=a.batch_size, num_actions=a.num_actions,
                              discounting=a.discounting, baseline_cost=a.baseline_cost, entropy_cost=a.entropy_cost,
                              reward_clipping=a.reward_clipping, max_grad_norm=a.max_grad_norm, learning_rate=a.learning_rate,
-                             alpha=a.alpha, momentum=a.momentum, epsilon=a.epsilon, optimizer=a.optimizer, use_lstm=a.use_lstm)
+                             alpha=a.alpha, momentum=a.momentum, epsilon=a.epsilon, optimizer=a.optimizer, use_lstm=a.use_lstm,
+                             lr_schedule=a.lr_schedule, min_learning_rate=a.min_learning_rate,
+                             total_frames=a.total_steps)     # total_steps counts frames: global_step += T * B (impala_atari.py:391)
 
     def create_buffers(self, obs_shape, num_actions) -> TrajectoryRing:
         """impala_atari.py:122-151 -- same keys/dtypes/shapes, slot-contiguous shared memory"""

@@ -3,6 +3,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <stdarg.h>
+#include <cmath>
 #include <new>
 
 #include "../../include/scalerl_b200.h"
@@ -180,7 +181,7 @@ struct srl_learner {
   float *dlogits, *dbaseline;     // [NB][A], [NB]
   float *scratch;                 // reductions (tail + grad norm)
   float* head_part;               // [HEAD_GROUPS][A+1][514+A] partial head weight gradients
-  float *coef;                    // {norm, clip coef}
+  float *coef;                    // {norm, clip coef, lr of the step}
   char* arena;                    // every workspace tensor (workspace_table)
   int64_t arena_bytes;
   int64_t small_len;              // floats before fc.weight in the flat buffer: the small gradients cleared at the start of a step
@@ -188,7 +189,9 @@ struct srl_learner {
   bool have_fwd;
   TmaMaps maps;                   // tensor maps of the TMA mainloop
   SideStream ss;                  // wgrad side stream + fork/join events
-  int* dstep;                     // device-side optimizer step count (graph-replay safe Adam bias correction)
+  int* dstep;                     // device-side optimizer step count (graph-replay safe Adam bias correction and lr schedule)
+  OptExtra ox;                    // lr schedule + RMSprop momentum of the optimizer step (srl_learner_set_lr_schedule / _set_momentum)
+  bool report_lr;                 // grad_norm_out receives coef[2] too (after srl_learner_set_lr_schedule)
   srl_lstm_t* lstm;               // use_lstm: the 2-layer LSTM core (csrc/lstm.cu) working on views of params/grads
   float *core, *lstm_out, *dout, *dcore;   // [NF][H], [NF][H], [NB][H], [NB][H]
   int64_t lstm_off0, lstm_len;    // LSTM gradient range inside the flat buffer
@@ -363,6 +366,13 @@ extern "C" int srl_debug_kernel_timeline(void* buffer) {
 
 extern "C" int64_t srl_learner_workspace_bytes(const srl_learner_t* L) { return L ? L->arena_bytes : 0; }
 
+// coef[2] = the configured lr.  The plain optimizer kernel (constant lr, no momentum) never writes coef[2]; the others overwrite
+// it with the lr of every step they run.
+static int publish_lr(srl_learner* L) {
+  CU(cudaMemcpy(L->coef + 2, &L->cfg.learning_rate, sizeof(float), cudaMemcpyHostToDevice), "publish lr");
+  return 0;
+}
+
 extern "C" int srl_learner_set_config(srl_learner_t* L, const srl_config_t* cfg) {
   REQ(L, "learner is NULL");
   int rc = check_cfg(cfg);
@@ -370,6 +380,34 @@ extern "C" int srl_learner_set_config(srl_learner_t* L, const srl_config_t* cfg)
   REQ(cfg->T == L->cfg.T && cfg->B == L->cfg.B && cfg->A == L->cfg.A && cfg->optimizer == L->cfg.optimizer &&
       cfg->precision == L->cfg.precision && cfg->use_lstm == L->cfg.use_lstm, "set_config: T/B/A/optimizer/precision/use_lstm are fixed at creation");
   L->cfg = *cfg;
+  return L->report_lr ? publish_lr(L) : 0;
+}
+
+extern "C" int srl_learner_set_lr_schedule(srl_learner_t* L, int kind, float lr_end, double frames_per_step, double total_frames) {
+  REQ(L, "set_lr_schedule: learner is NULL");
+  REQ(kind == SRL_LR_CONSTANT || kind == SRL_LR_LINEAR, "set_lr_schedule: unknown schedule kind %d (0 = constant, 1 = linear)", kind);
+  REQ(lr_end >= 0.f && std::isfinite(lr_end), "set_lr_schedule: lr_end=%g must be finite and >= 0", (double)lr_end);
+  if (kind == SRL_LR_LINEAR) {
+    REQ(total_frames > 0.0 && std::isfinite(total_frames), "set_lr_schedule: total_frames=%g must be finite and > 0", total_frames);
+    REQ(frames_per_step > 0.0 && std::isfinite(frames_per_step), "set_lr_schedule: frames_per_step=%g must be finite and > 0", frames_per_step);
+  }
+  OptExtra& x = L->ox;
+  x.schedule = kind == SRL_LR_LINEAR ? SCHED_LINEAR : SCHED_CONSTANT;
+  x.lr_end = lr_end;
+  x.frames_per_step = kind == SRL_LR_LINEAR ? frames_per_step : 0.0;
+  x.total_frames = kind == SRL_LR_LINEAR ? total_frames : 1.0;
+  L->report_lr = true;
+  return publish_lr(L);
+}
+
+extern "C" int srl_learner_set_momentum(srl_learner_t* L, float momentum, float* momentum_buf) {
+  REQ(L, "set_momentum: learner is NULL");
+  REQ(momentum >= 0.f && std::isfinite(momentum), "set_momentum: momentum=%g must be finite and >= 0", (double)momentum);
+  REQ(momentum == 0.f || L->cfg.optimizer == 0, "set_momentum: momentum is an RMSprop option; this learner runs Adam");
+  REQ(momentum == 0.f || momentum_buf, "set_momentum: momentum=%g needs a momentum buffer", (double)momentum);
+  REQ((reinterpret_cast<uintptr_t>(momentum_buf) & 15) == 0, "set_momentum: the momentum buffer must be 16-byte aligned");
+  L->ox.momentum = momentum;
+  L->ox.buf = momentum == 0.f ? nullptr : momentum_buf;
   return 0;
 }
 
@@ -633,13 +671,13 @@ extern "C" int srl_learner_apply_gradients(srl_learner_t* L, float* grad_norm_ou
   L->pf.b(PS_OPTIMIZER);
   if (c.optimizer == 0) {
     CU(launch_clip_optim(0, L->params, L->grads, L->opt0, nullptr, L->nparams, c.max_grad_norm, L->coef, L->scratch + 2048, c.learning_rate,
-                         c.alpha, 0.f, c.epsilon, L->step, L->dstep, st), "clip+rmsprop");
+                         c.alpha, 0.f, c.epsilon, L->step, L->dstep, L->ox, st), "clip+rmsprop");
   } else {
     CU(launch_clip_optim(1, L->params, L->grads, L->opt0, L->opt1, L->nparams, c.max_grad_norm, L->coef, L->scratch + 2048, c.learning_rate,
-                         c.adam_beta1, c.adam_beta2, c.adam_eps, L->step, L->dstep, st), "clip+adam");
+                         c.adam_beta1, c.adam_beta2, c.adam_eps, L->step, L->dstep, L->ox, st), "clip+adam");
   }
   L->pf.e(PS_OPTIMIZER);
-  if (grad_norm_out) CU(cudaMemcpyAsync(grad_norm_out, L->coef, 2 * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy coef");
+  if (grad_norm_out) CU(cudaMemcpyAsync(grad_norm_out, L->coef, (L->report_lr ? 3 : 2) * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy coef");
   return 0;
 }
 
@@ -663,13 +701,13 @@ extern "C" int srl_learner_apply_gradients_dp(srl_learner_t* L, const srl_dp_pee
   L->pf.b(PS_OPTIMIZER);
   if (c.optimizer == 0) {
     CU(launch_dp_clip_optim(0, L->params, L->grads, L->opt0, nullptr, L->nparams, c.max_grad_norm, L->coef, L->scratch + 2048,
-                            c.learning_rate, c.alpha, 0.f, c.epsilon, L->step, L->dstep, P, st), "dp clip+rmsprop");
+                            c.learning_rate, c.alpha, 0.f, c.epsilon, L->step, L->dstep, P, L->ox, st), "dp clip+rmsprop");
   } else {
     CU(launch_dp_clip_optim(1, L->params, L->grads, L->opt0, L->opt1, L->nparams, c.max_grad_norm, L->coef, L->scratch + 2048,
-                            c.learning_rate, c.adam_beta1, c.adam_beta2, c.adam_eps, L->step, L->dstep, P, st), "dp clip+adam");
+                            c.learning_rate, c.adam_beta1, c.adam_beta2, c.adam_eps, L->step, L->dstep, P, L->ox, st), "dp clip+adam");
   }
   L->pf.e(PS_OPTIMIZER);
-  if (grad_norm_out) CU(cudaMemcpyAsync(grad_norm_out, L->coef, 2 * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy coef");
+  if (grad_norm_out) CU(cudaMemcpyAsync(grad_norm_out, L->coef, (L->report_lr ? 3 : 2) * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy coef");
   return 0;
 }
 

@@ -413,20 +413,51 @@ cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n,
 // clip_grad_norm_ + optimizer step as ONE cooperative kernel (impala_atari.py:344-346): phase 1 sums g^2 (block partials
 // in a fixed slot each), grid barrier, every block adds the partials in the same fixed order (deterministic, identical
 // in all blocks), phase 2 applies the clipped update (g is re-read from L2).  OPT 0 = RMSprop, 1 = Adam.
+// clip_optim_kernel<OPT> is the plain step (constant lr, no momentum); clip_optim_ext_kernel<OPT, SCHED, MOM> adds the
+// learning-rate schedule (SCHED, OptExtra) and/or RMSprop momentum (MOM) and writes the step's lr to coef[2].  Both are
+// instantiations of one body, so the plain step's code is the one it always was.
 // ------------------------------------------------------------------------------------------------
-template <int OPT>
-__global__ void __launch_bounds__(512) clip_optim_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ s0,
-                                                         float* __restrict__ s1, int64_t n, float max_norm, float* __restrict__ coef,
-                                                         float* __restrict__ scratch, float lr, float a, float b, float eps, int step,
-                                                         int* __restrict__ dstep) {
+// lr of the 1-based step t: SCHED_LINEAR = max(lr (1 - min((t-1) F, Ftot) / Ftot), lr_end) -- torchbeast's LambdaLR
+// (scheduler.step() after optimizer.step(): step 1 runs at lr) with the floor of the reference's LinearDecayScheduler.
+// The whole expression is evaluated in double and rounded once, so the host's closed form gives the same float.
+SRL_DEVINL float scheduled_lr(float lr, int t, const OptExtra& x) {
+  const double f = 1.0 - fmin((double)(t - 1) * x.frames_per_step, x.total_frames) / x.total_frames;
+  return (float)fmax((double)lr * f, (double)x.lr_end);
+}
+// one element of torch.optim.RMSprop(centered=False) on the clipped gradient gk: v = a v + (1-a) gk^2, then
+// MOM: m = mu m + gk / (sqrt(v) + eps), p -= lr m;  else: p -= lr gk / (sqrt(v) + eps).  Every fused RMSprop kernel calls it.
+template <bool MOM>
+SRL_DEVINL void rmsprop_elem(float& p, float& v, float& m, float gk, float lr, float a, float eps, float mu) {
+  v = a * v + (1.f - a) * gk * gk;
+  if (MOM) {
+    m = mu * m + gk / (sqrtf(v) + eps);
+    p = p - lr * m;
+  } else {
+    p = p - lr * (gk / (sqrtf(v) + eps));
+  }
+}
+template <bool MOM>
+SRL_DEVINL void rmsprop_v4(float4& pp, float4& vv, float4& mm, const float4& gg, float c, float lr, float a, float eps, float mu) {
+  float* P = &pp.x; float* V = &vv.x; float* M = &mm.x; const float* G = &gg.x;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) rmsprop_elem<MOM>(P[k], V[k], M[k], G[k] * c, lr, a, eps, mu);
+}
+
+template <int OPT, int SCHED, bool MOM>
+SRL_DEVINL void clip_optim_body(float* __restrict__ p, float* __restrict__ g, float* __restrict__ s0, float* __restrict__ s1, int64_t n,
+                                float max_norm, float* __restrict__ coef, float* __restrict__ scratch, float lr, float a, float b, float eps,
+                                int step, int* __restrict__ dstep, const OptExtra& x) {
+  static_assert(!(MOM && OPT != 0), "momentum is an RMSprop option");
   cg::grid_group grid = cg::this_grid();
   pdl_wait(52);    // (cooperative launch, no attribute: returns at once; names the kernel in the diagnostics timeline)
   const int64_t n4 = n >> 2, stride = (int64_t)gridDim.x * blockDim.x, i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int t = dstep ? *dstep + 1 : step;          // 1-based step count: Adam bias correction; counted for RMSprop too (checkpoints)
+  const float lr_t = SCHED == SCHED_LINEAR ? scheduled_lr(lr, t, x) : lr;
+  float* __restrict__ mb = x.buf;                   // MOM: the momentum buffer
   // The thread's first HOLD float4 of g (and, for RMSprop, of p and the state) stay in registers across the grid barrier: phase 2 then
   // starts from registers instead of paying a second round of L2 / HBM latency (the grid covers n with <= HOLD items per thread).
   constexpr int HOLD = 2;
-  float4 gh[HOLD], ph[HOLD], vh[HOLD];
+  float4 gh[HOLD], ph[HOLD], vh[HOLD], mh[HOLD];
   float s = 0.f;
 #pragma unroll
   for (int h = 0; h < HOLD; ++h) {
@@ -434,6 +465,7 @@ __global__ void __launch_bounds__(512) clip_optim_kernel(float* __restrict__ p, 
     if (i < n4) {
       gh[h] = reinterpret_cast<const float4*>(g)[i];
       if (OPT == 0) { ph[h] = reinterpret_cast<const float4*>(p)[i]; vh[h] = reinterpret_cast<const float4*>(s0)[i]; }
+      if (MOM) mh[h] = reinterpret_cast<const float4*>(mb)[i];
     }
   }
 #pragma unroll
@@ -466,48 +498,39 @@ __global__ void __launch_bounds__(512) clip_optim_kernel(float* __restrict__ p, 
       c_sh = c;
       if (blockIdx.x == 0) {
         coef[0] = norm; coef[1] = c;
+        if (SCHED != SCHED_CONSTANT || MOM) coef[2] = lr_t;
         if (dstep) *dstep = t;
       }
     }
   }
   __syncthreads();
   const float c = c_sh;
+  const float mu = x.momentum;
+  float m1 = 0.f;                                   // !MOM: the unused momentum slot of the scalar tail
   if (OPT == 0) {
 #pragma unroll
     for (int h = 0; h < HOLD; ++h) {
       const int64_t i = i0 + h * stride;
       if (i < n4) {
-        float4 pp = ph[h], vv = vh[h];
-        const float4 gg = gh[h];
-        float* P = &pp.x; float* V = &vv.x; const float* G = &gg.x;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float gk = G[k] * c;
-          V[k] = a * V[k] + (1.f - a) * gk * gk;
-          P[k] = P[k] - lr * (gk / (sqrtf(V[k]) + eps));
-        }
+        float4 pp = ph[h], vv = vh[h], mm = MOM ? mh[h] : float4{};
+        rmsprop_v4<MOM>(pp, vv, mm, gh[h], c, lr_t, a, eps, mu);
         reinterpret_cast<float4*>(p)[i] = pp;
         reinterpret_cast<float4*>(s0)[i] = vv;
+        if (MOM) reinterpret_cast<float4*>(mb)[i] = mm;
       }
     }
     for (int64_t i = i0 + HOLD * stride; i < n4; i += stride) {
-      float4 pp = reinterpret_cast<float4*>(p)[i], vv = reinterpret_cast<float4*>(s0)[i];
+      float4 pp = reinterpret_cast<float4*>(p)[i], vv = reinterpret_cast<float4*>(s0)[i], mm = MOM ? reinterpret_cast<float4*>(mb)[i] : float4{};
       const float4 gg = reinterpret_cast<const float4*>(g)[i];
-      float* P = &pp.x; float* V = &vv.x; const float* G = &gg.x;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float gk = G[k] * c;
-        V[k] = a * V[k] + (1.f - a) * gk * gk;
-        P[k] = P[k] - lr * (gk / (sqrtf(V[k]) + eps));
-      }
+      rmsprop_v4<MOM>(pp, vv, mm, gg, c, lr_t, a, eps, mu);
       reinterpret_cast<float4*>(p)[i] = pp;
       reinterpret_cast<float4*>(s0)[i] = vv;
+      if (MOM) reinterpret_cast<float4*>(mb)[i] = mm;
     }
     if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
       const int64_t i = n4 * 4 + threadIdx.x;
-      const float gk = g[i] * c;
-      s0[i] = a * s0[i] + (1.f - a) * gk * gk;
-      p[i] = p[i] - lr * (gk / (sqrtf(s0[i]) + eps));
+      float* m = MOM ? mb + i : &m1;
+      rmsprop_elem<MOM>(p[i], s0[i], *m, g[i] * c, lr_t, a, eps, mu);
     }
   } else {
     const float inv_bc1 = 1.0f / (float)(1.0 - pow((double)a, (double)t));
@@ -517,39 +540,77 @@ __global__ void __launch_bounds__(512) clip_optim_kernel(float* __restrict__ p, 
       const float mk = a * s0[i] + (1.f - a) * gk;
       const float vk = b * s1[i] + (1.f - b) * gk * gk;
       s0[i] = mk; s1[i] = vk;
-      p[i] = p[i] - (lr * inv_bc1) * (mk / (sqrtf(vk) * inv_sqrt_bc2 + eps));
+      p[i] = p[i] - (lr_t * inv_bc1) * (mk / (sqrtf(vk) * inv_sqrt_bc2 + eps));
     }
   }
 }
 
+template <int OPT>
+__global__ void __launch_bounds__(512) clip_optim_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ s0,
+                                                         float* __restrict__ s1, int64_t n, float max_norm, float* __restrict__ coef,
+                                                         float* __restrict__ scratch, float lr, float a, float b, float eps, int step,
+                                                         int* __restrict__ dstep) {
+  clip_optim_body<OPT, SCHED_CONSTANT, false>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, OptExtra{});
+}
+template <int OPT, int SCHED, bool MOM>
+__global__ void __launch_bounds__(512) clip_optim_ext_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ s0,
+                                                             float* __restrict__ s1, int64_t n, float max_norm, float* __restrict__ coef,
+                                                             float* __restrict__ scratch, float lr, float a, float b, float eps, int step,
+                                                             int* __restrict__ dstep, const OptExtra x) {
+  clip_optim_body<OPT, SCHED, MOM>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, x);
+}
+
 SRL_KSTAMP_SETTER(kstamp_set_heads)
 
-template <int OPT>
-static cudaError_t launch_clip_optim_t(float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef, float* scratch,
-                                       float lr, float a, float b, float eps, int step, int* dstep, cudaStream_t st) {
-  static int per_sm_dev[64] = {}, sms_dev[64] = {};      // per device: one process may drive several GPUs
+// blocks of a cooperative optimizer launch: enough 512-thread blocks to cover n with one float4 per thread, at most what can be
+// co-resident and at most 592 (scratch holds 592 partials).  Occupancy is queried once per device and kernel.
+template <auto KERNEL>
+static cudaError_t coop_blocks(int64_t n, int* blocks_out) {
+  static int per_sm_dev[64] = {}, sms_dev[64] = {};      // per device and kernel: one process may drive several GPUs
   int dev = 0;
   SRL_TRY(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
   if (!per_sm_dev[dev]) {
     int sm_count = 0, occ = 0;
     SRL_TRY(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
-    SRL_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, clip_optim_kernel<OPT>, 512, 0));
+    SRL_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, KERNEL, 512, 0));
     if (occ < 1) return cudaErrorLaunchOutOfResources;
     sms_dev[dev] = sm_count; per_sm_dev[dev] = occ;
   }
   const int per_sm = per_sm_dev[dev], sms = sms_dev[dev];
   int64_t need = (n / 4 + 511) / 512;
   int blocks = (int)(need < 1 ? 1 : need);
-  int cap = per_sm * sms; if (cap > 592) cap = 592;          // scratch holds 592 partials
+  int cap = per_sm * sms; if (cap > 592) cap = 592;
   if (blocks > cap) blocks = cap;
-  void* args[] = {&p, &g, &s0, &s1, &n, &max_norm, &coef, &scratch, &lr, &a, &b, &eps, &step, &dstep};
-  return cudaLaunchCooperativeKernel((const void*)clip_optim_kernel<OPT>, dim3(blocks), dim3(512), args, 0, st);
+  *blocks_out = blocks;
+  return cudaSuccess;
+}
+
+template <int OPT, int SCHED, bool MOM>
+static cudaError_t launch_clip_optim_t(float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef, float* scratch,
+                                       float lr, float a, float b, float eps, int step, int* dstep, OptExtra x, cudaStream_t st) {
+  void* args[] = {&p, &g, &s0, &s1, &n, &max_norm, &coef, &scratch, &lr, &a, &b, &eps, &step, &dstep, &x};
+  int blocks = 0;
+  if constexpr (SCHED == SCHED_CONSTANT && !MOM) {
+    SRL_TRY(coop_blocks<clip_optim_kernel<OPT>>(n, &blocks));
+    return cudaLaunchCooperativeKernel((const void*)clip_optim_kernel<OPT>, dim3(blocks), dim3(512), args, 0, st);   // reads args[0..13]
+  } else {
+    SRL_TRY((coop_blocks<clip_optim_ext_kernel<OPT, SCHED, MOM>>(n, &blocks)));
+    return cudaLaunchCooperativeKernel((const void*)clip_optim_ext_kernel<OPT, SCHED, MOM>, dim3(blocks), dim3(512), args, 0, st);
+  }
 }
 cudaError_t launch_clip_optim(int optimizer, float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef,
-                              float* scratch, float lr, float a, float b, float eps, int step, int* dstep, cudaStream_t st) {
-  return optimizer == 0 ? launch_clip_optim_t<0>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, st)
-                        : launch_clip_optim_t<1>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, st);
+                              float* scratch, float lr, float a, float b, float eps, int step, int* dstep, const OptExtra& x,
+                              cudaStream_t st) {
+  const bool lin = x.schedule == SCHED_LINEAR, mom = x.buf != nullptr;
+  if (optimizer == 1)
+    return lin ? launch_clip_optim_t<1, SCHED_LINEAR, false>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, x, st)
+               : launch_clip_optim_t<1, SCHED_CONSTANT, false>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, x, st);
+  if (mom)
+    return lin ? launch_clip_optim_t<0, SCHED_LINEAR, true>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, x, st)
+               : launch_clip_optim_t<0, SCHED_CONSTANT, true>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, x, st);
+  return lin ? launch_clip_optim_t<0, SCHED_LINEAR, false>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, x, st)
+             : launch_clip_optim_t<0, SCHED_CONSTANT, false>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, x, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -640,15 +701,20 @@ SRL_DEVINL void dp_wait(const DpPeers& P, unsigned epoch) {        // all thread
 // buffer; after barrier 2 each rank holds the complete reduced gradient locally, so phase 2 is the plain single-GPU clip +
 // optimizer pass -- no peer pulls, no exchange buffer.  An element is read and then overwritten only by its slice's owner, so
 // the in-place broadcast cannot race with another rank's reduction.  All replicas consume the owner's bits: bit-identical.
-template <int OPT, bool NVLS>
-__global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ p, float* g, float* __restrict__ s0, float* __restrict__ s1,
-                                                            int64_t n, float max_norm, float* coef, float* scratch, float lr, float a,
-                                                            float b, float eps, int step, int* dstep, const DpPeers P) {
+// dp_clip_optim_kernel<OPT, NVLS> is the plain step; dp_clip_optim_ext_kernel<OPT, NVLS, SCHED, MOM> adds the learning-rate schedule
+// and/or RMSprop momentum, as clip_optim_ext_kernel does for one GPU (same scheduled_lr, same rmsprop_elem).
+template <int OPT, bool NVLS, int SCHED, bool MOM>
+SRL_DEVINL void dp_clip_optim_body(float* __restrict__ p, float* g, float* __restrict__ s0, float* __restrict__ s1, int64_t n, float max_norm,
+                                   float* coef, float* scratch, float lr, float a, float b, float eps, int step, int* dstep, const DpPeers& P,
+                                   const OptExtra& x) {
+  static_assert(!(MOM && OPT != 0), "momentum is an RMSprop option");
   cg::grid_group grid = cg::this_grid();
   const int64_t n4 = n >> 2, stride = (int64_t)gridDim.x * blockDim.x, i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int W = P.world, R = P.rank;
   const int64_t chunk = (n4 + W - 1) / W, lo = R * chunk, hi = min(n4, lo + chunk);
   const int t = dstep ? *reinterpret_cast<volatile int*>(dstep) + 1 : step;
+  const float lr_t = SCHED == SCHED_LINEAR ? scheduled_lr(lr, t, x) : lr;
+  float* __restrict__ mb = x.buf;                   // MOM: the momentum buffer (local, like the parameters)
   const unsigned e0 = reinterpret_cast<volatile unsigned*>(P.ctl[R])[32];     // epoch base (rewritten after the grid barrier)
   // ---- barrier 1: every rank's backward is complete
   if (blockIdx.x == 0) dp_signal(P, e0 + 1, false);      // the gradients were written by earlier kernels: already at L2
@@ -736,10 +802,14 @@ __global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ 
     const float norm = (float)sqrt(tot);
     const float c = max_norm >= 0.f ? fminf(max_norm / (norm + 1e-6f), 1.0f) : 1.0f;     // identical in every block of every rank
     c_sh = c;
-    if (blockIdx.x == 0) { coef[0] = norm; coef[1] = c; }
+    if (blockIdx.x == 0) {
+      coef[0] = norm; coef[1] = c;
+      if (SCHED != SCHED_CONSTANT || MOM) coef[2] = lr_t;
+    }
   }
   __syncthreads();
   const float c = c_sh;
+  const float mu = x.momentum;
   // ---- phase 2: clip + optimizer on my replica; the gradient buffer is local and fully reduced now
   float inv_bc1 = 0.f, inv_sqrt_bc2 = 0.f;
   if (OPT == 1) {
@@ -767,15 +837,12 @@ __global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ 
       const float4 gg = gpre[u];
       if (!NVLS && (int)min((int64_t)(W - 1), i / chunk) != R) reinterpret_cast<float4*>(g)[i] = gg;       // keep a copy: all-gather
       float4 pp = reinterpret_cast<float4*>(p)[i], vv = reinterpret_cast<float4*>(s0)[i];
-      float* Pp = &pp.x; float* V = &vv.x; const float* G = &gg.x;
       if (OPT == 0) {
-  #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float gk = G[k] * c;
-          V[k] = a * V[k] + (1.f - a) * gk * gk;
-          Pp[k] = Pp[k] - lr * (gk / (sqrtf(V[k]) + eps));
-        }
+        float4 mm = MOM ? reinterpret_cast<float4*>(mb)[i] : float4{};
+        rmsprop_v4<MOM>(pp, vv, mm, gg, c, lr_t, a, eps, mu);
+        if (MOM) reinterpret_cast<float4*>(mb)[i] = mm;
       } else {
+        float* Pp = &pp.x; float* V = &vv.x; const float* G = &gg.x;
         float4 ww = reinterpret_cast<float4*>(s1)[i];
         float* Wv = &ww.x;
   #pragma unroll
@@ -783,7 +850,7 @@ __global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ 
           const float gk = G[k] * c;
           V[k] = a * V[k] + (1.f - a) * gk;                    // exp_avg
           Wv[k] = b * Wv[k] + (1.f - b) * gk * gk;             // exp_avg_sq
-          Pp[k] = Pp[k] - (lr * inv_bc1) * (V[k] / (sqrtf(Wv[k]) * inv_sqrt_bc2 + eps));
+          Pp[k] = Pp[k] - (lr_t * inv_bc1) * (V[k] / (sqrtf(Wv[k]) * inv_sqrt_bc2 + eps));
         }
         reinterpret_cast<float4*>(s1)[i] = ww;
       }
@@ -799,38 +866,53 @@ __global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ 
     else { gv = ld_sys_f32(P.rs[W - 1] + 4 * chunk + threadIdx.x); g[i] = gv; }
     const float gk = gv * c;
     if (OPT == 0) {
-      s0[i] = a * s0[i] + (1.f - a) * gk * gk;
-      p[i] = p[i] - lr * (gk / (sqrtf(s0[i]) + eps));
+      float m1 = 0.f;                               // !MOM: the unused momentum slot
+      rmsprop_elem<MOM>(p[i], s0[i], MOM ? mb[i] : m1, gk, lr_t, a, eps, mu);
     } else {
       const float mk = a * s0[i] + (1.f - a) * gk, vk = b * s1[i] + (1.f - b) * gk * gk;
       s0[i] = mk; s1[i] = vk;
-      p[i] = p[i] - (lr * inv_bc1) * (mk / (sqrtf(vk) * inv_sqrt_bc2 + eps));
+      p[i] = p[i] - (lr_t * inv_bc1) * (mk / (sqrtf(vk) * inv_sqrt_bc2 + eps));
     }
   }
   // no closing barrier: after barrier 2 no rank touches another rank's memory until the next step's barrier 1
 }
 
 template <int OPT, bool NVLS>
+__global__ void __launch_bounds__(512) dp_clip_optim_kernel(float* __restrict__ p, float* g, float* __restrict__ s0, float* __restrict__ s1,
+                                                            int64_t n, float max_norm, float* coef, float* scratch, float lr, float a,
+                                                            float b, float eps, int step, int* dstep, const DpPeers P) {
+  dp_clip_optim_body<OPT, NVLS, SCHED_CONSTANT, false>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, P, OptExtra{});
+}
+template <int OPT, bool NVLS, int SCHED, bool MOM>
+__global__ void __launch_bounds__(512) dp_clip_optim_ext_kernel(float* __restrict__ p, float* g, float* __restrict__ s0, float* __restrict__ s1,
+                                                                int64_t n, float max_norm, float* coef, float* scratch, float lr, float a,
+                                                                float b, float eps, int step, int* dstep, const DpPeers P, const OptExtra x) {
+  dp_clip_optim_body<OPT, NVLS, SCHED, MOM>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, P, x);
+}
+
+template <int OPT, bool NVLS, int SCHED, bool MOM>
 static cudaError_t launch_dp_clip_optim_t(float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef, float* scratch,
-                                          float lr, float a, float b, float eps, int step, int* dstep, DpPeers P, cudaStream_t st) {
-  static int per_sm_dev[64] = {}, sms_dev[64] = {};      // per device: one process may drive several GPUs
-  int dev = 0;
-  SRL_TRY(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-  if (!per_sm_dev[dev]) {
-    int sm_count = 0, occ = 0;
-    SRL_TRY(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
-    SRL_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (dp_clip_optim_kernel<OPT, NVLS>), 512, 0));
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    sms_dev[dev] = sm_count; per_sm_dev[dev] = occ;
+                                          float lr, float a, float b, float eps, int step, int* dstep, DpPeers P, OptExtra x, cudaStream_t st) {
+  void* args[] = {&p, &g, &s0, &s1, &n, &max_norm, &coef, &scratch, &lr, &a, &b, &eps, &step, &dstep, &P, &x};
+  int blocks = 0;
+  if constexpr (SCHED == SCHED_CONSTANT && !MOM) {
+    SRL_TRY((coop_blocks<dp_clip_optim_kernel<OPT, NVLS>>(n, &blocks)));
+    return cudaLaunchCooperativeKernel((const void*)dp_clip_optim_kernel<OPT, NVLS>, dim3(blocks), dim3(512), args, 0, st);   // reads args[0..14]
+  } else {
+    SRL_TRY((coop_blocks<dp_clip_optim_ext_kernel<OPT, NVLS, SCHED, MOM>>(n, &blocks)));
+    return cudaLaunchCooperativeKernel((const void*)dp_clip_optim_ext_kernel<OPT, NVLS, SCHED, MOM>, dim3(blocks), dim3(512), args, 0, st);
   }
-  const int per_sm = per_sm_dev[dev], sms = sms_dev[dev];
-  int64_t need = (n / 4 + 511) / 512;
-  int blocks = (int)(need < 1 ? 1 : need);
-  int cap = per_sm * sms; if (cap > 592) cap = 592;
-  if (blocks > cap) blocks = cap;
-  void* args[] = {&p, &g, &s0, &s1, &n, &max_norm, &coef, &scratch, &lr, &a, &b, &eps, &step, &dstep, &P};
-  return cudaLaunchCooperativeKernel((const void*)dp_clip_optim_kernel<OPT, NVLS>, dim3(blocks), dim3(512), args, 0, st);
+}
+template <bool NVLS>
+static cudaError_t launch_dp_clip_optim_n(int optimizer, float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef,
+                                          float* scratch, float lr, float a, float b, float eps, int step, int* dstep, const DpPeers& P,
+                                          const OptExtra& x, cudaStream_t st) {
+  const bool lin = x.schedule == SCHED_LINEAR, mom = x.buf != nullptr;
+#define SRL_DP_LAUNCH(O, S, M) launch_dp_clip_optim_t<O, NVLS, S, M>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, P, x, st)
+  if (optimizer == 1) return lin ? SRL_DP_LAUNCH(1, SCHED_LINEAR, false) : SRL_DP_LAUNCH(1, SCHED_CONSTANT, false);
+  if (mom) return lin ? SRL_DP_LAUNCH(0, SCHED_LINEAR, true) : SRL_DP_LAUNCH(0, SCHED_CONSTANT, true);
+  return lin ? SRL_DP_LAUNCH(0, SCHED_LINEAR, false) : SRL_DP_LAUNCH(0, SCHED_CONSTANT, false);
+#undef SRL_DP_LAUNCH
 }
 // Weight-publish snapshot (impala_atari.py:348): dst = src when the step's total loss is finite, else dst keeps the last good
 // weights -- so the asynchronous D2H that follows never hands poisoned parameters to the actors.
@@ -853,12 +935,9 @@ cudaError_t launch_snapshot_if_finite(float* dst, const float* src, int64_t n, c
 
 cudaError_t launch_dp_clip_optim(int optimizer, float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef,
                                  float* scratch, float lr, float a, float b, float eps, int step, int* dstep, const DpPeers& P,
-                                 cudaStream_t st) {
-  if (P.mc_g)
-    return optimizer == 0 ? launch_dp_clip_optim_t<0, true>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, P, st)
-                          : launch_dp_clip_optim_t<1, true>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, P, st);
-  return optimizer == 0 ? launch_dp_clip_optim_t<0, false>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, P, st)
-                        : launch_dp_clip_optim_t<1, false>(p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, P, st);
+                                 const OptExtra& x, cudaStream_t st) {
+  return P.mc_g ? launch_dp_clip_optim_n<true>(optimizer, p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, P, x, st)
+                : launch_dp_clip_optim_n<false>(optimizer, p, g, s0, s1, n, max_norm, coef, scratch, lr, a, b, eps, step, dstep, P, x, st);
 }
 
 }  // namespace srl

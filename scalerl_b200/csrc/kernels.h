@@ -120,12 +120,23 @@ cudaError_t launch_head_dense_bwd(const float* X, const float* dlogits, const fl
 cudaError_t launch_dcore_to_dh(const float* dcore, const float* h, int N, int A, __nv_bfloat16* dh, cudaStream_t st);
 cudaError_t launch_unpack_slots(const uint8_t* staging, int64_t slot_bytes, const int64_t* off6, int T, int B, int A, uint8_t* obs, float* reward,
                                 uint8_t* done, int64_t* action, float* logits, float* episode_return, cudaStream_t st);
+// learning-rate schedule and RMSprop momentum of the fused clip + optimizer step (srl_learner_set_lr_schedule / _set_momentum).
+// The default value is the plain step: constant lr, no momentum.
+enum { SCHED_CONSTANT = 0, SCHED_LINEAR = 1 };
+struct OptExtra {
+  int schedule = SCHED_CONSTANT;
+  float lr_end = 0.f;                               // SCHED_LINEAR: floor of the decayed lr
+  double frames_per_step = 0.0, total_frames = 1.0; // SCHED_LINEAR: F (frames of one optimizer step, all ranks) and Ftot
+  float* buf = nullptr;                             // momentum buffer, parameter layout (null: no momentum)
+  float momentum = 0.f;
+};
 cudaError_t launch_clip_optim(int optimizer, float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef,
-                              float* scratch, float lr, float a, float b, float eps, int step, int* dstep, cudaStream_t st);
+                              float* scratch, float lr, float a, float b, float eps, int step, int* dstep, const OptExtra& x,
+                              cudaStream_t st);
 struct DpPeers { float* g[8]; float* rs[8]; unsigned* ctl[8]; int rank, world; float* mc_g; };      // peer-mapped gradient buffers / control blocks; mc_g: NVLS multicast address of the gradient buffers (or null)
 cudaError_t launch_dp_clip_optim(int optimizer, float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef,
                                  float* scratch, float lr, float a, float b, float eps, int step, int* dstep, const DpPeers& P,
-                                 cudaStream_t st);
+                                 const OptExtra& x, cudaStream_t st);
 cudaError_t launch_snapshot_if_finite(float* dst, const float* src, int64_t n, const float* losses, cudaStream_t st);
 cudaError_t launch_grad_norm(const float* g, int64_t n, float max_norm, float* coef, float* scratch, cudaStream_t st);
 cudaError_t launch_rmsprop(float* p, const float* g, float* v, int64_t n, const float* coef, float lr, float alpha, float eps,

@@ -79,7 +79,7 @@ class HostBatchFeeder:
         L.learn(self.slots[s], sync_stats=False)
         self.consumed[s].record(cur)
         self.result_host[s][:4].copy_(L._losses, non_blocking=True)
-        self.result_host[s][4:6].copy_(L._coef, non_blocking=True)
+        self.result_host[s][4:6].copy_(L._coef[:2], non_blocking=True)      # grad norm, clip coefficient
         self.result_ev[s].record(cur)
         self._learned += 1
         return s

@@ -34,21 +34,40 @@ def reference_param_order(use_lstm: bool = False):
     return PARAM_NAMES[:8] + (LSTM_PARAM_NAMES if use_lstm else ()) + PARAM_NAMES[8:]
 
 
-def _torch_param_groups(hp: 'ImpalaHParams', n: int):
-    """param_groups exactly as the installed torch writes them for the reference's optimizer (impala_atari.py:99-105)"""
+def scheduled_lr(lr: float, schedule: str, step: int, frames_per_step: float, total_frames: Optional[float], lr_end: float = 0.0) -> float:
+    """lr of the 1-based optimizer step ``step`` -- the closed form the optimizer kernels evaluate on the device count.
+    'linear': max(lr (1 - min((step-1) F, Ftot) / Ftot), lr_end), which is torchbeast's
+    ``LambdaLR(lambda epoch: 1 - min(epoch * T * B, total_steps) / total_steps)`` stepped after every optimizer step (lr_end = 0)
+    and ScaleRL's ``LinearDecayScheduler(lr, lr_end, total)`` stepped by F frames (scalerl/utils/lr_scheduler.py:50-88).
+    In double precision: pass float32-rounded lr / lr_end and round the result to float32 to get the kernel's bits."""
+    if schedule == 'constant':
+        return lr
+    f = 1.0 - min((step - 1) * float(frames_per_step), float(total_frames)) / float(total_frames)
+    return max(lr * f, lr_end)
+
+
+def _torch_param_groups(hp: 'ImpalaHParams', n: int, step: int = 0, frames_per_step: float = 0.0):
+    """param_groups exactly as the installed torch writes them for the reference's optimizer (impala_atari.py:99-105); with the
+    'linear' schedule as after ``step`` steps of a LambdaLR: 'lr' is the lr of the next step and 'initial_lr' the base lr"""
     dummy = [torch.nn.Parameter(torch.zeros(1)) for _ in range(n)]
     if hp.optimizer == 'rmsprop':
         opt = torch.optim.RMSprop(dummy, lr=hp.learning_rate, momentum=hp.momentum, eps=hp.epsilon, alpha=hp.alpha)
     else:
         opt = torch.optim.Adam(dummy, lr=hp.learning_rate, betas=(hp.adam_beta1, hp.adam_beta2), eps=hp.adam_eps)
-    return opt.state_dict()['param_groups']
+    groups = opt.state_dict()['param_groups']
+    if hp.lr_schedule != 'constant':
+        for g in groups:
+            g['initial_lr'] = hp.learning_rate
+            g['lr'] = scheduled_lr(hp.learning_rate, hp.lr_schedule, step + 1, frames_per_step, hp.total_frames, hp.min_learning_rate)
+    return groups
 
 
-def to_torch_optimizer_state(hp: 'ImpalaHParams', tensors: Dict[str, Dict[str, torch.Tensor]], step: int) -> dict:
+def to_torch_optimizer_state(hp: 'ImpalaHParams', tensors: Dict[str, Dict[str, torch.Tensor]], step: int,
+                             frames_per_step: float = 0.0) -> dict:
     """``torch.optim.RMSprop(...).state_dict()`` / ``Adam`` layout (what ImpalaTrainer.save_checkpoint stores,
-    impala_atari.py:506-511): {'state': {i: {'step', 'square_avg' | 'exp_avg','exp_avg_sq'}}, 'param_groups': [...]},
-    i = index in AtariNet.parameters() order.  ``tensors``: kind -> name -> tensor.  No state before the first step,
-    as torch (state is created lazily)."""
+    impala_atari.py:506-511): {'state': {i: {'step', 'square_avg' [, 'momentum_buffer'] | 'exp_avg','exp_avg_sq'}},
+    'param_groups': [...]}, i = index in AtariNet.parameters() order.  ``tensors``: kind -> name -> tensor.  No state before the
+    first step, as torch (state is created lazily).  ``frames_per_step``: F of the 'linear' schedule (the current lr)."""
     order = reference_param_order(hp.use_lstm)
     state = {}
     if step > 0:
@@ -57,12 +76,13 @@ def to_torch_optimizer_state(hp: 'ImpalaHParams', tensors: Dict[str, Dict[str, t
             for kind, d in tensors.items():
                 st[kind] = d[n].detach().cpu().clone()
             state[i] = st
-    return {'state': state, 'param_groups': _torch_param_groups(hp, len(order))}
+    return {'state': state, 'param_groups': _torch_param_groups(hp, len(order), step, frames_per_step)}
 
 
-def from_torch_optimizer_state(sd: dict, use_lstm: bool):
+def from_torch_optimizer_state(sd: dict, use_lstm: bool, momentum: bool = False):
     """inverse of to_torch_optimizer_state; also accepts round 1's {'step', 'state': {kind: {name: tensor}}} layout.
-    -> (step, {kind: {name: tensor}}).  Unknown layouts raise (never silently skipped)."""
+    -> (step, {kind: {name: tensor}}).  'momentum_buffer' is read only when ``momentum`` (the learner runs RMSprop momentum).
+    Unknown layouts raise (never silently skipped)."""
     if not sd:
         return 0, {}
     state = sd.get('state', {})
@@ -82,7 +102,7 @@ def from_torch_optimizer_state(sd: dict, use_lstm: bool):
         for kind, v in state[i].items():
             if kind == 'step':
                 steps.add(int(float(v)))
-            elif kind in ('square_avg', 'exp_avg', 'exp_avg_sq'):
+            elif kind in ('square_avg', 'exp_avg', 'exp_avg_sq') or (kind == 'momentum_buffer' and momentum):
                 out.setdefault(kind, {})[n] = v
             elif kind in ('momentum_buffer', 'grad_avg', 'max_exp_avg_sq'):
                 raise ValueError(f"optimizer_state_dict: '{kind}' (momentum / centered / amsgrad) is not supported by the fused optimizer")
@@ -127,7 +147,7 @@ class ImpalaHParams:
     max_grad_norm: float = 40.0          # rl_args.py:108
     learning_rate: float = 1e-4          # rl_args.py:112
     alpha: float = 0.99                  # rl_args.py:114
-    momentum: float = 0.0                # rl_args.py:116 (only 0 is supported, as the reference uses)
+    momentum: float = 0.0                # rl_args.py:116; RMSprop only (torch.optim.RMSprop(momentum=...))
     epsilon: float = 1e-5                # rl_args.py:117
     optimizer: str = 'rmsprop'           # 'rmsprop' (reference) | 'adam' (north_star)
     adam_beta1: float = 0.9
@@ -135,14 +155,29 @@ class ImpalaHParams:
     adam_eps: float = 1e-8
     precision: str = 'bf16'              # encoder operands: 'bf16' | 'fp32_split' (fp32-accurate hi/lo bf16 pairs; whole-step parity mode)
     use_lstm: bool = False               # AtariNet(use_lstm=True): 2-layer LSTM core (impala_atari.py:56; config 5)
+    lr_schedule: str = 'constant'        # 'constant' | 'linear' (decay to min_learning_rate over total_frames; torchbeast's LambdaLR)
+    min_learning_rate: float = 0.0       # floor of the 'linear' schedule (ScaleRL rl_args.py:233-252)
+    total_frames: Optional[int] = None   # frame budget of the 'linear' schedule (ImpalaArguments.total_steps)
+
+    def validate(self) -> None:
+        """the optimizer settings the fused kernels support; anything else raises ValueError"""
+        if self.optimizer not in ('rmsprop', 'adam'):
+            raise ValueError("optimizer must be 'rmsprop' or 'adam'")
+        if not self.momentum >= 0.0:
+            raise ValueError(f'momentum must be >= 0, got {self.momentum}')
+        if self.momentum != 0.0 and self.optimizer != 'rmsprop':
+            raise ValueError('momentum is an RMSprop option: Adam takes its betas instead')
+        if self.lr_schedule not in ('constant', 'linear'):
+            raise ValueError(f"lr_schedule must be 'constant' or 'linear', got {self.lr_schedule!r}")
+        if not self.min_learning_rate >= 0.0:
+            raise ValueError(f'min_learning_rate must be >= 0, got {self.min_learning_rate}')
+        if self.lr_schedule == 'linear' and not (self.total_frames is not None and self.total_frames > 0):
+            raise ValueError("lr_schedule='linear' needs total_frames > 0 (the frame budget the lr decays over)")
 
     def to_c(self) -> _lib.SrlConfig:
         if self.reward_clipping not in ('abs_one', 'none'):
             raise ValueError("reward_clipping must be 'abs_one' or 'none'")
-        if self.optimizer not in ('rmsprop', 'adam'):
-            raise ValueError("optimizer must be 'rmsprop' or 'adam'")
-        if self.momentum != 0.0:
-            raise ValueError('only momentum=0 is supported (the reference default)')
+        self.validate()
         c = _lib.SrlConfig()
         c.T, c.B, c.A = self.rollout_length, self.batch_size, self.num_actions
         c.optimizer = 0 if self.optimizer == 'rmsprop' else 1
@@ -191,6 +226,7 @@ class B200ImpalaLearner(BaseAgent):
             if self._dist and os.environ.get('SRL_DP_FUSED', '1') != '0':
                 self._setup_peer_memory(total)       # replaces flat_grads by a symmetric-memory buffer when that works
             self.opt_state1 = z() if hp.optimizer == 'adam' else None
+            self.opt_state2 = z() if hp.momentum != 0 else None      # RMSprop momentum buffer
             self.shapes = param_shapes(hp.num_actions, hp.use_lstm)
             self.params = OrderedDict((n, self._view(self.flat_params, i)) for i, n in enumerate(self.names))
             self.grads = OrderedDict((n, self._view(self.flat_grads, i)) for i, n in enumerate(self.names))
@@ -202,14 +238,20 @@ class B200ImpalaLearner(BaseAgent):
                 C.byref(self._cfg), self.flat_params.data_ptr(), self.flat_grads.data_ptr(), self.opt_state0.data_ptr(),
                 self.opt_state1.data_ptr() if self.opt_state1 is not None else None, C.byref(h)), 'srl_learner_create')
             self._h = h
+            # frames of one optimizer step over every rank: the unit the reference's global step counts (impala_atari.py:391)
+            self.frames_per_step = hp.rollout_length * hp.batch_size * self.world_size
+            _lib.check(self._L.srl_learner_set_lr_schedule(h, 1 if hp.lr_schedule == 'linear' else 0, hp.min_learning_rate,
+                                                           float(self.frames_per_step), float(hp.total_frames or 0)), 'srl_learner_set_lr_schedule')
+            _lib.check(self._L.srl_learner_set_momentum(h, hp.momentum, self.opt_state2.data_ptr() if self.opt_state2 is not None else None),
+                       'srl_learner_set_momentum')
             self.load_state_dict(init_state_dict)
             T, B, A = hp.rollout_length, hp.batch_size, hp.num_actions
             if hp.use_lstm:     # static copies of the initial LSTM state (graph-replay safe addresses)
                 self._h0 = torch.zeros(2, B, 513 + A, device=self.device)
                 self._c0 = torch.zeros(2, B, 513 + A, device=self.device)
-            self._resdev = torch.zeros(8, device=self.device)      # {pg, baseline, entropy, total loss | grad norm, clip coef | pad}: ONE D2H per step
+            self._resdev = torch.zeros(8, device=self.device)      # {pg, baseline, entropy, total loss | grad norm, clip coef, lr | pad}: ONE D2H per step
             self._losses = self._resdev[:4]
-            self._coef = self._resdev[4:6]
+            self._coef = self._resdev[4:7]
             self._vs = torch.empty(T, B, device=self.device)
             self._pg_adv = torch.empty(T, B, device=self.device)
             self._stats_host = torch.zeros(8, dtype=torch.float32).pin_memory()
@@ -217,6 +259,8 @@ class B200ImpalaLearner(BaseAgent):
         self.use_graph = use_graph and not os.environ.get('SRL_NO_GRAPH')   # SRL_NO_GRAPH=1: eager launches (for ncu)
         self._graphs = {}       # batch buffer addresses -> captured CUDA graph(s) of the step
         self._seen = set()
+        self._last_lr = None    # lr of the last step whose stats were read (learn() / result())
+        self._stepped = False
 
     def _setup_peer_memory(self, total):
         """Gradient buffer + 1 KiB control block in symmetric memory (every rank maps every rank's copy): the apply step
@@ -305,15 +349,18 @@ class B200ImpalaLearner(BaseAgent):
     def _opt_tensors(self):
         kinds = ('square_avg',) if self.hp.optimizer == 'rmsprop' else ('exp_avg', 'exp_avg_sq')
         flats = (self.opt_state0,) if self.hp.optimizer == 'rmsprop' else (self.opt_state0, self.opt_state1)
+        if self.opt_state2 is not None:
+            kinds, flats = kinds + ('momentum_buffer',), flats + (self.opt_state2,)
         return {k: OrderedDict((n, self._view(f, i)) for i, n in enumerate(self.names)) for k, f in zip(kinds, flats)}
 
     def optimizer_state_dict(self):
         """torch.optim state_dict layout of the reference's optimizer (impala_atari.py:99-105,509): loadable by
-        ``torch.optim.RMSprop(AtariNet(...).parameters(), ...).load_state_dict`` and back"""
-        return to_torch_optimizer_state(self.hp, self._opt_tensors(), self.global_opt_step)
+        ``torch.optim.RMSprop(AtariNet(...).parameters(), ...).load_state_dict`` and back.  With the 'linear' schedule the
+        param_groups carry the lr of the next step, as a LambdaLR leaves them; the schedule position is the step count."""
+        return to_torch_optimizer_state(self.hp, self._opt_tensors(), self.global_opt_step, self.frames_per_step)
 
     def load_optimizer_state_dict(self, sd) -> None:
-        step, kinds = from_torch_optimizer_state(sd, self.hp.use_lstm)
+        step, kinds = from_torch_optimizer_state(sd, self.hp.use_lstm, momentum=self.opt_state2 is not None)
         mine = self._opt_tensors()
         for kind in kinds:
             if kind not in mine:
@@ -334,6 +381,19 @@ class B200ImpalaLearner(BaseAgent):
         """optimizer step count = Adam's bias-correction t (host copy + the device counter the captured graphs read)"""
         _lib.check(self._L.srl_learner_set_step(self._h, int(step), self._stream()), 'srl_learner_set_step')
         self._opt_steps = int(step)
+
+    def learning_rate(self) -> float:
+        """lr of the last finished step, as the optimizer kernel used it: read with the step's stats (learn(), result()), or from
+        the device here after learn(sync_stats=False).  Before this learner ran a step: the float32 closed form at the step
+        count (a restored checkpoint's last step; step 1 for a fresh learner)."""
+        if self._last_lr is None:
+            if not self._stepped:
+                f32 = lambda v: float(torch.tensor(v, dtype=torch.float32))
+                hp = self.hp
+                return f32(scheduled_lr(f32(hp.learning_rate), hp.lr_schedule, max(self.global_opt_step, 1), self.frames_per_step,
+                                        hp.total_frames, f32(hp.min_learning_rate)))
+            self._last_lr = float(self._coef[2].item())
+        return self._last_lr
 
     def device_opt_step(self) -> int:
         """the step count as the kernels see it (device counter; synchronises)"""
@@ -474,6 +534,8 @@ class B200ImpalaLearner(BaseAgent):
         r = self._res[ticket % self._res_depth]
         r['ev'].synchronize()
         h = r['scal']
+        if ticket == self._tickets - 1:
+            self._last_lr = float(h[6])
         ep = r['ep'][r['done'].bool()] if r['has_ep'] else torch.empty(0)
         return {'episode_returns': tuple(ep.numpy()), 'mean_episode_return': float(ep.mean()) if ep.numel() else float('nan'),
                 'total_loss': float(h[3]), 'pg_loss': float(h[0]), 'baseline_loss': float(h[1]), 'entropy_loss': float(h[2]),
@@ -641,17 +703,19 @@ class B200ImpalaLearner(BaseAgent):
             self._enqueue_step(batch)
         # the reference counts the frames of the GLOBAL batch (impala_atari.py:391); a rank processes B_local columns of it
         self.global_step += self.hp.rollout_length * self.hp.batch_size * self.world_size
+        self._last_lr, self._stepped = None, True
         if not sync_stats:
             return {}
         host = self._stats_host
         if self._dist:      # loss scalars are SUMs over the global batch in the reference; reduced only when somebody reads them
             torch.distributed.all_reduce(self._losses, op=torch.distributed.ReduceOp.SUM, group=self.pg or None)
         host[:4].copy_(self._losses, non_blocking=True)
-        host[4:6].copy_(self._coef, non_blocking=True)
+        host[4:7].copy_(self._coef, non_blocking=True)
         done = batch['done'][1:]
         ep = batch['episode_return'][1:][done] if 'episode_return' in batch else torch.empty(0, device=self.device)
         ep_host = ep.cpu()                                  # synchronises the stream (the reference does 6 .item() syncs)
         torch.cuda.current_stream(self.device).synchronize()
+        self._last_lr = float(host[6])
         return {'episode_returns': tuple(ep_host.numpy()),
                 'mean_episode_return': float(ep_host.mean()) if ep_host.numel() else float('nan'),
                 'total_loss': float(host[3]), 'pg_loss': float(host[0]), 'baseline_loss': float(host[1]),
