@@ -209,7 +209,7 @@ int srl_learner_apply_gradients(srl_learner_t* L, float* grad_norm_out, void* st
 
 /* Data-parallel apply step over peer memory, replacing ncclAllReduce + srl_learner_apply_gradients (impala_atari.py:344-346
  * on every rank): reduce-scatter of the flat gradient through NVLink loads, global-norm clip, optimizer and all-gather in ONE
- * cooperative kernel (see heads_optim.cu).  grads[i] / exchange[i] / ctl[i] (i < world) are rank i's gradient buffer, its
+ * cooperative kernel (see optim.cu).  grads[i] / exchange[i] / ctl[i] (i < world) are rank i's gradient buffer, its
  * exchange buffer (4 * ceil(n/4 / world) + 4 floats: the reduced slice the peers pull) and its 1 KiB control block, all
  * mapped into this process (symmetric memory / CUDA IPC); grads[rank] must be the buffer given to srl_learner_create; the
  * control blocks start zeroed.  Every rank must call it once per step.  On return (stream order) the

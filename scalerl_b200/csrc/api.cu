@@ -124,7 +124,7 @@ extern "C" int srl_rmsprop_step(float* params, const float* grads, float* square
 extern "C" int srl_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, const float* coef, float lr,
                              float beta1, float beta2, float eps, int step, void* stream) {
   REQ(params && grads && exp_avg && exp_avg_sq && n >= 0 && step >= 1, "adam: bad argument");
-  CU(launch_adam(params, grads, exp_avg, exp_avg_sq, n, coef, lr, beta1, beta2, eps, step, nullptr, (cudaStream_t)stream), "adam");
+  CU(launch_adam(params, grads, exp_avg, exp_avg_sq, n, coef, lr, beta1, beta2, eps, step, (cudaStream_t)stream), "adam");
   return 0;
 }
 
@@ -356,6 +356,7 @@ extern "C" int srl_learner_destroy(srl_learner_t* L) {
 extern "C" int srl_debug_kernel_timeline(void* buffer) {
 #ifdef SRL_KSTAMP
   kstamp_set_encoder((unsigned long long*)buffer); kstamp_set_vtrace((unsigned long long*)buffer); kstamp_set_heads((unsigned long long*)buffer);
+  kstamp_set_optim((unsigned long long*)buffer);
   cudaError_t e = cudaDeviceSynchronize();
   return e == cudaSuccess ? 0 : cuda_fail(e, "debug_kernel_timeline");
 #else
@@ -661,24 +662,25 @@ extern "C" int srl_learner_forward_backward_lstm(srl_learner_t* L, const uint8_t
   return 0;
 }
 
-extern "C" int srl_learner_apply_gradients(srl_learner_t* L, float* grad_norm_out, void* stream) {
-  REQ(L, "learner is NULL");
-  cudaStream_t st = (cudaStream_t)stream;
+// clip_grad_norm_ + optimizer in one cooperative kernel (profile slot: optimizer); P: the data-parallel step over these peers
+static int apply_impl(srl_learner_t* L, const DpPeers* P, float* grad_norm_out, cudaStream_t st) {
   const srl_config_t& c = L->cfg;
+  const bool adam = c.optimizer != 0;
   L->pf.st = st;
   L->step += 1;
-  // clip_grad_norm_ + optimizer in one cooperative kernel (profile slot: optimizer)
+  const OptStep o = {adam ? 1 : 0, L->params, L->grads, L->opt0, adam ? L->opt1 : nullptr, L->nparams, c.max_grad_norm, L->coef,
+                     L->scratch + 2048, c.learning_rate, adam ? c.adam_beta1 : c.alpha, adam ? c.adam_beta2 : 0.f,
+                     adam ? c.adam_eps : c.epsilon, L->step, L->dstep, L->ox};
   L->pf.b(PS_OPTIMIZER);
-  if (c.optimizer == 0) {
-    CU(launch_clip_optim(0, L->params, L->grads, L->opt0, nullptr, L->nparams, c.max_grad_norm, L->coef, L->scratch + 2048, c.learning_rate,
-                         c.alpha, 0.f, c.epsilon, L->step, L->dstep, L->ox, st), "clip+rmsprop");
-  } else {
-    CU(launch_clip_optim(1, L->params, L->grads, L->opt0, L->opt1, L->nparams, c.max_grad_norm, L->coef, L->scratch + 2048, c.learning_rate,
-                         c.adam_beta1, c.adam_beta2, c.adam_eps, L->step, L->dstep, L->ox, st), "clip+adam");
-  }
+  CU(P ? launch_dp_clip_optim(o, *P, st) : launch_clip_optim(o, st), P ? (adam ? "dp clip+adam" : "dp clip+rmsprop") : (adam ? "clip+adam" : "clip+rmsprop"));
   L->pf.e(PS_OPTIMIZER);
   if (grad_norm_out) CU(cudaMemcpyAsync(grad_norm_out, L->coef, (L->report_lr ? 3 : 2) * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy coef");
   return 0;
+}
+
+extern "C" int srl_learner_apply_gradients(srl_learner_t* L, float* grad_norm_out, void* stream) {
+  REQ(L, "learner is NULL");
+  return apply_impl(L, nullptr, grad_norm_out, (cudaStream_t)stream);
 }
 
 extern "C" int srl_learner_apply_gradients_dp(srl_learner_t* L, const srl_dp_peers_t* peers, float* grad_norm_out, void* stream) {
@@ -686,8 +688,6 @@ extern "C" int srl_learner_apply_gradients_dp(srl_learner_t* L, const srl_dp_pee
   REQ(peers->world >= 2 && peers->world <= 8 && peers->rank >= 0 && peers->rank < peers->world, "apply_gradients_dp: world=%d rank=%d",
       peers->world, peers->rank);
   REQ(peers->grads[peers->rank] == (void*)L->grads, "apply_gradients_dp: grads[rank] must be the learner's gradient buffer");
-  cudaStream_t st = (cudaStream_t)stream;
-  const srl_config_t& c = L->cfg;
   DpPeers P;
   for (int i = 0; i < 8; ++i) {
     P.g[i] = i < peers->world ? (float*)peers->grads[i] : nullptr;
@@ -696,19 +696,7 @@ extern "C" int srl_learner_apply_gradients_dp(srl_learner_t* L, const srl_dp_pee
     REQ(i >= peers->world || (P.g[i] && P.ctl[i] && P.rs[i]), "apply_gradients_dp: NULL peer pointer %d", i);
   }
   P.rank = peers->rank; P.world = peers->world; P.mc_g = (float*)peers->grads_multicast;
-  L->pf.st = st;
-  L->step += 1;
-  L->pf.b(PS_OPTIMIZER);
-  if (c.optimizer == 0) {
-    CU(launch_dp_clip_optim(0, L->params, L->grads, L->opt0, nullptr, L->nparams, c.max_grad_norm, L->coef, L->scratch + 2048,
-                            c.learning_rate, c.alpha, 0.f, c.epsilon, L->step, L->dstep, P, L->ox, st), "dp clip+rmsprop");
-  } else {
-    CU(launch_dp_clip_optim(1, L->params, L->grads, L->opt0, L->opt1, L->nparams, c.max_grad_norm, L->coef, L->scratch + 2048,
-                            c.learning_rate, c.adam_beta1, c.adam_beta2, c.adam_eps, L->step, L->dstep, P, L->ox, st), "dp clip+adam");
-  }
-  L->pf.e(PS_OPTIMIZER);
-  if (grad_norm_out) CU(cudaMemcpyAsync(grad_norm_out, L->coef, (L->report_lr ? 3 : 2) * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy coef");
-  return 0;
+  return apply_impl(L, &P, grad_norm_out, (cudaStream_t)stream);
 }
 
 extern "C" int srl_learner_set_profiling(srl_learner_t* L, int enable) {

@@ -58,6 +58,7 @@ inline cudaError_t ensure_max_dynamic_smem(PerDeviceOnce& once, K kernel, int by
 }
 
 void kstamp_set_encoder(unsigned long long*); void kstamp_set_vtrace(unsigned long long*); void kstamp_set_heads(unsigned long long*);   // diagnostics build (common.cuh)
+void kstamp_set_optim(unsigned long long*);
 
 struct SideStream {
   cudaStream_t side = nullptr;      // fc wgrad, weight re-pack
@@ -77,7 +78,7 @@ constexpr int WS_TOTAL = WS_W1 + 2 * 128 * 32;
 constexpr int WG_PART_CTAS = 160;              // most CTAs a wgrad launch may use
 constexpr int WSP_W3 = 5 * 128 * 64 + 64, WSP_W2 = 4 * 128 * 64 + 64, WSP_W1 = 2 * 128 * 32 + 32;
 constexpr int64_t WSP_TOTAL = (int64_t)WG_PART_CTAS * (WSP_W3 + WSP_W2 + WSP_W1);
-constexpr int HEAD_GROUPS = 32;                // slab groups (partial sums) of the head weight gradients (heads_optim.cu)
+constexpr int HEAD_GROUPS = 32;                // slab groups (partial sums) of the head weight gradients (heads.cu)
 
 // ---- vtrace.cu
 cudaError_t launch_vtrace_iw(const float* log_rhos, const float* discounts, const float* rewards, const float* values,
@@ -103,7 +104,7 @@ cudaError_t launch_impala_tail(const float* bl, const float* tl, const float* ba
                                float clip_pg, float baseline_cost, float entropy_cost, float* vs, float* pg, float* dlogits,
                                float* dbaseline, float* losses, float* scratch, cudaStream_t st);
 
-// ---- heads_optim.cu
+// ---- heads.cu
 // hpart: FC_SPLITS split-K partials [s][N][512] of the fc layer; writes h = relu(sum_s hpart + bfc) and the head outputs
 cudaError_t launch_head_fwd(const float* hpart, int nsplit, const float* bfc, float* h, const float* reward, const int64_t* action,
                             const float* Wp, const float* bp, const float* Wb, const float* bb, int N, int A, float* logits,
@@ -120,6 +121,8 @@ cudaError_t launch_head_dense_bwd(const float* X, const float* dlogits, const fl
 cudaError_t launch_dcore_to_dh(const float* dcore, const float* h, int N, int A, __nv_bfloat16* dh, cudaStream_t st);
 cudaError_t launch_unpack_slots(const uint8_t* staging, int64_t slot_bytes, const int64_t* off6, int T, int B, int A, uint8_t* obs, float* reward,
                                 uint8_t* done, int64_t* action, float* logits, float* episode_return, cudaStream_t st);
+
+// ---- optim.cu
 // learning-rate schedule and RMSprop momentum of the fused clip + optimizer step (srl_learner_set_lr_schedule / _set_momentum).
 // The default value is the plain step: constant lr, no momentum.
 enum { SCHED_CONSTANT = 0, SCHED_LINEAR = 1 };
@@ -130,19 +133,29 @@ struct OptExtra {
   float* buf = nullptr;                             // momentum buffer, parameter layout (null: no momentum)
   float momentum = 0.f;
 };
-cudaError_t launch_clip_optim(int optimizer, float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef,
-                              float* scratch, float lr, float a, float b, float eps, int step, int* dstep, const OptExtra& x,
-                              cudaStream_t st);
+// one fused clip + optimizer step.  optimizer 0 = RMSprop: s0 = square_avg, a = alpha; 1 = Adam: s0, s1 = exp_avg, exp_avg_sq,
+// a, b = beta1, beta2.  coef receives the norm, the clip coefficient and (but for the constant-lr, no-momentum step) the lr;
+// scratch holds the block partials.  The step count is *dstep + 1 (step when dstep is null); the kernel stores it back to *dstep.
+struct OptStep {
+  int optimizer;
+  float *p, *g, *s0, *s1;
+  int64_t n;
+  float max_norm;
+  float *coef, *scratch;
+  float lr, a, b, eps;
+  int step;
+  int* dstep;
+  OptExtra x;
+};
+cudaError_t launch_clip_optim(const OptStep& o, cudaStream_t st);
 struct DpPeers { float* g[8]; float* rs[8]; unsigned* ctl[8]; int rank, world; float* mc_g; };      // peer-mapped gradient buffers / control blocks; mc_g: NVLS multicast address of the gradient buffers (or null)
-cudaError_t launch_dp_clip_optim(int optimizer, float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef,
-                                 float* scratch, float lr, float a, float b, float eps, int step, int* dstep, const DpPeers& P,
-                                 const OptExtra& x, cudaStream_t st);
+cudaError_t launch_dp_clip_optim(const OptStep& o, const DpPeers& P, cudaStream_t st);
 cudaError_t launch_snapshot_if_finite(float* dst, const float* src, int64_t n, const float* losses, cudaStream_t st);
 cudaError_t launch_grad_norm(const float* g, int64_t n, float max_norm, float* coef, float* scratch, cudaStream_t st);
 cudaError_t launch_rmsprop(float* p, const float* g, float* v, int64_t n, const float* coef, float lr, float alpha, float eps,
                            cudaStream_t st);
 cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, const float* coef, float lr, float b1, float b2, float eps,
-                        int step, int* dstep, cudaStream_t st);
+                        int step, cudaStream_t st);
 
 // ---- encoder.cu
 // packed bf16 operand copies of the conv/fc weights (element offsets into one buffer)

@@ -128,7 +128,7 @@ def fc_fwd(a3, Wfc, bfc):
 
 
 def core(h, reward, action, A):
-    """core = [h, clamp(reward, -1, 1), one_hot(action)] (heads_optim.cu head_fwd_kernel)"""
+    """core = [h, clamp(reward, -1, 1), one_hot(action)] (heads.cu head_fwd_kernel)"""
     N = h.shape[0]
     return torch.cat([h.to(F64), reward.reshape(N, 1).to(F64).clamp(-1, 1),
                       F.one_hot(action.reshape(N), A).to(F64)], 1)

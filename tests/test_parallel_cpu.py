@@ -39,8 +39,8 @@ def _worker(rank, world, port, out_q):
     flat = torch.cat([out['grads'][k].reshape(-1) for k in O.PARAM_ORDER])
     losses = torch.tensor([out['pg_loss'], out['baseline_loss'], out['entropy_loss'], out['total_loss']])
     par.allreduce_sum_(flat, losses)
-    if rank == 0:
-        out_q.put((flat, losses))
+    if rank == 0:      # numpy arrays travel by value: a tensor would be shared through a descriptor that this process must outlive
+        out_q.put((flat.numpy(), losses.numpy()))
     dist.destroy_process_group()
 
 
@@ -55,7 +55,7 @@ def test_two_rank_gloo_matches_full_batch():
     procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()
-    flat, losses = q.get()
+    flat, losses = (torch.from_numpy(a) for a in q.get())
     for p in procs:
         p.join(60)
         assert p.exitcode == 0
