@@ -258,8 +258,7 @@ static int workspace_table(srl_learner* L, WsRow* t) {
   t[n++] = ws_row(nullptr, 4096, &L->scratch);
   t[n++] = ws_row(nullptr, 4, &L->coef);
   t[n++] = ws_row(nullptr, 4, &L->dstep);
-  t[n++] = ws_row(nullptr, WS_TOTAL, &b.wgrad_ws);
-  t[n++] = ws_row(nullptr, WSP_TOTAL, &b.wgrad_part);
+  t[n++] = ws_row("wgrad_part", WSP_TOTAL, &b.wgrad_part);
   t[n++] = ws_row(nullptr, HEAD_GROUPS * (A + 1) * (514 + A), &L->head_part);
   t[n++] = ws_row("a3t", NF * 49 * 64, &b.a3t);
   if (c.use_lstm) {

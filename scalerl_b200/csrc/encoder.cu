@@ -294,58 +294,76 @@ static int side_wgrad_ctas() {
   return v;
 }
 
-// per-CTA partial slices -> workspace (float4 per thread) and bias gradients (added into the pre-zeroed gradient), summed in CTA order
-__global__ void __launch_bounds__(256) conv_wgrad_reduce_kernel(const float* __restrict__ part3, int n3, const float* __restrict__ part2, int n2,
-                                                                const float* __restrict__ part1, int n1, float* __restrict__ ws,
-                                                                float* __restrict__ db3, float* __restrict__ db2, float* __restrict__ db1) {
-  pdl_wait(55);    // launched with programmatic stream serialization: see common.cuh
-  pdl_launch();
-  constexpr int A3 = 5 * 128 * 64 / 4, A2 = 4 * 128 * 64 / 4, A1 = 2 * 128 * 32 / 4;     // float4s of accumulators per slice
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  auto sum4 = [](const float* part, int n, int stride, int k) {
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int c = 0; c < n; ++c) {
-      const float4 v = __ldg(reinterpret_cast<const float4*>(part + (size_t)c * stride) + k);
-      s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-    }
-    return s;
-  };
-  auto sum1 = [](const float* part, int n, int stride, int k) {
-    float s = 0.f;
-    for (int c = 0; c < n; ++c) s += __ldg(part + (size_t)c * stride + k);
-    return s;
-  };
-  float4* w4 = reinterpret_cast<float4*>(ws);
-  if (i < A3) w4[WS_W3 / 4 + i] = sum4(part3, n3, WSP_W3, i);
-  else if (i < A3 + A2) w4[WS_W2 / 4 + i - A3] = sum4(part2, n2, WSP_W2, i - A3);
-  else if (i < A3 + A2 + A1) w4[WS_W1 / 4 + i - A3 - A2] = sum4(part1, n1, WSP_W1, i - A3 - A2);
-  else {
-    const int k = i - (A3 + A2 + A1);
-    if (k < 64) db3[k] += sum1(part3, n3, WSP_W3, 4 * A3 + k);
-    else if (k < 128) db2[k - 64] += sum1(part2, n2, WSP_W2, 4 * A2 + k - 64);
-    else if (k < 160) db1[k - 128] += sum1(part1, n1, WSP_W1, 4 * A1 + k - 128);
+// Per-CTA partial slices of one conv wgrad launch (res_problems.cuh) -> that layer's PyTorch-layout weight gradient, and its bias
+// gradient added into the pre-zeroed g.b*.  A slice row is one K index of the wgrad GEMM (CO floats, one per output channel).
+// A tile is NR slice rows x 8 output channels chosen so that its NR entries of each channel's PyTorch row are consecutive:
+// dW[co0 + j][NR * rg + i] = sum over CTAs of slice[row(rg, i)][co0 + j].  The block copies the tile of every slice into shared
+// memory (16-byte cp.async, 32-byte runs of the slice rows, all of them in flight at once), then thread e = 8 i + j adds its element
+// over the slices in CTA order -- the same fp32 additions, in the same order, for every CTA count and stream placement -- and
+// stores it.  The block after the last tile does the bias the same way.
+// KID: diagnostics timeline id.  conv1's reduce, the one on the main chain, is stamped as `conv_wgrad_finalize` (the profile slot it
+// keeps); the side-stream reduces are not stamped (0).
+struct WgradReduce3 {   // dW3[co][c*9 + tap] = slice[tap*64 + c][co]          tile rg = 2 channels c x 9 taps
+  static constexpr int KID = 0, CO = 64, BIAS = 64, PART = WSP_W3, NR = 18, ROW_GROUPS = 32;
+  static constexpr bool FRAMES_U8 = false;
+  SRL_DEVINL static int row(int rg, int i) { return (i % 9) * 64 + 2 * rg + i / 9; }
+};
+struct WgradReduce2 {   // dW2[co][c*16 + kh*4 + kw] = slice[kh*128 + kw*32 + c][co]       tile rg = channel c x 16 taps
+  static constexpr int KID = 0, CO = 64, BIAS = 64, PART = WSP_W2, NR = 16, ROW_GROUPS = 32;
+  static constexpr bool FRAMES_U8 = false;
+  SRL_DEVINL static int row(int rg, int i) { return (i >> 2) * 128 + (i & 3) * 32 + rg; }
+};
+struct WgradReduce1 {   // dW1[co][c*64 + kh*8 + kw] = slice[(kh>>2)*128 + (kw>>2)*64 + c*16 + (kh&3)*4 + (kw&3)][co] / 255
+  static constexpr int KID = 51, CO = 32, BIAS = 32, PART = WSP_W1, NR = 16, ROW_GROUPS = 16;
+  static constexpr bool FRAMES_U8 = true;          // the frames entered the GEMM as u8 values: the 1/255 is applied to the sum
+  // rg = (c, kh2, dy >> 1), i = ((dy & 1), kw): kh = 4 kh2 + dy
+  SRL_DEVINL static int row(int rg, int i) {
+    const int c = rg >> 2, kh2 = (rg >> 1) & 1, dy = 2 * (rg & 1) + (i >> 3), kw = i & 7;
+    return kh2 * 128 + (kw >> 2) * 64 + c * 16 + dy * 4 + (kw & 3);
   }
+};
+template <class L>
+__global__ void __launch_bounds__(L::NR * 8) conv_wgrad_reduce_kernel(const float* __restrict__ part, int n, float* __restrict__ g,
+                                                                       float* __restrict__ db) {
+  constexpr int CG = L::CO / 8, TILES = L::ROW_GROUPS * CG;
+  static_assert(L::BIAS <= 8 * L::NR, "the bias block fits the tile's threads and shared memory");
+  extern __shared__ __align__(16) float stage[];          // [n][NR][8] (tile) or [n][BIAS] (bias block)
+  pdl_wait(L::KID);    // (not launched with the attribute: returns at once; names the kernel in the diagnostics timeline)
+  pdl_launch();
+  const int t = threadIdx.x, rg = blockIdx.x / CG, co0 = (blockIdx.x % CG) * 8;
+  const bool bias = blockIdx.x == TILES;
+  const int per = bias ? L::BIAS / 4 : 2 * L::NR;         // 16-byte pieces per slice
+  for (int k = t; k < n * per; k += L::NR * 8) {
+    const int c = k / per, q = k - c * per;
+    const float* src = part + (size_t)c * L::PART + (bias ? L::PART - L::BIAS + 4 * q : L::row(rg, q >> 1) * L::CO + co0 + 4 * (q & 1));
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(stage + 4 * k)), "l"(src) : "memory");
+  }
+  asm volatile("cp.async.wait_all;" ::: "memory");
+  __syncthreads();
+  const int w = bias ? L::BIAS : 8 * L::NR;
+  if (t >= w) return;
+  float s = 0.f;
+  for (int c = 0; c < n; ++c) s += stage[c * w + t];
+  if (bias) db[t] += s;
+  else g[(size_t)(co0 + (t & 7)) * (L::ROW_GROUPS * L::NR) + L::NR * rg + (t >> 3)] = L::FRAMES_U8 ? s * (1.0f / 255.0f) : s;
 }
 
-// workspace [tap-block][row][co] -> PyTorch-layout conv weight gradients (plain stores), and re-zero what was read
-__global__ void __launch_bounds__(256) conv_wgrad_finalize_kernel(float* __restrict__ ws, float* __restrict__ g1, float* __restrict__ g2,
-                                                                  float* __restrict__ g3) {
-  pdl_wait(51);    // launched with programmatic stream serialization: see common.cuh
-  pdl_launch();
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < 36864) {                       // dW3[co][c][tap] = ws3[tap>>1][(tap&1)*64 + c][co]
-    const int co = i / 576, r = i - co * 576, c = r / 9, tap = r - c * 9;
-    float* q = ws + WS_W3 + ((tap >> 1) * 128 + (tap & 1) * 64 + c) * 64 + co;
-    g3[i] = *q; *q = 0.f;        // self-cleaning: the workspace is zero again for the next step
-  } else if (i < 36864 + 32768) {        // dW2[co][c][kh][kw] = ws2[kh][kw*32 + c][co]
-    const int e = i - 36864, co = e >> 9, r = e & 511, c = r >> 4, kh = (r >> 2) & 3, kw = r & 3;
-    float* q = ws + WS_W2 + (kh * 128 + kw * 32 + c) * 64 + co;
-    g2[e] = *q; *q = 0.f;
-  } else if (i < 36864 + 32768 + 8192) { // dW1[co][c][kh][kw] = ws1[kh>>2][(kw>>2)*64 + c*16 + (kh&3)*4 + (kw&3)][co] / 255
-    const int e = i - 36864 - 32768, co = e >> 8, k = e & 255, c = k >> 6, kh = (k >> 3) & 7, kw = k & 7;
-    float* q = ws + WS_W1 + ((kh >> 2) * 128 + (kw >> 2) * 64 + c * 16 + (kh & 3) * 4 + (kw & 3)) * 32 + co;
-    g1[e] = *q * (1.0f / 255.0f); *q = 0.f;
-  }
+// The reduces gate the step's join and the optimizer, so they take the device's greatest stream priority: a side stream's reduce is
+// not queued behind the other side streams' GEMM CTAs.  They are launched without programmatic stream serialization: the wgrad
+// kernels release their dependents at once, and blocks parked in pdl_wait() for a whole wgrad would hold shared memory that the
+// other streams' GEMM CTAs need (measured: LSTM at T=100, B=128 ran 0.8 % slower with it).
+template <class L>
+static cudaError_t launch_wgrad_reduce(const float* part, int n, float* g, float* db, cudaStream_t st) {
+  static PerDeviceOnce once;
+  SRL_TRY(ensure_max_dynamic_smem(once, conv_wgrad_reduce_kernel<L>, WG_PART_CTAS * L::NR * 32));
+  static const int greatest = [] { int lo = 0, hi = 0; return cudaDeviceGetStreamPriorityRange(&lo, &hi) == cudaSuccess ? hi : 0; }();
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(L::ROW_GROUPS * (L::CO / 8) + 1); cfg.blockDim = dim3(L::NR * 8); cfg.dynamicSmemBytes = (size_t)n * L::NR * 32; cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributePriority;
+  attr[0].val.priority = greatest;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, conv_wgrad_reduce_kernel<L>, part, n, g, db);
 }
 
 cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, const EncoderBuffers& buf, const TmaMaps& maps, int mode,
@@ -420,26 +438,31 @@ cudaError_t encoder_backward(int frames, const EncoderBuffers& buf, const ParamP
   int n3 = 0, n2 = 0, n1 = 0;       // CTAs (partial slices) of the three wgrad launches
   { RConv3Wgrad::Params q{maps.hi.a2_w, maps.hi.da3g_b, maps.lo.a2_w, maps.lo.da3g_b, part3, frames * 81, 0};
     p2.b(PS_CONV3_WGRAD); SRL_TRY(res_wgrad_launch<RConv3Wgrad>(q, side_wgrad_ctas(), s2, &n3, sp)); p2.e(PS_CONV3_WGRAD); }
+  // forked: each side-stream layer is reduced on its own stream as soon as its wgrad ends; otherwise all three reduces run at the end,
+  // together in the conv_wgrad_finalize profile slot
+  if (fork) SRL_TRY(launch_wgrad_reduce<WgradReduce3>(part3, n3, g.w3, g.b3, s2));
   { RConv3Dgrad::Params q{maps.hi.da3g_w, maps.hi.w3d, maps.lo.da3g_w, maps.lo.w3d, buf.hi.a2, buf.hi.da2, buf.lo.da2, frames};
     pf.b(PS_CONV3_DGRAD); SRL_TRY(res_fwd_launch<RConv3Dgrad>(q, cdiv(frames * 81, 128), bwd_ctas(), st, sp)); pf.e(PS_CONV3_DGRAD); }
   if (fork) { SRL_TRY(cudaEventRecord(ss.ev[2], st)); SRL_TRY(cudaStreamWaitEvent(s3, ss.ev[2], 0)); }
   { RConv2Wgrad::Params q{maps.hi.a1p0_w, maps.hi.a1p1_w, maps.hi.da2g_b, maps.lo.a1p0_w, maps.lo.a1p1_w, maps.lo.da2g_b, part2, frames * 100, 0};
     p3.b(PS_CONV2_WGRAD); SRL_TRY(res_wgrad_launch<RConv2Wgrad>(q, side_wgrad_ctas(), s3, &n2, sp)); p3.e(PS_CONV2_WGRAD); }
+  if (fork) SRL_TRY(launch_wgrad_reduce<WgradReduce2>(part2, n2, g.w2, g.b2, s3));
   { RConv2Dgrad::Params q{maps.hi.da2g_w, maps.hi.w2d, maps.lo.da2g_w, maps.lo.w2d, buf.hi.a1, buf.hi.da1, buf.lo.da1, frames, buf.NF};
     pf.b(PS_CONV2_DGRAD); SRL_TRY(res_fwd_launch<RConv2Dgrad>(q, cdiv(frames * 100, 128), bwd_ctas(), st, sp)); pf.e(PS_CONV2_DGRAD); }
   { RConv1Wgrad::Params q{maps.xs_w, maps.hi.da1g_b, maps.lo.da1g_b, part1, frames * 441, 0};
     pf.b(PS_CONV1_WGRAD); SRL_TRY(res_wgrad_launch<RConv1Wgrad>(q, bwd_ctas(), st, &n1, sp)); pf.e(PS_CONV1_WGRAD); }
-  if (fork) {      // join: fc wgrad (phase 2 only: phase 1 was joined by the caller of phase 0), conv3 wgrad, conv2 wgrad
+  pf.b(PS_WGRAD_FINALIZE);
+  if (!fork) {
+    SRL_TRY(launch_wgrad_reduce<WgradReduce3>(part3, n3, g.w3, g.b3, st));
+    SRL_TRY(launch_wgrad_reduce<WgradReduce2>(part2, n2, g.w2, g.b2, st));
+  }
+  SRL_TRY(launch_wgrad_reduce<WgradReduce1>(part1, n1, g.w1, g.b1, st));
+  pf.e(PS_WGRAD_FINALIZE);
+  if (fork) {      // join: fc wgrad (phase 2 only: phase 1 was joined by the caller of phase 0), conv3 and conv2 wgrad + reduce
     if (do_fc) { SRL_TRY(cudaStreamWaitEvent(st, ss.ev[4], 0)); }
     SRL_TRY(cudaEventRecord(ss.ev[3], s2)); SRL_TRY(cudaStreamWaitEvent(st, ss.ev[3], 0));
     SRL_TRY(cudaEventRecord(ss.ev[7], s3)); SRL_TRY(cudaStreamWaitEvent(st, ss.ev[7], 0));
   }
-  pf.b(PS_WGRAD_FINALIZE);
-  SRL_TRY(launch_chain(conv_wgrad_reduce_kernel, dim3((WS_TOTAL / 4 + 160 + 255) / 256), dim3(256), 0, st, (const float*)part3, n3,
-                       (const float*)part2, n2, (const float*)part1, n1, buf.wgrad_ws, g.b3, g.b2, g.b1));
-  SRL_TRY(launch_chain(conv_wgrad_finalize_kernel, dim3((36864 + 32768 + 8192 + 255) / 256), dim3(256), 0, st, buf.wgrad_ws, g.w1, g.w2, g.w3));
-  SRL_TRY(cudaGetLastError());
-  pf.e(PS_WGRAD_FINALIZE);
   return cudaSuccess;
 }
 

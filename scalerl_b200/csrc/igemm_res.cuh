@@ -440,7 +440,7 @@ __global__ void __launch_bounds__(ResWgradCfg<P, SPLIT>::THREADS, 1) res_wgrad_k
   }
 }
 
-// *ctas: the CTAs launched, i.e. the per-CTA partial slices conv_wgrad_reduce_kernel must add (0: nothing launched)
+// *ctas: the CTAs launched, i.e. the per-CTA partial slices conv_wgrad_reduce_kernel<layer> must add (0: nothing launched)
 template <class P, int SPLIT>
 cudaError_t res_wgrad_launch_t(typename P::Params p, int target_ctas, cudaStream_t stream, int* ctas) {
   using C = ResWgradCfg<P, SPLIT>;

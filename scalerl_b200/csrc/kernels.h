@@ -68,13 +68,9 @@ struct SideStream {
   cudaEvent_t ev[12] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
 };
 
-// conv weight-gradient workspace (fp32, the wgrad kernels' native [tap-block][row][co] order; res_problems.cuh), float offsets:
-constexpr int WS_W3 = 0;                       // [5 acc][128 rows][64 co]   (tap 9 half unused)
-constexpr int WS_W2 = WS_W3 + 5 * 128 * 64;    // [4 kh][128 rows][64 co]
-constexpr int WS_W1 = WS_W2 + 4 * 128 * 64;    // [2 kh2][128 rows][32 co]
-constexpr int WS_TOTAL = WS_W1 + 2 * 128 * 32;
-// per-CTA partials of the wgrad kernels (each CTA stores its accumulators and bias sums; conv_wgrad_reduce_kernel adds the CTAs in a
-// fixed order into the workspace above, so the gradients are the same bits on every run).  Floats per CTA: accumulators, then bias.
+// per-CTA partials of the wgrad kernels (each CTA stores its accumulators, in the kernel's native [tap-block][row][co] order, and its
+// bias sums; conv_wgrad_reduce_kernel<layer> adds the CTAs in a fixed order into the PyTorch-layout gradient, so the gradients are the
+// same bits on every run).  Floats per CTA: accumulators, then bias.
 constexpr int WG_PART_CTAS = 160;              // most CTAs a wgrad launch may use
 constexpr int WSP_W3 = 5 * 128 * 64 + 64, WSP_W2 = 4 * 128 * 64 + 64, WSP_W1 = 2 * 128 * 32 + 32;
 constexpr int64_t WSP_TOTAL = (int64_t)WG_PART_CTAS * (WSP_W3 + WSP_W2 + WSP_W1);
@@ -188,7 +184,6 @@ struct EncoderBuffers {   // row layouts: see res_problems.cuh
   __nv_bfloat16* a3t = nullptr;         // [NF][64*49]: a3 of the learning frames in fc.weight's own column order (c,h,w) -- fc wgrad's B operand (bf16 mode)
   float* hpart;                         // [FC_SPLITS][NF][512] split-K partials of the fc layer
   float* h;                             // [NF][512] fc output (post-ReLU), fp32
-  float* wgrad_ws;                      // conv weight-gradient accumulation workspace (res_problems.cuh: WS_TOTAL floats)
   float* wgrad_part;                    // per-CTA partials of the conv wgrad kernels (WSP_TOTAL floats)
   int NF;                               // frames the forward buffers were sized for (plane stride of a1)
 };

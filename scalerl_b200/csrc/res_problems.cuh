@@ -154,9 +154,7 @@ struct RConv2Dgrad {   // the 4 stride-parity classes share A (da2g at (i'-kh', 
 // ================================================================================================ wgrad
 // Every wgrad CTA stores its accumulators (and bias sums) in its own slice of the per-CTA partials, PART floats at
 // ws + blockIdx.x * PART, in the kernels' native [tap-block][row][co] order followed by the bias; conv_wgrad_reduce_kernel
-// (encoder.cu) adds the slices in CTA order into the workspace and the bias gradients, and conv_wgrad_finalize_kernel then
-// writes the PyTorch-layout gradient tensors.  Workspace offsets (floats):
-// (WS_W3 / WS_W2 / WS_W1 / WS_TOTAL are defined in kernels.h: the optimizer kernel reads the workspace too)
+// (encoder.cu, one launch per layer) adds the slices in CTA order straight into the PyTorch-layout weight gradient and the bias gradient.
 // Tap block b = 64 rows of dW (one m64 wgmma accumulator) = window rows starting blk_shift(b) in window blk_win(b).
 struct RConv3Wgrad {   // block b = tap b.  ws: [10 taps][64 c][64 co] fp32 (co contiguous; the tenth block is not written), db3
   static constexpr int KID = 21;        // diagnostics timeline id

@@ -725,7 +725,7 @@ class B200ImpalaLearner(BaseAgent):
         """copy of an internal activation buffer (tests only)"""
         p, n = C.c_void_p(), C.c_int64()
         _lib.check(self._L.srl_learner_debug_buffer(self._h, name.encode(), C.byref(p), C.byref(n)), 'debug_buffer')
-        fp32 = name in ('h', 'logits', 'baseline', 'dlogits', 'dbaseline')      # everything else (xs, a1.., da.., wpack, *_lo) is bf16
+        fp32 = name in ('h', 'logits', 'baseline', 'dlogits', 'dbaseline', 'wgrad_part')      # everything else (xs, a1.., da.., wpack, *_lo) is bf16
         dt = torch.float32 if fp32 else torch.bfloat16
         nbytes = n.value * (4 if fp32 else 2)
         out = torch.empty(n.value, dtype=dt, device=self.device)

@@ -10,7 +10,7 @@ import sys
 SLOT = {'RConv1Fwd': 'conv1_fwd', 'RConv2Fwd': 'conv2_fwd', 'RConv3Fwd': 'conv3_fwd', 'TFcFwd': 'fc_fwd', 'TFcWgrad': 'fc_wgrad',
         'TFcDgrad': 'fc_dgrad', 'RConv3Wgrad': 'conv3_wgrad', 'RConv3Dgrad': 'conv3_dgrad', 'RConv2Wgrad': 'conv2_wgrad',
         'RConv2Dgrad': 'conv2_dgrad', 'RConv1Wgrad': 'conv1_wgrad', 'obs_s2d_kernel': 'obs_s2d', 'column_step_kernel': 'vtrace_loss_tail',
-        'clip_optim_kernel': 'optimizer', 'conv_wgrad_finalize_kernel': 'conv_wgrad_finalize', 'pack_weights_kernel': 'pack_weights',
+        'clip_optim_kernel': 'optimizer', 'WgradReduce1': 'conv_wgrad_finalize', 'pack_weights_kernel': 'pack_weights',
         'head_wgrad_kernel': 'head_bwd'}
 
 
