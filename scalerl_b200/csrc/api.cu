@@ -56,6 +56,17 @@ extern "C" int srl_vtrace_from_logits(const float* bl, const float* tl, const in
   return 0;
 }
 
+// a tail's shape and loss settings from c (fields assigned by name: several neighbours share a type)
+static TailStep tail_step(const srl_config_t& c, const float* bl, const int64_t* action, const float* reward, const uint8_t* done, float* vs,
+                          float* pg, float* dlogits, float* dbaseline, float* losses, float* scratch) {
+  TailStep s;
+  s.bl = bl; s.action = action; s.reward = reward; s.done = done; s.T = c.T; s.B = c.B; s.A = c.A;
+  s.discounting = c.discounting; s.clip_reward = c.reward_clip_abs_one; s.clip_rho = c.clip_rho_threshold; s.clip_pg = c.clip_pg_rho_threshold;
+  s.baseline_cost = c.baseline_cost; s.entropy_cost = c.entropy_cost;
+  s.vs = vs; s.pg = pg; s.dlogits = dlogits; s.dbaseline = dbaseline; s.losses = losses; s.scratch = scratch;
+  return s;
+}
+
 extern "C" int srl_impala_loss_and_head_grads(const float* bl, const float* tl, const float* baseline, const int64_t* action,
                                               const float* reward, const uint8_t* done, int T, int B, int A, float discounting,
                                               int reward_clip_abs_one, float clip_rho, float clip_pg, float baseline_cost,
@@ -63,8 +74,11 @@ extern "C" int srl_impala_loss_and_head_grads(const float* bl, const float* tl, 
                                               float* scratch, void* stream) {
   REQ(T >= 1 && B >= 1 && A >= 1, "impala_loss: bad shape T=%d B=%d A=%d", T, B, A);
   REQ(bl && tl && baseline && action && reward && done && dlogits && dbaseline && losses && scratch, "impala_loss: NULL pointer");
-  CU(launch_impala_tail(bl, tl, baseline, action, reward, done, T, B, A, discounting, reward_clip_abs_one, clip_rho, clip_pg,
-                        baseline_cost, entropy_cost, vs, pg, dlogits, dbaseline, losses, scratch, (cudaStream_t)stream), "impala_tail");
+  srl_config_t c = {};
+  c.T = T; c.B = B; c.A = A; c.discounting = discounting; c.reward_clip_abs_one = reward_clip_abs_one;
+  c.clip_rho_threshold = clip_rho; c.clip_pg_rho_threshold = clip_pg; c.baseline_cost = baseline_cost; c.entropy_cost = entropy_cost;
+  CU(launch_impala_tail(tail_step(c, bl, action, reward, done, vs, pg, dlogits, dbaseline, losses, scratch), tl, baseline, (cudaStream_t)stream),
+     "impala_tail");
   return 0;
 }
 
@@ -526,24 +540,21 @@ static int fb_begin(srl_learner* L, const uint8_t* obs, const float* reward, con
   const int NF = (c.T + 1) * c.B, NB = c.T * c.B;
   // heads + V-trace/losses + dh: one fused column kernel when its shared-memory footprint fits, else three kernels
   const bool fused = L->column_fusion && column_step_supported(c.T, c.B, c.A);
+  const TailStep ts = tail_step(c, behavior_logits, action, reward, done, vs, pg_advantages, L->dlogits, L->dbaseline, losses, L->scratch);
   int rc;
   if (fused) {
     REQ(!L->cfg.use_lstm, "this learner was created with use_lstm=1: call the *_lstm entry points");
     rc = encode_impl(L, obs, NF, st, true);
     if (rc) return rc;
     L->pf.b(PS_TAIL);
-    CU(launch_column_step(L->buf.hpart, FC_SPLITS, L->P.bf, L->buf.h, reward, action, done, behavior_logits, L->P.wp, L->P.bp, L->P.wb,
-                          L->P.bb, c.T, c.B, c.A, c.discounting, c.reward_clip_abs_one, c.clip_rho_threshold, c.clip_pg_rho_threshold,
-                          c.baseline_cost, c.entropy_cost, L->logits, L->baseline, vs, pg_advantages, L->dlogits, L->dbaseline, L->buf.hi.dh,
-                          losses, L->scratch, st, L->buf.lo.dh), "column_step");
+    CU(launch_column_step(ts, L->buf.hpart, FC_SPLITS, L->P.bf, L->buf.h, L->P.wp, L->P.bp, L->P.wb, L->P.bb, L->logits, L->baseline,
+                          L->buf.hi.dh, L->buf.lo.dh, st), "column_step");
     L->pf.e(PS_TAIL);
   } else {
     rc = forward_impl(L, obs, reward, action, NF, L->logits, L->baseline, st, true);
     if (rc) return rc;
     L->pf.b(PS_TAIL);
-    CU(launch_impala_tail(behavior_logits, L->logits, L->baseline, action, reward, done, c.T, c.B, c.A, c.discounting,
-                          c.reward_clip_abs_one, c.clip_rho_threshold, c.clip_pg_rho_threshold, c.baseline_cost, c.entropy_cost, vs,
-                          pg_advantages, L->dlogits, L->dbaseline, losses, L->scratch, st), "impala_tail");
+    CU(launch_impala_tail(ts, L->logits, L->baseline, st), "impala_tail");
     L->pf.e(PS_TAIL);
   }
   L->pf.b(PS_HEAD_BWD);
@@ -646,9 +657,8 @@ extern "C" int srl_learner_forward_backward_lstm(srl_learner_t* L, const uint8_t
   const int NB = c.T * c.B;
   int rc = forward_lstm_impl(L, obs, reward, done, action, h0, c0, L->logits, L->baseline, nullptr, nullptr, st);
   if (rc) return rc;
-  CU(launch_impala_tail(behavior_logits, L->logits, L->baseline, action, reward, done, c.T, c.B, c.A, c.discounting, c.reward_clip_abs_one,
-                        c.clip_rho_threshold, c.clip_pg_rho_threshold, c.baseline_cost, c.entropy_cost, vs, pg_advantages, L->dlogits,
-                        L->dbaseline, losses, L->scratch, st), "impala_tail");
+  CU(launch_impala_tail(tail_step(c, behavior_logits, action, reward, done, vs, pg_advantages, L->dlogits, L->dbaseline, losses, L->scratch),
+                        L->logits, L->baseline, st), "impala_tail");
   CU(cudaMemsetAsync(L->grads, 0, L->small_len * sizeof(float), st), "zero small grads");
   CU(cudaMemsetAsync(L->grads + L->lstm_off0, 0, L->lstm_len * sizeof(float), st), "zero lstm grads");
   CU(launch_head_dense_bwd(L->lstm_out, L->dlogits, L->dbaseline, L->P.wp, L->P.wb, NB, c.A, L->dout, L->G.wp, L->G.bp, L->G.wb, L->G.bb, st),

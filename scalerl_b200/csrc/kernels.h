@@ -88,17 +88,21 @@ cudaError_t launch_policy_rows_bwd(const float* logits, const int64_t* actions, 
                                    float* dlogits, cudaStream_t st);
 cudaError_t launch_sample_actions(const float* logits, const float* u, int64_t N, int A, int64_t* actions, cudaStream_t st);
 cudaError_t launch_reduce_sum(const float* x, int64_t n, int square, float scale, float* out, cudaStream_t st);
+// one learner tail over [T+1, B] batch rows (V-trace, losses, head gradients): trajectory (rows 1..T used), shape, srl_config_t's loss
+// settings (clip < 0: none), outputs as srl_impala_loss_and_head_grads (vs, pg may be null; scratch zero before the first launch)
+struct TailStep {
+  const float* bl; const int64_t* action; const float* reward; const uint8_t* done;
+  int T, B, A;
+  float discounting; int clip_reward; float clip_rho, clip_pg, baseline_cost, entropy_cost;
+  float *vs, *pg, *dlogits, *dbaseline, *losses, *scratch;
+};
+// the tail from target logits tl [T+1][B][A] and baseline [T+1][B] in global memory
+cudaError_t launch_impala_tail(const TailStep& s, const float* tl, const float* baseline, cudaStream_t st);
+// the heads from the fc layer's split-K partials, then the tail, then dh (and dh_lo when not null), one block per column
 bool column_step_supported(int T, int B, int A);
-cudaError_t launch_column_step(const float* hpart, int nsplit, const float* bfc, float* h, const float* reward, const int64_t* action,
-                               const uint8_t* done, const float* bl, const float* Wp, const float* bp, const float* Wb, const float* bb,
-                               int T, int B, int A, float discounting, int clip_reward, float clip_rho, float clip_pg,
-                               float baseline_cost, float entropy_cost, float* logits, float* baseline, float* vs, float* pg,
-                               float* dlogits, float* dbaseline, __nv_bfloat16* dh, float* losses, float* scratch, cudaStream_t st,
-                               __nv_bfloat16* dh_lo = nullptr);
-cudaError_t launch_impala_tail(const float* bl, const float* tl, const float* baseline, const int64_t* action, const float* reward,
-                               const uint8_t* done, int T, int B, int A, float discounting, int clip_reward, float clip_rho,
-                               float clip_pg, float baseline_cost, float entropy_cost, float* vs, float* pg, float* dlogits,
-                               float* dbaseline, float* losses, float* scratch, cudaStream_t st);
+cudaError_t launch_column_step(const TailStep& s, const float* hpart, int nsplit, const float* bfc, float* h, const float* Wp, const float* bp,
+                               const float* Wb, const float* bb, float* logits, float* baseline, __nv_bfloat16* dh, __nv_bfloat16* dh_lo,
+                               cudaStream_t st);
 
 // ---- heads.cu
 // hpart: FC_SPLITS split-K partials [s][N][512] of the fc layer; writes h = relu(sum_s hpart + bfc) and the head outputs

@@ -7,15 +7,18 @@
 //   vtrace_logits_kernel       from_logits (log-softmax gather for both policies, then the recursion)
 //   impala_tail_kernel         one pass over the [T+1,B] batch rows: shifts, reward clip, discounts, V-trace,
 //                              pg/baseline/entropy losses (deterministic two-level reduction), dlogits, dbaseline
+//   impala_tail_warp_kernel    the same tail with one warp per column (tail_column_warp), for B <= 2048
+// Shared device pieces (a copy that stays written out says why at the copy: through the helper, that kernel compiles differently):
+//   row_lse / row_logp / row_entropy   log-softmax and sum_a p log p of one row: impala_tail_kernel, policy row operators
+//   scan_compose                       the warp's Kogge-Stone suffix composition: vtrace_iw_scan_kernel, tail_column_warp
+//   tail_reward_discount               the tail's per-step reward clip and discount: impala_tail_kernel, tail_column_warp
+//   publish_block_partials             a 4-warp block's loss partials and its ticket: both tail kernels
+//   take_ticket / write_losses         the reduction's ticket, and the losses with the re-armed ticket: also column_step_kernel
+// Each reducing kernel keeps its own final summation order.  The sequential V-trace step stays written out in its three kernels.
 #include "common.cuh"
 #include "kernels.h"
 
 namespace srl {
-
-struct F4 { float v[4]; };
-template <int VEC> struct VecT;
-template <> struct VecT<1> { typedef float type; };
-template <> struct VecT<4> { typedef float4 type; };
 
 template <int VEC>
 SRL_DEVINL void ldv(const float* p, float (&o)[VEC]) {
@@ -26,6 +29,77 @@ template <int VEC>
 SRL_DEVINL void stv(float* p, const float (&o)[VEC]) {
   if (VEC == 4) *reinterpret_cast<float4*>(p) = make_float4(o[0], o[1 % VEC], o[2 % VEC], o[3 % VEC]);
   else *p = o[0];
+}
+
+// Element loads of the row helpers: NC = true reads global memory through the read-only path (ld.global.nc), NC = false is a plain
+// load (the shared-memory copies of the column kernel).
+template <bool NC>
+SRL_DEVINL float ldf(const float* p) { return NC ? __ldg(p) : *p; }
+// log_softmax of one row of A logits (vtrace.py:31-40): log p[a] = (x[a] - mx) - lse
+struct RowLse { float mx, lse; };
+template <bool NC>
+SRL_DEVINL RowLse row_lse(const float* row, int A) {
+  float mx = -INFINITY;
+  for (int a = 0; a < A; ++a) mx = fmaxf(mx, ldf<NC>(row + a));
+  float se = 0.f;
+  for (int a = 0; a < A; ++a) se += expf(ldf<NC>(row + a) - mx);
+  return {mx, logf(se)};
+}
+template <bool NC>
+SRL_DEVINL float row_logp(const float* row, RowLse s, int a) { return (ldf<NC>(row + a) - s.mx) - s.lse; }
+template <bool NC>
+SRL_DEVINL float row_entropy(const float* row, RowLse s, int A) {   // sum_a p log p (loss_fn.py:9-13)
+  float e = 0.f;
+  for (int a = 0; a < A; ++a) { const float lp = row_logp<NC>(row, s, a); e += expf(lp) * lp; }
+  return e;
+}
+
+// Kogge-Stone suffix composition over the warp (lane = step): (aa, bb) becomes F_t = f_t o f_{t+1} o ... o f_{31}
+SRL_DEVINL void scan_compose(int lane, float& aa, float& bb) {
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const float a2 = __shfl_down_sync(0xffffffffu, aa, d);
+    const float b2 = __shfl_down_sync(0xffffffffu, bb, d);
+    if (lane + d < 32) { bb = fmaf(aa, b2, bb); aa = aa * a2; }
+  }
+}
+
+// Deterministic loss reduction: scratch[0] counts the blocks that have published their partials (scratch[4 + 3 k ..] for block k).
+// One thread per block calls take_ticket after its stores: true in the block that published last, which sums the partials in its
+// kernel's fixed order and calls write_losses.
+SRL_DEVINL bool take_ticket(float* scratch) {
+  __threadfence();
+  return atomicAdd(reinterpret_cast<unsigned*>(scratch), 1u) == gridDim.x - 1;
+}
+SRL_DEVINL void write_losses(float* losses, float* scratch, float s_pg, float s_bl, float s_ent, float baseline_cost, float entropy_cost) {
+  const float a = s_pg, c = baseline_cost * s_bl, e = entropy_cost * s_ent;
+  losses[0] = a; losses[1] = c; losses[2] = e; losses[3] = a + c + e;
+  *reinterpret_cast<unsigned*>(scratch) = 0u;   // re-arm the ticket
+}
+
+// per-step tail input: the reward (clipped to [-1, 1] when clip_reward) and the discount of trajectory row o1
+SRL_DEVINL void tail_reward_discount(const float* __restrict__ reward, const uint8_t* __restrict__ done, size_t o1, float discounting,
+                                     int clip_reward, float& r, float& g) {
+  r = __ldg(reward + o1);
+  if (clip_reward) r = fminf(fmaxf(r, -1.f), 1.f);
+  g = done[o1] ? 0.f : discounting;
+}
+
+// the loss partials of a block of 4 warps: warp sums, then (w0 + w1) + (w2 + w3) per loss into the block's slot, then the ticket.
+// Returns true, in every thread, in the block that published last.
+SRL_DEVINL bool publish_block_partials(float* scratch, float l_pg, float l_bl, float l_ent) {
+  __shared__ float red[3][4];
+  __shared__ bool is_last;
+  l_pg = warp_sum(l_pg); l_bl = warp_sum(l_bl); l_ent = warp_sum(l_ent);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) { red[0][warp] = l_pg; red[1][warp] = l_bl; red[2][warp] = l_ent; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < 3; ++i) scratch[4 + blockIdx.x * 3 + i] = (red[i][0] + red[i][1]) + (red[i][2] + red[i][3]);
+    is_last = take_ticket(scratch);
+  }
+  __syncthreads();
+  return is_last;
 }
 
 // vtrace.py:135-169.  Each thread owns VEC adjacent columns; the reverse loop carries acc and vs_{t+1}.
@@ -46,7 +120,8 @@ __global__ void __launch_bounds__(128) vtrace_iw_seq_kernel(const float* __restr
     float lr[VEC], g[VEC], r[VEC], v[VEC], ovs[VEC], opg[VEC];
     ldv<VEC>(log_rhos + o, lr); ldv<VEC>(discounts + o, g); ldv<VEC>(rewards + o, r); ldv<VEC>(values + o, v);
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) {
+    for (int i = 0; i < VEC; ++i) {   // the sequential step, written out here, in vtrace_logits_kernel and in impala_tail_kernel:
+                                      // through one shared helper this kernel and impala_tail_kernel compile differently
       const float rho = expf(lr[i]);
       const float crho = clip_rho >= 0.f ? fminf(rho, clip_rho) : rho;
       const float c = fminf(rho, 1.0f);
@@ -109,12 +184,7 @@ __global__ void __launch_bounds__(256) vtrace_iw_scan_kernel(const float* __rest
       // affine map of this step: x -> bb + aa * x ; identity for padding lanes
       float aa = ok ? g * fminf(rho, 1.0f) : 1.f;
       float bb = ok ? crho * (r + g * vn - v) : 0.f;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {   // suffix composition F_t = f_t o F_{t+d}
-        const float a2 = __shfl_down_sync(0xffffffffu, aa, d);
-        const float b2 = __shfl_down_sync(0xffffffffu, bb, d);
-        if (lane + d < 32) { bb = fmaf(aa, b2, bb); aa = aa * a2; }
-      }
+      scan_compose(lane, aa, bb);
       const float acc = fmaf(aa, carry_acc, bb);
       const float myvs = acc + v;
       float vsn = __shfl_down_sync(0xffffffffu, myvs, 1);
@@ -138,7 +208,8 @@ __global__ void __launch_bounds__(256) vtrace_iw_scan_kernel(const float* __rest
   }
 }
 
-// log_softmax(logits)[action] for one row of A logits (vtrace.py:31-40)
+// log_softmax(logits)[action] for one row of A logits (vtrace.py:31-40).  Written out: through row_lse, which takes the log before
+// the gather, vtrace_logits_kernel and the tail kernels compile differently.
 SRL_DEVINL float action_logp(const float* __restrict__ row, int A, int act) {
   float mx = -INFINITY;
   for (int a = 0; a < A; ++a) mx = fmaxf(mx, __ldg(row + a));
@@ -163,7 +234,7 @@ __global__ void __launch_bounds__(128) vtrace_logits_kernel(const float* __restr
     const float balp = action_logp(bl + o * A, A, act);
     const float lr = talp - balp;
     const float g = __ldg(discounts + o), r = __ldg(rewards + o), v = __ldg(values + o);
-    const float rho = expf(lr);
+    const float rho = expf(lr);   // the sequential step, also in vtrace_iw_seq_kernel and impala_tail_kernel (see there)
     const float crho = clip_rho >= 0.f ? fminf(rho, clip_rho) : rho;
     acc = crho * (r + g * vnext - v) + g * fminf(rho, 1.0f) * acc;
     const float prho = clip_pg >= 0.f ? fminf(rho, clip_pg) : rho;
@@ -200,25 +271,20 @@ __global__ void __launch_bounds__(128) impala_tail_kernel(const float* __restric
       const size_t o1 = o + B;                   // trajectory row t+1
       const int act = ld_action(action + o1, A);
       const float* trow = tl + o * A;
-      float mx = -INFINITY;
-      for (int a = 0; a < A; ++a) mx = fmaxf(mx, __ldg(trow + a));
-      float se = 0.f;
-      for (int a = 0; a < A; ++a) se += expf(__ldg(trow + a) - mx);
-      const float lse = logf(se);
-      float ent = 0.f;                           // sum_a p log p
-      for (int a = 0; a < A; ++a) { const float lp = (__ldg(trow + a) - mx) - lse; ent += expf(lp) * lp; }
-      const float talp = (__ldg(trow + act) - mx) - lse;
+      const RowLse s = row_lse<true>(trow, A);
+      const float ent = row_entropy<true>(trow, s, A);
+      const float talp = row_logp<true>(trow, s, act);
       const float balp = action_logp(bl + o1 * A, A, act);
       const float rho = expf(talp - balp);
-      float r = __ldg(reward + o1);
-      if (clip_reward) r = fminf(fmaxf(r, -1.f), 1.f);
-      const float g = done[o1] ? 0.f : discounting;
+      float r, g;
+      tail_reward_discount(reward, done, o1, discounting, clip_reward, r, g);
       const float v = __ldg(baseline + o);
       const float crho = clip_rho >= 0.f ? fminf(rho, clip_rho) : rho;
-      acc = crho * (r + g * vnext - v) + g * fminf(rho, 1.0f) * acc;
+      acc = crho * (r + g * vnext - v) + g * fminf(rho, 1.0f) * acc;   // the sequential step: see vtrace_iw_seq_kernel
       const float prho = clip_pg >= 0.f ? fminf(rho, clip_pg) : rho;
       const float adv = prho * (r + g * vsnext - v);
       const float myvs = acc + v;
+      // output stage, also in tail_column_warp: written out twice, as through one helper both tail kernels compile differently
       if (vs) vs[o] = myvs;
       if (pg) pg[o] = adv;
       l_pg += -talp * adv;                                   // loss_fn.py:16-23
@@ -227,7 +293,7 @@ __global__ void __launch_bounds__(128) impala_tail_kernel(const float* __restric
       dbaseline[o] = -baseline_cost * (myvs - v);
       float* drow = dlogits + o * A;
       for (int a = 0; a < A; ++a) {
-        const float lp = (__ldg(trow + a) - mx) - lse;
+        const float lp = row_logp<true>(trow, s, a);
         const float p = expf(lp);
         drow[a] = adv * (p - (a == act ? 1.f : 0.f)) + entropy_cost * p * (lp - ent);
       }
@@ -235,28 +301,12 @@ __global__ void __launch_bounds__(128) impala_tail_kernel(const float* __restric
       vnext = v;
     }
   }
-  // deterministic reduction: warp -> block -> per-block partial; the last block sums partials in order
-  __shared__ float red[3][4];
-  __shared__ bool is_last;
-  l_pg = warp_sum(l_pg); l_bl = warp_sum(l_bl); l_ent = warp_sum(l_ent);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) { red[0][warp] = l_pg; red[1][warp] = l_bl; red[2][warp] = l_ent; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 3; ++i) scratch[4 + blockIdx.x * 3 + i] = (red[i][0] + red[i][1]) + (red[i][2] + red[i][3]);
-    __threadfence();
-    const unsigned ticket = atomicAdd(reinterpret_cast<unsigned*>(scratch), 1u);
-    is_last = (ticket == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last && threadIdx.x == 0) {
+  if (publish_block_partials(scratch, l_pg, l_bl, l_ent) && threadIdx.x == 0) {
     __threadfence();
     double s[3] = {0, 0, 0};
     for (unsigned k = 0; k < gridDim.x; ++k)
       for (int i = 0; i < 3; ++i) s[i] += (double)reinterpret_cast<volatile float*>(scratch)[4 + k * 3 + i];
-    const float a = (float)s[0], c = baseline_cost * (float)s[1], e = entropy_cost * (float)s[2];
-    losses[0] = a; losses[1] = c; losses[2] = e; losses[3] = a + c + e;
-    *reinterpret_cast<unsigned*>(scratch) = 0u;   // re-arm the ticket
+    write_losses(losses, scratch, (float)s[0], (float)s[1], (float)s[2], baseline_cost, entropy_cost);
   }
 }
 
@@ -265,8 +315,7 @@ __global__ void __launch_bounds__(128) impala_tail_kernel(const float* __restric
 // Target logits / baseline are read through (row pointer, stride) so the same code serves global memory (NC = true: ld.nc)
 // and the shared-memory copies of the fused column kernel (NC = false).  sdl (optional): [T][A+1] copy of
 // (dlogits..., dbaseline) for the caller.  l_* are per-lane partial loss sums.
-template <bool NC>
-SRL_DEVINL float ldf(const float* p) { return NC ? __ldg(p) : *p; }
+// The row arithmetic is written out here: through row_lse / row_entropy / row_logp the warp and column kernels compile differently.
 template <bool NC>
 SRL_DEVINL void tail_column_warp(const float* __restrict__ bl, const float* trow0, size_t tstride, const float* base0, size_t bstride,
                                  const int64_t* __restrict__ action, const float* __restrict__ reward, const uint8_t* __restrict__ done,
@@ -294,27 +343,21 @@ SRL_DEVINL void tail_column_warp(const float* __restrict__ bl, const float* trow
     const float talp = (ldf<NC>(trow + act) - mx) - lse;
     const float balp = action_logp(bl + o1 * A, A, act);
     const float rho = expf(talp - balp);
-    float r = __ldg(reward + o1);
-    if (clip_reward) r = fminf(fmaxf(r, -1.f), 1.f);
-    const float g = done[o1] ? 0.f : discounting;
+    float r, g;
+    tail_reward_discount(reward, done, o1, discounting, clip_reward, r, g);
     const float v = ldf<NC>(base0 + (size_t)tt * bstride);
     const float vn = ldf<NC>(base0 + (size_t)(tt + 1) * bstride);     // V_{t+1}; row T is the bootstrap value
     const float crho = clip_rho >= 0.f ? fminf(rho, clip_rho) : rho;
     float aa = ok ? g * fminf(rho, 1.0f) : 1.f;          // x -> bb + aa x ; identity on padding lanes
     float bb = ok ? crho * (r + g * vn - v) : 0.f;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const float a2 = __shfl_down_sync(0xffffffffu, aa, d);
-      const float b2 = __shfl_down_sync(0xffffffffu, bb, d);
-      if (lane + d < 32) { bb = fmaf(aa, b2, bb); aa = aa * a2; }
-    }
+    scan_compose(lane, aa, bb);
     const float acc = fmaf(aa, carry_acc, bb);
     const float myvs = acc + v;
     float vsn = __shfl_down_sync(0xffffffffu, myvs, 1);
     if (lane == 31 || t + 1 >= T) vsn = carry_vs;
     const float prho = clip_pg >= 0.f ? fminf(rho, clip_pg) : rho;
     const float adv = prho * (r + g * vsn - v);
-    if (ok) {
+    if (ok) {   // output stage, also in impala_tail_kernel: written out twice, as through one helper both tail kernels compile differently
       if (vs) vs[o] = myvs;
       if (pg) pg[o] = adv;
       l_pg += -talp * adv;
@@ -358,28 +401,13 @@ __global__ void __launch_bounds__(128) impala_tail_warp_kernel(const float* __re
     tail_column_warp<true>(bl, tl + (size_t)b * A, (size_t)B * A, baseline + b, (size_t)B, action, reward, done, T, B, A, b, lane, discounting,
                            clip_reward, clip_rho, clip_pg, baseline_cost, entropy_cost, vs, pg, dlogits, dbaseline, nullptr, l_pg, l_bl,
                            l_ent);
-  __shared__ float red[3][4];
-  __shared__ bool is_last;
-  l_pg = warp_sum(l_pg); l_bl = warp_sum(l_bl); l_ent = warp_sum(l_ent);
-  if (lane == 0) { red[0][warp] = l_pg; red[1][warp] = l_bl; red[2][warp] = l_ent; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 3; ++i) scratch[4 + blockIdx.x * 3 + i] = (red[i][0] + red[i][1]) + (red[i][2] + red[i][3]);
-    __threadfence();
-    is_last = atomicAdd(reinterpret_cast<unsigned*>(scratch), 1u) == gridDim.x - 1;
-  }
-  __syncthreads();
-  if (is_last && warp == 0) {   // fixed-order parallel sum of the block partials: deterministic
+  if (publish_block_partials(scratch, l_pg, l_bl, l_ent) && warp == 0) {   // fixed-order parallel sum of the block partials, also in column_step_kernel
     __threadfence();
     float s[3] = {0.f, 0.f, 0.f};
     for (unsigned k = lane; k < gridDim.x; k += 32)
       for (int i = 0; i < 3; ++i) s[i] += reinterpret_cast<volatile float*>(scratch)[4 + k * 3 + i];
     for (int i = 0; i < 3; ++i) s[i] = warp_sum(s[i]);
-    if (lane == 0) {
-      const float a = s[0], c = baseline_cost * s[1], e = entropy_cost * s[2];
-      losses[0] = a; losses[1] = c; losses[2] = e; losses[3] = a + c + e;
-      *reinterpret_cast<unsigned*>(scratch) = 0u;
-    }
+    if (lane == 0) write_losses(losses, scratch, s[0], s[1], s[2], baseline_cost, entropy_cost);
   }
 }
 
@@ -397,17 +425,9 @@ __global__ void __launch_bounds__(128) policy_rows_fwd_kernel(const float* __res
   const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= N) return;
   const float* row = logits + n * A;
-  float mx = -INFINITY;
-  for (int a = 0; a < A; ++a) mx = fmaxf(mx, __ldg(row + a));
-  float se = 0.f;
-  for (int a = 0; a < A; ++a) se += expf(__ldg(row + a) - mx);
-  const float lse = logf(se);
-  if (logp) logp[n] = (__ldg(row + ld_action(actions + n, A)) - mx) - lse;
-  if (ent) {
-    float e = 0.f;
-    for (int a = 0; a < A; ++a) { const float lp = (__ldg(row + a) - mx) - lse; e += expf(lp) * lp; }
-    ent[n] = e;
-  }
+  const RowLse s = row_lse<true>(row, A);
+  if (logp) logp[n] = row_logp<true>(row, s, ld_action(actions + n, A));
+  if (ent) ent[n] = row_entropy<true>(row, s, A);
 }
 __global__ void __launch_bounds__(128) policy_rows_bwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ actions,
                                                               const float* __restrict__ w_logp, const float* __restrict__ w_ent, int64_t N,
@@ -415,18 +435,12 @@ __global__ void __launch_bounds__(128) policy_rows_bwd_kernel(const float* __res
   const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= N) return;
   const float* row = logits + n * A;
-  float mx = -INFINITY;
-  for (int a = 0; a < A; ++a) mx = fmaxf(mx, __ldg(row + a));
-  float se = 0.f;
-  for (int a = 0; a < A; ++a) se += expf(__ldg(row + a) - mx);
-  const float lse = logf(se);
+  const RowLse s = row_lse<true>(row, A);
   const float wl = w_logp ? __ldg(w_logp + n) : 0.f, we = w_ent ? __ldg(w_ent + n) : 0.f;
-  float e = 0.f;
-  if (w_ent)
-    for (int a = 0; a < A; ++a) { const float lp = (__ldg(row + a) - mx) - lse; e += expf(lp) * lp; }
+  const float e = w_ent ? row_entropy<true>(row, s, A) : 0.f;
   const int act = actions ? ld_action(actions + n, A) : -1;
   for (int a = 0; a < A; ++a) {
-    const float lp = (__ldg(row + a) - mx) - lse, p = expf(lp);
+    const float lp = row_logp<true>(row, s, a), p = expf(lp);
     dlogits[n * A + a] = wl * ((a == act ? 1.f : 0.f) - p) + we * p * (lp - e);
   }
 }
@@ -630,22 +644,18 @@ __global__ void __launch_bounds__(COL_THREADS) column_step_kernel(
     l_pg = warp_sum(l_pg); l_bl = warp_sum(l_bl); l_ent = warp_sum(l_ent);
     if (lane == 0) {
       scratch[4 + b * 3 + 0] = l_pg; scratch[4 + b * 3 + 1] = l_bl; scratch[4 + b * 3 + 2] = l_ent;
-      __threadfence();
-      is_last = atomicAdd(reinterpret_cast<unsigned*>(scratch), 1u) == gridDim.x - 1;
+      is_last = take_ticket(scratch);
     }
   }
   __syncthreads();
-  if (is_last && warp == 0) {   // fixed-order sum of the column partials: deterministic
+  // fixed-order sum of the column partials, as in impala_tail_warp_kernel: through one helper this kernel compiles differently
+  if (is_last && warp == 0) {
     __threadfence();
     float s3[3] = {0.f, 0.f, 0.f};
     for (unsigned k = lane; k < gridDim.x; k += 32)
       for (int i = 0; i < 3; ++i) s3[i] += reinterpret_cast<volatile float*>(scratch)[4 + k * 3 + i];
     for (int i = 0; i < 3; ++i) s3[i] = warp_sum(s3[i]);
-    if (lane == 0) {
-      const float a = s3[0], c = baseline_cost * s3[1], e = entropy_cost * s3[2];
-      losses[0] = a; losses[1] = c; losses[2] = e; losses[3] = a + c + e;
-      *reinterpret_cast<unsigned*>(scratch) = 0u;
-    }
+    if (lane == 0) write_losses(losses, scratch, s3[0], s3[1], s3[2], baseline_cost, entropy_cost);
   }
   // ---- C: dh[n][j] for the T learning frames of the column; thread = (feature j, parity of t)
   {
@@ -676,44 +686,26 @@ SRL_KSTAMP_SETTER(kstamp_set_vtrace)
 bool column_step_supported(int T, int B, int A) {
   return T >= 1 && B >= 1 && B <= 512 && A >= 1 && A <= COL_MAX_A && column_smem_bytes(T, A) <= 200 * 1024;
 }
-cudaError_t launch_column_step(const float* hpart, int nsplit, const float* bfc, float* h, const float* reward, const int64_t* action,
-                               const uint8_t* done, const float* bl, const float* Wp, const float* bp, const float* Wb, const float* bb,
-                               int T, int B, int A, float discounting, int clip_reward, float clip_rho, float clip_pg,
-                               float baseline_cost, float entropy_cost, float* logits, float* baseline, float* vs, float* pg,
-                               float* dlogits, float* dbaseline, __nv_bfloat16* dh, float* losses, float* scratch, cudaStream_t st,
-                               __nv_bfloat16* dh_lo) {
-  if (!column_step_supported(T, B, A) || nsplit != 4) return cudaErrorInvalidValue;
-  static PerDeviceOnce once;
-  {
-    bool first;
-    const int dev = once.device(&first);
-    if (first) {
-      cudaError_t e = cudaFuncSetAttribute(column_step_kernel<4, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(column_step_kernel<4, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      if (e != cudaSuccess) return e;
-      once.mark(dev);
-    }
-  }
-#define SRL_COL_ARGS dim3(B), dim3(COL_THREADS), column_smem_bytes(T, A), st, hpart, bfc, h, reward, action, done, bl, Wp, bp, Wb, bb, T, B, A, \
-                     discounting, clip_reward, clip_rho, clip_pg, baseline_cost, entropy_cost, logits, baseline, vs, pg, dlogits, dbaseline, dh, \
-                     losses, scratch, dh_lo
-  if (A <= 8) return launch_chain(column_step_kernel<4, 8>, SRL_COL_ARGS);
-  return launch_chain(column_step_kernel<4, 32>, SRL_COL_ARGS);
-#undef SRL_COL_ARGS
+cudaError_t launch_column_step(const TailStep& s, const float* hpart, int nsplit, const float* bfc, float* h, const float* Wp, const float* bp,
+                               const float* Wb, const float* bb, float* logits, float* baseline, __nv_bfloat16* dh, __nv_bfloat16* dh_lo,
+                               cudaStream_t st) {
+  if (!column_step_supported(s.T, s.B, s.A) || nsplit != 4) return cudaErrorInvalidValue;
+  static PerDeviceOnce once[2];
+  const bool narrow = s.A <= 8;
+  const auto kernel = narrow ? column_step_kernel<4, 8> : column_step_kernel<4, 32>;
+  const cudaError_t e = ensure_max_dynamic_smem(once[narrow ? 0 : 1], kernel, 200 * 1024);
+  if (e != cudaSuccess) return e;
+  return launch_chain(kernel, dim3(s.B), dim3(COL_THREADS), column_smem_bytes(s.T, s.A), st, hpart, bfc, h, s.reward, s.action, s.done, s.bl,
+                      Wp, bp, Wb, bb, s.T, s.B, s.A, s.discounting, s.clip_reward, s.clip_rho, s.clip_pg, s.baseline_cost, s.entropy_cost, logits,
+                      baseline, s.vs, s.pg, s.dlogits, s.dbaseline, dh, s.losses, s.scratch, dh_lo);
 }
 
-cudaError_t launch_impala_tail(const float* bl, const float* tl, const float* baseline, const int64_t* action, const float* reward,
-                               const uint8_t* done, int T, int B, int A, float discounting, int clip_reward, float clip_rho,
-                               float clip_pg, float baseline_cost, float entropy_cost, float* vs, float* pg, float* dlogits,
-                               float* dbaseline, float* losses, float* scratch, cudaStream_t st) {
-  if (B <= 2048) {   // latency-bound sizes: one warp per column, shuffle scan over T (block partials: 3*ceil(B/4) <= 1536 floats)
-    return launch_chain(impala_tail_warp_kernel, dim3((B + 3) / 4), dim3(128), 0, st, bl, tl, baseline, action, reward, done, T, B, A, discounting,
-                        clip_reward, clip_rho, clip_pg, baseline_cost, entropy_cost, vs, pg, dlogits, dbaseline, losses, scratch);
-  } else {
-    return launch_chain(impala_tail_kernel, dim3((B + 127) / 128), dim3(128), 0, st, bl, tl, baseline, action, reward, done, T, B, A, discounting,
-                        clip_reward, clip_rho, clip_pg, baseline_cost, entropy_cost, vs, pg, dlogits, dbaseline, losses, scratch);
-  }
-  return cudaGetLastError();
+cudaError_t launch_impala_tail(const TailStep& s, const float* tl, const float* baseline, cudaStream_t st) {
+  // latency-bound sizes: one warp per column, shuffle scan over T (block partials: 3*ceil(B/4) <= 1536 floats)
+  const bool warp = s.B <= 2048;
+  return launch_chain(warp ? impala_tail_warp_kernel : impala_tail_kernel, dim3(warp ? (s.B + 3) / 4 : (s.B + 127) / 128), dim3(128), 0, st,
+                      s.bl, tl, baseline, s.action, s.reward, s.done, s.T, s.B, s.A, s.discounting, s.clip_reward, s.clip_rho, s.clip_pg,
+                      s.baseline_cost, s.entropy_cost, s.vs, s.pg, s.dlogits, s.dbaseline, s.losses, s.scratch);
 }
 
 }  // namespace srl

@@ -125,7 +125,8 @@ def test_from_logits_vs_oracle(ops, T, B, A):
         assert_close(got, want, 1e-4, name)
 
 
-@pytest.mark.parametrize('T,B,A,clip', [(20, 32, 6, 'abs_one'), (20, 64, 4, 'none'), (3, 200, 18, 'abs_one'), (20, 512, 4, 'abs_one')])
+@pytest.mark.parametrize('T,B,A,clip', [(20, 32, 6, 'abs_one'), (20, 64, 4, 'none'), (3, 200, 18, 'abs_one'), (20, 512, 4, 'abs_one'),
+                                        (3, 2100, 6, 'abs_one'), (2, 4099, 4, 'none')])      # B > 2048: the thread-per-column kernel
 def test_fused_tail_vs_oracle(ops, T, B, A, clip):
     batch = O.synthetic_batch(T, B, A, seed=B, done_p=0.05)
     rng = np.random.RandomState(B)
