@@ -77,6 +77,7 @@ extern "C" int srl_impala_loss_and_head_grads(const float* bl, const float* tl, 
   srl_config_t c = {};
   c.T = T; c.B = B; c.A = A; c.discounting = discounting; c.reward_clip_abs_one = reward_clip_abs_one;
   c.clip_rho_threshold = clip_rho; c.clip_pg_rho_threshold = clip_pg; c.baseline_cost = baseline_cost; c.entropy_cost = entropy_cost;
+  pdl_set_active(true);      // no learner call: SRL_PDL alone decides
   CU(launch_impala_tail(tail_step(c, bl, action, reward, done, vs, pg, dlogits, dbaseline, losses, scratch), tl, baseline, (cudaStream_t)stream),
      "impala_tail");
   return 0;
@@ -202,7 +203,7 @@ struct srl_learner {
   int step;                       // optimizer step count (Adam bias correction)
   bool have_fwd;
   TmaMaps maps;                   // tensor maps of the TMA mainloop
-  SideStream ss;                  // wgrad side stream + fork/join events
+  StepStreams S;                  // the lanes beside the caller's stream, and the per-kernel profiler
   int* dstep;                     // device-side optimizer step count (graph-replay safe Adam bias correction and lr schedule)
   OptExtra ox;                    // lr schedule + RMSprop momentum of the optimizer step (srl_learner_set_lr_schedule / _set_momentum)
   bool report_lr;                 // grad_norm_out receives coef[2] too (after srl_learner_set_lr_schedule)
@@ -213,8 +214,6 @@ struct srl_learner {
   int lstm_step_ksplit;           // K split of its GEMM (cluster size; srl_learner_set_option "lstm_step_ksplit")
   bool fused_front;               // frame conversion + conv1 + conv2 as one kernel (SRL_FUSED_FWD / srl_learner_set_option "fused_fwd")
   bool column_fusion;             // heads + V-trace/loss + dh in one column kernel (SRL_NO_COLUMN_FUSION / srl_learner_set_option)
-  Profiler pf;                    // per-kernel event bracketing (off by default)
-  cudaEvent_t events[2 * PS_COUNT];
 };
 
 static const char* kSlotNames[PS_COUNT] = {"obs_s2d", "conv1_fwd", "conv2_fwd", "conv3_fwd", "fc_fwd", "head_fwd", "vtrace_loss_tail",
@@ -286,7 +285,12 @@ static int workspace_table(srl_learner* L, WsRow* t) {
 }
 static int64_t ws_bytes(const WsRow& r) { return ((int64_t)r.elem * r.count + 255) & ~int64_t(255); }
 
-static int pack_priority(int least, int greatest);
+// the re-pack lane sits one level BELOW the greatest priority (which the learner's capture stream uses for the main chain) and above the wgrad
+// lanes (default = least): its short blocks fill the slots the frame conversion leaves free without delaying it
+static int pack_priority(int least, int greatest) {
+  return greatest + 1 > least ? least : greatest + 1;
+}
+
 extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float* grads, float* opt0, float* opt1, srl_learner_t** out) {
   int rc = check_cfg(cfg);
   if (rc) return rc;
@@ -325,17 +329,17 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
     if (split && t[i].lo) { *t[i].lo = q; q += ws_bytes(t[i]); }
   }
   L->buf.NF = (int)NF;
-  if (cudaStreamCreateWithFlags(&L->ss.side, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&L->ss.side2, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&L->ss.side3, cudaStreamNonBlocking) != cudaSuccess) L->ss.side = nullptr;
-  {
+  {     // the lanes: without them every call runs collapsed on the caller's stream
+    StepStreams& S = L->S;
     int lo = 0, hi = 0;       // (numerically lowest = greatest priority)
-    if (L->ss.side && (cudaDeviceGetStreamPriorityRange(&lo, &hi) != cudaSuccess ||
-                       cudaStreamCreateWithPriority(&L->ss.pack, cudaStreamNonBlocking, pack_priority(lo, hi)) != cudaSuccess)) L->ss.side = nullptr;
+    bool ok = cudaDeviceGetStreamPriorityRange(&lo, &hi) == cudaSuccess;
+    for (int l = 0; l < LANE_COUNT && ok; ++l)        // the wgrad lanes take the default priority (0, the least)
+      ok = cudaStreamCreateWithPriority(&S.side[l], cudaStreamNonBlocking, l == LANE_PACK ? pack_priority(lo, hi) : 0) == cudaSuccess &&
+           cudaEventCreateWithFlags(&S.forked[l], cudaEventDisableTiming) == cudaSuccess &&
+           cudaEventCreateWithFlags(&S.joined[l], cudaEventDisableTiming) == cudaSuccess;
+    S.have_lanes = ok;
+    cudaGetLastError();
   }
-  for (int e2 = 0; e2 < 12 && L->ss.side; ++e2)
-    if (cudaEventCreateWithFlags(&L->ss.ev[e2], cudaEventDisableTiming) != cudaSuccess) { L->ss.side = nullptr; }
-  cudaGetLastError();
   const char* why = nullptr;
   if (build_tma_maps(L->buf, (int)NF, (int)NB, &L->maps, &why) != cudaSuccess)
     return undo(fail(SRL_ESTATE, "learner_create: building TMA tensor map '%s' failed (driver without cuTensorMapEncodeTiled?)", why ? why : "?"));
@@ -354,12 +358,12 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
 
 extern "C" int srl_learner_destroy(srl_learner_t* L) {
   if (!L) return 0;
-  for (int i = 0; i < 2 * PS_COUNT; ++i) if (L->events[i]) cudaEventDestroy(L->events[i]);
-  for (int i = 0; i < 12; ++i) if (L->ss.ev[i]) cudaEventDestroy(L->ss.ev[i]);
-  if (L->ss.side) cudaStreamDestroy(L->ss.side);
-  if (L->ss.side2) cudaStreamDestroy(L->ss.side2);
-  if (L->ss.side3) cudaStreamDestroy(L->ss.side3);
-  if (L->ss.pack) cudaStreamDestroy(L->ss.pack);
+  for (int i = 0; i < 2 * PS_COUNT; ++i) if (L->S.slot_events[i]) cudaEventDestroy(L->S.slot_events[i]);
+  for (int l = 0; l < LANE_COUNT; ++l) {
+    if (L->S.forked[l]) cudaEventDestroy(L->S.forked[l]);
+    if (L->S.joined[l]) cudaEventDestroy(L->S.joined[l]);
+    if (L->S.side[l]) cudaStreamDestroy(L->S.side[l]);
+  }
   if (L->lstm) srl_lstm_destroy(L->lstm);
   lstm_step_destroy(L->lstm_step);
   cudaFree(L->arena);
@@ -455,9 +459,10 @@ extern "C" int64_t srl_learner_get_step(srl_learner_t* L, void* stream) {
 
 extern "C" int srl_learner_pack_weights(srl_learner_t* L, void* stream) {
   REQ(L, "learner is NULL");
-  CU(launch_pack_weights(L->P, L->buf.hi.wpack, (cudaStream_t)stream, L->buf.lo.wpack), "pack_weights");
+  L->S.begin_call((cudaStream_t)stream);
+  CU(launch_pack_weights(L->P, L->buf.hi.wpack, L->S.main, L->buf.lo.wpack), "pack_weights");
   // the actor step's [W_ih | W_hh] copy: packed here, once per weight version, and never by the learner's own forward
-  if (L->lstm_step) CU(lstm_step_pack(L->lstm_step, (cudaStream_t)stream), "lstm_step_pack");
+  if (L->lstm_step) CU(lstm_step_pack(L->lstm_step, L->S.main), "lstm_step_pack");
   return 0;
 }
 
@@ -470,59 +475,41 @@ bool pdl_active() {
 void pdl_set_active(bool on) { g_pdl_on = on; }
 }  // namespace srl
 
-// the re-pack stream sits one level BELOW the greatest priority (which the learner's capture stream uses for the main chain) and above the wgrad
-// streams (default = least): its short blocks fill the slots the frame conversion leaves free without delaying it
-static int pack_priority(int least, int greatest) {
-  return greatest + 1 > least ? least : greatest + 1;
-}
+// learner step (bf16 mode, lanes): a3 -> fc.weight column order for the fc wgrad GEMM runs on the fc_wgrad lane right after the fc
+// forward, under the column kernel (32 CTAs, the GPU is otherwise idle), not in the crowded backward phase; else encoder_backward runs it
+static bool early_a3_transpose(const srl_learner* L) { return !L->S.collapsed && L->cfg.precision == 0; }
 
-static int encode_impl(srl_learner* L, const uint8_t* obs, int frames, cudaStream_t st, bool zero_small_grads = false) {
-  L->pf.st = st;
-  pdl_set_active(!L->pf.on);
+// step: the forward of the non-LSTM learner step (clears the small gradients; early a3 transpose)
+static int encode_impl(srl_learner* L, const uint8_t* obs, int frames, bool step = false) {
+  StepStreams& S = L->S;
   // The bf16 operand copies are re-derived from the fp32 master weights at the START of every forward (not at the end
-  // of the optimizer step): the pack kernel runs on the side stream underneath the frame conversion.
-  // Without side streams, or with per-kernel profiling on, both run on `st` (the profiler brackets are no-ops otherwise).
-  const bool fork = L->ss.side && !L->pf.on;
-  cudaStream_t pack_st = fork ? L->ss.pack : st;
-  if (fork) {
-    CU(cudaEventRecord(L->ss.ev[5], st), "fork pack");
-    CU(cudaStreamWaitEvent(pack_st, L->ss.ev[5], 0), "fork pack");
+  // of the optimizer step): the pack kernel runs on the pack lane underneath the frame conversion.
+  CU(S.fork(LANE_PACK), "fork pack");
+  if (step) {     // the accumulated gradient segments (everything before fc.weight) are cleared under the frame conversion
+    S.b(PS_ZERO_GRADS);
+    CU(cudaMemsetAsync(L->grads, 0, L->small_len * sizeof(float), S.lane(LANE_PACK)), "zero small grads");
+    S.e(PS_ZERO_GRADS);
   }
-  if (zero_small_grads) {     // the accumulated gradient segments (everything before fc.weight) are cleared under the frame conversion
-    L->pf.b(PS_ZERO_GRADS);
-    CU(cudaMemsetAsync(L->grads, 0, L->small_len * sizeof(float), pack_st), "zero small grads");
-    L->pf.e(PS_ZERO_GRADS);
-  }
-  L->pf.b(PS_PACK);
-  CU(launch_pack_weights(L->P, L->buf.hi.wpack, pack_st, L->buf.lo.wpack, true), "pack_weights");
-  L->pf.e(PS_PACK);
-  cudaEvent_t packed = nullptr;
-  if (fork) {
-    CU(cudaEventRecord(L->ss.ev[6], pack_st), "join pack");
-    packed = L->ss.ev[6];
-  }
-  CU(encoder_forward(obs, frames, L->P, L->buf, L->maps, L->cfg.precision, st, L->pf, packed, L->fused_front), "encoder_forward");
-  // learner step (bf16 mode): a3 -> fc.weight column order for the fc weight-gradient GEMM, on the wgrad side stream right after the fc forward,
-  // i.e. under the column kernel (32 CTAs, the GPU is otherwise idle) instead of in the crowded backward phase
-  L->buf.a3t_ready = false;
-  if (zero_small_grads && fork && L->cfg.precision == 0 && L->buf.a3t && !L->cfg.use_lstm) {
-    CU(cudaEventRecord(L->ss.ev[10], st), "fork a3 transpose");
-    CU(cudaStreamWaitEvent(L->ss.side, L->ss.ev[10], 0), "fork a3 transpose");
-    CU(launch_a3_transpose(L->buf.hi.a3, L->buf.a3t, L->cfg.T * L->cfg.B, L->ss.side), "a3_transpose");
-    L->buf.a3t_ready = true;
+  S.b(PS_PACK);
+  CU(launch_pack_weights(L->P, L->buf.hi.wpack, S.lane(LANE_PACK), L->buf.lo.wpack, true), "pack_weights");
+  S.e(PS_PACK);
+  CU(encoder_forward(obs, frames, L->P, L->buf, L->maps, L->cfg.precision, S, L->fused_front), "encoder_forward");
+  if (step && early_a3_transpose(L)) {
+    CU(S.fork(LANE_FC_WGRAD), "fork a3 transpose");
+    CU(launch_a3_transpose(L->buf.hi.a3, L->buf.a3t, L->cfg.T * L->cfg.B, S.lane(LANE_FC_WGRAD)), "a3_transpose");
   }
   return 0;
 }
 
 static int forward_impl(srl_learner* L, const uint8_t* obs, const float* reward, const int64_t* action, int frames, float* logits,
-                        float* baseline, cudaStream_t st, bool zero_small_grads = false) {
+                        float* baseline, bool step = false) {
   REQ(!L->cfg.use_lstm, "this learner was created with use_lstm=1: call the *_lstm entry points");
-  int rc = encode_impl(L, obs, frames, st, zero_small_grads);
+  int rc = encode_impl(L, obs, frames, step);
   if (rc) return rc;
-  L->pf.b(PS_HEAD_FWD);
+  L->S.b(PS_HEAD_FWD);
   CU(launch_head_fwd(L->buf.hpart, FC_SPLITS, L->P.bf, L->buf.h, reward, action, L->P.wp, L->P.bp, L->P.wb, L->P.bb, frames, L->cfg.A,
-                     logits, baseline, st), "head_fwd");
-  L->pf.e(PS_HEAD_FWD);
+                     logits, baseline, L->S.main), "head_fwd");
+  L->S.e(PS_HEAD_FWD);
   return 0;
 }
 
@@ -531,12 +518,14 @@ extern "C" int srl_learner_forward(srl_learner_t* L, const uint8_t* obs, const f
   REQ(L && obs && reward && action && policy_logits && baseline, "learner_forward: NULL pointer");
   REQ(rows >= 1 && rows <= L->cfg.T + 1, "learner_forward: rows=%d must be in [1, T+1=%d]", rows, L->cfg.T + 1);
   REQ((reinterpret_cast<uintptr_t>(obs) & 3) == 0, "learner_forward: obs must be 4-byte aligned");
-  return forward_impl(L, obs, reward, action, rows * L->cfg.B, policy_logits, baseline, (cudaStream_t)stream);
+  L->S.begin_call((cudaStream_t)stream);
+  return forward_impl(L, obs, reward, action, rows * L->cfg.B, policy_logits, baseline);
 }
 
 static int fb_begin(srl_learner* L, const uint8_t* obs, const float* reward, const uint8_t* done, const int64_t* action,
-                    const float* behavior_logits, float* losses, float* vs, float* pg_advantages, cudaStream_t st, int phase) {
+                    const float* behavior_logits, float* losses, float* vs, float* pg_advantages, BwdParts parts) {
   const srl_config_t& c = L->cfg;
+  const StepStreams& S = L->S;
   const int NF = (c.T + 1) * c.B, NB = c.T * c.B;
   // heads + V-trace/losses + dh: one fused column kernel when its shared-memory footprint fits, else three kernels
   const bool fused = L->column_fusion && column_step_supported(c.T, c.B, c.A);
@@ -544,29 +533,25 @@ static int fb_begin(srl_learner* L, const uint8_t* obs, const float* reward, con
   int rc;
   if (fused) {
     REQ(!L->cfg.use_lstm, "this learner was created with use_lstm=1: call the *_lstm entry points");
-    rc = encode_impl(L, obs, NF, st, true);
+    rc = encode_impl(L, obs, NF, true);
     if (rc) return rc;
-    L->pf.b(PS_TAIL);
+    S.b(PS_TAIL);
     CU(launch_column_step(ts, L->buf.hpart, FC_SPLITS, L->P.bf, L->buf.h, L->P.wp, L->P.bp, L->P.wb, L->P.bb, L->logits, L->baseline,
-                          L->buf.hi.dh, L->buf.lo.dh, st), "column_step");
-    L->pf.e(PS_TAIL);
+                          L->buf.hi.dh, L->buf.lo.dh, S.main), "column_step");
+    S.e(PS_TAIL);
   } else {
-    rc = forward_impl(L, obs, reward, action, NF, L->logits, L->baseline, st, true);
+    rc = forward_impl(L, obs, reward, action, NF, L->logits, L->baseline, true);
     if (rc) return rc;
-    L->pf.b(PS_TAIL);
-    CU(launch_impala_tail(ts, L->logits, L->baseline, st), "impala_tail");
-    L->pf.e(PS_TAIL);
+    S.b(PS_TAIL);
+    CU(launch_impala_tail(ts, L->logits, L->baseline, S.main), "impala_tail");
+    S.e(PS_TAIL);
   }
-  L->pf.b(PS_HEAD_BWD);
-  {
-    const bool fork = L->ss.side != nullptr && !L->pf.on;
-    cudaStream_t sw = fork ? L->ss.side : st;
-    if (fork) { CU(cudaEventRecord(L->ss.ev[8], st), "fork head wgrad"); CU(cudaStreamWaitEvent(sw, L->ss.ev[8], 0), "fork head wgrad"); }
-    CU(launch_head_bwd(L->dlogits, L->dbaseline, L->buf.h, reward, action, L->P.wp, L->P.wb, NB, c.A, L->buf.hi.dh, L->G.wp, L->G.bp, L->G.wb,
-                       L->G.bb, L->head_part, st, sw, !fused, L->buf.lo.dh), "head_bwd");      // side stream `side` is joined by encoder_backward (after the fc wgrad)
-  }
-  L->pf.e(PS_HEAD_BWD);
-  CU(encoder_backward(NB, L->buf, L->G, L->maps, c.precision, st, L->pf, L->ss, phase), "encoder_backward");
+  S.b(PS_HEAD_BWD);
+  CU(S.fork(LANE_FC_WGRAD), "fork head wgrad");      // joined by encoder_backward with the fc wgrad
+  CU(launch_head_bwd(L->dlogits, L->dbaseline, L->buf.h, reward, action, L->P.wp, L->P.wb, NB, c.A, L->buf.hi.dh, L->G.wp, L->G.bp, L->G.wb,
+                     L->G.bb, L->head_part, S.main, S.lane(LANE_FC_WGRAD), !fused, L->buf.lo.dh), "head_bwd");
+  S.e(PS_HEAD_BWD);
+  CU(encoder_backward(NB, L->buf, L->G, L->maps, c.precision, S, parts, early_a3_transpose(L)), "encoder_backward");
   L->have_fwd = true;
   return 0;
 }
@@ -576,7 +561,8 @@ extern "C" int srl_learner_forward_backward(srl_learner_t* L, const uint8_t* obs
                                             float* pg_advantages, void* stream) {
   REQ(L && obs && reward && done && action && behavior_logits && losses, "learner_forward_backward: NULL pointer");
   REQ((reinterpret_cast<uintptr_t>(obs) & 3) == 0, "learner_forward_backward: obs must be 4-byte aligned");
-  return fb_begin(L, obs, reward, done, action, behavior_logits, losses, vs, pg_advantages, (cudaStream_t)stream, 2);
+  L->S.begin_call((cudaStream_t)stream);
+  return fb_begin(L, obs, reward, done, action, behavior_logits, losses, vs, pg_advantages, BWD_BOTH);
 }
 
 extern "C" int srl_learner_forward_backward_begin(srl_learner_t* L, const uint8_t* obs, const float* reward, const uint8_t* done,
@@ -584,25 +570,26 @@ extern "C" int srl_learner_forward_backward_begin(srl_learner_t* L, const uint8_
                                                   float* pg_advantages, void* stream) {
   REQ(L && obs && reward && done && action && behavior_logits && losses, "learner_forward_backward_begin: NULL pointer");
   REQ((reinterpret_cast<uintptr_t>(obs) & 3) == 0, "learner_forward_backward_begin: obs must be 4-byte aligned");
-  return fb_begin(L, obs, reward, done, action, behavior_logits, losses, vs, pg_advantages, (cudaStream_t)stream, 0);
+  L->S.begin_call((cudaStream_t)stream);
+  return fb_begin(L, obs, reward, done, action, behavior_logits, losses, vs, pg_advantages, BWD_FC);
 }
 
 extern "C" int srl_learner_backward_finish(srl_learner_t* L, const uint8_t* obs, void* stream) {
   REQ(L && obs, "learner_backward_finish: NULL pointer");
   REQ(L->have_fwd, "learner_backward_finish: call srl_learner_forward_backward_begin first");
   const srl_config_t& c = L->cfg;
-  L->pf.st = (cudaStream_t)stream;
-  pdl_set_active(!L->pf.on);
-  CU(encoder_backward(c.T * c.B, L->buf, L->G, L->maps, c.precision, (cudaStream_t)stream, L->pf, L->ss, 1), "encoder_backward");
+  L->S.begin_call((cudaStream_t)stream);
+  CU(encoder_backward(c.T * c.B, L->buf, L->G, L->maps, c.precision, L->S, BWD_CONV, false), "encoder_backward");
   return 0;
 }
 
 static int forward_lstm_impl(srl_learner* L, const uint8_t* obs, const float* reward, const uint8_t* done, const int64_t* action,
-                             const float* h0, const float* c0, float* logits, float* baseline, float* hT, float* cT, cudaStream_t st) {
+                             const float* h0, const float* c0, float* logits, float* baseline, float* hT, float* cT) {
   REQ(L->cfg.use_lstm && L->lstm, "this learner was created with use_lstm=0");
   const srl_config_t& c = L->cfg;
+  const cudaStream_t st = L->S.main;
   const int NF = (c.T + 1) * c.B;
-  int rc = encode_impl(L, obs, NF, st);
+  int rc = encode_impl(L, obs, NF);
   if (rc) return rc;
   CU(launch_core_build(L->buf.hpart, FC_SPLITS, L->P.bf, reward, action, NF, c.A, L->buf.h, L->core, st), "core_build");
   rc = srl_lstm_forward(L->lstm, L->core, done, h0, c0, L->lstm_out, hT, cT, st);
@@ -615,7 +602,8 @@ extern "C" int srl_learner_forward_lstm(srl_learner_t* L, const uint8_t* obs, co
                                         const float* h0, const float* c0, float* policy_logits, float* baseline, float* hT, float* cT,
                                         void* stream) {
   REQ(L && obs && reward && done && action && h0 && c0 && policy_logits && baseline, "learner_forward_lstm: NULL pointer");
-  return forward_lstm_impl(L, obs, reward, done, action, h0, c0, policy_logits, baseline, hT, cT, (cudaStream_t)stream);
+  L->S.begin_call((cudaStream_t)stream);
+  return forward_lstm_impl(L, obs, reward, done, action, h0, c0, policy_logits, baseline, hT, cT);
 }
 
 static bool overlaps(const void* a, const void* b, int64_t bytes) {
@@ -639,8 +627,8 @@ extern "C" int srl_learner_forward_lstm_step(srl_learner_t* L, const uint8_t* ob
   REQ(!overlaps(h_out, h_in, sb) && !overlaps(h_out, c_in, sb) && !overlaps(c_out, h_in, sb) && !overlaps(c_out, c_in, sb) &&
       !overlaps(h_out, c_out, sb), "learner_forward_lstm_step: h_out / c_out must not alias h_in, c_in or each other");
   REQ((reinterpret_cast<uintptr_t>(obs) & 3) == 0, "learner_forward_lstm_step: obs must be 4-byte aligned");
-  cudaStream_t st = (cudaStream_t)stream;
-  int rc = encode_impl(L, obs, B, st);
+  const cudaStream_t st = L->S.begin_call((cudaStream_t)stream);
+  int rc = encode_impl(L, obs, B);
   if (rc) return rc;
   CU(launch_core_build(L->buf.hpart, FC_SPLITS, L->P.bf, reward, action, B, c.A, L->buf.h, L->core, st), "core_build");
   CU(lstm_step_forward(L->lstm_step, L->core, done, h_in, c_in, h_out, c_out, L->lstm_step_ksplit, st), "lstm_step");
@@ -652,10 +640,10 @@ extern "C" int srl_learner_forward_backward_lstm(srl_learner_t* L, const uint8_t
                                                  const int64_t* action, const float* behavior_logits, const float* h0, const float* c0,
                                                  float* losses, float* vs, float* pg_advantages, void* stream) {
   REQ(L && obs && reward && done && action && behavior_logits && h0 && c0 && losses, "learner_forward_backward_lstm: NULL pointer");
-  cudaStream_t st = (cudaStream_t)stream;
+  const cudaStream_t st = L->S.begin_call((cudaStream_t)stream);
   const srl_config_t& c = L->cfg;
   const int NB = c.T * c.B;
-  int rc = forward_lstm_impl(L, obs, reward, done, action, h0, c0, L->logits, L->baseline, nullptr, nullptr, st);
+  int rc = forward_lstm_impl(L, obs, reward, done, action, h0, c0, L->logits, L->baseline, nullptr, nullptr);
   if (rc) return rc;
   CU(launch_impala_tail(tail_step(c, behavior_logits, action, reward, done, vs, pg_advantages, L->dlogits, L->dbaseline, losses, L->scratch),
                         L->logits, L->baseline, st), "impala_tail");
@@ -666,30 +654,31 @@ extern "C" int srl_learner_forward_backward_lstm(srl_learner_t* L, const uint8_t
   rc = srl_lstm_backward(L->lstm, L->dout, done, L->dcore, st);
   if (rc) return fail(rc, "lstm_backward: %s", srl_lstm_last_error());
   CU(launch_dcore_to_dh(L->dcore, L->buf.h, NB, c.A, L->buf.hi.dh, st), "dcore_to_dh");
-  CU(encoder_backward(NB, L->buf, L->G, L->maps, c.precision, st, L->pf, L->ss, 2), "encoder_backward");
+  CU(encoder_backward(NB, L->buf, L->G, L->maps, c.precision, L->S, BWD_BOTH, false), "encoder_backward");
   L->have_fwd = true;
   return 0;
 }
 
 // clip_grad_norm_ + optimizer in one cooperative kernel (profile slot: optimizer); P: the data-parallel step over these peers
-static int apply_impl(srl_learner_t* L, const DpPeers* P, float* grad_norm_out, cudaStream_t st) {
+static int apply_impl(srl_learner_t* L, const DpPeers* P, float* grad_norm_out) {
   const srl_config_t& c = L->cfg;
   const bool adam = c.optimizer != 0;
-  L->pf.st = st;
+  const cudaStream_t st = L->S.main;
   L->step += 1;
   const OptStep o = {adam ? 1 : 0, L->params, L->grads, L->opt0, adam ? L->opt1 : nullptr, L->nparams, c.max_grad_norm, L->coef,
                      L->scratch + 2048, c.learning_rate, adam ? c.adam_beta1 : c.alpha, adam ? c.adam_beta2 : 0.f,
                      adam ? c.adam_eps : c.epsilon, L->step, L->dstep, L->ox};
-  L->pf.b(PS_OPTIMIZER);
+  L->S.b(PS_OPTIMIZER);
   CU(P ? launch_dp_clip_optim(o, *P, st) : launch_clip_optim(o, st), P ? (adam ? "dp clip+adam" : "dp clip+rmsprop") : (adam ? "clip+adam" : "clip+rmsprop"));
-  L->pf.e(PS_OPTIMIZER);
+  L->S.e(PS_OPTIMIZER);
   if (grad_norm_out) CU(cudaMemcpyAsync(grad_norm_out, L->coef, (L->report_lr ? 3 : 2) * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy coef");
   return 0;
 }
 
 extern "C" int srl_learner_apply_gradients(srl_learner_t* L, float* grad_norm_out, void* stream) {
   REQ(L, "learner is NULL");
-  return apply_impl(L, nullptr, grad_norm_out, (cudaStream_t)stream);
+  L->S.begin_call((cudaStream_t)stream);
+  return apply_impl(L, nullptr, grad_norm_out);
 }
 
 extern "C" int srl_learner_apply_gradients_dp(srl_learner_t* L, const srl_dp_peers_t* peers, float* grad_norm_out, void* stream) {
@@ -705,26 +694,26 @@ extern "C" int srl_learner_apply_gradients_dp(srl_learner_t* L, const srl_dp_pee
     REQ(i >= peers->world || (P.g[i] && P.ctl[i] && P.rs[i]), "apply_gradients_dp: NULL peer pointer %d", i);
   }
   P.rank = peers->rank; P.world = peers->world; P.mc_g = (float*)peers->grads_multicast;
-  return apply_impl(L, &P, grad_norm_out, (cudaStream_t)stream);
+  L->S.begin_call((cudaStream_t)stream);
+  return apply_impl(L, &P, grad_norm_out);
 }
 
 extern "C" int srl_learner_set_profiling(srl_learner_t* L, int enable) {
   REQ(L, "learner is NULL");
-  if (enable && !L->events[0])
-    for (int i = 0; i < 2 * PS_COUNT; ++i) CU(cudaEventCreate(&L->events[i]), "cudaEventCreate");
-  L->pf.on = enable != 0;
-  L->pf.ev = L->events;
+  if (enable && !L->S.slot_events[0])
+    for (int i = 0; i < 2 * PS_COUNT; ++i) CU(cudaEventCreate(&L->S.slot_events[i]), "cudaEventCreate");
+  L->S.profiling = enable != 0;
   return 0;
 }
 extern "C" int srl_profile_slot_count(void) { return PS_COUNT; }
 extern "C" const char* srl_profile_slot_name(int slot) { return (slot >= 0 && slot < PS_COUNT) ? kSlotNames[slot] : ""; }
 extern "C" int srl_learner_profile_collect(srl_learner_t* L, float* ms_out_host) {
   REQ(L && ms_out_host, "profile_collect: NULL argument");
-  REQ(L->pf.on, "profile_collect: profiling is off");
+  REQ(L->S.profiling, "profile_collect: profiling is off");
   for (int i = 0; i < PS_COUNT; ++i) {
     float ms = 0.f;
-    cudaError_t e = cudaEventSynchronize(L->events[2 * i + 1]);
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, L->events[2 * i], L->events[2 * i + 1]);
+    cudaError_t e = cudaEventSynchronize(L->S.slot_events[2 * i + 1]);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, L->S.slot_events[2 * i], L->S.slot_events[2 * i + 1]);
     if (e != cudaSuccess) { cudaGetLastError(); ms = -1.f; }   // slot not recorded in the last step
     ms_out_host[i] = ms;
   }

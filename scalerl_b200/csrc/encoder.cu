@@ -367,102 +367,99 @@ static cudaError_t launch_wgrad_reduce(const float* part, int n, float* g, float
 }
 
 cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, const EncoderBuffers& buf, const TmaMaps& maps, int mode,
-                            cudaStream_t st, const Profiler& pf, cudaEvent_t wait_before_conv1, bool fused_front) {
+                            const StepStreams& S, bool fused_front) {
   if (frames <= 0) return cudaSuccess;
   if ((mode != 0 && mode != 1) || !maps.valid) return cudaErrorInvalidValue;
   const int sp = mode;                                    // 1: fp32-accurate split operands
   if (sp && !buf.lo.wpack) return cudaErrorInvalidValue;  // bf16 mode: the kernels never touch the low tensors and maps
+  const cudaStream_t st = S.main;
   // bf16 mode: frame conversion + conv1 + conv2 as ONE persistent kernel (enc_fused.cuh); SRL_FUSED_FWD=0 or the fp32-accurate
   // operand mode use the three separate kernels
   if (fused_front && !sp && (reinterpret_cast<uintptr_t>(obs) & 15) == 0) {
     EncFusedParams q{obs, p.w1, p.b1, p.w2, p.b2, buf.xs, buf.hi.a1, buf.hi.a2, frames, buf.NF};
-    pf.b(PS_ENC_FUSED); SRL_TRY(enc_fused_fwd_launch(q, kPersistentCtas, st)); pf.e(PS_ENC_FUSED);
-    if (wait_before_conv1) SRL_TRY(cudaStreamWaitEvent(st, wait_before_conv1, 0));      // conv3 / fc read the packed weights
+    S.b(PS_ENC_FUSED); SRL_TRY(enc_fused_fwd_launch(q, kPersistentCtas, st)); S.e(PS_ENC_FUSED);
+    SRL_TRY(S.join(LANE_PACK));      // conv3 / fc read the packed weights
   } else {
-  pf.b(PS_S2D); SRL_TRY(launch_s2d(obs, frames, buf.xs, st, p.w1, buf.hi.wpack + WPack::W1K, sp ? buf.lo.wpack + WPack::W1K : nullptr)); pf.e(PS_S2D);
+  S.b(PS_S2D); SRL_TRY(launch_s2d(obs, frames, buf.xs, st, p.w1, buf.hi.wpack + WPack::W1K, sp ? buf.lo.wpack + WPack::W1K : nullptr)); S.e(PS_S2D);
   { RConv1Fwd::Params q{maps.xs_w, maps.hi.w1k, maps.lo.w1k, p.b1, buf.hi.a1, buf.lo.a1, frames, buf.NF};
-    pf.b(PS_CONV1_FWD); SRL_TRY(res_fwd_launch<RConv1Fwd>(q, cdiv(frames * 441, 128), 2 * kPersistentCtas, st, sp)); pf.e(PS_CONV1_FWD); }
-  if (wait_before_conv1) SRL_TRY(cudaStreamWaitEvent(st, wait_before_conv1, 0));      // conv1's weight copy comes from the frame-conversion kernel; conv2 is the first reader of the re-packed copies
+    S.b(PS_CONV1_FWD); SRL_TRY(res_fwd_launch<RConv1Fwd>(q, cdiv(frames * 441, 128), 2 * kPersistentCtas, st, sp)); S.e(PS_CONV1_FWD); }
+  SRL_TRY(S.join(LANE_PACK));      // conv1's weight copy comes from the frame-conversion kernel; conv2 is the first reader of the re-packed copies
   { RConv2Fwd::Params q{maps.hi.a1p0_w, maps.hi.a1p1_w, maps.hi.w2k, maps.lo.a1p0_w, maps.lo.a1p1_w, maps.lo.w2k, p.b2, buf.hi.a2, buf.lo.a2, frames};
-    pf.b(PS_CONV2_FWD); SRL_TRY(res_fwd_launch<RConv2Fwd>(q, cdiv(frames * 100, 128), kPersistentCtas, st, sp)); pf.e(PS_CONV2_FWD); }
+    S.b(PS_CONV2_FWD); SRL_TRY(res_fwd_launch<RConv2Fwd>(q, cdiv(frames * 100, 128), kPersistentCtas, st, sp)); S.e(PS_CONV2_FWD); }
   }
   { RConv3Fwd::Params q{maps.hi.a2_w, maps.hi.w3k, maps.lo.a2_w, maps.lo.w3k, p.b3, buf.hi.a3, buf.lo.a3, frames};
-    pf.b(PS_CONV3_FWD); SRL_TRY(res_fwd_launch<RConv3Fwd>(q, cdiv(frames * 81, 128), kPersistentCtas, st, sp)); pf.e(PS_CONV3_FWD); }
+    S.b(PS_CONV3_FWD); SRL_TRY(res_fwd_launch<RConv3Fwd>(q, cdiv(frames * 81, 128), kPersistentCtas, st, sp)); S.e(PS_CONV3_FWD); }
   { TFcFwd::Params q{maps.hi.a3m128, maps.hi.wfk, maps.lo.a3m128, maps.lo.wfk, buf.hpart, frames};
     static_assert(TFcFwd::SPLITS == FC_SPLITS, "split count");
-    pf.b(PS_FC_FWD);
+    S.b(PS_FC_FWD);
     if (sp) SRL_TRY((igemm_tma_launch<TFcFwd, 1>(q, dim3(cdiv(frames, 128), 8 * FC_SPLITS), st)));
     else SRL_TRY((igemm_tma_launch<TFcFwd, 0>(q, dim3(cdiv(frames, 128), 8 * FC_SPLITS), st)));
-    pf.e(PS_FC_FWD); }
+    S.e(PS_FC_FWD); }
   return cudaSuccess;
 }
 
 cudaError_t encoder_backward(int frames, const EncoderBuffers& buf, const ParamPtrs& g, const TmaMaps& maps, int mode,
-                             cudaStream_t st, const Profiler& pf, const SideStream& ss, int phase) {
+                             const StepStreams& S, BwdParts parts, bool a3t_done) {
   if (frames <= 0) return cudaSuccess;
   if ((mode != 0 && mode != 1) || !maps.valid) return cudaErrorInvalidValue;
   const int sp = mode;
   if (sp && !buf.lo.wpack) return cudaErrorInvalidValue;
-  const bool do_fc = phase != 1, do_conv = phase != 0;
-  // The wgrad GEMMs only feed the optimizer: each runs on its own side stream beside the dgrad chain
-  // (dh -> da3 -> da2 -> da1) and beside each other.  With per-kernel profiling on everything stays on `st`.
-  const bool fork = ss.side != nullptr && !pf.on;
-  cudaStream_t s1 = fork ? ss.side : st, s2 = fork ? ss.side2 : st, s3 = fork ? ss.side3 : st;
-  Profiler p1 = pf, p2 = pf, p3 = pf; p1.st = s1; p2.st = s2; p3.st = s3;
+  const bool do_fc = parts & BWD_FC, do_conv = parts & BWD_CONV;
+  // The wgrad GEMMs only feed the optimizer: each runs on its own lane beside the dgrad chain (dh -> da3 -> da2 -> da1) and beside
+  // each other.
+  const cudaStream_t st = S.main, s1 = S.lane(LANE_FC_WGRAD), s2 = S.lane(LANE_CONV3_WGRAD), s3 = S.lane(LANE_CONV2_WGRAD);
   if (do_fc) {
-    if (fork) { SRL_TRY(cudaEventRecord(ss.ev[0], st)); SRL_TRY(cudaStreamWaitEvent(s1, ss.ev[0], 0)); }
+    SRL_TRY(S.fork(LANE_FC_WGRAD));
     { const bool native = !sp && buf.a3t != nullptr;          // bf16 mode: B operand = a3 transposed into fc.weight's column order, 256-column tiles
-      p1.b(PS_FC_WGRAD);
+      S.b(PS_FC_WGRAD);
       if (native) {
-        if (!buf.a3t_ready) SRL_TRY(launch_a3_transpose(buf.hi.a3, buf.a3t, frames, s1));
+        if (!a3t_done) SRL_TRY(launch_a3_transpose(buf.hi.a3, buf.a3t, frames, s1));
         TFcWgradN::Params q{maps.hi.dhm64, maps.a3tm64, g.wf, g.bf, frames};
         SRL_TRY((igemm_tma_launch<TFcWgradN, 0>(q, dim3(1, 4 * (TFcWgradN::NCT + 1)), s1)));
       } else {
         TFcWgrad::Params q{maps.hi.dhm64, maps.hi.a3m64, maps.lo.dhm64, maps.lo.a3m64, g.wf, g.bf, frames};
         if (sp) SRL_TRY((igemm_tma_launch<TFcWgrad, 1>(q, dim3(1, 4 * 50), s1))); else SRL_TRY((igemm_tma_launch<TFcWgrad, 0>(q, dim3(1, 4 * 50), s1)));
       }
-      buf.a3t_ready = false;
-      p1.e(PS_FC_WGRAD); }
+      S.e(PS_FC_WGRAD); }
     { TFcDgrad::Params q{maps.hi.dhm128, maps.hi.wfd, maps.lo.dhm128, maps.lo.wfd, buf.hi.a3, buf.hi.da3, buf.lo.da3, frames};
-      pf.b(PS_FC_DGRAD);
+      S.b(PS_FC_DGRAD);
       if (sp) SRL_TRY((igemm_tma_launch<TFcDgrad, 1>(q, dim3(cdiv(frames, 128), 49), st))); else SRL_TRY((igemm_tma_launch<TFcDgrad, 0>(q, dim3(cdiv(frames, 128), 49), st)));
-      pf.e(PS_FC_DGRAD); }
-    if (fork) { SRL_TRY(cudaEventRecord(ss.ev[4], s1)); }
-    if (fork && !do_conv) { SRL_TRY(cudaStreamWaitEvent(st, ss.ev[4], 0)); }
+      S.e(PS_FC_DGRAD); }
+    // the fc_wgrad lane also holds the head wgrad that the learner step forked there before this call: this join ends both
+    if (!do_conv) SRL_TRY(S.join(LANE_FC_WGRAD));
   }
   if (!do_conv) return cudaSuccess;
-  if (fork) { SRL_TRY(cudaEventRecord(ss.ev[1], st)); SRL_TRY(cudaStreamWaitEvent(s2, ss.ev[1], 0)); }
+  SRL_TRY(S.fork(LANE_CONV3_WGRAD));
   float* part3 = buf.wgrad_part;
   float* part2 = part3 + (size_t)WG_PART_CTAS * WSP_W3;
   float* part1 = part2 + (size_t)WG_PART_CTAS * WSP_W2;
   int n3 = 0, n2 = 0, n1 = 0;       // CTAs (partial slices) of the three wgrad launches
   { RConv3Wgrad::Params q{maps.hi.a2_w, maps.hi.da3g_b, maps.lo.a2_w, maps.lo.da3g_b, part3, frames * 81, 0};
-    p2.b(PS_CONV3_WGRAD); SRL_TRY(res_wgrad_launch<RConv3Wgrad>(q, side_wgrad_ctas(), s2, &n3, sp)); p2.e(PS_CONV3_WGRAD); }
-  // forked: each side-stream layer is reduced on its own stream as soon as its wgrad ends; otherwise all three reduces run at the end,
+    S.b(PS_CONV3_WGRAD); SRL_TRY(res_wgrad_launch<RConv3Wgrad>(q, side_wgrad_ctas(), s2, &n3, sp)); S.e(PS_CONV3_WGRAD); }
+  // lanes: each side layer is reduced on its own lane as soon as its wgrad ends; collapsed: all three reduces run at the end,
   // together in the conv_wgrad_finalize profile slot
-  if (fork) SRL_TRY(launch_wgrad_reduce<WgradReduce3>(part3, n3, g.w3, g.b3, s2));
+  if (!S.collapsed) SRL_TRY(launch_wgrad_reduce<WgradReduce3>(part3, n3, g.w3, g.b3, s2));
   { RConv3Dgrad::Params q{maps.hi.da3g_w, maps.hi.w3d, maps.lo.da3g_w, maps.lo.w3d, buf.hi.a2, buf.hi.da2, buf.lo.da2, frames};
-    pf.b(PS_CONV3_DGRAD); SRL_TRY(res_fwd_launch<RConv3Dgrad>(q, cdiv(frames * 81, 128), bwd_ctas(), st, sp)); pf.e(PS_CONV3_DGRAD); }
-  if (fork) { SRL_TRY(cudaEventRecord(ss.ev[2], st)); SRL_TRY(cudaStreamWaitEvent(s3, ss.ev[2], 0)); }
+    S.b(PS_CONV3_DGRAD); SRL_TRY(res_fwd_launch<RConv3Dgrad>(q, cdiv(frames * 81, 128), bwd_ctas(), st, sp)); S.e(PS_CONV3_DGRAD); }
+  SRL_TRY(S.fork(LANE_CONV2_WGRAD));
   { RConv2Wgrad::Params q{maps.hi.a1p0_w, maps.hi.a1p1_w, maps.hi.da2g_b, maps.lo.a1p0_w, maps.lo.a1p1_w, maps.lo.da2g_b, part2, frames * 100, 0};
-    p3.b(PS_CONV2_WGRAD); SRL_TRY(res_wgrad_launch<RConv2Wgrad>(q, side_wgrad_ctas(), s3, &n2, sp)); p3.e(PS_CONV2_WGRAD); }
-  if (fork) SRL_TRY(launch_wgrad_reduce<WgradReduce2>(part2, n2, g.w2, g.b2, s3));
+    S.b(PS_CONV2_WGRAD); SRL_TRY(res_wgrad_launch<RConv2Wgrad>(q, side_wgrad_ctas(), s3, &n2, sp)); S.e(PS_CONV2_WGRAD); }
+  if (!S.collapsed) SRL_TRY(launch_wgrad_reduce<WgradReduce2>(part2, n2, g.w2, g.b2, s3));
   { RConv2Dgrad::Params q{maps.hi.da2g_w, maps.hi.w2d, maps.lo.da2g_w, maps.lo.w2d, buf.hi.a1, buf.hi.da1, buf.lo.da1, frames, buf.NF};
-    pf.b(PS_CONV2_DGRAD); SRL_TRY(res_fwd_launch<RConv2Dgrad>(q, cdiv(frames * 100, 128), bwd_ctas(), st, sp)); pf.e(PS_CONV2_DGRAD); }
+    S.b(PS_CONV2_DGRAD); SRL_TRY(res_fwd_launch<RConv2Dgrad>(q, cdiv(frames * 100, 128), bwd_ctas(), st, sp)); S.e(PS_CONV2_DGRAD); }
   { RConv1Wgrad::Params q{maps.xs_w, maps.hi.da1g_b, maps.lo.da1g_b, part1, frames * 441, 0};
-    pf.b(PS_CONV1_WGRAD); SRL_TRY(res_wgrad_launch<RConv1Wgrad>(q, bwd_ctas(), st, &n1, sp)); pf.e(PS_CONV1_WGRAD); }
-  pf.b(PS_WGRAD_FINALIZE);
-  if (!fork) {
+    S.b(PS_CONV1_WGRAD); SRL_TRY(res_wgrad_launch<RConv1Wgrad>(q, bwd_ctas(), st, &n1, sp)); S.e(PS_CONV1_WGRAD); }
+  S.b(PS_WGRAD_FINALIZE);
+  if (S.collapsed) {
     SRL_TRY(launch_wgrad_reduce<WgradReduce3>(part3, n3, g.w3, g.b3, st));
     SRL_TRY(launch_wgrad_reduce<WgradReduce2>(part2, n2, g.w2, g.b2, st));
   }
   SRL_TRY(launch_wgrad_reduce<WgradReduce1>(part1, n1, g.w1, g.b1, st));
-  pf.e(PS_WGRAD_FINALIZE);
-  if (fork) {      // join: fc wgrad (phase 2 only: phase 1 was joined by the caller of phase 0), conv3 and conv2 wgrad + reduce
-    if (do_fc) { SRL_TRY(cudaStreamWaitEvent(st, ss.ev[4], 0)); }
-    SRL_TRY(cudaEventRecord(ss.ev[3], s2)); SRL_TRY(cudaStreamWaitEvent(st, ss.ev[3], 0));
-    SRL_TRY(cudaEventRecord(ss.ev[7], s3)); SRL_TRY(cudaStreamWaitEvent(st, ss.ev[7], 0));
-  }
+  S.e(PS_WGRAD_FINALIZE);
+  // the fc_wgrad lane (with the learner step's head wgrad) only if this call ran the fc part: a BWD_FC call joined it already
+  if (do_fc) SRL_TRY(S.join(LANE_FC_WGRAD));
+  SRL_TRY(S.join(LANE_CONV3_WGRAD));
+  SRL_TRY(S.join(LANE_CONV2_WGRAD));
   return cudaSuccess;
 }
 

@@ -11,19 +11,11 @@ namespace srl {
 enum ProfSlot { PS_S2D = 0, PS_CONV1_FWD, PS_CONV2_FWD, PS_CONV3_FWD, PS_FC_FWD, PS_HEAD_FWD, PS_TAIL, PS_ZERO_GRADS, PS_HEAD_BWD,
                 PS_FC_WGRAD, PS_FC_DGRAD, PS_CONV3_WGRAD, PS_CONV3_DGRAD, PS_CONV2_WGRAD, PS_CONV2_DGRAD, PS_CONV1_WGRAD,
                 PS_WGRAD_FINALIZE, PS_GRAD_NORM, PS_OPTIMIZER, PS_PACK, PS_ENC_FUSED, PS_COUNT };
-struct Profiler {
-  bool on = false;
-  cudaEvent_t* ev = nullptr;   // 2 * PS_COUNT events
-  cudaStream_t st = nullptr;
-  void b(int slot) const { if (on) cudaEventRecord(ev[2 * slot], st); }
-  void e(int slot) const { if (on) cudaEventRecord(ev[2 * slot + 1], st); }
-};
-// second stream + fork/join events: the wgrad GEMMs run beside the dgrad chain (also under stream capture)
 // ---- programmatic dependent launch (see common.cuh) ----------------------------------------------------------
 // pdl_active(): SRL_PDL != 0 (default on) and not switched off by the caller (per-kernel profiling records events between
 // the kernels, which would serialise them anyway).
 bool pdl_active();
-void pdl_set_active(bool on);      // per calling thread: every C-ABI entry point sets it for the launches it makes
+void pdl_set_active(bool on);      // per calling thread: every C-ABI entry point that reaches launch_chain sets it first
 template <class... KA, class... A>
 inline cudaError_t launch_chain(void (*kernel)(KA...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A... args) {
   cudaLaunchConfig_t cfg = {};
@@ -60,12 +52,32 @@ inline cudaError_t ensure_max_dynamic_smem(PerDeviceOnce& once, K kernel, int by
 void kstamp_set_encoder(unsigned long long*); void kstamp_set_vtrace(unsigned long long*); void kstamp_set_heads(unsigned long long*);   // diagnostics build (common.cuh)
 void kstamp_set_optim(unsigned long long*);
 
-struct SideStream {
-  cudaStream_t side = nullptr;      // fc wgrad, weight re-pack
-  cudaStream_t side2 = nullptr;     // conv3 wgrad
-  cudaStream_t side3 = nullptr;     // conv2 wgrad
-  cudaStream_t pack = nullptr;      // weight re-pack + gradient memset at the start of a step: above the wgrad streams' priority (conv2 waits for it; api.cu pack_priority)
-  cudaEvent_t ev[12] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+// The stream schedule of one learner call: `main` is the caller's stream, each lane a stream of the learner context that runs work
+// beside it (also under capture): pack (weight re-pack + gradient memset; priority: api.cu pack_priority), fc_wgrad (a3 transpose,
+// head wgrad, fc wgrad), conv3_wgrad and conv2_wgrad (each with its reduce).  fork(l): the lane waits for all work on main so far;
+// join(l): main waits for all work on the lane so far.  cudaStreamWaitEvent binds to the event's latest record (eagerly and under
+// capture), so one fork and one join event per lane serve every edge.  Collapsed (per-kernel profiling on, or the lanes could not be
+// created): every lane is main and fork / join do nothing.
+enum Lane { LANE_PACK, LANE_FC_WGRAD, LANE_CONV3_WGRAD, LANE_CONV2_WGRAD, LANE_COUNT };
+struct StepStreams {
+  cudaStream_t main = nullptr;
+  cudaStream_t side[LANE_COUNT] = {};
+  cudaEvent_t forked[LANE_COUNT] = {}, joined[LANE_COUNT] = {};
+  bool have_lanes = false;          // every lane stream and event was created (srl_learner_create)
+  bool collapsed = true;
+  bool profiling = false;           // per-kernel event bracketing on main (srl_learner_set_profiling): slots of one learner step
+  cudaEvent_t slot_events[2 * PS_COUNT] = {};
+  // the start of every learner call that launches work: main, the collapse state and the PDL mode; returns main
+  cudaStream_t begin_call(cudaStream_t st) { main = st; collapsed = !have_lanes || profiling; pdl_set_active(!profiling); return st; }
+  cudaStream_t lane(Lane l) const { return collapsed ? main : side[l]; }
+  cudaError_t fork(Lane l) const { return collapsed ? cudaSuccess : edge(forked[l], main, side[l]); }
+  cudaError_t join(Lane l) const { return collapsed ? cudaSuccess : edge(joined[l], side[l], main); }
+  void b(int slot) const { if (profiling) cudaEventRecord(slot_events[2 * slot], main); }
+  void e(int slot) const { if (profiling) cudaEventRecord(slot_events[2 * slot + 1], main); }
+  static cudaError_t edge(cudaEvent_t ev, cudaStream_t from, cudaStream_t to) {
+    const cudaError_t e = cudaEventRecord(ev, from);
+    return e != cudaSuccess ? e : cudaStreamWaitEvent(to, ev, 0);
+  }
 };
 
 // per-CTA partials of the wgrad kernels (each CTA stores its accumulators, in the kernel's native [tap-block][row][co] order, and its
@@ -184,7 +196,6 @@ struct OperandTensors {
 struct EncoderBuffers {   // row layouts: see res_problems.cuh
   __nv_bfloat16* xs;                    // space-to-depth bf16 copy of the u8 frames [NF*441][64], 64 = (c,dy,dx)
   OperandTensors hi, lo = {};           // lo: all null in the bf16 mode
-  mutable bool a3t_ready = false;       // the transpose below was already launched for this step (early, under the column kernel: api.cu encode_impl)
   __nv_bfloat16* a3t = nullptr;         // [NF][64*49]: a3 of the learning frames in fc.weight's own column order (c,h,w) -- fc wgrad's B operand (bf16 mode)
   float* hpart;                         // [FC_SPLITS][NF][512] split-K partials of the fc layer
   float* h;                             // [NF][512] fc output (post-ReLU), fp32
@@ -211,16 +222,17 @@ cudaError_t build_tma_maps(const EncoderBuffers& buf, int NF, int NB, TmaMaps* m
 // wpack_lo != nullptr: also the low copies bf16(w - bf16(w)) in the same layouts
 cudaError_t launch_a3_transpose(const __nv_bfloat16* a3, __nv_bfloat16* a3t, int frames, cudaStream_t st);
 cudaError_t launch_pack_weights(const ParamPtrs& p, __nv_bfloat16* wpack, cudaStream_t st, __nv_bfloat16* wpack_lo = nullptr, bool skip_w1k = false);
-// wait_before_conv1: optional event (weight re-pack running on the side stream) that conv1 must wait for
+// on S.main; joins the pack lane (the weight re-pack forked by the caller) before the first reader of the re-packed weights.
 // mode: 0 = bf16 operands, 1 = fp32-accurate split operands (buf.lo and maps.lo must be built)
+// fused_front: frame conversion + conv1 + conv2 in one kernel (enc_fused.cuh; bf16 mode)
 cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, const EncoderBuffers& buf, const TmaMaps& maps, int mode,
-                            cudaStream_t st, const Profiler& pf, cudaEvent_t wait_before_conv1,
-                            bool fused_front = true);      // fused_front: frame conversion + conv1 + conv2 in one kernel (enc_fused.cuh; bf16 mode)
-// backward for the first `frames` frames given buf.hi.dh; accumulates into the (pre-zeroed) gradient tensors in `g`
-// phase: 0 = fc layer only (fc.weight / fc.bias gradients complete and joined to `st` on return: 95 % of the gradient
-//        bytes, ready for an early all-reduce), 1 = conv layers only, 2 = both
+                            const StepStreams& S, bool fused_front);
+// backward for the first `frames` frames given buf.hi.dh; accumulates into the (pre-zeroed) gradient tensors in `g`.  BWD_FC: the fc
+// layer only (fc.weight / fc.bias gradients complete and joined to main on return: 95 % of the gradient bytes, ready for an early
+// all-reduce); BWD_CONV: the conv layers only.  a3t_done: the caller already launched a3 -> buf.a3t on the fc_wgrad lane (bf16 mode)
+enum BwdParts { BWD_FC = 1, BWD_CONV = 2, BWD_BOTH = BWD_FC | BWD_CONV };
 cudaError_t encoder_backward(int frames, const EncoderBuffers& buf, const ParamPtrs& g, const TmaMaps& maps, int mode,
-                             cudaStream_t st, const Profiler& pf, const SideStream& ss, int phase);
+                             const StepStreams& S, BwdParts parts, bool a3t_done);
 // ---- lstm.cu: the actor step of the 2-layer LSTM core (one row of B environments, no BPTT)
 struct LstmStep;
 // weights8: the 8 nn.LSTM tensors of the flat parameter buffer (srl_lstm_create order); H = 513 + A
