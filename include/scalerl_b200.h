@@ -253,6 +253,29 @@ int srl_host_unregister(void* ptr_host);
 /* asynchronous device-to-device copy on `stream` (used by tests to read the borrowed buffers) */
 int srl_memcpy_d2d(void* dst, const void* src, int64_t bytes, void* stream);
 
+/* ---- stand-alone encoder: the trainable AtariNet's conv/fc stack under autograd --------------------------------------------
+ * replaces atari_model.py:91-107 (obs -> /255 -> conv1..3 -> fc -> ReLU -> [h, clamp(reward,-1,1), one_hot(action)]) and its
+ * autograd; the LSTM core and the heads stay with the caller (scalerl_b200.algorithms.utils.atari_model.AtariNet).  The kernels
+ * and the stream lanes are the learner's; every activation lives in two caller-owned blocks, so each forward keeps its own:
+ *   saved   : written by the forward, read by its backward (activations + the packed weights the forward ran with);
+ *   scratch : one call's temporaries (forward and backward alike; its contents do not outlive the call).
+ * srl_encoder_sizes gives both blocks' bytes for a frame count and precision (0 = bf16 operands, 1 = fp32-accurate split operands, as
+ * srl_config_t.precision).  Both blocks are 256-byte aligned, need no initialisation and must not overlap each other or any other argument.
+ * A context holds only the lanes, their events and the precision: one per device, created on that device. */
+typedef struct srl_encoder srl_encoder_t;
+int srl_encoder_create(int precision, srl_encoder_t** out);
+int srl_encoder_destroy(srl_encoder_t* E);
+int srl_encoder_sizes(int frames, int precision, int64_t* saved_bytes, int64_t* scratch_bytes);
+/* forward for `frames` <= 65536 frames: obs u8 [frames,4,84,84], reward f32 [frames], action i64 [frames] (clamped to [0,A)),
+ * weights8 = {conv1.weight, conv1.bias, conv2.weight, conv2.bias, conv3.weight, conv3.bias, fc.weight, fc.bias} (f32, PyTorch layouts,
+ * 16-byte aligned) -> core_out f32 [frames, 513+A] = [h (512), clamp(reward,-1,1), one_hot(action) (A)]. */
+int srl_encoder_forward(srl_encoder_t* E, const uint8_t* obs, const float* reward, const int64_t* action, int frames, int A,
+                        const float* const* weights8, void* saved, void* scratch, float* core_out, void* stream);
+/* backward of the forward that filled `saved` (same frames, A and context precision): dcore f32 [frames, 513+A] (columns >= 512 are
+ * not read) -> the 8 gradients of weights8's tensors, PyTorch layouts, 16-byte aligned, OVERWRITTEN (not accumulated). */
+int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int frames, int A, void* saved, void* scratch, float* const* grads8,
+                         void* stream);
+
 /* ---- LSTM core (AtariNet use_lstm=True; atari_model.py:52-55,109-120; SURVEY.md §8 row a17) -------------------------------
  * 2-layer LSTM(H, H), H = 513 + A, stepped with the state multiplied by (1 - done_t) before every step.
  * weights8 / grads8: 8 device pointers in nn.LSTM state_dict order {weight_ih_l0 [4H,H], weight_hh_l0 [4H,H], bias_ih_l0 [4H],

@@ -54,6 +54,11 @@ _SIGS = {
     'srl_learner_apply_gradients': [_P, _P, _P],
     'srl_learner_apply_gradients_dp': [_P, _P, _P, _P],
     'srl_learner_debug_buffer': [_P, C.c_char_p, C.POINTER(_P), C.POINTER(_L)],
+    'srl_encoder_create': [_I, C.POINTER(_P)],
+    'srl_encoder_destroy': [_P],
+    'srl_encoder_sizes': [_I, _I, C.POINTER(_L), C.POINTER(_L)],
+    'srl_encoder_forward': [_P, _P, _P, _P, _I, _I, C.POINTER(_P), _P, _P, _P, _P],
+    'srl_encoder_backward': [_P, _P, _I, _I, _P, _P, C.POINTER(_P), _P],
     'srl_lstm_create': [_I, _I, _I, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)],
     'srl_lstm_destroy': [_P],
     'srl_lstm_forward': [_P, _P, _P, _P, _P, _P, _P, _P, _P],

@@ -9,12 +9,19 @@ layouts -- so ImpalaTrainer treats it and the reference's own ``AtariNet`` ident
 ``actor_model_fn``); its parameters live in shared memory and are overwritten by the learner's weight publish.
 ``SyntheticAtariEnv`` emits the TorchEnvWrapper record schema (scalerl/envs/torch_envwrapper.py:43-50,77-84)
 with random frames; it exists so the actor/ring/learner plumbing can be exercised without gymnasium/ale_py.
+``AtariNet`` is the trainable drop-in for the reference's ``AtariNet`` (atari_model.py:8-143): the same submodules, parameters
+and calling convention, with the encoder (obs -> conv1..3 -> fc -> [h, clipped reward, one-hot last action]) and its backward on
+the learner's sm_90a kernels under torch autograd.
 """
+import ctypes as C
 from collections import OrderedDict
 
 import torch
 import torch.nn.functional as F
+from torch import nn
+from torch.autograd.function import once_differentiable
 
+from ... import _lib
 from ...learner import param_shapes, reference_param_order
 
 
@@ -126,6 +133,202 @@ class ActorNet(torch.nn.Module):
         else:
             action = torch.argmax(logits, dim=1)
         return dict(policy_logits=logits.view(T, B, -1), baseline=baseline.view(T, B), action=action.view(T, B)), rnn_state
+
+
+PRECISIONS = {'bf16': 0, 'fp32_split': 1}     # ImpalaHParams.precision -> srl_config_t.precision
+MAX_ACTIONS = 31                             # one warp lane per action plus one for the baseline, as B200ImpalaLearner
+MAX_FRAMES = 65536                           # T * B of one call
+
+
+class _EncoderContexts:
+    """The native encoder contexts of one AtariNet, one per device: the stream lanes, their events and the precision (no
+    activations: those belong to each call).  Created on the first forward on a device, released with the module; a deep copy
+    starts without any."""
+
+    def __init__(self, precision: int):
+        self.precision = precision
+        self.handles = {}
+
+    def get(self, device: torch.device) -> C.c_void_p:
+        h = self.handles.get(device.index)
+        if h is None:
+            h = C.c_void_p()
+            with torch.cuda.device(device):
+                _lib.check(_lib.lib().srl_encoder_create(self.precision, C.byref(h)), 'srl_encoder_create')
+            self.handles[device.index] = h
+        return h
+
+    def __deepcopy__(self, memo):
+        return _EncoderContexts(self.precision)
+
+    def __getstate__(self):
+        return {'precision': self.precision}
+
+    def __setstate__(self, state):
+        self.precision, self.handles = state['precision'], {}
+
+    def __del__(self):
+        try:
+            for h in self.handles.values():
+                _lib.lib().srl_encoder_destroy(h)
+        except Exception:      # interpreter shutdown: the library may already be gone
+            pass
+        self.handles = {}
+
+
+def encoder_block_sizes(frames: int, precision: str = 'bf16'):
+    """(bytes a forward keeps for its backward, bytes of one call's scratch) for ``frames`` frames"""
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be one of {sorted(PRECISIONS)}, got {precision!r}")
+    saved, scratch = C.c_int64(), C.c_int64()
+    _lib.check(_lib.lib().srl_encoder_sizes(int(frames), PRECISIONS[precision], C.byref(saved), C.byref(scratch)), 'srl_encoder_sizes')
+    return saved.value, scratch.value
+
+
+def _ptrs8(tensors):
+    return (C.c_void_p * 8)(*[t.data_ptr() for t in tensors])
+
+
+def _encoder_forward(handle, precision, num_actions, obs, reward, action, weights):
+    """-> (core [N, 513+A], the forward's saved block); obs / reward / action flat over N frames, on the weights' device"""
+    n, dev = reward.numel(), reward.device
+    saved_bytes, scratch_bytes = encoder_block_sizes(n, precision)
+    saved = torch.empty(saved_bytes, dtype=torch.uint8, device=dev)
+    scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev)
+    core = torch.empty(n, 513 + num_actions, dtype=torch.float32, device=dev)
+    _lib.check(_lib.lib().srl_encoder_forward(handle, obs.data_ptr(), reward.data_ptr(), action.data_ptr(), n, num_actions, _ptrs8(weights),
+                                              saved.data_ptr(), scratch.data_ptr(), core.data_ptr(), torch.cuda.current_stream(dev).cuda_stream),
+               'srl_encoder_forward')
+    return core, saved
+
+
+class _EncoderCore(torch.autograd.Function):
+    """core = [relu(fc(conv3(conv2(conv1(obs / 255))))), clamp(reward, -1, 1), one_hot(action)] (atari_model.py:91-107), differentiable
+    in the 8 conv / fc tensors.  The forward's activations and packed weights are one block saved on ``ctx``: every call keeps its own,
+    and the gradient is taken at the weights the forward ran with."""
+
+    @staticmethod
+    def forward(ctx, handle, precision, num_actions, obs, reward, action, *weights):
+        core, saved = _encoder_forward(handle, precision, num_actions, obs, reward, action, weights)
+        ctx.save_for_backward(saved)
+        ctx.call = (handle, precision, num_actions, reward.numel(), [w.shape for w in weights])
+        return core
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dcore):
+        handle, precision, num_actions, n, shapes = ctx.call
+        (saved,) = ctx.saved_tensors
+        dev = saved.device
+        dcore = dcore.contiguous()
+        grads = [torch.empty(s, dtype=torch.float32, device=dev) for s in shapes]
+        scratch = torch.empty(encoder_block_sizes(n, precision)[1], dtype=torch.uint8, device=dev)
+        _lib.check(_lib.lib().srl_encoder_backward(handle, dcore.data_ptr(), n, num_actions, saved.data_ptr(), scratch.data_ptr(),
+                                                   _ptrs8(grads), torch.cuda.current_stream(dev).cuda_stream), 'srl_encoder_backward')
+        return (None,) * 6 + tuple(grads)
+
+
+class AtariNet(nn.Module):
+    """Drop-in for the reference's ``AtariNet`` (scalerl/algorithms/utils/atari_model.py:8-143) that trains on the sm_90a encoder.
+
+    Submodules, their names, creation order and initialisation are the reference's, so ``state_dict()`` and the initial weights under
+    ``torch.manual_seed`` match it.  ``forward(inputs, rnn_state)`` takes and returns what the reference's does; the encoder up to the
+    LSTM / head input runs as one autograd function on the learner's kernels, the LSTM loop, the heads and the action sampling are torch.
+    ``precision``: 'bf16' or 'fp32_split', as ``ImpalaHParams.precision``.  ``validate_inputs``: raise on actions outside [0, A) as
+    ``F.one_hot`` does (one host synchronisation per forward); otherwise they are clamped.  CUDA only: CPU actors use ``ActorNet``."""
+
+    def __init__(self, observation_shape, num_actions, use_lstm=False, *, precision='bf16', validate_inputs=False):
+        super().__init__()
+        if tuple(observation_shape) != (4, 84, 84):
+            raise ValueError(f'observation_shape must be (4, 84, 84), got {tuple(observation_shape)}')
+        if not 1 <= int(num_actions) <= MAX_ACTIONS:
+            raise ValueError(f'num_actions={num_actions} must be in [1, {MAX_ACTIONS}]')
+        if precision not in PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(PRECISIONS)}, got {precision!r}")
+        self.observation_shape = observation_shape
+        self.num_actions = int(num_actions)
+        self.precision = precision
+        self.validate_inputs = validate_inputs
+        self.conv1 = nn.Conv2d(4, 32, kernel_size=8, stride=4)
+        self.conv2 = nn.Conv2d(32, 64, kernel_size=4, stride=2)
+        self.conv3 = nn.Conv2d(64, 64, kernel_size=3, stride=1)
+        self.fc = nn.Linear(3136, 512)
+        core_size = 512 + 1 + self.num_actions
+        self.use_lstm = use_lstm
+        if use_lstm:
+            self.rnn_layer = nn.LSTM(core_size, core_size, num_layers=2)
+        self.policy = nn.Linear(core_size, self.num_actions)
+        self.baseline = nn.Linear(core_size, 1)
+        self._contexts = _EncoderContexts(PRECISIONS[precision])
+
+    def initial_hidden_state(self, batch_size: int):
+        """() without the LSTM, else (h0, c0): zeros [num_layers, batch_size, hidden_size] on the CPU (atari_model.py:61-75)"""
+        if not self.use_lstm:
+            return tuple()
+        return tuple(torch.zeros(self.rnn_layer.num_layers, batch_size, self.rnn_layer.hidden_size) for _ in range(2))
+
+    def _encoder_weights(self):
+        return [self.conv1.weight, self.conv1.bias, self.conv2.weight, self.conv2.bias, self.conv3.weight, self.conv3.bias,
+                self.fc.weight, self.fc.bias]
+
+    def encode(self, obs, reward, action):
+        """core f32 [T*B, 513+A] = [relu(fc(...conv1(obs / 255))), clamp(reward, -1, 1), one_hot(action)] for obs u8 [T,B,4,84,84],
+        reward f32 [T,B] and action i64 [T,B] on the module's CUDA device; differentiable in the conv / fc parameters."""
+        weights = self._encoder_weights()
+        for name, t in (('obs', obs), ('reward', reward), ('action', action)):
+            if not isinstance(t, torch.Tensor) or not t.is_cuda:
+                raise ValueError(f"inputs['{name}'] must be a CUDA tensor: AtariNet has no CPU path (CPU actors use ActorNet)")
+        dev = weights[0].device
+        if not dev.type == 'cuda':
+            raise ValueError('AtariNet has no CPU path: move the module to a CUDA device (.cuda() / .to(device))')
+        if any(t.device != dev for t in (obs, reward, action)):
+            raise ValueError(f'inputs must be on the parameters\' device {dev}')
+        if any(w.dtype != torch.float32 for w in weights):
+            raise ValueError('the conv / fc parameters must be float32')
+        if obs.dtype != torch.uint8 or obs.dim() != 5 or tuple(obs.shape[2:]) != (4, 84, 84):
+            raise ValueError(f"inputs['obs'] must be uint8 [T, B, 4, 84, 84], got {obs.dtype} {tuple(obs.shape)}")
+        T, B = obs.shape[:2]
+        if not 1 <= T * B <= MAX_FRAMES:
+            raise ValueError(f'T*B = {T * B} frames: must be in [1, {MAX_FRAMES}]')
+        if reward.dtype != torch.float32 or tuple(reward.shape) != (T, B):
+            raise ValueError(f"inputs['reward'] must be float32 [{T}, {B}], got {reward.dtype} {tuple(reward.shape)}")
+        if action.dtype != torch.int64 or tuple(action.shape) != (T, B):
+            raise ValueError(f"inputs['action'] must be int64 [{T}, {B}], got {action.dtype} {tuple(action.shape)}")
+        if reward.requires_grad:
+            raise ValueError("inputs['reward'] requires grad, but the encoder gives the reward column no gradient")
+        if self.validate_inputs and bool(((action < 0) | (action >= self.num_actions)).any()):
+            raise RuntimeError(f'Class values must be smaller than num_classes ({self.num_actions}) and non-negative: '
+                               f"inputs['action'] has min {int(action.min())}, max {int(action.max())}")
+        obs, reward, action = obs.contiguous(), reward.contiguous(), action.contiguous()
+        weights = [w.contiguous() for w in weights]
+        handle, prec = self._contexts.get(dev), self.precision
+        if torch.is_grad_enabled() and any(w.requires_grad for w in weights):
+            return _EncoderCore.apply(handle, prec, self.num_actions, obs, reward, action, *weights)
+        return _encoder_forward(handle, prec, self.num_actions, obs, reward, action, weights)[0]
+
+    def forward(self, inputs, rnn_state=()):
+        """(dict(policy_logits [T,B,A], baseline [T,B], action [T,B]), rnn_state), as atari_model.py:77-143"""
+        T, B = inputs['obs'].shape[:2]
+        core = self.encode(inputs['obs'], inputs['reward'], inputs['action'])
+        if self.use_lstm:
+            steps = core.view(T, B, -1).unbind()
+            notdone = (~inputs['done']).float().unbind()
+            outs = []
+            for x, nd in zip(steps, notdone):          # the state is zeroed where an episode ended before the step
+                rnn_state = tuple(nd.view(1, -1, 1) * s for s in rnn_state)
+                y, rnn_state = self.rnn_layer(x.unsqueeze(0), rnn_state)
+                outs.append(y)
+            core = torch.cat(outs).flatten(0, 1)
+        else:
+            rnn_state = tuple()
+        policy_logits = self.policy(core)
+        baseline = self.baseline(core)
+        if self.training:
+            action = torch.multinomial(F.softmax(policy_logits, dim=1), num_samples=1)
+        else:
+            action = torch.argmax(policy_logits, dim=1)
+        return (dict(policy_logits=policy_logits.view(T, B, self.num_actions), baseline=baseline.view(T, B), action=action.view(T, B)),
+                rnn_state)
 
 
 class SyntheticAtariEnv:

@@ -247,23 +247,47 @@ static WsRow ws_row(const char* name, int64_t count, T** hi, T** lo = nullptr) {
   return {name, (int)sizeof(T), count, reinterpret_cast<void**>(hi), reinterpret_cast<void**>(lo)};
 }
 constexpr int WS_MAX_ROWS = 32;
-static int workspace_table(srl_learner* L, WsRow* t) {
-  const srl_config_t& c = L->cfg;
-  const int64_t NF = (int64_t)(c.T + 1) * c.B, NB = (int64_t)c.T * c.B, A = c.A, H = 513 + A;
-  EncoderBuffers& b = L->buf;
+// The encoder's rows, for NF forward and NB backward frames.  The first ENC_SAVED_ROWS are what a backward reads of its forward: the
+// activations and the packed weights the forward ran with.  The rest live for one call: the fc layer's split-K partials (forward),
+// the gradient operands and the wgrad partials (backward).  da3, da2 and da1 are adjacent, low twins included: one memset clears them.
+constexpr int ENC_SAVED_ROWS = 6, ENC_ROWS = 13;
+static int encoder_rows(EncoderBuffers& b, int64_t NF, int64_t NB, WsRow* t) {
   OperandTensors &hi = b.hi, &lo = b.lo;
   int n = 0;
   t[n++] = ws_row("xs", NF * 441 * 64, &b.xs);
-  t[n++] = ws_row(nullptr, FC_SPLITS * NF * 512, &b.hpart);
   t[n++] = ws_row("a1", NF * 400 * 32, &hi.a1, &lo.a1);
   t[n++] = ws_row("a2", NF * 81 * 64, &hi.a2, &lo.a2);
   t[n++] = ws_row("a3", NF * 49 * 64, &hi.a3, &lo.a3);
   t[n++] = ws_row("h", NF * 512, &b.h);
+  t[n++] = ws_row("wpack", WPack::TOTAL, &hi.wpack, &lo.wpack);
+  t[n++] = ws_row(nullptr, FC_SPLITS * NF * 512, &b.hpart);
   t[n++] = ws_row("dh", NB * 512, &hi.dh, &lo.dh);
   t[n++] = ws_row("da3", NB * 81 * 64, &hi.da3, &lo.da3);      // da3g (9x9 grid)
   t[n++] = ws_row("da2", NB * 100 * 64, &hi.da2, &lo.da2);     // da2g (10x10 grid)
   t[n++] = ws_row("da1", NB * 441 * 32, &hi.da1, &lo.da1);     // da1g (21x21 grid, 32 channels)
-  t[n++] = ws_row("wpack", WPack::TOTAL, &hi.wpack, &lo.wpack);
+  t[n++] = ws_row("wgrad_part", WSP_TOTAL, &b.wgrad_part);
+  t[n++] = ws_row("a3t", NF * 49 * 64, &b.a3t);
+  return n;
+}
+static int64_t ws_bytes(const WsRow& r) { return ((int64_t)r.elem * r.count + 255) & ~int64_t(255); }
+// bytes of rows [0, n), a low twin after each row that has one in the fp32-accurate mode (split)
+static int64_t rows_bytes(const WsRow* t, int n, bool split) {
+  int64_t total = 0;
+  for (int i = 0; i < n; ++i) total += ws_bytes(t[i]) * (split && t[i].lo ? 2 : 1);
+  return total;
+}
+// gives rows [0, n) consecutive addresses from q (each row padded to 256 bytes), in table order
+static void carve_rows(const WsRow* t, int n, bool split, char* q) {
+  for (int i = 0; i < n; ++i) {
+    if (t[i].hi) *t[i].hi = q;
+    q += ws_bytes(t[i]);
+    if (split && t[i].lo) { *t[i].lo = q; q += ws_bytes(t[i]); }
+  }
+}
+static int workspace_table(srl_learner* L, WsRow* t) {
+  const srl_config_t& c = L->cfg;
+  const int64_t NF = (int64_t)(c.T + 1) * c.B, NB = (int64_t)c.T * c.B, A = c.A, H = 513 + A;
+  int n = encoder_rows(L->buf, NF, NB, t);
   t[n++] = ws_row("logits", NF * A, &L->logits);
   t[n++] = ws_row("baseline", NF, &L->baseline);
   t[n++] = ws_row("dlogits", NB * A, &L->dlogits);
@@ -271,9 +295,7 @@ static int workspace_table(srl_learner* L, WsRow* t) {
   t[n++] = ws_row(nullptr, 4096, &L->scratch);
   t[n++] = ws_row(nullptr, 4, &L->coef);
   t[n++] = ws_row(nullptr, 4, &L->dstep);
-  t[n++] = ws_row("wgrad_part", WSP_TOTAL, &b.wgrad_part);
   t[n++] = ws_row(nullptr, HEAD_GROUPS * (A + 1) * (514 + A), &L->head_part);
-  t[n++] = ws_row("a3t", NF * 49 * 64, &b.a3t);
   if (c.use_lstm) {
     t[n++] = ws_row(nullptr, NF * H, &L->core);
     t[n++] = ws_row(nullptr, NF * H, &L->lstm_out);
@@ -283,12 +305,29 @@ static int workspace_table(srl_learner* L, WsRow* t) {
   }
   return n;
 }
-static int64_t ws_bytes(const WsRow& r) { return ((int64_t)r.elem * r.count + 255) & ~int64_t(255); }
 
 // the re-pack lane sits one level BELOW the greatest priority (which the learner's capture stream uses for the main chain) and above the wgrad
 // lanes (default = least): its short blocks fill the slots the frame conversion leaves free without delaying it
 static int pack_priority(int least, int greatest) {
   return greatest + 1 > least ? least : greatest + 1;
+}
+// the lanes of a context: without them every call runs collapsed on the caller's stream
+static void create_lanes(StepStreams& S) {
+  int lo = 0, hi = 0;       // (numerically lowest = greatest priority)
+  bool ok = cudaDeviceGetStreamPriorityRange(&lo, &hi) == cudaSuccess;
+  for (int l = 0; l < LANE_COUNT && ok; ++l)        // the wgrad lanes take the default priority (0, the least)
+    ok = cudaStreamCreateWithPriority(&S.side[l], cudaStreamNonBlocking, l == LANE_PACK ? pack_priority(lo, hi) : 0) == cudaSuccess &&
+         cudaEventCreateWithFlags(&S.forked[l], cudaEventDisableTiming) == cudaSuccess &&
+         cudaEventCreateWithFlags(&S.joined[l], cudaEventDisableTiming) == cudaSuccess;
+  S.have_lanes = ok;
+  cudaGetLastError();
+}
+static void destroy_lanes(StepStreams& S) {
+  for (int l = 0; l < LANE_COUNT; ++l) {
+    if (S.forked[l]) cudaEventDestroy(S.forked[l]);
+    if (S.joined[l]) cudaEventDestroy(S.joined[l]);
+    if (S.side[l]) cudaStreamDestroy(S.side[l]);
+  }
 }
 
 extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float* grads, float* opt0, float* opt1, srl_learner_t** out) {
@@ -315,31 +354,15 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
   WsRow t[WS_MAX_ROWS];
   const int n = workspace_table(L, t);
   const bool split = cfg->precision == 1;
-  int64_t total = 0;
-  for (int i = 0; i < n; ++i) total += ws_bytes(t[i]) * (split && t[i].lo ? 2 : 1);
+  const int64_t total = rows_bytes(t, n, split);
   cudaError_t e = cudaMalloc(&L->arena, total);
   if (e != cudaSuccess) return undo(cuda_fail(e, "learner_create: cudaMalloc workspace"));
   e = cudaMemset(L->arena, 0, total);
   if (e != cudaSuccess) return undo(cuda_fail(e, "learner_create: cudaMemset"));
   L->arena_bytes = total;
-  char* q = L->arena;
-  for (int i = 0; i < n; ++i) {
-    if (t[i].hi) *t[i].hi = q;
-    q += ws_bytes(t[i]);
-    if (split && t[i].lo) { *t[i].lo = q; q += ws_bytes(t[i]); }
-  }
+  carve_rows(t, n, split, L->arena);
   L->buf.NF = (int)NF;
-  {     // the lanes: without them every call runs collapsed on the caller's stream
-    StepStreams& S = L->S;
-    int lo = 0, hi = 0;       // (numerically lowest = greatest priority)
-    bool ok = cudaDeviceGetStreamPriorityRange(&lo, &hi) == cudaSuccess;
-    for (int l = 0; l < LANE_COUNT && ok; ++l)        // the wgrad lanes take the default priority (0, the least)
-      ok = cudaStreamCreateWithPriority(&S.side[l], cudaStreamNonBlocking, l == LANE_PACK ? pack_priority(lo, hi) : 0) == cudaSuccess &&
-           cudaEventCreateWithFlags(&S.forked[l], cudaEventDisableTiming) == cudaSuccess &&
-           cudaEventCreateWithFlags(&S.joined[l], cudaEventDisableTiming) == cudaSuccess;
-    S.have_lanes = ok;
-    cudaGetLastError();
-  }
+  create_lanes(L->S);
   const char* why = nullptr;
   if (build_tma_maps(L->buf, (int)NF, (int)NB, &L->maps, &why) != cudaSuccess)
     return undo(fail(SRL_ESTATE, "learner_create: building TMA tensor map '%s' failed (driver without cuTensorMapEncodeTiled?)", why ? why : "?"));
@@ -359,11 +382,7 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
 extern "C" int srl_learner_destroy(srl_learner_t* L) {
   if (!L) return 0;
   for (int i = 0; i < 2 * PS_COUNT; ++i) if (L->S.slot_events[i]) cudaEventDestroy(L->S.slot_events[i]);
-  for (int l = 0; l < LANE_COUNT; ++l) {
-    if (L->S.forked[l]) cudaEventDestroy(L->S.forked[l]);
-    if (L->S.joined[l]) cudaEventDestroy(L->S.joined[l]);
-    if (L->S.side[l]) cudaStreamDestroy(L->S.side[l]);
-  }
+  destroy_lanes(L->S);
   if (L->lstm) srl_lstm_destroy(L->lstm);
   lstm_step_destroy(L->lstm_step);
   cudaFree(L->arena);
@@ -606,10 +625,11 @@ extern "C" int srl_learner_forward_lstm(srl_learner_t* L, const uint8_t* obs, co
   return forward_lstm_impl(L, obs, reward, done, action, h0, c0, policy_logits, baseline, hT, cT);
 }
 
-static bool overlaps(const void* a, const void* b, int64_t bytes) {
+static bool overlaps(const void* a, int64_t a_bytes, const void* b, int64_t b_bytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
-  return x < y + (uintptr_t)bytes && y < x + (uintptr_t)bytes;
+  return x < y + (uintptr_t)b_bytes && y < x + (uintptr_t)a_bytes;
 }
+static bool overlaps(const void* a, const void* b, int64_t bytes) { return overlaps(a, bytes, b, bytes); }
 
 extern "C" int srl_learner_forward_lstm_step(srl_learner_t* L, const uint8_t* obs, const float* reward, const uint8_t* done,
                                              const int64_t* action, const float* h_in, const float* c_in, float* policy_logits,
@@ -780,4 +800,163 @@ extern "C" int srl_learner_debug_buffer(srl_learner_t* L, const char* name, void
     }
   }
   return fail(SRL_EINVAL, "debug_buffer: unknown buffer '%s'", name);
+}
+
+// ------------------------------------------------------------------------------------------------
+// stand-alone encoder: the learner's encoder kernels on caller-owned blocks, one forward and its backward per autograd call
+// ------------------------------------------------------------------------------------------------
+struct srl_encoder {
+  int precision;
+  StepStreams S;                  // the lanes beside the caller's stream (no per-kernel profiling)
+};
+
+constexpr int ENC_MAX_FRAMES = 65536;
+
+static int check_precision(int precision, const char* what) {
+  REQ(precision == 0 || precision == 1, "%s: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", what, precision);
+  return 0;
+}
+
+extern "C" int srl_encoder_create(int precision, srl_encoder_t** out) {
+  REQ(out, "encoder_create: NULL argument");
+  int rc = check_precision(precision, "encoder_create");
+  if (rc) return rc;
+  srl_encoder* E = new (std::nothrow) srl_encoder();
+  REQ(E, "out of host memory");
+  E->precision = precision;
+  create_lanes(E->S);
+  *out = E;
+  return 0;
+}
+
+extern "C" int srl_encoder_destroy(srl_encoder_t* E) {
+  if (!E) return 0;
+  destroy_lanes(E->S);
+  delete E;
+  return 0;
+}
+
+extern "C" int srl_encoder_sizes(int frames, int precision, int64_t* saved_bytes, int64_t* scratch_bytes) {
+  REQ(saved_bytes && scratch_bytes, "encoder_sizes: NULL argument");
+  REQ(frames >= 1 && frames <= ENC_MAX_FRAMES, "encoder_sizes: frames=%d must be in [1, %d]", frames, ENC_MAX_FRAMES);
+  int rc = check_precision(precision, "encoder_sizes");
+  if (rc) return rc;
+  EncoderBuffers b = {};
+  WsRow t[ENC_ROWS];
+  encoder_rows(b, frames, frames, t);
+  *saved_bytes = rows_bytes(t, ENC_SAVED_ROWS, precision == 1);
+  *scratch_bytes = rows_bytes(t + ENC_SAVED_ROWS, ENC_ROWS - ENC_SAVED_ROWS, precision == 1);
+  return 0;
+}
+
+static bool misaligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
+
+// the argument checks both calls share: shape, the two blocks' alignment, and that neither block overlaps the other
+static int check_encoder_call(const srl_encoder* E, int frames, int A, const void* saved, const void* scratch, int64_t* sb, int64_t* kb,
+                              const char* what) {
+  REQ(frames >= 1 && frames <= ENC_MAX_FRAMES, "%s: frames=%d must be in [1, %d]", what, frames, ENC_MAX_FRAMES);
+  REQ(A >= 1 && A <= 31, "%s: A=%d must be in [1,31]", what, A);
+  REQ(!misaligned(saved, 256) && !misaligned(scratch, 256), "%s: saved and scratch must be 256-byte aligned", what);
+  srl_encoder_sizes(frames, E->precision, sb, kb);
+  REQ(!overlaps(saved, *sb, scratch, *kb), "%s: saved and scratch overlap", what);
+  return 0;
+}
+
+// the blocks of one call -> the encoder buffers and their tensor maps, encoded on the host for this call (legal under stream capture)
+static int encoder_call_setup(const srl_encoder* E, int frames, void* saved, void* scratch, EncoderBuffers* b, TmaMaps* maps,
+                              const char* what) {
+  const bool split = E->precision == 1;
+  WsRow t[ENC_ROWS];
+  *b = EncoderBuffers{};
+  encoder_rows(*b, frames, frames, t);
+  carve_rows(t, ENC_SAVED_ROWS, split, static_cast<char*>(saved));
+  carve_rows(t + ENC_SAVED_ROWS, ENC_ROWS - ENC_SAVED_ROWS, split, static_cast<char*>(scratch));
+  b->NF = frames;
+  // encoding needs the device's context current on this thread, and this may be the thread's first CUDA call (torch runs a backward
+  // on an autograd thread of its own): cudaSetDevice makes the primary context current
+  int dev = 0;
+  CU(cudaGetDevice(&dev), "cudaGetDevice");
+  CU(cudaSetDevice(dev), "cudaSetDevice");
+  const char* why = nullptr;
+  if (build_tma_maps(*b, frames, frames, maps, &why) != cudaSuccess)
+    return fail(SRL_ESTATE, "%s: building TMA tensor map '%s' failed (driver without cuTensorMapEncodeTiled?)", what, why ? why : "?");
+  return 0;
+}
+
+extern "C" int srl_encoder_forward(srl_encoder_t* E, const uint8_t* obs, const float* reward, const int64_t* action, int frames, int A,
+                                   const float* const* weights8, void* saved, void* scratch, float* core_out, void* stream) {
+  REQ(E && obs && reward && action && weights8 && saved && scratch && core_out, "encoder_forward: NULL pointer");
+  for (int i = 0; i < 8; ++i) REQ(weights8[i], "encoder_forward: weights8[%d] is NULL", i);
+  int64_t sb = 0, kb = 0;
+  int rc = check_encoder_call(E, frames, A, saved, scratch, &sb, &kb, "encoder_forward");
+  if (rc) return rc;
+  REQ(!misaligned(obs, 4), "encoder_forward: obs must be 4-byte aligned");
+  int64_t cnt[12];
+  layout(A, nullptr, cnt);
+  const int64_t core_bytes = (int64_t)frames * (513 + A) * 4;
+  for (int i = 0; i < 8; ++i) {
+    REQ(!misaligned(weights8[i], 16), "encoder_forward: weights8[%d] must be 16-byte aligned", i);
+    REQ(!overlaps(weights8[i], cnt[i] * 4, saved, sb) && !overlaps(weights8[i], cnt[i] * 4, scratch, kb) &&
+        !overlaps(weights8[i], cnt[i] * 4, core_out, core_bytes), "encoder_forward: weights8[%d] overlaps an output", i);
+  }
+  const void* in[3] = {obs, reward, action};
+  const int64_t in_bytes[3] = {(int64_t)frames * 28224, (int64_t)frames * 4, (int64_t)frames * 8};
+  for (int i = 0; i < 3; ++i)
+    REQ(!overlaps(in[i], in_bytes[i], saved, sb) && !overlaps(in[i], in_bytes[i], scratch, kb) && !overlaps(in[i], in_bytes[i], core_out, core_bytes),
+        "encoder_forward: an output overlaps obs, reward or action");
+  REQ(!overlaps(core_out, core_bytes, saved, sb) && !overlaps(core_out, core_bytes, scratch, kb), "encoder_forward: core_out overlaps saved or scratch");
+  ParamPtrs P = {};
+  P.w1 = const_cast<float*>(weights8[0]); P.b1 = const_cast<float*>(weights8[1]); P.w2 = const_cast<float*>(weights8[2]);
+  P.b2 = const_cast<float*>(weights8[3]); P.w3 = const_cast<float*>(weights8[4]); P.b3 = const_cast<float*>(weights8[5]);
+  P.wf = const_cast<float*>(weights8[6]); P.bf = const_cast<float*>(weights8[7]);
+  EncoderBuffers b;
+  TmaMaps maps;
+  rc = encoder_call_setup(E, frames, saved, scratch, &b, &maps, "encoder_forward");
+  if (rc) return rc;
+  StepStreams& S = E->S;
+  const cudaStream_t st = S.begin_call((cudaStream_t)stream);
+  // as the learner's forward: the weights are packed into `saved` on the pack lane under the frame conversion (which writes conv1's copy)
+  CU(S.fork(LANE_PACK), "fork pack");
+  CU(launch_pack_weights(P, b.hi.wpack, S.lane(LANE_PACK), b.lo.wpack, true), "pack_weights");
+  CU(encoder_forward(obs, frames, P, b, maps, E->precision, S, false), "encoder_forward");
+  CU(launch_core_build(b.hpart, FC_SPLITS, P.bf, reward, action, frames, A, b.h, core_out, st), "core_build");
+  return 0;
+}
+
+extern "C" int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int frames, int A, void* saved, void* scratch, float* const* grads8,
+                                    void* stream) {
+  REQ(E && dcore && saved && scratch && grads8, "encoder_backward: NULL pointer");
+  for (int i = 0; i < 8; ++i) REQ(grads8[i], "encoder_backward: grads8[%d] is NULL", i);
+  int64_t sb = 0, kb = 0;
+  int rc = check_encoder_call(E, frames, A, saved, scratch, &sb, &kb, "encoder_backward");
+  if (rc) return rc;
+  int64_t cnt[12];
+  layout(A, nullptr, cnt);
+  const int64_t dcore_bytes = (int64_t)frames * (513 + A) * 4;
+  REQ(!overlaps(dcore, dcore_bytes, scratch, kb), "encoder_backward: dcore overlaps scratch");
+  for (int i = 0; i < 8; ++i) {
+    REQ(!misaligned(grads8[i], 16), "encoder_backward: grads8[%d] must be 16-byte aligned", i);
+    const int64_t gb = cnt[i] * 4;
+    REQ(!overlaps(grads8[i], gb, saved, sb) && !overlaps(grads8[i], gb, scratch, kb) && !overlaps(grads8[i], gb, dcore, dcore_bytes),
+        "encoder_backward: grads8[%d] overlaps dcore, saved or scratch", i);
+    for (int j = 0; j < i; ++j) REQ(!overlaps(grads8[i], gb, grads8[j], cnt[j] * 4), "encoder_backward: grads8[%d] overlaps grads8[%d]", i, j);
+  }
+  ParamPtrs G = {};
+  G.w1 = grads8[0]; G.b1 = grads8[1]; G.w2 = grads8[2]; G.b2 = grads8[3]; G.w3 = grads8[4]; G.b3 = grads8[5]; G.wf = grads8[6]; G.bf = grads8[7];
+  EncoderBuffers b;
+  TmaMaps maps;
+  rc = encoder_call_setup(E, frames, saved, scratch, &b, &maps, "encoder_backward");
+  if (rc) return rc;
+  StepStreams& S = E->S;
+  const cudaStream_t st = S.begin_call((cudaStream_t)stream);
+  // the zeros of the gradient grids are the padding of the transposed convolutions: da3 .. da1, low twins included, lie between
+  // hi.da3 and wgrad_part (encoder_rows)
+  CU(cudaMemsetAsync(b.hi.da3, 0, reinterpret_cast<char*>(b.wgrad_part) - reinterpret_cast<char*>(b.hi.da3), st), "clear gradient grids");
+  // the conv bias sums are added into their gradients; every other gradient is stored
+  CU(cudaMemsetAsync(G.b1, 0, cnt[1] * 4, st), "zero conv1 bias grad");
+  CU(cudaMemsetAsync(G.b2, 0, cnt[3] * 4, st), "zero conv2 bias grad");
+  CU(cudaMemsetAsync(G.b3, 0, cnt[5] * 4, st), "zero conv3 bias grad");
+  CU(launch_dcore_to_dh(dcore, b.h, frames, A, b.hi.dh, st, b.lo.dh), "dcore_to_dh");
+  CU(encoder_backward(frames, b, G, maps, E->precision, S, BWD_BOTH, false), "encoder_backward");
+  return 0;
 }

@@ -215,13 +215,16 @@ __global__ void __launch_bounds__(128) head_dense_bwd_kernel(const float* __rest
     if (a < A) { if (j < H) atomicAdd(gWp + (size_t)a * H + j, acc[a]); else atomicAdd(gbp + a, acc[a]); }
   if (j < H) atomicAdd(gWb + j, acc[HEAD_MAX_A]); else atomicAdd(gbb, acc[HEAD_MAX_A]);
 }
-// dh[n][j] = bf16(dcore[n][j] * (h[n][j] > 0)), j < 512 (the reward / one-hot columns of core have no parameters below them)
+// dh[n][j] = bf16(dcore[n][j] * (h[n][j] > 0)), j < 512 (the reward / one-hot columns of core have no parameters below them);
+// dh_lo (when not null) = the low twin bf16(v - bf16(v)) of the fp32-accurate operand mode
 __global__ void __launch_bounds__(128) dcore_to_dh_kernel(const float* __restrict__ dcore, const float* __restrict__ h, int A,
-                                                          __nv_bfloat16* __restrict__ dh) {
+                                                          __nv_bfloat16* __restrict__ dh, __nv_bfloat16* __restrict__ dh_lo) {
   const int n = blockIdx.x, H = 513 + A;
   for (int j = threadIdx.x; j < 512; j += 128) {
     const float v = __ldg(h + (size_t)n * 512 + j) > 0.f ? __ldg(dcore + (size_t)n * H + j) : 0.f;
-    dh[(size_t)n * 512 + j] = __float2bfloat16_rn(v);
+    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+    dh[(size_t)n * 512 + j] = hi;
+    if (dh_lo) dh_lo[(size_t)n * 512 + j] = __float2bfloat16_rn(v - __bfloat162float(hi));
   }
 }
 
@@ -241,8 +244,8 @@ cudaError_t launch_head_dense_bwd(const float* X, const float* dlogits, const fl
   head_dense_bwd_kernel<<<dim3((H + 1 + 127) / 128, (N + 15) / 16), 128, 0, st>>>(X, dlogits, dbaseline, Wp, Wb, N, A, dX, gWp, gbp, gWb, gbb);
   return cudaGetLastError();
 }
-cudaError_t launch_dcore_to_dh(const float* dcore, const float* h, int N, int A, __nv_bfloat16* dh, cudaStream_t st) {
-  dcore_to_dh_kernel<<<N, 128, 0, st>>>(dcore, h, A, dh);
+cudaError_t launch_dcore_to_dh(const float* dcore, const float* h, int N, int A, __nv_bfloat16* dh, cudaStream_t st, __nv_bfloat16* dh_lo) {
+  dcore_to_dh_kernel<<<N, 128, 0, st>>>(dcore, h, A, dh, dh_lo);
   return cudaGetLastError();
 }
 

@@ -130,7 +130,8 @@ cudaError_t launch_head_dense_fwd(const float* X, const float* Wp, const float* 
                                   float* baseline, cudaStream_t st);
 cudaError_t launch_head_dense_bwd(const float* X, const float* dlogits, const float* dbaseline, const float* Wp, const float* Wb, int N, int A,
                                   float* dX, float* gWp, float* gbp, float* gWb, float* gbb, cudaStream_t st);
-cudaError_t launch_dcore_to_dh(const float* dcore, const float* h, int N, int A, __nv_bfloat16* dh, cudaStream_t st);
+// dh_lo != nullptr: also the low twin bf16(v - bf16(v)) of the fp32-accurate operand mode
+cudaError_t launch_dcore_to_dh(const float* dcore, const float* h, int N, int A, __nv_bfloat16* dh, cudaStream_t st, __nv_bfloat16* dh_lo = nullptr);
 cudaError_t launch_unpack_slots(const uint8_t* staging, int64_t slot_bytes, const int64_t* off6, int T, int B, int A, uint8_t* obs, float* reward,
                                 uint8_t* done, int64_t* action, float* logits, float* episode_return, cudaStream_t st);
 

@@ -1,0 +1,121 @@
+"""CPU: the trainable AtariNet drop-in (scalerl_b200.algorithms.utils.atari_model.AtariNet) -- the reference's parameters and
+initialisation, its constructor and input errors, and the stand-alone encoder entry points' argument checks (no GPU needed)."""
+import ctypes as C
+
+import pytest
+import torch
+
+from oracle import ref_learner
+from scalerl_b200 import _lib, build as srl_build
+from scalerl_b200.algorithms.utils.atari_model import AtariNet
+
+
+@pytest.mark.skipif(not ref_learner.available(), reason='oracle/_ref (the reference modules) is not built')
+@pytest.mark.parametrize('use_lstm', [False, True])
+@pytest.mark.parametrize('A', [4, 6, 18])
+def test_state_dict_and_init_match_the_reference(A, use_lstm):
+    am = ref_learner._load('atari_model')
+    torch.manual_seed(11)
+    ref = am.AtariNet((4, 84, 84), A, use_lstm=use_lstm)
+    torch.manual_seed(11)
+    mine = AtariNet((4, 84, 84), A, use_lstm=use_lstm)
+    rs, ms = ref.state_dict(), mine.state_dict()
+    assert list(rs) == list(ms)
+    for k in rs:
+        assert rs[k].shape == ms[k].shape, k
+        assert torch.equal(rs[k], ms[k]), k
+    assert [n for n, _ in ref.named_parameters()] == [n for n, _ in mine.named_parameters()]
+
+
+@pytest.mark.parametrize('kw', [dict(observation_shape=(3, 84, 84), num_actions=6), dict(observation_shape=(4, 84, 84), num_actions=0),
+                                dict(observation_shape=(4, 84, 84), num_actions=32),
+                                dict(observation_shape=(4, 84, 84), num_actions=6, precision='fp16')])
+def test_constructor_errors(kw):
+    with pytest.raises(ValueError):
+        AtariNet(**kw)
+
+
+def test_deepcopy_and_optimizer_work_as_on_any_module():
+    import copy
+    net = AtariNet((4, 84, 84), 6, use_lstm=True)
+    twin = copy.deepcopy(net)
+    assert twin._contexts is not net._contexts and twin._contexts.handles == {}
+    for (n, p), (m, q) in zip(net.named_parameters(), twin.named_parameters()):
+        assert n == m and torch.equal(p, q) and p.data_ptr() != q.data_ptr()
+    torch.optim.RMSprop(net.parameters(), lr=1e-4)
+    net.zero_grad(set_to_none=True)
+
+
+def test_forward_on_cpu_tensors_raises():
+    net = AtariNet((4, 84, 84), 6)
+    T, B = 2, 3
+    inputs = dict(obs=torch.zeros(T, B, 4, 84, 84, dtype=torch.uint8), reward=torch.zeros(T, B), action=torch.zeros(T, B, dtype=torch.int64),
+                  done=torch.zeros(T, B, dtype=torch.bool))
+    with pytest.raises(ValueError, match='CUDA'):
+        net(inputs)
+
+
+@pytest.fixture(scope='module')
+def lib():
+    srl_build.build()
+    return _lib.lib()
+
+
+def _err(L):
+    return L.srl_last_error().decode()
+
+
+def test_size_query_argument_errors(lib):
+    L = lib
+    s, k = C.c_int64(), C.c_int64()
+    for frames, prec in ((0, 0), (65537, 0), (8, 2)):
+        assert L.srl_encoder_sizes(frames, prec, C.byref(s), C.byref(k)) == -1
+    assert L.srl_encoder_sizes(8, 0, None, C.byref(k)) == -1 and 'NULL' in _err(L)
+    assert L.srl_encoder_sizes(672, 0, C.byref(s), C.byref(k)) == 0
+    # the forward keeps xs, a1, a2, a3, h and the packed weights: about 74 MB at T+1 = 21, B = 32 in the bf16 mode
+    assert 74.0e6 < s.value < 75.0e6
+    s1 = C.c_int64()
+    assert L.srl_encoder_sizes(672, 1, C.byref(s1), C.byref(k)) == 0 and s1.value > s.value      # + the low twins
+
+
+def test_entry_points_reject_bad_arguments_before_any_cuda_call(lib):
+    L = lib
+    h = C.c_void_p()
+    assert L.srl_encoder_create(2, C.byref(h)) == -1 and 'precision' in _err(L)
+    assert L.srl_encoder_create(0, None) == -1
+    assert L.srl_encoder_forward(None, None, None, None, 8, 6, None, None, None, None, None) == -1 and 'NULL' in _err(L)
+    assert L.srl_encoder_backward(None, None, 8, 6, None, None, None, None) == -1 and 'NULL' in _err(L)
+    assert L.srl_encoder_create(0, C.byref(h)) == 0          # lanes are optional: no device needed to hold a context
+    try:
+        frames, A = 8, 6
+        base = 1 << 40                                        # fake device addresses, far apart and 256-byte aligned
+        at = lambda i: base + (i << 32)
+        obs, reward, action, saved, scratch, core = at(0), at(1), at(2), at(3), at(4), at(5)
+        w = (C.c_void_p * 8)(*[at(10 + i) for i in range(8)])
+
+        def fwd(**kw):
+            a = dict(obs=obs, reward=reward, action=action, frames=frames, A=A, w=w, saved=saved, scratch=scratch, core=core)
+            a.update(kw)
+            return L.srl_encoder_forward(h, a['obs'], a['reward'], a['action'], a['frames'], a['A'], a['w'], a['saved'], a['scratch'],
+                                         a['core'], None)
+
+        assert fwd(frames=0) == -1 and 'frames' in _err(L)
+        assert fwd(frames=65537) == -1 and 'frames' in _err(L)
+        assert fwd(A=32) == -1 and 'A=32' in _err(L)
+        assert fwd(saved=saved + 16) == -1 and 'aligned' in _err(L)
+        assert fwd(obs=obs + 1) == -1 and 'aligned' in _err(L)
+        assert fwd(scratch=saved + 256) == -1 and 'overlap' in _err(L)
+        assert fwd(core=obs) == -1 and 'overlap' in _err(L)
+        assert fwd(core=at(16)) == -1 and 'overlap' in _err(L)                    # core_out on fc.weight
+        assert fwd(w=(C.c_void_p * 8)(*([at(10)] + [None] * 7))) == -1 and 'NULL' in _err(L)
+        assert fwd(w=(C.c_void_p * 8)(*([at(10) + 4] + [at(11 + i) for i in range(7)]))) == -1 and 'aligned' in _err(L)
+        g = (C.c_void_p * 8)(*[at(20 + i) for i in range(8)])
+        dcore = at(6)
+        assert L.srl_encoder_backward(h, dcore, 0, A, saved, scratch, g, None) == -1 and 'frames' in _err(L)
+        assert L.srl_encoder_backward(h, dcore, frames, A, saved, saved, g, None) == -1 and 'overlap' in _err(L)
+        assert L.srl_encoder_backward(h, dcore, frames, A, saved, scratch, (C.c_void_p * 8)(*([saved] + list(g)[1:])), None) == -1
+        assert 'overlap' in _err(L)
+        assert L.srl_encoder_backward(h, dcore, frames, A, saved, scratch, (C.c_void_p * 8)(*([at(20)] * 8)), None) == -1
+        assert 'overlap' in _err(L)
+    finally:
+        assert L.srl_encoder_destroy(h) == 0
