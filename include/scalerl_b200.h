@@ -281,7 +281,9 @@ int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int frames, int A
  * weights8 / grads8: 8 device pointers in nn.LSTM state_dict order {weight_ih_l0 [4H,H], weight_hh_l0 [4H,H], bias_ih_l0 [4H],
  * bias_hh_l0 [4H], *_l1 ...} (fp32, caller-owned); gradients are ACCUMULATED into grads8 (zero them before the step).
  * forward : core f32 [T1,B,H], done u8 [T1,B], h0/c0 f32 [2,B,H] -> out f32 [T1,B,H], hT/cT f32 [2,B,H] (may be NULL)
- * backward: dout f32 [T1-1,B,H] (steps 0..T-1; the bootstrap row T carries no gradient) -> dcore f32 [T1-1,B,H] */
+ * backward: dout f32 [T1-1,B,H] (rows 0..T1-2 only: the learner's bootstrap row T1-1 carries no gradient) -> dcore f32 [T1-1,B,H].
+ *           The bias gradients are reduced without atomics (fixed 64-row chunks added in order): the same bits on every run.
+ * Errors of these calls and of srl_lstm_core_* are reported by srl_lstm_last_error. */
 typedef struct srl_lstm srl_lstm_t;
 int srl_lstm_create(int T1, int B, int H, const float* const* weights8, float* const* grads8, srl_lstm_t** out);
 int srl_lstm_destroy(srl_lstm_t* L);
@@ -289,6 +291,23 @@ int srl_lstm_forward(srl_lstm_t* L, const float* core, const uint8_t* done, cons
                      float* hT, float* cT, void* stream);
 int srl_lstm_backward(srl_lstm_t* L, const float* dout, const uint8_t* done, float* dcore, void* stream);
 const char* srl_lstm_last_error(void);
+
+/* ---- stand-alone LSTM core: the trainable AtariNet's use_lstm=True core under autograd ---------------------------------------
+ * The same kernels as srl_lstm_*, on two caller-owned blocks as srl_encoder_*: `saved` is written by the forward and read by its
+ * backward (layer inputs, m.h, h, gate activations, cell states, the packed weights the forward ran with, copies of done and of the
+ * padded initial cell state); `scratch` holds one call's temporaries.  No context: tensor maps are encoded on the host per call
+ * (legal under stream capture) on the current device.  H = 513 + A, A in [1, 31], 1 <= T1*B <= 65536 (T1 = 1 is one step).
+ * Both blocks are 256-byte aligned, need no initialisation, and no output may overlap another argument.  Everything runs on `stream`.
+ * forward : core f32 [T1,B,H], done u8 [T1,B], h0/c0 f32 [2,B,H], weights8 (srl_lstm_create order) -> out f32 [T1,B,H],
+ *           hT/cT f32 [2,B,H] (the state after row T1-1).
+ * backward: dout f32 [T1,B,H] (every row, the last included), dhT/dcT f32 [2,B,H] (gradients of hT/cT; NULL = zero)
+ *           -> grads8 (the 8 tensors' gradients, OVERWRITTEN), dcore f32 [T1,B,H], dh0/dc0 f32 [2,B,H] (gradients of h0/c0; NULL = not
+ *           wanted, which skips their extra GEMM). */
+int srl_lstm_core_sizes(int T1, int B, int A, int64_t* saved_bytes, int64_t* scratch_bytes);
+int srl_lstm_core_forward(const float* core, const uint8_t* done, const float* h0, const float* c0, int A, int T1, int B,
+                          const float* const* weights8, void* saved, void* scratch, float* out, float* hT, float* cT, void* stream);
+int srl_lstm_core_backward(const float* dout, const float* dhT, const float* dcT, int A, int T1, int B, void* saved, void* scratch,
+                           float* const* grads8, float* dcore, float* dh0, float* dc0, void* stream);
 
 /* ---- prioritized-replay sampler (BASELINE.json configs[3]; SURVEY.md §8f) ---------------------------------------------------
  * Device-resident float64 sum/min segment trees; replaces PrioritizedReplayBuffer's tree arithmetic

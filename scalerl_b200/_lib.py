@@ -63,6 +63,9 @@ _SIGS = {
     'srl_lstm_destroy': [_P],
     'srl_lstm_forward': [_P, _P, _P, _P, _P, _P, _P, _P, _P],
     'srl_lstm_backward': [_P, _P, _P, _P, _P],
+    'srl_lstm_core_sizes': [_I, _I, _I, C.POINTER(_L), C.POINTER(_L)],
+    'srl_lstm_core_forward': [_P, _P, _P, _P, _I, _I, _I, C.POINTER(_P), _P, _P, _P, _P, _P, _P],
+    'srl_lstm_core_backward': [_P, _P, _P, _I, _I, _I, _P, _P, C.POINTER(_P), _P, _P, _P, _P],
     'srl_per_create': [_L, C.c_double, C.POINTER(_P)],
     'srl_per_destroy': [_P],
     'srl_per_add': [_P, _L, _P],

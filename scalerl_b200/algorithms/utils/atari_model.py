@@ -10,8 +10,8 @@ layouts -- so ImpalaTrainer treats it and the reference's own ``AtariNet`` ident
 ``SyntheticAtariEnv`` emits the TorchEnvWrapper record schema (scalerl/envs/torch_envwrapper.py:43-50,77-84)
 with random frames; it exists so the actor/ring/learner plumbing can be exercised without gymnasium/ale_py.
 ``AtariNet`` is the trainable drop-in for the reference's ``AtariNet`` (atari_model.py:8-143): the same submodules, parameters
-and calling convention, with the encoder (obs -> conv1..3 -> fc -> [h, clipped reward, one-hot last action]) and its backward on
-the learner's sm_90a kernels under torch autograd.
+and calling convention, with the encoder (obs -> conv1..3 -> fc -> [h, clipped reward, one-hot last action]), the 2-layer LSTM core
+(use_lstm=True, bf16) and their backward on the learner's sm_90a kernels under torch autograd.
 """
 import ctypes as C
 from collections import OrderedDict
@@ -138,6 +138,7 @@ class ActorNet(torch.nn.Module):
 PRECISIONS = {'bf16': 0, 'fp32_split': 1}     # ImpalaHParams.precision -> srl_config_t.precision
 MAX_ACTIONS = 31                             # one warp lane per action plus one for the baseline, as B200ImpalaLearner
 MAX_FRAMES = 65536                           # T * B of one call
+LSTM_WEIGHTS = tuple(f'{w}_l{l}' for l in (0, 1) for w in ('weight_ih', 'weight_hh', 'bias_ih', 'bias_hh'))   # srl_lstm_create order
 
 
 class _EncoderContexts:
@@ -228,14 +229,83 @@ class _EncoderCore(torch.autograd.Function):
         return (None,) * 6 + tuple(grads)
 
 
+def _lstm_check(rc, what):
+    if rc != 0:
+        msg = _lib.lib().srl_lstm_last_error().decode()
+        raise (ValueError if rc == -1 else RuntimeError)(f'{what}: {msg}')
+
+
+def lstm_block_sizes(T1: int, B: int, num_actions: int):
+    """(bytes an LSTM core forward keeps for its backward, bytes of one call's scratch) for T1 x B rows"""
+    saved, scratch = C.c_int64(), C.c_int64()
+    _lstm_check(_lib.lib().srl_lstm_core_sizes(int(T1), int(B), int(num_actions), C.byref(saved), C.byref(scratch)), 'srl_lstm_core_sizes')
+    return saved.value, scratch.value
+
+
+def _lstm_forward(num_actions, core, done, h0, c0, weights):
+    """-> (out [T1,B,H], hT, cT [2,B,H], the forward's saved block); core f32 [T1,B,H], done u8 [T1,B], all contiguous on one device"""
+    T1, B, H = core.shape
+    dev = core.device
+    saved_bytes, scratch_bytes = lstm_block_sizes(T1, B, num_actions)
+    saved = torch.empty(saved_bytes, dtype=torch.uint8, device=dev)
+    scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev)
+    out = torch.empty(T1, B, H, dtype=torch.float32, device=dev)
+    hT, cT = (torch.empty(2, B, H, dtype=torch.float32, device=dev) for _ in range(2))
+    _lstm_check(_lib.lib().srl_lstm_core_forward(core.data_ptr(), done.data_ptr(), h0.data_ptr(), c0.data_ptr(), num_actions, T1, B,
+                                                 _ptrs8(weights), saved.data_ptr(), scratch.data_ptr(), out.data_ptr(), hT.data_ptr(),
+                                                 cT.data_ptr(), torch.cuda.current_stream(dev).cuda_stream), 'srl_lstm_core_forward')
+    return out, hT, cT, saved
+
+
+def _ptr_or_none(t):
+    return None if t is None else t.data_ptr()
+
+
+class _LstmCore(torch.autograd.Function):
+    """(out, hT, cT) of the 2-layer LSTM over T1 steps with the state reset where done (atari_model.py:109-120), differentiable in the
+    core, the initial state (h0, c0) and the 8 nn.LSTM tensors.  As _EncoderCore, the forward's activations and packed weights are one
+    block saved on ``ctx``.  Unused gradients of hT / cT reach the kernels as NULL (no materialised zeros)."""
+
+    @staticmethod
+    def forward(ctx, num_actions, core, done, h0, c0, *weights):
+        out, hT, cT, saved = _lstm_forward(num_actions, core, done, h0, c0, weights)
+        ctx.save_for_backward(saved)
+        ctx.call = (num_actions, tuple(core.shape), [w.shape for w in weights])
+        ctx.set_materialize_grads(False)
+        return out, hT, cT
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout, dhT, dcT):
+        num_actions, (T1, B, H), shapes = ctx.call
+        (saved,) = ctx.saved_tensors
+        dev = saved.device
+        dout = torch.zeros(T1, B, H, device=dev) if dout is None else dout.contiguous()
+        dhT = None if dhT is None else dhT.contiguous()
+        dcT = None if dcT is None else dcT.contiguous()
+        want_h0, want_c0 = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
+        dcore = torch.empty(T1, B, H, device=dev)
+        dh0 = torch.empty(2, B, H, device=dev) if want_h0 else None
+        dc0 = torch.empty(2, B, H, device=dev) if want_c0 else None
+        grads = [torch.empty(s, dtype=torch.float32, device=dev) for s in shapes]
+        scratch = torch.empty(lstm_block_sizes(T1, B, num_actions)[1], dtype=torch.uint8, device=dev)
+        _lstm_check(_lib.lib().srl_lstm_core_backward(dout.data_ptr(), _ptr_or_none(dhT), _ptr_or_none(dcT), num_actions, T1, B, saved.data_ptr(),
+                                                      scratch.data_ptr(), _ptrs8(grads), dcore.data_ptr(), _ptr_or_none(dh0), _ptr_or_none(dc0),
+                                                      torch.cuda.current_stream(dev).cuda_stream), 'srl_lstm_core_backward')
+        return (None, dcore if ctx.needs_input_grad[1] else None, None, dh0, dc0) + tuple(grads)
+
+
 class AtariNet(nn.Module):
     """Drop-in for the reference's ``AtariNet`` (scalerl/algorithms/utils/atari_model.py:8-143) that trains on the sm_90a encoder.
 
     Submodules, their names, creation order and initialisation are the reference's, so ``state_dict()`` and the initial weights under
     ``torch.manual_seed`` match it.  ``forward(inputs, rnn_state)`` takes and returns what the reference's does; the encoder up to the
-    LSTM / head input runs as one autograd function on the learner's kernels, the LSTM loop, the heads and the action sampling are torch.
-    ``precision``: 'bf16' or 'fp32_split', as ``ImpalaHParams.precision``.  ``validate_inputs``: raise on actions outside [0, A) as
-    ``F.one_hot`` does (one host synchronisation per forward); otherwise they are clamped.  CUDA only: CPU actors use ``ActorNet``."""
+    LSTM / head input runs as one autograd function on the learner's kernels, and so does the LSTM core with ``precision='bf16'``
+    (``rnn_state`` = (h0, c0) float32 [2, B, 513 + A] on the module's device; it returns (hT, cT) as ``nn.LSTM`` does).  ``rnn_layer``
+    stays an ``nn.LSTM``: its tensors are the kernels' weights.  The heads and the action sampling are torch.
+    ``precision``: 'bf16' or 'fp32_split', as ``ImpalaHParams.precision``; 'fp32_split' steps the LSTM with ``nn.LSTM`` (the LSTM kernels
+    have bf16 operands only).  ``validate_inputs``: raise on actions outside [0, A) as ``F.one_hot`` does (one host synchronisation per
+    forward); otherwise they are clamped.  CUDA only: CPU actors use ``ActorNet``."""
 
     def __init__(self, observation_shape, num_actions, use_lstm=False, *, precision='bf16', validate_inputs=False):
         super().__init__()
@@ -306,11 +376,51 @@ class AtariNet(nn.Module):
             return _EncoderCore.apply(handle, prec, self.num_actions, obs, reward, action, *weights)
         return _encoder_forward(handle, prec, self.num_actions, obs, reward, action, weights)[0]
 
+    def _check_lstm_inputs(self, done, rnn_state, T, B):
+        H = self.rnn_layer.hidden_size
+        if not isinstance(done, torch.Tensor) or done.dtype != torch.bool or tuple(done.shape) != (T, B):
+            raise ValueError(f"inputs['done'] must be bool [{T}, {B}], got "
+                             f"{(done.dtype, tuple(done.shape)) if isinstance(done, torch.Tensor) else type(done).__name__}")
+        if not isinstance(rnn_state, (tuple, list)) or len(rnn_state) != 2:
+            raise ValueError('rnn_state must be the 2-tuple (h, c) of float32 [2, B, 513 + A] tensors (initial_hidden_state(B) on the '
+                             'module\'s device)')
+        dev = self.conv1.weight.device
+        for name, s in zip(('h', 'c'), rnn_state):
+            if not isinstance(s, torch.Tensor) or s.dtype != torch.float32 or tuple(s.shape) != (2, B, H):
+                raise ValueError(f'rnn_state {name} must be float32 [2, {B}, {H}], got '
+                                 f'{(s.dtype, tuple(s.shape)) if isinstance(s, torch.Tensor) else type(s).__name__}')
+        for name, s in zip(('h', 'c'), rnn_state):
+            if not s.is_cuda or s.device != dev:
+                raise ValueError(f"rnn_state {name} must be a CUDA tensor on the module's device {dev}, got {s.device}")
+        if not done.is_cuda or done.device != dev:
+            raise ValueError(f"inputs['done'] must be a CUDA tensor on the module's device {dev}, got {done.device}")
+
+    def _lstm_core(self, core, done, rnn_state):
+        """(out f32 [T,B,H], (hT, cT) [2,B,H]) of rnn_layer over core f32 [T,B,H] from rnn_state = (h0, c0), the state zeroed where
+        done [T,B] before a step (atari_model.py:109-120), on the sm_90a LSTM kernels; differentiable in core, h0, c0 and rnn_layer's
+        tensors.  forward checks the inputs first (_check_lstm_inputs)."""
+        weights = [getattr(self.rnn_layer, n).contiguous() for n in LSTM_WEIGHTS]
+        if any(w.dtype != torch.float32 for w in weights):
+            raise ValueError('the rnn_layer parameters must be float32')
+        h0, c0 = (s.contiguous() for s in rnn_state)
+        core, done = core.contiguous(), done.contiguous().view(torch.uint8)
+        if torch.is_grad_enabled() and any(t.requires_grad for t in [core, h0, c0, *weights]):
+            out, hT, cT = _LstmCore.apply(self.num_actions, core, done, h0, c0, *weights)
+        else:
+            out, hT, cT, _ = _lstm_forward(self.num_actions, core, done, h0, c0, weights)
+        return out, (hT, cT)
+
     def forward(self, inputs, rnn_state=()):
         """(dict(policy_logits [T,B,A], baseline [T,B], action [T,B]), rnn_state), as atari_model.py:77-143"""
         T, B = inputs['obs'].shape[:2]
+        lstm_kernels = self.use_lstm and self.precision == 'bf16'      # the LSTM kernels have bf16 operands only
+        if lstm_kernels:
+            self._check_lstm_inputs(inputs.get('done'), rnn_state, T, B)
         core = self.encode(inputs['obs'], inputs['reward'], inputs['action'])
-        if self.use_lstm:
+        if lstm_kernels:
+            core, rnn_state = self._lstm_core(core.view(T, B, -1), inputs['done'], rnn_state)
+            core = core.flatten(0, 1)
+        elif self.use_lstm:
             steps = core.view(T, B, -1).unbind()
             notdone = (~inputs['done']).float().unbind()
             outs = []

@@ -232,20 +232,9 @@ static int check_cfg(const srl_config_t* c) {
   return 0;
 }
 
-// The device workspace of a learner context, one row per tensor in carving order.  Every tensor is 256-byte aligned and zero-filled
-// at creation (the zeros of the da*g grids are the padding of the transposed convolutions).  In the fp32-accurate operand mode a row
+// The device workspace of a learner context, one row per tensor in carving order (WsRow, kernels.h).  The arena is zero-filled at
+// creation (the zeros of the da*g grids are the padding of the transposed convolutions).  In the fp32-accurate operand mode a row
 // with a low twin is followed by the twin, which srl_learner_debug_buffer calls "<name>_lo".  Rows without a name are internal.
-struct WsRow {
-  const char* name;
-  int elem;                       // bytes per element
-  int64_t count;                  // elements
-  void** hi;                      // receives the tensor's address (null: zeros only)
-  void** lo;                      // receives the low twin's address (null: no twin)
-};
-template <class T>
-static WsRow ws_row(const char* name, int64_t count, T** hi, T** lo = nullptr) {
-  return {name, (int)sizeof(T), count, reinterpret_cast<void**>(hi), reinterpret_cast<void**>(lo)};
-}
 constexpr int WS_MAX_ROWS = 32;
 // The encoder's rows, for NF forward and NB backward frames.  The first ENC_SAVED_ROWS are what a backward reads of its forward: the
 // activations and the packed weights the forward ran with.  The rest live for one call: the fc layer's split-K partials (forward),
@@ -268,21 +257,6 @@ static int encoder_rows(EncoderBuffers& b, int64_t NF, int64_t NB, WsRow* t) {
   t[n++] = ws_row("wgrad_part", WSP_TOTAL, &b.wgrad_part);
   t[n++] = ws_row("a3t", NF * 49 * 64, &b.a3t);
   return n;
-}
-static int64_t ws_bytes(const WsRow& r) { return ((int64_t)r.elem * r.count + 255) & ~int64_t(255); }
-// bytes of rows [0, n), a low twin after each row that has one in the fp32-accurate mode (split)
-static int64_t rows_bytes(const WsRow* t, int n, bool split) {
-  int64_t total = 0;
-  for (int i = 0; i < n; ++i) total += ws_bytes(t[i]) * (split && t[i].lo ? 2 : 1);
-  return total;
-}
-// gives rows [0, n) consecutive addresses from q (each row padded to 256 bytes), in table order
-static void carve_rows(const WsRow* t, int n, bool split, char* q) {
-  for (int i = 0; i < n; ++i) {
-    if (t[i].hi) *t[i].hi = q;
-    q += ws_bytes(t[i]);
-    if (split && t[i].lo) { *t[i].lo = q; q += ws_bytes(t[i]); }
-  }
 }
 static int workspace_table(srl_learner* L, WsRow* t) {
   const srl_config_t& c = L->cfg;

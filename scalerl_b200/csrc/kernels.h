@@ -80,6 +80,35 @@ struct StepStreams {
   }
 };
 
+// A device buffer table: one row per tensor in carving order, every tensor 256-byte aligned.  The learner's workspace (api.cu), the
+// stand-alone encoder's blocks (api.cu encoder_rows) and the LSTM core's (lstm.cu lstm_rows) are carved from such tables.
+struct WsRow {
+  const char* name;
+  int elem;                       // bytes per element
+  int64_t count;                  // elements
+  void** hi;                      // receives the tensor's address (null: zeros only)
+  void** lo;                      // receives the low twin's address (null: no twin)
+};
+template <class T>
+inline WsRow ws_row(const char* name, int64_t count, T** hi, T** lo = nullptr) {
+  return {name, (int)sizeof(T), count, reinterpret_cast<void**>(hi), reinterpret_cast<void**>(lo)};
+}
+inline int64_t ws_bytes(const WsRow& r) { return ((int64_t)r.elem * r.count + 255) & ~int64_t(255); }
+// bytes of rows [0, n), a low twin after each row that has one in the fp32-accurate mode (split)
+inline int64_t rows_bytes(const WsRow* t, int n, bool split) {
+  int64_t total = 0;
+  for (int i = 0; i < n; ++i) total += ws_bytes(t[i]) * (split && t[i].lo ? 2 : 1);
+  return total;
+}
+// gives rows [0, n) consecutive addresses from q (each row padded to 256 bytes), in table order
+inline void carve_rows(const WsRow* t, int n, bool split, char* q) {
+  for (int i = 0; i < n; ++i) {
+    if (t[i].hi) *t[i].hi = q;
+    q += ws_bytes(t[i]);
+    if (split && t[i].lo) { *t[i].lo = q; q += ws_bytes(t[i]); }
+  }
+}
+
 // per-CTA partials of the wgrad kernels (each CTA stores its accumulators, in the kernel's native [tap-block][row][co] order, and its
 // bias sums; conv_wgrad_reduce_kernel<layer> adds the CTAs in a fixed order into the PyTorch-layout gradient, so the gradients are the
 // same bits on every run).  Floats per CTA: accumulators, then bias.

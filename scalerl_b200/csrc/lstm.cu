@@ -1,5 +1,6 @@
-// 2-layer LSTM core of AtariNet(use_lstm=True): forward over T1 = T+1 steps with done-resets and BPTT over the first T
-// steps (reference: scalerl/algorithms/utils/atari_model.py:52-55,61-75,109-120; SURVEY.md §8 row a17).
+// 2-layer LSTM core of AtariNet(use_lstm=True): forward over T1 steps with done-resets and BPTT over the first T steps (the learner:
+// T = T1 - 1; the trainable AtariNet's stand-alone core: T = T1, with the gradients of the initial and the returned state)
+// (reference: scalerl/algorithms/utils/atari_model.py:52-55,61-75,109-120; SURVEY.md §8 row a17).
 //
 //   gates_t = x_t Wih^T + b_ih + (m_t . h_{t-1}) Whh^T + b_hh ;  i,f,g,o ;  c_t = f (m_t . c_{t-1}) + i g ;  h_t = o tanh(c_t)
 //
@@ -7,7 +8,8 @@
 //   * input projection of ALL steps in one wgmma GEMM     [T1*B x Hp] x [Hp x 4Hp]          (LGemmK)
 //   * per step: recurrent wgmma GEMM [B x Hp] x [Hp x 4Hp] + one fused cell kernel     (sequential over t)
 //   * BPTT per step: cell backward kernel + recurrent GEMM [B x 4Hp] x [4Hp x Hp]
-//   * after the scan: dX (one GEMM), dWih / dWhh (two MN-major GEMMs over all T*B rows), bias gradients (column sums)
+//   * after the scan: dX (one GEMM), dWih / dWhh (two MN-major GEMMs over all T*B rows), bias gradients (column sums over fixed
+//     64-row chunks, added in chunk order: no atomics)
 // H = 513 + A is padded to Hp (multiple of 64); the gate dimension is laid out [4][Hp] so every GEMM has K = Hp or 4Hp.
 // All GEMM operands are bf16 (fp32 accumulate); cell state, gate activations and gradients are fp32.
 // The actor's single step (one row of B environments, no BPTT) has its own fused kernel further down (lstm_step_kernel).
@@ -122,7 +124,8 @@ __global__ void lstm_cell_fwd_kernel(const float* __restrict__ gx, const float* 
   if (hm_next) hm_next[i] = __float2bfloat16_rn(done_next[b] ? 0.f : hv);
 }
 
-// BPTT cell: dh = dh_out[t] + m_{t+1} . dhm_{t+1};  writes dgates (bf16) and the carried dc
+// BPTT cell: dh = dh_out[t] + m_{t+1} . dhm_{t+1};  writes dgates (bf16) and the carried dc.  done_next == nullptr: dhm_next is added
+// unmasked (the gradient of the returned state hT, seeding the last step)
 __global__ void lstm_cell_bwd_kernel(const float* __restrict__ dh_out, const float* __restrict__ dhm_next, const uint8_t* __restrict__ done_next,
                                      const float* __restrict__ gates, const float* __restrict__ c_t, const float* __restrict__ c_prev,
                                      const uint8_t* __restrict__ done_t, float* __restrict__ dc_carry, int B, int H, int Hp,
@@ -134,7 +137,7 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ dh_out, const flo
   float dc_out = 0.f;
   if (j < H) {
     float dh = dh_out ? dh_out[i] : 0.f;
-    if (dhm_next && !done_next[b]) dh += dhm_next[i];
+    if (dhm_next && !(done_next && done_next[b])) dh += dhm_next[i];
     const float ig = gates[(size_t)b * G + j], fg = gates[(size_t)b * G + Hp + j], gg = gates[(size_t)b * G + 2 * Hp + j],
                 og = gates[(size_t)b * G + 3 * Hp + j];
     const float tc = tanhf(c_t[i]);
@@ -151,18 +154,32 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ dh_out, const flo
   for (int q = 0; q < 4; ++q) dgates[(size_t)b * G + q * Hp + j] = __float2bfloat16_rn(d[q]);
 }
 
-// db[q*H + j] += sum_rows dgates[row][q*Hp + j]
-__global__ void lstm_bias_grad_kernel(const __nv_bfloat16* __restrict__ dgates, int rows, int H, int Hp, int rows_per_block, float* __restrict__ db_ih,
-                                      float* __restrict__ db_hh) {
-  const int col = blockIdx.x * blockDim.x + threadIdx.x, G = 4 * Hp;
+// Bias gradient without atomics, the same bits on every run: part[c][col] = sum of dgates[row][col] over the fixed chunk
+// c = [64c, 64c + 64) of rows counted from row 0 (grid.y = chunk), then db[q*H + j] += sum_c part[c][q*Hp + j] in chunk order
+constexpr int LSTM_BIAS_CHUNK = 64;
+__global__ void lstm_bias_part_kernel(const __nv_bfloat16* __restrict__ dgates, int rows, int G, float* __restrict__ part) {
+  const int col = blockIdx.x * blockDim.x + threadIdx.x;
   if (col >= G) return;
-  const int q = col / Hp, j = col - q * Hp;
-  if (j >= H) return;
-  const int r0 = blockIdx.y * rows_per_block, r1 = min(rows, r0 + rows_per_block);
+  const int r0 = blockIdx.y * LSTM_BIAS_CHUNK, r1 = min(rows, r0 + LSTM_BIAS_CHUNK);
   float s = 0.f;
   for (int r = r0; r < r1; ++r) s += __bfloat162float(dgates[(size_t)r * G + col]);
-  atomicAdd(db_ih + q * H + j, s);
-  atomicAdd(db_hh + q * H + j, s);
+  part[(size_t)blockIdx.y * G + col] = s;
+}
+__global__ void lstm_bias_sum_kernel(const float* __restrict__ part, int chunks, int H, int Hp, float* __restrict__ db_ih, float* __restrict__ db_hh) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 4 * H) return;
+  const int q = i / H, col = q * Hp + (i - q * H), G = 4 * Hp;
+  float s = 0.f;
+  for (int c = 0; c < chunks; ++c) s += part[(size_t)c * G + col];
+  db_ih[i] += s;
+  db_hh[i] += s;
+}
+// dst[b][j] = done[b] ? 0 : src[b][j] for j < H: the gradient w.r.t. the initial h, which reaches the cell through m_0 . h0
+__global__ void lstm_unpad_masked_kernel(const float* __restrict__ src, const uint8_t* __restrict__ done, int B, int H, int Hp, float* __restrict__ dst) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * H) return;
+  const int b = i / H, j = i - b * H;
+  dst[i] = done[b] ? 0.f : src[(size_t)b * Hp + j];
 }
 // padded fp32 [4Hp][Hp] -> PyTorch [4H][H] (accumulate)
 __global__ void lstm_unpad_w_kernel(const float* __restrict__ src, int H, int Hp, float* __restrict__ dst) {
@@ -384,161 +401,330 @@ __global__ void lstm_step_pack_kernel(const float* __restrict__ wih0, const floa
 
 using namespace srl;
 
-// ------------------------------------------------------------------------------------------------ context
-struct srl_lstm {
-  int T1, B, H, Hp, G;
-  const float* w[2][4];      // weight_ih, weight_hh, bias_ih, bias_hh (fp32, PyTorch layouts, caller-owned)
-  float* g[2][4];            // gradients (same layouts), accumulated
-  char* arena;
-  // bf16 operands
-  __nv_bfloat16 *xin[2];     // layer input rows [T1*B][Hp]        (xin[1] == hbf[0])
-  __nv_bfloat16 *hm[2];      // m_t . h_{t-1} rows [T1*B][Hp]
-  __nv_bfloat16 *hbf[2];     // h_t rows [T1*B][Hp]
-  __nv_bfloat16 *Wih[2], *WihT[2], *Whh[2], *WhhT[2];
-  __nv_bfloat16 *dgates[2];  // [T*B][G]
-  // fp32
-  float *gx, *r, *gates[2], *cseq[2], *hseq[2], *dc, *dhm, *dx, *dwpad;
-  float *h_init, *c_init;    // [2][B][Hp] padded copies
-  CUtensorMap m_xin[2], m_hm[2], m_hm64[2], m_xin64[2], m_Wih[2], m_Whh[2], m_WihT[2], m_WhhT[2], m_dg128[2], m_dg64[2];
-};
-
+// ------------------------------------------------------------------------------------------------ buffers
 static thread_local char g_lerr[256] = "";
 extern "C" const char* srl_lstm_last_error(void) { return g_lerr; }
 #define LCU(x, what) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { snprintf(g_lerr, sizeof(g_lerr), "%s: %s", what, cudaGetErrorString(e_)); return (int)e_; } } while (0)
-#define LREQ(c, msg) do { if (!(c)) { snprintf(g_lerr, sizeof(g_lerr), "%s", msg); return SRL_EINVAL; } } while (0)
+#define LREQ(c, ...) do { if (!(c)) { snprintf(g_lerr, sizeof(g_lerr), __VA_ARGS__); return SRL_EINVAL; } } while (0)
 
+namespace srl {
+// shape of one forward over N1 = T1*B rows and its backward over the first NB rows (T*B for the learner, T1*B for the stand-alone core)
+struct LstmDims {
+  int T1, B, H, Hp, G;
+  int64_t N1, NB;
+};
+static LstmDims lstm_dims(int T1, int B, int H, int64_t NB) {
+  const int Hp = (H + 63) / 64 * 64;
+  return {T1, B, H, Hp, 4 * Hp, (int64_t)T1 * B, NB};
+}
+struct LstmBuffers {
+  // saved: what a backward reads of its forward
+  __nv_bfloat16* xin0;                                    // layer 0 input rows [N1][Hp] (layer 1's input is hbf[0])
+  __nv_bfloat16 *hm[2], *hbf[2];                          // m_t . h_{t-1} and h_t rows [N1][Hp]
+  __nv_bfloat16 *Wih[2], *WihT[2], *Whh[2], *WhhT[2];     // the weights the forward ran with: [4Hp][Hp] and the transposes [Hp][4Hp]
+  float *gates[2], *cseq[2];                              // gate activations [N1][4Hp], c_t [N1][Hp]
+  float* c_init;                                          // padded initial cell state [2][B][Hp]
+  uint8_t* done;                                          // copy of done [N1] (stand-alone core; the learner passes its own)
+  // scratch: one call's temporaries
+  float *gx, *r, *hseq[2];                                // input projections [N1][4Hp], one step's recurrent product [B][4Hp], h_t [N1][Hp]
+  __nv_bfloat16* dgates[2];                               // [NB][4Hp]
+  float *dx, *dwpad, *dc, *dhm;                           // dh_out / dx [NB][Hp], padded weight gradient [4Hp][Hp], carries [B][Hp]
+  float* bias_part;                                       // per-chunk bias column sums [ceil(NB/64)][4Hp]
+};
+// The LSTM core's rows.  The first LSTM_SAVED_ROWS are what a backward reads of its forward; the rest live for one call.
+constexpr int LSTM_SAVED_ROWS = 19, LSTM_ROWS = 30;
+static int lstm_rows(LstmBuffers& b, const LstmDims& d, WsRow* t) {
+  const int64_t N1 = d.N1, NB = d.NB, B = d.B, Hp = d.Hp, G = d.G;
+  int n = 0;
+  t[n++] = ws_row("xin0", N1 * Hp, &b.xin0);
+  for (int l = 0; l < 2; ++l) {
+    t[n++] = ws_row("hm", N1 * Hp, &b.hm[l]);
+    t[n++] = ws_row("hbf", N1 * Hp, &b.hbf[l]);
+    t[n++] = ws_row("Wih", G * Hp, &b.Wih[l]);
+    t[n++] = ws_row("WihT", G * Hp, &b.WihT[l]);
+    t[n++] = ws_row("Whh", G * Hp, &b.Whh[l]);
+    t[n++] = ws_row("WhhT", G * Hp, &b.WhhT[l]);
+    t[n++] = ws_row("gates", N1 * G, &b.gates[l]);
+    t[n++] = ws_row("cseq", N1 * Hp, &b.cseq[l]);
+  }
+  t[n++] = ws_row("c_init", 2 * B * Hp, &b.c_init);
+  t[n++] = ws_row("done", N1, &b.done);
+  t[n++] = ws_row("gx", N1 * G, &b.gx);
+  t[n++] = ws_row("r", B * G, &b.r);
+  for (int l = 0; l < 2; ++l) t[n++] = ws_row("hseq", N1 * Hp, &b.hseq[l]);
+  for (int l = 0; l < 2; ++l) t[n++] = ws_row("dgates", NB * G, &b.dgates[l]);
+  t[n++] = ws_row("dx", NB * Hp, &b.dx);
+  t[n++] = ws_row("dwpad", G * Hp, &b.dwpad);
+  t[n++] = ws_row("dc", B * Hp, &b.dc);
+  t[n++] = ws_row("dhm", B * Hp, &b.dhm);
+  t[n++] = ws_row("bias_part", (NB + LSTM_BIAS_CHUNK - 1) / LSTM_BIAS_CHUNK * G, &b.bias_part);
+  return n;
+}
+
+struct LstmMaps {
+  CUtensorMap xin[2], hm[2], hm64[2], xin64[2], Wih[2], Whh[2], WihT[2], WhhT[2], dg128[2], dg64[2];
+};
 static bool map2(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint32_t boxrows) {
   const uint64_t d[2] = {cols, rows}, s[1] = {cols};
   const uint32_t bx[2] = {64, boxrows};
   return make_map(m, base, 2, d, s, bx);
 }
-
-extern "C" int srl_lstm_create(int T1, int B, int H, const float* const* weights8, float* const* grads8, srl_lstm_t** out) {
-  LREQ(T1 >= 2 && B >= 1 && H >= 1 && weights8 && grads8 && out, "lstm_create: bad argument");
-  srl_lstm* L = new (std::nothrow) srl_lstm();
-  LREQ(L, "out of memory");
-  L->T1 = T1; L->B = B; L->H = H; L->Hp = (H + 63) / 64 * 64; L->G = 4 * L->Hp;
-  for (int l = 0; l < 2; ++l) for (int k = 0; k < 4; ++k) { L->w[l][k] = weights8[l * 4 + k]; L->g[l][k] = grads8[l * 4 + k]; }
-  const int64_t N1 = (int64_t)T1 * B, NB = (int64_t)(T1 - 1) * B, Hp = L->Hp, G = L->G;
-  auto al = [](int64_t b) { return (b + 255) & ~int64_t(255); };
-  int64_t total = 0;
-  auto take = [&](int64_t bytes) { const int64_t o = total; total += al(bytes); return o; };
-  int64_t o_xin0 = take(N1 * Hp * 2), o_hm[2], o_hbf[2], o_W[2][4], o_dg[2], o_gates[2], o_c[2], o_h[2];
-  for (int l = 0; l < 2; ++l) {
-    o_hm[l] = take(N1 * Hp * 2); o_hbf[l] = take(N1 * Hp * 2);
-    for (int k = 0; k < 4; ++k) o_W[l][k] = take(G * Hp * 2);
-    o_dg[l] = take(NB * G * 2); o_gates[l] = take(N1 * G * 4); o_c[l] = take(N1 * Hp * 4); o_h[l] = take(N1 * Hp * 4);
-  }
-  const int64_t o_gx = take(N1 * G * 4), o_r = take((int64_t)B * G * 4), o_dc = take((int64_t)B * Hp * 4), o_dhm = take((int64_t)B * Hp * 4),
-                o_dx = take(NB * Hp * 4), o_dw = take(G * Hp * 4), o_hi = take(2 * (int64_t)B * Hp * 4), o_ci = take(2 * (int64_t)B * Hp * 4);
-  if (cudaMalloc(&L->arena, total) != cudaSuccess || cudaMemset(L->arena, 0, total) != cudaSuccess) { delete L; LREQ(false, "lstm_create: cudaMalloc failed"); }
-  char* a = L->arena;
-  L->xin[0] = (__nv_bfloat16*)(a + o_xin0);
-  for (int l = 0; l < 2; ++l) {
-    L->hm[l] = (__nv_bfloat16*)(a + o_hm[l]); L->hbf[l] = (__nv_bfloat16*)(a + o_hbf[l]);
-    L->Wih[l] = (__nv_bfloat16*)(a + o_W[l][0]); L->WihT[l] = (__nv_bfloat16*)(a + o_W[l][1]);
-    L->Whh[l] = (__nv_bfloat16*)(a + o_W[l][2]); L->WhhT[l] = (__nv_bfloat16*)(a + o_W[l][3]);
-    L->dgates[l] = (__nv_bfloat16*)(a + o_dg[l]); L->gates[l] = (float*)(a + o_gates[l]); L->cseq[l] = (float*)(a + o_c[l]); L->hseq[l] = (float*)(a + o_h[l]);
-  }
-  L->xin[1] = L->hbf[0];
-  L->gx = (float*)(a + o_gx); L->r = (float*)(a + o_r); L->dc = (float*)(a + o_dc); L->dhm = (float*)(a + o_dhm); L->dx = (float*)(a + o_dx);
-  L->dwpad = (float*)(a + o_dw); L->h_init = (float*)(a + o_hi); L->c_init = (float*)(a + o_ci);
+static bool lstm_maps(const LstmBuffers& b, const LstmDims& d, LstmMaps* m) {
+  const uint64_t N1 = d.N1, NB = d.NB, Hp = d.Hp, G = d.G;
   bool ok = true;
   for (int l = 0; l < 2 && ok; ++l) {
-    ok = ok && map2(&L->m_xin[l], L->xin[l], Hp, N1, 128) && map2(&L->m_xin64[l], L->xin[l], Hp, NB, 64) && map2(&L->m_hm[l], L->hm[l], Hp, N1, 128) &&
-         map2(&L->m_hm64[l], L->hm[l], Hp, NB, 64) && map2(&L->m_Wih[l], L->Wih[l], Hp, G, 64) && map2(&L->m_Whh[l], L->Whh[l], Hp, G, 64) &&
-         map2(&L->m_WihT[l], L->WihT[l], G, Hp, 64) && map2(&L->m_WhhT[l], L->WhhT[l], G, Hp, 64) && map2(&L->m_dg128[l], L->dgates[l], G, NB, 128) &&
-         map2(&L->m_dg64[l], L->dgates[l], G, NB, 64);
+    const __nv_bfloat16* xin = l ? b.hbf[0] : b.xin0;
+    ok = map2(&m->xin[l], xin, Hp, N1, 128) && map2(&m->xin64[l], xin, Hp, NB, 64) && map2(&m->hm[l], b.hm[l], Hp, N1, 128) &&
+         map2(&m->hm64[l], b.hm[l], Hp, NB, 64) && map2(&m->Wih[l], b.Wih[l], Hp, G, 64) && map2(&m->Whh[l], b.Whh[l], Hp, G, 64) &&
+         map2(&m->WihT[l], b.WihT[l], G, Hp, 64) && map2(&m->WhhT[l], b.WhhT[l], G, Hp, 64) && map2(&m->dg128[l], b.dgates[l], G, NB, 128) &&
+         map2(&m->dg64[l], b.dgates[l], G, NB, 64);
   }
-  if (!ok) { cudaFree(L->arena); delete L; LREQ(false, "lstm_create: tensor map creation failed"); }
-  *out = L;
-  return 0;
+  return ok;
 }
-extern "C" int srl_lstm_destroy(srl_lstm_t* L) { if (L) { cudaFree(L->arena); delete L; } return 0; }
 
 static inline int cdiv_(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
-// core fp32 [T1*B][H], done u8 [T1*B], h0/c0 fp32 [2][B][H] -> out fp32 [T1*B][H], hT/cT fp32 [2][B][H] (may be NULL)
-extern "C" int srl_lstm_forward(srl_lstm_t* L, const float* core, const uint8_t* done, const float* h0, const float* c0, float* out,
-                                float* hT, float* cT, void* stream) {
-  LREQ(L && core && done && h0 && c0 && out, "lstm_forward: NULL pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int T1 = L->T1, B = L->B, H = L->H, Hp = L->Hp, G = L->G;
-  const int64_t N1 = (int64_t)T1 * B;
-  lstm_pad_bf16_kernel<<<cdiv_(N1 * Hp, 256), 256, 0, st>>>(core, (int)N1, H, Hp, L->xin[0]);
+// core f32 [N1][H], done u8 [N1], h0/c0 f32 [2][B][H], w8 = the 8 nn.LSTM tensors -> out f32 [N1][H], hT/cT f32 [2][B][H] (may be NULL)
+static int lstm_forward_rows(const LstmDims& d, const LstmBuffers& b, const LstmMaps& m, const float* const* w8, const float* core,
+                             const uint8_t* done, const float* h0, const float* c0, float* out, float* hT, float* cT, cudaStream_t st) {
+  const int T1 = d.T1, B = d.B, H = d.H, Hp = d.Hp, G = d.G;
+  const int64_t N1 = d.N1;
+  lstm_pad_bf16_kernel<<<cdiv_(N1 * Hp, 256), 256, 0, st>>>(core, (int)N1, H, Hp, b.xin0);
   for (int l = 0; l < 2; ++l) {
-    lstm_pack_w_kernel<<<cdiv_((int64_t)G * Hp, 256), 256, 0, st>>>(L->w[l][0], H, Hp, L->Wih[l], L->WihT[l]);
-    lstm_pack_w_kernel<<<cdiv_((int64_t)G * Hp, 256), 256, 0, st>>>(L->w[l][1], H, Hp, L->Whh[l], L->WhhT[l]);
+    lstm_pack_w_kernel<<<cdiv_((int64_t)G * Hp, 256), 256, 0, st>>>(w8[4 * l], H, Hp, b.Wih[l], b.WihT[l]);
+    lstm_pack_w_kernel<<<cdiv_((int64_t)G * Hp, 256), 256, 0, st>>>(w8[4 * l + 1], H, Hp, b.Whh[l], b.WhhT[l]);
   }
   LCU(cudaGetLastError(), "lstm pack");
   const int cell_blocks = cdiv_((int64_t)B * Hp, 256);
   for (int l = 0; l < 2; ++l) {
-    // padded copies of the initial state of this layer
-    LCU(cudaMemcpy2DAsync(L->h_init + (size_t)l * B * Hp, Hp * 4, h0 + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "h0 copy");
-    LCU(cudaMemcpy2DAsync(L->c_init + (size_t)l * B * Hp, Hp * 4, c0 + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "c0 copy");
-    lstm_init_hm_kernel<<<cell_blocks, 256, 0, st>>>(h0 + (size_t)l * B * H, done, B, H, Hp, L->hm[l]);
-    { LGemmK::Params q{L->m_xin[l], L->m_Wih[l], L->gx, (int)N1, Hp / 64, G, 0, 0};      // input projection of every step
+    // padded copy of this layer's initial cell state
+    LCU(cudaMemcpy2DAsync(b.c_init + (size_t)l * B * Hp, Hp * 4, c0 + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "c0 copy");
+    lstm_init_hm_kernel<<<cell_blocks, 256, 0, st>>>(h0 + (size_t)l * B * H, done, B, H, Hp, b.hm[l]);
+    { LGemmK::Params q{m.xin[l], m.Wih[l], b.gx, (int)N1, Hp / 64, G, 0, 0};      // input projection of every step
       LCU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(N1, 128), G / 64), st), "lstm gx gemm"); }
     for (int t = 0; t < T1; ++t) {
-      { LGemmK::Params q{L->m_hm[l], L->m_Whh[l], L->r, B, Hp / 64, G, t * B, 0};
+      { LGemmK::Params q{m.hm[l], m.Whh[l], b.r, B, Hp / 64, G, t * B, 0};
         LCU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(B, 128), G / 64), st), "lstm recurrent gemm"); }
-      const float* cprev = t == 0 ? L->c_init + (size_t)l * B * Hp : L->cseq[l] + (size_t)(t - 1) * B * Hp;
+      const float* cprev = t == 0 ? b.c_init + (size_t)l * B * Hp : b.cseq[l] + (size_t)(t - 1) * B * Hp;
       lstm_cell_fwd_kernel<<<cell_blocks, 256, 0, st>>>(
-          L->gx + (size_t)t * B * G, L->r, L->w[l][2], L->w[l][3], cprev, done + (size_t)t * B, t + 1 < T1 ? done + (size_t)(t + 1) * B : nullptr, B, H, Hp,
-          L->gates[l] + (size_t)t * B * G, L->cseq[l] + (size_t)t * B * Hp, L->hseq[l] + (size_t)t * B * Hp, L->hbf[l] + (size_t)t * B * Hp,
-          t + 1 < T1 ? L->hm[l] + (size_t)(t + 1) * B * Hp : nullptr);
+          b.gx + (size_t)t * B * G, b.r, w8[4 * l + 2], w8[4 * l + 3], cprev, done + (size_t)t * B, t + 1 < T1 ? done + (size_t)(t + 1) * B : nullptr, B,
+          H, Hp, b.gates[l] + (size_t)t * B * G, b.cseq[l] + (size_t)t * B * Hp, b.hseq[l] + (size_t)t * B * Hp, b.hbf[l] + (size_t)t * B * Hp,
+          t + 1 < T1 ? b.hm[l] + (size_t)(t + 1) * B * Hp : nullptr);
     }
     LCU(cudaGetLastError(), "lstm cell");
   }
-  lstm_unpad_rows_kernel<<<cdiv_(N1 * H, 256), 256, 0, st>>>(L->hseq[1], (int)N1, H, Hp, out);
+  lstm_unpad_rows_kernel<<<cdiv_(N1 * H, 256), 256, 0, st>>>(b.hseq[1], (int)N1, H, Hp, out);
   for (int l = 0; l < 2; ++l) {
-    if (hT) LCU(cudaMemcpy2DAsync(hT + (size_t)l * B * H, H * 4, L->hseq[l] + (size_t)(T1 - 1) * B * Hp, Hp * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "hT");
-    if (cT) LCU(cudaMemcpy2DAsync(cT + (size_t)l * B * H, H * 4, L->cseq[l] + (size_t)(T1 - 1) * B * Hp, Hp * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "cT");
+    if (hT) LCU(cudaMemcpy2DAsync(hT + (size_t)l * B * H, H * 4, b.hseq[l] + (size_t)(T1 - 1) * B * Hp, Hp * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "hT");
+    if (cT) LCU(cudaMemcpy2DAsync(cT + (size_t)l * B * H, H * 4, b.cseq[l] + (size_t)(T1 - 1) * B * Hp, Hp * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "cT");
   }
   LCU(cudaGetLastError(), "lstm forward");
   return 0;
 }
 
-// dout fp32 [T*B][H] (gradient w.r.t. the LSTM output of steps 0..T-1) -> dcore fp32 [T*B][H]; weight/bias gradients are
-// ACCUMULATED into the grads8 buffers given at creation.  Must follow srl_lstm_forward on the same inputs.
-extern "C" int srl_lstm_backward(srl_lstm_t* L, const float* dout, const uint8_t* done, float* dcore, void* stream) {
-  LREQ(L && dout && done && dcore, "lstm_backward: NULL pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int T = L->T1 - 1, B = L->B, H = L->H, Hp = L->Hp, G = L->G;
-  const int64_t NB = (int64_t)T * B;
+// BPTT over the first d.NB rows (steps 0 .. NB/B - 1) of the forward that filled b: dout f32 [NB][H] -> dcore f32 [NB][H]; the weight and
+// bias gradients are ACCUMULATED into g8.  dhT / dcT f32 [2][B][H] (NULL: zero) seed the last step: dhT[l] is added to that step's dh
+// unmasked, dcT[l] is its incoming cell-state carry.  dh0 / dc0 f32 [2][B][H] (NULL: not wanted) receive the gradient of the initial state.
+static int lstm_backward_rows(const LstmDims& d, const LstmBuffers& b, const LstmMaps& m, float* const* g8, const uint8_t* done, const float* dout,
+                              const float* dhT, const float* dcT, float* dcore, float* dh0, float* dc0, cudaStream_t st) {
+  const int B = d.B, H = d.H, Hp = d.Hp, G = d.G;
+  const int64_t NB = d.NB;
+  const int steps = (int)(NB / B);
   const int cell_blocks = cdiv_((int64_t)B * Hp, 256);
-  // dh_out of the top layer, padded to Hp (reuse dx as the padded buffer)
-  LCU(cudaMemsetAsync(L->dx, 0, NB * Hp * 4, st), "zero dx");
-  LCU(cudaMemcpy2DAsync(L->dx, Hp * 4, dout, H * 4, H * 4, NB, cudaMemcpyDeviceToDevice, st), "pad dout");
+  // dh_out of the top layer, padded to Hp (dx is the padded buffer)
+  LCU(cudaMemsetAsync(b.dx, 0, NB * Hp * 4, st), "zero dx");
+  LCU(cudaMemcpy2DAsync(b.dx, Hp * 4, dout, H * 4, H * 4, NB, cudaMemcpyDeviceToDevice, st), "pad dout");
   for (int l = 1; l >= 0; --l) {
-    LCU(cudaMemsetAsync(L->dc, 0, (size_t)B * Hp * 4, st), "zero dc");
-    for (int t = T - 1; t >= 0; --t) {
-      const float* cprev = t == 0 ? L->c_init + (size_t)l * B * Hp : L->cseq[l] + (size_t)(t - 1) * B * Hp;
+    if (dcT) LCU(cudaMemcpy2DAsync(b.dc, Hp * 4, dcT + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "dcT copy");
+    else LCU(cudaMemsetAsync(b.dc, 0, (size_t)B * Hp * 4, st), "zero dc");
+    if (dhT) LCU(cudaMemcpy2DAsync(b.dhm, Hp * 4, dhT + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "dhT copy");
+    for (int t = steps - 1; t >= 0; --t) {
+      const bool last = t + 1 == steps;
+      const float* cprev = t == 0 ? b.c_init + (size_t)l * B * Hp : b.cseq[l] + (size_t)(t - 1) * B * Hp;
       lstm_cell_bwd_kernel<<<cell_blocks, 256, 0, st>>>(
-          L->dx + (size_t)t * B * Hp, t + 1 < T ? L->dhm : nullptr, done + (size_t)(t + 1) * B, L->gates[l] + (size_t)t * B * G,
-          L->cseq[l] + (size_t)t * B * Hp, cprev, done + (size_t)t * B, L->dc, B, H, Hp, L->dgates[l] + (size_t)t * B * G);
-      if (t > 0) {   // dhm_t = dgates_t . Whh  (gradient w.r.t. m_t . h_{t-1})
-        LGemmK::Params q{L->m_dg128[l], L->m_WhhT[l], L->dhm, B, G / 64, Hp, t * B, 0};
+          b.dx + (size_t)t * B * Hp, last && !dhT ? nullptr : b.dhm, last ? nullptr : done + (size_t)(t + 1) * B, b.gates[l] + (size_t)t * B * G,
+          b.cseq[l] + (size_t)t * B * Hp, cprev, done + (size_t)t * B, b.dc, B, H, Hp, b.dgates[l] + (size_t)t * B * G);
+      if (t > 0 || dh0) {   // dhm_t = dgates_t . Whh  (gradient w.r.t. m_t . h_{t-1})
+        LGemmK::Params q{m.dg128[l], m.WhhT[l], b.dhm, B, G / 64, Hp, t * B, 0};
         LCU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(B, 128), Hp / 64), st), "lstm bwd recurrent gemm");
       }
     }
     LCU(cudaGetLastError(), "lstm cell bwd");
-    // weight gradients over all T*B rows (MN-major operands), then un-pad + accumulate
-    { LGemmMN::Params q{L->m_dg64[l], L->m_xin64[l], L->dwpad, (int)NB, Hp};
+    if (dh0) lstm_unpad_masked_kernel<<<cdiv_((int64_t)B * H, 256), 256, 0, st>>>(b.dhm, done, B, H, Hp, dh0 + (size_t)l * B * H);
+    if (dc0) lstm_unpad_rows_kernel<<<cdiv_((int64_t)B * H, 256), 256, 0, st>>>(b.dc, B, H, Hp, dc0 + (size_t)l * B * H);
+    // weight gradients over all NB rows (MN-major operands), then un-pad + accumulate
+    { LGemmMN::Params q{m.dg64[l], m.xin64[l], b.dwpad, (int)NB, Hp};
       LCU(igemm_tma_launch<LGemmMN>(q, dim3(G / 128, Hp / 64), st), "lstm dWih gemm");
-      lstm_unpad_w_kernel<<<cdiv_((int64_t)4 * H * H, 256), 256, 0, st>>>(L->dwpad, H, Hp, L->g[l][0]); }
-    { LGemmMN::Params q{L->m_dg64[l], L->m_hm64[l], L->dwpad, (int)NB, Hp};
+      lstm_unpad_w_kernel<<<cdiv_((int64_t)4 * H * H, 256), 256, 0, st>>>(b.dwpad, H, Hp, g8[4 * l]); }
+    { LGemmMN::Params q{m.dg64[l], m.hm64[l], b.dwpad, (int)NB, Hp};
       LCU(igemm_tma_launch<LGemmMN>(q, dim3(G / 128, Hp / 64), st), "lstm dWhh gemm");
-      lstm_unpad_w_kernel<<<cdiv_((int64_t)4 * H * H, 256), 256, 0, st>>>(L->dwpad, H, Hp, L->g[l][1]); }
-    { const int rpb = 64;
-      lstm_bias_grad_kernel<<<dim3(cdiv_(G, 128), cdiv_(NB, rpb)), 128, 0, st>>>(L->dgates[l], (int)NB, H, Hp, rpb, L->g[l][2], L->g[l][3]); }
+      lstm_unpad_w_kernel<<<cdiv_((int64_t)4 * H * H, 256), 256, 0, st>>>(b.dwpad, H, Hp, g8[4 * l + 1]); }
+    { const int chunks = cdiv_(NB, LSTM_BIAS_CHUNK);
+      lstm_bias_part_kernel<<<dim3(cdiv_(G, 128), chunks), 128, 0, st>>>(b.dgates[l], (int)NB, G, b.bias_part);
+      lstm_bias_sum_kernel<<<cdiv_((int64_t)4 * H, 256), 256, 0, st>>>(b.bias_part, chunks, H, Hp, g8[4 * l + 2], g8[4 * l + 3]); }
     // gradient w.r.t. this layer's input = dh_out of the layer below (or dcore)
-    { LGemmK::Params q{L->m_dg128[l], L->m_WihT[l], L->dx, (int)NB, G / 64, Hp, 0, 0};
+    { LGemmK::Params q{m.dg128[l], m.WihT[l], b.dx, (int)NB, G / 64, Hp, 0, 0};
       LCU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(NB, 128), Hp / 64), st), "lstm dx gemm"); }
   }
-  lstm_unpad_rows_kernel<<<cdiv_(NB * H, 256), 256, 0, st>>>(L->dx, (int)NB, H, Hp, dcore);
+  lstm_unpad_rows_kernel<<<cdiv_(NB * H, 256), 256, 0, st>>>(b.dx, (int)NB, H, Hp, dcore);
   LCU(cudaGetLastError(), "lstm backward");
   return 0;
+}
+}  // namespace srl
+
+// ------------------------------------------------------------------------------------------------ learner context
+struct srl_lstm {
+  LstmDims d;                // backward over the first T = T1 - 1 steps
+  const float* w[8];         // weight_ih, weight_hh, bias_ih, bias_hh per layer (fp32, PyTorch layouts, caller-owned)
+  float* g[8];               // gradients (same layouts), accumulated
+  char* arena;               // every row of lstm_rows
+  LstmBuffers b;
+  LstmMaps m;
+};
+
+extern "C" int srl_lstm_create(int T1, int B, int H, const float* const* weights8, float* const* grads8, srl_lstm_t** out) {
+  LREQ(T1 >= 2 && B >= 1 && H >= 1 && weights8 && grads8 && out, "lstm_create: bad argument");
+  srl_lstm* L = new (std::nothrow) srl_lstm();
+  LREQ(L, "out of memory");
+  L->d = lstm_dims(T1, B, H, (int64_t)(T1 - 1) * B);
+  for (int i = 0; i < 8; ++i) { L->w[i] = weights8[i]; L->g[i] = grads8[i]; }
+  WsRow t[LSTM_ROWS];
+  lstm_rows(L->b, L->d, t);
+  const int64_t total = rows_bytes(t, LSTM_ROWS, false);
+  if (cudaMalloc(&L->arena, total) != cudaSuccess || cudaMemset(L->arena, 0, total) != cudaSuccess) { delete L; LREQ(false, "lstm_create: cudaMalloc failed"); }
+  carve_rows(t, LSTM_ROWS, false, L->arena);
+  if (!lstm_maps(L->b, L->d, &L->m)) { cudaFree(L->arena); delete L; LREQ(false, "lstm_create: tensor map creation failed"); }
+  *out = L;
+  return 0;
+}
+extern "C" int srl_lstm_destroy(srl_lstm_t* L) { if (L) { cudaFree(L->arena); delete L; } return 0; }
+
+extern "C" int srl_lstm_forward(srl_lstm_t* L, const float* core, const uint8_t* done, const float* h0, const float* c0, float* out,
+                                float* hT, float* cT, void* stream) {
+  LREQ(L && core && done && h0 && c0 && out, "lstm_forward: NULL pointer");
+  return lstm_forward_rows(L->d, L->b, L->m, L->w, core, done, h0, c0, out, hT, cT, (cudaStream_t)stream);
+}
+
+extern "C" int srl_lstm_backward(srl_lstm_t* L, const float* dout, const uint8_t* done, float* dcore, void* stream) {
+  LREQ(L && dout && done && dcore, "lstm_backward: NULL pointer");
+  return lstm_backward_rows(L->d, L->b, L->m, L->g, done, dout, nullptr, nullptr, dcore, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------------------ stand-alone core on caller-owned blocks
+constexpr int LSTM_CORE_MAX_ROWS = 65536;
+
+static int check_core_shape(int T1, int B, int A, const char* what) {
+  LREQ(T1 >= 1 && B >= 1 && (int64_t)T1 * B <= LSTM_CORE_MAX_ROWS, "%s: T1=%d B=%d: need T1 >= 1, B >= 1 and T1*B <= %d", what, T1, B,
+       LSTM_CORE_MAX_ROWS);
+  LREQ(A >= 1 && A <= 31, "%s: A=%d must be in [1, 31]", what, A);
+  return 0;
+}
+
+extern "C" int srl_lstm_core_sizes(int T1, int B, int A, int64_t* saved_bytes, int64_t* scratch_bytes) {
+  LREQ(saved_bytes && scratch_bytes, "lstm_core_sizes: NULL argument");
+  int rc = check_core_shape(T1, B, A, "lstm_core_sizes");
+  if (rc) return rc;
+  LstmBuffers b = {};
+  WsRow t[LSTM_ROWS];
+  lstm_rows(b, lstm_dims(T1, B, 513 + A, (int64_t)T1 * B), t);
+  *saved_bytes = rows_bytes(t, LSTM_SAVED_ROWS, false);
+  *scratch_bytes = rows_bytes(t + LSTM_SAVED_ROWS, LSTM_ROWS - LSTM_SAVED_ROWS, false);
+  return 0;
+}
+
+// one argument of a call: outputs may overlap nothing, inputs may overlap each other
+struct Span { const void* p; int64_t bytes; bool out; const char* name; };
+static int check_spans(const Span* s, int n, const char* what) {
+  for (int i = 0; i < n; ++i)
+    for (int j = 0; j < i; ++j) {
+      if (!s[i].p || !s[j].p || !(s[i].out || s[j].out)) continue;
+      const uintptr_t x = reinterpret_cast<uintptr_t>(s[i].p), y = reinterpret_cast<uintptr_t>(s[j].p);
+      LREQ(!(x < y + (uintptr_t)s[j].bytes && y < x + (uintptr_t)s[i].bytes), "%s: %s overlaps %s", what, s[i].name, s[j].name);
+    }
+  return 0;
+}
+static const char* const kW8[8] = {"weights8[0]", "weights8[1]", "weights8[2]", "weights8[3]", "weights8[4]", "weights8[5]", "weights8[6]", "weights8[7]"};
+static const char* const kG8[8] = {"grads8[0]", "grads8[1]", "grads8[2]", "grads8[3]", "grads8[4]", "grads8[5]", "grads8[6]", "grads8[7]"};
+static int64_t lstm_tensor_bytes(int i, int H) { return (i % 4 < 2 ? (int64_t)4 * H * H : (int64_t)4 * H) * 4; }
+
+// the checks both calls share: shape, the blocks' alignment and sizes
+static int check_core_call(int T1, int B, int A, const void* saved, const void* scratch, int64_t* sb, int64_t* kb, const char* what) {
+  int rc = check_core_shape(T1, B, A, what);
+  if (rc) return rc;
+  LREQ(((reinterpret_cast<uintptr_t>(saved) | reinterpret_cast<uintptr_t>(scratch)) & 255) == 0, "%s: saved and scratch must be 256-byte aligned", what);
+  return srl_lstm_core_sizes(T1, B, A, sb, kb);
+}
+
+// the blocks of one call -> the buffers and their tensor maps, encoded on the host for this call (legal under stream capture)
+static int core_call_setup(const LstmDims& d, void* saved, void* scratch, LstmBuffers* b, LstmMaps* m, const char* what) {
+  WsRow t[LSTM_ROWS];
+  *b = LstmBuffers{};
+  lstm_rows(*b, d, t);
+  carve_rows(t, LSTM_SAVED_ROWS, false, static_cast<char*>(saved));
+  carve_rows(t + LSTM_SAVED_ROWS, LSTM_ROWS - LSTM_SAVED_ROWS, false, static_cast<char*>(scratch));
+  // encoding needs the device's context current on this thread, and this may be the thread's first CUDA call (torch runs a backward
+  // on an autograd thread of its own): cudaSetDevice makes the primary context current
+  int dev = 0;
+  LCU(cudaGetDevice(&dev), "cudaGetDevice");
+  LCU(cudaSetDevice(dev), "cudaSetDevice");
+  if (!lstm_maps(*b, d, m)) {
+    snprintf(g_lerr, sizeof(g_lerr), "%s: tensor map creation failed (driver without cuTensorMapEncodeTiled?)", what);
+    return SRL_ESTATE;
+  }
+  pdl_set_active(true);
+  return 0;
+}
+
+extern "C" int srl_lstm_core_forward(const float* core, const uint8_t* done, const float* h0, const float* c0, int A, int T1, int B,
+                                     const float* const* weights8, void* saved, void* scratch, float* out, float* hT, float* cT, void* stream) {
+  LREQ(core && done && h0 && c0 && weights8 && saved && scratch && out && hT && cT, "lstm_core_forward: NULL pointer");
+  for (int i = 0; i < 8; ++i) LREQ(weights8[i], "lstm_core_forward: weights8[%d] is NULL", i);
+  int64_t sb = 0, kb = 0;
+  int rc = check_core_call(T1, B, A, saved, scratch, &sb, &kb, "lstm_core_forward");
+  if (rc) return rc;
+  const int H = 513 + A;
+  const int64_t N1 = (int64_t)T1 * B, rows = N1 * H * 4, state = (int64_t)2 * B * H * 4;
+  Span s[17] = {{core, rows, false, "core"}, {done, N1, false, "done"}, {h0, state, false, "h0"}, {c0, state, false, "c0"}};
+  int n = 4;
+  for (int i = 0; i < 8; ++i) s[n++] = {weights8[i], lstm_tensor_bytes(i, H), false, kW8[i]};
+  s[n++] = {saved, sb, true, "saved"}; s[n++] = {scratch, kb, true, "scratch"};
+  s[n++] = {out, rows, true, "out"}; s[n++] = {hT, state, true, "hT"}; s[n++] = {cT, state, true, "cT"};
+  rc = check_spans(s, n, "lstm_core_forward");
+  if (rc) return rc;
+  const LstmDims d = lstm_dims(T1, B, H, N1);
+  LstmBuffers b;
+  LstmMaps m;
+  rc = core_call_setup(d, saved, scratch, &b, &m, "lstm_core_forward");
+  if (rc) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  LCU(cudaMemcpyAsync(b.done, done, N1, cudaMemcpyDeviceToDevice, st), "done copy");
+  return lstm_forward_rows(d, b, m, weights8, core, b.done, h0, c0, out, hT, cT, st);
+}
+
+extern "C" int srl_lstm_core_backward(const float* dout, const float* dhT, const float* dcT, int A, int T1, int B, void* saved, void* scratch,
+                                      float* const* grads8, float* dcore, float* dh0, float* dc0, void* stream) {
+  LREQ(dout && saved && scratch && grads8 && dcore, "lstm_core_backward: NULL pointer");
+  for (int i = 0; i < 8; ++i) LREQ(grads8[i], "lstm_core_backward: grads8[%d] is NULL", i);
+  int64_t sb = 0, kb = 0;
+  int rc = check_core_call(T1, B, A, saved, scratch, &sb, &kb, "lstm_core_backward");
+  if (rc) return rc;
+  const int H = 513 + A;
+  const int64_t N1 = (int64_t)T1 * B, rows = N1 * H * 4, state = (int64_t)2 * B * H * 4;
+  Span s[16] = {{dout, rows, false, "dout"}, {dhT, state, false, "dhT"}, {dcT, state, false, "dcT"}, {saved, sb, false, "saved"},
+                {scratch, kb, true, "scratch"}};
+  int n = 5;
+  for (int i = 0; i < 8; ++i) s[n++] = {grads8[i], lstm_tensor_bytes(i, H), true, kG8[i]};
+  s[n++] = {dcore, rows, true, "dcore"}; s[n++] = {dh0, state, true, "dh0"}; s[n++] = {dc0, state, true, "dc0"};
+  rc = check_spans(s, n, "lstm_core_backward");
+  if (rc) return rc;
+  const LstmDims d = lstm_dims(T1, B, H, N1);
+  LstmBuffers b;
+  LstmMaps m;
+  rc = core_call_setup(d, saved, scratch, &b, &m, "lstm_core_backward");
+  if (rc) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  for (int i = 0; i < 8; ++i) LCU(cudaMemsetAsync(grads8[i], 0, lstm_tensor_bytes(i, H), st), "zero grads8");     // overwritten, not accumulated
+  return lstm_backward_rows(d, b, m, grads8, b.done, dout, dhT, dcT, dcore, dh0, dc0, st);
 }
 
 // ------------------------------------------------------------------------------------------------ actor step: host side

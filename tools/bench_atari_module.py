@@ -7,7 +7,9 @@ zero_grad, backward, clip_grad_norm_(40), RMSprop step; the stats dict and its h
   dropin_graph  the same statements captured once in a CUDA graph and replayed (RMSprop(capturable=True))
   learner       B200ImpalaLearner.learn(sync_stats=False), the whole step on the library's kernels: the floor
 
-python tools/bench_atari_module.py [--T 20 --B 32 --A 6 --steps 50 --warmup 10 --rounds 5 --precision bf16]
+python tools/bench_atari_module.py [--T 20 --B 32 --A 6 --steps 50 --warmup 10 --rounds 5 --precision bf16] [--use-lstm]
+--use-lstm: the same four rows with AtariNet(use_lstm=True) and B200ImpalaLearner(use_lstm=True); every model starts from the same random
+initial state (h0, c0).  The drop-in runs its LSTM on the sm_90a kernels in the bf16 mode, on nn.LSTM in fp32_split.
 Each round times every model over --steps steps (host clock around work that ends in a device synchronise), alternating the models;
 ms per step is reported as the median and the range over the rounds.  Prints the GPU name and power limit first, then one JSON line
 per model.  Needs a CUDA device; writes nothing."""
@@ -36,9 +38,9 @@ def gpu_info():
     return {'torch_name': torch.cuda.get_device_name(), 'nvidia_smi': q.stdout.strip() or q.stderr.strip()}
 
 
-def learn_statements(model, vtrace, loss_fn, batch, optimizer):
+def learn_statements(model, vtrace, loss_fn, batch, optimizer, initial_rnn_state=()):
     """impala_atari.py:289-346 without the stats dict"""
-    learner_outputs, _ = model(batch, ())
+    learner_outputs, _ = model(batch, initial_rnn_state)
     bootstrap_value = learner_outputs['baseline'][-1]
     batch = {key: tensor[1:] for key, tensor in batch.items()}
     learner_outputs = {key: tensor[:-1] for key, tensor in learner_outputs.items()}
@@ -70,48 +72,54 @@ def main():
     ap.add_argument('--warmup', type=int, default=10)
     ap.add_argument('--rounds', type=int, default=5)
     ap.add_argument('--precision', default='bf16', choices=['bf16', 'fp32_split'])
+    ap.add_argument('--use-lstm', action='store_true')
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('bench_atari_module.py needs a CUDA device')
     from scalerl_b200.algorithms.impala import loss_fn as lf_mine, vtrace as vt_mine
     from scalerl_b200.algorithms.utils.atari_model import AtariNet
     from scalerl_b200.learner import B200ImpalaLearner, ImpalaHParams
-    print(json.dumps({'gpu': gpu_info(), 'T': a.T, 'B': a.B, 'A': a.A, 'precision': a.precision,
+    print(json.dumps({'gpu': gpu_info(), 'T': a.T, 'B': a.B, 'A': a.A, 'precision': a.precision, 'use_lstm': a.use_lstm,
                       'cudnn_allow_tf32': torch.backends.cudnn.allow_tf32, 'matmul_allow_tf32': torch.backends.cuda.matmul.allow_tf32}), flush=True)
     params = O.init_params(a.A, seed=0)
+    if a.use_lstm:
+        params.update(O.init_lstm_params(a.A, seed=0))
     batch = {k: v.cuda() for k, v in O.synthetic_batch(a.T, a.B, a.A, seed=0, done_p=0.05).items()}
+    g = torch.Generator().manual_seed(1)
+    state = tuple((torch.randn(2, a.B, 513 + a.A, generator=g) * 0.3).cuda() for _ in range(2)) if a.use_lstm else ()
     steps = {}
 
     if ref_learner.available():
-        ref = ref_learner.ReferenceLearner(num_actions=a.A, state_dict=params)
+        ref = ref_learner.ReferenceLearner(num_actions=a.A, use_lstm=a.use_lstm, state_dict=params)
         ref.model.cuda()
         ref_opt = rmsprop(ref.model)
-        steps['reference'] = lambda: learn_statements(ref.model, ref.vtrace, ref.loss_fn, batch, ref_opt)
+        steps['reference'] = lambda: learn_statements(ref.model, ref.vtrace, ref.loss_fn, batch, ref_opt, state)
     else:
         print(json.dumps({'model': 'reference', 'ms_per_step': 'not measured: oracle/_ref is missing (python oracle/make_ref.py)'}))
 
-    net = AtariNet((4, 84, 84), a.A, precision=a.precision).cuda()
+    net = AtariNet((4, 84, 84), a.A, a.use_lstm, precision=a.precision).cuda()
     net.load_state_dict(params)
     opt = rmsprop(net)
-    steps['dropin_eager'] = lambda: learn_statements(net, vt_mine, lf_mine, batch, opt)
+    steps['dropin_eager'] = lambda: learn_statements(net, vt_mine, lf_mine, batch, opt, state)
 
-    gnet = AtariNet((4, 84, 84), a.A, precision=a.precision).cuda()
+    gnet = AtariNet((4, 84, 84), a.A, a.use_lstm, precision=a.precision).cuda()
     gnet.load_state_dict(params)
     gopt = rmsprop(gnet, capturable=True)
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(side):
         for _ in range(3):
-            learn_statements(gnet, vt_mine, lf_mine, batch, gopt)
+            learn_statements(gnet, vt_mine, lf_mine, batch, gopt, state)
     torch.cuda.current_stream().wait_stream(side)
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph):
-        learn_statements(gnet, vt_mine, lf_mine, batch, gopt)
+        learn_statements(gnet, vt_mine, lf_mine, batch, gopt, state)
     steps['dropin_graph'] = graph.replay
 
-    hp = ImpalaHParams(rollout_length=a.T, batch_size=a.B, num_actions=a.A, precision=a.precision)
-    learner = B200ImpalaLearner(hp, init_state_dict=params, process_group=False)
-    steps['learner'] = lambda: learner.learn(batch, sync_stats=False)
+    if not (a.use_lstm and a.precision == 'fp32_split'):       # the learner's LSTM has bf16 operands only
+        hp = ImpalaHParams(rollout_length=a.T, batch_size=a.B, num_actions=a.A, precision=a.precision, use_lstm=a.use_lstm)
+        learner = B200ImpalaLearner(hp, init_state_dict=params, process_group=False)
+        steps['learner'] = lambda: learner.learn(batch, state, sync_stats=False)
 
     for fn in steps.values():
         for _ in range(a.warmup):
