@@ -6,7 +6,7 @@
  * only -- no torch types.  Every pointer is a DEVICE pointer unless the name ends in `_host`.
  * `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).  Return value: 0 on
  * success, otherwise a cudaError_t (>0) or a negative SRL_E* argument error; srl_last_error()
- * returns a message for the calling thread.  Nothing here synchronises the stream.
+ * returns the message of the calling thread's last failed call, whichever entry point it was.  Nothing here synchronises the stream.
  */
 #ifndef SCALERL_B200_H_
 #define SCALERL_B200_H_
@@ -283,7 +283,8 @@ int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int frames, int A
  * forward : core f32 [T1,B,H], done u8 [T1,B], h0/c0 f32 [2,B,H] -> out f32 [T1,B,H], hT/cT f32 [2,B,H] (may be NULL)
  * backward: dout f32 [T1-1,B,H] (rows 0..T1-2 only: the learner's bootstrap row T1-1 carries no gradient) -> dcore f32 [T1-1,B,H].
  *           The bias gradients are reduced without atomics (fixed 64-row chunks added in order): the same bits on every run.
- * Errors of these calls and of srl_lstm_core_* are reported by srl_lstm_last_error. */
+ * Errors of these calls and of srl_lstm_core_* are reported by srl_last_error, as every other call's; srl_lstm_last_error returns
+ * the same message (kept for existing hosts). */
 typedef struct srl_lstm srl_lstm_t;
 int srl_lstm_create(int T1, int B, int H, const float* const* weights8, float* const* grads8, srl_lstm_t** out);
 int srl_lstm_destroy(srl_lstm_t* L);
@@ -312,7 +313,8 @@ int srl_lstm_core_backward(const float* dout, const float* dhT, const float* dcT
 /* ---- prioritized-replay sampler (BASELINE.json configs[3]; SURVEY.md §8f) ---------------------------------------------------
  * Device-resident float64 sum/min segment trees; replaces PrioritizedReplayBuffer's tree arithmetic
  * (scalerl/data/replay_buffer.py:305-381 over scalerl/data/segment_tree.py:7-196).  Index results are identical to the
- * reference's Python-float trees given identical leaf values.  The transition storage itself stays with the caller. */
+ * reference's Python-float trees given identical leaf values.  The transition storage itself stays with the caller.
+ * Errors are reported by srl_last_error; srl_per_last_error returns the same message (kept for existing hosts). */
 typedef struct srl_per srl_per_t;
 int srl_per_create(int64_t memory_size, double alpha, srl_per_t** out);
 int srl_per_destroy(srl_per_t* P);

@@ -117,12 +117,6 @@ def hooks():
     return _hooks
 
 
-def check_hook(rc, what=''):
-    if rc != 0:
-        msg = hooks().srl_test_last_error().decode()
-        raise (ValueError if rc == -1 else RuntimeError)(f'{what}: rc={rc}: {msg}')
-
-
 EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step'])
 
 
@@ -162,12 +156,19 @@ def lib():
     return _lib
 
 
-def check(rc, what=''):
+def check(rc, what='', last_error=None):
+    """raises on a non-zero return code: ValueError for a bad argument (SRL_EINVAL), RuntimeError otherwise, with the library's
+    message (``last_error``: its getter, the product library's srl_last_error by default)"""
     if rc != 0:
-        msg = lib().srl_last_error().decode()
+        msg = (last_error or lib().srl_last_error)().decode()
         if rc == -1:
             raise ValueError(f'{what}: {msg}')
         raise RuntimeError(f'{what}: rc={rc}: {msg}')
+
+
+def check_hook(rc, what=''):
+    """check() for the test-hook library"""
+    check(rc, what, hooks().srl_test_last_error)
 
 
 def param_layout(A, use_lstm=False):

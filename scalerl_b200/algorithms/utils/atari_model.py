@@ -137,7 +137,7 @@ class ActorNet(torch.nn.Module):
 
 PRECISIONS = {'bf16': 0, 'fp32_split': 1}     # ImpalaHParams.precision -> srl_config_t.precision
 MAX_ACTIONS = 31                             # one warp lane per action plus one for the baseline, as B200ImpalaLearner
-MAX_FRAMES = 65536                           # T * B of one call
+MAX_FRAMES = 65536                           # T * B of one call (MAX_FRAMES in csrc/kernels.h)
 LSTM_WEIGHTS = tuple(f'{w}_l{l}' for l in (0, 1) for w in ('weight_ih', 'weight_hh', 'bias_ih', 'bias_hh'))   # srl_lstm_create order
 
 
@@ -229,16 +229,10 @@ class _EncoderCore(torch.autograd.Function):
         return (None,) * 6 + tuple(grads)
 
 
-def _lstm_check(rc, what):
-    if rc != 0:
-        msg = _lib.lib().srl_lstm_last_error().decode()
-        raise (ValueError if rc == -1 else RuntimeError)(f'{what}: {msg}')
-
-
 def lstm_block_sizes(T1: int, B: int, num_actions: int):
     """(bytes an LSTM core forward keeps for its backward, bytes of one call's scratch) for T1 x B rows"""
     saved, scratch = C.c_int64(), C.c_int64()
-    _lstm_check(_lib.lib().srl_lstm_core_sizes(int(T1), int(B), int(num_actions), C.byref(saved), C.byref(scratch)), 'srl_lstm_core_sizes')
+    _lib.check(_lib.lib().srl_lstm_core_sizes(int(T1), int(B), int(num_actions), C.byref(saved), C.byref(scratch)), 'srl_lstm_core_sizes')
     return saved.value, scratch.value
 
 
@@ -251,9 +245,9 @@ def _lstm_forward(num_actions, core, done, h0, c0, weights):
     scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev)
     out = torch.empty(T1, B, H, dtype=torch.float32, device=dev)
     hT, cT = (torch.empty(2, B, H, dtype=torch.float32, device=dev) for _ in range(2))
-    _lstm_check(_lib.lib().srl_lstm_core_forward(core.data_ptr(), done.data_ptr(), h0.data_ptr(), c0.data_ptr(), num_actions, T1, B,
-                                                 _ptrs8(weights), saved.data_ptr(), scratch.data_ptr(), out.data_ptr(), hT.data_ptr(),
-                                                 cT.data_ptr(), torch.cuda.current_stream(dev).cuda_stream), 'srl_lstm_core_forward')
+    _lib.check(_lib.lib().srl_lstm_core_forward(core.data_ptr(), done.data_ptr(), h0.data_ptr(), c0.data_ptr(), num_actions, T1, B,
+                                                _ptrs8(weights), saved.data_ptr(), scratch.data_ptr(), out.data_ptr(), hT.data_ptr(),
+                                                cT.data_ptr(), torch.cuda.current_stream(dev).cuda_stream), 'srl_lstm_core_forward')
     return out, hT, cT, saved
 
 
@@ -289,9 +283,9 @@ class _LstmCore(torch.autograd.Function):
         dc0 = torch.empty(2, B, H, device=dev) if want_c0 else None
         grads = [torch.empty(s, dtype=torch.float32, device=dev) for s in shapes]
         scratch = torch.empty(lstm_block_sizes(T1, B, num_actions)[1], dtype=torch.uint8, device=dev)
-        _lstm_check(_lib.lib().srl_lstm_core_backward(dout.data_ptr(), _ptr_or_none(dhT), _ptr_or_none(dcT), num_actions, T1, B, saved.data_ptr(),
-                                                      scratch.data_ptr(), _ptrs8(grads), dcore.data_ptr(), _ptr_or_none(dh0), _ptr_or_none(dc0),
-                                                      torch.cuda.current_stream(dev).cuda_stream), 'srl_lstm_core_backward')
+        _lib.check(_lib.lib().srl_lstm_core_backward(dout.data_ptr(), _ptr_or_none(dhT), _ptr_or_none(dcT), num_actions, T1, B, saved.data_ptr(),
+                                                     scratch.data_ptr(), _ptrs8(grads), dcore.data_ptr(), _ptr_or_none(dh0), _ptr_or_none(dc0),
+                                                     torch.cuda.current_stream(dev).cuda_stream), 'srl_lstm_core_backward')
         return (None, dcore if ctx.needs_input_grad[1] else None, None, dh0, dc0) + tuple(grads)
 
 

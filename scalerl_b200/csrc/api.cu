@@ -1,33 +1,16 @@
 // extern "C" entry points (include/scalerl_b200.h).  Argument checking + the learner context that owns
 // the activation workspaces and sequences the kernels of one learner step on the caller's stream.
-#include <stdio.h>
 #include <string.h>
-#include <stdarg.h>
 #include <cmath>
 #include <new>
 
 #include "../../include/scalerl_b200.h"
+#include "errors.h"
 #include "kernels.h"
 
 using namespace srl;
 
-static thread_local char g_err[512] = "";
-
-static int fail(int code, const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_err, sizeof(g_err), fmt, ap);
-  va_end(ap);
-  return code;
-}
-static int cuda_fail(cudaError_t e, const char* what) {
-  snprintf(g_err, sizeof(g_err), "%s: %s (%s)", what, cudaGetErrorName(e), cudaGetErrorString(e));
-  return (int)e;
-}
-#define CU(x, what) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return cuda_fail(e_, what); } while (0)
-#define REQ(c, ...) do { if (!(c)) return fail(SRL_EINVAL, __VA_ARGS__); } while (0)
-
-extern "C" const char* srl_last_error(void) { return g_err; }
+extern "C" const char* srl_last_error(void) { return error_message(); }
 extern "C" int srl_version(void) { return 100; }
 
 // ------------------------------------------------------------------------------------------------
@@ -115,8 +98,8 @@ extern "C" int srl_unpack_slots(const uint8_t* staging, int64_t slot_bytes, cons
                                 float* reward, uint8_t* done, int64_t* action, float* policy_logits, float* episode_return, void* stream) {
   REQ(staging && offsets6_host && obs && reward && done && action && policy_logits, "unpack_slots: NULL pointer");
   REQ(T >= 1 && B >= 1 && A >= 1 && A <= 32 && slot_bytes > 0, "unpack_slots: bad shape");
-  REQ((slot_bytes & 15) == 0 && (offsets6_host[0] & 15) == 0 && (reinterpret_cast<uintptr_t>(staging) & 15) == 0 &&
-      (reinterpret_cast<uintptr_t>(obs) & 15) == 0, "unpack_slots: obs record and buffers must be 16-byte aligned");
+  REQ((slot_bytes & 15) == 0 && (offsets6_host[0] & 15) == 0 && !misaligned(staging, 16) && !misaligned(obs, 16),
+      "unpack_slots: obs record and buffers must be 16-byte aligned");
   CU(launch_unpack_slots(staging, slot_bytes, offsets6_host, T, B, A, obs, reward, done, action, policy_logits, episode_return,
                          (cudaStream_t)stream), "unpack_slots");
   return 0;
@@ -124,15 +107,14 @@ extern "C" int srl_unpack_slots(const uint8_t* staging, int64_t slot_bytes, cons
 
 extern "C" int srl_grad_norm_clip_coef(const float* grads, int64_t n, float max_norm, float* coef, float* scratch, void* stream) {
   REQ(grads && coef && scratch && n >= 0, "grad_norm: bad argument");
-  REQ((reinterpret_cast<uintptr_t>(grads) & 15) == 0, "grad_norm: grads must be 16-byte aligned");
+  REQ(!misaligned(grads, 16), "grad_norm: grads must be 16-byte aligned");
   CU(launch_grad_norm(grads, n, max_norm, coef, scratch, (cudaStream_t)stream), "grad_norm");
   return 0;
 }
 extern "C" int srl_rmsprop_step(float* params, const float* grads, float* square_avg, int64_t n, const float* coef, float lr, float alpha,
                                 float eps, void* stream) {
   REQ(params && grads && square_avg && n >= 0, "rmsprop: bad argument");
-  REQ(((reinterpret_cast<uintptr_t>(params) | reinterpret_cast<uintptr_t>(grads) | reinterpret_cast<uintptr_t>(square_avg)) & 15) == 0,
-      "rmsprop: buffers must be 16-byte aligned");
+  REQ(!misaligned(params, 16) && !misaligned(grads, 16) && !misaligned(square_avg, 16), "rmsprop: buffers must be 16-byte aligned");
   CU(launch_rmsprop(params, grads, square_avg, n, coef, lr, alpha, eps, (cudaStream_t)stream), "rmsprop");
   return 0;
 }
@@ -224,7 +206,7 @@ static int check_cfg(const srl_config_t* c) {
   REQ(c, "config is NULL");
   REQ(c->T >= 1 && c->B >= 1, "config: T=%d B=%d must be >= 1", c->T, c->B);
   REQ(c->A >= 1 && c->A <= 31, "config: A=%d must be in [1,31] (one warp lane per action plus one for the baseline)", c->A);
-  REQ((int64_t)(c->T + 1) * c->B <= 65536, "config: (T+1)*B=%lld frames per GPU exceeds 65536", (long long)(c->T + 1) * c->B);
+  REQ((int64_t)(c->T + 1) * c->B <= MAX_FRAMES, "config: (T+1)*B=%lld frames per GPU exceeds %d", (long long)(c->T + 1) * c->B, MAX_FRAMES);
   REQ(c->optimizer == 0 || c->optimizer == 1, "config: optimizer must be 0 (rmsprop) or 1 (adam)");
   REQ(c->use_lstm == 0 || c->use_lstm == 1, "config: use_lstm must be 0 or 1");
   REQ(c->precision == 0 || c->precision == 1, "config: precision must be 0 (bf16 operands) or 1 (fp32-accurate split operands)");
@@ -309,8 +291,8 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
   if (rc) return rc;
   REQ(params && grads && opt0 && out, "learner_create: NULL buffer");
   REQ(cfg->optimizer == 0 || opt1, "learner_create: Adam needs opt_state1");
-  REQ(((reinterpret_cast<uintptr_t>(params) | reinterpret_cast<uintptr_t>(grads) | reinterpret_cast<uintptr_t>(opt0) |
-        reinterpret_cast<uintptr_t>(opt1)) & 15) == 0, "learner_create: flat buffers must be 16-byte aligned");
+  REQ(!misaligned(params, 16) && !misaligned(grads, 16) && !misaligned(opt0, 16) && !misaligned(opt1, 16),
+      "learner_create: flat buffers must be 16-byte aligned");
   srl_learner* L = new (std::nothrow) srl_learner();      // value-initialised: srl_learner_destroy can release any partial context
   REQ(L, "out of host memory");
   auto undo = [L](int code) { srl_learner_destroy(L); return code; };      // the error message is written before the release
@@ -345,9 +327,8 @@ extern "C" int srl_learner_create(const srl_config_t* cfg, float* params, float*
     const float* wp[8]; float* gp[8];
     for (int i = 0; i < 8; ++i) { wp[i] = params + off[12 + i]; gp[i] = grads + off[12 + i]; }
     L->lstm_off0 = off[12]; L->lstm_len = L->nparams - off[12];
-    why = srl_lstm_last_error();
-    if (srl_lstm_create(cfg->T + 1, cfg->B, H, wp, gp, &L->lstm) != 0 || lstm_step_create(cfg->B, H, wp, &L->lstm_step, &why) != cudaSuccess)
-      return undo(fail(SRL_ESTATE, "learner_create: LSTM core allocation failed: %s", why));
+    // the callee's message stays in place
+    if (srl_lstm_create(cfg->T + 1, cfg->B, H, wp, gp, &L->lstm) != 0 || lstm_step_create(cfg->B, H, wp, &L->lstm_step) != 0) return undo(SRL_ESTATE);
   }
   *out = L;
   return 0;
@@ -416,7 +397,7 @@ extern "C" int srl_learner_set_momentum(srl_learner_t* L, float momentum, float*
   REQ(momentum >= 0.f && std::isfinite(momentum), "set_momentum: momentum=%g must be finite and >= 0", (double)momentum);
   REQ(momentum == 0.f || L->cfg.optimizer == 0, "set_momentum: momentum is an RMSprop option; this learner runs Adam");
   REQ(momentum == 0.f || momentum_buf, "set_momentum: momentum=%g needs a momentum buffer", (double)momentum);
-  REQ((reinterpret_cast<uintptr_t>(momentum_buf) & 15) == 0, "set_momentum: the momentum buffer must be 16-byte aligned");
+  REQ(!misaligned(momentum_buf, 16), "set_momentum: the momentum buffer must be 16-byte aligned");
   L->ox.momentum = momentum;
   L->ox.buf = momentum == 0.f ? nullptr : momentum_buf;
   return 0;
@@ -510,7 +491,7 @@ extern "C" int srl_learner_forward(srl_learner_t* L, const uint8_t* obs, const f
                                    float* policy_logits, float* baseline, void* stream) {
   REQ(L && obs && reward && action && policy_logits && baseline, "learner_forward: NULL pointer");
   REQ(rows >= 1 && rows <= L->cfg.T + 1, "learner_forward: rows=%d must be in [1, T+1=%d]", rows, L->cfg.T + 1);
-  REQ((reinterpret_cast<uintptr_t>(obs) & 3) == 0, "learner_forward: obs must be 4-byte aligned");
+  REQ(!misaligned(obs, 4), "learner_forward: obs must be 4-byte aligned");
   L->S.begin_call((cudaStream_t)stream);
   return forward_impl(L, obs, reward, action, rows * L->cfg.B, policy_logits, baseline);
 }
@@ -553,7 +534,7 @@ extern "C" int srl_learner_forward_backward(srl_learner_t* L, const uint8_t* obs
                                             const int64_t* action, const float* behavior_logits, float* losses, float* vs,
                                             float* pg_advantages, void* stream) {
   REQ(L && obs && reward && done && action && behavior_logits && losses, "learner_forward_backward: NULL pointer");
-  REQ((reinterpret_cast<uintptr_t>(obs) & 3) == 0, "learner_forward_backward: obs must be 4-byte aligned");
+  REQ(!misaligned(obs, 4), "learner_forward_backward: obs must be 4-byte aligned");
   L->S.begin_call((cudaStream_t)stream);
   return fb_begin(L, obs, reward, done, action, behavior_logits, losses, vs, pg_advantages, BWD_BOTH);
 }
@@ -562,7 +543,7 @@ extern "C" int srl_learner_forward_backward_begin(srl_learner_t* L, const uint8_
                                                   const int64_t* action, const float* behavior_logits, float* losses, float* vs,
                                                   float* pg_advantages, void* stream) {
   REQ(L && obs && reward && done && action && behavior_logits && losses, "learner_forward_backward_begin: NULL pointer");
-  REQ((reinterpret_cast<uintptr_t>(obs) & 3) == 0, "learner_forward_backward_begin: obs must be 4-byte aligned");
+  REQ(!misaligned(obs, 4), "learner_forward_backward_begin: obs must be 4-byte aligned");
   L->S.begin_call((cudaStream_t)stream);
   return fb_begin(L, obs, reward, done, action, behavior_logits, losses, vs, pg_advantages, BWD_FC);
 }
@@ -586,7 +567,7 @@ static int forward_lstm_impl(srl_learner* L, const uint8_t* obs, const float* re
   if (rc) return rc;
   CU(launch_core_build(L->buf.hpart, FC_SPLITS, L->P.bf, reward, action, NF, c.A, L->buf.h, L->core, st), "core_build");
   rc = srl_lstm_forward(L->lstm, L->core, done, h0, c0, L->lstm_out, hT, cT, st);
-  if (rc) return fail(rc, "lstm_forward: %s", srl_lstm_last_error());
+  if (rc) return rc;
   CU(launch_head_dense_fwd(L->lstm_out, L->P.wp, L->P.bp, L->P.wb, L->P.bb, NF, c.A, logits, baseline, st), "head_dense_fwd");
   return 0;
 }
@@ -598,12 +579,6 @@ extern "C" int srl_learner_forward_lstm(srl_learner_t* L, const uint8_t* obs, co
   L->S.begin_call((cudaStream_t)stream);
   return forward_lstm_impl(L, obs, reward, done, action, h0, c0, policy_logits, baseline, hT, cT);
 }
-
-static bool overlaps(const void* a, int64_t a_bytes, const void* b, int64_t b_bytes) {
-  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
-  return x < y + (uintptr_t)b_bytes && y < x + (uintptr_t)a_bytes;
-}
-static bool overlaps(const void* a, const void* b, int64_t bytes) { return overlaps(a, bytes, b, bytes); }
 
 extern "C" int srl_learner_forward_lstm_step(srl_learner_t* L, const uint8_t* obs, const float* reward, const uint8_t* done,
                                              const int64_t* action, const float* h_in, const float* c_in, float* policy_logits,
@@ -618,11 +593,12 @@ extern "C" int srl_learner_forward_lstm_step(srl_learner_t* L, const uint8_t* ob
   const srl_config_t& c = L->cfg;
   const int B = c.B, H = 513 + c.A;
   const int64_t sb = (int64_t)2 * B * H * 4;
-  REQ(!overlaps(h_out, h_in, sb) && !overlaps(h_out, c_in, sb) && !overlaps(c_out, h_in, sb) && !overlaps(c_out, c_in, sb) &&
-      !overlaps(h_out, c_out, sb), "learner_forward_lstm_step: h_out / c_out must not alias h_in, c_in or each other");
-  REQ((reinterpret_cast<uintptr_t>(obs) & 3) == 0, "learner_forward_lstm_step: obs must be 4-byte aligned");
+  const Span s[4] = {{h_in, sb, false, "h_in"}, {c_in, sb, false, "c_in"}, {h_out, sb, true, "h_out"}, {c_out, sb, true, "c_out"}};
+  int rc = check_spans(s, 4, "learner_forward_lstm_step");
+  if (rc) return rc;
+  REQ(!misaligned(obs, 4), "learner_forward_lstm_step: obs must be 4-byte aligned");
   const cudaStream_t st = L->S.begin_call((cudaStream_t)stream);
-  int rc = encode_impl(L, obs, B);
+  rc = encode_impl(L, obs, B);
   if (rc) return rc;
   CU(launch_core_build(L->buf.hpart, FC_SPLITS, L->P.bf, reward, action, B, c.A, L->buf.h, L->core, st), "core_build");
   CU(lstm_step_forward(L->lstm_step, L->core, done, h_in, c_in, h_out, c_out, L->lstm_step_ksplit, st), "lstm_step");
@@ -646,7 +622,7 @@ extern "C" int srl_learner_forward_backward_lstm(srl_learner_t* L, const uint8_t
   CU(launch_head_dense_bwd(L->lstm_out, L->dlogits, L->dbaseline, L->P.wp, L->P.wb, NB, c.A, L->dout, L->G.wp, L->G.bp, L->G.wb, L->G.bb, st),
      "head_dense_bwd");
   rc = srl_lstm_backward(L->lstm, L->dout, done, L->dcore, st);
-  if (rc) return fail(rc, "lstm_backward: %s", srl_lstm_last_error());
+  if (rc) return rc;
   CU(launch_dcore_to_dh(L->dcore, L->buf.h, NB, c.A, L->buf.hi.dh, st), "dcore_to_dh");
   CU(encoder_backward(NB, L->buf, L->G, L->maps, c.precision, L->S, BWD_BOTH, false), "encoder_backward");
   L->have_fwd = true;
@@ -716,7 +692,7 @@ extern "C" int srl_learner_profile_collect(srl_learner_t* L, float* ms_out_host)
 
 extern "C" int srl_learner_snapshot_params(srl_learner_t* L, float* dst, const float* losses, void* stream) {
   REQ(L && dst, "snapshot_params: NULL argument");
-  REQ((reinterpret_cast<uintptr_t>(dst) & 15) == 0, "snapshot_params: dst must be 16-byte aligned");
+  REQ(!misaligned(dst, 16), "snapshot_params: dst must be 16-byte aligned");
   CU(launch_snapshot_if_finite(dst, L->params, L->nparams, losses, (cudaStream_t)stream), "snapshot_params");
   return 0;
 }
@@ -784,8 +760,6 @@ struct srl_encoder {
   StepStreams S;                  // the lanes beside the caller's stream (no per-kernel profiling)
 };
 
-constexpr int ENC_MAX_FRAMES = 65536;
-
 static int check_precision(int precision, const char* what) {
   REQ(precision == 0 || precision == 1, "%s: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", what, precision);
   return 0;
@@ -812,45 +786,33 @@ extern "C" int srl_encoder_destroy(srl_encoder_t* E) {
 
 extern "C" int srl_encoder_sizes(int frames, int precision, int64_t* saved_bytes, int64_t* scratch_bytes) {
   REQ(saved_bytes && scratch_bytes, "encoder_sizes: NULL argument");
-  REQ(frames >= 1 && frames <= ENC_MAX_FRAMES, "encoder_sizes: frames=%d must be in [1, %d]", frames, ENC_MAX_FRAMES);
+  REQ(frames >= 1 && frames <= MAX_FRAMES, "encoder_sizes: frames=%d must be in [1, %d]", frames, MAX_FRAMES);
   int rc = check_precision(precision, "encoder_sizes");
   if (rc) return rc;
   EncoderBuffers b = {};
   WsRow t[ENC_ROWS];
   encoder_rows(b, frames, frames, t);
-  *saved_bytes = rows_bytes(t, ENC_SAVED_ROWS, precision == 1);
-  *scratch_bytes = rows_bytes(t + ENC_SAVED_ROWS, ENC_ROWS - ENC_SAVED_ROWS, precision == 1);
+  block_bytes(t, ENC_ROWS, ENC_SAVED_ROWS, precision == 1, saved_bytes, scratch_bytes);
   return 0;
 }
 
-static bool misaligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
-
-// the argument checks both calls share: shape, the two blocks' alignment, and that neither block overlaps the other
+// the argument checks both calls share: shape, the two blocks' alignment and sizes
 static int check_encoder_call(const srl_encoder* E, int frames, int A, const void* saved, const void* scratch, int64_t* sb, int64_t* kb,
                               const char* what) {
-  REQ(frames >= 1 && frames <= ENC_MAX_FRAMES, "%s: frames=%d must be in [1, %d]", what, frames, ENC_MAX_FRAMES);
+  REQ(frames >= 1 && frames <= MAX_FRAMES, "%s: frames=%d must be in [1, %d]", what, frames, MAX_FRAMES);
   REQ(A >= 1 && A <= 31, "%s: A=%d must be in [1,31]", what, A);
   REQ(!misaligned(saved, 256) && !misaligned(scratch, 256), "%s: saved and scratch must be 256-byte aligned", what);
-  srl_encoder_sizes(frames, E->precision, sb, kb);
-  REQ(!overlaps(saved, *sb, scratch, *kb), "%s: saved and scratch overlap", what);
-  return 0;
+  return srl_encoder_sizes(frames, E->precision, sb, kb);
 }
 
 // the blocks of one call -> the encoder buffers and their tensor maps, encoded on the host for this call (legal under stream capture)
 static int encoder_call_setup(const srl_encoder* E, int frames, void* saved, void* scratch, EncoderBuffers* b, TmaMaps* maps,
                               const char* what) {
-  const bool split = E->precision == 1;
   WsRow t[ENC_ROWS];
   *b = EncoderBuffers{};
   encoder_rows(*b, frames, frames, t);
-  carve_rows(t, ENC_SAVED_ROWS, split, static_cast<char*>(saved));
-  carve_rows(t + ENC_SAVED_ROWS, ENC_ROWS - ENC_SAVED_ROWS, split, static_cast<char*>(scratch));
   b->NF = frames;
-  // encoding needs the device's context current on this thread, and this may be the thread's first CUDA call (torch runs a backward
-  // on an autograd thread of its own): cudaSetDevice makes the primary context current
-  int dev = 0;
-  CU(cudaGetDevice(&dev), "cudaGetDevice");
-  CU(cudaSetDevice(dev), "cudaSetDevice");
+  CU(carve_blocks(t, ENC_ROWS, ENC_SAVED_ROWS, E->precision == 1, saved, scratch), "cudaSetDevice");
   const char* why = nullptr;
   if (build_tma_maps(*b, frames, frames, maps, &why) != cudaSuccess)
     return fail(SRL_ESTATE, "%s: building TMA tensor map '%s' failed (driver without cuTensorMapEncodeTiled?)", what, why ? why : "?");
@@ -865,20 +827,16 @@ extern "C" int srl_encoder_forward(srl_encoder_t* E, const uint8_t* obs, const f
   int rc = check_encoder_call(E, frames, A, saved, scratch, &sb, &kb, "encoder_forward");
   if (rc) return rc;
   REQ(!misaligned(obs, 4), "encoder_forward: obs must be 4-byte aligned");
+  for (int i = 0; i < 8; ++i) REQ(!misaligned(weights8[i], 16), "encoder_forward: weights8[%d] must be 16-byte aligned", i);
   int64_t cnt[12];
   layout(A, nullptr, cnt);
-  const int64_t core_bytes = (int64_t)frames * (513 + A) * 4;
-  for (int i = 0; i < 8; ++i) {
-    REQ(!misaligned(weights8[i], 16), "encoder_forward: weights8[%d] must be 16-byte aligned", i);
-    REQ(!overlaps(weights8[i], cnt[i] * 4, saved, sb) && !overlaps(weights8[i], cnt[i] * 4, scratch, kb) &&
-        !overlaps(weights8[i], cnt[i] * 4, core_out, core_bytes), "encoder_forward: weights8[%d] overlaps an output", i);
-  }
-  const void* in[3] = {obs, reward, action};
-  const int64_t in_bytes[3] = {(int64_t)frames * 28224, (int64_t)frames * 4, (int64_t)frames * 8};
-  for (int i = 0; i < 3; ++i)
-    REQ(!overlaps(in[i], in_bytes[i], saved, sb) && !overlaps(in[i], in_bytes[i], scratch, kb) && !overlaps(in[i], in_bytes[i], core_out, core_bytes),
-        "encoder_forward: an output overlaps obs, reward or action");
-  REQ(!overlaps(core_out, core_bytes, saved, sb) && !overlaps(core_out, core_bytes, scratch, kb), "encoder_forward: core_out overlaps saved or scratch");
+  Span s[14] = {{obs, (int64_t)frames * 28224, false, "obs"}, {reward, (int64_t)frames * 4, false, "reward"},
+                {action, (int64_t)frames * 8, false, "action"}};
+  int n = 3;
+  for (int i = 0; i < 8; ++i) s[n++] = {weights8[i], cnt[i] * 4, false, kW8[i]};
+  s[n++] = {saved, sb, true, "saved"}; s[n++] = {scratch, kb, true, "scratch"}; s[n++] = {core_out, (int64_t)frames * (513 + A) * 4, true, "core_out"};
+  rc = check_spans(s, n, "encoder_forward");
+  if (rc) return rc;
   ParamPtrs P = {};
   P.w1 = const_cast<float*>(weights8[0]); P.b1 = const_cast<float*>(weights8[1]); P.w2 = const_cast<float*>(weights8[2]);
   P.b2 = const_cast<float*>(weights8[3]); P.w3 = const_cast<float*>(weights8[4]); P.b3 = const_cast<float*>(weights8[5]);
@@ -904,17 +862,14 @@ extern "C" int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int fr
   int64_t sb = 0, kb = 0;
   int rc = check_encoder_call(E, frames, A, saved, scratch, &sb, &kb, "encoder_backward");
   if (rc) return rc;
+  for (int i = 0; i < 8; ++i) REQ(!misaligned(grads8[i], 16), "encoder_backward: grads8[%d] must be 16-byte aligned", i);
   int64_t cnt[12];
   layout(A, nullptr, cnt);
-  const int64_t dcore_bytes = (int64_t)frames * (513 + A) * 4;
-  REQ(!overlaps(dcore, dcore_bytes, scratch, kb), "encoder_backward: dcore overlaps scratch");
-  for (int i = 0; i < 8; ++i) {
-    REQ(!misaligned(grads8[i], 16), "encoder_backward: grads8[%d] must be 16-byte aligned", i);
-    const int64_t gb = cnt[i] * 4;
-    REQ(!overlaps(grads8[i], gb, saved, sb) && !overlaps(grads8[i], gb, scratch, kb) && !overlaps(grads8[i], gb, dcore, dcore_bytes),
-        "encoder_backward: grads8[%d] overlaps dcore, saved or scratch", i);
-    for (int j = 0; j < i; ++j) REQ(!overlaps(grads8[i], gb, grads8[j], cnt[j] * 4), "encoder_backward: grads8[%d] overlaps grads8[%d]", i, j);
-  }
+  Span s[11] = {{dcore, (int64_t)frames * (513 + A) * 4, false, "dcore"}, {saved, sb, false, "saved"}, {scratch, kb, true, "scratch"}};
+  int n = 3;
+  for (int i = 0; i < 8; ++i) s[n++] = {grads8[i], cnt[i] * 4, true, kG8[i]};
+  rc = check_spans(s, n, "encoder_backward");
+  if (rc) return rc;
   ParamPtrs G = {};
   G.w1 = grads8[0]; G.b1 = grads8[1]; G.w2 = grads8[2]; G.b2 = grads8[3]; G.w3 = grads8[4]; G.b3 = grads8[5]; G.wf = grads8[6]; G.bf = grads8[7];
   EncoderBuffers b;

@@ -108,6 +108,23 @@ inline void carve_rows(const WsRow* t, int n, bool split, char* q) {
     if (split && t[i].lo) { *t[i].lo = q; q += ws_bytes(t[i]); }
   }
 }
+// The two caller-owned blocks of the stand-alone encoder and LSTM core calls: rows [0, n_saved) of a table form the saved block (what
+// a backward reads of its forward), rows [n_saved, n) the scratch block (one call's temporaries).
+inline void block_bytes(const WsRow* t, int n, int n_saved, bool split, int64_t* saved, int64_t* scratch) {
+  *saved = rows_bytes(t, n_saved, split);
+  *scratch = rows_bytes(t + n_saved, n - n_saved, split);
+}
+// carves both blocks, then makes the device's primary context current on this thread: encoding the call's tensor maps needs it, and
+// this may be the thread's first CUDA call (torch runs a backward on an autograd thread of its own)
+inline cudaError_t carve_blocks(const WsRow* t, int n, int n_saved, bool split, void* saved, void* scratch) {
+  carve_rows(t, n_saved, split, static_cast<char*>(saved));
+  carve_rows(t + n_saved, n - n_saved, split, static_cast<char*>(scratch));
+  int dev = 0;
+  const cudaError_t e = cudaGetDevice(&dev);
+  return e != cudaSuccess ? e : cudaSetDevice(dev);
+}
+// most frames of one call: (T+1)*B of a learner context, the stand-alone encoder's frames, the stand-alone LSTM core's T1*B rows
+constexpr int MAX_FRAMES = 65536;
 
 // per-CTA partials of the wgrad kernels (each CTA stores its accumulators, in the kernel's native [tap-block][row][co] order, and its
 // bias sums; conv_wgrad_reduce_kernel<layer> adds the CTAs in a fixed order into the PyTorch-layout gradient, so the gradients are the
@@ -265,8 +282,9 @@ cudaError_t encoder_backward(int frames, const EncoderBuffers& buf, const ParamP
                              const StepStreams& S, BwdParts parts, bool a3t_done);
 // ---- lstm.cu: the actor step of the 2-layer LSTM core (one row of B environments, no BPTT)
 struct LstmStep;
-// weights8: the 8 nn.LSTM tensors of the flat parameter buffer (srl_lstm_create order); H = 513 + A
-cudaError_t lstm_step_create(int B, int H, const float* const* weights8, LstmStep** out, const char** why);
+// weights8: the 8 nn.LSTM tensors of the flat parameter buffer (srl_lstm_create order); H = 513 + A.  0, or an error code with the
+// message set (errors.h)
+int lstm_step_create(int B, int H, const float* const* weights8, LstmStep** out);
 void lstm_step_destroy(LstmStep* S);
 cudaError_t lstm_step_pack(LstmStep* S, cudaStream_t st);           // packed [W_ih | W_hh] bf16 copy of both layers from the fp32 parameters
 bool lstm_step_ksplit_supported(int ks);                            // K split (cluster size) of the step GEMM: 1, 2, 3 or 6

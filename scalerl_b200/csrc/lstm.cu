@@ -13,10 +13,10 @@
 // H = 513 + A is padded to Hp (multiple of 64); the gate dimension is laid out [4][Hp] so every GEMM has K = Hp or 4Hp.
 // All GEMM operands are bf16 (fp32 accumulate); cell state, gate activations and gradients are fp32.
 // The actor's single step (one row of B environments, no BPTT) has its own fused kernel further down (lstm_step_kernel).
-#include <stdio.h>
 #include <new>
 #include "tma_problems.cuh"
 #include "kernels.h"
+#include "errors.h"
 #include "../../include/scalerl_b200.h"
 
 namespace srl {
@@ -402,10 +402,7 @@ __global__ void lstm_step_pack_kernel(const float* __restrict__ wih0, const floa
 using namespace srl;
 
 // ------------------------------------------------------------------------------------------------ buffers
-static thread_local char g_lerr[256] = "";
-extern "C" const char* srl_lstm_last_error(void) { return g_lerr; }
-#define LCU(x, what) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { snprintf(g_lerr, sizeof(g_lerr), "%s: %s", what, cudaGetErrorString(e_)); return (int)e_; } } while (0)
-#define LREQ(c, ...) do { if (!(c)) { snprintf(g_lerr, sizeof(g_lerr), __VA_ARGS__); return SRL_EINVAL; } } while (0)
+extern "C" const char* srl_lstm_last_error(void) { return srl_last_error(); }
 
 namespace srl {
 // shape of one forward over N1 = T1*B rows and its backward over the first NB rows (T*B for the learner, T1*B for the stand-alone core)
@@ -494,31 +491,31 @@ static int lstm_forward_rows(const LstmDims& d, const LstmBuffers& b, const Lstm
     lstm_pack_w_kernel<<<cdiv_((int64_t)G * Hp, 256), 256, 0, st>>>(w8[4 * l], H, Hp, b.Wih[l], b.WihT[l]);
     lstm_pack_w_kernel<<<cdiv_((int64_t)G * Hp, 256), 256, 0, st>>>(w8[4 * l + 1], H, Hp, b.Whh[l], b.WhhT[l]);
   }
-  LCU(cudaGetLastError(), "lstm pack");
+  CU(cudaGetLastError(), "lstm pack");
   const int cell_blocks = cdiv_((int64_t)B * Hp, 256);
   for (int l = 0; l < 2; ++l) {
     // padded copy of this layer's initial cell state
-    LCU(cudaMemcpy2DAsync(b.c_init + (size_t)l * B * Hp, Hp * 4, c0 + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "c0 copy");
+    CU(cudaMemcpy2DAsync(b.c_init + (size_t)l * B * Hp, Hp * 4, c0 + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "c0 copy");
     lstm_init_hm_kernel<<<cell_blocks, 256, 0, st>>>(h0 + (size_t)l * B * H, done, B, H, Hp, b.hm[l]);
     { LGemmK::Params q{m.xin[l], m.Wih[l], b.gx, (int)N1, Hp / 64, G, 0, 0};      // input projection of every step
-      LCU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(N1, 128), G / 64), st), "lstm gx gemm"); }
+      CU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(N1, 128), G / 64), st), "lstm gx gemm"); }
     for (int t = 0; t < T1; ++t) {
       { LGemmK::Params q{m.hm[l], m.Whh[l], b.r, B, Hp / 64, G, t * B, 0};
-        LCU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(B, 128), G / 64), st), "lstm recurrent gemm"); }
+        CU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(B, 128), G / 64), st), "lstm recurrent gemm"); }
       const float* cprev = t == 0 ? b.c_init + (size_t)l * B * Hp : b.cseq[l] + (size_t)(t - 1) * B * Hp;
       lstm_cell_fwd_kernel<<<cell_blocks, 256, 0, st>>>(
           b.gx + (size_t)t * B * G, b.r, w8[4 * l + 2], w8[4 * l + 3], cprev, done + (size_t)t * B, t + 1 < T1 ? done + (size_t)(t + 1) * B : nullptr, B,
           H, Hp, b.gates[l] + (size_t)t * B * G, b.cseq[l] + (size_t)t * B * Hp, b.hseq[l] + (size_t)t * B * Hp, b.hbf[l] + (size_t)t * B * Hp,
           t + 1 < T1 ? b.hm[l] + (size_t)(t + 1) * B * Hp : nullptr);
     }
-    LCU(cudaGetLastError(), "lstm cell");
+    CU(cudaGetLastError(), "lstm cell");
   }
   lstm_unpad_rows_kernel<<<cdiv_(N1 * H, 256), 256, 0, st>>>(b.hseq[1], (int)N1, H, Hp, out);
   for (int l = 0; l < 2; ++l) {
-    if (hT) LCU(cudaMemcpy2DAsync(hT + (size_t)l * B * H, H * 4, b.hseq[l] + (size_t)(T1 - 1) * B * Hp, Hp * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "hT");
-    if (cT) LCU(cudaMemcpy2DAsync(cT + (size_t)l * B * H, H * 4, b.cseq[l] + (size_t)(T1 - 1) * B * Hp, Hp * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "cT");
+    if (hT) CU(cudaMemcpy2DAsync(hT + (size_t)l * B * H, H * 4, b.hseq[l] + (size_t)(T1 - 1) * B * Hp, Hp * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "hT");
+    if (cT) CU(cudaMemcpy2DAsync(cT + (size_t)l * B * H, H * 4, b.cseq[l] + (size_t)(T1 - 1) * B * Hp, Hp * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "cT");
   }
-  LCU(cudaGetLastError(), "lstm forward");
+  CU(cudaGetLastError(), "lstm forward");
   return 0;
 }
 
@@ -532,12 +529,12 @@ static int lstm_backward_rows(const LstmDims& d, const LstmBuffers& b, const Lst
   const int steps = (int)(NB / B);
   const int cell_blocks = cdiv_((int64_t)B * Hp, 256);
   // dh_out of the top layer, padded to Hp (dx is the padded buffer)
-  LCU(cudaMemsetAsync(b.dx, 0, NB * Hp * 4, st), "zero dx");
-  LCU(cudaMemcpy2DAsync(b.dx, Hp * 4, dout, H * 4, H * 4, NB, cudaMemcpyDeviceToDevice, st), "pad dout");
+  CU(cudaMemsetAsync(b.dx, 0, NB * Hp * 4, st), "zero dx");
+  CU(cudaMemcpy2DAsync(b.dx, Hp * 4, dout, H * 4, H * 4, NB, cudaMemcpyDeviceToDevice, st), "pad dout");
   for (int l = 1; l >= 0; --l) {
-    if (dcT) LCU(cudaMemcpy2DAsync(b.dc, Hp * 4, dcT + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "dcT copy");
-    else LCU(cudaMemsetAsync(b.dc, 0, (size_t)B * Hp * 4, st), "zero dc");
-    if (dhT) LCU(cudaMemcpy2DAsync(b.dhm, Hp * 4, dhT + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "dhT copy");
+    if (dcT) CU(cudaMemcpy2DAsync(b.dc, Hp * 4, dcT + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "dcT copy");
+    else CU(cudaMemsetAsync(b.dc, 0, (size_t)B * Hp * 4, st), "zero dc");
+    if (dhT) CU(cudaMemcpy2DAsync(b.dhm, Hp * 4, dhT + (size_t)l * B * H, H * 4, H * 4, B, cudaMemcpyDeviceToDevice, st), "dhT copy");
     for (int t = steps - 1; t >= 0; --t) {
       const bool last = t + 1 == steps;
       const float* cprev = t == 0 ? b.c_init + (size_t)l * B * Hp : b.cseq[l] + (size_t)(t - 1) * B * Hp;
@@ -546,28 +543,28 @@ static int lstm_backward_rows(const LstmDims& d, const LstmBuffers& b, const Lst
           b.cseq[l] + (size_t)t * B * Hp, cprev, done + (size_t)t * B, b.dc, B, H, Hp, b.dgates[l] + (size_t)t * B * G);
       if (t > 0 || dh0) {   // dhm_t = dgates_t . Whh  (gradient w.r.t. m_t . h_{t-1})
         LGemmK::Params q{m.dg128[l], m.WhhT[l], b.dhm, B, G / 64, Hp, t * B, 0};
-        LCU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(B, 128), Hp / 64), st), "lstm bwd recurrent gemm");
+        CU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(B, 128), Hp / 64), st), "lstm bwd recurrent gemm");
       }
     }
-    LCU(cudaGetLastError(), "lstm cell bwd");
+    CU(cudaGetLastError(), "lstm cell bwd");
     if (dh0) lstm_unpad_masked_kernel<<<cdiv_((int64_t)B * H, 256), 256, 0, st>>>(b.dhm, done, B, H, Hp, dh0 + (size_t)l * B * H);
     if (dc0) lstm_unpad_rows_kernel<<<cdiv_((int64_t)B * H, 256), 256, 0, st>>>(b.dc, B, H, Hp, dc0 + (size_t)l * B * H);
     // weight gradients over all NB rows (MN-major operands), then un-pad + accumulate
     { LGemmMN::Params q{m.dg64[l], m.xin64[l], b.dwpad, (int)NB, Hp};
-      LCU(igemm_tma_launch<LGemmMN>(q, dim3(G / 128, Hp / 64), st), "lstm dWih gemm");
+      CU(igemm_tma_launch<LGemmMN>(q, dim3(G / 128, Hp / 64), st), "lstm dWih gemm");
       lstm_unpad_w_kernel<<<cdiv_((int64_t)4 * H * H, 256), 256, 0, st>>>(b.dwpad, H, Hp, g8[4 * l]); }
     { LGemmMN::Params q{m.dg64[l], m.hm64[l], b.dwpad, (int)NB, Hp};
-      LCU(igemm_tma_launch<LGemmMN>(q, dim3(G / 128, Hp / 64), st), "lstm dWhh gemm");
+      CU(igemm_tma_launch<LGemmMN>(q, dim3(G / 128, Hp / 64), st), "lstm dWhh gemm");
       lstm_unpad_w_kernel<<<cdiv_((int64_t)4 * H * H, 256), 256, 0, st>>>(b.dwpad, H, Hp, g8[4 * l + 1]); }
     { const int chunks = cdiv_(NB, LSTM_BIAS_CHUNK);
       lstm_bias_part_kernel<<<dim3(cdiv_(G, 128), chunks), 128, 0, st>>>(b.dgates[l], (int)NB, G, b.bias_part);
       lstm_bias_sum_kernel<<<cdiv_((int64_t)4 * H, 256), 256, 0, st>>>(b.bias_part, chunks, H, Hp, g8[4 * l + 2], g8[4 * l + 3]); }
     // gradient w.r.t. this layer's input = dh_out of the layer below (or dcore)
     { LGemmK::Params q{m.dg128[l], m.WihT[l], b.dx, (int)NB, G / 64, Hp, 0, 0};
-      LCU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(NB, 128), Hp / 64), st), "lstm dx gemm"); }
+      CU(igemm_tma_launch<LGemmK>(q, dim3(cdiv_(NB, 128), Hp / 64), st), "lstm dx gemm"); }
   }
   lstm_unpad_rows_kernel<<<cdiv_(NB * H, 256), 256, 0, st>>>(b.dx, (int)NB, H, Hp, dcore);
-  LCU(cudaGetLastError(), "lstm backward");
+  CU(cudaGetLastError(), "lstm backward");
   return 0;
 }
 }  // namespace srl
@@ -583,17 +580,17 @@ struct srl_lstm {
 };
 
 extern "C" int srl_lstm_create(int T1, int B, int H, const float* const* weights8, float* const* grads8, srl_lstm_t** out) {
-  LREQ(T1 >= 2 && B >= 1 && H >= 1 && weights8 && grads8 && out, "lstm_create: bad argument");
+  REQ(T1 >= 2 && B >= 1 && H >= 1 && weights8 && grads8 && out, "lstm_create: bad argument");
   srl_lstm* L = new (std::nothrow) srl_lstm();
-  LREQ(L, "out of memory");
+  REQ(L, "out of memory");
   L->d = lstm_dims(T1, B, H, (int64_t)(T1 - 1) * B);
   for (int i = 0; i < 8; ++i) { L->w[i] = weights8[i]; L->g[i] = grads8[i]; }
   WsRow t[LSTM_ROWS];
   lstm_rows(L->b, L->d, t);
   const int64_t total = rows_bytes(t, LSTM_ROWS, false);
-  if (cudaMalloc(&L->arena, total) != cudaSuccess || cudaMemset(L->arena, 0, total) != cudaSuccess) { delete L; LREQ(false, "lstm_create: cudaMalloc failed"); }
+  if (cudaMalloc(&L->arena, total) != cudaSuccess || cudaMemset(L->arena, 0, total) != cudaSuccess) { delete L; return fail(SRL_EINVAL, "lstm_create: cudaMalloc failed"); }
   carve_rows(t, LSTM_ROWS, false, L->arena);
-  if (!lstm_maps(L->b, L->d, &L->m)) { cudaFree(L->arena); delete L; LREQ(false, "lstm_create: tensor map creation failed"); }
+  if (!lstm_maps(L->b, L->d, &L->m)) { cudaFree(L->arena); delete L; return fail(SRL_EINVAL, "lstm_create: tensor map creation failed"); }
   *out = L;
   return 0;
 }
@@ -601,57 +598,40 @@ extern "C" int srl_lstm_destroy(srl_lstm_t* L) { if (L) { cudaFree(L->arena); de
 
 extern "C" int srl_lstm_forward(srl_lstm_t* L, const float* core, const uint8_t* done, const float* h0, const float* c0, float* out,
                                 float* hT, float* cT, void* stream) {
-  LREQ(L && core && done && h0 && c0 && out, "lstm_forward: NULL pointer");
+  REQ(L && core && done && h0 && c0 && out, "lstm_forward: NULL pointer");
   return lstm_forward_rows(L->d, L->b, L->m, L->w, core, done, h0, c0, out, hT, cT, (cudaStream_t)stream);
 }
 
 extern "C" int srl_lstm_backward(srl_lstm_t* L, const float* dout, const uint8_t* done, float* dcore, void* stream) {
-  LREQ(L && dout && done && dcore, "lstm_backward: NULL pointer");
+  REQ(L && dout && done && dcore, "lstm_backward: NULL pointer");
   return lstm_backward_rows(L->d, L->b, L->m, L->g, done, dout, nullptr, nullptr, dcore, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------ stand-alone core on caller-owned blocks
-constexpr int LSTM_CORE_MAX_ROWS = 65536;
-
 static int check_core_shape(int T1, int B, int A, const char* what) {
-  LREQ(T1 >= 1 && B >= 1 && (int64_t)T1 * B <= LSTM_CORE_MAX_ROWS, "%s: T1=%d B=%d: need T1 >= 1, B >= 1 and T1*B <= %d", what, T1, B,
-       LSTM_CORE_MAX_ROWS);
-  LREQ(A >= 1 && A <= 31, "%s: A=%d must be in [1, 31]", what, A);
+  REQ(T1 >= 1 && B >= 1 && (int64_t)T1 * B <= MAX_FRAMES, "%s: T1=%d B=%d: need T1 >= 1, B >= 1 and T1*B <= %d", what, T1, B, MAX_FRAMES);
+  REQ(A >= 1 && A <= 31, "%s: A=%d must be in [1, 31]", what, A);
   return 0;
 }
 
 extern "C" int srl_lstm_core_sizes(int T1, int B, int A, int64_t* saved_bytes, int64_t* scratch_bytes) {
-  LREQ(saved_bytes && scratch_bytes, "lstm_core_sizes: NULL argument");
+  REQ(saved_bytes && scratch_bytes, "lstm_core_sizes: NULL argument");
   int rc = check_core_shape(T1, B, A, "lstm_core_sizes");
   if (rc) return rc;
   LstmBuffers b = {};
   WsRow t[LSTM_ROWS];
   lstm_rows(b, lstm_dims(T1, B, 513 + A, (int64_t)T1 * B), t);
-  *saved_bytes = rows_bytes(t, LSTM_SAVED_ROWS, false);
-  *scratch_bytes = rows_bytes(t + LSTM_SAVED_ROWS, LSTM_ROWS - LSTM_SAVED_ROWS, false);
+  block_bytes(t, LSTM_ROWS, LSTM_SAVED_ROWS, false, saved_bytes, scratch_bytes);
   return 0;
 }
 
-// one argument of a call: outputs may overlap nothing, inputs may overlap each other
-struct Span { const void* p; int64_t bytes; bool out; const char* name; };
-static int check_spans(const Span* s, int n, const char* what) {
-  for (int i = 0; i < n; ++i)
-    for (int j = 0; j < i; ++j) {
-      if (!s[i].p || !s[j].p || !(s[i].out || s[j].out)) continue;
-      const uintptr_t x = reinterpret_cast<uintptr_t>(s[i].p), y = reinterpret_cast<uintptr_t>(s[j].p);
-      LREQ(!(x < y + (uintptr_t)s[j].bytes && y < x + (uintptr_t)s[i].bytes), "%s: %s overlaps %s", what, s[i].name, s[j].name);
-    }
-  return 0;
-}
-static const char* const kW8[8] = {"weights8[0]", "weights8[1]", "weights8[2]", "weights8[3]", "weights8[4]", "weights8[5]", "weights8[6]", "weights8[7]"};
-static const char* const kG8[8] = {"grads8[0]", "grads8[1]", "grads8[2]", "grads8[3]", "grads8[4]", "grads8[5]", "grads8[6]", "grads8[7]"};
 static int64_t lstm_tensor_bytes(int i, int H) { return (i % 4 < 2 ? (int64_t)4 * H * H : (int64_t)4 * H) * 4; }
 
 // the checks both calls share: shape, the blocks' alignment and sizes
 static int check_core_call(int T1, int B, int A, const void* saved, const void* scratch, int64_t* sb, int64_t* kb, const char* what) {
   int rc = check_core_shape(T1, B, A, what);
   if (rc) return rc;
-  LREQ(((reinterpret_cast<uintptr_t>(saved) | reinterpret_cast<uintptr_t>(scratch)) & 255) == 0, "%s: saved and scratch must be 256-byte aligned", what);
+  REQ(!misaligned(saved, 256) && !misaligned(scratch, 256), "%s: saved and scratch must be 256-byte aligned", what);
   return srl_lstm_core_sizes(T1, B, A, sb, kb);
 }
 
@@ -660,25 +640,16 @@ static int core_call_setup(const LstmDims& d, void* saved, void* scratch, LstmBu
   WsRow t[LSTM_ROWS];
   *b = LstmBuffers{};
   lstm_rows(*b, d, t);
-  carve_rows(t, LSTM_SAVED_ROWS, false, static_cast<char*>(saved));
-  carve_rows(t + LSTM_SAVED_ROWS, LSTM_ROWS - LSTM_SAVED_ROWS, false, static_cast<char*>(scratch));
-  // encoding needs the device's context current on this thread, and this may be the thread's first CUDA call (torch runs a backward
-  // on an autograd thread of its own): cudaSetDevice makes the primary context current
-  int dev = 0;
-  LCU(cudaGetDevice(&dev), "cudaGetDevice");
-  LCU(cudaSetDevice(dev), "cudaSetDevice");
-  if (!lstm_maps(*b, d, m)) {
-    snprintf(g_lerr, sizeof(g_lerr), "%s: tensor map creation failed (driver without cuTensorMapEncodeTiled?)", what);
-    return SRL_ESTATE;
-  }
+  CU(carve_blocks(t, LSTM_ROWS, LSTM_SAVED_ROWS, false, saved, scratch), "cudaSetDevice");
+  if (!lstm_maps(*b, d, m)) return fail(SRL_ESTATE, "%s: tensor map creation failed (driver without cuTensorMapEncodeTiled?)", what);
   pdl_set_active(true);
   return 0;
 }
 
 extern "C" int srl_lstm_core_forward(const float* core, const uint8_t* done, const float* h0, const float* c0, int A, int T1, int B,
                                      const float* const* weights8, void* saved, void* scratch, float* out, float* hT, float* cT, void* stream) {
-  LREQ(core && done && h0 && c0 && weights8 && saved && scratch && out && hT && cT, "lstm_core_forward: NULL pointer");
-  for (int i = 0; i < 8; ++i) LREQ(weights8[i], "lstm_core_forward: weights8[%d] is NULL", i);
+  REQ(core && done && h0 && c0 && weights8 && saved && scratch && out && hT && cT, "lstm_core_forward: NULL pointer");
+  for (int i = 0; i < 8; ++i) REQ(weights8[i], "lstm_core_forward: weights8[%d] is NULL", i);
   int64_t sb = 0, kb = 0;
   int rc = check_core_call(T1, B, A, saved, scratch, &sb, &kb, "lstm_core_forward");
   if (rc) return rc;
@@ -697,14 +668,14 @@ extern "C" int srl_lstm_core_forward(const float* core, const uint8_t* done, con
   rc = core_call_setup(d, saved, scratch, &b, &m, "lstm_core_forward");
   if (rc) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
-  LCU(cudaMemcpyAsync(b.done, done, N1, cudaMemcpyDeviceToDevice, st), "done copy");
+  CU(cudaMemcpyAsync(b.done, done, N1, cudaMemcpyDeviceToDevice, st), "done copy");
   return lstm_forward_rows(d, b, m, weights8, core, b.done, h0, c0, out, hT, cT, st);
 }
 
 extern "C" int srl_lstm_core_backward(const float* dout, const float* dhT, const float* dcT, int A, int T1, int B, void* saved, void* scratch,
                                       float* const* grads8, float* dcore, float* dh0, float* dc0, void* stream) {
-  LREQ(dout && saved && scratch && grads8 && dcore, "lstm_core_backward: NULL pointer");
-  for (int i = 0; i < 8; ++i) LREQ(grads8[i], "lstm_core_backward: grads8[%d] is NULL", i);
+  REQ(dout && saved && scratch && grads8 && dcore, "lstm_core_backward: NULL pointer");
+  for (int i = 0; i < 8; ++i) REQ(grads8[i], "lstm_core_backward: grads8[%d] is NULL", i);
   int64_t sb = 0, kb = 0;
   int rc = check_core_call(T1, B, A, saved, scratch, &sb, &kb, "lstm_core_backward");
   if (rc) return rc;
@@ -723,7 +694,7 @@ extern "C" int srl_lstm_core_backward(const float* dout, const float* dhT, const
   rc = core_call_setup(d, saved, scratch, &b, &m, "lstm_core_backward");
   if (rc) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
-  for (int i = 0; i < 8; ++i) LCU(cudaMemsetAsync(grads8[i], 0, lstm_tensor_bytes(i, H), st), "zero grads8");     // overwritten, not accumulated
+  for (int i = 0; i < 8; ++i) CU(cudaMemsetAsync(grads8[i], 0, lstm_tensor_bytes(i, H), st), "zero grads8");     // overwritten, not accumulated
   return lstm_backward_rows(d, b, m, grads8, b.done, dout, dhT, dcT, dcore, dh0, dc0, st);
 }
 
@@ -736,27 +707,27 @@ struct LstmStep {
   alignas(64) CUtensorMap m_w, m_xh[2];
 };
 
-cudaError_t lstm_step_create(int B, int H, const float* const* weights8, LstmStep** out, const char** why) {
+int lstm_step_create(int B, int H, const float* const* weights8, LstmStep** out) {
   *out = nullptr;
-  if (B < 1 || H < 1 || (H + 63) / 64 * 64 != LS_HP) { *why = "lstm_step: H must be 513 + A with A in [1, 31]"; return cudaErrorInvalidValue; }
+  REQ(B >= 1 && H >= 1 && (H + 63) / 64 * 64 == LS_HP, "lstm_step: H must be 513 + A with A in [1, 31]");
   LstmStep* S = new (std::nothrow) LstmStep();
-  if (!S) { *why = "out of host memory"; return cudaErrorMemoryAllocation; }
+  REQ(S, "out of host memory");
   S->B = B; S->H = H;
   for (int l = 0; l < 2; ++l) for (int k = 0; k < 4; ++k) S->w[l][k] = weights8[4 * l + k];
   const size_t wbytes = (size_t)2 * LS_G * LS_K * 2, xbytes = (size_t)2 * B * LS_K * 2;
   char* a = nullptr;
   cudaError_t e = cudaMalloc(&a, wbytes + xbytes);
   if (e == cudaSuccess) e = cudaMemset(a, 0, wbytes + xbytes);      // the operands' padding columns stay zero from here on
-  if (e != cudaSuccess) { if (a) cudaFree(a); delete S; *why = "lstm_step: cudaMalloc failed"; return e; }
+  if (e != cudaSuccess) { if (a) cudaFree(a); delete S; return cuda_fail(e, "lstm_step: cudaMalloc"); }
   S->wp = (__nv_bfloat16*)a; S->xh = (__nv_bfloat16*)(a + wbytes);
   const uint64_t dw[2] = {LS_K, 2 * LS_G}, dx[2] = {LS_K, (uint64_t)B}, st[1] = {LS_K};
   const uint32_t box[2] = {64, 128};
   if (!make_map(&S->m_w, S->wp, 2, dw, st, box) || !make_map(&S->m_xh[0], S->xh, 2, dx, st, box) ||
       !make_map(&S->m_xh[1], S->xh + (size_t)B * LS_K, 2, dx, st, box)) {
-    cudaFree(a); delete S; *why = "lstm_step: tensor map creation failed"; return cudaErrorInvalidValue;
+    cudaFree(a); delete S; return fail(SRL_ESTATE, "lstm_step: tensor map creation failed");
   }
   *out = S;
-  return cudaSuccess;
+  return 0;
 }
 void lstm_step_destroy(LstmStep* S) { if (S) { cudaFree(S->wp); delete S; } }
 

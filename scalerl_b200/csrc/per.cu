@@ -4,9 +4,9 @@
 //   scalerl/data/replay_buffer.py:318-322 (_add), :346-351 (update_priorities), :353-381 (_sample_proprtional, _calculate_weight)
 // float64 so that sampled INDICES are identical to the reference's Python-float trees; HBM/latency-bound integer+fp64 work,
 // no tensor cores.  `retrieve` (missing upstream) = find_prefixsum_idx; p_total excludes the last stored item as upstream does.
-#include <stdio.h>
 #include <new>
 #include "common.cuh"
+#include "errors.h"
 #include "../../include/scalerl_b200.h"
 
 namespace srl {
@@ -113,24 +113,21 @@ struct srl_per {
   double alpha;
   double *sum, *mn, *scal;
 };
-static thread_local char g_perr[256] = "";
-extern "C" const char* srl_per_last_error(void) { return g_perr; }
-#define PREQ(c, msg) do { if (!(c)) { snprintf(g_perr, sizeof(g_perr), "%s", msg); return SRL_EINVAL; } } while (0)
-#define PCU(x, what) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { snprintf(g_perr, sizeof(g_perr), "%s: %s", what, cudaGetErrorString(e_)); return (int)e_; } } while (0)
+extern "C" const char* srl_per_last_error(void) { return srl_last_error(); }
 
 extern "C" int srl_per_create(int64_t memory_size, double alpha, srl_per_t** out) {
-  PREQ(memory_size >= 2 && memory_size <= (int64_t(1) << 30) && out, "per_create: memory_size must be in [2, 2^30]");
+  REQ(memory_size >= 2 && memory_size <= (int64_t(1) << 30) && out, "per_create: memory_size must be in [2, 2^30]");
   srl_per* P = new (std::nothrow) srl_per();
-  PREQ(P, "out of memory");
+  REQ(P, "out of memory");
   P->memory_size = memory_size; P->alpha = alpha; P->tree_ptr = 0; P->size = 0;
   P->capacity = 1; P->levels = 0;
   while (P->capacity < memory_size) { P->capacity *= 2; P->levels++; }
   const int64_t n2 = 2 * P->capacity;
   if (cudaMalloc(&P->sum, n2 * 8) != cudaSuccess || cudaMalloc(&P->mn, n2 * 8) != cudaSuccess || cudaMalloc(&P->scal, 64) != cudaSuccess) {
-    delete P; PREQ(false, "per_create: cudaMalloc failed");
+    delete P; return fail(SRL_EINVAL, "per_create: cudaMalloc failed");
   }
   per_fill_kernel<<<(int)((n2 + 255) / 256), 256>>>(P->sum, P->mn, n2, P->scal);
-  PCU(cudaDeviceSynchronize(), "per_create");
+  CU(cudaDeviceSynchronize(), "per_create");
   *out = P;
   return 0;
 }
@@ -140,7 +137,7 @@ extern "C" int64_t srl_per_capacity(const srl_per_t* P) { return P ? P->capacity
 
 // n new transitions written at tree_ptr.. with priority max_priority^alpha (_add, replay_buffer.py:318-322)
 extern "C" int srl_per_add(srl_per_t* P, int64_t n, void* stream) {
-  PREQ(P && n >= 0, "per_add: bad argument");
+  REQ(P && n >= 0, "per_add: bad argument");
   while (n > 0) {
     const int c = (int)(n < 1024 ? n : 1024);
     const int cc = c < P->memory_size ? c : (int)P->memory_size;       // never two writes to one leaf inside a launch
@@ -150,18 +147,18 @@ extern "C" int srl_per_add(srl_per_t* P, int64_t n, void* stream) {
     P->size = P->size + cc < P->memory_size ? P->size + cc : P->memory_size;
     n -= cc;
   }
-  PCU(cudaGetLastError(), "per_add");
+  CU(cudaGetLastError(), "per_add");
   return 0;
 }
 // idxs i64 [n], priorities f64 [n] (device): leaf = priority^alpha, max_priority updated (update_priorities, replay_buffer.py:346-351)
 extern "C" int srl_per_update_priorities(srl_per_t* P, const int64_t* idxs, const double* priorities, int64_t n, void* stream) {
-  PREQ(P && idxs && priorities && n >= 0, "per_update_priorities: bad argument");
+  REQ(P && idxs && priorities && n >= 0, "per_update_priorities: bad argument");
   for (int64_t o = 0; o < n; o += 1024) {
     const int c = (int)(n - o < 1024 ? n - o : 1024);
     per_update_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(P->sum, P->mn, P->capacity, P->levels, idxs + o, priorities + o, c, P->alpha, P->scal, 0,
                                                             0, P->size);        // mode 0: the last argument bounds the valid indices (idx < len(self))
   }
-  PCU(cudaGetLastError(), "per_update_priorities");
+  CU(cudaGetLastError(), "per_update_priorities");
   return 0;
 }
 // number of (idx, priority) pairs skipped so far because idx was outside [0, size) or priority <= 0 (the reference asserts,
@@ -176,19 +173,19 @@ extern "C" int64_t srl_per_invalid_updates(srl_per_t* P, void* stream) {
 // uniforms f64 [batch] in [0,1) (device) -> idxs i64 [batch], IS weights (f64 and/or f32, either may be NULL)
 extern "C" int srl_per_sample(srl_per_t* P, const double* uniforms, int batch, double beta, int64_t* idxs, double* weights64, float* weights32,
                               void* stream) {
-  PREQ(P && uniforms && idxs && batch >= 1, "per_sample: bad argument");
-  PREQ(P->size >= 2, "per_sample: need at least 2 stored transitions");
+  REQ(P && uniforms && idxs && batch >= 1, "per_sample: bad argument");
+  REQ(P->size >= 2, "per_sample: need at least 2 stored transitions");
   per_sample_kernel<<<(batch + 127) / 128, 128, 0, (cudaStream_t)stream>>>(P->sum, P->mn, P->capacity, uniforms, batch, P->size, beta, idxs, weights64,
                                                                            weights32);
-  PCU(cudaGetLastError(), "per_sample");
+  CU(cudaGetLastError(), "per_sample");
   return 0;
 }
 // copies the trees (2*capacity doubles each, root at [1], leaves at [capacity..)) and max_priority to device buffers
 extern "C" int srl_per_debug_trees(srl_per_t* P, double* sum_out, double* min_out, double* max_priority_out, void* stream) {
-  PREQ(P, "per_debug_trees: NULL");
+  REQ(P, "per_debug_trees: NULL");
   cudaStream_t st = (cudaStream_t)stream;
-  if (sum_out) PCU(cudaMemcpyAsync(sum_out, P->sum, 2 * P->capacity * 8, cudaMemcpyDeviceToDevice, st), "copy sum");
-  if (min_out) PCU(cudaMemcpyAsync(min_out, P->mn, 2 * P->capacity * 8, cudaMemcpyDeviceToDevice, st), "copy min");
-  if (max_priority_out) PCU(cudaMemcpyAsync(max_priority_out, P->scal, 8, cudaMemcpyDeviceToDevice, st), "copy max");
+  if (sum_out) CU(cudaMemcpyAsync(sum_out, P->sum, 2 * P->capacity * 8, cudaMemcpyDeviceToDevice, st), "copy sum");
+  if (min_out) CU(cudaMemcpyAsync(min_out, P->mn, 2 * P->capacity * 8, cudaMemcpyDeviceToDevice, st), "copy min");
+  if (max_priority_out) CU(cudaMemcpyAsync(max_priority_out, P->scal, 8, cudaMemcpyDeviceToDevice, st), "copy max");
   return 0;
 }

@@ -3,30 +3,14 @@
 // SWIZZLE_128B wgmma operand descriptors that start at an arbitrary 128-byte row of a swizzled tile (the "resident
 // window" trick of igemm_res.cuh), programmatic dependent launch, and a shared-memory poisoner (kernels must never
 // depend on stale shared memory).
-#include <stdio.h>
-#include <stdarg.h>
 #include <stdlib.h>
 #include "../../include/scalerl_b200_testhooks.h"
+#include "errors.h"
 #include "kernels.h"
 
 using namespace srl;
 
-static thread_local char g_err[512] = "";
-static int fail(int code, const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_err, sizeof(g_err), fmt, ap);
-  va_end(ap);
-  return code;
-}
-static int cuda_fail(cudaError_t e, const char* what) {
-  snprintf(g_err, sizeof(g_err), "%s: %s (%s)", what, cudaGetErrorName(e), cudaGetErrorString(e));
-  return (int)e;
-}
-#define CU(x, what) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return cuda_fail(e_, what); } while (0)
-#define REQ(c, ...) do { if (!(c)) return fail(-1, __VA_ARGS__); } while (0)
-
-extern "C" const char* srl_test_last_error(void) { return g_err; }
+extern "C" const char* srl_test_last_error(void) { return error_message(); }
 
 namespace srl {
 // the hooks library is self-contained: its own copies of the launch switches declared in kernels.h

@@ -17,14 +17,9 @@ class GpuPrioritizedSampler:
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._L = _lib.lib()
         h = C.c_void_p()
-        self._check(self._L.srl_per_create(self.memory_size, self.alpha, C.byref(h)), 'srl_per_create')
+        _lib.check(self._L.srl_per_create(self.memory_size, self.alpha, C.byref(h)), 'srl_per_create')
         self._h = h
         self._invalid_seen = 0
-
-    def _check(self, rc, what):
-        if rc != 0:
-            msg = self._L.srl_per_last_error().decode()
-            raise (ValueError if rc == -1 else RuntimeError)(f'{what}: rc={rc}: {msg}')
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
@@ -38,7 +33,7 @@ class GpuPrioritizedSampler:
 
     def add(self, n: int = 1):
         """n new transitions enter with priority max_priority ** alpha (replay_buffer.py:318-322)"""
-        self._check(self._L.srl_per_add(self._h, int(n), self._stream()), 'srl_per_add')
+        _lib.check(self._L.srl_per_add(self._h, int(n), self._stream()), 'srl_per_add')
 
     def update_priorities(self, idxs: torch.Tensor, priorities: torch.Tensor, validate: bool = True):
         """replay_buffer.py:346-351.  The reference asserts ``priority > 0`` and ``0 <= idx < len(self)``; with ``validate``
@@ -48,7 +43,7 @@ class GpuPrioritizedSampler:
         pr = priorities.to(self.device, torch.float64).contiguous()
         if idxs.numel() != pr.numel():
             raise ValueError('idxs and priorities must have the same length')
-        self._check(self._L.srl_per_update_priorities(self._h, idxs.data_ptr(), pr.data_ptr(), idxs.numel(), self._stream()), 'srl_per_update_priorities')
+        _lib.check(self._L.srl_per_update_priorities(self._h, idxs.data_ptr(), pr.data_ptr(), idxs.numel(), self._stream()), 'srl_per_update_priorities')
         if validate:
             bad = int(self._L.srl_per_invalid_updates(self._h, self._stream()))
             if bad != self._invalid_seen:
@@ -63,8 +58,8 @@ class GpuPrioritizedSampler:
         idxs = torch.empty(batch_size, dtype=torch.int64, device=self.device)
         w32 = torch.empty(batch_size, dtype=torch.float32, device=self.device)
         self._w64 = torch.empty(batch_size, dtype=torch.float64, device=self.device)
-        self._check(self._L.srl_per_sample(self._h, u.data_ptr(), int(batch_size), float(beta), idxs.data_ptr(), self._w64.data_ptr(), w32.data_ptr(),
-                                           self._stream()), 'srl_per_sample')
+        _lib.check(self._L.srl_per_sample(self._h, u.data_ptr(), int(batch_size), float(beta), idxs.data_ptr(), self._w64.data_ptr(), w32.data_ptr(),
+                                          self._stream()), 'srl_per_sample')
         return idxs, w32
 
     def trees(self):
@@ -72,7 +67,7 @@ class GpuPrioritizedSampler:
         s = torch.empty(2 * cap, dtype=torch.float64, device=self.device)
         m = torch.empty(2 * cap, dtype=torch.float64, device=self.device)
         mp = torch.empty(1, dtype=torch.float64, device=self.device)
-        self._check(self._L.srl_per_debug_trees(self._h, s.data_ptr(), m.data_ptr(), mp.data_ptr(), self._stream()), 'srl_per_debug_trees')
+        _lib.check(self._L.srl_per_debug_trees(self._h, s.data_ptr(), m.data_ptr(), mp.data_ptr(), self._stream()), 'srl_per_debug_trees')
         torch.cuda.current_stream(self.device).synchronize()
         return s, m, float(mp.item())
 

@@ -32,13 +32,8 @@ class B200LstmCore:
         gp = (C.c_void_p * 8)(*[self.grads[n].data_ptr() for n in LSTM_PARAM_NAMES])
         h = C.c_void_p()
         self._L = _lib.lib()
-        self._check(self._L.srl_lstm_create(T1, B, H, wp, gp, C.byref(h)), 'srl_lstm_create')
+        _lib.check(self._L.srl_lstm_create(T1, B, H, wp, gp, C.byref(h)), 'srl_lstm_create')
         self._h = h
-
-    def _check(self, rc, what):
-        if rc != 0:
-            msg = self._L.srl_lstm_last_error().decode()
-            raise (ValueError if rc == -1 else RuntimeError)(f'{what}: rc={rc}: {msg}')
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
@@ -61,8 +56,8 @@ class B200LstmCore:
         out = torch.empty(T1, B, H, device=self.device)
         hT, cT = torch.empty(2, B, H, device=self.device), torch.empty(2, B, H, device=self.device)
         self._done = d
-        self._check(self._L.srl_lstm_forward(self._h, core.contiguous().data_ptr(), d.data_ptr(), h0.data_ptr(), c0.data_ptr(), out.data_ptr(),
-                                             hT.data_ptr(), cT.data_ptr(), self._stream()), 'srl_lstm_forward')
+        _lib.check(self._L.srl_lstm_forward(self._h, core.contiguous().data_ptr(), d.data_ptr(), h0.data_ptr(), c0.data_ptr(), out.data_ptr(),
+                                            hT.data_ptr(), cT.data_ptr(), self._stream()), 'srl_lstm_forward')
         return out, (hT, cT)
 
     @torch.no_grad()
@@ -72,8 +67,8 @@ class B200LstmCore:
         if tuple(dout.shape) != (T, B, H):
             raise ValueError(f'dout must be {(T, B, H)}')
         dcore = torch.empty(T, B, H, device=self.device)
-        self._check(self._L.srl_lstm_backward(self._h, dout.contiguous().data_ptr(), self._done.data_ptr(), dcore.data_ptr(), self._stream()),
-                    'srl_lstm_backward')
+        _lib.check(self._L.srl_lstm_backward(self._h, dout.contiguous().data_ptr(), self._done.data_ptr(), dcore.data_ptr(), self._stream()),
+                   'srl_lstm_backward')
         return dcore
 
     def close(self):

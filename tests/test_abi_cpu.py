@@ -104,6 +104,20 @@ def test_argument_errors_without_gpu(lib):
     assert b'A=99' in L.srl_last_error()
 
 
+def test_one_error_message_per_library(lib):
+    """the replay sampler reports through srl_last_error (srl_per_last_error returns the same message); the test-hook library keeps
+    a message of its own"""
+    L, H = _lib.lib(), _lib.hooks()
+    h = ctypes.c_void_p()
+    assert H.srl_test_shifted_operand(None, None, None, 0, 0, 0, None) == -1
+    assert L.srl_vtrace_from_importance_weights(None, None, None, None, None, 4, 4, 1.0, 1.0, None, None, 0, None) == -1
+    assert L.srl_per_create(1, 0.6, ctypes.byref(h)) == -1
+    msg = L.srl_last_error()
+    assert msg.startswith(b'per_create: ') and b'memory_size' in msg
+    assert L.srl_per_last_error() == msg
+    assert H.srl_test_last_error().startswith(b'test_shifted_operand: ')
+
+
 def test_timeline_entry_is_inert_in_the_product_build(lib):
     """srl_debug_kernel_timeline only works in a diagnostics build (SRL_DEFINES=SRL_KSTAMP): the shipped library refuses, without touching CUDA"""
     L = _lib.lib()

@@ -119,3 +119,37 @@ def test_entry_points_reject_bad_arguments_before_any_cuda_call(lib):
         assert 'overlap' in _err(L)
     finally:
         assert L.srl_encoder_destroy(h) == 0
+
+
+def test_every_output_against_every_other_argument(lib):
+    """each output of srl_encoder_forward / _backward placed on each other argument is rejected before any CUDA call"""
+    L = lib
+    h = C.c_void_p()
+    assert L.srl_encoder_create(0, C.byref(h)) == 0
+    try:
+        at = lambda i: (1 << 40) + (i << 32)                  # fake device addresses, far apart and 256-byte aligned
+        fa = dict(obs=at(0), reward=at(1), action=at(2), saved=at(3), scratch=at(4), core=at(5), **{f'w{i}': at(10 + i) for i in range(8)})
+        ba = dict(dcore=at(6), saved=at(3), scratch=at(4), **{f'g{i}': at(20 + i) for i in range(8)})
+
+        def fwd(**kw):
+            a = {**fa, **kw}
+            return L.srl_encoder_forward(h, a['obs'], a['reward'], a['action'], 8, 6, (C.c_void_p * 8)(*[a[f'w{i}'] for i in range(8)]),
+                                         a['saved'], a['scratch'], a['core'], None)
+
+        def bwd(**kw):
+            a = {**ba, **kw}
+            return L.srl_encoder_backward(h, a['dcore'], 8, 6, a['saved'], a['scratch'], (C.c_void_p * 8)(*[a[f'g{i}'] for i in range(8)]), None)
+
+        for o in ('saved', 'scratch', 'core'):
+            for other in fa:
+                if other != o:
+                    assert fwd(**{o: fa[other]}) == -1 and 'overlaps' in _err(L), (o, other)
+        for o in ['scratch'] + [f'g{i}' for i in range(8)]:
+            for other in ba:
+                if other != o:
+                    assert bwd(**{o: ba[other]}) == -1 and 'overlaps' in _err(L), (o, other)
+        assert fwd(core=at(16)) == -1 and _err(L) == 'encoder_forward: core_out overlaps weights8[6]'
+        assert bwd(g7=at(20)) == -1 and _err(L) == 'encoder_backward: grads8[7] overlaps grads8[0]'
+        assert bwd(g2=at(3)) == -1 and 'grads8[2] overlaps saved' in _err(L)
+    finally:
+        assert L.srl_encoder_destroy(h) == 0

@@ -126,6 +126,16 @@ def test_backward_rejects_bad_arguments_before_any_cuda_call(lib):
     assert _rejects(_bwd(L, g=(C.c_void_p * 8)(*([_at(0)] + g[1:]))), L, 'overlaps dout')
 
 
+def test_errors_are_reported_by_srl_last_error(lib):
+    """the LSTM core reports through the library's one message: srl_lstm_last_error returns what srl_last_error does"""
+    L = lib
+    assert L.srl_encoder_sizes(0, 0, None, None) == -1                 # another entry point's message first
+    assert _fwd(L, A=32) == -1
+    msg = L.srl_last_error().decode()
+    assert msg.startswith('lstm_core_forward: ') and 'A=32' in msg
+    assert _err(L) == msg
+
+
 # ---- AtariNet(use_lstm=True): state and done errors come before the encoder (no device needed to see them)
 def _inputs(T, B, A=6, done=None):
     return dict(obs=torch.zeros(T, B, 4, 84, 84, dtype=torch.uint8), reward=torch.zeros(T, B), action=torch.zeros(T, B, dtype=torch.int64),
