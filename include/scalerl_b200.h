@@ -330,6 +330,57 @@ int srl_per_sample(srl_per_t* P, const double* uniforms, int batch, double beta,
 int srl_per_debug_trees(srl_per_t* P, double* sum_out, double* min_out, double* max_priority_out, void* stream);
 const char* srl_per_last_error(void);
 
+/* ---- Ape-X learner step: a prioritized (double) DQN update on the encoder (BASELINE.json configs[3]) --------------------------
+ * replaces the learner statements of the reference's Ape-X Learner.train (scalerl/algorithms/apex/worker.py:134-161) and, with
+ * double DQN, clipping and the target cadence, DQNAgent.learn (scalerl/algorithms/dqn/dqn_agent.py:136-190).  The Q network is
+ * Nature DQN: AtariNet's conv1..3 + fc + ReLU (atari_model.py:30-47,91-101) followed by q = Linear(512, A), A in [1, 31].
+ * Actors, transition storage and n-step folding stay with the caller (pass gamma^n for n-step transitions).
+ * Parameters in state_dict order {conv1.weight, conv1.bias, conv2.weight, conv2.bias, conv3.weight, conv3.bias, fc.weight, fc.bias,
+ * q.weight [A,512], q.bias [A]}; srl_apex_param_layout returns the flat buffer's floats and each tensor's offset / count (int64[10]).
+ * In memory the small tensors come first and fc.weight last; segments are padded to 4 floats.  Params, grads, both Adam states
+ * and the target copy share the layout. */
+typedef struct srl_apex_learner srl_apex_learner_t;
+typedef struct srl_apex_config {
+  int32_t B;                 /* transitions per step, 1 <= B <= 65536                                        */
+  int32_t A;                 /* actions, [1, 31]                                                             */
+  int32_t precision;         /* encoder operands, as srl_config_t.precision: 0 = bf16, 1 = fp32-accurate split */
+  int32_t double_dqn;        /* 1: a* = argmax of the online network at s' (dqn_agent.py:155-160)              */
+  float gamma;               /* discount (gamma^n for n-step transitions)                                    */
+  float max_grad_norm;       /* clip_grad_norm_ threshold (dqn_agent.py:178-181), > 0; +inf: no clip (coef 1) */
+  float learning_rate, adam_beta1, adam_beta2, adam_eps;   /* torch.optim.Adam (apex/worker.py:132)            */
+  float priority_eps;        /* priority = |q - y| + priority_eps (in double), >= 0                           */
+} srl_apex_config_t;
+int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10);
+/* params / grads / exp_avg / exp_avg_sq / target_params: caller-owned flat f32 device buffers of srl_apex_param_layout floats,
+ * 16-byte aligned and disjoint.  The context owns the encoder's blocks (one saved block for the forward over s, one for the
+ * forwards over s', their scratch) and the tail's buffers.  Synchronous. */
+int srl_apex_learner_create(const srl_apex_config_t* cfg, float* params, float* grads, float* exp_avg, float* exp_avg_sq,
+                            float* target_params, srl_apex_learner_t** out);
+int srl_apex_learner_destroy(srl_apex_learner_t* L);
+/* One learner step on B transitions (apex/memory.py:7-8): obs / next_obs u8 [B,4,84,84], action i64 [B], reward f32 [B],
+ * done u8/bool [B], weights f32 [B] (importance weights; NULL = 1), idxs i64 [B] with per (both NULL, or both set).
+ *   q = Q(s)[a];  y = r + gamma Q_t(s')[a*] (1 - d), a* = argmax Q_t(s') or, double_dqn, argmax Q(s')   (worker.py:148-150)
+ *   loss = mean(w (q - y)^2)                                                                             (worker.py:156-157)
+ *   priority = |q - y| + priority_eps from the pre-update weights -> the sampler's trees, last occurrence of an idx wins (:152-154)
+ *   clip_grad_norm_(max_grad_norm), torch.optim.Adam step with the step count kept on the device       (dqn_agent.py:172-182)
+ * stats_out: f32 [3] device = {loss, gradient norm, clip coefficient} (may be NULL).  No host synchronisation; capturable. */
+int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, const int64_t* action, const float* reward, const uint8_t* next_obs,
+                          const uint8_t* done, const float* weights, const int64_t* idxs, srl_per_t* per, float* stats_out, void* stream);
+/* target_params = tau * params + (1 - tau) * target_params, each product and the sum rounded separately (soft_target_update,
+ * utils/model_utils.py:29-32; dqn_agent.py:185-190): tau = 1 copies exactly.  tau in [0, 1]. */
+int srl_apex_learner_update_target(srl_apex_learner_t* L, float tau, void* stream);
+/* Adam's step count (torch.optim state['step']) for a resumed run: writes the device counter; synchronises `stream` */
+int srl_apex_learner_set_step(srl_apex_learner_t* L, int64_t step, void* stream);
+/* Q(obs) with the online parameters for n >= 1 frames: obs u8 [n,4,84,84] -> q_out f32 [n,A] (predict / get_action).  Runs on its own
+ * encoder context and blocks, so it may run on another stream than srl_apex_learner_step without touching the step's buffers; it reads
+ * the parameters as they are when it runs (order it with the step on one stream for a given parameter version).  Calls of it on two
+ * streams at once share its blocks and must be ordered. */
+int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* obs, int n, float* q_out, void* stream);
+/* borrow the step's buffers for tests: "core", "core_next" (double DQN only), "core_next_target" f32 [B,514] (the encoder's core rows;
+ * h = columns < 512), "dcore" f32 [B,514], "q", "y" f32 [B], "priorities" f64 [B], "loss" f32 [1], "step" i32 [1] (device step count),
+ * and the bf16 activations the forward over s saved, in the learner's layouts (srl_learner_debug_buffer): "a1", "a2", "a3" */
+int srl_apex_learner_debug_buffer(srl_apex_learner_t* L, const char* name, void** ptr, int64_t* count);
+
 /* ---- trajectory ring -> time-major batch (the stacking step of ImpalaTrainer.get_batch, impala_atari.py:248-251) -----------
  * staging: B trajectory slots on the DEVICE, each one contiguous record of slot_bytes holding every key of create_buffers
  * (impala_atari.py:135-147) for T+1 steps; offsets6_host (HOST array) = byte offsets of {obs u8[T+1,4,84,84], reward f32[T+1],

@@ -88,6 +88,13 @@ _SIGS = {
     'srl_profile_slot_count': [],
     'srl_learner_profile_collect': [_P, _P],
     'srl_version': [],
+    'srl_apex_learner_create': [C.c_void_p, _P, _P, _P, _P, _P, C.POINTER(_P)],
+    'srl_apex_learner_destroy': [_P],
+    'srl_apex_learner_step': [_P] * 11,
+    'srl_apex_learner_update_target': [_P, _F, _P],
+    'srl_apex_learner_set_step': [_P, _L, _P],
+    'srl_apex_learner_q_values': [_P, _P, _I, _P, _P],
+    'srl_apex_learner_debug_buffer': [_P, C.c_char_p, C.POINTER(_P), C.POINTER(_L)],
 }
 # libscalerl_b200_testhooks.so (include/scalerl_b200_testhooks.h): unit-test entry points, loaded by tests only
 _HOOK_SIGS = {
@@ -117,7 +124,7 @@ def hooks():
     return _hooks
 
 
-EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step'])
+EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout'])
 
 
 def lib():
@@ -150,6 +157,8 @@ def lib():
         L.srl_lstm_last_error.argtypes = []
         L.srl_profile_slot_name.restype = C.c_char_p
         L.srl_profile_slot_name.argtypes = [_I]
+        L.srl_apex_param_layout.restype = C.c_int64
+        L.srl_apex_param_layout.argtypes = [_I, C.POINTER(_L), C.POINTER(_L)]
         L.srl_learner_workspace_bytes.restype = C.c_int64
         L.srl_learner_workspace_bytes.argtypes = [_P]
         _lib = L
@@ -169,6 +178,21 @@ def check(rc, what='', last_error=None):
 def check_hook(rc, what=''):
     """check() for the test-hook library"""
     check(rc, what, hooks().srl_test_last_error)
+
+
+class SrlApexConfig(C.Structure):
+    """mirror of srl_apex_config_t"""
+    _fields_ = [('B', C.c_int32), ('A', C.c_int32), ('precision', C.c_int32), ('double_dqn', C.c_int32),
+                ('gamma', C.c_float), ('max_grad_norm', C.c_float), ('learning_rate', C.c_float), ('adam_beta1', C.c_float),
+                ('adam_beta2', C.c_float), ('adam_eps', C.c_float), ('priority_eps', C.c_float)]
+
+
+def apex_param_layout(A):
+    """(total floats, offsets, counts) of the Ape-X Q network's flat buffer, 10 tensors in state_dict order"""
+    off = (_L * 10)()
+    cnt = (_L * 10)()
+    total = lib().srl_apex_param_layout(int(A), off, cnt)
+    return int(total), [int(x) for x in off], [int(x) for x in cnt]
 
 
 def param_layout(A, use_lstm=False):

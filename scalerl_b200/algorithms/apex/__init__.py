@@ -1,0 +1,3 @@
+from .learner import APEX_PARAM_NAMES, ApexHParams, AtariQNet, B200ApexLearner, apex_param_shapes, default_q_state_dict
+
+__all__ = ['APEX_PARAM_NAMES', 'ApexHParams', 'AtariQNet', 'B200ApexLearner', 'apex_param_shapes', 'default_q_state_dict']

@@ -1,0 +1,375 @@
+"""B200ApexLearner -- the learner step of Ape-X DQN on the sm_90a encoder, behind the interface of ScaleRL's ``DQNAgent``.
+
+One ``learn`` call is the reference's Ape-X learner update (scalerl/algorithms/apex/worker.py:134-161) with the double-DQN,
+clipping and target-update statements of ``DQNAgent.learn`` (scalerl/algorithms/dqn/dqn_agent.py:136-190): the Q values of the
+batch, the bootstrapped targets, the importance-weighted squared TD loss, the new priorities written straight into a
+``GpuPrioritizedSampler``, ``clip_grad_norm_`` and a ``torch.optim.Adam`` step -- all in libscalerl_b200.so (srl_apex_learner_*),
+captured as one CUDA graph.  Actors, transition storage, n-step folding and the exploration schedule stay with the caller.
+``AtariQNet`` is the CPU torch Q network with the learner's parameter names and shapes (the actors' copy).
+"""
+from __future__ import annotations
+
+import ctypes as C
+import math
+import random
+from collections import OrderedDict
+from dataclasses import dataclass
+from typing import ClassVar, Dict, Optional
+
+import numpy as np
+import torch
+import torch.nn.functional as F
+from torch import nn
+
+from ... import _lib
+from ...learner import from_torch_optimizer_state, to_torch_optimizer_state
+from ..base import BaseAgent
+
+# state_dict order = AtariQNet.parameters() order = the integer keys of the Adam state (srl_apex_param_layout order)
+APEX_PARAM_NAMES = ('conv1.weight', 'conv1.bias', 'conv2.weight', 'conv2.bias', 'conv3.weight', 'conv3.bias',
+                    'fc.weight', 'fc.bias', 'q.weight', 'q.bias')
+MAX_FRAMES = 65536           # frames of one encoder call (MAX_FRAMES in csrc/kernels.h)
+
+
+def apex_param_shapes(num_actions: int):
+    return OrderedDict([
+        ('conv1.weight', (32, 4, 8, 8)), ('conv1.bias', (32,)), ('conv2.weight', (64, 32, 4, 4)), ('conv2.bias', (64,)),
+        ('conv3.weight', (64, 64, 3, 3)), ('conv3.bias', (64,)), ('fc.weight', (512, 3136)), ('fc.bias', (512,)),
+        ('q.weight', (num_actions, 512)), ('q.bias', (num_actions,))])
+
+
+class AtariQNet(nn.Module):
+    """Nature DQN on 4 stacked 84x84 frames: AtariNet's conv1..3 and fc (scalerl/algorithms/utils/atari_model.py:30-47, 91-101)
+    followed by ``q = nn.Linear(512, num_actions)``.  Initialised by torch's default layer init, so ``torch.manual_seed(s)`` before
+    construction fixes the weights."""
+
+    def __init__(self, num_actions: int, observation_shape=(4, 84, 84)):
+        super().__init__()
+        self.observation_shape = tuple(observation_shape)
+        self.num_actions = int(num_actions)
+        self.conv1 = nn.Conv2d(self.observation_shape[0], 32, kernel_size=8, stride=4)
+        self.conv2 = nn.Conv2d(32, 64, kernel_size=4, stride=2)
+        self.conv3 = nn.Conv2d(64, 64, kernel_size=3, stride=1)
+        self.fc = nn.Linear(3136, 512)
+        self.q = nn.Linear(512, self.num_actions)
+
+    def forward(self, obs: torch.Tensor) -> torch.Tensor:
+        """obs u8 [N, 4, 84, 84] -> Q values [N, A]"""
+        x = obs.float() / 255.0
+        x = F.relu(self.conv1(x))
+        x = F.relu(self.conv2(x))
+        x = F.relu(self.conv3(x))
+        x = F.relu(self.fc(x.reshape(x.shape[0], -1)))
+        return self.q(x)
+
+
+@dataclass
+class ApexHParams:
+    """The learner's settings, with the names and defaults of ScaleRL's ``DQNArguments`` and the Ape-X ``Learner``
+    (apex/worker.py:120-132): Adam at lr 1e-3 with torch's default betas / eps, no clipping, a hard target copy every 100 steps."""
+    batch_size: int = 32
+    num_actions: int = 6
+    gamma: float = 0.99                  # pass gamma ** n for n-step transitions
+    learning_rate: float = 1e-3
+    max_grad_norm: Optional[float] = None
+    double_dqn: bool = False
+    target_update_frequency: int = 100
+    soft_update_tau: float = 1.0
+    precision: str = 'bf16'              # encoder operands: 'bf16' | 'fp32_split' (fp32-accurate hi/lo bf16 pairs)
+    priority_eps: float = 1e-6           # priority = |q - y| + priority_eps; 0 is the reference's value (which the tree asserts > 0)
+    adam_beta1: float = 0.9
+    adam_beta2: float = 0.999
+    adam_eps: float = 1e-8
+    optimizer: ClassVar[str] = 'adam'            # read by learner.py's optimizer-state converters
+    lr_schedule: ClassVar[str] = 'constant'
+
+    def validate(self) -> None:
+        if not (isinstance(self.batch_size, int) and 1 <= self.batch_size <= MAX_FRAMES):
+            raise ValueError(f'batch_size must be an int in [1, {MAX_FRAMES}], got {self.batch_size!r}')
+        if not (isinstance(self.num_actions, int) and 1 <= self.num_actions <= 31):
+            raise ValueError(f'num_actions must be an int in [1, 31], got {self.num_actions!r}')
+        if not (math.isfinite(self.gamma) and self.gamma >= 0.0):
+            raise ValueError(f'gamma must be finite and >= 0, got {self.gamma}')
+        if not (math.isfinite(self.learning_rate) and self.learning_rate > 0.0):
+            raise ValueError(f'learning_rate must be finite and > 0, got {self.learning_rate}')
+        if self.max_grad_norm is not None and not self.max_grad_norm > 0.0:
+            raise ValueError(f'max_grad_norm must be None or > 0, got {self.max_grad_norm}')
+        if not (isinstance(self.target_update_frequency, int) and self.target_update_frequency >= 1):
+            raise ValueError(f'target_update_frequency must be an int >= 1, got {self.target_update_frequency!r}')
+        if not 0.0 <= self.soft_update_tau <= 1.0:
+            raise ValueError(f'soft_update_tau must be in [0, 1], got {self.soft_update_tau}')
+        if self.precision not in ('bf16', 'fp32_split'):
+            raise ValueError(f"precision must be 'bf16' or 'fp32_split', got {self.precision!r}")
+        if not (math.isfinite(self.priority_eps) and self.priority_eps >= 0.0):
+            raise ValueError(f'priority_eps must be finite and >= 0, got {self.priority_eps}')
+        if not (0.0 <= self.adam_beta1 < 1.0 and 0.0 <= self.adam_beta2 < 1.0):
+            raise ValueError(f'Adam betas must be in [0, 1), got ({self.adam_beta1}, {self.adam_beta2})')
+        if not (math.isfinite(self.adam_eps) and self.adam_eps >= 0.0):
+            raise ValueError(f'adam_eps must be finite and >= 0, got {self.adam_eps}')
+
+    def to_c(self) -> _lib.SrlApexConfig:
+        self.validate()
+        c = _lib.SrlApexConfig()
+        c.B, c.A = self.batch_size, self.num_actions
+        c.precision = 0 if self.precision == 'bf16' else 1
+        c.double_dqn = 1 if self.double_dqn else 0
+        c.gamma = self.gamma
+        c.max_grad_norm = math.inf if self.max_grad_norm is None else self.max_grad_norm
+        c.learning_rate, c.adam_beta1, c.adam_beta2, c.adam_eps = self.learning_rate, self.adam_beta1, self.adam_beta2, self.adam_eps
+        c.priority_eps = self.priority_eps
+        return c
+
+
+def default_q_state_dict(num_actions: int, seed: int = 0) -> 'OrderedDict[str, torch.Tensor]':
+    """AtariQNet's initial weights under ``torch.manual_seed(seed)``, drawn without disturbing the global RNG"""
+    with torch.random.fork_rng(devices=[]):
+        torch.manual_seed(seed)
+        net = AtariQNet(num_actions)
+    return OrderedDict((k, v.detach().clone()) for k, v in net.state_dict().items())
+
+
+class B200ApexLearner(BaseAgent):
+    """The Ape-X learner on one GPU.  ``learn((obs, action, reward, next_obs, done), weights, idxs, sampler)`` runs one update:
+    obs / next_obs u8 [B, 4, 84, 84], action int64 [B], reward float32 [B], done bool / uint8 [B], importance weights float32 [B]
+    (None = 1) and the sampled indices int64 [B] of ``sampler`` (a GpuPrioritizedSampler), all contiguous CUDA tensors.  The step
+    is captured as a CUDA graph per set of input addresses (first call eager, second captures, later calls replay), so a caller that
+    gathers into fixed buffers replays -- the sampled idxs and weights included: ``GpuPrioritizedSampler.sample`` returns new tensors,
+    copy them into fixed ones (each new address set costs an eager step and a capture, and its graph is kept).  The target network follows DQNAgent's cadence: after update k (from 0), when
+    k % target_update_frequency == 0, target <- tau * online + (1 - tau) * target."""
+
+    def __init__(self, hp: ApexHParams, device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None, seed: int = 0,
+                 use_graph: bool = True):
+        if not torch.cuda.is_available():
+            raise RuntimeError('B200ApexLearner needs a CUDA device: scalerl_b200 has no CPU fallback')
+        super().__init__(hp)
+        cfg = hp.to_c()
+        self.hp = hp
+        self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+        self._L = _lib.lib()
+        self.shapes = apex_param_shapes(hp.num_actions)
+        with torch.cuda.device(self.device):
+            total, self._off, self._cnt = _lib.apex_param_layout(hp.num_actions)
+            z = lambda: torch.zeros(total, dtype=torch.float32, device=self.device)
+            self.flat_params, self.flat_grads, self.exp_avg, self.exp_avg_sq, self.flat_target = z(), z(), z(), z(), z()
+            self.params = self._views(self.flat_params)
+            self.grads = self._views(self.flat_grads)
+            self.target_params = self._views(self.flat_target)
+            self._cfg = cfg
+            h = C.c_void_p()
+            _lib.check(self._L.srl_apex_learner_create(C.addressof(cfg), self.flat_params.data_ptr(), self.flat_grads.data_ptr(),
+                                                       self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), self.flat_target.data_ptr(),
+                                                       C.byref(h)), 'srl_apex_learner_create')
+            self._h = h
+            self._stats = torch.zeros(4, device=self.device)      # {loss, gradient norm, clip coefficient, pad}
+        sd = default_q_state_dict(hp.num_actions, seed) if init_state_dict is None else init_state_dict
+        self.load_state_dict(sd)
+        self.load_state_dict(sd, target=True)       # actor_target starts as a copy (dqn_agent.py:66-67)
+        self.use_graph = use_graph
+        self._graphs = {}
+        self._seen = set()
+        self._opt_steps = 0
+        self.learner_update_step = 0
+        self.target_model_update_step = 0
+
+    # ------------------------------------------------------------------ parameters
+    def _views(self, flat):
+        return OrderedDict((n, flat[self._off[i]:self._off[i] + self._cnt[i]].view(shp))
+                           for i, (n, shp) in enumerate(self.shapes.items()))
+
+    def _stream(self):
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def state_dict(self, target: bool = False) -> 'OrderedDict[str, torch.Tensor]':
+        """AtariQNet-compatible state_dict of the online (or, ``target``, the target) network"""
+        src = self.target_params if target else self.params
+        return OrderedDict((n, p.detach().clone()) for n, p in src.items())
+
+    def load_state_dict(self, sd: Dict[str, torch.Tensor], target: bool = False) -> None:
+        dst = self.target_params if target else self.params
+        for n, shp in self.shapes.items():
+            if n not in sd:
+                raise KeyError(f'missing key {n} in state_dict')
+            if tuple(sd[n].shape) != tuple(shp):
+                raise ValueError(f'{n}: shape {tuple(sd[n].shape)} != {tuple(shp)}')
+            dst[n].copy_(sd[n].to(self.device, torch.float32))
+
+    def get_weights(self):
+        return {k: v.cpu() for k, v in self.state_dict().items()}
+
+    def set_weights(self, weights) -> None:
+        self.load_state_dict(weights)
+
+    # ------------------------------------------------------------------ optimizer state and checkpoints
+    def _opt_tensors(self):
+        return {'exp_avg': self._views(self.exp_avg), 'exp_avg_sq': self._views(self.exp_avg_sq)}
+
+    def optimizer_state_dict(self) -> dict:
+        """``torch.optim.Adam(AtariQNet(...).parameters()).state_dict()`` layout"""
+        return to_torch_optimizer_state(self.hp, self._opt_tensors(), self._opt_steps, order=APEX_PARAM_NAMES)
+
+    def load_optimizer_state_dict(self, sd: dict) -> None:
+        step, kinds = from_torch_optimizer_state(sd, False, order=APEX_PARAM_NAMES)
+        for kind in kinds:
+            if kind not in ('exp_avg', 'exp_avg_sq'):
+                raise ValueError(f"optimizer_state_dict holds '{kind}' but this learner runs Adam")
+        for kind, views in self._opt_tensors().items():
+            if kind not in kinds and step > 0:
+                raise ValueError(f"optimizer_state_dict lacks '{kind}' for Adam")
+            for n, v in views.items():
+                v.copy_(kinds[kind][n]) if kind in kinds else v.zero_()
+        self.set_step(step)
+
+    def set_step(self, step: int) -> None:
+        """Adam's step count (the device counter the captured step reads) and the target cadence's counters: one learn() is one
+        optimizer step, so a resumed run continues all three where the checkpoint left them (updates k < step with k % freq == 0
+        have refreshed the target)"""
+        _lib.check(self._L.srl_apex_learner_set_step(self._h, int(step), self._stream()), 'srl_apex_learner_set_step')
+        self._opt_steps = int(step)
+        self.learner_update_step = int(step)
+        self.target_model_update_step = -(-int(step) // self.hp.target_update_frequency)
+
+    def save_checkpoint(self, path: str) -> None:
+        """the keys of DQNAgent.save_checkpoint (dqn_agent.py:210-219)"""
+        torch.save({'actor_state_dict': {k: v.cpu() for k, v in self.state_dict().items()},
+                    'actor_target_state_dict': {k: v.cpu() for k, v in self.state_dict(target=True).items()},
+                    'optimizer_state_dict': self.optimizer_state_dict()}, path)
+
+    def load_checkpoint(self, path: str) -> None:
+        ck = torch.load(path, map_location='cpu', weights_only=False)
+        self.load_state_dict(ck['actor_state_dict'])
+        self.load_state_dict(ck['actor_target_state_dict'], target=True)
+        self.load_optimizer_state_dict(ck.get('optimizer_state_dict', {}))
+
+    # ------------------------------------------------------------------ acting
+    def _obs(self, obs):
+        obs = torch.as_tensor(obs)
+        if obs.dim() == 3:
+            obs = obs.unsqueeze(0)
+        if obs.dtype != torch.uint8 or tuple(obs.shape[1:]) != (4, 84, 84) or obs.shape[0] < 1:
+            raise ValueError(f'obs must be uint8 [N, 4, 84, 84], got {tuple(obs.shape)} {obs.dtype}')
+        return obs.to(self.device).contiguous()
+
+    @torch.no_grad()
+    def q_values(self, obs) -> torch.Tensor:
+        """Q(obs) with the online network: uint8 [N, 4, 84, 84] (or one [4, 84, 84] frame stack) -> float32 [N, A].  Runs on its own
+        encoder context and buffers, so actors may call it on another stream than learn(); it reads the parameters as they are when
+        it runs."""
+        obs = self._obs(obs)
+        q = torch.empty(obs.shape[0], self.hp.num_actions, device=self.device)
+        _lib.check(self._L.srl_apex_learner_q_values(self._h, obs.data_ptr(), obs.shape[0], q.data_ptr(), self._stream()),
+                   'srl_apex_learner_q_values')
+        return q
+
+    def predict(self, obs) -> torch.Tensor:
+        """greedy actions argmax_a Q(obs, a), int64 [N] on the learner's device (dqn_agent.py:114-134)"""
+        return torch.argmax(self.q_values(obs), dim=-1)
+
+    def get_action(self, obs, eps: float) -> torch.Tensor:
+        """epsilon-greedy (dqn_agent.py:90-112) at the caller's epsilon: with probability eps one uniformly random action per row,
+        drawn as the reference draws it, else predict(obs).  The decay schedule belongs to the agent loop."""
+        obs = self._obs(obs)
+        if random.random() < eps:
+            a = np.argmax(np.random.uniform(0, 1, (obs.shape[0], self.hp.num_actions)), axis=1)
+            return torch.from_numpy(a).to(self.device)
+        return self.predict(obs)
+
+    # ------------------------------------------------------------------ learning
+    def _check(self, t, name, shape, dtypes):
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != shape or t.dtype not in dtypes:
+            got = (tuple(t.shape), t.dtype) if isinstance(t, torch.Tensor) else type(t)
+            raise ValueError(f'{name}: expected {shape} {" or ".join(str(d) for d in dtypes)}, got {got}')
+        if t.device != self.device or not t.is_contiguous():
+            raise ValueError(f'{name} must be a contiguous tensor on {self.device}')
+
+    def _inputs(self, experiences, weights, idxs, sampler):
+        if len(experiences) != 5:
+            raise ValueError('experiences must be (obs, action, reward, next_obs, done)')
+        obs, action, reward, next_obs, done = experiences
+        B = self.hp.batch_size
+        self._check(obs, 'obs', (B, 4, 84, 84), (torch.uint8,))
+        self._check(next_obs, 'next_obs', (B, 4, 84, 84), (torch.uint8,))
+        self._check(action, 'action', (B,), (torch.int64,))
+        self._check(reward, 'reward', (B,), (torch.float32,))
+        self._check(done, 'done', (B,), (torch.bool, torch.uint8))
+        if weights is not None:
+            self._check(weights, 'weights', (B,), (torch.float32,))
+        if (idxs is None) != (sampler is None):
+            raise ValueError('idxs and sampler go together: pass both or neither')
+        if idxs is not None:
+            self._check(idxs, 'idxs', (B,), (torch.int64,))
+        return obs, action, reward, next_obs, done.view(torch.uint8)
+
+    def _enqueue(self, obs, action, reward, next_obs, done, weights, idxs, sampler):
+        _lib.check(self._L.srl_apex_learner_step(
+            self._h, obs.data_ptr(), action.data_ptr(), reward.data_ptr(), next_obs.data_ptr(), done.data_ptr(),
+            weights.data_ptr() if weights is not None else None, idxs.data_ptr() if idxs is not None else None,
+            sampler._h if sampler is not None else None, self._stats.data_ptr(), self._stream()), 'srl_apex_learner_step')
+
+    def _graph_step(self, args):
+        key = tuple(a.data_ptr() if isinstance(a, torch.Tensor) else (a._h.value if a is not None else None) for a in args)
+        g = self._graphs.get(key)
+        if g is None:
+            if key not in self._seen:          # first sight: eager (warm-up of attributes and allocator state)
+                self._seen.add(key)
+                self._enqueue(*args)
+                return
+            torch.cuda.current_stream(self.device).synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._enqueue(*args)
+            self._graphs[key] = g
+        g.replay()
+
+    @torch.no_grad()
+    def learn(self, experiences, weights: Optional[torch.Tensor] = None, idxs: Optional[torch.Tensor] = None, sampler=None,
+              sync_stats: bool = True, use_graph: Optional[bool] = None) -> Dict[str, float]:
+        """one update (apex/worker.py:134-161; dqn_agent.py:136-190) -> {'loss': float}, or {} with nothing synchronised"""
+        obs, action, reward, next_obs, done = self._inputs(experiences, weights, idxs, sampler)
+        args = (obs, action, reward, next_obs, done, weights, idxs, sampler)
+        if self.use_graph if use_graph is None else use_graph:
+            self._graph_step(args)
+        else:
+            self._enqueue(*args)
+        self._opt_steps += 1
+        if self.learner_update_step % self.hp.target_update_frequency == 0:
+            self.update_target(self.hp.soft_update_tau)
+            self.target_model_update_step += 1
+        self.learner_update_step += 1
+        if not sync_stats:
+            return {}
+        return {'loss': float(self._stats[0].item())}
+
+    def update_target(self, tau: float) -> None:
+        """soft_target_update(online, target, tau) (utils/model_utils.py:29-32) on the current stream"""
+        _lib.check(self._L.srl_apex_learner_update_target(self._h, float(tau), self._stream()), 'srl_apex_learner_update_target')
+
+    def stats(self) -> Dict[str, float]:
+        """{loss, grad_norm, clip_coef} of the last step (synchronises)"""
+        s = self._stats.tolist()
+        return {'loss': s[0], 'grad_norm': s[1], 'clip_coef': s[2]}
+
+    def debug_buffer(self, name: str) -> torch.Tensor:
+        """copy of one of the step's device buffers (tests only; names: srl_apex_learner_debug_buffer)"""
+        p, n = C.c_void_p(), C.c_int64()
+        _lib.check(self._L.srl_apex_learner_debug_buffer(self._h, name.encode(), C.byref(p), C.byref(n)), 'debug_buffer')
+        dt = {'priorities': torch.float64, 'step': torch.int32, 'a1': torch.bfloat16, 'a2': torch.bfloat16, 'a3': torch.bfloat16}.get(name, torch.float32)
+        out = torch.empty(n.value, dtype=dt, device=self.device)
+        _lib.check(self._L.srl_memcpy_d2d(out.data_ptr(), p.value, n.value * out.element_size(), self._stream()), 'memcpy_d2d')
+        torch.cuda.current_stream(self.device).synchronize()
+        return out
+
+    def release_graphs(self):
+        torch.cuda.synchronize(self.device)
+        self._graphs.clear()
+        self._seen.clear()
+
+    def close(self):
+        if getattr(self, '_h', None) is not None:
+            self._L.srl_apex_learner_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -889,3 +889,234 @@ extern "C" int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int fr
   CU(encoder_backward(frames, b, G, maps, E->precision, S, BWD_BOTH, false), "encoder_backward");
   return 0;
 }
+
+// ------------------------------------------------------------------------------------------------
+// Ape-X learner step: three encoder forwards on the context's blocks, the Q-learning tail (dqn.cu), the encoder backward over s,
+// clip + Adam, and the priorities into the sampler's trees
+// ------------------------------------------------------------------------------------------------
+// state_dict order {conv1.w, conv1.b, conv2.w, conv2.b, conv3.w, conv3.b, fc.w, fc.b, q.w, q.b}; in memory fc.weight last
+static int64_t apex_layout(int A, int64_t* off, int64_t* cnt) {
+  const int64_t counts[10] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, (int64_t)A * 512, A};
+  const int order[10] = {0, 1, 2, 3, 4, 5, 7, 8, 9, 6};
+  int64_t o = 0;
+  for (int k = 0; k < 10; ++k) {
+    const int i = order[k];
+    if (off) off[i] = o;
+    if (cnt) cnt[i] = counts[i];
+    o += (counts[i] + 3) & ~int64_t(3);
+  }
+  return o;
+}
+extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) { return apex_layout(A, offsets10, counts10); }
+
+struct srl_apex_learner {
+  srl_apex_config_t cfg;
+  float *params, *grads, *m, *v, *target;
+  int64_t nparams;
+  const float *w8[8], *t8[8];     // the encoder tensors of the online and target parameters
+  float* g8[8];
+  float *Wq, *bq, *Wt, *bt, *gWq, *gbq;
+  srl_encoder_t *E, *Eq;          // the step's encoder context, and the q-value forwards' own (lanes, events)
+  char *saved_s, *saved_n, *enc_scratch;   // encoder blocks: the forward over s (read by the backward), the forwards over s'
+  char *saved_q, *scratch_q;      // the q-value forwards' blocks: they may run on another stream than the step
+  float *core_s, *core_n, *core_nt, *dcore, *core_q;
+  float *q, *y, *dq, *loss, *tail_scratch, *head_part, *coef, *opt_scratch, *zero_reward;
+  double* prio;
+  int64_t* zero_action;
+  int* dstep;
+  char* arena;
+};
+
+// frames per q-value forward: srl_apex_learner_q_values runs n frames in chunks of at most this many
+constexpr int APEX_Q_CHUNK = 256;
+static int q_chunk(const srl_apex_config_t& c) { return c.B < APEX_Q_CHUNK ? c.B : APEX_Q_CHUNK; }
+// the encoder blocks' bytes for the step's B frames and for one q-value chunk: {saved, scratch, saved_q, scratch_q}
+static int apex_block_bytes(const srl_apex_config_t& c, int64_t* b4) {
+  int rc = srl_encoder_sizes(c.B, c.precision, &b4[0], &b4[1]);
+  return rc ? rc : srl_encoder_sizes(q_chunk(c), c.precision, &b4[2], &b4[3]);
+}
+// the context's device buffers in carving order; rows with a name are what srl_apex_learner_debug_buffer lends
+static int apex_rows(srl_apex_learner* L, const int64_t* b4, WsRow* t) {
+  const int64_t B = L->cfg.B, A = L->cfg.A, QC = q_chunk(L->cfg);
+  int n = 0;
+  t[n++] = ws_row<char>(nullptr, b4[0], &L->saved_s);
+  t[n++] = ws_row<char>(nullptr, b4[0], &L->saved_n);
+  t[n++] = ws_row<char>(nullptr, b4[1], &L->enc_scratch);
+  t[n++] = ws_row<char>(nullptr, b4[2], &L->saved_q);
+  t[n++] = ws_row<char>(nullptr, b4[3], &L->scratch_q);
+  t[n++] = ws_row(nullptr, QC * ENC_CORE, &L->core_q);
+  t[n++] = ws_row("core", B * ENC_CORE, &L->core_s);
+  t[n++] = ws_row("core_next", L->cfg.double_dqn ? B * ENC_CORE : 0, &L->core_n);
+  t[n++] = ws_row("core_next_target", B * ENC_CORE, &L->core_nt);
+  t[n++] = ws_row("dcore", B * ENC_CORE, &L->dcore);
+  t[n++] = ws_row("q", B, &L->q);
+  t[n++] = ws_row("y", B, &L->y);
+  t[n++] = ws_row("priorities", B, &L->prio);
+  t[n++] = ws_row("loss", 4, &L->loss);
+  t[n++] = ws_row("step", 4, &L->dstep);
+  t[n++] = ws_row(nullptr, B, &L->dq);
+  t[n++] = ws_row(nullptr, 4 + dqn_tail_blocks((int)B), &L->tail_scratch);
+  t[n++] = ws_row(nullptr, HEAD_GROUPS * A * 513, &L->head_part);
+  t[n++] = ws_row(nullptr, 4, &L->coef);
+  t[n++] = ws_row(nullptr, 2048, &L->opt_scratch);
+  t[n++] = ws_row(nullptr, QC, &L->zero_reward);     // the reward / action columns of the q-value forwards (the Q head reads h only)
+  t[n++] = ws_row(nullptr, QC, &L->zero_action);
+  return n;
+}
+constexpr int APEX_ROWS = 22;
+
+static int check_apex_cfg(const srl_apex_config_t* c) {
+  REQ(c, "apex_learner: config is NULL");
+  REQ(c->B >= 1 && c->B <= MAX_FRAMES, "apex_learner: B=%d must be in [1, %d]", c->B, MAX_FRAMES);
+  REQ(c->A >= 1 && c->A <= 31, "apex_learner: A=%d must be in [1,31]", c->A);
+  REQ(c->precision == 0 || c->precision == 1, "apex_learner: precision must be 0 (bf16 operands) or 1 (fp32-accurate split operands)");
+  REQ(c->double_dqn == 0 || c->double_dqn == 1, "apex_learner: double_dqn must be 0 or 1");
+  REQ(std::isfinite(c->gamma) && c->gamma >= 0.f, "apex_learner: gamma=%g must be finite and >= 0", (double)c->gamma);
+  REQ(c->max_grad_norm > 0.f, "apex_learner: max_grad_norm=%g must be > 0 (+inf: no clipping)", (double)c->max_grad_norm);
+  REQ(std::isfinite(c->learning_rate) && c->learning_rate > 0.f, "apex_learner: learning_rate=%g must be finite and > 0", (double)c->learning_rate);
+  REQ(c->adam_beta1 >= 0.f && c->adam_beta1 < 1.f && c->adam_beta2 >= 0.f && c->adam_beta2 < 1.f, "apex_learner: Adam betas must be in [0, 1)");
+  REQ(std::isfinite(c->adam_eps) && c->adam_eps >= 0.f, "apex_learner: adam_eps=%g must be finite and >= 0", (double)c->adam_eps);
+  REQ(std::isfinite(c->priority_eps) && c->priority_eps >= 0.f, "apex_learner: priority_eps=%g must be finite and >= 0", (double)c->priority_eps);
+  return 0;
+}
+
+extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* params, float* grads, float* exp_avg, float* exp_avg_sq,
+                                       float* target_params, srl_apex_learner_t** out) {
+  int rc = check_apex_cfg(cfg);
+  if (rc) return rc;
+  REQ(params && grads && exp_avg && exp_avg_sq && target_params && out, "apex_learner_create: NULL argument");
+  REQ(!misaligned(params, 16) && !misaligned(grads, 16) && !misaligned(exp_avg, 16) && !misaligned(exp_avg_sq, 16) &&
+      !misaligned(target_params, 16), "apex_learner_create: flat buffers must be 16-byte aligned");
+  int64_t off[10];
+  const int64_t np = apex_layout(cfg->A, off, nullptr);
+  const Span s[5] = {{params, np * 4, true, "params"}, {grads, np * 4, true, "grads"}, {exp_avg, np * 4, true, "exp_avg"},
+                     {exp_avg_sq, np * 4, true, "exp_avg_sq"}, {target_params, np * 4, true, "target_params"}};
+  rc = check_spans(s, 5, "apex_learner_create");
+  if (rc) return rc;
+  srl_apex_learner* L = new (std::nothrow) srl_apex_learner();
+  REQ(L, "out of host memory");
+  auto undo = [L](int code) { srl_apex_learner_destroy(L); return code; };
+  L->cfg = *cfg; L->params = params; L->grads = grads; L->m = exp_avg; L->v = exp_avg_sq; L->target = target_params; L->nparams = np;
+  for (int i = 0; i < 8; ++i) { L->w8[i] = params + off[i]; L->t8[i] = target_params + off[i]; L->g8[i] = grads + off[i]; }
+  L->Wq = params + off[8]; L->bq = params + off[9]; L->Wt = target_params + off[8]; L->bt = target_params + off[9];
+  L->gWq = grads + off[8]; L->gbq = grads + off[9];
+  rc = srl_encoder_create(cfg->precision, &L->E);
+  if (!rc) rc = srl_encoder_create(cfg->precision, &L->Eq);
+  if (rc) return undo(rc);
+  int64_t b4[4];
+  rc = apex_block_bytes(*cfg, b4);
+  if (rc) return undo(rc);
+  WsRow t[APEX_ROWS];
+  const int n = apex_rows(L, b4, t);
+  const int64_t total = rows_bytes(t, n, false);
+  cudaError_t e = cudaMalloc(&L->arena, total);
+  if (e != cudaSuccess) return undo(cuda_fail(e, "apex_learner_create: cudaMalloc workspace"));
+  e = cudaMemset(L->arena, 0, total);        // the tail's ticket, the step count and the zero reward / action columns
+  if (e == cudaSuccess) e = cudaMemset(grads, 0, np * 4);      // the padding between the segments enters the gradient norm
+  if (e != cudaSuccess) return undo(cuda_fail(e, "apex_learner_create: cudaMemset"));
+  carve_rows(t, n, false, L->arena);
+  *out = L;
+  return 0;
+}
+
+extern "C" int srl_apex_learner_destroy(srl_apex_learner_t* L) {
+  if (!L) return 0;
+  srl_encoder_destroy(L->E);
+  srl_encoder_destroy(L->Eq);
+  cudaFree(L->arena);
+  delete L;
+  return 0;
+}
+
+extern "C" int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, const int64_t* action, const float* reward, const uint8_t* next_obs,
+                                     const uint8_t* done, const float* weights, const int64_t* idxs, srl_per_t* per, float* stats_out, void* stream) {
+  REQ(L && obs && action && reward && next_obs && done, "apex_learner_step: NULL pointer");
+  REQ(!idxs == !per, "apex_learner_step: idxs and per go together (both NULL or both set)");
+  const srl_apex_config_t& c = L->cfg;
+  const int B = c.B;
+  const cudaStream_t st = (cudaStream_t)stream;
+  // the three forwards (the encoder checks obs / next_obs and the blocks); the target forward runs last so that its rows are the
+  // ones left in saved_n
+  int rc = srl_encoder_forward(L->E, obs, reward, action, B, 1, L->w8, L->saved_s, L->enc_scratch, L->core_s, stream);
+  if (!rc && c.double_dqn) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->w8, L->saved_n, L->enc_scratch, L->core_n, stream);
+  if (!rc) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->t8, L->saved_n, L->enc_scratch, L->core_nt, stream);
+  if (rc) return rc;
+  DqnTail t;
+  t.core_s = L->core_s; t.core_n = c.double_dqn ? L->core_n : nullptr; t.core_nt = L->core_nt;
+  t.Wq = L->Wq; t.bq = L->bq; t.Wt = L->Wt; t.bt = L->bt;
+  t.action = action; t.reward = reward; t.done = done; t.weight = weights;
+  t.B = B; t.A = c.A; t.gamma = c.gamma; t.two_over_B = 2.f / (float)B; t.priority_eps = c.priority_eps;
+  t.q = L->q; t.y = L->y; t.dq = L->dq; t.dcore = L->dcore; t.loss = L->loss; t.scratch = L->tail_scratch; t.prio = L->prio;
+  CU(launch_dqn_tail(t, st), "dqn_tail");
+  CU(launch_dqn_wgrad(L->dq, action, L->core_s, B, c.A, L->head_part, L->gWq, L->gbq, st), "dqn_wgrad");
+  rc = srl_encoder_backward(L->E, L->dcore, B, 1, L->saved_s, L->enc_scratch, L->g8, stream);
+  if (rc) return rc;
+  const OptStep o = {1, L->params, L->grads, L->m, L->v, L->nparams, c.max_grad_norm, L->coef, L->opt_scratch, c.learning_rate,
+                     c.adam_beta1, c.adam_beta2, c.adam_eps, 0, L->dstep, OptExtra{}};
+  CU(launch_clip_optim(o, st), "clip+adam");
+  if (per) {
+    rc = srl_per_update_priorities(per, idxs, L->prio, B, stream);       // <= 1024 pairs per launch, in order: the last idx wins
+    if (rc) return rc;
+  }
+  if (stats_out) {
+    CU(cudaMemcpyAsync(stats_out, L->loss, sizeof(float), cudaMemcpyDeviceToDevice, st), "copy loss");
+    CU(cudaMemcpyAsync(stats_out + 1, L->coef, 2 * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy coef");
+  }
+  return 0;
+}
+
+extern "C" int srl_apex_learner_update_target(srl_apex_learner_t* L, float tau, void* stream) {
+  REQ(L, "apex_learner_update_target: learner is NULL");
+  REQ(tau >= 0.f && tau <= 1.f, "apex_learner_update_target: tau=%g must be in [0, 1]", (double)tau);
+  // torch evaluates (1.0 - tau) in double and rounds it once to the tensor's float
+  CU(launch_apex_soft_update(L->params, L->target, L->nparams, tau, (float)(1.0 - (double)tau), (cudaStream_t)stream), "apex_soft_update");
+  return 0;
+}
+
+extern "C" int srl_apex_learner_set_step(srl_apex_learner_t* L, int64_t step, void* stream) {
+  REQ(L && step >= 0 && step < (int64_t(1) << 31), "apex_learner_set_step: bad argument");
+  const int v = (int)step;
+  CU(cudaMemcpyAsync(L->dstep, &v, sizeof(int), cudaMemcpyHostToDevice, (cudaStream_t)stream), "apex_learner_set_step");
+  CU(cudaStreamSynchronize((cudaStream_t)stream), "apex_learner_set_step");      // `v` is a stack variable
+  return 0;
+}
+
+extern "C" int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* obs, int n, float* q_out, void* stream) {
+  REQ(L && obs && q_out, "apex_learner_q_values: NULL pointer");
+  REQ(n >= 1, "apex_learner_q_values: n=%d must be >= 1", n);
+  const int QC = q_chunk(L->cfg), A = L->cfg.A;
+  const Span s[2] = {{obs, (int64_t)n * 28224, false, "obs"}, {q_out, (int64_t)n * A * 4, true, "q_out"}};
+  int rc = check_spans(s, 2, "apex_learner_q_values");
+  if (rc) return rc;
+  for (int f0 = 0; f0 < n; f0 += QC) {       // chunks through the q-value forwards' own context and blocks
+    const int f = n - f0 < QC ? n - f0 : QC;
+    rc = srl_encoder_forward(L->Eq, obs + (size_t)f0 * 28224, L->zero_reward, L->zero_action, f, 1, L->w8, L->saved_q, L->scratch_q,
+                             L->core_q, stream);
+    if (rc) return rc;
+    CU(launch_dqn_q_values(L->core_q, L->Wq, L->bq, f, A, q_out + (size_t)f0 * A, (cudaStream_t)stream), "dqn_q_values");
+  }
+  return 0;
+}
+
+extern "C" int srl_apex_learner_debug_buffer(srl_apex_learner_t* L, const char* name, void** ptr, int64_t* count) {
+  REQ(L && name && ptr && count, "apex_learner_debug_buffer: NULL argument");
+  {   // the activations the forward over s saved for its backward (bf16; the high parts in the fp32-accurate mode)
+    EncoderBuffers b = {};
+    WsRow e[ENC_ROWS];
+    encoder_rows(b, L->cfg.B, L->cfg.B, e);
+    carve_rows(e, ENC_SAVED_ROWS, L->cfg.precision == 1, L->saved_s);
+    for (int i = 0; i < ENC_SAVED_ROWS; ++i)
+      if (strcmp(name, "a1") == 0 || strcmp(name, "a2") == 0 || strcmp(name, "a3") == 0)
+        if (strcmp(e[i].name, name) == 0) { *ptr = *e[i].hi; *count = e[i].count; return 0; }
+  }
+  int64_t b4[4];
+  int rc = apex_block_bytes(L->cfg, b4);
+  if (rc) return rc;
+  srl_apex_learner shadow = *L;        // the table's rows re-derived on a copy: the same sizes give the same addresses
+  WsRow t[APEX_ROWS];
+  const int n = apex_rows(&shadow, b4, t);
+  carve_rows(t, n, false, L->arena);
+  for (int i = 0; i < n; ++i)
+    if (t[i].name && strcmp(t[i].name, name) == 0 && t[i].count > 0) { *ptr = *t[i].hi; *count = t[i].count; return 0; }
+  return fail(SRL_EINVAL, "apex_learner_debug_buffer: unknown buffer '%s'", name);
+}

@@ -229,4 +229,12 @@ SRL_DEVINL float warp_sum(float v) {
   return v;
 }
 
+// The ticket of a two-level deterministic reduction (the IMPALA and DQN loss tails): scratch[0] counts the blocks that have
+// published their partials.  One thread per block calls it after its stores; true in the block that published last, which then
+// sums the partials in its kernel's fixed order and re-arms the ticket (scratch[0] = 0).
+SRL_DEVINL bool take_ticket(float* scratch) {
+  __threadfence();
+  return atomicAdd(reinterpret_cast<unsigned*>(scratch), 1u) == gridDim.x - 1;
+}
+
 }  // namespace srl

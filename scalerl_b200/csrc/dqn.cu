@@ -1,0 +1,177 @@
+// The Q-learning tail of the Ape-X / DQN learner step, fp32 on the CUDA cores (the Q head is 512 x A: no tensor-core work):
+//   dqn_tail_kernel           q(s,a), the bootstrapped target y, priorities |q - y| + eps, the loss mean(w (q - y)^2) through the
+//                             ticket reduction of the IMPALA tail, dq and the dcore rows of the encoder backward
+//                             (apex/worker.py:148-157; dqn/dqn_agent.py:155-171)
+//   dqn_wgrad_kernel /        the Q head's weight and bias gradients: slab-group partials added in group order (the order of
+//   dqn_wgrad_reduce_kernel   heads.cu's head_wgrad kernels), so every run computes the same bits
+//   dqn_q_values_kernel       the forward-only Q head (predict / get_action)
+//   apex_soft_update_kernel   theta_t <- tau theta + (1 - tau) theta_t (dqn_agent.py:185-190, utils/model_utils.py:29-32)
+// The Q head reads the encoder's core rows [h (512), clamp(reward), one-hot] (ENC_CORE floats per row) and only their h columns.
+#include "common.cuh"
+#include "kernels.h"
+
+namespace srl {
+
+// q = h . W[a] + b[a] for one 512-float row h of a core row and one 512-float weight row: lane-strided products, then the warp sum
+SRL_DEVINL float q_dot(const float* __restrict__ h, const float* __restrict__ w, int lane) {
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) s = fmaf(__ldg(h + lane + 32 * i), __ldg(w + lane + 32 * i), s);
+  return warp_sum(s);
+}
+// max_a Q(h)[a] and its first argmax (torch.max(dim=1) returns the first maximal index)
+SRL_DEVINL float q_max(const float* h, const float* W, const float* b, int A, int lane, int* arg) {
+  float best = -INFINITY;
+  int ib = 0;
+  for (int a = 0; a < A; ++a) {
+    const float v = q_dot(h, W + (size_t)a * 512, lane) + __ldg(b + a);
+    if (v > best) { best = v; ib = a; }
+  }
+  *arg = ib;
+  return best;
+}
+
+// One warp per transition, 4 per block.  scratch: [0] the ticket, [4 + k] block k's partial of sum_n w_n (q_n - y_n)^2.
+__global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int n = blockIdx.x * 4 + warp;
+  float l = 0.f;
+  if (n < t.B) {
+    const int act = ld_action(t.action + n, t.A);
+    const float* hs = t.core_s + (size_t)n * ENC_CORE;
+    const float q = q_dot(hs, t.Wq + (size_t)act * 512, lane) + __ldg(t.bq + act);
+    const float* hn = t.core_nt + (size_t)n * ENC_CORE;
+    int a_star;
+    float nx;
+    if (t.core_n) {     // double DQN: the online network picks a*, the target network values it (dqn_agent.py:155-160)
+      q_max(t.core_n + (size_t)n * ENC_CORE, t.Wq, t.bq, t.A, lane, &a_star);
+      nx = q_dot(hn, t.Wt + (size_t)a_star * 512, lane) + __ldg(t.bt + a_star);
+    } else {            // max_a Q_target(s', a) (apex/worker.py:149, dqn_agent.py:162-163)
+      nx = q_max(hn, t.Wt, t.bt, t.A, lane, &a_star);
+    }
+    // y = r + gamma * Q' * (1 - d), the products and the add rounded one by one as torch evaluates them (no FMA contraction)
+    const float nd = t.done[n] ? 0.f : 1.f;
+    const float y = __fadd_rn(__ldg(t.reward + n), __fmul_rn(__fmul_rn(t.gamma, nx), nd));
+    const float w = t.weight ? __ldg(t.weight + n) : 1.f;
+    const float delta = __fsub_rn(q, y);
+    l = __fmul_rn(w, __fmul_rn(delta, delta));
+    // d loss / d q of mean(w (q - y)^2): the gradient flows through q only (y is detached)
+    const float dq = t.two_over_B * w * delta;
+    if (lane == 0) {
+      t.q[n] = q; t.y[n] = y; t.dq[n] = dq;
+      t.prio[n] = (double)fabsf(delta) + (double)t.priority_eps;      // apex/worker.py:152-154 (+ eps > 0 keeps the tree's assert)
+    }
+    const float* wa = t.Wq + (size_t)act * 512;
+    float* dc = t.dcore + (size_t)n * ENC_CORE;
+    for (int j = lane; j < ENC_CORE; j += 32) dc[j] = j < 512 ? dq * __ldg(wa + j) : 0.f;
+  }
+  // block partial: the warps' losses in warp order, then the ticket; the last block adds the partials in block order
+  __shared__ float red[4];
+  __shared__ bool is_last;
+  if (lane == 0) red[warp] = l;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    t.scratch[4 + blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
+    is_last = take_ticket(t.scratch);
+  }
+  __syncthreads();
+  if (is_last && warp == 0) {
+    __threadfence();
+    float s = 0.f;
+    for (unsigned k = lane; k < gridDim.x; k += 32) s += reinterpret_cast<volatile float*>(t.scratch)[4 + k];
+    s = warp_sum(s);
+    if (lane == 0) {
+      t.loss[0] = s / (float)t.B;
+      *reinterpret_cast<unsigned*>(t.scratch) = 0u;      // re-arm the ticket
+    }
+  }
+}
+
+// Q head weight/bias gradients: thread = one column j of h (j == 512 is the bias "ones" column), blockIdx.y = a group of consecutive
+// slabs of transitions.  Row a of a slab carries dq only for the transition's action.  Each group writes part[group][a][j].
+constexpr int DQN_SLAB = 16, DQN_MAX_A = 32;
+__global__ void __launch_bounds__(128) dqn_wgrad_kernel(const float* __restrict__ dq, const int64_t* __restrict__ action,
+                                                        const float* __restrict__ core, int N, int A, int slabs_per_group,
+                                                        float* __restrict__ part) {
+  __shared__ float sd[DQN_SLAB][DQN_MAX_A];
+  const int j = blockIdx.x * 128 + threadIdx.x;
+  const int nslab = (N + DQN_SLAB - 1) / DQN_SLAB;
+  const int s0 = blockIdx.y * slabs_per_group, s1 = min(nslab, s0 + slabs_per_group);
+  float acc[DQN_MAX_A];
+#pragma unroll
+  for (int a = 0; a < DQN_MAX_A; ++a) acc[a] = 0.f;
+  for (int sl = s0; sl < s1; ++sl) {
+    const int n0 = sl * DQN_SLAB, cnt = min(DQN_SLAB, N - n0);
+    __syncthreads();                 // the previous slab's shared rows have been read
+    for (int i = threadIdx.x; i < DQN_SLAB * A; i += 128) {     // rows past the ragged end are zero
+      const int r = i / A, a = i - r * A;
+      sd[r][a] = (r < cnt && ld_action(action + n0 + r, A) == a) ? __ldg(dq + n0 + r) : 0.f;
+    }
+    __syncthreads();
+    if (j > 512) continue;
+    float c[DQN_SLAB];
+#pragma unroll
+    for (int r = 0; r < DQN_SLAB; ++r) c[r] = r < cnt ? (j < 512 ? __ldg(core + (size_t)(n0 + r) * ENC_CORE + j) : 1.f) : 0.f;
+#pragma unroll
+    for (int a = 0; a < DQN_MAX_A; ++a) {
+      if (a >= A) break;
+#pragma unroll
+      for (int r = 0; r < DQN_SLAB; ++r) acc[a] = fmaf(sd[r][a], c[r], acc[a]);
+    }
+  }
+  if (j > 512) return;
+#pragma unroll
+  for (int a = 0; a < DQN_MAX_A; ++a)
+    if (a < A) part[((size_t)blockIdx.y * A + a) * 513 + j] = acc[a];
+}
+// sums the groups' partials in group order into the Q head gradients (stored, not accumulated)
+__global__ void __launch_bounds__(256) dqn_wgrad_reduce_kernel(const float* __restrict__ part, int groups, int A, float* __restrict__ gW,
+                                                               float* __restrict__ gb) {
+  const int n = A * 513, i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float s = 0.f;
+  for (int g = 0; g < groups; ++g) s += __ldg(part + (size_t)g * n + i);
+  const int a = i / 513, j = i - a * 513;
+  if (j < 512) gW[(size_t)a * 512 + j] = s; else gb[a] = s;
+}
+
+// q_out[n][a] = h[n] . W[a] + b[a]: the tail's head arithmetic without the loss (one warp per frame)
+__global__ void __launch_bounds__(128) dqn_q_values_kernel(const float* __restrict__ core, const float* __restrict__ W, const float* __restrict__ b,
+                                                           int N, int A, float* __restrict__ q_out) {
+  const int lane = threadIdx.x & 31, n = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (n >= N) return;
+  for (int a = 0; a < A; ++a) {
+    const float v = q_dot(core + (size_t)n * ENC_CORE, W + (size_t)a * 512, lane) + __ldg(b + a);
+    if (lane == 0) q_out[(size_t)n * A + a] = v;
+  }
+}
+
+// theta_t = tau * theta + one_minus_tau * theta_t, each product and the sum rounded separately as torch computes it
+__global__ void __launch_bounds__(256) apex_soft_update_kernel(const float* __restrict__ p, float* __restrict__ pt, int64_t n, float tau,
+                                                               float one_minus_tau) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    pt[i] = __fadd_rn(__fmul_rn(tau, p[i]), __fmul_rn(one_minus_tau, pt[i]));
+}
+
+cudaError_t launch_dqn_tail(const DqnTail& t, cudaStream_t st) {
+  dqn_tail_kernel<<<dqn_tail_blocks(t.B), 128, 0, st>>>(t);
+  return cudaGetLastError();
+}
+cudaError_t launch_dqn_wgrad(const float* dq, const int64_t* action, const float* core, int N, int A, float* part, float* gW, float* gb,
+                             cudaStream_t st) {
+  const int nslab = (N + DQN_SLAB - 1) / DQN_SLAB, spg = (nslab + HEAD_GROUPS - 1) / HEAD_GROUPS, groups = (nslab + spg - 1) / spg;
+  dqn_wgrad_kernel<<<dim3((513 + 127) / 128, groups), 128, 0, st>>>(dq, action, core, N, A, spg, part);
+  dqn_wgrad_reduce_kernel<<<(A * 513 + 255) / 256, 256, 0, st>>>(part, groups, A, gW, gb);
+  return cudaGetLastError();
+}
+cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* b, int N, int A, float* q_out, cudaStream_t st) {
+  dqn_q_values_kernel<<<(N + 3) / 4, 128, 0, st>>>(core, W, b, N, A, q_out);
+  return cudaGetLastError();
+}
+cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st) {
+  const int64_t blocks = (n + 255) / 256;
+  apex_soft_update_kernel<<<(int)(blocks < 1024 ? blocks : 1024), 256, 0, st>>>(p, pt, n, tau, one_minus_tau);
+  return cudaGetLastError();
+}
+
+}  // namespace srl

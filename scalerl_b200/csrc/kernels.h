@@ -216,6 +216,29 @@ cudaError_t launch_rmsprop(float* p, const float* g, float* v, int64_t n, const 
 cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, const float* coef, float lr, float b1, float b2, float eps,
                         int step, cudaStream_t st);
 
+// ---- dqn.cu: the Q-learning tail of the Ape-X learner step (srl_apex_learner_*)
+// The encoder runs with a one-hot width of 1 for the Q network: its core rows are [h (512), clamp(reward), 1], ENC_CORE floats.
+constexpr int ENC_CORE = 514;
+// one batch of B transitions: core rows of the online forward over s, the online forward over s' (null: plain max, no double DQN) and
+// the target forward over s'; the Q heads [A][512] + [A]; the batch columns; outputs q, y, dq f32 [B], priorities f64 [B], dcore
+// [B][ENC_CORE] and loss f32 [1].  scratch: 4 + dqn_tail_blocks(B) floats, zero before the first launch (re-armed by the kernel).
+struct DqnTail {
+  const float *core_s, *core_n, *core_nt;
+  const float *Wq, *bq, *Wt, *bt;
+  const int64_t* action; const float* reward; const uint8_t* done; const float* weight;
+  int B, A;
+  float gamma, two_over_B, priority_eps;
+  float *q, *y, *dq, *dcore, *loss, *scratch;
+  double* prio;
+};
+inline int dqn_tail_blocks(int B) { return (B + 3) / 4; }
+cudaError_t launch_dqn_tail(const DqnTail& t, cudaStream_t st);
+// the Q head gradients gW [A][512], gb [A] (stored) from dq and the actions over the core rows; part: HEAD_GROUPS * A * 513 floats
+cudaError_t launch_dqn_wgrad(const float* dq, const int64_t* action, const float* core, int N, int A, float* part, float* gW, float* gb,
+                             cudaStream_t st);
+cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* b, int N, int A, float* q_out, cudaStream_t st);
+cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
+
 // ---- encoder.cu
 // packed bf16 operand copies of the conv/fc weights (element offsets into one buffer)
 struct WPack {

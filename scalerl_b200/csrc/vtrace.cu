@@ -65,12 +65,8 @@ SRL_DEVINL void scan_compose(int lane, float& aa, float& bb) {
 }
 
 // Deterministic loss reduction: scratch[0] counts the blocks that have published their partials (scratch[4 + 3 k ..] for block k).
-// One thread per block calls take_ticket after its stores: true in the block that published last, which sums the partials in its
-// kernel's fixed order and calls write_losses.
-SRL_DEVINL bool take_ticket(float* scratch) {
-  __threadfence();
-  return atomicAdd(reinterpret_cast<unsigned*>(scratch), 1u) == gridDim.x - 1;
-}
+// One thread per block calls take_ticket (common.cuh) after its stores: true in the block that published last, which sums the
+// partials in its kernel's fixed order and calls write_losses.
 SRL_DEVINL void write_losses(float* losses, float* scratch, float s_pg, float s_bl, float s_ent, float baseline_cost, float entropy_cost) {
   const float a = s_pg, c = baseline_cost * s_bl, e = entropy_cost * s_ent;
   losses[0] = a; losses[1] = c; losses[2] = e; losses[3] = a + c + e;

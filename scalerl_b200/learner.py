@@ -63,12 +63,13 @@ def _torch_param_groups(hp: 'ImpalaHParams', n: int, step: int = 0, frames_per_s
 
 
 def to_torch_optimizer_state(hp: 'ImpalaHParams', tensors: Dict[str, Dict[str, torch.Tensor]], step: int,
-                             frames_per_step: float = 0.0) -> dict:
+                             frames_per_step: float = 0.0, order=None) -> dict:
     """``torch.optim.RMSprop(...).state_dict()`` / ``Adam`` layout (what ImpalaTrainer.save_checkpoint stores,
     impala_atari.py:506-511): {'state': {i: {'step', 'square_avg' [, 'momentum_buffer'] | 'exp_avg','exp_avg_sq'}},
     'param_groups': [...]}, i = index in AtariNet.parameters() order.  ``tensors``: kind -> name -> tensor.  No state before the
-    first step, as torch (state is created lazily).  ``frames_per_step``: F of the 'linear' schedule (the current lr)."""
-    order = reference_param_order(hp.use_lstm)
+    first step, as torch (state is created lazily).  ``frames_per_step``: F of the 'linear' schedule (the current lr).  ``order``: the
+    parameter names in the model's ``parameters()`` order (default: AtariNet's)."""
+    order = reference_param_order(hp.use_lstm) if order is None else order
     state = {}
     if step > 0:
         for i, n in enumerate(order):
@@ -79,10 +80,10 @@ def to_torch_optimizer_state(hp: 'ImpalaHParams', tensors: Dict[str, Dict[str, t
     return {'state': state, 'param_groups': _torch_param_groups(hp, len(order), step, frames_per_step)}
 
 
-def from_torch_optimizer_state(sd: dict, use_lstm: bool, momentum: bool = False):
+def from_torch_optimizer_state(sd: dict, use_lstm: bool, momentum: bool = False, order=None):
     """inverse of to_torch_optimizer_state; also accepts round 1's {'step', 'state': {kind: {name: tensor}}} layout.
     -> (step, {kind: {name: tensor}}).  'momentum_buffer' is read only when ``momentum`` (the learner runs RMSprop momentum).
-    Unknown layouts raise (never silently skipped)."""
+    Unknown layouts raise (never silently skipped).  ``order``: as to_torch_optimizer_state."""
     if not sd:
         return 0, {}
     state = sd.get('state', {})
@@ -91,7 +92,7 @@ def from_torch_optimizer_state(sd: dict, use_lstm: bool, momentum: bool = False)
         if state and not kinds:
             raise ValueError(f'optimizer_state_dict: unknown layout (keys {list(state)[:4]})')
         return int(sd.get('step', 0)), kinds
-    order = reference_param_order(use_lstm)
+    order = reference_param_order(use_lstm) if order is None else order
     if not state:
         return 0, {}
     if sorted(state) != list(range(len(order))):

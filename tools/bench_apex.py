@@ -1,0 +1,140 @@
+"""Learner steps/s and transitions/s of the Ape-X learner step (B200ApexLearner, captured, bf16 operands) against the reference's
+statements (apex/worker.py:148-161) on torch/cuDNN with AtariQNet, eager and captured as a CUDA graph.  Each variant writes its
+priorities into a GpuPrioritizedSampler of its own.  Rounds alternate between the variants; the median and range over rounds are
+printed with the card's name and power limit, one JSON line per configuration.
+
+    python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from scalerl_b200.algorithms.apex import ApexHParams, AtariQNet, B200ApexLearner, default_q_state_dict  # noqa: E402
+from scalerl_b200.data.per_sampler import GpuPrioritizedSampler  # noqa: E402
+
+MEMORY = 4096        # sampler capacity: the sampled indices' range
+
+
+def card():
+    """'<name>, <power limit>' as nvidia-smi reports them (the name alone when nvidia-smi is unavailable)"""
+    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
+
+
+def batch(B, A):
+    g = torch.Generator(device='cuda').manual_seed(0)
+    obs = torch.randint(0, 256, (B, 4, 84, 84), dtype=torch.uint8, device='cuda', generator=g)
+    nobs = torch.randint(0, 256, (B, 4, 84, 84), dtype=torch.uint8, device='cuda', generator=g)
+    act = torch.randint(0, A, (B,), device='cuda', generator=g)
+    rew = torch.randn(B, device='cuda', generator=g)
+    done = torch.rand(B, device='cuda', generator=g) < 0.05
+    w = torch.rand(B, device='cuda', generator=g)
+    idxs = torch.randint(0, MEMORY, (B,), device='cuda', generator=g)
+    return (obs, act, rew, nobs, done), w, idxs
+
+
+def sampler():
+    S = GpuPrioritizedSampler(MEMORY)
+    S.add(MEMORY)
+    return S
+
+
+class TorchStep:
+    """the reference's statements on torch/cuDNN (the priorities stay on the device and go into the GPU sampler).  The object owns
+    every tensor the step reads or writes, so a captured replay of it stays valid as long as the object lives."""
+
+    def __init__(self, B, A, exp, w, idxs, gamma=0.99):
+        sd = default_q_state_dict(A)
+        self.model, self.target = AtariQNet(A).cuda(), AtariQNet(A).cuda()
+        self.model.load_state_dict(sd)
+        self.target.load_state_dict(sd)
+        self.opt = torch.optim.Adam(self.model.parameters(), lr=1e-3, capturable=True)
+        self.S, self.gamma, self.idxs = sampler(), gamma, idxs
+        obs, act, rew, nobs, done = exp
+        self.obs, self.nobs = obs, nobs
+        self.actions, self.rewards, self.dones, self.weights = act.unsqueeze(1), rew.unsqueeze(1), done.float().unsqueeze(1), w.unsqueeze(1)
+        self.prio = torch.empty(B, dtype=torch.float64, device='cuda')
+
+    def __call__(self):
+        current_q_values = self.model(self.obs).gather(1, self.actions)                       # worker.py:148
+        with torch.no_grad():
+            next_q_values = self.target(self.nobs).max(1, keepdim=True)[0]                    # :149
+        target_q_values = self.rewards + (1 - self.dones) * self.gamma * next_q_values        # :150
+        self.prio.copy_(torch.abs(current_q_values - target_q_values).detach().squeeze(1))    # :152-154
+        loss = (self.weights * (current_q_values - target_q_values.detach()) ** 2).mean()     # :156-157
+        self.opt.zero_grad(set_to_none=False)
+        loss.backward()
+        self.opt.step()
+        self.S.update_priorities(self.idxs, self.prio, validate=False)
+
+
+class Captured:
+    """a CUDA graph of `step` (warmed up on a side stream first); holds `step`, whose tensors the graph reads and writes"""
+
+    def __init__(self, step):
+        self.step = step
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            for _ in range(3):
+                step()
+        torch.cuda.current_stream().wait_stream(s)
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            step()
+
+    def __call__(self):
+        self.graph.replay()
+
+
+def timed(fn, steps):
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(steps):
+        fn()
+    torch.cuda.synchronize()
+    return steps / (time.perf_counter() - t0)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--rounds', type=int, default=5)
+    ap.add_argument('--steps', type=int, default=50)
+    ap.add_argument('--configs', default='32x6,32x18,512x6,512x18')
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit('bench_apex.py measures on a CUDA device; none is present')
+    name = card()
+    for cfg in a.configs.split(','):
+        B, A = (int(x) for x in cfg.split('x'))
+        exp, w, idxs = batch(B, A)
+        L, S = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A)), sampler()
+        variants = {'b200_captured': lambda: L.learn(exp, weights=w, idxs=idxs, sampler=S, sync_stats=False),
+                    'torch_eager': TorchStep(B, A, exp, w, idxs),
+                    'torch_captured': Captured(TorchStep(B, A, exp, w, idxs))}
+        for fn in variants.values():           # warm-up: the learner's first call runs eagerly, the second captures
+            for _ in range(3):
+                fn()
+        rates = {k: [] for k in variants}
+        for _ in range(a.rounds):
+            for k, fn in variants.items():
+                rates[k].append(timed(fn, a.steps))
+        out = {'card': name, 'B': B, 'A': A, 'precision': 'bf16', 'rounds': a.rounds, 'steps_per_round': a.steps}
+        for k, r in rates.items():
+            r = sorted(r)
+            out[k] = {'steps_per_s_median': r[len(r) // 2], 'steps_per_s_range': [r[0], r[-1]],
+                      'transitions_per_s_median': r[len(r) // 2] * B}
+        print(json.dumps(out), flush=True)
+        del variants
+        L.release_graphs()
+        L.close()
+
+
+if __name__ == '__main__':
+    main()
