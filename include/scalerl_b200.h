@@ -313,7 +313,7 @@ int srl_lstm_core_backward(const float* dout, const float* dhT, const float* dcT
 /* ---- prioritized-replay sampler (BASELINE.json configs[3]; SURVEY.md §8f) ---------------------------------------------------
  * Device-resident float64 sum/min segment trees; replaces PrioritizedReplayBuffer's tree arithmetic
  * (scalerl/data/replay_buffer.py:305-381 over scalerl/data/segment_tree.py:7-196).  Index results are identical to the
- * reference's Python-float trees given identical leaf values.  The transition storage itself stays with the caller.
+ * reference's Python-float trees given identical leaf values.  srl_replay_* below stores transitions over such trees.
  * Errors are reported by srl_last_error; srl_per_last_error returns the same message (kept for existing hosts). */
 typedef struct srl_per srl_per_t;
 int srl_per_create(int64_t memory_size, double alpha, srl_per_t** out);
@@ -329,12 +329,41 @@ int srl_per_sample(srl_per_t* P, const double* uniforms, int batch, double beta,
                    float* weights32, void* stream);                                      /* :353-381, uniforms f64 [batch] in [0,1) */
 int srl_per_debug_trees(srl_per_t* P, double* sum_out, double* min_out, double* max_priority_out, void* stream);
 const char* srl_per_last_error(void);
+/* The stored count is also kept on the device, written by the add kernel: srl_per_sample and srl_per_update_priorities read it when
+ * their kernels run, so a captured sample or update sees every add made before the graph replays. */
+
+/* ---- prioritized replay memory: n-step transitions on the device, sampled and gathered there -------------------------------
+ * PrioritizedReplayBuffer (scalerl/data/replay_buffer.py:132-381) with its storage on the GPU: a ring of memory_size transitions,
+ * state / next_state u8 [M,4,84,84], action i64 [M], reward f32 [M], done u8 [M], whose slot i is leaf i of the memory's own sampler
+ * (srl_replay_per).  An n_step-deep window of raw vector steps per env folds into n-step transitions as _get_n_step_info does
+ * (:230-273): state and action of the oldest step, reward r0 + r1*g1 + r2*g2 ... in fp32 (g_k = fp32(gamma^k) in double, every product
+ * and sum rounded separately), stopping at the first done, whose step gives next_state and done.  Every call is stream-ordered. */
+typedef struct srl_replay srl_replay_t;
+/* memory_size in [2, 2^30], num_envs in [1, min(65536, memory_size)], n_step in [1, 32], gamma finite, alpha the trees' exponent.
+ * Allocates memory_size * 56,461 B plus the window (a failed allocation names the bytes asked for).  Synchronous. */
+int srl_replay_create(int64_t memory_size, int num_envs, int n_step, double gamma, double alpha, srl_replay_t** out);
+int srl_replay_destroy(srl_replay_t* R);
+int64_t srl_replay_size(const srl_replay_t* R);         /* stored transitions (len of the reference's memory) */
+srl_per_t* srl_replay_per(srl_replay_t* R);              /* its trees: srl_apex_learner_step's `per`, srl_per_update_priorities */
+/* one vector env step of num_envs envs: state / next_state u8 [E,4,84,84], action i64 [E], reward f32 [E], done u8 [E] (device or host
+ * memory, copied on `stream`).  Once n_step steps are staged, E transitions enter the ring at slots (ptr + e) mod memory_size in env
+ * order (replay_buffer.py:197-218, 319-323) with priority max_priority^alpha. */
+int srl_replay_add(srl_replay_t* R, const uint8_t* state, const int64_t* action, const float* reward, const uint8_t* next_state,
+                   const uint8_t* done, void* stream);
+/* srl_per_sample with beta read from the device (beta_dev f64 [1], so a replayed graph sees every change), then srl_replay_gather of the
+ * sampled idxs: uniforms f64 [batch] in [0,1), outputs state / next_state u8 [batch,4,84,84] (16-byte aligned), action i64, reward f32,
+ * done u8, idxs i64, weights f32 [batch] (may be NULL).  Needs size >= 2 when called; no host synchronisation, capturable. */
+int srl_replay_sample(srl_replay_t* R, const double* uniforms, int batch, const double* beta_dev, uint8_t* state, int64_t* action,
+                      float* reward, uint8_t* next_state, uint8_t* done, int64_t* idxs, float* weights, void* stream);
+/* copies ring slots idxs i64 [n] (device) into the outputs, as srl_replay_sample's; a slot outside [0, memory_size) leaves its rows */
+int srl_replay_gather(srl_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* state, int64_t* action, float* reward, uint8_t* next_state,
+                      uint8_t* done, void* stream);
 
 /* ---- Ape-X learner step: a prioritized (double) DQN update on the encoder (BASELINE.json configs[3]) --------------------------
  * replaces the learner statements of the reference's Ape-X Learner.train (scalerl/algorithms/apex/worker.py:134-161) and, with
  * double DQN, clipping and the target cadence, DQNAgent.learn (scalerl/algorithms/dqn/dqn_agent.py:136-190).  The Q network is
  * Nature DQN: AtariNet's conv1..3 + fc + ReLU (atari_model.py:30-47,91-101) followed by q = Linear(512, A), A in [1, 31].
- * Actors, transition storage and n-step folding stay with the caller (pass gamma^n for n-step transitions).
+ * Actors stay with the caller; srl_replay_* stores and folds n-step transitions (pass gamma^n for them, and srl_replay_per as `per`).
  * Parameters in state_dict order {conv1.weight, conv1.bias, conv2.weight, conv2.bias, conv3.weight, conv3.bias, fc.weight, fc.bias,
  * q.weight [A,512], q.bias [A]}; srl_apex_param_layout returns the flat buffer's floats and each tensor's offset / count (int64[10]).
  * In memory the small tensors come first and fc.weight last; segments are padded to 4 floats.  Params, grads, both Adam states

@@ -72,6 +72,11 @@ _SIGS = {
     'srl_per_update_priorities': [_P, _P, _P, _L, _P],
     'srl_per_sample': [_P, _P, _I, C.c_double, _P, _P, _P, _P],
     'srl_per_debug_trees': [_P, _P, _P, _P, _P],
+    'srl_replay_create': [_L, _I, _I, C.c_double, C.c_double, C.POINTER(_P)],
+    'srl_replay_destroy': [_P],
+    'srl_replay_add': [_P] * 7,
+    'srl_replay_sample': [_P, _P, _I] + [_P] * 9,
+    'srl_replay_gather': [_P, _P, _L] + [_P] * 6,
     'srl_unpack_slots': [_P, _L, C.POINTER(_L), _I, _I, _I, _P, _P, _P, _P, _P, _P, _P],
     'srl_grad_norm_clip_coef': [_P, _L, _F, _P, _P, _P],
     'srl_rmsprop_step': [_P, _P, _P, _L, _P, _F, _F, _F, _P],
@@ -124,7 +129,7 @@ def hooks():
     return _hooks
 
 
-EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout'])
+EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout', 'srl_replay_size', 'srl_replay_per'])
 
 
 def lib():
@@ -149,6 +154,10 @@ def lib():
         for nm in ('srl_per_size', 'srl_per_capacity'):
             getattr(L, nm).restype = C.c_int64
             getattr(L, nm).argtypes = [_P]
+        L.srl_replay_size.restype = C.c_int64
+        L.srl_replay_size.argtypes = [_P]
+        L.srl_replay_per.restype = _P
+        L.srl_replay_per.argtypes = [_P]
         L.srl_learner_get_step.restype = C.c_int64
         L.srl_learner_get_step.argtypes = [_P, _P]
         L.srl_per_invalid_updates.restype = C.c_int64

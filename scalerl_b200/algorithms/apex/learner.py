@@ -4,7 +4,8 @@ One ``learn`` call is the reference's Ape-X learner update (scalerl/algorithms/a
 clipping and target-update statements of ``DQNAgent.learn`` (scalerl/algorithms/dqn/dqn_agent.py:136-190): the Q values of the
 batch, the bootstrapped targets, the importance-weighted squared TD loss, the new priorities written straight into a
 ``GpuPrioritizedSampler``, ``clip_grad_norm_`` and a ``torch.optim.Adam`` step -- all in libscalerl_b200.so (srl_apex_learner_*),
-captured as one CUDA graph.  Actors, transition storage, n-step folding and the exploration schedule stay with the caller.
+captured as one CUDA graph.  ``learn_from`` samples and gathers its batch from a ``GpuPrioritizedReplayBuffer`` (device-resident
+n-step storage) inside the same graph.  Actors and the exploration schedule stay with the caller.
 ``AtariQNet`` is the CPU torch Q network with the learner's parameter names and shapes (the actors' copy).
 """
 from __future__ import annotations
@@ -167,6 +168,7 @@ class B200ApexLearner(BaseAgent):
         self.use_graph = use_graph
         self._graphs = {}
         self._seen = set()
+        self._from = None
         self._opt_steps = 0
         self.learner_update_step = 0
         self.target_model_update_step = 0
@@ -305,20 +307,28 @@ class B200ApexLearner(BaseAgent):
             weights.data_ptr() if weights is not None else None, idxs.data_ptr() if idxs is not None else None,
             sampler._h if sampler is not None else None, self._stats.data_ptr(), self._stream()), 'srl_apex_learner_step')
 
-    def _graph_step(self, args):
-        key = tuple(a.data_ptr() if isinstance(a, torch.Tensor) else (a._h.value if a is not None else None) for a in args)
+    def _graph_step(self, key, enqueue, keep=None):
+        """enqueue() through the graph of `key` (`keep`: what the graph's buffers belong to, held while the graph lives)"""
         g = self._graphs.get(key)
         if g is None:
             if key not in self._seen:          # first sight: eager (warm-up of attributes and allocator state)
                 self._seen.add(key)
-                self._enqueue(*args)
+                enqueue()
                 return
             torch.cuda.current_stream(self.device).synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._enqueue(*args)
-            self._graphs[key] = g
+                enqueue()
+            self._graphs[key] = (g, keep)
+        else:
+            g = g[0]
         g.replay()
+
+    def _run(self, key, enqueue, use_graph, keep=None):
+        if self.use_graph if use_graph is None else use_graph:
+            self._graph_step(key, enqueue, keep)
+        else:
+            enqueue()
 
     @torch.no_grad()
     def learn(self, experiences, weights: Optional[torch.Tensor] = None, idxs: Optional[torch.Tensor] = None, sampler=None,
@@ -326,10 +336,47 @@ class B200ApexLearner(BaseAgent):
         """one update (apex/worker.py:134-161; dqn_agent.py:136-190) -> {'loss': float}, or {} with nothing synchronised"""
         obs, action, reward, next_obs, done = self._inputs(experiences, weights, idxs, sampler)
         args = (obs, action, reward, next_obs, done, weights, idxs, sampler)
-        if self.use_graph if use_graph is None else use_graph:
-            self._graph_step(args)
-        else:
-            self._enqueue(*args)
+        key = tuple(a.data_ptr() if isinstance(a, torch.Tensor) else (a._h.value if a is not None else None) for a in args)
+        self._run(key, lambda: self._enqueue(*args), use_graph)
+        return self._finish_update(sync_stats)
+
+    @torch.no_grad()
+    def learn_from(self, memory, beta: float = 0.4, sync_stats: bool = True, use_graph: Optional[bool] = None) -> Dict[str, float]:
+        """one update on a batch of ``batch_size`` transitions sampled from ``memory`` (a GpuPrioritizedReplayBuffer on this
+        learner's device), all on the device: uniforms drawn by ``torch.rand`` (the default CUDA generator) into a fixed buffer, the
+        prioritized sample and the gather into learner-owned fixed buffers, the step, and the new priorities written into
+        ``memory``'s trees.  It is captured as one graph per memory (first call eager, second captures, later calls replay); the
+        sampler reads the stored count and ``beta`` from the device, so a replay sees every add made since and a new ``beta`` costs
+        one fill, not a recapture.  ``hp.gamma`` is used as given: for n-step memories pass ``gamma ** n_step``.  The target cadence
+        and the step counters are learn()'s.  -> {'loss': float}, or {} with nothing synchronised."""
+        from ...data.replay_memory import GpuPrioritizedReplayBuffer
+        if not isinstance(memory, GpuPrioritizedReplayBuffer):
+            raise ValueError(f'memory must be a GpuPrioritizedReplayBuffer, got {type(memory).__name__}')
+        if memory.device != self.device:
+            raise ValueError(f'memory is on {memory.device}, the learner on {self.device}')
+        if len(memory) < 2:
+            raise ValueError(f'learn_from needs at least 2 stored transitions, the memory has {len(memory)}')
+        memory._set_beta(beta)
+        b = self._from_buffers()
+
+        def enqueue():
+            torch.rand(b['u'].shape, dtype=torch.float64, device=self.device, out=b['u'])
+            memory._sample_into(b['u'], b['obs'], b['action'], b['reward'], b['next_obs'], b['done'], b['idxs'], b['weights'])
+            self._enqueue(b['obs'], b['action'], b['reward'], b['next_obs'], b['done'], b['weights'], b['idxs'], memory.sampler)
+
+        self._run(('learn_from', memory._h.value), enqueue, use_graph, keep=memory)
+        return self._finish_update(sync_stats)
+
+    def _from_buffers(self):
+        """learn_from's fixed inputs: the uniforms and the gathered batch (the graph is keyed by the memory, not by these)"""
+        if self._from is None:
+            B, z = self.hp.batch_size, lambda *shape, dtype: torch.empty(*shape, dtype=dtype, device=self.device)
+            self._from = {'u': z(B, dtype=torch.float64), 'obs': z(B, 4, 84, 84, dtype=torch.uint8), 'action': z(B, dtype=torch.int64),
+                          'reward': z(B, dtype=torch.float32), 'next_obs': z(B, 4, 84, 84, dtype=torch.uint8), 'done': z(B, dtype=torch.uint8),
+                          'idxs': z(B, dtype=torch.int64), 'weights': z(B, dtype=torch.float32)}
+        return self._from
+
+    def _finish_update(self, sync_stats):
         self._opt_steps += 1
         if self.learner_update_step % self.hp.target_update_frequency == 0:
             self.update_target(self.hp.soft_update_tau)

@@ -239,6 +239,15 @@ cudaError_t launch_dqn_wgrad(const float* dq, const int64_t* action, const float
 cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* b, int N, int A, float* q_out, cudaStream_t st);
 cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
 
+}  // namespace srl
+struct srl_per;
+namespace srl {
+// ---- per.cu: what the replay memory (replay.cu) shares with its sampler, whose leaf i is the memory's ring slot i
+int64_t per_tree_ptr(const srl_per* P);          // the leaf the next add writes
+// srl_per_sample with an optional device beta (beta_dev, read when the kernel runs; NULL: `beta`)
+int per_sample(srl_per* P, const double* uniforms, int batch, double beta, const double* beta_dev, int64_t* idxs, double* weights64,
+               float* weights32, cudaStream_t st);
+
 // ---- encoder.cu
 // packed bf16 operand copies of the conv/fc weights (element offsets into one buffer)
 struct WPack {

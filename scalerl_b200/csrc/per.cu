@@ -7,13 +7,19 @@
 #include <new>
 #include "common.cuh"
 #include "errors.h"
+#include "kernels.h"
 #include "../../include/scalerl_b200.h"
 
 namespace srl {
 
+// scal: [0] max_priority, [1] invalid-update counter (u64 bits), [2] stored transitions (i64 bits).  The count lives on the device so
+// that a captured sample or priority update reads the size as it is when the graph replays, not as it was at capture.
+__device__ __forceinline__ int64_t* per_count_slot(double* scal) { return reinterpret_cast<int64_t*>(scal + 2); }
+
 // Batched tree update by ONE block (n <= 1024 leaves per launch): write the leaves (duplicates: the LAST occurrence wins, as a
 // sequential loop would), then recompute every touched ancestor level by level.
-//   mode 0: idxs/priorities given, leaf = priority^alpha, max_priority updated.   mode 1: leaves ptr.. (mod memory_size) = max_priority^alpha
+//   mode 0: idxs/priorities given, leaf = priority^alpha, max_priority updated; idxs at or above the stored count are skipped.
+//   mode 1: leaves ptr.. (mod memory_size) = max_priority^alpha, stored count = min(count + n, memory_size)
 __global__ void __launch_bounds__(1024) per_update_kernel(double* __restrict__ sum, double* __restrict__ mn, int64_t cap, int levels,
                                                           const int64_t* __restrict__ idxs, const double* __restrict__ prios, int n,
                                                           double alpha, double* __restrict__ scal, int mode, int64_t ptr, int64_t memory_size) {
@@ -25,14 +31,16 @@ __global__ void __launch_bounds__(1024) per_update_kernel(double* __restrict__ s
   bool valid = t < n;
   if (t < n) {
     if (mode == 0) {
+      const int64_t count = *per_count_slot(scal);
       leaf = idxs[t]; pr = prios[t]; v = pow(pr, alpha);
       // the reference asserts priority > 0 and 0 <= idx < len(self) (replay_buffer.py:346-351): an invalid entry is
       // skipped here (never an out-of-bounds write) and counted in scal[1]; the Python wrapper raises on it
-      if (!(leaf >= 0 && leaf < memory_size) || !(pr > 0.0)) { valid = false; leaf = -1; atomicAdd(reinterpret_cast<unsigned long long*>(scal + 1), 1ull); }
+      if (!(leaf >= 0 && leaf < count) || !(pr > 0.0)) { valid = false; leaf = -1; atomicAdd(reinterpret_cast<unsigned long long*>(scal + 1), 1ull); }
     } else { leaf = (ptr + t) % memory_size; v = pow(scal[0], alpha); }
   }
   sidx[t] = leaf;
   __syncthreads();
+  if (mode == 1 && t == 0) { int64_t* c = per_count_slot(scal); *c = *c + n < memory_size ? *c + n : memory_size; }
   bool winner = valid;
   if (winner && mode == 0)
     for (int u = t + 1; u < n; ++u)
@@ -73,10 +81,14 @@ __device__ double prefix_sum_ref_order(const double* __restrict__ sum, int64_t c
   return r;
 }
 
+// beta_dev (optional): beta read from the device when the kernel runs, so a replayed graph sees every change; else `beta`
 __global__ void per_sample_kernel(const double* __restrict__ sum, const double* __restrict__ mn, int64_t cap, const double* __restrict__ u,
-                                  int batch, int64_t n, double beta, int64_t* __restrict__ idxs, double* __restrict__ w64, float* __restrict__ w32) {
+                                  int batch, const double* __restrict__ scal, double beta, const double* __restrict__ beta_dev,
+                                  int64_t* __restrict__ idxs, double* __restrict__ w64, float* __restrict__ w32) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= batch) return;
+  const int64_t n = *reinterpret_cast<const int64_t*>(scal + 2);
+  if (beta_dev) beta = *beta_dev;
   const double p_total = prefix_sum_ref_order(sum, cap, n - 2);  // sum_tree.sum(0, len - 1)  (replay_buffer.py:359)
   const double segment = p_total / batch;
   const double a = segment * i, b = segment * (i + 1);
@@ -101,7 +113,7 @@ __global__ void per_sample_kernel(const double* __restrict__ sum, const double* 
 __global__ void per_fill_kernel(double* __restrict__ sum, double* __restrict__ mn, int64_t n2, double* scal) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n2) { sum[i] = 0.0; mn[i] = INFINITY; }
-  if (i == 0) { scal[0] = 1.0; scal[1] = 0.0; }                  // max_priority (replay_buffer.py:308); [1] = invalid-update counter (u64 bits)
+  if (i == 0) { scal[0] = 1.0; scal[1] = 0.0; *per_count_slot(scal) = 0; }   // max_priority (replay_buffer.py:308), counter, count
 }
 
 }  // namespace srl
@@ -156,7 +168,7 @@ extern "C" int srl_per_update_priorities(srl_per_t* P, const int64_t* idxs, cons
   for (int64_t o = 0; o < n; o += 1024) {
     const int c = (int)(n - o < 1024 ? n - o : 1024);
     per_update_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(P->sum, P->mn, P->capacity, P->levels, idxs + o, priorities + o, c, P->alpha, P->scal, 0,
-                                                            0, P->size);        // mode 0: the last argument bounds the valid indices (idx < len(self))
+                                                            0, P->memory_size);  // mode 0 bounds idx by the device count (idx < len(self))
   }
   CU(cudaGetLastError(), "per_update_priorities");
   return 0;
@@ -170,15 +182,22 @@ extern "C" int64_t srl_per_invalid_updates(srl_per_t* P, void* stream) {
   if (cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess) return -1;
   return (int64_t)c;
 }
+namespace srl {
+int64_t per_tree_ptr(const srl_per* P) { return P->tree_ptr; }
+int per_sample(srl_per* P, const double* uniforms, int batch, double beta, const double* beta_dev, int64_t* idxs, double* weights64,
+               float* weights32, cudaStream_t st) {
+  REQ(P && uniforms && idxs && batch >= 1, "per_sample: bad argument");
+  REQ(P->size >= 2, "per_sample: need at least 2 stored transitions");
+  per_sample_kernel<<<(batch + 127) / 128, 128, 0, st>>>(P->sum, P->mn, P->capacity, uniforms, batch, P->scal, beta, beta_dev, idxs, weights64,
+                                                         weights32);
+  CU(cudaGetLastError(), "per_sample");
+  return 0;
+}
+}  // namespace srl
 // uniforms f64 [batch] in [0,1) (device) -> idxs i64 [batch], IS weights (f64 and/or f32, either may be NULL)
 extern "C" int srl_per_sample(srl_per_t* P, const double* uniforms, int batch, double beta, int64_t* idxs, double* weights64, float* weights32,
                               void* stream) {
-  REQ(P && uniforms && idxs && batch >= 1, "per_sample: bad argument");
-  REQ(P->size >= 2, "per_sample: need at least 2 stored transitions");
-  per_sample_kernel<<<(batch + 127) / 128, 128, 0, (cudaStream_t)stream>>>(P->sum, P->mn, P->capacity, uniforms, batch, P->size, beta, idxs, weights64,
-                                                                           weights32);
-  CU(cudaGetLastError(), "per_sample");
-  return 0;
+  return per_sample(P, uniforms, batch, beta, nullptr, idxs, weights64, weights32, (cudaStream_t)stream);
 }
 // copies the trees (2*capacity doubles each, root at [1], leaves at [capacity..)) and max_priority to device buffers
 extern "C" int srl_per_debug_trees(srl_per_t* P, double* sum_out, double* min_out, double* max_priority_out, void* stream) {

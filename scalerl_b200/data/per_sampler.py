@@ -20,6 +20,15 @@ class GpuPrioritizedSampler:
         _lib.check(self._L.srl_per_create(self.memory_size, self.alpha, C.byref(h)), 'srl_per_create')
         self._h = h
         self._invalid_seen = 0
+        self._owned = True
+
+    @classmethod
+    def _view(cls, handle, memory_size: int, alpha: float, device):
+        """the sampler over trees another object owns (GpuPrioritizedReplayBuffer's): close() leaves them to their owner"""
+        s = cls.__new__(cls)
+        s.memory_size, s.alpha, s.device = int(memory_size), float(alpha), torch.device(device)
+        s._L, s._h, s._invalid_seen, s._owned = _lib.lib(), handle, 0, False
+        return s
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
@@ -73,7 +82,8 @@ class GpuPrioritizedSampler:
 
     def close(self):
         if getattr(self, '_h', None) is not None:
-            self._L.srl_per_destroy(self._h)
+            if self._owned:
+                self._L.srl_per_destroy(self._h)
             self._h = None
 
     def __del__(self):
