@@ -382,7 +382,7 @@ cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, 
   } else {
   S.b(PS_S2D); SRL_TRY(launch_s2d(obs, frames, buf.xs, st, p.w1, buf.hi.wpack + WPack::W1K, sp ? buf.lo.wpack + WPack::W1K : nullptr)); S.e(PS_S2D);
   { RConv1Fwd::Params q{maps.xs_w, maps.hi.w1k, maps.lo.w1k, p.b1, buf.hi.a1, buf.lo.a1, frames, buf.NF};
-    S.b(PS_CONV1_FWD); SRL_TRY(res_fwd_launch<RConv1Fwd>(q, cdiv(frames * 441, 128), 2 * kPersistentCtas, st, sp)); S.e(PS_CONV1_FWD); }
+    S.b(PS_CONV1_FWD); SRL_TRY(res_fwd_launch<RConv1Fwd>(q, cdiv(frames * 441, 128), kPersistentCtas, st, sp)); S.e(PS_CONV1_FWD); }
   SRL_TRY(S.join(LANE_PACK));      // conv1's weight copy comes from the frame-conversion kernel; conv2 is the first reader of the re-packed copies
   { RConv2Fwd::Params q{maps.hi.a1p0_w, maps.hi.a1p1_w, maps.hi.w2k, maps.lo.a1p0_w, maps.lo.a1p1_w, maps.lo.w2k, p.b2, buf.hi.a2, buf.lo.a2, frames};
     S.b(PS_CONV2_FWD); SRL_TRY(res_fwd_launch<RConv2Fwd>(q, cdiv(frames * 100, 128), kPersistentCtas, st, sp)); S.e(PS_CONV2_FWD); }

@@ -50,5 +50,9 @@ SRL_DEVINL void relu_mask16_pre(const uint4 (&m)[2], float (&v)[16]) {
   }
 }
 SRL_DEVINL void ld_mask16(const bf16* mask, uint4 (&m)[2]) { m[0] = ldg16(mask); m[1] = ldg16(mask + 8); }
+// two bf16 values x, each kept where its bf16 mask value is > 0 and +0 elsewhere
+SRL_DEVINL uint32_t relu_mask_bf16x2(uint32_t x, uint32_t m) {
+  return (bf16_lo(m) > 0.f ? x & 0xFFFFu : 0u) | (bf16_hi(m) > 0.f ? x & 0xFFFF0000u : 0u);
+}
 
 }  // namespace srl

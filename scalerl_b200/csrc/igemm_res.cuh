@@ -37,8 +37,30 @@ constexpr int RES_MAX_TAPS = 10;
 // forward / dgrad
 //   P: BN, NT (taps), NWIN (input windows per tile: 1, or 2 for conv2's two row-parity planes), WROWS (rows per window,
 //      128 + max shift - min shift), SHIFT_MIN, STAGES, Params{ in[NWIN] maps, w map, ... },
-//      tap_win(j), tap_shift(j) (relative to SHIFT_MIN, i.e. >= 0), num_tiles(p), epilogue16(p, tile, row, c0, v)
+//      tap_win(j), tap_shift(j) (relative to SHIFT_MIN, i.e. >= 0), num_tiles(p), epilogue16(p, tile, row, c0, v),
+//      TILE_ROWB: 0, or (bf16 mode) the row pitch of a shared-memory bf16 image of the whole output tile that
+//      epilogue_tile(p, tile, wt, acc, image, bar, pre) stages and copies out in whole, coalesced output rows
+//      (prefetch_tile(p, tile, wt, pre) then requests its global operands instead of prefetch16)
 // ------------------------------------------------------------------------------------------------------------------
+
+// bf16 image of a warpgroup's 128 x N accumulator in shared memory: row r at buf + r * ROWB bytes, column c at byte 2c, each value
+// f(column, value) rounded as store_bf16x16 rounds it.  With ROWB = 2N + 16 the 8 rows x 4 words of a warp's stores hit 32
+// distinct banks.  Brackets the writes with the warpgroup's named barrier: the previous tile's readers are done before, every
+// row is complete after.
+template <int N, int ROWB, class F>
+SRL_DEVINL void wg_acc_stage_bf16(const float (&d)[2][N / 2], uint8_t* buf, int wt, int bar, F f) {
+  static_assert(ROWB % 16 == 0 && ROWB >= 2 * N, "16-byte aligned rows that hold N bf16");
+  const int w = wt >> 5, l = wt & 31;
+  named_bar(bar, 128);
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < N / 2; i += 2) {
+      const int row = 64 * h + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
+      *reinterpret_cast<uint32_t*>(buf + row * ROWB + col * 2) = pack_bf16x2(f(col, d[h][i]), f(col + 1, d[h][i + 1]));
+    }
+  named_bar(bar, 128);
+}
 //
 // SPLIT = 1 is the fp32-accurate operand mode (srl_config_t.precision = 1): every bf16 operand tensor has a second, "low"
 // tensor holding bf16(v - bf16(v)), and each product is issued as hi*hi + hi*lo + lo*hi into the same fp32 accumulator
@@ -54,9 +76,12 @@ struct ResFwdCfg {
   static constexpr int IN_BYTES = IN_HI_BYTES * (1 + ALO);
   static constexpr int W_HI_BYTES = P::NT * P::BN * 128;
   static constexpr int W_BYTES = W_HI_BYTES * (1 + SPLIT);
+  // the output tile leaves through a bf16 image in shared memory (bf16 mode of the problems that define one), or row by row
+  static constexpr bool TILE_EPI = P::TILE_ROWB > 0 && !SPLIT;
+  static constexpr int TILE_IMG_BYTES = 128 * P::TILE_ROWB > WG_IMG_BYTES ? 128 * P::TILE_ROWB : WG_IMG_BYTES;
   // row hand-off buffers of the two consumer warpgroups: single-buffered where one input stage would not fit beside double ones
-  static constexpr bool IMG1 = W_BYTES + IN_BYTES + 2 * WG_IMG_BYTES + 1024 + 256 > 232448;
-  static constexpr int IMG_BYTES = IMG1 ? WG_IMG_BYTES / 2 : WG_IMG_BYTES;
+  static constexpr bool IMG1 = !TILE_EPI && W_BYTES + IN_BYTES + 2 * WG_IMG_BYTES + 1024 + 256 > 232448;
+  static constexpr int IMG_BYTES = TILE_EPI ? TILE_IMG_BYTES : IMG1 ? WG_IMG_BYTES / 2 : WG_IMG_BYTES;
   // the two consumer warpgroups take alternate tiles: with an even depth every stage (and every phase of its barrier) belongs to one
   // warpgroup, so a warpgroup never waits for phase k of a stage whose phase k-1 (the other warpgroup's tile) may still be filling
   static constexpr int FIT = fit_stages(SPLIT ? P::SPLIT_STAGES : P::STAGES, W_BYTES + 2 * IMG_BYTES + 1024 + 256, IN_BYTES);
@@ -138,8 +163,11 @@ __global__ void __launch_bounds__(RES_THREADS, 1) res_fwd_kernel(const __grid_co
       const int s = it % STAGES;
       // global operands of the epilogue (ReLU masks of the dgrads) are requested before the MMAs: their L2 latency overlaps them
       uint4 pre[P::BN / 16][2];
+      if constexpr (C::TILE_EPI) P::prefetch_tile(p, t, wt, pre);
+      else {
 #pragma unroll
-      for (int c = 0; c < P::BN / 16; ++c) P::prefetch16(p, t, wt, c * 16, pre[c]);
+        for (int c = 0; c < P::BN / 16; ++c) P::prefetch16(p, t, wt, c * 16, pre[c]);
+      }
       float acc[2][P::BN / 2];
       mbar_wait(&in_full[s], (it / STAGES) & 1);
       const uint64_t ind = make_smem_desc(smem_u32(sIn + s * C::IN_BYTES), 16, 1024);
@@ -162,11 +190,14 @@ __global__ void __launch_bounds__(RES_THREADS, 1) res_fwd_kernel(const __grid_co
       wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
       __syncwarp();
       if ((tid & 31) == 0) mbar_arrive(&in_empty[s]);
+      if constexpr (C::TILE_EPI) P::epilogue_tile(p, t, wt, acc, reinterpret_cast<uint8_t*>(my_img), 2 + g, pre);
+      else {
 #pragma unroll
-      for (int c = 0; c < P::BN / 16; ++c) {
-        float v[16];
-        wg_acc_row16<P::BN, C::IMG1>(acc, c, my_img, wt, 2 + g, v);
-        P::template epilogue16<SPLIT>(p, t, wt, c * 16, v, pre[c]);
+        for (int c = 0; c < P::BN / 16; ++c) {
+          float v[16];
+          wg_acc_row16<P::BN, C::IMG1>(acc, c, my_img, wt, 2 + g, v);
+          P::template epilogue16<SPLIT>(p, t, wt, c * 16, v, pre[c]);
+        }
       }
     }
   }

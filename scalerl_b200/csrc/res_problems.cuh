@@ -43,6 +43,23 @@ struct RConv1Fwd {   // 2x2 s1 over xs (== 8x8 s4 over the frame): taps (kh2,kw2
   SRL_DEVINL static constexpr int tap_shift(int j) { return (j >> 1) * 21 + (j & 1); }
   SRL_DEVINL static void load_windows(const Params& p, int t, uint8_t* dst, int, uint64_t* bar, bool) { tma_load_2d(dst, &p.in0, bar, 0, t * 128); }
   SRL_DEVINL static void prefetch16(const Params&, int, int, int, uint4 (&)[2]) {}
+  // bf16 mode: the tile's 128 positions x 32 channels (64 B each) are staged in shared memory and leave as 16-byte pieces, four per
+  // position, consecutive lanes on consecutive pieces: positions ow, ow + 1 fill one 128-byte a1 row, so a warp stores 512
+  // contiguous bytes of an output row where a row per thread touched 16 rows per store
+  static constexpr int TILE_ROWB = 80;
+  SRL_DEVINL static void prefetch_tile(const Params&, int, int, uint4 (&)[BN / 16][2]) {}
+  SRL_DEVINL static void epilogue_tile(const Params& p, int t, int wt, const float (&acc)[2][BN / 2], uint8_t* img, int bar,
+                                       const uint4 (&)[BN / 16][2]) {
+    wg_acc_stage_bf16<BN, TILE_ROWB>(acc, img, wt, bar, [&](int c, float v) { return fmaxf(fmaf(v, 1.0f / 255.0f, __ldg(p.bias + c)), 0.f); });
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int e = s * 128 + wt, q = e >> 2, k = e & 3;
+      const int Q = t * 128 + q, n = Q / 441, r = Q - n * 441, oh = r / 21, ow = r - oh * 21;
+      if (n >= p.NF || oh >= 20 || ow >= 20) continue;
+      const size_t prow = (size_t)(oh & 1) * p.NFS * 100 + (size_t)n * 100 + (oh >> 1) * 10 + (ow >> 1);
+      *reinterpret_cast<uint4*>(p.out + prow * 64 + (ow & 1) * 32 + k * 8) = *reinterpret_cast<const uint4*>(img + q * TILE_ROWB + k * 16);
+    }
+  }
   template <int SPLIT>
   SRL_DEVINL static void epilogue16(const Params& p, int t, int row, int c0, float (&v)[16], const uint4 (&)[2]) {
     const int Q = t * 128 + row, n = Q / 441, r = Q - n * 441, oh = r / 21, ow = r - oh * 21;
@@ -58,6 +75,7 @@ struct RConv2Fwd {   // 4x4 s2 over a1: tap j = (kh, kww): plane kh&1, shift (kh
   static constexpr int KID = 12;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
   static constexpr int BN = 64, NT = 8, NWIN = 2, WROWS = 128 + 11, STAGES = 3, SPLIT_STAGES = 1;
+  static constexpr int TILE_ROWB = 0;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP in1; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP in1_lo; SRL_TMAP w_lo; const float* bias; bf16* out; bf16* out_lo; int NF; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.in1); tma_prefetch_desc(&p.w); }
@@ -83,6 +101,7 @@ struct RConv3Fwd {   // 3x3 s1 over a2: tap (kh,kw) -> shift kh*9 + kw
   static constexpr int KID = 13;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
   static constexpr int BN = 64, NT = 9, NWIN = 1, WROWS = 128 + 20, STAGES = 4, SPLIT_STAGES = 2;
+  static constexpr int TILE_ROWB = 0;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP w_lo; const float* bias; bf16* out; bf16* out_lo; int NF; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.w); }
@@ -106,6 +125,7 @@ struct RConv3Dgrad {   // da2[ih,iw] = sum_{kh,kw} da3g[(ih-kh),(iw-kw)] W3[:, :
   static constexpr int KID = 14;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
   static constexpr int BN = 64, NT = 9, NWIN = 1, WROWS = 128 + 20, STAGES = 4, SPLIT_STAGES = 2;
+  static constexpr int TILE_ROWB = 0;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP w_lo; const bf16* act; bf16* dx; bf16* dx_lo; int NB; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.w); }
@@ -140,6 +160,32 @@ struct RConv2Dgrad {   // the 4 stride-parity classes share A (da2g at (i'-kh', 
   SRL_DEVINL static void prefetch16(const Params& p, int t, int row, int c0, uint4 (&m)[2]) {
     const int Q = t * 128 + row, cls = c0 >> 5, c = c0 & 31;
     if (Q < p.NB * 100) ld_mask16(p.act + ((size_t)(cls >> 1) * p.NF * 100 + Q) * 64 + (cls & 1) * 32 + c, m);   // a1 plane ph, same row Q
+  }
+  // bf16 mode: the tile (128 positions x 4 classes x 32 channels) is staged in shared memory; it leaves as 16-byte pieces
+  // e = s * 128 + wt (ph = e >> 10, position q = (e >> 3) & 127, piece k = e & 7 of the 128 bytes (pw, c) of row q, plane ph).
+  // Those 128 bytes are the a1 row the ReLU mask comes from and the two da1g rows (2i + ph, 2j + pw) they go to, and position q + 1
+  // continues both two rows on: a warp loads 512 contiguous bytes of mask and stores 512 contiguous bytes of da1g where a row per
+  // thread touched 32 rows per instruction.  Masking the rounded value gives the bits of rounding the masked one.
+  static constexpr int TILE_ROWB = 272;
+  SRL_DEVINL static void prefetch_tile(const Params& p, int t, int wt, uint4 (&m)[BN / 16][2]) {
+#pragma unroll
+    for (int s = 0; s < 16; ++s) {
+      const int e = s * 128 + wt, ph = e >> 10, Q = t * 128 + ((e >> 3) & 127);
+      if (Q < p.NB * 100) m[s >> 1][s & 1] = ldg16(p.act + ((size_t)ph * p.NF * 100 + Q) * 64 + (e & 7) * 8);
+    }
+  }
+  SRL_DEVINL static void epilogue_tile(const Params& p, int t, int wt, const float (&acc)[2][BN / 2], uint8_t* img, int bar,
+                                       const uint4 (&m)[BN / 16][2]) {
+    wg_acc_stage_bf16<BN, TILE_ROWB>(acc, img, wt, bar, [](int, float v) { return v; });
+#pragma unroll
+    for (int s = 0; s < 16; ++s) {
+      const int e = s * 128 + wt, ph = e >> 10, q = (e >> 3) & 127, k = e & 7;
+      const int Q = t * 128 + q, n = Q / 100, r = Q - n * 100, i = r / 10, j = r - i * 10;
+      if (n >= p.NB) continue;
+      const uint4 x = *reinterpret_cast<const uint4*>(img + q * TILE_ROWB + ph * 128 + k * 16), mk = m[s >> 1][s & 1];
+      *reinterpret_cast<uint4*>(p.dx + ((size_t)n * 441 + (2 * i + ph) * 21 + 2 * j) * 32 + k * 8) =
+          make_uint4(relu_mask_bf16x2(x.x, mk.x), relu_mask_bf16x2(x.y, mk.y), relu_mask_bf16x2(x.z, mk.z), relu_mask_bf16x2(x.w, mk.w));
+    }
   }
   template <int SPLIT>
   SRL_DEVINL static void epilogue16(const Params& p, int t, int row, int c0, float (&v)[16], const uint4 (&m)[2]) {
