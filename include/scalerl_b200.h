@@ -323,7 +323,8 @@ int64_t srl_per_capacity(const srl_per_t* P);
 int srl_per_add(srl_per_t* P, int64_t n, void* stream);                                  /* _add x n  (replay_buffer.py:318-322) */
 int srl_per_update_priorities(srl_per_t* P, const int64_t* idxs, const double* priorities, int64_t n, void* stream);   /* :346-351 */
 /* pairs skipped so far by srl_per_update_priorities because idx was outside [0, size) or priority <= 0 (the reference asserts
- * both, replay_buffer.py:346-351); synchronises `stream`; -1 on error */
+ * both, replay_buffer.py:346-351), plus the non-finite priorities srl_replay_add_prioritized stored as max_priority^alpha;
+ * synchronises `stream`; -1 on error */
 int64_t srl_per_invalid_updates(srl_per_t* P, void* stream);
 int srl_per_sample(srl_per_t* P, const double* uniforms, int batch, double beta, int64_t* idxs, double* weights64,
                    float* weights32, void* stream);                                      /* :353-381, uniforms f64 [batch] in [0,1) */
@@ -363,7 +364,8 @@ int srl_replay_gather(srl_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* 
  * replaces the learner statements of the reference's Ape-X Learner.train (scalerl/algorithms/apex/worker.py:134-161) and, with
  * double DQN, clipping and the target cadence, DQNAgent.learn (scalerl/algorithms/dqn/dqn_agent.py:136-190).  The Q network is
  * Nature DQN: AtariNet's conv1..3 + fc + ReLU (atari_model.py:30-47,91-101) followed by q = Linear(512, A), A in [1, 31].
- * Actors stay with the caller; srl_replay_* stores and folds n-step transitions (pass gamma^n for them, and srl_replay_per as `per`).
+ * srl_replay_* stores and folds n-step transitions (pass gamma^n for them, and srl_replay_per as `per`); srl_apex_actor_* acts and computes
+ * their initial priorities.
  * Parameters in state_dict order {conv1.weight, conv1.bias, conv2.weight, conv2.bias, conv3.weight, conv3.bias, fc.weight, fc.bias,
  * q.weight [A,512], q.bias [A]}; srl_apex_param_layout returns the flat buffer's floats and each tensor's offset / count (int64[10]).
  * In memory the small tensors come first and fc.weight last; segments are padded to 4 floats.  Params, grads, both Adam states
@@ -409,6 +411,30 @@ int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* obs, int n, 
  * h = columns < 512), "dcore" f32 [B,514], "q", "y" f32 [B], "priorities" f64 [B], "loss" f32 [1], "step" i32 [1] (device step count),
  * and the bf16 activations the forward over s saved, in the learner's layouts (srl_learner_debug_buffer): "a1", "a2", "a3" */
 int srl_apex_learner_debug_buffer(srl_apex_learner_t* L, const char* name, void** ptr, int64_t* count);
+
+/* ---- Ape-X actor: per-env epsilon-greedy acting and actor-computed initial priorities (apex/worker.py:59-79, apex/memory.py:43-64) --
+ * A forward-only Q network for num_envs envs on a caller-owned flat f32 parameter snapshot (srl_apex_param_layout order, 16-byte
+ * aligned; the actor reads it when its kernels run, so the caller refreshes it with one device copy from the learner's parameters).
+ * The context owns one encoder context, encoder blocks for num_envs frames, core rows for 2 * num_envs frames and a device draw counter;
+ * no optimizer state, gradients or target copy.  Its calls share those buffers: order them on one stream.  Synchronous create. */
+typedef struct srl_apex_actor srl_apex_actor_t;
+/* A in [1, 31], num_envs in [1, 65536], precision as srl_apex_config_t.precision, seed: the key of the actor's random numbers */
+int srl_apex_actor_create(int A, int num_envs, int precision, uint64_t seed, const float* params, srl_apex_actor_t** out);
+int srl_apex_actor_destroy(srl_apex_actor_t* X);
+/* obs u8 [E,4,84,84], epsilons f32 [E] (device) -> actions i64 [E]: with probability epsilons[e] a uniform action, else the first
+ * argmax of Q(obs[e]) (torch.argmax's pick).  The random numbers are Philox4x32-10 keyed by seed, counted by (draw, env); the launch
+ * advances the device draw counter, so a captured call draws new numbers on every replay.  No host synchronisation; capturable. */
+int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const float* epsilons, int64_t* actions, void* stream);
+/* Q(obs) with the snapshot for n >= 1 frames: obs u8 [n,4,84,84] -> q_out f32 [n,A] */
+int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, int n, float* q_out, void* stream);
+/* srl_replay_add, then, for the E transitions the call completes, their initial priorities computed by `actor` (built for the memory's
+ * num_envs) instead of max_priority:  p = |Q(s)[a] - y| + priority_eps,  y = R + fp32(gamma^n_step) (1 - d) max_a Q(s')  with the
+ * arithmetic of srl_apex_learner_step's target and priority (the same bits for the same weights).  R, a and d are the fold's; s is the
+ * oldest staged step's state, s' the newest step's next_state (only read when d = 0).  Leaves ptr.. = p^alpha, max_priority =
+ * max(max_priority, p); a non-finite p is stored as max_priority^alpha and counted by srl_per_invalid_updates.  priority_eps finite,
+ * > 0.  While the window fills nothing runs beyond the copy. */
+int srl_replay_add_prioritized(srl_replay_t* R, srl_apex_actor_t* actor, const uint8_t* state, const int64_t* action, const float* reward,
+                               const uint8_t* next_state, const uint8_t* done, float priority_eps, void* stream);
 
 /* ---- trajectory ring -> time-major batch (the stacking step of ImpalaTrainer.get_batch, impala_atari.py:248-251) -----------
  * staging: B trajectory slots on the DEVICE, each one contiguous record of slot_bytes holding every key of create_buffers

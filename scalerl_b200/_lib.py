@@ -100,6 +100,11 @@ _SIGS = {
     'srl_apex_learner_set_step': [_P, _L, _P],
     'srl_apex_learner_q_values': [_P, _P, _I, _P, _P],
     'srl_apex_learner_debug_buffer': [_P, C.c_char_p, C.POINTER(_P), C.POINTER(_L)],
+    'srl_apex_actor_create': [_I, _I, _I, C.c_uint64, _P, C.POINTER(_P)],
+    'srl_apex_actor_destroy': [_P],
+    'srl_apex_actor_act': [_P] * 5,
+    'srl_apex_actor_q_values': [_P, _P, _I, _P, _P],
+    'srl_replay_add_prioritized': [_P] * 7 + [_F, _P],
 }
 # libscalerl_b200_testhooks.so (include/scalerl_b200_testhooks.h): unit-test entry points, loaded by tests only
 _HOOK_SIGS = {

@@ -5,7 +5,7 @@ clipping and target-update statements of ``DQNAgent.learn`` (scalerl/algorithms/
 batch, the bootstrapped targets, the importance-weighted squared TD loss, the new priorities written straight into a
 ``GpuPrioritizedSampler``, ``clip_grad_norm_`` and a ``torch.optim.Adam`` step -- all in libscalerl_b200.so (srl_apex_learner_*),
 captured as one CUDA graph.  ``learn_from`` samples and gathers its batch from a ``GpuPrioritizedReplayBuffer`` (device-resident
-n-step storage) inside the same graph.  Actors and the exploration schedule stay with the caller.
+n-step storage) inside the same graph.  ``B200ApexActor`` (actor.py) acts and computes initial priorities on a copy of its weights.
 ``AtariQNet`` is the CPU torch Q network with the learner's parameter names and shapes (the actors' copy).
 """
 from __future__ import annotations
@@ -121,6 +121,21 @@ class ApexHParams:
         return c
 
 
+def flat_views(flat: torch.Tensor, off, cnt, shapes) -> 'OrderedDict[str, torch.Tensor]':
+    """the named tensors of a flat buffer in srl_apex_param_layout order, as views"""
+    return OrderedDict((n, flat[off[i]:off[i] + cnt[i]].view(shp)) for i, (n, shp) in enumerate(shapes.items()))
+
+
+def load_views(dst: Dict[str, torch.Tensor], sd: Dict[str, torch.Tensor]) -> None:
+    """copies an AtariQNet-compatible state_dict into the views ``dst`` (KeyError on a missing name, ValueError on a shape)"""
+    for n, v in dst.items():
+        if n not in sd:
+            raise KeyError(f'missing key {n} in state_dict')
+        if tuple(sd[n].shape) != tuple(v.shape):
+            raise ValueError(f'{n}: shape {tuple(sd[n].shape)} != {tuple(v.shape)}')
+        v.copy_(sd[n].to(v.device, torch.float32))
+
+
 def default_q_state_dict(num_actions: int, seed: int = 0) -> 'OrderedDict[str, torch.Tensor]':
     """AtariQNet's initial weights under ``torch.manual_seed(seed)``, drawn without disturbing the global RNG"""
     with torch.random.fork_rng(devices=[]):
@@ -175,8 +190,7 @@ class B200ApexLearner(BaseAgent):
 
     # ------------------------------------------------------------------ parameters
     def _views(self, flat):
-        return OrderedDict((n, flat[self._off[i]:self._off[i] + self._cnt[i]].view(shp))
-                           for i, (n, shp) in enumerate(self.shapes.items()))
+        return flat_views(flat, self._off, self._cnt, self.shapes)
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
@@ -187,13 +201,7 @@ class B200ApexLearner(BaseAgent):
         return OrderedDict((n, p.detach().clone()) for n, p in src.items())
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor], target: bool = False) -> None:
-        dst = self.target_params if target else self.params
-        for n, shp in self.shapes.items():
-            if n not in sd:
-                raise KeyError(f'missing key {n} in state_dict')
-            if tuple(sd[n].shape) != tuple(shp):
-                raise ValueError(f'{n}: shape {tuple(sd[n].shape)} != {tuple(shp)}')
-            dst[n].copy_(sd[n].to(self.device, torch.float32))
+        load_views(self.target_params if target else self.params, sd)
 
     def get_weights(self):
         return {k: v.cpu() for k, v in self.state_dict().items()}

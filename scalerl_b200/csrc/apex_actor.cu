@@ -1,0 +1,202 @@
+// The Ape-X actor: per-env epsilon-greedy acting and the initial priorities of new transitions, forward-only on a parameter snapshot.
+// Restates the reference's
+//   scalerl/algorithms/apex/worker.py:14-30 (Actor: one eps per actor), :59-79 (compute_prior: |Q(s)[a] - (r + mask gamma^steps max Q(s'))|)
+//   scalerl/algorithms/apex/memory.py:43-64 (PrioritizedReplayBuffer.add: each transition enters with its actor's priority)
+// with one encoder forward (srl_encoder_forward) per frame set and the Q head of the learner (dqn_head.cuh), so that a priority computed
+// here has the bits of the learner's for the same weights.  fp32 on the CUDA cores: the Q head is 512 x A, no tensor-core work.
+//   apex_act_kernel       the Q row, its first argmax and the epsilon-greedy draw (one warp per env)
+//   apex_priority_kernel  q(s, a), the n-step target from max_a Q(s') and the priority (one warp per transition)
+#include <math.h>
+#include <new>
+#include "common.cuh"
+#include "dqn_head.cuh"
+#include "errors.h"
+#include "kernels.h"
+#include "../../include/scalerl_b200.h"
+
+namespace srl {
+
+constexpr int64_t ACTOR_OBS_BYTES = 4 * 84 * 84;
+
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011): four 32-bit words of counter c under key k
+SRL_DEVINL uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u; k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// One warp per env, 4 per block.  draws[0]: the draw counter (u64), read by every block and advanced by the block that finishes
+// last (draws[1] low word: the ticket, re-armed by that block), so every env of one launch uses the same draw.
+__global__ void __launch_bounds__(128) apex_act_kernel(const float* __restrict__ core, const float* __restrict__ W, const float* __restrict__ b,
+                                                       int E, int A, const float* __restrict__ eps, uint2 key,
+                                                       unsigned long long* draws, int64_t* __restrict__ actions) {
+  const int lane = threadIdx.x & 31, e = blockIdx.x * 4 + (threadIdx.x >> 5);
+  const unsigned long long d = *reinterpret_cast<volatile unsigned long long*>(draws);
+  if (e < E) {
+    int greedy;
+    q_max(core + (size_t)e * ENC_CORE, W, b, A, lane, &greedy);
+    if (lane == 0) {
+      const uint4 r = philox4x32_10(make_uint4((uint32_t)d, (uint32_t)(d >> 32), (uint32_t)e, 0u), key);
+      const float u = (float)(r.x >> 8) * 0x1p-24f;                            // uniform in [0, 1)
+      const int random_action = (int)(((unsigned long long)r.y * (unsigned)A) >> 32);   // uniform in [0, A)
+      actions[e] = u < __ldg(eps + e) ? random_action : greedy;
+    }
+  }
+  __shared__ bool is_last;
+  __syncthreads();                 // every warp of the block has read the counter
+  if (threadIdx.x == 0) is_last = take_ticket(reinterpret_cast<float*>(draws + 1));
+  __syncthreads();
+  if (is_last && threadIdx.x == 0) {
+    draws[0] = d + 1;
+    *reinterpret_cast<unsigned*>(draws + 1) = 0u;
+  }
+}
+
+// One warp per transition e in ring slot (ptr + e) mod M, 4 per block: q = Q(s)[a], y = R + gamma_n (1 - d) max_a Q(s'), the
+// learner tail's arithmetic (dqn_tail_kernel with the snapshot as online and target network, no double DQN)
+__global__ void __launch_bounds__(128) apex_priority_kernel(const float* __restrict__ core_s, const float* __restrict__ core_n,
+                                                            const float* __restrict__ W, const float* __restrict__ b, int E, int A,
+                                                            const int64_t* __restrict__ action, const float* __restrict__ reward,
+                                                            const uint8_t* __restrict__ done, int64_t ptr, int64_t M, float gamma_n, float eps,
+                                                            double* __restrict__ prio) {
+  const int lane = threadIdx.x & 31, e = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (e >= E) return;
+  const int64_t slot = (ptr + e) % M;
+  const int act = ld_action(action + slot, A);
+  const float q = q_dot(core_s + (size_t)e * ENC_CORE, W + (size_t)act * 512, lane) + __ldg(b + act);
+  int a_star;
+  const float nx = q_max(core_n + (size_t)e * ENC_CORE, W, b, A, lane, &a_star);
+  const float y = td_target(__ldg(reward + slot), gamma_n, nx, done[slot] != 0);
+  if (lane == 0) prio[e] = td_priority(__fsub_rn(q, y), eps);
+}
+
+}  // namespace srl
+using namespace srl;
+
+struct srl_apex_actor {
+  int A, E;
+  uint2 key;
+  const float* w8[8];              // the encoder tensors of the snapshot
+  const float *Wq, *bq;
+  srl_encoder_t* enc;
+  char *saved, *scratch;           // encoder blocks for E frames: the two forwards of an add run one after the other
+  float* core;                     // [2E][ENC_CORE]: the forward over s (and act's), then the one over s'
+  float* zero_reward;              // the reward / action columns of the forwards (the Q head reads h only)
+  int64_t* zero_action;
+  double* prio;                    // [E] the priorities of the last add
+  unsigned long long* draws;       // [0] draw counter, [1] the act kernel's ticket
+  char* arena;
+};
+
+namespace {
+int actor_rows(srl_apex_actor* X, int64_t saved, int64_t scratch, WsRow* t) {
+  const int64_t E = X->E;
+  int n = 0;
+  t[n++] = ws_row<char>(nullptr, saved, &X->saved);
+  t[n++] = ws_row<char>(nullptr, scratch, &X->scratch);
+  t[n++] = ws_row(nullptr, 2 * E * ENC_CORE, &X->core);
+  t[n++] = ws_row(nullptr, E, &X->zero_reward);
+  t[n++] = ws_row(nullptr, E, &X->zero_action);
+  t[n++] = ws_row(nullptr, E, &X->prio);
+  t[n++] = ws_row(nullptr, 2, &X->draws);
+  return n;
+}
+constexpr int ACTOR_ROWS = 7;
+
+// Q head rows of `frames` frames of obs into core (f <= E frames per call)
+int actor_forward(srl_apex_actor* X, const uint8_t* obs, int frames, float* core, cudaStream_t st) {
+  return srl_encoder_forward(X->enc, obs, X->zero_reward, X->zero_action, frames, 1, X->w8, X->saved, X->scratch, core, st);
+}
+}  // namespace
+
+extern "C" int srl_apex_actor_create(int A, int num_envs, int precision, uint64_t seed, const float* params, srl_apex_actor_t** out) {
+  REQ(params && out, "apex_actor_create: NULL argument");
+  REQ(A >= 1 && A <= 31, "apex_actor_create: A=%d must be in [1,31]", A);
+  REQ(num_envs >= 1 && num_envs <= MAX_FRAMES, "apex_actor_create: num_envs=%d must be in [1, %d]", num_envs, MAX_FRAMES);
+  REQ(precision == 0 || precision == 1, "apex_actor_create: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", precision);
+  REQ(!misaligned(params, 16), "apex_actor_create: params must be 16-byte aligned");
+  int64_t off[10];
+  srl_apex_param_layout(A, off, nullptr);
+  int64_t sb = 0, kb = 0;
+  int rc = srl_encoder_sizes(num_envs, precision, &sb, &kb);
+  if (rc) return rc;
+  srl_apex_actor* X = new (std::nothrow) srl_apex_actor();
+  REQ(X, "out of host memory");
+  auto undo = [X](int code) { srl_apex_actor_destroy(X); return code; };
+  X->A = A; X->E = num_envs;
+  X->key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  for (int i = 0; i < 8; ++i) X->w8[i] = params + off[i];
+  X->Wq = params + off[8]; X->bq = params + off[9];
+  rc = srl_encoder_create(precision, &X->enc);
+  if (rc) return undo(rc);
+  WsRow t[ACTOR_ROWS];
+  const int n = actor_rows(X, sb, kb, t);
+  const int64_t total = rows_bytes(t, n, false);
+  cudaError_t e = cudaMalloc(&X->arena, total);
+  if (e != cudaSuccess) return undo(cuda_fail(e, "apex_actor_create: cudaMalloc"));
+  e = cudaMemset(X->arena, 0, total);          // the zero columns, the draw counter and the ticket
+  if (e != cudaSuccess) return undo(cuda_fail(e, "apex_actor_create: cudaMemset"));
+  carve_rows(t, n, false, X->arena);
+  *out = X;
+  return 0;
+}
+
+extern "C" int srl_apex_actor_destroy(srl_apex_actor_t* X) {
+  if (!X) return 0;
+  srl_encoder_destroy(X->enc);
+  cudaFree(X->arena);
+  delete X;
+  return 0;
+}
+
+extern "C" int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const float* epsilons, int64_t* actions, void* stream) {
+  REQ(X && obs && epsilons && actions, "apex_actor_act: NULL pointer");
+  const int E = X->E;
+  const Span s[3] = {{obs, E * ACTOR_OBS_BYTES, false, "obs"}, {epsilons, (int64_t)E * 4, false, "epsilons"}, {actions, (int64_t)E * 8, true, "actions"}};
+  int rc = check_spans(s, 3, "apex_actor_act");
+  if (rc) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  rc = actor_forward(X, obs, E, X->core, st);
+  if (rc) return rc;
+  apex_act_kernel<<<(E + 3) / 4, 128, 0, st>>>(X->core, X->Wq, X->bq, E, X->A, epsilons, X->key, X->draws, actions);
+  CU(cudaGetLastError(), "apex_act_kernel");
+  return 0;
+}
+
+extern "C" int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, int n, float* q_out, void* stream) {
+  REQ(X && obs && q_out, "apex_actor_q_values: NULL pointer");
+  REQ(n >= 1, "apex_actor_q_values: n=%d must be >= 1", n);
+  const Span s[2] = {{obs, n * ACTOR_OBS_BYTES, false, "obs"}, {q_out, (int64_t)n * X->A * 4, true, "q_out"}};
+  int rc = check_spans(s, 2, "apex_actor_q_values");
+  if (rc) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  for (int f0 = 0; f0 < n; f0 += X->E) {        // chunks of at most E frames: the blocks' size
+    const int f = n - f0 < X->E ? n - f0 : X->E;
+    rc = actor_forward(X, obs + (size_t)f0 * ACTOR_OBS_BYTES, f, X->core, st);
+    if (rc) return rc;
+    CU(launch_dqn_q_values(X->core, X->Wq, X->bq, f, X->A, q_out + (size_t)f0 * X->A, st), "dqn_q_values");
+  }
+  return 0;
+}
+
+namespace srl {
+int apex_actor_num_envs(const srl_apex_actor* X) { return X->E; }
+
+int apex_actor_priorities(srl_apex_actor* X, const uint8_t* s, const uint8_t* s_next, const int64_t* action, const float* reward,
+                          const uint8_t* done, int64_t ptr, int64_t M, float gamma_n, float eps, const double** prio, cudaStream_t st) {
+  const int E = X->E;
+  float* core_n = X->core + (size_t)E * ENC_CORE;
+  int rc = actor_forward(X, s, E, X->core, st);
+  if (!rc) rc = actor_forward(X, s_next, E, core_n, st);
+  if (rc) return rc;
+  apex_priority_kernel<<<(E + 3) / 4, 128, 0, st>>>(X->core, core_n, X->Wq, X->bq, E, X->A, action, reward, done, ptr, M, gamma_n, eps, X->prio);
+  CU(cudaGetLastError(), "apex_priority_kernel");
+  *prio = X->prio;
+  return 0;
+}
+}  // namespace srl

@@ -6,30 +6,12 @@
 //   dqn_wgrad_reduce_kernel   heads.cu's head_wgrad kernels), so every run computes the same bits
 //   dqn_q_values_kernel       the forward-only Q head (predict / get_action)
 //   apex_soft_update_kernel   theta_t <- tau theta + (1 - tau) theta_t (dqn_agent.py:185-190, utils/model_utils.py:29-32)
-// The Q head reads the encoder's core rows [h (512), clamp(reward), one-hot] (ENC_CORE floats per row) and only their h columns.
+// The Q head arithmetic (q_dot, q_max, the target and the priority) is dqn_head.cuh's, shared with the Ape-X actor.
 #include "common.cuh"
+#include "dqn_head.cuh"
 #include "kernels.h"
 
 namespace srl {
-
-// q = h . W[a] + b[a] for one 512-float row h of a core row and one 512-float weight row: lane-strided products, then the warp sum
-SRL_DEVINL float q_dot(const float* __restrict__ h, const float* __restrict__ w, int lane) {
-  float s = 0.f;
-#pragma unroll
-  for (int i = 0; i < 16; ++i) s = fmaf(__ldg(h + lane + 32 * i), __ldg(w + lane + 32 * i), s);
-  return warp_sum(s);
-}
-// max_a Q(h)[a] and its first argmax (torch.max(dim=1) returns the first maximal index)
-SRL_DEVINL float q_max(const float* h, const float* W, const float* b, int A, int lane, int* arg) {
-  float best = -INFINITY;
-  int ib = 0;
-  for (int a = 0; a < A; ++a) {
-    const float v = q_dot(h, W + (size_t)a * 512, lane) + __ldg(b + a);
-    if (v > best) { best = v; ib = a; }
-  }
-  *arg = ib;
-  return best;
-}
 
 // One warp per transition, 4 per block.  scratch: [0] the ticket, [4 + k] block k's partial of sum_n w_n (q_n - y_n)^2.
 __global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
@@ -49,9 +31,7 @@ __global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
     } else {            // max_a Q_target(s', a) (apex/worker.py:149, dqn_agent.py:162-163)
       nx = q_max(hn, t.Wt, t.bt, t.A, lane, &a_star);
     }
-    // y = r + gamma * Q' * (1 - d), the products and the add rounded one by one as torch evaluates them (no FMA contraction)
-    const float nd = t.done[n] ? 0.f : 1.f;
-    const float y = __fadd_rn(__ldg(t.reward + n), __fmul_rn(__fmul_rn(t.gamma, nx), nd));
+    const float y = td_target(__ldg(t.reward + n), t.gamma, nx, t.done[n] != 0);
     const float w = t.weight ? __ldg(t.weight + n) : 1.f;
     const float delta = __fsub_rn(q, y);
     l = __fmul_rn(w, __fmul_rn(delta, delta));
@@ -59,7 +39,7 @@ __global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
     const float dq = t.two_over_B * w * delta;
     if (lane == 0) {
       t.q[n] = q; t.y[n] = y; t.dq[n] = dq;
-      t.prio[n] = (double)fabsf(delta) + (double)t.priority_eps;      // apex/worker.py:152-154 (+ eps > 0 keeps the tree's assert)
+      t.prio[n] = td_priority(delta, t.priority_eps);
     }
     const float* wa = t.Wq + (size_t)act * 512;
     float* dc = t.dcore + (size_t)n * ENC_CORE;

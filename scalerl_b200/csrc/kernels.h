@@ -241,9 +241,20 @@ cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float 
 
 }  // namespace srl
 struct srl_per;
+struct srl_apex_actor;
 namespace srl {
 // ---- per.cu: what the replay memory (replay.cu) shares with its sampler, whose leaf i is the memory's ring slot i
 int64_t per_tree_ptr(const srl_per* P);          // the leaf the next add writes
+// n new leaves at tree_ptr.. = priorities[i]^alpha (f64 [n], device), max_priority updated, the count advanced as by srl_per_add; a
+// non-finite priority is stored as max_priority^alpha and counted by srl_per_invalid_updates.  0, or an error code with the message set
+int per_add_prioritized(srl_per* P, const double* priorities, int64_t n, cudaStream_t st);
+// ---- apex_actor.cu: what the prioritized add (replay.cu) uses of an Ape-X actor
+int apex_actor_num_envs(const srl_apex_actor* X);
+// the actor's initial priorities of E transitions that sit in ring slots (ptr + e) mod M: s = state rows, s' = next_state rows (u8
+// [E,4,84,84] each), action / reward / done read from the ring's slots.  p = |Q(s)[a] - (R + gamma_n (1 - d) max_a Q(s'))| + eps with
+// the learner tail's arithmetic (dqn_head.cuh) -> *prio, the actor's f64 [E] device buffer.  0, or an error code with the message set
+int apex_actor_priorities(srl_apex_actor* X, const uint8_t* s, const uint8_t* s_next, const int64_t* action, const float* reward,
+                          const uint8_t* done, int64_t ptr, int64_t M, float gamma_n, float eps, const double** prio, cudaStream_t st);
 // srl_per_sample with an optional device beta (beta_dev, read when the kernel runs; NULL: `beta`)
 int per_sample(srl_per* P, const double* uniforms, int batch, double beta, const double* beta_dev, int64_t* idxs, double* weights64,
                float* weights32, cudaStream_t st);

@@ -20,6 +20,8 @@ __device__ __forceinline__ int64_t* per_count_slot(double* scal) { return reinte
 // sequential loop would), then recompute every touched ancestor level by level.
 //   mode 0: idxs/priorities given, leaf = priority^alpha, max_priority updated; idxs at or above the stored count are skipped.
 //   mode 1: leaves ptr.. (mod memory_size) = max_priority^alpha, stored count = min(count + n, memory_size)
+//   mode 2: leaves ptr.. (mod memory_size) = priority^alpha from prios, max_priority updated, the count as mode 1.  A non-finite priority
+//           is counted in scal[1] and stored as mode 1 would store it (max_priority^alpha as the launch found it)
 __global__ void __launch_bounds__(1024) per_update_kernel(double* __restrict__ sum, double* __restrict__ mn, int64_t cap, int levels,
                                                           const int64_t* __restrict__ idxs, const double* __restrict__ prios, int n,
                                                           double alpha, double* __restrict__ scal, int mode, int64_t ptr, int64_t memory_size) {
@@ -32,21 +34,29 @@ __global__ void __launch_bounds__(1024) per_update_kernel(double* __restrict__ s
   if (t < n) {
     if (mode == 0) {
       const int64_t count = *per_count_slot(scal);
-      leaf = idxs[t]; pr = prios[t]; v = pow(pr, alpha);
+      leaf = idxs[t]; pr = prios[t];
       // the reference asserts priority > 0 and 0 <= idx < len(self) (replay_buffer.py:346-351): an invalid entry is
       // skipped here (never an out-of-bounds write) and counted in scal[1]; the Python wrapper raises on it
       if (!(leaf >= 0 && leaf < count) || !(pr > 0.0)) { valid = false; leaf = -1; atomicAdd(reinterpret_cast<unsigned long long*>(scal + 1), 1ull); }
-    } else { leaf = (ptr + t) % memory_size; v = pow(scal[0], alpha); }
+    } else {
+      leaf = (ptr + t) % memory_size;
+      if (mode == 2) pr = prios[t];
+      if (mode == 1 || !isfinite(pr)) {
+        if (mode == 2) atomicAdd(reinterpret_cast<unsigned long long*>(scal + 1), 1ull);
+        pr = scal[0];                  // read before the barrier that precedes thread 0's max_priority store: max(max, max) = max
+      }
+    }
+    v = pow(pr, alpha);
   }
   sidx[t] = leaf;
   __syncthreads();
-  if (mode == 1 && t == 0) { int64_t* c = per_count_slot(scal); *c = *c + n < memory_size ? *c + n : memory_size; }
+  if (mode != 0 && t == 0) { int64_t* c = per_count_slot(scal); *c = *c + n < memory_size ? *c + n : memory_size; }
   bool winner = valid;
   if (winner && mode == 0)
     for (int u = t + 1; u < n; ++u)
       if (sidx[u] == leaf) { winner = false; break; }
   if (winner) { sum[cap + leaf] = v; mn[cap + leaf] = v; }
-  if (mode == 0) {       // max_priority = max(max_priority, priorities...)
+  if (mode != 1) {       // max_priority = max(max_priority, priorities...)
     double m = valid ? pr : 0.0;
     for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((t & 31) == 0) smax[t >> 5] = m;
@@ -147,19 +157,27 @@ extern "C" int srl_per_destroy(srl_per_t* P) { if (P) { cudaFree(P->sum); cudaFr
 extern "C" int64_t srl_per_size(const srl_per_t* P) { return P ? P->size : 0; }
 extern "C" int64_t srl_per_capacity(const srl_per_t* P) { return P ? P->capacity : 0; }
 
+namespace {
+// n new leaves at tree_ptr.., in launches of at most 1024 (and at most memory_size: never two writes to one leaf inside a launch):
+// max_priority^alpha (prios NULL, mode 1), or prios[i]^alpha (mode 2)
+cudaError_t per_insert(srl_per* P, const double* prios, int64_t n, cudaStream_t st) {
+  for (int64_t o = 0; o < n;) {
+    const int64_t c = n - o < 1024 ? n - o : 1024;
+    const int cc = (int)(c < P->memory_size ? c : P->memory_size);
+    per_update_kernel<<<1, 1024, 0, st>>>(P->sum, P->mn, P->capacity, P->levels, nullptr, prios ? prios + o : nullptr, cc, P->alpha, P->scal,
+                                          prios ? 2 : 1, P->tree_ptr, P->memory_size);
+    P->tree_ptr = (P->tree_ptr + cc) % P->memory_size;
+    P->size = P->size + cc < P->memory_size ? P->size + cc : P->memory_size;
+    o += cc;
+  }
+  return cudaGetLastError();
+}
+}  // namespace
+
 // n new transitions written at tree_ptr.. with priority max_priority^alpha (_add, replay_buffer.py:318-322)
 extern "C" int srl_per_add(srl_per_t* P, int64_t n, void* stream) {
   REQ(P && n >= 0, "per_add: bad argument");
-  while (n > 0) {
-    const int c = (int)(n < 1024 ? n : 1024);
-    const int cc = c < P->memory_size ? c : (int)P->memory_size;       // never two writes to one leaf inside a launch
-    per_update_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(P->sum, P->mn, P->capacity, P->levels, nullptr, nullptr, cc, P->alpha, P->scal, 1,
-                                                            P->tree_ptr, P->memory_size);
-    P->tree_ptr = (P->tree_ptr + cc) % P->memory_size;
-    P->size = P->size + cc < P->memory_size ? P->size + cc : P->memory_size;
-    n -= cc;
-  }
-  CU(cudaGetLastError(), "per_add");
+  CU(per_insert(P, nullptr, n, (cudaStream_t)stream), "per_add");
   return 0;
 }
 // idxs i64 [n], priorities f64 [n] (device): leaf = priority^alpha, max_priority updated (update_priorities, replay_buffer.py:346-351)
@@ -184,6 +202,10 @@ extern "C" int64_t srl_per_invalid_updates(srl_per_t* P, void* stream) {
 }
 namespace srl {
 int64_t per_tree_ptr(const srl_per* P) { return P->tree_ptr; }
+int per_add_prioritized(srl_per* P, const double* priorities, int64_t n, cudaStream_t st) {
+  CU(per_insert(P, priorities, n, st), "per_add_prioritized");
+  return 0;
+}
 int per_sample(srl_per* P, const double* uniforms, int batch, double beta, const double* beta_dev, int64_t* idxs, double* weights64,
                float* weights32, cudaStream_t st) {
   REQ(P && uniforms && idxs && batch >= 1, "per_sample: bad argument");

@@ -90,6 +90,7 @@ struct srl_replay {
   int64_t memory_size;
   int num_envs, n_step;
   GammaPowers gp;
+  float gamma_n;                   // fp32(gamma^n_step): the bootstrap discount of an n-step transition (srl_replay_add_prioritized)
   int64_t steps;                   // vector steps added so far (host-known: adds are host calls)
   void* arena;
   ReplayRows ring, win;
@@ -141,6 +142,7 @@ extern "C" int srl_replay_create(int64_t memory_size, int num_envs, int n_step, 
   REQ(R, "out of memory");
   R->memory_size = memory_size; R->num_envs = num_envs; R->n_step = n_step; R->steps = 0;
   for (int k = 0; k < REPLAY_MAX_NSTEP; ++k) R->gp.g[k] = (float)pow(gamma, (double)k);    // numpy's float32(gamma ** k)
+  R->gamma_n = (float)pow(gamma, (double)n_step);
   WsRow t[10];
   const int nrows = replay_rows(R, t);
   const int64_t bytes = rows_bytes(t, nrows, false);
@@ -165,10 +167,11 @@ extern "C" int srl_replay_destroy(srl_replay_t* R) {
 extern "C" int64_t srl_replay_size(const srl_replay_t* R) { return R ? srl_per_size(R->per) : 0; }
 extern "C" srl_per_t* srl_replay_per(srl_replay_t* R) { return R ? R->per : nullptr; }
 
-extern "C" int srl_replay_add(srl_replay_t* R, const uint8_t* state, const int64_t* action, const float* reward, const uint8_t* next_state,
-                              const uint8_t* done, void* stream) {
-  REQ(R && state && action && reward && next_state && done, "replay_add: NULL pointer");
-  const cudaStream_t st = (cudaStream_t)stream;
+namespace {
+// one vector step into the window and, once the window is full, its fold into ring slots (ptr + e) mod M.  *oldest: the window slot
+// of the step the fold took state and action from, -1 while the window is filling (replay_buffer.py:208-210: no transition yet)
+int stage_and_fold(srl_replay* R, const uint8_t* state, const int64_t* action, const float* reward, const uint8_t* next_state,
+                   const uint8_t* done, cudaStream_t st, int* oldest) {
   const int E = R->num_envs, n = R->n_step;
   const int64_t w = (R->steps % n) * E;                       // this vector step's window slot
   CU(cudaMemcpyAsync(R->win.state + w * OBS_VEC, state, E * OBS_BYTES, cudaMemcpyDefault, st), "replay_add: copy state");
@@ -177,12 +180,46 @@ extern "C" int srl_replay_add(srl_replay_t* R, const uint8_t* state, const int64
   CU(cudaMemcpyAsync(R->win.reward + w, reward, E * sizeof(float), cudaMemcpyDefault, st), "replay_add: copy reward");
   CU(cudaMemcpyAsync(R->win.done + w, done, E, cudaMemcpyDefault, st), "replay_add: copy done");
   R->steps++;
-  if (R->steps < n) return 0;                                  // the window is not full yet: no transition (replay_buffer.py:208-210)
-  const int oldest = (int)(R->steps % n);
-  replay_fold_kernel<<<dim3(E, (ROW_PAIR_VEC + FOLD_THREADS - 1) / FOLD_THREADS), FOLD_THREADS, 0, st>>>(R->win, R->ring, E, n, oldest, R->gp,
+  *oldest = -1;
+  if (R->steps < n) return 0;
+  *oldest = (int)(R->steps % n);
+  replay_fold_kernel<<<dim3(E, (ROW_PAIR_VEC + FOLD_THREADS - 1) / FOLD_THREADS), FOLD_THREADS, 0, st>>>(R->win, R->ring, E, n, *oldest, R->gp,
                                                                                                        per_tree_ptr(R->per), R->memory_size);
   CU(cudaGetLastError(), "replay_add: fold");
-  return srl_per_add(R->per, E, stream);                       // the trees' _add of E leaves, env order (replay_buffer.py:319-323)
+  return 0;
+}
+}  // namespace
+
+extern "C" int srl_replay_add(srl_replay_t* R, const uint8_t* state, const int64_t* action, const float* reward, const uint8_t* next_state,
+                              const uint8_t* done, void* stream) {
+  REQ(R && state && action && reward && next_state && done, "replay_add: NULL pointer");
+  int oldest;
+  const int rc = stage_and_fold(R, state, action, reward, next_state, done, (cudaStream_t)stream, &oldest);
+  if (rc || oldest < 0) return rc;
+  return srl_per_add(R->per, R->num_envs, stream);            // the trees' _add of E leaves, env order (replay_buffer.py:319-323)
+}
+
+extern "C" int srl_replay_add_prioritized(srl_replay_t* R, srl_apex_actor_t* actor, const uint8_t* state, const int64_t* action, const float* reward,
+                                          const uint8_t* next_state, const uint8_t* done, float priority_eps, void* stream) {
+  REQ(R && actor && state && action && reward && next_state && done, "replay_add_prioritized: NULL pointer");
+  REQ(isfinite(priority_eps) && priority_eps > 0.f, "replay_add_prioritized: priority_eps=%g must be finite and > 0", (double)priority_eps);
+  REQ(apex_actor_num_envs(actor) == R->num_envs, "replay_add_prioritized: the actor has num_envs=%d, the memory %d", apex_actor_num_envs(actor),
+      R->num_envs);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int E = R->num_envs;
+  const int64_t ptr = per_tree_ptr(R->per);                   // the fold's first ring slot
+  int oldest;
+  int rc = stage_and_fold(R, state, action, reward, next_state, done, st, &oldest);
+  if (rc || oldest < 0) return rc;
+  // s: the oldest step's state rows; s': the newest step's next_state rows, the s' of every transition without a done in its window
+  // (one with a done has d = 1, which zeroes its bootstrap term)
+  const int newest = (int)((R->steps - 1) % R->n_step);
+  const double* prio = nullptr;
+  rc = apex_actor_priorities(actor, reinterpret_cast<const uint8_t*>(R->win.state + (int64_t)oldest * E * OBS_VEC),
+                             reinterpret_cast<const uint8_t*>(R->win.next_state + (int64_t)newest * E * OBS_VEC), R->ring.action, R->ring.reward,
+                             R->ring.done, ptr, R->memory_size, R->gamma_n, priority_eps, &prio, st);
+  if (rc) return rc;
+  return per_add_prioritized(R->per, prio, E, st);           // leaves ptr .. ptr + E - 1 in env order
 }
 
 extern "C" int srl_replay_sample(srl_replay_t* R, const double* uniforms, int batch, const double* beta_dev, uint8_t* state, int64_t* action,

@@ -79,11 +79,22 @@ class GpuPrioritizedReplayBuffer:
             raise ValueError(f'{name} is on {t.device}, the memory on {self.device}')
         return t, dtype
 
-    def save_to_memory(self, state, action, reward, next_state, done, is_vectorised: bool = False) -> None:
+    def save_to_memory(self, state, action, reward, next_state, done, is_vectorised: bool = False, priorities_from=None) -> None:
         """one env step: states uint8 [E, 4, 84, 84], action integer [E], reward floating [E], done bool / uint8 [E] (vectorised), or
         one env's [4, 84, 84] and scalars (``num_envs == 1``).  CUDA tensors of the stored dtypes are read in place; numpy arrays and
         CPU tensors are copied on the current stream.  Once n_step steps are staged, every call adds E n-step transitions at maximum
-        priority (replay_buffer.py:197-218, 319-323)."""
+        priority (replay_buffer.py:197-218, 319-323) or, with ``priorities_from`` (a B200ApexActor on this device with this memory's
+        num_envs), at the priorities that actor computes for them: |Q(s)[a] - (R + gamma^n (1 - d) max_a Q(s'))| + its priority_eps
+        (apex/worker.py:59-79, apex/memory.py:43-64).  A non-finite priority enters as the plain add's and is counted by the sampler's
+        invalid-update counter."""
+        if priorities_from is not None:
+            from ..algorithms.apex.actor import B200ApexActor
+            if not isinstance(priorities_from, B200ApexActor):
+                raise ValueError(f'priorities_from must be a B200ApexActor, got {type(priorities_from).__name__}')
+            if priorities_from.device != self.device:
+                raise ValueError(f'priorities_from is on {priorities_from.device}, the memory on {self.device}')
+            if priorities_from.num_envs != self.num_envs:
+                raise ValueError(f'priorities_from has num_envs={priorities_from.num_envs}, the memory {self.num_envs}')
         E = self.num_envs
         if is_vectorised:
             lead = (E,)
@@ -100,8 +111,13 @@ class GpuPrioritizedReplayBuffer:
         # every field is checked before the first copy: a bad step adds nothing
         s, a, r, ns, d = ((t.view(torch.uint8) if t.dtype == torch.bool else t).to(self.device, dt).contiguous() for t, dt in (s, a, r, ns, d))
         with torch.cuda.device(self.device):
-            _lib.check(self._L.srl_replay_add(self._h, s.data_ptr(), a.data_ptr(), r.data_ptr(), ns.data_ptr(), d.data_ptr(), self._stream()),
-                       'srl_replay_add')
+            if priorities_from is None:
+                _lib.check(self._L.srl_replay_add(self._h, s.data_ptr(), a.data_ptr(), r.data_ptr(), ns.data_ptr(), d.data_ptr(), self._stream()),
+                           'srl_replay_add')
+            else:
+                _lib.check(self._L.srl_replay_add_prioritized(self._h, priorities_from._h, s.data_ptr(), a.data_ptr(), r.data_ptr(), ns.data_ptr(),
+                                                              d.data_ptr(), priorities_from.priority_eps, self._stream()),
+                           'srl_replay_add_prioritized')
 
     # ------------------------------------------------------------------ sampling
     def _set_beta(self, beta: float) -> None:
