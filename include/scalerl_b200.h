@@ -363,11 +363,16 @@ int srl_replay_gather(srl_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* 
 /* ---- Ape-X learner step: a prioritized (double) DQN update on the encoder (BASELINE.json configs[3]) --------------------------
  * replaces the learner statements of the reference's Ape-X Learner.train (scalerl/algorithms/apex/worker.py:134-161) and, with
  * double DQN, clipping and the target cadence, DQNAgent.learn (scalerl/algorithms/dqn/dqn_agent.py:136-190).  The Q network is
- * Nature DQN: AtariNet's conv1..3 + fc + ReLU (atari_model.py:30-47,91-101) followed by q = Linear(512, A), A in [1, 31].
+ * Nature DQN: AtariNet's conv1..3 + fc + ReLU (atari_model.py:30-47,91-101) followed by q = Linear(512, A), A in [1, 31], or, with
+ * `dueling`, the dueling head of Wang et al. 2016 (eq. 9) on the same 512 fc features: V = value(h) = Linear(512, 1), Adv =
+ * advantage(h) = Linear(512, A), Q = V + Adv - mean_a Adv.  Both heads read the shared fc output (the paper's Atari network has two
+ * separate 512-unit fc streams): the encoder is the same for both.
  * srl_replay_* stores and folds n-step transitions (pass gamma^n for them, and srl_replay_per as `per`); srl_apex_actor_* acts and computes
  * their initial priorities.
  * Parameters in state_dict order {conv1.weight, conv1.bias, conv2.weight, conv2.bias, conv3.weight, conv3.bias, fc.weight, fc.bias,
  * q.weight [A,512], q.bias [A]}; srl_apex_param_layout returns the flat buffer's floats and each tensor's offset / count (int64[10]).
+ * The dueling head's state_dict order is {conv1..3, fc, value.weight [1,512], value.bias [1], advantage.weight [A,512],
+ * advantage.bias [A]} (int64[12], srl_apex_param_layout_ex); value.weight lies directly before advantage.weight.
  * In memory the small tensors come first and fc.weight last; segments are padded to 4 floats.  Params, grads, both Adam states
  * and the target copy share the layout. */
 typedef struct srl_apex_learner srl_apex_learner_t;
@@ -380,8 +385,12 @@ typedef struct srl_apex_config {
   float max_grad_norm;       /* clip_grad_norm_ threshold (dqn_agent.py:178-181), > 0; +inf: no clip (coef 1) */
   float learning_rate, adam_beta1, adam_beta2, adam_eps;   /* torch.optim.Adam (apex/worker.py:132)            */
   float priority_eps;        /* priority = |q - y| + priority_eps (in double), >= 0                           */
+  int32_t dueling;           /* 0: q = Linear(512, A); 1: the dueling head Q = V + Adv - mean(Adv)             */
 } srl_apex_config_t;
 int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10);
+/* the layout of either head: dueling 0 -> 10 tensors (srl_apex_param_layout's), 1 -> 12; -1 with srl_last_error set for A outside
+ * [1, 31] or dueling outside {0, 1} */
+int64_t srl_apex_param_layout_ex(int A, int dueling, int64_t* offsets12, int64_t* counts12);
 /* params / grads / exp_avg / exp_avg_sq / target_params: caller-owned flat f32 device buffers of srl_apex_param_layout floats,
  * 16-byte aligned and disjoint.  The context owns the encoder's blocks (one saved block for the forward over s, one for the
  * forwards over s', their scratch) and the tail's buffers.  Synchronous. */
@@ -420,6 +429,9 @@ int srl_apex_learner_debug_buffer(srl_apex_learner_t* L, const char* name, void*
 typedef struct srl_apex_actor srl_apex_actor_t;
 /* A in [1, 31], num_envs in [1, 65536], precision as srl_apex_config_t.precision, seed: the key of the actor's random numbers */
 int srl_apex_actor_create(int A, int num_envs, int precision, uint64_t seed, const float* params, srl_apex_actor_t** out);
+/* the same with the head kind: dueling 0 (q = Linear(512, A), srl_apex_actor_create's) or 1 (the dueling head; params in
+ * srl_apex_param_layout_ex(A, 1) order) */
+int srl_apex_actor_create_ex(int A, int num_envs, int precision, int dueling, uint64_t seed, const float* params, srl_apex_actor_t** out);
 int srl_apex_actor_destroy(srl_apex_actor_t* X);
 /* obs u8 [E,4,84,84], epsilons f32 [E] (device) -> actions i64 [E]: with probability epsilons[e] a uniform action, else the first
  * argmax of Q(obs[e]) (torch.argmax's pick).  The random numbers are Philox4x32-10 keyed by seed, counted by (draw, env); the launch

@@ -11,6 +11,8 @@ epsilon, from a parameter snapshot on the device (srl_apex_actor_*, csrc/apex_ac
   * ``GpuPrioritizedReplayBuffer.save_to_memory(..., priorities_from=actor)``: the transitions the add completes enter the trees with
     |Q(s)[a] - (R + gamma^n (1 - d) max_a Q(s'))| + priority_eps, computed with the learner's target and priority arithmetic.
   * ``sync_from(learner)``: one device copy of the learner's online parameters into the snapshot.
+
+``dueling_dqn=True`` gives the actor the dueling head of ``ApexHParams(dueling_dqn=True)``; it syncs from dueling learners only.
 """
 from __future__ import annotations
 
@@ -41,11 +43,11 @@ def apex_epsilons(num_envs: int, eps: float = 0.4, alpha: float = 7.0) -> np.nda
 class B200ApexActor:
     """``num_envs`` Ape-X actors on one GPU, acting on a snapshot of a ``B200ApexLearner``'s Q network (``AtariQNet`` names and
     shapes).  ``epsilons``: [num_envs] values in [0, 1] (None: ``apex_epsilons(num_envs)``); ``precision``: the encoder operands, as
-    the learner's; ``priority_eps`` (> 0) is added to every priority the actor computes.  Calls run on the current stream and share the
-    actor's buffers: issue them from one stream."""
+    the learner's; ``priority_eps`` (> 0) is added to every priority the actor computes; ``dueling_dqn``: the learner's head kind.
+    Calls run on the current stream and share the actor's buffers: issue them from one stream."""
 
     def __init__(self, num_envs: int, num_actions: int, epsilons=None, seed: int = 0, precision: str = 'bf16', priority_eps: float = 1e-6,
-                 device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None):
+                 device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None, dueling_dqn: bool = False):
         for name, v, hi in (('num_envs', num_envs, MAX_FRAMES), ('num_actions', num_actions, 31)):
             if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= hi:
                 raise ValueError(f'{name} must be an int in [1, {hi}], got {v!r}')
@@ -53,27 +55,29 @@ class B200ApexActor:
             raise ValueError(f'seed must be an int in [0, 2**64), got {seed!r}')
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be 'bf16' or 'fp32_split', got {precision!r}")
+        if not isinstance(dueling_dqn, bool):
+            raise ValueError(f'dueling_dqn must be a bool, got {dueling_dqn!r}')
         priority_eps = float(priority_eps)
         if not (math.isfinite(priority_eps) and priority_eps > 0.0):
             raise ValueError(f'priority_eps must be finite and > 0 (a zero leaf makes the sampler\'s IS weight infinite), got {priority_eps}')
         self.num_envs, self.num_actions, self.seed, self.precision = int(num_envs), int(num_actions), int(seed), precision
-        self.priority_eps = priority_eps
+        self.priority_eps, self.dueling_dqn = priority_eps, dueling_dqn
         eps = self._epsilons(apex_epsilons(self.num_envs) if epsilons is None else epsilons)
         if not torch.cuda.is_available():
             raise RuntimeError('B200ApexActor needs a CUDA device: scalerl_b200 has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._L = _lib.lib()
-        self.shapes = apex_param_shapes(self.num_actions)
+        self.shapes = apex_param_shapes(self.num_actions, dueling_dqn)
         with torch.cuda.device(self.device):
-            total, off, cnt = _lib.apex_param_layout(self.num_actions)
+            total, off, cnt = _lib.apex_param_layout(self.num_actions, dueling_dqn)
             self.flat_params = torch.zeros(total, dtype=torch.float32, device=self.device)
             self.params = flat_views(self.flat_params, off, cnt, self.shapes)
             self.epsilons = eps.to(self.device)           # read by the act kernel when it runs
             h = C.c_void_p()
-            _lib.check(self._L.srl_apex_actor_create(self.num_actions, self.num_envs, PRECISIONS[precision], self.seed,
-                                                     self.flat_params.data_ptr(), C.byref(h)), 'srl_apex_actor_create')
+            _lib.check(self._L.srl_apex_actor_create_ex(self.num_actions, self.num_envs, PRECISIONS[precision], int(dueling_dqn), self.seed,
+                                                        self.flat_params.data_ptr(), C.byref(h)), 'srl_apex_actor_create_ex')
             self._h = h
-        self.load_state_dict(default_q_state_dict(self.num_actions, self.seed) if init_state_dict is None else init_state_dict)
+        self.load_state_dict(default_q_state_dict(self.num_actions, self.seed, dueling_dqn) if init_state_dict is None else init_state_dict)
         self.weights_version = 0
 
     def _stream(self):
@@ -103,6 +107,8 @@ class B200ApexActor:
             raise ValueError(f'sync_from needs a B200ApexLearner, got {type(learner).__name__}')
         if learner.hp.num_actions != self.num_actions:
             raise ValueError(f'the learner has num_actions={learner.hp.num_actions}, the actor {self.num_actions}')
+        if learner.hp.dueling_dqn != self.dueling_dqn:
+            raise ValueError(f'the learner has dueling_dqn={learner.hp.dueling_dqn}, the actor {self.dueling_dqn}')
         if learner.device != self.device:
             raise ValueError(f'the learner is on {learner.device}, the actor on {self.device}')
         self.flat_params.copy_(learner.flat_params)

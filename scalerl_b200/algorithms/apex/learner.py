@@ -7,6 +7,10 @@ batch, the bootstrapped targets, the importance-weighted squared TD loss, the ne
 captured as one CUDA graph.  ``learn_from`` samples and gathers its batch from a ``GpuPrioritizedReplayBuffer`` (device-resident
 n-step storage) inside the same graph.  ``B200ApexActor`` (actor.py) acts and computes initial priorities on a copy of its weights.
 ``AtariQNet`` is the CPU torch Q network with the learner's parameter names and shapes (the actors' copy).
+
+``ApexHParams(dueling_dqn=True)`` replaces the Q head ``q = Linear(512, A)`` by the dueling head of Wang et al. 2016 (eq. 9):
+``V = value(h)``, ``Adv = advantage(h)``, ``Q = V + Adv - Adv.mean(1, keepdim=True)``.  Both streams read the encoder's shared 512-unit
+fc output (the paper's Atari network gives each stream an fc layer of its own), so the encoder is the plain network's.
 """
 from __future__ import annotations
 
@@ -29,30 +33,43 @@ from ..base import BaseAgent
 # state_dict order = AtariQNet.parameters() order = the integer keys of the Adam state (srl_apex_param_layout order)
 APEX_PARAM_NAMES = ('conv1.weight', 'conv1.bias', 'conv2.weight', 'conv2.bias', 'conv3.weight', 'conv3.bias',
                     'fc.weight', 'fc.bias', 'q.weight', 'q.bias')
+# the same for the dueling head (srl_apex_param_layout_ex(A, 1) order)
+APEX_DUELING_PARAM_NAMES = APEX_PARAM_NAMES[:8] + ('value.weight', 'value.bias', 'advantage.weight', 'advantage.bias')
 MAX_FRAMES = 65536           # frames of one encoder call (MAX_FRAMES in csrc/kernels.h)
 
 
-def apex_param_shapes(num_actions: int):
+def apex_param_names(dueling: bool = False):
+    return APEX_DUELING_PARAM_NAMES if dueling else APEX_PARAM_NAMES
+
+
+def apex_param_shapes(num_actions: int, dueling: bool = False):
+    head = [('value.weight', (1, 512)), ('value.bias', (1,)), ('advantage.weight', (num_actions, 512)), ('advantage.bias', (num_actions,))] \
+        if dueling else [('q.weight', (num_actions, 512)), ('q.bias', (num_actions,))]
     return OrderedDict([
         ('conv1.weight', (32, 4, 8, 8)), ('conv1.bias', (32,)), ('conv2.weight', (64, 32, 4, 4)), ('conv2.bias', (64,)),
-        ('conv3.weight', (64, 64, 3, 3)), ('conv3.bias', (64,)), ('fc.weight', (512, 3136)), ('fc.bias', (512,)),
-        ('q.weight', (num_actions, 512)), ('q.bias', (num_actions,))])
+        ('conv3.weight', (64, 64, 3, 3)), ('conv3.bias', (64,)), ('fc.weight', (512, 3136)), ('fc.bias', (512,))] + head)
 
 
 class AtariQNet(nn.Module):
     """Nature DQN on 4 stacked 84x84 frames: AtariNet's conv1..3 and fc (scalerl/algorithms/utils/atari_model.py:30-47, 91-101)
-    followed by ``q = nn.Linear(512, num_actions)``.  Initialised by torch's default layer init, so ``torch.manual_seed(s)`` before
-    construction fixes the weights."""
+    followed by ``q = nn.Linear(512, num_actions)``, or, with ``dueling``, by ``value = nn.Linear(512, 1)`` and ``advantage =
+    nn.Linear(512, num_actions)`` combined as Q = V + Adv - mean_a Adv (Wang et al. 2016, eq. 9).  Initialised by torch's default
+    layer init, so ``torch.manual_seed(s)`` before construction fixes the weights."""
 
-    def __init__(self, num_actions: int, observation_shape=(4, 84, 84)):
+    def __init__(self, num_actions: int, observation_shape=(4, 84, 84), dueling: bool = False):
         super().__init__()
         self.observation_shape = tuple(observation_shape)
         self.num_actions = int(num_actions)
+        self.dueling = bool(dueling)
         self.conv1 = nn.Conv2d(self.observation_shape[0], 32, kernel_size=8, stride=4)
         self.conv2 = nn.Conv2d(32, 64, kernel_size=4, stride=2)
         self.conv3 = nn.Conv2d(64, 64, kernel_size=3, stride=1)
         self.fc = nn.Linear(3136, 512)
-        self.q = nn.Linear(512, self.num_actions)
+        if self.dueling:
+            self.value = nn.Linear(512, 1)
+            self.advantage = nn.Linear(512, self.num_actions)
+        else:
+            self.q = nn.Linear(512, self.num_actions)
 
     def forward(self, obs: torch.Tensor) -> torch.Tensor:
         """obs u8 [N, 4, 84, 84] -> Q values [N, A]"""
@@ -61,6 +78,9 @@ class AtariQNet(nn.Module):
         x = F.relu(self.conv2(x))
         x = F.relu(self.conv3(x))
         x = F.relu(self.fc(x.reshape(x.shape[0], -1)))
+        if self.dueling:
+            v, adv = self.value(x), self.advantage(x)
+            return v + adv - adv.mean(dim=1, keepdim=True)
         return self.q(x)
 
 
@@ -74,6 +94,7 @@ class ApexHParams:
     learning_rate: float = 1e-3
     max_grad_norm: Optional[float] = None
     double_dqn: bool = False
+    dueling_dqn: bool = False            # the dueling head V + Adv - mean(Adv) on the shared fc output instead of q = Linear(512, A)
     target_update_frequency: int = 100
     soft_update_tau: float = 1.0
     precision: str = 'bf16'              # encoder operands: 'bf16' | 'fp32_split' (fp32-accurate hi/lo bf16 pairs)
@@ -89,6 +110,8 @@ class ApexHParams:
             raise ValueError(f'batch_size must be an int in [1, {MAX_FRAMES}], got {self.batch_size!r}')
         if not (isinstance(self.num_actions, int) and 1 <= self.num_actions <= 31):
             raise ValueError(f'num_actions must be an int in [1, 31], got {self.num_actions!r}')
+        if not isinstance(self.dueling_dqn, bool):
+            raise ValueError(f'dueling_dqn must be a bool, got {self.dueling_dqn!r}')
         if not (math.isfinite(self.gamma) and self.gamma >= 0.0):
             raise ValueError(f'gamma must be finite and >= 0, got {self.gamma}')
         if not (math.isfinite(self.learning_rate) and self.learning_rate > 0.0):
@@ -118,6 +141,7 @@ class ApexHParams:
         c.max_grad_norm = math.inf if self.max_grad_norm is None else self.max_grad_norm
         c.learning_rate, c.adam_beta1, c.adam_beta2, c.adam_eps = self.learning_rate, self.adam_beta1, self.adam_beta2, self.adam_eps
         c.priority_eps = self.priority_eps
+        c.dueling = 1 if self.dueling_dqn else 0
         return c
 
 
@@ -136,11 +160,11 @@ def load_views(dst: Dict[str, torch.Tensor], sd: Dict[str, torch.Tensor]) -> Non
         v.copy_(sd[n].to(v.device, torch.float32))
 
 
-def default_q_state_dict(num_actions: int, seed: int = 0) -> 'OrderedDict[str, torch.Tensor]':
+def default_q_state_dict(num_actions: int, seed: int = 0, dueling: bool = False) -> 'OrderedDict[str, torch.Tensor]':
     """AtariQNet's initial weights under ``torch.manual_seed(seed)``, drawn without disturbing the global RNG"""
     with torch.random.fork_rng(devices=[]):
         torch.manual_seed(seed)
-        net = AtariQNet(num_actions)
+        net = AtariQNet(num_actions, dueling=dueling)
     return OrderedDict((k, v.detach().clone()) for k, v in net.state_dict().items())
 
 
@@ -162,9 +186,10 @@ class B200ApexLearner(BaseAgent):
         self.hp = hp
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._L = _lib.lib()
-        self.shapes = apex_param_shapes(hp.num_actions)
+        self.names = apex_param_names(hp.dueling_dqn)
+        self.shapes = apex_param_shapes(hp.num_actions, hp.dueling_dqn)
         with torch.cuda.device(self.device):
-            total, self._off, self._cnt = _lib.apex_param_layout(hp.num_actions)
+            total, self._off, self._cnt = _lib.apex_param_layout(hp.num_actions, hp.dueling_dqn)
             z = lambda: torch.zeros(total, dtype=torch.float32, device=self.device)
             self.flat_params, self.flat_grads, self.exp_avg, self.exp_avg_sq, self.flat_target = z(), z(), z(), z(), z()
             self.params = self._views(self.flat_params)
@@ -177,7 +202,7 @@ class B200ApexLearner(BaseAgent):
                                                        C.byref(h)), 'srl_apex_learner_create')
             self._h = h
             self._stats = torch.zeros(4, device=self.device)      # {loss, gradient norm, clip coefficient, pad}
-        sd = default_q_state_dict(hp.num_actions, seed) if init_state_dict is None else init_state_dict
+        sd = default_q_state_dict(hp.num_actions, seed, hp.dueling_dqn) if init_state_dict is None else init_state_dict
         self.load_state_dict(sd)
         self.load_state_dict(sd, target=True)       # actor_target starts as a copy (dqn_agent.py:66-67)
         self.use_graph = use_graph
@@ -214,11 +239,11 @@ class B200ApexLearner(BaseAgent):
         return {'exp_avg': self._views(self.exp_avg), 'exp_avg_sq': self._views(self.exp_avg_sq)}
 
     def optimizer_state_dict(self) -> dict:
-        """``torch.optim.Adam(AtariQNet(...).parameters()).state_dict()`` layout"""
-        return to_torch_optimizer_state(self.hp, self._opt_tensors(), self._opt_steps, order=APEX_PARAM_NAMES)
+        """``torch.optim.Adam(AtariQNet(A, dueling=hp.dueling_dqn).parameters()).state_dict()`` layout"""
+        return to_torch_optimizer_state(self.hp, self._opt_tensors(), self._opt_steps, order=self.names)
 
     def load_optimizer_state_dict(self, sd: dict) -> None:
-        step, kinds = from_torch_optimizer_state(sd, False, order=APEX_PARAM_NAMES)
+        step, kinds = from_torch_optimizer_state(sd, False, order=self.names)
         for kind in kinds:
             if kind not in ('exp_avg', 'exp_avg_sq'):
                 raise ValueError(f"optimizer_state_dict holds '{kind}' but this learner runs Adam")

@@ -6,6 +6,7 @@
 // here has the bits of the learner's for the same weights.  fp32 on the CUDA cores: the Q head is 512 x A, no tensor-core work.
 //   apex_act_kernel       the Q row, its first argmax and the epsilon-greedy draw (one warp per env)
 //   apex_priority_kernel  q(s, a), the n-step target from max_a Q(s') and the priority (one warp per transition)
+// Both are templates on the head: plain q = Linear(512, A), or the dueling V + Adv - mean(Adv) (dqn_head.cuh's dueling_q).
 #include <math.h>
 #include <new>
 #include "common.cuh"
@@ -32,14 +33,17 @@ SRL_DEVINL uint4 philox4x32_10(uint4 c, uint2 k) {
 
 // One warp per env, 4 per block.  draws[0]: the draw counter (u64), read by every block and advanced by the block that finishes
 // last (draws[1] low word: the ticket, re-armed by that block), so every env of one launch uses the same draw.
+// DUELING: W = [(A + 1)][512], b the value bias, ba the advantage biases.
+template <bool DUELING>
 __global__ void __launch_bounds__(128) apex_act_kernel(const float* __restrict__ core, const float* __restrict__ W, const float* __restrict__ b,
                                                        int E, int A, const float* __restrict__ eps, uint2 key,
-                                                       unsigned long long* draws, int64_t* __restrict__ actions) {
+                                                       unsigned long long* draws, int64_t* __restrict__ actions, const float* __restrict__ ba) {
   const int lane = threadIdx.x & 31, e = blockIdx.x * 4 + (threadIdx.x >> 5);
   const unsigned long long d = *reinterpret_cast<volatile unsigned long long*>(draws);
   if (e < E) {
     int greedy;
-    q_max(core + (size_t)e * ENC_CORE, W, b, A, lane, &greedy);
+    if constexpr (DUELING) q_row_max(dueling_q<false>(core + (size_t)e * ENC_CORE, W, b, ba, A, lane, nullptr), A, &greedy);
+    else q_max(core + (size_t)e * ENC_CORE, W, b, A, lane, &greedy);
     if (lane == 0) {
       const uint4 r = philox4x32_10(make_uint4((uint32_t)d, (uint32_t)(d >> 32), (uint32_t)e, 0u), key);
       const float u = (float)(r.x >> 8) * 0x1p-24f;                            // uniform in [0, 1)
@@ -59,18 +63,25 @@ __global__ void __launch_bounds__(128) apex_act_kernel(const float* __restrict__
 
 // One warp per transition e in ring slot (ptr + e) mod M, 4 per block: q = Q(s)[a], y = R + gamma_n (1 - d) max_a Q(s'), the
 // learner tail's arithmetic (dqn_tail_kernel with the snapshot as online and target network, no double DQN)
+template <bool DUELING>
 __global__ void __launch_bounds__(128) apex_priority_kernel(const float* __restrict__ core_s, const float* __restrict__ core_n,
                                                             const float* __restrict__ W, const float* __restrict__ b, int E, int A,
                                                             const int64_t* __restrict__ action, const float* __restrict__ reward,
                                                             const uint8_t* __restrict__ done, int64_t ptr, int64_t M, float gamma_n, float eps,
-                                                            double* __restrict__ prio) {
+                                                            double* __restrict__ prio, const float* __restrict__ ba) {
   const int lane = threadIdx.x & 31, e = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (e >= E) return;
   const int64_t slot = (ptr + e) % M;
   const int act = ld_action(action + slot, A);
-  const float q = q_dot(core_s + (size_t)e * ENC_CORE, W + (size_t)act * 512, lane) + __ldg(b + act);
+  float q, nx;
   int a_star;
-  const float nx = q_max(core_n + (size_t)e * ENC_CORE, W, b, A, lane, &a_star);
+  if constexpr (DUELING) {
+    q = __shfl_sync(0xffffffffu, dueling_q<false>(core_s + (size_t)e * ENC_CORE, W, b, ba, A, lane, nullptr), act);
+    nx = q_row_max(dueling_q<false>(core_n + (size_t)e * ENC_CORE, W, b, ba, A, lane, nullptr), A, &a_star);
+  } else {
+    q = q_dot(core_s + (size_t)e * ENC_CORE, W + (size_t)act * 512, lane) + __ldg(b + act);
+    nx = q_max(core_n + (size_t)e * ENC_CORE, W, b, A, lane, &a_star);
+  }
   const float y = td_target(__ldg(reward + slot), gamma_n, nx, done[slot] != 0);
   if (lane == 0) prio[e] = td_priority(__fsub_rn(q, y), eps);
 }
@@ -82,7 +93,8 @@ struct srl_apex_actor {
   int A, E;
   uint2 key;
   const float* w8[8];              // the encoder tensors of the snapshot
-  const float *Wq, *bq;
+  const float *Wq, *bq;            // plain: q.weight, q.bias; dueling: [value.weight; advantage.weight], value.bias
+  const float* bqa;                // dueling: advantage.bias (NULL: the plain head)
   srl_encoder_t* enc;
   char *saved, *scratch;           // encoder blocks for E frames: the two forwards of an add run one after the other
   float* core;                     // [2E][ENC_CORE]: the forward over s (and act's), then the one over s'
@@ -115,13 +127,19 @@ int actor_forward(srl_apex_actor* X, const uint8_t* obs, int frames, float* core
 }  // namespace
 
 extern "C" int srl_apex_actor_create(int A, int num_envs, int precision, uint64_t seed, const float* params, srl_apex_actor_t** out) {
+  return srl_apex_actor_create_ex(A, num_envs, precision, 0, seed, params, out);
+}
+
+extern "C" int srl_apex_actor_create_ex(int A, int num_envs, int precision, int dueling, uint64_t seed, const float* params,
+                                        srl_apex_actor_t** out) {
   REQ(params && out, "apex_actor_create: NULL argument");
   REQ(A >= 1 && A <= 31, "apex_actor_create: A=%d must be in [1,31]", A);
   REQ(num_envs >= 1 && num_envs <= MAX_FRAMES, "apex_actor_create: num_envs=%d must be in [1, %d]", num_envs, MAX_FRAMES);
   REQ(precision == 0 || precision == 1, "apex_actor_create: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", precision);
+  REQ(dueling == 0 || dueling == 1, "apex_actor_create: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", dueling);
   REQ(!misaligned(params, 16), "apex_actor_create: params must be 16-byte aligned");
-  int64_t off[10];
-  srl_apex_param_layout(A, off, nullptr);
+  int64_t off[12];
+  srl_apex_param_layout_ex(A, dueling, off, nullptr);
   int64_t sb = 0, kb = 0;
   int rc = srl_encoder_sizes(num_envs, precision, &sb, &kb);
   if (rc) return rc;
@@ -132,6 +150,7 @@ extern "C" int srl_apex_actor_create(int A, int num_envs, int precision, uint64_
   X->key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   for (int i = 0; i < 8; ++i) X->w8[i] = params + off[i];
   X->Wq = params + off[8]; X->bq = params + off[9];
+  X->bqa = dueling ? params + off[11] : nullptr;
   rc = srl_encoder_create(precision, &X->enc);
   if (rc) return undo(rc);
   WsRow t[ACTOR_ROWS];
@@ -163,7 +182,8 @@ extern "C" int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const
   const cudaStream_t st = (cudaStream_t)stream;
   rc = actor_forward(X, obs, E, X->core, st);
   if (rc) return rc;
-  apex_act_kernel<<<(E + 3) / 4, 128, 0, st>>>(X->core, X->Wq, X->bq, E, X->A, epsilons, X->key, X->draws, actions);
+  if (X->bqa) apex_act_kernel<true><<<(E + 3) / 4, 128, 0, st>>>(X->core, X->Wq, X->bq, E, X->A, epsilons, X->key, X->draws, actions, X->bqa);
+  else apex_act_kernel<false><<<(E + 3) / 4, 128, 0, st>>>(X->core, X->Wq, X->bq, E, X->A, epsilons, X->key, X->draws, actions, nullptr);
   CU(cudaGetLastError(), "apex_act_kernel");
   return 0;
 }
@@ -179,7 +199,7 @@ extern "C" int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, 
     const int f = n - f0 < X->E ? n - f0 : X->E;
     rc = actor_forward(X, obs + (size_t)f0 * ACTOR_OBS_BYTES, f, X->core, st);
     if (rc) return rc;
-    CU(launch_dqn_q_values(X->core, X->Wq, X->bq, f, X->A, q_out + (size_t)f0 * X->A, st), "dqn_q_values");
+    CU(launch_dqn_q_values(X->core, X->Wq, X->bq, X->bqa, f, X->A, q_out + (size_t)f0 * X->A, st), "dqn_q_values");
   }
   return 0;
 }
@@ -194,7 +214,12 @@ int apex_actor_priorities(srl_apex_actor* X, const uint8_t* s, const uint8_t* s_
   int rc = actor_forward(X, s, E, X->core, st);
   if (!rc) rc = actor_forward(X, s_next, E, core_n, st);
   if (rc) return rc;
-  apex_priority_kernel<<<(E + 3) / 4, 128, 0, st>>>(X->core, core_n, X->Wq, X->bq, E, X->A, action, reward, done, ptr, M, gamma_n, eps, X->prio);
+  if (X->bqa)
+    apex_priority_kernel<true><<<(E + 3) / 4, 128, 0, st>>>(X->core, core_n, X->Wq, X->bq, E, X->A, action, reward, done, ptr, M, gamma_n, eps,
+                                                             X->prio, X->bqa);
+  else
+    apex_priority_kernel<false><<<(E + 3) / 4, 128, 0, st>>>(X->core, core_n, X->Wq, X->bq, E, X->A, action, reward, done, ptr, M, gamma_n, eps,
+                                                              X->prio, nullptr);
   CU(cudaGetLastError(), "apex_priority_kernel");
   *prio = X->prio;
   return 0;

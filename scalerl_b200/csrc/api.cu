@@ -894,12 +894,19 @@ extern "C" int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int fr
 // Ape-X learner step: three encoder forwards on the context's blocks, the Q-learning tail (dqn.cu), the encoder backward over s,
 // clip + Adam, and the priorities into the sampler's trees
 // ------------------------------------------------------------------------------------------------
-// state_dict order {conv1.w, conv1.b, conv2.w, conv2.b, conv3.w, conv3.b, fc.w, fc.b, q.w, q.b}; in memory fc.weight last
-static int64_t apex_layout(int A, int64_t* off, int64_t* cnt) {
-  const int64_t counts[10] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, (int64_t)A * 512, A};
-  const int order[10] = {0, 1, 2, 3, 4, 5, 7, 8, 9, 6};
+// state_dict order {conv1.w, conv1.b, conv2.w, conv2.b, conv3.w, conv3.b, fc.w, fc.b, q.w, q.b}; in memory fc.weight last.
+// dueling: {..., fc.b, value.w [1,512], value.b [1], advantage.w [A,512], advantage.b [A]}; in memory value.weight directly before
+// advantage.weight (one [(A + 1)][512] head block for the kernels) and value.bias before advantage.bias
+static int64_t apex_layout(int A, int dueling, int64_t* off, int64_t* cnt) {
+  const int64_t plain[10] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, (int64_t)A * 512, A};
+  const int64_t duel[12] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, 512, 1, (int64_t)A * 512, A};
+  const int plain_order[10] = {0, 1, 2, 3, 4, 5, 7, 8, 9, 6};
+  const int duel_order[12] = {0, 1, 2, 3, 4, 5, 7, 8, 10, 9, 11, 6};
+  const int64_t* counts = dueling ? duel : plain;
+  const int* order = dueling ? duel_order : plain_order;
+  const int n = dueling ? 12 : 10;
   int64_t o = 0;
-  for (int k = 0; k < 10; ++k) {
+  for (int k = 0; k < n; ++k) {
     const int i = order[k];
     if (off) off[i] = o;
     if (cnt) cnt[i] = counts[i];
@@ -907,7 +914,12 @@ static int64_t apex_layout(int A, int64_t* off, int64_t* cnt) {
   }
   return o;
 }
-extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) { return apex_layout(A, offsets10, counts10); }
+extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) { return apex_layout(A, 0, offsets10, counts10); }
+extern "C" int64_t srl_apex_param_layout_ex(int A, int dueling, int64_t* offsets12, int64_t* counts12) {
+  REQ(A >= 1 && A <= 31, "apex_param_layout: A=%d must be in [1,31]", A);
+  REQ(dueling == 0 || dueling == 1, "apex_param_layout: dueling=%d must be 0 or 1", dueling);
+  return apex_layout(A, dueling, offsets12, counts12);
+}
 
 struct srl_apex_learner {
   srl_apex_config_t cfg;
@@ -915,7 +927,8 @@ struct srl_apex_learner {
   int64_t nparams;
   const float *w8[8], *t8[8];     // the encoder tensors of the online and target parameters
   float* g8[8];
-  float *Wq, *bq, *Wt, *bt, *gWq, *gbq;
+  float *Wq, *bq, *Wt, *bt, *gWq, *gbq;   // dueling: the [(A + 1)][512] head block and value.bias (of params / target / grads)
+  float *bqa, *bta, *gbqa;              // dueling: advantage.bias; NULL for the plain head
   srl_encoder_t *E, *Eq;          // the step's encoder context, and the q-value forwards' own (lanes, events)
   char *saved_s, *saved_n, *enc_scratch;   // encoder blocks: the forward over s (read by the backward), the forwards over s'
   char *saved_q, *scratch_q;      // the q-value forwards' blocks: they may run on another stream than the step
@@ -956,7 +969,7 @@ static int apex_rows(srl_apex_learner* L, const int64_t* b4, WsRow* t) {
   t[n++] = ws_row("step", 4, &L->dstep);
   t[n++] = ws_row(nullptr, B, &L->dq);
   t[n++] = ws_row(nullptr, 4 + dqn_tail_blocks((int)B), &L->tail_scratch);
-  t[n++] = ws_row(nullptr, HEAD_GROUPS * A * 513, &L->head_part);
+  t[n++] = ws_row(nullptr, HEAD_GROUPS * (A + L->cfg.dueling) * 513, &L->head_part);
   t[n++] = ws_row(nullptr, 4, &L->coef);
   t[n++] = ws_row(nullptr, 2048, &L->opt_scratch);
   t[n++] = ws_row(nullptr, QC, &L->zero_reward);     // the reward / action columns of the q-value forwards (the Q head reads h only)
@@ -977,6 +990,7 @@ static int check_apex_cfg(const srl_apex_config_t* c) {
   REQ(c->adam_beta1 >= 0.f && c->adam_beta1 < 1.f && c->adam_beta2 >= 0.f && c->adam_beta2 < 1.f, "apex_learner: Adam betas must be in [0, 1)");
   REQ(std::isfinite(c->adam_eps) && c->adam_eps >= 0.f, "apex_learner: adam_eps=%g must be finite and >= 0", (double)c->adam_eps);
   REQ(std::isfinite(c->priority_eps) && c->priority_eps >= 0.f, "apex_learner: priority_eps=%g must be finite and >= 0", (double)c->priority_eps);
+  REQ(c->dueling == 0 || c->dueling == 1, "apex_learner: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", (int)c->dueling);
   return 0;
 }
 
@@ -987,8 +1001,8 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   REQ(params && grads && exp_avg && exp_avg_sq && target_params && out, "apex_learner_create: NULL argument");
   REQ(!misaligned(params, 16) && !misaligned(grads, 16) && !misaligned(exp_avg, 16) && !misaligned(exp_avg_sq, 16) &&
       !misaligned(target_params, 16), "apex_learner_create: flat buffers must be 16-byte aligned");
-  int64_t off[10];
-  const int64_t np = apex_layout(cfg->A, off, nullptr);
+  int64_t off[12];
+  const int64_t np = apex_layout(cfg->A, cfg->dueling, off, nullptr);
   const Span s[5] = {{params, np * 4, true, "params"}, {grads, np * 4, true, "grads"}, {exp_avg, np * 4, true, "exp_avg"},
                      {exp_avg_sq, np * 4, true, "exp_avg_sq"}, {target_params, np * 4, true, "target_params"}};
   rc = check_spans(s, 5, "apex_learner_create");
@@ -1000,6 +1014,7 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   for (int i = 0; i < 8; ++i) { L->w8[i] = params + off[i]; L->t8[i] = target_params + off[i]; L->g8[i] = grads + off[i]; }
   L->Wq = params + off[8]; L->bq = params + off[9]; L->Wt = target_params + off[8]; L->bt = target_params + off[9];
   L->gWq = grads + off[8]; L->gbq = grads + off[9];
+  if (cfg->dueling) { L->bqa = params + off[11]; L->bta = target_params + off[11]; L->gbqa = grads + off[11]; }
   rc = srl_encoder_create(cfg->precision, &L->E);
   if (!rc) rc = srl_encoder_create(cfg->precision, &L->Eq);
   if (rc) return undo(rc);
@@ -1047,8 +1062,9 @@ extern "C" int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, 
   t.action = action; t.reward = reward; t.done = done; t.weight = weights;
   t.B = B; t.A = c.A; t.gamma = c.gamma; t.two_over_B = 2.f / (float)B; t.priority_eps = c.priority_eps;
   t.q = L->q; t.y = L->y; t.dq = L->dq; t.dcore = L->dcore; t.loss = L->loss; t.scratch = L->tail_scratch; t.prio = L->prio;
+  t.bqa = L->bqa; t.bta = L->bta; t.dueling = c.dueling;
   CU(launch_dqn_tail(t, st), "dqn_tail");
-  CU(launch_dqn_wgrad(L->dq, action, L->core_s, B, c.A, L->head_part, L->gWq, L->gbq, st), "dqn_wgrad");
+  CU(launch_dqn_wgrad(L->dq, action, L->core_s, B, c.A, L->head_part, L->gWq, L->gbq, L->gbqa, st), "dqn_wgrad");
   rc = srl_encoder_backward(L->E, L->dcore, B, 1, L->saved_s, L->enc_scratch, L->g8, stream);
   if (rc) return rc;
   const OptStep o = {1, L->params, L->grads, L->m, L->v, L->nparams, c.max_grad_norm, L->coef, L->opt_scratch, c.learning_rate,
@@ -1093,7 +1109,7 @@ extern "C" int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* o
     rc = srl_encoder_forward(L->Eq, obs + (size_t)f0 * 28224, L->zero_reward, L->zero_action, f, 1, L->w8, L->saved_q, L->scratch_q,
                              L->core_q, stream);
     if (rc) return rc;
-    CU(launch_dqn_q_values(L->core_q, L->Wq, L->bq, f, A, q_out + (size_t)f0 * A, (cudaStream_t)stream), "dqn_q_values");
+    CU(launch_dqn_q_values(L->core_q, L->Wq, L->bq, L->bqa, f, A, q_out + (size_t)f0 * A, (cudaStream_t)stream), "dqn_q_values");
   }
   return 0;
 }

@@ -6,7 +6,10 @@
 //   dqn_wgrad_reduce_kernel   heads.cu's head_wgrad kernels), so every run computes the same bits
 //   dqn_q_values_kernel       the forward-only Q head (predict / get_action)
 //   apex_soft_update_kernel   theta_t <- tau theta + (1 - tau) theta_t (dqn_agent.py:185-190, utils/model_utils.py:29-32)
-// The Q head arithmetic (q_dot, q_max, the target and the priority) is dqn_head.cuh's, shared with the Ape-X actor.
+// The Q head arithmetic (q_dot, q_max, dueling_q, q_row_max, the target and the priority) is dqn_head.cuh's, shared with the Ape-X actor.
+// The tail, the head gradients and the Q values are templates on the head: DUELING = the dueling head V + Adv - mean(Adv) on the shared
+// fc output (Wang et al. 2016, eq. 9), whose A + 1 rows (the value row first) lie as one [(A + 1)][512] block; the plain instantiations
+// are the single-head kernels unchanged.
 #include "common.cuh"
 #include "dqn_head.cuh"
 #include "kernels.h"
@@ -14,6 +17,8 @@
 namespace srl {
 
 // One warp per transition, 4 per block.  scratch: [0] the ticket, [4 + k] block k's partial of sum_n w_n (q_n - y_n)^2.
+// DUELING: the dueling head (dqn_head.cuh's dueling_q) in place of q = Linear(512, A); the target, loss and priority are the same.
+template <bool DUELING>
 __global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = blockIdx.x * 4 + warp;
@@ -21,15 +26,28 @@ __global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
   if (n < t.B) {
     const int act = ld_action(t.action + n, t.A);
     const float* hs = t.core_s + (size_t)n * ENC_CORE;
-    const float q = q_dot(hs, t.Wq + (size_t)act * 512, lane) + __ldg(t.bq + act);
-    const float* hn = t.core_nt + (size_t)n * ENC_CORE;
-    int a_star;
-    float nx;
-    if (t.core_n) {     // double DQN: the online network picks a*, the target network values it (dqn_agent.py:155-160)
-      q_max(t.core_n + (size_t)n * ENC_CORE, t.Wq, t.bq, t.A, lane, &a_star);
-      nx = q_dot(hn, t.Wt + (size_t)a_star * 512, lane) + __ldg(t.bt + a_star);
-    } else {            // max_a Q_target(s', a) (apex/worker.py:149, dqn_agent.py:162-163)
-      nx = q_max(hn, t.Wt, t.bt, t.A, lane, &a_star);
+    float q, nx;
+    float wsum[16];     // dueling: the advantage rows' column sums (lane + 32 i)
+    if constexpr (!DUELING) {
+      q = q_dot(hs, t.Wq + (size_t)act * 512, lane) + __ldg(t.bq + act);
+      const float* hn = t.core_nt + (size_t)n * ENC_CORE;
+      int a_star;
+      if (t.core_n) {     // double DQN: the online network picks a*, the target network values it (dqn_agent.py:155-160)
+        q_max(t.core_n + (size_t)n * ENC_CORE, t.Wq, t.bq, t.A, lane, &a_star);
+        nx = q_dot(hn, t.Wt + (size_t)a_star * 512, lane) + __ldg(t.bt + a_star);
+      } else {            // max_a Q_target(s', a) (apex/worker.py:149, dqn_agent.py:162-163)
+        nx = q_max(hn, t.Wt, t.bt, t.A, lane, &a_star);
+      }
+    } else {            // the same statements on the dueling Q rows (lane a holds Q_a)
+      q = __shfl_sync(0xffffffffu, dueling_q<true>(hs, t.Wq, t.bq, t.bqa, t.A, lane, wsum), act);
+      const float qt = dueling_q<false>(t.core_nt + (size_t)n * ENC_CORE, t.Wt, t.bt, t.bta, t.A, lane, nullptr);
+      int a_star;
+      if (t.core_n) {
+        q_row_max(dueling_q<false>(t.core_n + (size_t)n * ENC_CORE, t.Wq, t.bq, t.bqa, t.A, lane, nullptr), t.A, &a_star);
+        nx = __shfl_sync(0xffffffffu, qt, a_star);
+      } else {
+        nx = q_row_max(qt, t.A, &a_star);
+      }
     }
     const float y = td_target(__ldg(t.reward + n), t.gamma, nx, t.done[n] != 0);
     const float w = t.weight ? __ldg(t.weight + n) : 1.f;
@@ -41,9 +59,20 @@ __global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
       t.q[n] = q; t.y[n] = y; t.dq[n] = dq;
       t.prio[n] = td_priority(delta, t.priority_eps);
     }
-    const float* wa = t.Wq + (size_t)act * 512;
-    float* dc = t.dcore + (size_t)n * ENC_CORE;
-    for (int j = lane; j < ENC_CORE; j += 32) dc[j] = j < 512 ? dq * __ldg(wa + j) : 0.f;
+    if constexpr (!DUELING) {
+      const float* wa = t.Wq + (size_t)act * 512;
+      float* dc = t.dcore + (size_t)n * ENC_CORE;
+      for (int j = lane; j < ENC_CORE; j += 32) dc[j] = j < 512 ? dq * __ldg(wa + j) : 0.f;
+    } else {            // dL/dV = dq, dL/dAdv_a = dq (1[a = act] - 1/A): dL/dh = dq (w_v + W_adv[act] - mean_a W_adv[a])
+      const float* wa = t.Wq + (size_t)(act + 1) * 512;
+      float* dc = t.dcore + (size_t)n * ENC_CORE;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const int j = lane + 32 * i;
+        dc[j] = dq * __fsub_rn(__fadd_rn(__ldg(t.Wq + j), __ldg(wa + j)), __fdiv_rn(wsum[i], (float)t.A));
+      }
+      if (lane < ENC_CORE - 512) dc[512 + lane] = 0.f;
+    }
   }
   // block partial: the warps' losses in warp order, then the ticket; the last block adds the partials in block order
   __shared__ float red[4];
@@ -68,12 +97,15 @@ __global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
 }
 
 // Q head weight/bias gradients: thread = one column j of h (j == 512 is the bias "ones" column), blockIdx.y = a group of consecutive
-// slabs of transitions.  Row a of a slab carries dq only for the transition's action.  Each group writes part[group][a][j].
+// slabs of transitions.  Plain head: row a of a slab carries dq only for the transition's action.  Dueling head (A + 1 rows, the
+// value row first): row 0 carries dq, row 1 + a carries dq (1[a = act] - 1/A).  Each group writes part[group][row][j].
 constexpr int DQN_SLAB = 16, DQN_MAX_A = 32;
+template <bool DUELING>
 __global__ void __launch_bounds__(128) dqn_wgrad_kernel(const float* __restrict__ dq, const int64_t* __restrict__ action,
                                                         const float* __restrict__ core, int N, int A, int slabs_per_group,
                                                         float* __restrict__ part) {
   __shared__ float sd[DQN_SLAB][DQN_MAX_A];
+  const int R = DUELING ? A + 1 : A;          // head rows
   const int j = blockIdx.x * 128 + threadIdx.x;
   const int nslab = (N + DQN_SLAB - 1) / DQN_SLAB;
   const int s0 = blockIdx.y * slabs_per_group, s1 = min(nslab, s0 + slabs_per_group);
@@ -83,9 +115,18 @@ __global__ void __launch_bounds__(128) dqn_wgrad_kernel(const float* __restrict_
   for (int sl = s0; sl < s1; ++sl) {
     const int n0 = sl * DQN_SLAB, cnt = min(DQN_SLAB, N - n0);
     __syncthreads();                 // the previous slab's shared rows have been read
-    for (int i = threadIdx.x; i < DQN_SLAB * A; i += 128) {     // rows past the ragged end are zero
-      const int r = i / A, a = i - r * A;
-      sd[r][a] = (r < cnt && ld_action(action + n0 + r, A) == a) ? __ldg(dq + n0 + r) : 0.f;
+    for (int i = threadIdx.x; i < DQN_SLAB * R; i += 128) {     // rows past the ragged end are zero
+      const int r = i / R, a = i - r * R;
+      if constexpr (!DUELING) {
+        sd[r][a] = (r < cnt && ld_action(action + n0 + r, A) == a) ? __ldg(dq + n0 + r) : 0.f;
+      } else {
+        float g = 0.f;
+        if (r < cnt) {
+          const float d = __ldg(dq + n0 + r);
+          g = a == 0 ? d : d * ((ld_action(action + n0 + r, A) == a - 1 ? 1.f : 0.f) - __fdiv_rn(1.f, (float)A));
+        }
+        sd[r][a] = g;
+      }
     }
     __syncthreads();
     if (j > 512) continue;
@@ -94,7 +135,7 @@ __global__ void __launch_bounds__(128) dqn_wgrad_kernel(const float* __restrict_
     for (int r = 0; r < DQN_SLAB; ++r) c[r] = r < cnt ? (j < 512 ? __ldg(core + (size_t)(n0 + r) * ENC_CORE + j) : 1.f) : 0.f;
 #pragma unroll
     for (int a = 0; a < DQN_MAX_A; ++a) {
-      if (a >= A) break;
+      if (a >= R) break;
 #pragma unroll
       for (int r = 0; r < DQN_SLAB; ++r) acc[a] = fmaf(sd[r][a], c[r], acc[a]);
     }
@@ -102,27 +143,36 @@ __global__ void __launch_bounds__(128) dqn_wgrad_kernel(const float* __restrict_
   if (j > 512) return;
 #pragma unroll
   for (int a = 0; a < DQN_MAX_A; ++a)
-    if (a < A) part[((size_t)blockIdx.y * A + a) * 513 + j] = acc[a];
+    if (a < R) part[((size_t)blockIdx.y * R + a) * 513 + j] = acc[a];
 }
-// sums the groups' partials in group order into the Q head gradients (stored, not accumulated)
+// sums the groups' partials in group order into the Q head gradients (stored, not accumulated); dueling: row 0's bias -> gb[0], row
+// 1 + a's -> gba[a]
+template <bool DUELING>
 __global__ void __launch_bounds__(256) dqn_wgrad_reduce_kernel(const float* __restrict__ part, int groups, int A, float* __restrict__ gW,
-                                                               float* __restrict__ gb) {
-  const int n = A * 513, i = blockIdx.x * blockDim.x + threadIdx.x;
+                                                               float* __restrict__ gb, float* __restrict__ gba) {
+  const int n = (DUELING ? A + 1 : A) * 513, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float s = 0.f;
   for (int g = 0; g < groups; ++g) s += __ldg(part + (size_t)g * n + i);
   const int a = i / 513, j = i - a * 513;
-  if (j < 512) gW[(size_t)a * 512 + j] = s; else gb[a] = s;
+  if (j < 512) gW[(size_t)a * 512 + j] = s; else if (!DUELING || a == 0) gb[a] = s; else gba[a - 1] = s;
 }
 
-// q_out[n][a] = h[n] . W[a] + b[a]: the tail's head arithmetic without the loss (one warp per frame)
+// q_out[n][a] = Q(h[n])[a]: the tail's head arithmetic without the loss (one warp per frame).  Plain: h[n] . W[a] + b[a]; DUELING:
+// dueling_q with the value bias b and the advantage biases ba
+template <bool DUELING>
 __global__ void __launch_bounds__(128) dqn_q_values_kernel(const float* __restrict__ core, const float* __restrict__ W, const float* __restrict__ b,
-                                                           int N, int A, float* __restrict__ q_out) {
+                                                           int N, int A, float* __restrict__ q_out, const float* __restrict__ ba) {
   const int lane = threadIdx.x & 31, n = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (n >= N) return;
-  for (int a = 0; a < A; ++a) {
-    const float v = q_dot(core + (size_t)n * ENC_CORE, W + (size_t)a * 512, lane) + __ldg(b + a);
-    if (lane == 0) q_out[(size_t)n * A + a] = v;
+  if constexpr (DUELING) {
+    const float q = dueling_q<false>(core + (size_t)n * ENC_CORE, W, b, ba, A, lane, nullptr);
+    if (lane < A) q_out[(size_t)n * A + lane] = q;
+  } else {
+    for (int a = 0; a < A; ++a) {
+      const float v = q_dot(core + (size_t)n * ENC_CORE, W + (size_t)a * 512, lane) + __ldg(b + a);
+      if (lane == 0) q_out[(size_t)n * A + a] = v;
+    }
   }
 }
 
@@ -134,18 +184,27 @@ __global__ void __launch_bounds__(256) apex_soft_update_kernel(const float* __re
 }
 
 cudaError_t launch_dqn_tail(const DqnTail& t, cudaStream_t st) {
-  dqn_tail_kernel<<<dqn_tail_blocks(t.B), 128, 0, st>>>(t);
+  if (t.dueling) dqn_tail_kernel<true><<<dqn_tail_blocks(t.B), 128, 0, st>>>(t);
+  else dqn_tail_kernel<false><<<dqn_tail_blocks(t.B), 128, 0, st>>>(t);
   return cudaGetLastError();
 }
 cudaError_t launch_dqn_wgrad(const float* dq, const int64_t* action, const float* core, int N, int A, float* part, float* gW, float* gb,
-                             cudaStream_t st) {
+                             float* gba, cudaStream_t st) {
   const int nslab = (N + DQN_SLAB - 1) / DQN_SLAB, spg = (nslab + HEAD_GROUPS - 1) / HEAD_GROUPS, groups = (nslab + spg - 1) / spg;
-  dqn_wgrad_kernel<<<dim3((513 + 127) / 128, groups), 128, 0, st>>>(dq, action, core, N, A, spg, part);
-  dqn_wgrad_reduce_kernel<<<(A * 513 + 255) / 256, 256, 0, st>>>(part, groups, A, gW, gb);
+  const dim3 grid((513 + 127) / 128, groups);
+  if (gba) {
+    dqn_wgrad_kernel<true><<<grid, 128, 0, st>>>(dq, action, core, N, A, spg, part);
+    dqn_wgrad_reduce_kernel<true><<<((A + 1) * 513 + 255) / 256, 256, 0, st>>>(part, groups, A, gW, gb, gba);
+  } else {
+    dqn_wgrad_kernel<false><<<grid, 128, 0, st>>>(dq, action, core, N, A, spg, part);
+    dqn_wgrad_reduce_kernel<false><<<(A * 513 + 255) / 256, 256, 0, st>>>(part, groups, A, gW, gb, nullptr);
+  }
   return cudaGetLastError();
 }
-cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* b, int N, int A, float* q_out, cudaStream_t st) {
-  dqn_q_values_kernel<<<(N + 3) / 4, 128, 0, st>>>(core, W, b, N, A, q_out);
+cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* b, const float* ba, int N, int A, float* q_out,
+                                cudaStream_t st) {
+  if (ba) dqn_q_values_kernel<true><<<(N + 3) / 4, 128, 0, st>>>(core, W, b, N, A, q_out, ba);
+  else dqn_q_values_kernel<false><<<(N + 3) / 4, 128, 0, st>>>(core, W, b, N, A, q_out, nullptr);
   return cudaGetLastError();
 }
 cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st) {

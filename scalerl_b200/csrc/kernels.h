@@ -222,6 +222,8 @@ constexpr int ENC_CORE = 514;
 // one batch of B transitions: core rows of the online forward over s, the online forward over s' (null: plain max, no double DQN) and
 // the target forward over s'; the Q heads [A][512] + [A]; the batch columns; outputs q, y, dq f32 [B], priorities f64 [B], dcore
 // [B][ENC_CORE] and loss f32 [1].  scratch: 4 + dqn_tail_blocks(B) floats, zero before the first launch (re-armed by the kernel).
+// dueling: W* = [(A + 1)][512] (value row, then the advantage rows), b* = the value bias [1], b*a = the advantage biases [A]
+// (dqn_head.cuh's dueling_q); the plain head leaves bqa / bta unused.
 struct DqnTail {
   const float *core_s, *core_n, *core_nt;
   const float *Wq, *bq, *Wt, *bt;
@@ -230,13 +232,19 @@ struct DqnTail {
   float gamma, two_over_B, priority_eps;
   float *q, *y, *dq, *dcore, *loss, *scratch;
   double* prio;
+  const float *bqa, *bta;
+  int dueling;
 };
 inline int dqn_tail_blocks(int B) { return (B + 3) / 4; }
 cudaError_t launch_dqn_tail(const DqnTail& t, cudaStream_t st);
-// the Q head gradients gW [A][512], gb [A] (stored) from dq and the actions over the core rows; part: HEAD_GROUPS * A * 513 floats
+// the Q head gradients (stored) from dq and the actions over the core rows.  Plain head (gba NULL): gW [A][512], gb [A]; part:
+// HEAD_GROUPS * A * 513 floats.  Dueling head (gba set): gW [(A + 1)][512] (value row first), gb [1] the value bias, gba [A] the
+// advantage biases; part: HEAD_GROUPS * (A + 1) * 513 floats.
 cudaError_t launch_dqn_wgrad(const float* dq, const int64_t* action, const float* core, int N, int A, float* part, float* gW, float* gb,
-                             cudaStream_t st);
-cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* b, int N, int A, float* q_out, cudaStream_t st);
+                             float* gba, cudaStream_t st);
+// q_out [N][A] = Q(h) of the plain head (ba NULL) or of the dueling head (W [(A + 1)][512], b the value bias, ba the advantage biases)
+cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* b, const float* ba, int N, int A, float* q_out,
+                                cudaStream_t st);
 cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
 
 }  // namespace srl

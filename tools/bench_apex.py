@@ -3,7 +3,10 @@ statements (apex/worker.py:148-161) on torch/cuDNN with AtariQNet, eager and cap
 priorities into a GpuPrioritizedSampler of its own.  Rounds alternate between the variants; the median and range over rounds are
 printed with the card's name and power limit, one JSON line per configuration.
 
-    python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18]
+With --dueling the learner runs the dueling head (ApexHParams(dueling_dqn=True)) beside the plain one, alternated in the same rounds,
+and the torch statements use AtariQNet(A, dueling=True).
+
+    python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18] [--dueling]
 """
 import argparse
 import json
@@ -49,9 +52,9 @@ class TorchStep:
     """the reference's statements on torch/cuDNN (the priorities stay on the device and go into the GPU sampler).  The object owns
     every tensor the step reads or writes, so a captured replay of it stays valid as long as the object lives."""
 
-    def __init__(self, B, A, exp, w, idxs, gamma=0.99):
-        sd = default_q_state_dict(A)
-        self.model, self.target = AtariQNet(A).cuda(), AtariQNet(A).cuda()
+    def __init__(self, B, A, exp, w, idxs, gamma=0.99, dueling=False):
+        sd = default_q_state_dict(A, dueling=dueling)
+        self.model, self.target = AtariQNet(A, dueling=dueling).cuda(), AtariQNet(A, dueling=dueling).cuda()
         self.model.load_state_dict(sd)
         self.target.load_state_dict(sd)
         self.opt = torch.optim.Adam(self.model.parameters(), lr=1e-3, capturable=True)
@@ -107,6 +110,7 @@ def main():
     ap.add_argument('--rounds', type=int, default=5)
     ap.add_argument('--steps', type=int, default=50)
     ap.add_argument('--configs', default='32x6,32x18,512x6,512x18')
+    ap.add_argument('--dueling', action='store_true', help='add the dueling learner and run the torch statements on the dueling net')
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('bench_apex.py measures on a CUDA device; none is present')
@@ -115,9 +119,14 @@ def main():
         B, A = (int(x) for x in cfg.split('x'))
         exp, w, idxs = batch(B, A)
         L, S = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A)), sampler()
-        variants = {'b200_captured': lambda: L.learn(exp, weights=w, idxs=idxs, sampler=S, sync_stats=False),
-                    'torch_eager': TorchStep(B, A, exp, w, idxs),
-                    'torch_captured': Captured(TorchStep(B, A, exp, w, idxs))}
+        variants = {'b200_captured': lambda: L.learn(exp, weights=w, idxs=idxs, sampler=S, sync_stats=False)}
+        learners = [L]
+        if a.dueling:
+            LD, SD = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, dueling_dqn=True)), sampler()
+            learners.append(LD)
+            variants['b200_dueling_captured'] = lambda: LD.learn(exp, weights=w, idxs=idxs, sampler=SD, sync_stats=False)
+        variants['torch_eager'] = TorchStep(B, A, exp, w, idxs, dueling=a.dueling)
+        variants['torch_captured'] = Captured(TorchStep(B, A, exp, w, idxs, dueling=a.dueling))
         for fn in variants.values():           # warm-up: the learner's first call runs eagerly, the second captures
             for _ in range(3):
                 fn()
@@ -125,15 +134,17 @@ def main():
         for _ in range(a.rounds):
             for k, fn in variants.items():
                 rates[k].append(timed(fn, a.steps))
-        out = {'card': name, 'B': B, 'A': A, 'precision': 'bf16', 'rounds': a.rounds, 'steps_per_round': a.steps}
+        out = {'card': name, 'B': B, 'A': A, 'precision': 'bf16', 'torch_net': 'dueling' if a.dueling else 'plain', 'rounds': a.rounds,
+               'steps_per_round': a.steps}
         for k, r in rates.items():
             r = sorted(r)
             out[k] = {'steps_per_s_median': r[len(r) // 2], 'steps_per_s_range': [r[0], r[-1]],
                       'transitions_per_s_median': r[len(r) // 2] * B}
         print(json.dumps(out), flush=True)
         del variants
-        L.release_graphs()
-        L.close()
+        for x in learners:
+            x.release_graphs()
+            x.close()
 
 
 if __name__ == '__main__':
