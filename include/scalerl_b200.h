@@ -366,13 +366,16 @@ int srl_replay_gather(srl_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* 
  * Nature DQN: AtariNet's conv1..3 + fc + ReLU (atari_model.py:30-47,91-101) followed by q = Linear(512, A), A in [1, 31], or, with
  * `dueling`, the dueling head of Wang et al. 2016 (eq. 9) on the same 512 fc features: V = value(h) = Linear(512, 1), Adv =
  * advantage(h) = Linear(512, A), Q = V + Adv - mean_a Adv.  Both heads read the shared fc output (the paper's Atari network has two
- * separate 512-unit fc streams): the encoder is the same for both.
+ * separate 512-unit fc streams): the encoder is the same for both.  With `num_atoms` = K > 0 the head is categorical (C51,
+ * Bellemare et al. 2017): q = Linear(512, A K), row a K + k atom k of action a, p(s)[a] = softmax over the action's K logits, Q(s, a) =
+ * sum_k z_k p_k on the support z_k = v_min + k dz, dz = (v_max - v_min) / (K - 1) rounded once to fp32.
  * srl_replay_* stores and folds n-step transitions (pass gamma^n for them, and srl_replay_per as `per`); srl_apex_actor_* acts and computes
  * their initial priorities.
  * Parameters in state_dict order {conv1.weight, conv1.bias, conv2.weight, conv2.bias, conv3.weight, conv3.bias, fc.weight, fc.bias,
  * q.weight [A,512], q.bias [A]}; srl_apex_param_layout returns the flat buffer's floats and each tensor's offset / count (int64[10]).
  * The dueling head's state_dict order is {conv1..3, fc, value.weight [1,512], value.bias [1], advantage.weight [A,512],
  * advantage.bias [A]} (int64[12], srl_apex_param_layout_ex); value.weight lies directly before advantage.weight.
+ * The categorical head keeps the 10 plain names with q.weight [A K, 512] and q.bias [A K] (srl_apex_param_layout_cat).
  * In memory the small tensors come first and fc.weight last; segments are padded to 4 floats.  Params, grads, both Adam states
  * and the target copy share the layout. */
 typedef struct srl_apex_learner srl_apex_learner_t;
@@ -386,11 +389,16 @@ typedef struct srl_apex_config {
   float learning_rate, adam_beta1, adam_beta2, adam_eps;   /* torch.optim.Adam (apex/worker.py:132)            */
   float priority_eps;        /* priority = |q - y| + priority_eps (in double), >= 0                           */
   int32_t dueling;           /* 0: q = Linear(512, A); 1: the dueling head Q = V + Adv - mean(Adv)             */
+  int32_t num_atoms;         /* 0: a scalar Q head; K in [2, 64]: the categorical head (not with dueling = 1)  */
+  float v_min, v_max;        /* the categorical support [v_min, v_max], finite, v_min < v_max (read when num_atoms > 0) */
 } srl_apex_config_t;
 int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10);
 /* the layout of either head: dueling 0 -> 10 tensors (srl_apex_param_layout's), 1 -> 12; -1 with srl_last_error set for A outside
  * [1, 31] or dueling outside {0, 1} */
 int64_t srl_apex_param_layout_ex(int A, int dueling, int64_t* offsets12, int64_t* counts12);
+/* the 10-tensor layout with q.weight [A num_atoms, 512] and q.bias [A num_atoms] (num_atoms 0: srl_apex_param_layout's); -1 with
+ * srl_last_error set for A outside [1, 31] or num_atoms outside {0} and [2, 64] */
+int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offsets10, int64_t* counts10);
 /* params / grads / exp_avg / exp_avg_sq / target_params: caller-owned flat f32 device buffers of srl_apex_param_layout floats,
  * 16-byte aligned and disjoint.  The context owns the encoder's blocks (one saved block for the forward over s, one for the
  * forwards over s', their scratch) and the tail's buffers.  Synchronous. */
@@ -402,6 +410,10 @@ int srl_apex_learner_destroy(srl_apex_learner_t* L);
  *   q = Q(s)[a];  y = r + gamma Q_t(s')[a*] (1 - d), a* = argmax Q_t(s') or, double_dqn, argmax Q(s')   (worker.py:148-150)
  *   loss = mean(w (q - y)^2)                                                                             (worker.py:156-157)
  *   priority = |q - y| + priority_eps from the pre-update weights -> the sampler's trees, last occurrence of an idx wins (:152-154)
+ * The categorical head (num_atoms = K > 0) replaces the squared TD error by the distributional update of Bellemare et al. 2017:
+ *   a* as above on the expected Q;  m = the projection of p_t(s')[a*] moved to clamp(r + gamma (1 - d) z_j, v_min, v_max) onto the
+ *   support (Algorithm 1, j ascending);  ce = -sum_k m_k log p(s)[a, k];  loss = mean(w ce);  priority = max(KL(m || p(s)[a]), 0) +
+ *   priority_eps (Hessel et al. 2018).  q holds sum_k z_k p(s)[a, k], y holds sum_k z_k m_k.
  *   clip_grad_norm_(max_grad_norm), torch.optim.Adam step with the step count kept on the device       (dqn_agent.py:172-182)
  * stats_out: f32 [3] device = {loss, gradient norm, clip coefficient} (may be NULL).  No host synchronisation; capturable. */
 int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, const int64_t* action, const float* reward, const uint8_t* next_obs,
@@ -418,7 +430,9 @@ int srl_apex_learner_set_step(srl_apex_learner_t* L, int64_t step, void* stream)
 int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* obs, int n, float* q_out, void* stream);
 /* borrow the step's buffers for tests: "core", "core_next" (double DQN only), "core_next_target" f32 [B,514] (the encoder's core rows;
  * h = columns < 512), "dcore" f32 [B,514], "q", "y" f32 [B], "priorities" f64 [B], "loss" f32 [1], "step" i32 [1] (device step count),
- * and the bf16 activations the forward over s saved, in the learner's layouts (srl_learner_debug_buffer): "a1", "a2", "a3" */
+ * and the bf16 activations the forward over s saved, in the learner's layouts (srl_learner_debug_buffer): "a1", "a2", "a3".
+ * The categorical head adds "logits", "logits_next" (double DQN only), "logits_next_target" and "dlogits" f32 [B,A*K], "m" f32 [B,K]
+ * (the projected targets) and "ce" f32 [B] (the cross-entropies); its "y" is sum_k z_k m_k. */
 int srl_apex_learner_debug_buffer(srl_apex_learner_t* L, const char* name, void** ptr, int64_t* count);
 
 /* ---- Ape-X actor: per-env epsilon-greedy acting and actor-computed initial priorities (apex/worker.py:59-79, apex/memory.py:43-64) --
@@ -432,6 +446,11 @@ int srl_apex_actor_create(int A, int num_envs, int precision, uint64_t seed, con
 /* the same with the head kind: dueling 0 (q = Linear(512, A), srl_apex_actor_create's) or 1 (the dueling head; params in
  * srl_apex_param_layout_ex(A, 1) order) */
 int srl_apex_actor_create_ex(int A, int num_envs, int precision, int dueling, uint64_t seed, const float* params, srl_apex_actor_t** out);
+/* the same with the categorical head: num_atoms in [2, 64] (0: srl_apex_actor_create's plain head), the support [v_min, v_max] as
+ * srl_apex_config_t's; params in srl_apex_param_layout_cat(A, num_atoms) order.  Its Q values are the expectations sum_k z_k p_k and its
+ * priorities max(KL(m || p(s)[a]), 0) + priority_eps with the snapshot as online and target network (srl_apex_learner_step's bits) */
+int srl_apex_actor_create_cat(int A, int num_envs, int precision, int num_atoms, float v_min, float v_max, uint64_t seed, const float* params,
+                              srl_apex_actor_t** out);
 int srl_apex_actor_destroy(srl_apex_actor_t* X);
 /* obs u8 [E,4,84,84], epsilons f32 [E] (device) -> actions i64 [E]: with probability epsilons[e] a uniform action, else the first
  * argmax of Q(obs[e]) (torch.argmax's pick).  The random numbers are Philox4x32-10 keyed by seed, counted by (draw, env); the launch
@@ -439,6 +458,9 @@ int srl_apex_actor_destroy(srl_apex_actor_t* X);
 int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const float* epsilons, int64_t* actions, void* stream);
 /* Q(obs) with the snapshot for n >= 1 frames: obs u8 [n,4,84,84] -> q_out f32 [n,A] */
 int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, int n, float* q_out, void* stream);
+/* borrow the actor's buffers for tests: "core" f32 [2E,514] (rows 0..E-1: the last act or the states of the last prioritized add,
+ * rows E..2E-1: its next states) and, categorical head only, "logits" f32 [2E,A*K] of the same rows */
+int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name, void** ptr, int64_t* count);
 /* srl_replay_add, then, for the E transitions the call completes, their initial priorities computed by `actor` (built for the memory's
  * num_envs) instead of max_priority:  p = |Q(s)[a] - y| + priority_eps,  y = R + fp32(gamma^n_step) (1 - d) max_a Q(s')  with the
  * arithmetic of srl_apex_learner_step's target and priority (the same bits for the same weights).  R, a and d are the fold's; s is the

@@ -102,6 +102,8 @@ _SIGS = {
     'srl_apex_learner_debug_buffer': [_P, C.c_char_p, C.POINTER(_P), C.POINTER(_L)],
     'srl_apex_actor_create': [_I, _I, _I, C.c_uint64, _P, C.POINTER(_P)],
     'srl_apex_actor_create_ex': [_I, _I, _I, _I, C.c_uint64, _P, C.POINTER(_P)],
+    'srl_apex_actor_create_cat': [_I, _I, _I, _I, _F, _F, C.c_uint64, _P, C.POINTER(_P)],
+    'srl_apex_actor_debug_buffer': [_P, C.c_char_p, C.POINTER(_P), C.POINTER(_L)],
     'srl_apex_actor_destroy': [_P],
     'srl_apex_actor_act': [_P] * 5,
     'srl_apex_actor_q_values': [_P, _P, _I, _P, _P],
@@ -135,7 +137,7 @@ def hooks():
     return _hooks
 
 
-EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout', 'srl_apex_param_layout_ex', 'srl_replay_size', 'srl_replay_per'])
+EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout', 'srl_apex_param_layout_ex', 'srl_apex_param_layout_cat', 'srl_replay_size', 'srl_replay_per'])
 
 
 def lib():
@@ -176,6 +178,8 @@ def lib():
         L.srl_apex_param_layout.argtypes = [_I, C.POINTER(_L), C.POINTER(_L)]
         L.srl_apex_param_layout_ex.restype = C.c_int64
         L.srl_apex_param_layout_ex.argtypes = [_I, _I, C.POINTER(_L), C.POINTER(_L)]
+        L.srl_apex_param_layout_cat.restype = C.c_int64
+        L.srl_apex_param_layout_cat.argtypes = [_I, _I, C.POINTER(_L), C.POINTER(_L)]
         L.srl_learner_workspace_bytes.restype = C.c_int64
         L.srl_learner_workspace_bytes.argtypes = [_P]
         _lib = L
@@ -201,17 +205,21 @@ class SrlApexConfig(C.Structure):
     """mirror of srl_apex_config_t"""
     _fields_ = [('B', C.c_int32), ('A', C.c_int32), ('precision', C.c_int32), ('double_dqn', C.c_int32),
                 ('gamma', C.c_float), ('max_grad_norm', C.c_float), ('learning_rate', C.c_float), ('adam_beta1', C.c_float),
-                ('adam_beta2', C.c_float), ('adam_eps', C.c_float), ('priority_eps', C.c_float), ('dueling', C.c_int32)]
+                ('adam_beta2', C.c_float), ('adam_eps', C.c_float), ('priority_eps', C.c_float), ('dueling', C.c_int32),
+                ('num_atoms', C.c_int32), ('v_min', C.c_float), ('v_max', C.c_float)]
 
 
-def apex_param_layout(A, dueling=False):
+def apex_param_layout(A, dueling=False, num_atoms=0):
     """(total floats, offsets, counts) of the Ape-X Q network's flat buffer in state_dict order: 10 tensors, or 12 with the dueling
-    head"""
+    head; num_atoms > 0: the categorical head's 10 (q.weight [A num_atoms, 512], q.bias [A num_atoms])"""
     off = (_L * 12)()
     cnt = (_L * 12)()
-    total = lib().srl_apex_param_layout_ex(int(A), 1 if dueling else 0, off, cnt)
+    if num_atoms:
+        total = lib().srl_apex_param_layout_cat(int(A), int(num_atoms), off, cnt)
+    else:
+        total = lib().srl_apex_param_layout_ex(int(A), 1 if dueling else 0, off, cnt)
     if total < 0:
-        check(-1, 'srl_apex_param_layout_ex')
+        check(-1, 'srl_apex_param_layout')
     n = 12 if dueling else 10
     return int(total), [int(x) for x in off][:n], [int(x) for x in cnt][:n]
 

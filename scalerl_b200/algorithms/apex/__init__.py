@@ -1,6 +1,6 @@
 from .actor import B200ApexActor, apex_epsilons
 from .learner import (APEX_DUELING_PARAM_NAMES, APEX_PARAM_NAMES, ApexHParams, AtariQNet, B200ApexLearner, apex_param_names,
-                      apex_param_shapes, default_q_state_dict)
+                      apex_param_shapes, categorical_support, default_q_state_dict)
 
 __all__ = ['APEX_DUELING_PARAM_NAMES', 'APEX_PARAM_NAMES', 'ApexHParams', 'AtariQNet', 'B200ApexActor', 'B200ApexLearner', 'apex_epsilons',
-           'apex_param_names', 'apex_param_shapes', 'default_q_state_dict']
+           'apex_param_names', 'apex_param_shapes', 'categorical_support', 'default_q_state_dict']

@@ -13,6 +13,8 @@ epsilon, from a parameter snapshot on the device (srl_apex_actor_*, csrc/apex_ac
   * ``sync_from(learner)``: one device copy of the learner's online parameters into the snapshot.
 
 ``dueling_dqn=True`` gives the actor the dueling head of ``ApexHParams(dueling_dqn=True)``; it syncs from dueling learners only.
+``categorical_dqn=True`` (with ``v_min``, ``v_max``, ``num_atoms``) gives it the categorical head of ``ApexHParams(categorical_dqn=True)``:
+it acts on the expected Q and prioritises by the learner's KL divergence, and syncs from learners with the same atoms and support only.
 """
 from __future__ import annotations
 
@@ -25,7 +27,7 @@ import numpy as np
 import torch
 
 from ... import _lib
-from .learner import MAX_FRAMES, apex_param_shapes, default_q_state_dict, flat_views, load_views
+from .learner import MAX_FRAMES, apex_param_shapes, check_categorical, default_q_state_dict, flat_views, load_views
 
 PRECISIONS = {'bf16': 0, 'fp32_split': 1}
 
@@ -43,11 +45,13 @@ def apex_epsilons(num_envs: int, eps: float = 0.4, alpha: float = 7.0) -> np.nda
 class B200ApexActor:
     """``num_envs`` Ape-X actors on one GPU, acting on a snapshot of a ``B200ApexLearner``'s Q network (``AtariQNet`` names and
     shapes).  ``epsilons``: [num_envs] values in [0, 1] (None: ``apex_epsilons(num_envs)``); ``precision``: the encoder operands, as
-    the learner's; ``priority_eps`` (> 0) is added to every priority the actor computes; ``dueling_dqn``: the learner's head kind.
-    Calls run on the current stream and share the actor's buffers: issue them from one stream."""
+    the learner's; ``priority_eps`` (> 0) is added to every priority the actor computes; ``dueling_dqn``, ``categorical_dqn`` (with
+    ``v_min``, ``v_max``, ``num_atoms``): the learner's head.  Calls run on the current stream and share the actor's buffers: issue them
+    from one stream."""
 
     def __init__(self, num_envs: int, num_actions: int, epsilons=None, seed: int = 0, precision: str = 'bf16', priority_eps: float = 1e-6,
-                 device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None, dueling_dqn: bool = False):
+                 device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None, dueling_dqn: bool = False,
+                 categorical_dqn: bool = False, v_min: float = 0.0, v_max: float = 200.0, num_atoms: int = 51):
         for name, v, hi in (('num_envs', num_envs, MAX_FRAMES), ('num_actions', num_actions, 31)):
             if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= hi:
                 raise ValueError(f'{name} must be an int in [1, {hi}], got {v!r}')
@@ -57,27 +61,38 @@ class B200ApexActor:
             raise ValueError(f"precision must be 'bf16' or 'fp32_split', got {precision!r}")
         if not isinstance(dueling_dqn, bool):
             raise ValueError(f'dueling_dqn must be a bool, got {dueling_dqn!r}')
+        if not isinstance(categorical_dqn, bool):
+            raise ValueError(f'categorical_dqn must be a bool, got {categorical_dqn!r}')
+        check_categorical(num_atoms, v_min, v_max)
+        if categorical_dqn and dueling_dqn:
+            raise ValueError('categorical_dqn with dueling_dqn is not supported: choose one head')
         priority_eps = float(priority_eps)
         if not (math.isfinite(priority_eps) and priority_eps > 0.0):
             raise ValueError(f'priority_eps must be finite and > 0 (a zero leaf makes the sampler\'s IS weight infinite), got {priority_eps}')
         self.num_envs, self.num_actions, self.seed, self.precision = int(num_envs), int(num_actions), int(seed), precision
-        self.priority_eps, self.dueling_dqn = priority_eps, dueling_dqn
+        self.priority_eps, self.dueling_dqn, self.categorical_dqn = priority_eps, dueling_dqn, categorical_dqn
+        self.v_min, self.v_max, self.num_atoms = float(v_min), float(v_max), int(num_atoms)
+        atoms = self.num_atoms if categorical_dqn else 0
         eps = self._epsilons(apex_epsilons(self.num_envs) if epsilons is None else epsilons)
         if not torch.cuda.is_available():
             raise RuntimeError('B200ApexActor needs a CUDA device: scalerl_b200 has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._L = _lib.lib()
-        self.shapes = apex_param_shapes(self.num_actions, dueling_dqn)
+        self.shapes = apex_param_shapes(self.num_actions, dueling_dqn, atoms)
         with torch.cuda.device(self.device):
-            total, off, cnt = _lib.apex_param_layout(self.num_actions, dueling_dqn)
+            total, off, cnt = _lib.apex_param_layout(self.num_actions, dueling_dqn, atoms)
             self.flat_params = torch.zeros(total, dtype=torch.float32, device=self.device)
             self.params = flat_views(self.flat_params, off, cnt, self.shapes)
             self.epsilons = eps.to(self.device)           # read by the act kernel when it runs
             h = C.c_void_p()
-            _lib.check(self._L.srl_apex_actor_create_ex(self.num_actions, self.num_envs, PRECISIONS[precision], int(dueling_dqn), self.seed,
-                                                        self.flat_params.data_ptr(), C.byref(h)), 'srl_apex_actor_create_ex')
+            if atoms:
+                _lib.check(self._L.srl_apex_actor_create_cat(self.num_actions, self.num_envs, PRECISIONS[precision], atoms, self.v_min, self.v_max,
+                                                             self.seed, self.flat_params.data_ptr(), C.byref(h)), 'srl_apex_actor_create_cat')
+            else:
+                _lib.check(self._L.srl_apex_actor_create_ex(self.num_actions, self.num_envs, PRECISIONS[precision], int(dueling_dqn), self.seed,
+                                                            self.flat_params.data_ptr(), C.byref(h)), 'srl_apex_actor_create_ex')
             self._h = h
-        self.load_state_dict(default_q_state_dict(self.num_actions, self.seed, dueling_dqn) if init_state_dict is None else init_state_dict)
+        self.load_state_dict(default_q_state_dict(self.num_actions, self.seed, dueling_dqn, atoms) if init_state_dict is None else init_state_dict)
         self.weights_version = 0
 
     def _stream(self):
@@ -109,6 +124,12 @@ class B200ApexActor:
             raise ValueError(f'the learner has num_actions={learner.hp.num_actions}, the actor {self.num_actions}')
         if learner.hp.dueling_dqn != self.dueling_dqn:
             raise ValueError(f'the learner has dueling_dqn={learner.hp.dueling_dqn}, the actor {self.dueling_dqn}')
+        if learner.hp.categorical_dqn != self.categorical_dqn:
+            raise ValueError(f'the learner has categorical_dqn={learner.hp.categorical_dqn}, the actor {self.categorical_dqn}')
+        if self.categorical_dqn:
+            mine, theirs = (self.num_atoms, self.v_min, self.v_max), (learner.hp.num_atoms, float(learner.hp.v_min), float(learner.hp.v_max))
+            if mine != theirs:
+                raise ValueError(f'the learner has (num_atoms, v_min, v_max)={theirs}, the actor {mine}')
         if learner.device != self.device:
             raise ValueError(f'the learner is on {learner.device}, the actor on {self.device}')
         self.flat_params.copy_(learner.flat_params)
@@ -148,6 +169,15 @@ class B200ApexActor:
         _lib.check(self._L.srl_apex_actor_q_values(self._h, obs.data_ptr(), obs.shape[0], q.data_ptr(), self._stream()),
                    'srl_apex_actor_q_values')
         return q
+
+    def debug_buffer(self, name: str) -> torch.Tensor:
+        """copy of one of the actor's device buffers (tests only; names: srl_apex_actor_debug_buffer), flat"""
+        p, n = C.c_void_p(), C.c_int64()
+        _lib.check(self._L.srl_apex_actor_debug_buffer(self._h, name.encode(), C.byref(p), C.byref(n)), 'debug_buffer')
+        out = torch.empty(n.value, dtype=torch.float32, device=self.device)
+        _lib.check(self._L.srl_memcpy_d2d(out.data_ptr(), p.value, n.value * 4, self._stream()), 'memcpy_d2d')
+        torch.cuda.current_stream(self.device).synchronize()
+        return out
 
     def close(self):
         if getattr(self, '_h', None) is not None:

@@ -11,6 +11,11 @@ n-step storage) inside the same graph.  ``B200ApexActor`` (actor.py) acts and co
 ``ApexHParams(dueling_dqn=True)`` replaces the Q head ``q = Linear(512, A)`` by the dueling head of Wang et al. 2016 (eq. 9):
 ``V = value(h)``, ``Adv = advantage(h)``, ``Q = V + Adv - Adv.mean(1, keepdim=True)``.  Both streams read the encoder's shared 512-unit
 fc output (the paper's Atari network gives each stream an fc layer of its own), so the encoder is the plain network's.
+
+``ApexHParams(categorical_dqn=True)`` makes the head categorical (C51, Bellemare et al. 2017): ``q = Linear(512, A * num_atoms)``,
+a softmax over each action's ``num_atoms`` logits on the support ``z_k = v_min + k dz``, Q = sum_k z_k p_k for acting and the greedy
+target, and the cross-entropy against the projected target distribution as the loss.  Priorities are the KL divergence of the target
+from the online distribution (Hessel et al. 2018).  The state-dict names stay the plain head's ten.
 """
 from __future__ import annotations
 
@@ -42,25 +47,42 @@ def apex_param_names(dueling: bool = False):
     return APEX_DUELING_PARAM_NAMES if dueling else APEX_PARAM_NAMES
 
 
-def apex_param_shapes(num_actions: int, dueling: bool = False):
+def apex_param_shapes(num_actions: int, dueling: bool = False, num_atoms: int = 0):
+    """the named shapes of the Q network's parameters; num_atoms > 0: the categorical head q = Linear(512, num_actions * num_atoms)"""
+    R = num_actions * num_atoms if num_atoms else num_actions
     head = [('value.weight', (1, 512)), ('value.bias', (1,)), ('advantage.weight', (num_actions, 512)), ('advantage.bias', (num_actions,))] \
-        if dueling else [('q.weight', (num_actions, 512)), ('q.bias', (num_actions,))]
+        if dueling else [('q.weight', (R, 512)), ('q.bias', (R,))]
     return OrderedDict([
         ('conv1.weight', (32, 4, 8, 8)), ('conv1.bias', (32,)), ('conv2.weight', (64, 32, 4, 4)), ('conv2.bias', (64,)),
         ('conv3.weight', (64, 64, 3, 3)), ('conv3.bias', (64,)), ('fc.weight', (512, 3136)), ('fc.bias', (512,))] + head)
 
 
+def categorical_support(num_atoms: int, v_min: float, v_max: float) -> torch.Tensor:
+    """z_k = v_min + k dz in fp32, dz = (v_max - v_min) / (num_atoms - 1) rounded once to fp32 (the bounds rounded to fp32 first, as
+    the C ABI receives them)"""
+    lo, hi = float(np.float32(v_min)), float(np.float32(v_max))
+    dz = torch.tensor((hi - lo) / (num_atoms - 1), dtype=torch.float32)
+    return torch.tensor(lo, dtype=torch.float32) + torch.arange(num_atoms, dtype=torch.float32) * dz
+
+
 class AtariQNet(nn.Module):
     """Nature DQN on 4 stacked 84x84 frames: AtariNet's conv1..3 and fc (scalerl/algorithms/utils/atari_model.py:30-47, 91-101)
     followed by ``q = nn.Linear(512, num_actions)``, or, with ``dueling``, by ``value = nn.Linear(512, 1)`` and ``advantage =
-    nn.Linear(512, num_actions)`` combined as Q = V + Adv - mean_a Adv (Wang et al. 2016, eq. 9).  Initialised by torch's default
-    layer init, so ``torch.manual_seed(s)`` before construction fixes the weights."""
+    nn.Linear(512, num_actions)`` combined as Q = V + Adv - mean_a Adv (Wang et al. 2016, eq. 9), or, with ``categorical``, by
+    ``q = nn.Linear(512, num_actions * num_atoms)`` whose row a * num_atoms + k is atom k of action a (C51): ``dist(obs)`` gives the
+    softmax per action, ``forward`` its expectation on the support (a non-persistent buffer: the state-dict names are the plain ten).
+    Initialised by torch's default layer init, so ``torch.manual_seed(s)`` before construction fixes the weights."""
 
-    def __init__(self, num_actions: int, observation_shape=(4, 84, 84), dueling: bool = False):
+    def __init__(self, num_actions: int, observation_shape=(4, 84, 84), dueling: bool = False, categorical: bool = False,
+                 num_atoms: int = 51, v_min: float = 0.0, v_max: float = 200.0):
         super().__init__()
+        if dueling and categorical:
+            raise ValueError('the categorical head with the dueling head is not supported')
         self.observation_shape = tuple(observation_shape)
         self.num_actions = int(num_actions)
         self.dueling = bool(dueling)
+        self.categorical = bool(categorical)
+        self.num_atoms = int(num_atoms) if self.categorical else 0
         self.conv1 = nn.Conv2d(self.observation_shape[0], 32, kernel_size=8, stride=4)
         self.conv2 = nn.Conv2d(32, 64, kernel_size=4, stride=2)
         self.conv3 = nn.Conv2d(64, 64, kernel_size=3, stride=1)
@@ -68,16 +90,30 @@ class AtariQNet(nn.Module):
         if self.dueling:
             self.value = nn.Linear(512, 1)
             self.advantage = nn.Linear(512, self.num_actions)
+        elif self.categorical:
+            self.q = nn.Linear(512, self.num_actions * self.num_atoms)
+            self.register_buffer('support', categorical_support(self.num_atoms, v_min, v_max), persistent=False)
         else:
             self.q = nn.Linear(512, self.num_actions)
 
-    def forward(self, obs: torch.Tensor) -> torch.Tensor:
-        """obs u8 [N, 4, 84, 84] -> Q values [N, A]"""
+    def _features(self, obs: torch.Tensor) -> torch.Tensor:
         x = obs.float() / 255.0
         x = F.relu(self.conv1(x))
         x = F.relu(self.conv2(x))
         x = F.relu(self.conv3(x))
-        x = F.relu(self.fc(x.reshape(x.shape[0], -1)))
+        return F.relu(self.fc(x.reshape(x.shape[0], -1)))
+
+    def dist(self, obs: torch.Tensor) -> torch.Tensor:
+        """categorical head: obs u8 [N, 4, 84, 84] -> the atom probabilities p [N, A, num_atoms]"""
+        if not self.categorical:
+            raise ValueError('dist() needs the categorical head (AtariQNet(..., categorical=True))')
+        return F.softmax(self.q(self._features(obs)).view(-1, self.num_actions, self.num_atoms), dim=2)
+
+    def forward(self, obs: torch.Tensor) -> torch.Tensor:
+        """obs u8 [N, 4, 84, 84] -> Q values [N, A]"""
+        if self.categorical:
+            return (self.dist(obs) * self.support).sum(2)
+        x = self._features(obs)
         if self.dueling:
             v, adv = self.value(x), self.advantage(x)
             return v + adv - adv.mean(dim=1, keepdim=True)
@@ -95,6 +131,10 @@ class ApexHParams:
     max_grad_norm: Optional[float] = None
     double_dqn: bool = False
     dueling_dqn: bool = False            # the dueling head V + Adv - mean(Adv) on the shared fc output instead of q = Linear(512, A)
+    categorical_dqn: bool = False        # the categorical (C51) head q = Linear(512, A num_atoms) on the support [v_min, v_max]
+    v_min: float = 0.0
+    v_max: float = 200.0
+    num_atoms: int = 51
     target_update_frequency: int = 100
     soft_update_tau: float = 1.0
     precision: str = 'bf16'              # encoder operands: 'bf16' | 'fp32_split' (fp32-accurate hi/lo bf16 pairs)
@@ -112,6 +152,11 @@ class ApexHParams:
             raise ValueError(f'num_actions must be an int in [1, 31], got {self.num_actions!r}')
         if not isinstance(self.dueling_dqn, bool):
             raise ValueError(f'dueling_dqn must be a bool, got {self.dueling_dqn!r}')
+        if not isinstance(self.categorical_dqn, bool):
+            raise ValueError(f'categorical_dqn must be a bool, got {self.categorical_dqn!r}')
+        check_categorical(self.num_atoms, self.v_min, self.v_max)
+        if self.categorical_dqn and self.dueling_dqn:
+            raise ValueError('categorical_dqn with dueling_dqn is not supported: choose one head')
         if not (math.isfinite(self.gamma) and self.gamma >= 0.0):
             raise ValueError(f'gamma must be finite and >= 0, got {self.gamma}')
         if not (math.isfinite(self.learning_rate) and self.learning_rate > 0.0):
@@ -142,7 +187,23 @@ class ApexHParams:
         c.learning_rate, c.adam_beta1, c.adam_beta2, c.adam_eps = self.learning_rate, self.adam_beta1, self.adam_beta2, self.adam_eps
         c.priority_eps = self.priority_eps
         c.dueling = 1 if self.dueling_dqn else 0
+        c.num_atoms = self.atoms()
+        c.v_min, c.v_max = self.v_min, self.v_max
         return c
+
+    def atoms(self) -> int:
+        """the categorical head's atom count, 0 for a scalar head"""
+        return self.num_atoms if self.categorical_dqn else 0
+
+
+def check_categorical(num_atoms, v_min, v_max) -> None:
+    """the categorical head's settings: num_atoms an int in [2, 64], v_min < v_max finite (also as fp32, as the kernels read them)"""
+    if isinstance(num_atoms, bool) or not isinstance(num_atoms, (int, np.integer)) or not 2 <= num_atoms <= 64:
+        raise ValueError(f'num_atoms must be an int in [2, 64], got {num_atoms!r}')
+    with np.errstate(over='ignore'):
+        lo, hi = np.float32(v_min), np.float32(v_max)
+    if not (np.isfinite(lo) and np.isfinite(hi) and lo < hi and np.isfinite(np.float32((float(hi) - float(lo)) / (num_atoms - 1)))):
+        raise ValueError(f'v_min and v_max must be finite fp32 values with v_min < v_max, got ({v_min}, {v_max})')
 
 
 def flat_views(flat: torch.Tensor, off, cnt, shapes) -> 'OrderedDict[str, torch.Tensor]':
@@ -160,11 +221,12 @@ def load_views(dst: Dict[str, torch.Tensor], sd: Dict[str, torch.Tensor]) -> Non
         v.copy_(sd[n].to(v.device, torch.float32))
 
 
-def default_q_state_dict(num_actions: int, seed: int = 0, dueling: bool = False) -> 'OrderedDict[str, torch.Tensor]':
-    """AtariQNet's initial weights under ``torch.manual_seed(seed)``, drawn without disturbing the global RNG"""
+def default_q_state_dict(num_actions: int, seed: int = 0, dueling: bool = False, num_atoms: int = 0) -> 'OrderedDict[str, torch.Tensor]':
+    """AtariQNet's initial weights under ``torch.manual_seed(seed)``, drawn without disturbing the global RNG (num_atoms > 0: the
+    categorical head's)"""
     with torch.random.fork_rng(devices=[]):
         torch.manual_seed(seed)
-        net = AtariQNet(num_actions, dueling=dueling)
+        net = AtariQNet(num_actions, dueling=dueling, categorical=num_atoms > 0, num_atoms=num_atoms or 51)
     return OrderedDict((k, v.detach().clone()) for k, v in net.state_dict().items())
 
 
@@ -187,9 +249,9 @@ class B200ApexLearner(BaseAgent):
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._L = _lib.lib()
         self.names = apex_param_names(hp.dueling_dqn)
-        self.shapes = apex_param_shapes(hp.num_actions, hp.dueling_dqn)
+        self.shapes = apex_param_shapes(hp.num_actions, hp.dueling_dqn, hp.atoms())
         with torch.cuda.device(self.device):
-            total, self._off, self._cnt = _lib.apex_param_layout(hp.num_actions, hp.dueling_dqn)
+            total, self._off, self._cnt = _lib.apex_param_layout(hp.num_actions, hp.dueling_dqn, hp.atoms())
             z = lambda: torch.zeros(total, dtype=torch.float32, device=self.device)
             self.flat_params, self.flat_grads, self.exp_avg, self.exp_avg_sq, self.flat_target = z(), z(), z(), z(), z()
             self.params = self._views(self.flat_params)
@@ -202,7 +264,7 @@ class B200ApexLearner(BaseAgent):
                                                        C.byref(h)), 'srl_apex_learner_create')
             self._h = h
             self._stats = torch.zeros(4, device=self.device)      # {loss, gradient norm, clip coefficient, pad}
-        sd = default_q_state_dict(hp.num_actions, seed, hp.dueling_dqn) if init_state_dict is None else init_state_dict
+        sd = default_q_state_dict(hp.num_actions, seed, hp.dueling_dqn, hp.atoms()) if init_state_dict is None else init_state_dict
         self.load_state_dict(sd)
         self.load_state_dict(sd, target=True)       # actor_target starts as a copy (dqn_agent.py:66-67)
         self.use_graph = use_graph
@@ -239,7 +301,8 @@ class B200ApexLearner(BaseAgent):
         return {'exp_avg': self._views(self.exp_avg), 'exp_avg_sq': self._views(self.exp_avg_sq)}
 
     def optimizer_state_dict(self) -> dict:
-        """``torch.optim.Adam(AtariQNet(A, dueling=hp.dueling_dqn).parameters()).state_dict()`` layout"""
+        """``torch.optim.Adam(AtariQNet(A, dueling=hp.dueling_dqn, categorical=hp.categorical_dqn, ...).parameters()).state_dict()``
+        layout"""
         return to_torch_optimizer_state(self.hp, self._opt_tensors(), self._opt_steps, order=self.names)
 
     def load_optimizer_state_dict(self, sd: dict) -> None:
@@ -366,7 +429,8 @@ class B200ApexLearner(BaseAgent):
     @torch.no_grad()
     def learn(self, experiences, weights: Optional[torch.Tensor] = None, idxs: Optional[torch.Tensor] = None, sampler=None,
               sync_stats: bool = True, use_graph: Optional[bool] = None) -> Dict[str, float]:
-        """one update (apex/worker.py:134-161; dqn_agent.py:136-190) -> {'loss': float}, or {} with nothing synchronised"""
+        """one update (apex/worker.py:134-161; dqn_agent.py:136-190) -> {'loss': float}, or {} with nothing synchronised.  The
+        categorical head's loss is mean(w * cross-entropy)."""
         obs, action, reward, next_obs, done = self._inputs(experiences, weights, idxs, sampler)
         args = (obs, action, reward, next_obs, done, weights, idxs, sampler)
         key = tuple(a.data_ptr() if isinstance(a, torch.Tensor) else (a._h.value if a is not None else None) for a in args)
@@ -429,7 +493,8 @@ class B200ApexLearner(BaseAgent):
         return {'loss': s[0], 'grad_norm': s[1], 'clip_coef': s[2]}
 
     def debug_buffer(self, name: str) -> torch.Tensor:
-        """copy of one of the step's device buffers (tests only; names: srl_apex_learner_debug_buffer)"""
+        """copy of one of the step's device buffers (tests only; names: srl_apex_learner_debug_buffer; the categorical head's
+        logits, dlogits and m come flat, [B * A * num_atoms] and [B * num_atoms])"""
         p, n = C.c_void_p(), C.c_int64()
         _lib.check(self._L.srl_apex_learner_debug_buffer(self._h, name.encode(), C.byref(p), C.byref(n)), 'debug_buffer')
         dt = {'priorities': torch.float64, 'step': torch.int32, 'a1': torch.bfloat16, 'a2': torch.bfloat16, 'a3': torch.bfloat16}.get(name, torch.float32)

@@ -6,10 +6,14 @@
 // here has the bits of the learner's for the same weights.  fp32 on the CUDA cores: the Q head is 512 x A, no tensor-core work.
 //   apex_act_kernel       the Q row, its first argmax and the epsilon-greedy draw (one warp per env)
 //   apex_priority_kernel  q(s, a), the n-step target from max_a Q(s') and the priority (one warp per transition)
-// Both are templates on the head: plain q = Linear(512, A), or the dueling V + Adv - mean(Adv) (dqn_head.cuh's dueling_q).
+// Both are templates on the head: plain q = Linear(512, A), or the dueling V + Adv - mean(Adv) (dqn_head.cuh's dueling_q).  The
+// categorical head (C51) runs the learner's logits GEMM (dqn_cat.cu) first; apex_cat_act_kernel and apex_cat_priority_kernel then
+// read the logits through dqn_cat.cuh's functions, the learner tail's.
 #include <math.h>
+#include <string.h>
 #include <new>
 #include "common.cuh"
+#include "dqn_cat.cuh"
 #include "dqn_head.cuh"
 #include "errors.h"
 #include "kernels.h"
@@ -31,6 +35,25 @@ SRL_DEVINL uint4 philox4x32_10(uint4 c, uint2 k) {
   return c;
 }
 
+// env e's action of draw d: with probability eps[e] a uniform action, else `greedy`
+SRL_DEVINL int64_t eps_greedy(unsigned long long d, int e, uint2 key, int A, const float* __restrict__ eps, int greedy) {
+  const uint4 r = philox4x32_10(make_uint4((uint32_t)d, (uint32_t)(d >> 32), (uint32_t)e, 0u), key);
+  const float u = (float)(r.x >> 8) * 0x1p-24f;                            // uniform in [0, 1)
+  const int random_action = (int)(((unsigned long long)r.y * (unsigned)A) >> 32);   // uniform in [0, A)
+  return u < __ldg(eps + e) ? random_action : greedy;
+}
+// the end of an act launch: the block that finishes last advances the draw counter d and re-arms the ticket
+SRL_DEVINL void advance_draws(unsigned long long* draws, unsigned long long d) {
+  __shared__ bool is_last;
+  __syncthreads();                 // every warp of the block has read the counter
+  if (threadIdx.x == 0) is_last = take_ticket(reinterpret_cast<float*>(draws + 1));
+  __syncthreads();
+  if (is_last && threadIdx.x == 0) {
+    draws[0] = d + 1;
+    *reinterpret_cast<unsigned*>(draws + 1) = 0u;
+  }
+}
+
 // One warp per env, 4 per block.  draws[0]: the draw counter (u64), read by every block and advanced by the block that finishes
 // last (draws[1] low word: the ticket, re-armed by that block), so every env of one launch uses the same draw.
 // DUELING: W = [(A + 1)][512], b the value bias, ba the advantage biases.
@@ -44,21 +67,22 @@ __global__ void __launch_bounds__(128) apex_act_kernel(const float* __restrict__
     int greedy;
     if constexpr (DUELING) q_row_max(dueling_q<false>(core + (size_t)e * ENC_CORE, W, b, ba, A, lane, nullptr), A, &greedy);
     else q_max(core + (size_t)e * ENC_CORE, W, b, A, lane, &greedy);
-    if (lane == 0) {
-      const uint4 r = philox4x32_10(make_uint4((uint32_t)d, (uint32_t)(d >> 32), (uint32_t)e, 0u), key);
-      const float u = (float)(r.x >> 8) * 0x1p-24f;                            // uniform in [0, 1)
-      const int random_action = (int)(((unsigned long long)r.y * (unsigned)A) >> 32);   // uniform in [0, A)
-      actions[e] = u < __ldg(eps + e) ? random_action : greedy;
-    }
+    if (lane == 0) actions[e] = eps_greedy(d, e, key, A, eps, greedy);
   }
-  __shared__ bool is_last;
-  __syncthreads();                 // every warp of the block has read the counter
-  if (threadIdx.x == 0) is_last = take_ticket(reinterpret_cast<float*>(draws + 1));
-  __syncthreads();
-  if (is_last && threadIdx.x == 0) {
-    draws[0] = d + 1;
-    *reinterpret_cast<unsigned*>(draws + 1) = 0u;
+  advance_draws(draws, d);
+}
+// the same on the categorical head's logits [E][A K]: greedy = the first argmax of the expected Q
+__global__ void __launch_bounds__(128) apex_cat_act_kernel(const float* __restrict__ logits, int E, int A, const CatSupport c,
+                                                           const float* __restrict__ eps, uint2 key, unsigned long long* draws,
+                                                           int64_t* __restrict__ actions) {
+  const int lane = threadIdx.x & 31, e = blockIdx.x * 4 + (threadIdx.x >> 5);
+  const unsigned long long d = *reinterpret_cast<volatile unsigned long long*>(draws);
+  if (e < E) {
+    int greedy;
+    q_row_max(cat_q_lane(logits + (size_t)e * A * c.K, A, c, lane), A, &greedy);
+    if (lane == 0) actions[e] = eps_greedy(d, e, key, A, eps, greedy);
   }
+  advance_draws(draws, d);
 }
 
 // One warp per transition e in ring slot (ptr + e) mod M, 4 per block: q = Q(s)[a], y = R + gamma_n (1 - d) max_a Q(s'), the
@@ -85,6 +109,21 @@ __global__ void __launch_bounds__(128) apex_priority_kernel(const float* __restr
   const float y = td_target(__ldg(reward + slot), gamma_n, nx, done[slot] != 0);
   if (lane == 0) prio[e] = td_priority(__fsub_rn(q, y), eps);
 }
+// the categorical head: the learner tail's cat_transition with the snapshot's logits of s (logits_s) and s' (logits_n) as the online and
+// target network's, no double DQN -> max(KL(m || p(s)[a]), 0) + eps
+__global__ void __launch_bounds__(128) apex_cat_priority_kernel(const float* __restrict__ logits_s, const float* __restrict__ logits_n, int E,
+                                                                int A, const CatSupport c, const int64_t* __restrict__ action,
+                                                                const float* __restrict__ reward, const uint8_t* __restrict__ done, int64_t ptr,
+                                                                int64_t M, float gamma_n, float eps, double* __restrict__ prio) {
+  __shared__ float sm[4][CAT_MAX_ATOMS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, e = blockIdx.x * 4 + warp;
+  if (e >= E) return;
+  const int64_t slot = (ptr + e) % M;
+  const int act = ld_action(action + slot, A), R = A * c.K;
+  const CatLoss r = cat_transition(logits_s + (size_t)e * R + (size_t)act * c.K, nullptr, logits_n + (size_t)e * R, A, __ldg(reward + slot),
+                                   done[slot] ? 0.f : gamma_n, c, lane, sm[warp], 0.f, nullptr);
+  if (lane == 0) prio[e] = cat_priority(r.kl, eps);
+}
 
 }  // namespace srl
 using namespace srl;
@@ -95,6 +134,8 @@ struct srl_apex_actor {
   const float* w8[8];              // the encoder tensors of the snapshot
   const float *Wq, *bq;            // plain: q.weight, q.bias; dueling: [value.weight; advantage.weight], value.bias
   const float* bqa;                // dueling: advantage.bias (NULL: the plain head)
+  CatSupport cs;                   // the categorical head (cs.K > 0)
+  float* logits;                   // categorical: [2E][A K], the logits of the core rows
   srl_encoder_t* enc;
   char *saved, *scratch;           // encoder blocks for E frames: the two forwards of an add run one after the other
   float* core;                     // [2E][ENC_CORE]: the forward over s (and act's), then the one over s'
@@ -116,9 +157,10 @@ int actor_rows(srl_apex_actor* X, int64_t saved, int64_t scratch, WsRow* t) {
   t[n++] = ws_row(nullptr, E, &X->zero_action);
   t[n++] = ws_row(nullptr, E, &X->prio);
   t[n++] = ws_row(nullptr, 2, &X->draws);
+  t[n++] = ws_row(nullptr, 2 * E * X->A * X->cs.K, &X->logits);
   return n;
 }
-constexpr int ACTOR_ROWS = 7;
+constexpr int ACTOR_ROWS = 8;
 
 // Q head rows of `frames` frames of obs into core (f <= E frames per call)
 int actor_forward(srl_apex_actor* X, const uint8_t* obs, int frames, float* core, cudaStream_t st) {
@@ -126,22 +168,38 @@ int actor_forward(srl_apex_actor* X, const uint8_t* obs, int frames, float* core
 }
 }  // namespace
 
+static int actor_create(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, uint64_t seed,
+                        const float* params, srl_apex_actor_t** out);
+
 extern "C" int srl_apex_actor_create(int A, int num_envs, int precision, uint64_t seed, const float* params, srl_apex_actor_t** out) {
   return srl_apex_actor_create_ex(A, num_envs, precision, 0, seed, params, out);
 }
 
 extern "C" int srl_apex_actor_create_ex(int A, int num_envs, int precision, int dueling, uint64_t seed, const float* params,
                                         srl_apex_actor_t** out) {
+  return actor_create(A, num_envs, precision, dueling, 0, 0.f, 0.f, seed, params, out);
+}
+
+extern "C" int srl_apex_actor_create_cat(int A, int num_envs, int precision, int num_atoms, float v_min, float v_max, uint64_t seed,
+                                         const float* params, srl_apex_actor_t** out) {
+  return actor_create(A, num_envs, precision, 0, num_atoms, v_min, v_max, seed, params, out);
+}
+
+static int actor_create(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max,
+                                          uint64_t seed, const float* params, srl_apex_actor_t** out) {
   REQ(params && out, "apex_actor_create: NULL argument");
   REQ(A >= 1 && A <= 31, "apex_actor_create: A=%d must be in [1,31]", A);
   REQ(num_envs >= 1 && num_envs <= MAX_FRAMES, "apex_actor_create: num_envs=%d must be in [1, %d]", num_envs, MAX_FRAMES);
   REQ(precision == 0 || precision == 1, "apex_actor_create: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", precision);
   REQ(dueling == 0 || dueling == 1, "apex_actor_create: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", dueling);
+  int rc = check_cat_head("apex_actor_create", num_atoms, v_min, v_max, dueling);
+  if (rc) return rc;
   REQ(!misaligned(params, 16), "apex_actor_create: params must be 16-byte aligned");
   int64_t off[12];
-  srl_apex_param_layout_ex(A, dueling, off, nullptr);
+  if (num_atoms) srl_apex_param_layout_cat(A, num_atoms, off, nullptr);
+  else srl_apex_param_layout_ex(A, dueling, off, nullptr);
   int64_t sb = 0, kb = 0;
-  int rc = srl_encoder_sizes(num_envs, precision, &sb, &kb);
+  rc = srl_encoder_sizes(num_envs, precision, &sb, &kb);
   if (rc) return rc;
   srl_apex_actor* X = new (std::nothrow) srl_apex_actor();
   REQ(X, "out of host memory");
@@ -151,6 +209,7 @@ extern "C" int srl_apex_actor_create_ex(int A, int num_envs, int precision, int 
   for (int i = 0; i < 8; ++i) X->w8[i] = params + off[i];
   X->Wq = params + off[8]; X->bq = params + off[9];
   X->bqa = dueling ? params + off[11] : nullptr;
+  if (num_atoms) X->cs = cat_support(num_atoms, v_min, v_max);
   rc = srl_encoder_create(precision, &X->enc);
   if (rc) return undo(rc);
   WsRow t[ACTOR_ROWS];
@@ -182,7 +241,10 @@ extern "C" int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const
   const cudaStream_t st = (cudaStream_t)stream;
   rc = actor_forward(X, obs, E, X->core, st);
   if (rc) return rc;
-  if (X->bqa) apex_act_kernel<true><<<(E + 3) / 4, 128, 0, st>>>(X->core, X->Wq, X->bq, E, X->A, epsilons, X->key, X->draws, actions, X->bqa);
+  if (X->cs.K) {
+    CU(launch_cat_logits(X->core, X->Wq, X->bq, E, X->A * X->cs.K, X->logits, st), "cat_logits");
+    apex_cat_act_kernel<<<(E + 3) / 4, 128, 0, st>>>(X->logits, E, X->A, X->cs, epsilons, X->key, X->draws, actions);
+  } else if (X->bqa) apex_act_kernel<true><<<(E + 3) / 4, 128, 0, st>>>(X->core, X->Wq, X->bq, E, X->A, epsilons, X->key, X->draws, actions, X->bqa);
   else apex_act_kernel<false><<<(E + 3) / 4, 128, 0, st>>>(X->core, X->Wq, X->bq, E, X->A, epsilons, X->key, X->draws, actions, nullptr);
   CU(cudaGetLastError(), "apex_act_kernel");
   return 0;
@@ -199,9 +261,18 @@ extern "C" int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, 
     const int f = n - f0 < X->E ? n - f0 : X->E;
     rc = actor_forward(X, obs + (size_t)f0 * ACTOR_OBS_BYTES, f, X->core, st);
     if (rc) return rc;
-    CU(launch_dqn_q_values(X->core, X->Wq, X->bq, X->bqa, f, X->A, q_out + (size_t)f0 * X->A, st), "dqn_q_values");
+    if (X->cs.K) CU(launch_cat_q_values(X->core, X->Wq, X->bq, f, X->A, X->cs, X->logits, q_out + (size_t)f0 * X->A, st), "cat_q_values");
+    else CU(launch_dqn_q_values(X->core, X->Wq, X->bq, X->bqa, f, X->A, q_out + (size_t)f0 * X->A, st), "dqn_q_values");
   }
   return 0;
+}
+
+extern "C" int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name, void** ptr, int64_t* count) {
+  REQ(X && name && ptr && count, "apex_actor_debug_buffer: NULL argument");
+  const int64_t rows = 2 * (int64_t)X->E;
+  if (strcmp(name, "core") == 0) { *ptr = X->core; *count = rows * ENC_CORE; return 0; }
+  if (strcmp(name, "logits") == 0 && X->cs.K) { *ptr = X->logits; *count = rows * X->A * X->cs.K; return 0; }
+  return fail(SRL_EINVAL, "apex_actor_debug_buffer: unknown buffer '%s'", name);
 }
 
 namespace srl {
@@ -214,7 +285,12 @@ int apex_actor_priorities(srl_apex_actor* X, const uint8_t* s, const uint8_t* s_
   int rc = actor_forward(X, s, E, X->core, st);
   if (!rc) rc = actor_forward(X, s_next, E, core_n, st);
   if (rc) return rc;
-  if (X->bqa)
+  if (X->cs.K) {
+    const int R = X->A * X->cs.K;
+    CU(launch_cat_logits(X->core, X->Wq, X->bq, 2 * E, R, X->logits, st), "cat_logits");      // s and s' rows in one GEMM
+    apex_cat_priority_kernel<<<(E + 3) / 4, 128, 0, st>>>(X->logits, X->logits + (size_t)E * R, E, X->A, X->cs, action, reward, done, ptr, M,
+                                                          gamma_n, eps, X->prio);
+  } else if (X->bqa)
     apex_priority_kernel<true><<<(E + 3) / 4, 128, 0, st>>>(X->core, core_n, X->Wq, X->bq, E, X->A, action, reward, done, ptr, M, gamma_n, eps,
                                                              X->prio, X->bqa);
   else

@@ -897,8 +897,10 @@ extern "C" int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int fr
 // state_dict order {conv1.w, conv1.b, conv2.w, conv2.b, conv3.w, conv3.b, fc.w, fc.b, q.w, q.b}; in memory fc.weight last.
 // dueling: {..., fc.b, value.w [1,512], value.b [1], advantage.w [A,512], advantage.b [A]}; in memory value.weight directly before
 // advantage.weight (one [(A + 1)][512] head block for the kernels) and value.bias before advantage.bias
-static int64_t apex_layout(int A, int dueling, int64_t* off, int64_t* cnt) {
-  const int64_t plain[10] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, (int64_t)A * 512, A};
+// categorical (atoms = K > 0): the plain order with q.weight [A K, 512] and q.bias [A K] (row a K + k: atom k of action a)
+static int64_t apex_layout(int A, int dueling, int atoms, int64_t* off, int64_t* cnt) {
+  const int64_t R = (int64_t)A * (atoms ? atoms : 1);
+  const int64_t plain[10] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, R * 512, R};
   const int64_t duel[12] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, 512, 1, (int64_t)A * 512, A};
   const int plain_order[10] = {0, 1, 2, 3, 4, 5, 7, 8, 9, 6};
   const int duel_order[12] = {0, 1, 2, 3, 4, 5, 7, 8, 10, 9, 11, 6};
@@ -914,12 +916,32 @@ static int64_t apex_layout(int A, int dueling, int64_t* off, int64_t* cnt) {
   }
   return o;
 }
-extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) { return apex_layout(A, 0, offsets10, counts10); }
+extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) { return apex_layout(A, 0, 0, offsets10, counts10); }
 extern "C" int64_t srl_apex_param_layout_ex(int A, int dueling, int64_t* offsets12, int64_t* counts12) {
   REQ(A >= 1 && A <= 31, "apex_param_layout: A=%d must be in [1,31]", A);
   REQ(dueling == 0 || dueling == 1, "apex_param_layout: dueling=%d must be 0 or 1", dueling);
-  return apex_layout(A, dueling, offsets12, counts12);
+  return apex_layout(A, dueling, 0, offsets12, counts12);
 }
+extern "C" int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offsets10, int64_t* counts10) {
+  REQ(A >= 1 && A <= 31, "apex_param_layout: A=%d must be in [1,31]", A);
+  REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "apex_param_layout: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]",
+      num_atoms, CAT_MAX_ATOMS);
+  return apex_layout(A, 0, num_atoms, offsets10, counts10);
+}
+
+namespace srl {
+int check_cat_head(const char* who, int num_atoms, float v_min, float v_max, int dueling) {
+  REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "%s: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]", who,
+      num_atoms, CAT_MAX_ATOMS);
+  if (num_atoms == 0) return 0;
+  REQ(std::isfinite(v_min) && std::isfinite(v_max) && v_min < v_max, "%s: v_min=%g, v_max=%g must be finite with v_min < v_max", who,
+      (double)v_min, (double)v_max);
+  const float dz = cat_support(num_atoms, v_min, v_max).dz;
+  REQ(std::isfinite(dz) && dz > 0.f, "%s: the atom spacing (v_max - v_min) / (num_atoms - 1) = %g is not a positive finite float", who, (double)dz);
+  REQ(dueling == 0, "%s: the categorical head (num_atoms=%d) with dueling=1 is not supported", who, num_atoms);
+  return 0;
+}
+}  // namespace srl
 
 struct srl_apex_learner {
   srl_apex_config_t cfg;
@@ -937,6 +959,10 @@ struct srl_apex_learner {
   double* prio;
   int64_t* zero_action;
   int* dstep;
+  // the categorical head (cfg.num_atoms = K > 0): logits [B][A K] over s, s' (online, double DQN only) and s' (target), their
+  // gradient, the projected targets m [B][K], the cross-entropies [B] and the q-value chunk's logits
+  float *logits_s, *logits_n, *logits_nt, *dlogits, *mproj, *ce, *logits_q;
+  CatSupport cs;
   char* arena;
 };
 
@@ -969,14 +995,22 @@ static int apex_rows(srl_apex_learner* L, const int64_t* b4, WsRow* t) {
   t[n++] = ws_row("step", 4, &L->dstep);
   t[n++] = ws_row(nullptr, B, &L->dq);
   t[n++] = ws_row(nullptr, 4 + dqn_tail_blocks((int)B), &L->tail_scratch);
-  t[n++] = ws_row(nullptr, HEAD_GROUPS * (A + L->cfg.dueling) * 513, &L->head_part);
+  const int64_t K = L->cfg.num_atoms, R = A * K;     // K = 0: the scalar heads, whose rows below are empty
+  t[n++] = ws_row(nullptr, K ? 0 : HEAD_GROUPS * (A + L->cfg.dueling) * 513, &L->head_part);
   t[n++] = ws_row(nullptr, 4, &L->coef);
   t[n++] = ws_row(nullptr, 2048, &L->opt_scratch);
   t[n++] = ws_row(nullptr, QC, &L->zero_reward);     // the reward / action columns of the q-value forwards (the Q head reads h only)
   t[n++] = ws_row(nullptr, QC, &L->zero_action);
+  t[n++] = ws_row("logits", B * R, &L->logits_s);
+  t[n++] = ws_row("logits_next", L->cfg.double_dqn ? B * R : 0, &L->logits_n);
+  t[n++] = ws_row("logits_next_target", B * R, &L->logits_nt);
+  t[n++] = ws_row("dlogits", B * R, &L->dlogits);
+  t[n++] = ws_row("m", B * K, &L->mproj);
+  t[n++] = ws_row("ce", B * (K ? 1 : 0), &L->ce);
+  t[n++] = ws_row(nullptr, QC * R, &L->logits_q);
   return n;
 }
-constexpr int APEX_ROWS = 22;
+constexpr int APEX_ROWS = 29;
 
 static int check_apex_cfg(const srl_apex_config_t* c) {
   REQ(c, "apex_learner: config is NULL");
@@ -991,7 +1025,7 @@ static int check_apex_cfg(const srl_apex_config_t* c) {
   REQ(std::isfinite(c->adam_eps) && c->adam_eps >= 0.f, "apex_learner: adam_eps=%g must be finite and >= 0", (double)c->adam_eps);
   REQ(std::isfinite(c->priority_eps) && c->priority_eps >= 0.f, "apex_learner: priority_eps=%g must be finite and >= 0", (double)c->priority_eps);
   REQ(c->dueling == 0 || c->dueling == 1, "apex_learner: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", (int)c->dueling);
-  return 0;
+  return check_cat_head("apex_learner", c->num_atoms, c->v_min, c->v_max, c->dueling);
 }
 
 extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* params, float* grads, float* exp_avg, float* exp_avg_sq,
@@ -1002,7 +1036,7 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   REQ(!misaligned(params, 16) && !misaligned(grads, 16) && !misaligned(exp_avg, 16) && !misaligned(exp_avg_sq, 16) &&
       !misaligned(target_params, 16), "apex_learner_create: flat buffers must be 16-byte aligned");
   int64_t off[12];
-  const int64_t np = apex_layout(cfg->A, cfg->dueling, off, nullptr);
+  const int64_t np = apex_layout(cfg->A, cfg->dueling, cfg->num_atoms, off, nullptr);
   const Span s[5] = {{params, np * 4, true, "params"}, {grads, np * 4, true, "grads"}, {exp_avg, np * 4, true, "exp_avg"},
                      {exp_avg_sq, np * 4, true, "exp_avg_sq"}, {target_params, np * 4, true, "target_params"}};
   rc = check_spans(s, 5, "apex_learner_create");
@@ -1015,6 +1049,7 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   L->Wq = params + off[8]; L->bq = params + off[9]; L->Wt = target_params + off[8]; L->bt = target_params + off[9];
   L->gWq = grads + off[8]; L->gbq = grads + off[9];
   if (cfg->dueling) { L->bqa = params + off[11]; L->bta = target_params + off[11]; L->gbqa = grads + off[11]; }
+  if (cfg->num_atoms) L->cs = cat_support(cfg->num_atoms, cfg->v_min, cfg->v_max);
   rc = srl_encoder_create(cfg->precision, &L->E);
   if (!rc) rc = srl_encoder_create(cfg->precision, &L->Eq);
   if (rc) return undo(rc);
@@ -1056,15 +1091,30 @@ extern "C" int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, 
   if (!rc && c.double_dqn) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->w8, L->saved_n, L->enc_scratch, L->core_n, stream);
   if (!rc) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->t8, L->saved_n, L->enc_scratch, L->core_nt, stream);
   if (rc) return rc;
-  DqnTail t;
-  t.core_s = L->core_s; t.core_n = c.double_dqn ? L->core_n : nullptr; t.core_nt = L->core_nt;
-  t.Wq = L->Wq; t.bq = L->bq; t.Wt = L->Wt; t.bt = L->bt;
-  t.action = action; t.reward = reward; t.done = done; t.weight = weights;
-  t.B = B; t.A = c.A; t.gamma = c.gamma; t.two_over_B = 2.f / (float)B; t.priority_eps = c.priority_eps;
-  t.q = L->q; t.y = L->y; t.dq = L->dq; t.dcore = L->dcore; t.loss = L->loss; t.scratch = L->tail_scratch; t.prio = L->prio;
-  t.bqa = L->bqa; t.bta = L->bta; t.dueling = c.dueling;
-  CU(launch_dqn_tail(t, st), "dqn_tail");
-  CU(launch_dqn_wgrad(L->dq, action, L->core_s, B, c.A, L->head_part, L->gWq, L->gbq, L->gbqa, st), "dqn_wgrad");
+  if (c.num_atoms) {       // the categorical head: the three logit sets, the projection / cross-entropy tail, the head gradients
+    const int R = c.A * c.num_atoms;
+    CU(launch_cat_logits(L->core_s, L->Wq, L->bq, B, R, L->logits_s, st), "cat_logits");
+    if (c.double_dqn) CU(launch_cat_logits(L->core_n, L->Wq, L->bq, B, R, L->logits_n, st), "cat_logits");
+    CU(launch_cat_logits(L->core_nt, L->Wt, L->bt, B, R, L->logits_nt, st), "cat_logits");
+    CatTail t;
+    t.logits_s = L->logits_s; t.logits_n = c.double_dqn ? L->logits_n : nullptr; t.logits_nt = L->logits_nt; t.W = L->Wq;
+    t.action = action; t.reward = reward; t.done = done; t.weight = weights;
+    t.B = B; t.A = c.A; t.c = L->cs; t.gamma = c.gamma; t.inv_B = 1.f / (float)B; t.priority_eps = c.priority_eps;
+    t.q = L->q; t.y = L->y; t.ce = L->ce; t.m = L->mproj; t.dlogits = L->dlogits; t.dcore = L->dcore; t.loss = L->loss;
+    t.scratch = L->tail_scratch; t.prio = L->prio;
+    CU(launch_cat_tail(t, st), "cat_tail");
+    CU(launch_cat_wgrad(L->dlogits, L->core_s, B, R, L->gWq, L->gbq, st), "cat_wgrad");
+  } else {
+    DqnTail t;
+    t.core_s = L->core_s; t.core_n = c.double_dqn ? L->core_n : nullptr; t.core_nt = L->core_nt;
+    t.Wq = L->Wq; t.bq = L->bq; t.Wt = L->Wt; t.bt = L->bt;
+    t.action = action; t.reward = reward; t.done = done; t.weight = weights;
+    t.B = B; t.A = c.A; t.gamma = c.gamma; t.two_over_B = 2.f / (float)B; t.priority_eps = c.priority_eps;
+    t.q = L->q; t.y = L->y; t.dq = L->dq; t.dcore = L->dcore; t.loss = L->loss; t.scratch = L->tail_scratch; t.prio = L->prio;
+    t.bqa = L->bqa; t.bta = L->bta; t.dueling = c.dueling;
+    CU(launch_dqn_tail(t, st), "dqn_tail");
+    CU(launch_dqn_wgrad(L->dq, action, L->core_s, B, c.A, L->head_part, L->gWq, L->gbq, L->gbqa, st), "dqn_wgrad");
+  }
   rc = srl_encoder_backward(L->E, L->dcore, B, 1, L->saved_s, L->enc_scratch, L->g8, stream);
   if (rc) return rc;
   const OptStep o = {1, L->params, L->grads, L->m, L->v, L->nparams, c.max_grad_norm, L->coef, L->opt_scratch, c.learning_rate,
@@ -1109,7 +1159,10 @@ extern "C" int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* o
     rc = srl_encoder_forward(L->Eq, obs + (size_t)f0 * 28224, L->zero_reward, L->zero_action, f, 1, L->w8, L->saved_q, L->scratch_q,
                              L->core_q, stream);
     if (rc) return rc;
-    CU(launch_dqn_q_values(L->core_q, L->Wq, L->bq, L->bqa, f, A, q_out + (size_t)f0 * A, (cudaStream_t)stream), "dqn_q_values");
+    if (L->cfg.num_atoms)
+      CU(launch_cat_q_values(L->core_q, L->Wq, L->bq, f, A, L->cs, L->logits_q, q_out + (size_t)f0 * A, (cudaStream_t)stream), "cat_q_values");
+    else
+      CU(launch_dqn_q_values(L->core_q, L->Wq, L->bq, L->bqa, f, A, q_out + (size_t)f0 * A, (cudaStream_t)stream), "dqn_q_values");
   }
   return 0;
 }

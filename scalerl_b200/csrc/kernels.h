@@ -247,6 +247,42 @@ cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* 
                                 cudaStream_t st);
 cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
 
+// ---- dqn_cat.cu: the categorical (C51) Q head, q = Linear(512, A K), K atoms on the support z_k = v_min + k dz (dqn_cat.cuh)
+constexpr int CAT_MAX_ATOMS = 64;
+struct CatSupport {
+  float v_min, v_max, dz;
+  int K;
+};
+// dz = (v_max - v_min) / (K - 1) in double, rounded once to fp32
+inline CatSupport cat_support(int K, float v_min, float v_max) {
+  return {v_min, v_max, (float)(((double)v_max - (double)v_min) / (double)(K - 1)), K};
+}
+// api.cu: the checks of a head setting shared by the learner and the actor (num_atoms 0: a scalar head, nothing else is read).  0, or
+// SRL_EINVAL with "<who>: ..." as the message
+int check_cat_head(const char* who, int num_atoms, float v_min, float v_max, int dueling);
+// one batch of B transitions on the categorical head: the logits [B][A K] of the online network over s, of the online network over s'
+// (null: no double DQN) and of the target network over s'; the online head weights W [A K][512] (dcore); the batch columns; outputs q
+// (sum z p at the taken action), y (sum z m), ce f32 [B], m f32 [B][K], dlogits f32 [B][A K] (zero outside the taken action's K
+// rows), dcore f32 [B][ENC_CORE], priorities f64 [B] and loss f32 [1] = mean(w ce); scratch as DqnTail's
+struct CatTail {
+  const float *logits_s, *logits_n, *logits_nt, *W;
+  const int64_t* action; const float* reward; const uint8_t* done; const float* weight;
+  int B, A;
+  CatSupport c;
+  float gamma, inv_B, priority_eps;
+  float *q, *y, *ce, *m, *dlogits, *dcore, *loss, *scratch;
+  double* prio;
+};
+cudaError_t launch_cat_tail(const CatTail& t, cudaStream_t st);
+// logits [N][R] = h W^T + b over N core rows (stride ENC_CORE), W [R][512]: one fmaf chain per logit over j = 0 .. 511 from 0, then
+// + b rounded once, whatever the tiling
+cudaError_t launch_cat_logits(const float* core, const float* W, const float* b, int N, int R, float* logits, cudaStream_t st);
+// gW [R][512] = dlogits^T h, gb [R] = dlogits^T 1 over the N core rows (stored), each a fmaf chain over n = 0 .. N-1 in order
+cudaError_t launch_cat_wgrad(const float* dlogits, const float* core, int N, int R, float* gW, float* gb, cudaStream_t st);
+// q_out [N][A] = the expected Q of the categorical head over N core rows, through logits [N][A K]
+cudaError_t launch_cat_q_values(const float* core, const float* W, const float* b, int N, int A, const CatSupport& c, float* logits,
+                                float* q_out, cudaStream_t st);
+
 }  // namespace srl
 struct srl_per;
 struct srl_apex_actor;

@@ -4,9 +4,12 @@ priorities into a GpuPrioritizedSampler of its own.  Rounds alternate between th
 printed with the card's name and power limit, one JSON line per configuration.
 
 With --dueling the learner runs the dueling head (ApexHParams(dueling_dqn=True)) beside the plain one, alternated in the same rounds,
-and the torch statements use AtariQNet(A, dueling=True).
+and the torch statements use AtariQNet(A, dueling=True).  With --categorical it runs the categorical head (ApexHParams(categorical_dqn=True,
+num_atoms=--atoms, v_min=-10, v_max=10)) beside the plain one, the torch statements become C51's (projection, cross-entropy, KL
+priorities) on AtariQNet(A, categorical=True), and a last line gives the head kernels' times from torch.profiler at B = 512, A = 18
+with their FLOP rate against the fp32 data-sheet rate (67 TFLOP/s).
 
-    python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18] [--dueling]
+    python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18] [--dueling | --categorical [--atoms 51]]
 """
 import argparse
 import json
@@ -16,12 +19,14 @@ import sys
 import time
 
 import torch
+import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from scalerl_b200.algorithms.apex import ApexHParams, AtariQNet, B200ApexLearner, default_q_state_dict  # noqa: E402
 from scalerl_b200.data.per_sampler import GpuPrioritizedSampler  # noqa: E402
 
 MEMORY = 4096        # sampler capacity: the sampled indices' range
+V_MIN, V_MAX = -10.0, 10.0      # the categorical support (Atari rewards clipped to [-1, 1])
 
 
 def card():
@@ -52,9 +57,11 @@ class TorchStep:
     """the reference's statements on torch/cuDNN (the priorities stay on the device and go into the GPU sampler).  The object owns
     every tensor the step reads or writes, so a captured replay of it stays valid as long as the object lives."""
 
-    def __init__(self, B, A, exp, w, idxs, gamma=0.99, dueling=False):
-        sd = default_q_state_dict(A, dueling=dueling)
-        self.model, self.target = AtariQNet(A, dueling=dueling).cuda(), AtariQNet(A, dueling=dueling).cuda()
+    def __init__(self, B, A, exp, w, idxs, gamma=0.99, dueling=False, atoms=0):
+        sd = default_q_state_dict(A, dueling=dueling, num_atoms=atoms)
+        net = lambda: AtariQNet(A, dueling=dueling, categorical=atoms > 0, num_atoms=atoms or 51, v_min=V_MIN, v_max=V_MAX).cuda()
+        self.model, self.target, self.A, self.K = net(), net(), A, atoms
+        self.rows = torch.arange(B, device='cuda')
         self.model.load_state_dict(sd)
         self.target.load_state_dict(sd)
         self.opt = torch.optim.Adam(self.model.parameters(), lr=1e-3, capturable=True)
@@ -65,6 +72,8 @@ class TorchStep:
         self.prio = torch.empty(B, dtype=torch.float64, device='cuda')
 
     def __call__(self):
+        if self.K:
+            return self.c51()
         current_q_values = self.model(self.obs).gather(1, self.actions)                       # worker.py:148
         with torch.no_grad():
             next_q_values = self.target(self.nobs).max(1, keepdim=True)[0]                    # :149
@@ -75,6 +84,62 @@ class TorchStep:
         loss.backward()
         self.opt.step()
         self.S.update_priorities(self.idxs, self.prio, validate=False)
+
+    def c51(self):
+        """the categorical update (Bellemare et al. 2017, Algorithm 1) in torch statements, KL priorities"""
+        A, K, z = self.A, self.K, self.model.support
+        dz = z[1] - z[0]
+        logp = F.log_softmax(self.model.q(self.model._features(self.obs)).view(-1, A, K), dim=2)[self.rows, self.actions[:, 0]]
+        with torch.no_grad():
+            pt = F.softmax(self.target.q(self.target._features(self.nobs)).view(-1, A, K), dim=2)
+            pn = pt[self.rows, (pt * z).sum(2).argmax(1)]
+            tz = (self.rewards + (1 - self.dones) * self.gamma * z).clamp(V_MIN, V_MAX)
+            b = (tz - V_MIN) / dz
+            lo, up = b.floor().long().clamp(0, K - 1), b.ceil().long().clamp(0, K - 1)
+            m = torch.zeros_like(pn)
+            m.scatter_add_(1, lo, pn * (up.float() - b) + pn * (lo == up).float())
+            m.scatter_add_(1, up, pn * (b - lo.float()))
+        ce = -(m * logp).sum(1)
+        self.prio.copy_((torch.xlogy(m, m) - m * logp.detach()).sum(1).clamp(min=0))
+        loss = (self.weights[:, 0] * ce).mean()
+        self.opt.zero_grad(set_to_none=False)
+        loss.backward()
+        self.opt.step()
+        self.S.update_priorities(self.idxs, self.prio, validate=False)
+
+
+def head_profile(atoms, B=512, A=18, steps=20):
+    """the categorical head's kernels in one captured learner step (torch.profiler over `steps` replays): mean µs per step and the
+    GEMMs' FLOP rate against the fp32 data-sheet rate"""
+    from torch.profiler import ProfilerActivity, profile
+    exp, w, idxs = batch(B, A)
+    L, S = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, categorical_dqn=True, num_atoms=atoms, v_min=V_MIN, v_max=V_MAX)), sampler()
+    step = lambda: L.learn(exp, weights=w, idxs=idxs, sampler=S, sync_stats=False)
+    for _ in range(3):
+        step()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            step()
+        torch.cuda.synchronize()
+    R = A * atoms
+    flops = {'cat_gemm_kernel<false>': 2.0 * B * R * 512 * 2, 'cat_gemm_kernel<true>': 2.0 * B * R * 513}    # two logit sets: s, s' target
+    out, total = {}, 0.0
+    for e in prof.key_averages():
+        if 'cat_' not in e.key:
+            continue
+        us = e.device_time_total / steps
+        name = 'cat_gemm_kernel<true>' if 'Lb1' in e.key or '<true>' in e.key else ('cat_gemm_kernel<false>' if 'gemm' in e.key else e.key.split('(')[0])
+        out[name] = {'us_per_step': us}
+        if name in flops:
+            out[name]['tflops'] = flops[name] / us * 1e-6
+            out[name]['fraction_of_67_tflops'] = flops[name] / us * 1e-6 / 67.0
+        total += us
+    step_us = 1e6 / timed(step, 50)
+    L.release_graphs()
+    L.close()
+    return {'card': card(), 'B': B, 'A': A, 'K': atoms, 'head_kernels': out, 'head_us_per_step': total, 'step_us': step_us,
+            'head_share_of_step': total / step_us}
 
 
 class Captured:
@@ -111,7 +176,12 @@ def main():
     ap.add_argument('--steps', type=int, default=50)
     ap.add_argument('--configs', default='32x6,32x18,512x6,512x18')
     ap.add_argument('--dueling', action='store_true', help='add the dueling learner and run the torch statements on the dueling net')
+    ap.add_argument('--categorical', action='store_true', help='add the categorical learner and run C51 in torch statements')
+    ap.add_argument('--atoms', type=int, default=51)
     a = ap.parse_args()
+    if a.dueling and a.categorical:
+        sys.exit('--dueling and --categorical are separate comparisons: pass one')
+    atoms = a.atoms if a.categorical else 0
     if not torch.cuda.is_available():
         sys.exit('bench_apex.py measures on a CUDA device; none is present')
     name = card()
@@ -125,8 +195,13 @@ def main():
             LD, SD = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, dueling_dqn=True)), sampler()
             learners.append(LD)
             variants['b200_dueling_captured'] = lambda: LD.learn(exp, weights=w, idxs=idxs, sampler=SD, sync_stats=False)
-        variants['torch_eager'] = TorchStep(B, A, exp, w, idxs, dueling=a.dueling)
-        variants['torch_captured'] = Captured(TorchStep(B, A, exp, w, idxs, dueling=a.dueling))
+        if atoms:
+            LC = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, categorical_dqn=True, num_atoms=atoms, v_min=V_MIN, v_max=V_MAX))
+            SC = sampler()
+            learners.append(LC)
+            variants['b200_categorical_captured'] = lambda: LC.learn(exp, weights=w, idxs=idxs, sampler=SC, sync_stats=False)
+        variants['torch_eager'] = TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms)
+        variants['torch_captured'] = Captured(TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms))
         for fn in variants.values():           # warm-up: the learner's first call runs eagerly, the second captures
             for _ in range(3):
                 fn()
@@ -134,7 +209,8 @@ def main():
         for _ in range(a.rounds):
             for k, fn in variants.items():
                 rates[k].append(timed(fn, a.steps))
-        out = {'card': name, 'B': B, 'A': A, 'precision': 'bf16', 'torch_net': 'dueling' if a.dueling else 'plain', 'rounds': a.rounds,
+        torch_net = 'dueling' if a.dueling else (f'categorical K={atoms}' if atoms else 'plain')
+        out = {'card': name, 'B': B, 'A': A, 'precision': 'bf16', 'torch_net': torch_net, 'rounds': a.rounds,
                'steps_per_round': a.steps}
         for k, r in rates.items():
             r = sorted(r)
@@ -145,6 +221,8 @@ def main():
         for x in learners:
             x.release_graphs()
             x.close()
+    if atoms:
+        print(json.dumps(head_profile(atoms)), flush=True)
 
 
 if __name__ == '__main__':
