@@ -292,6 +292,9 @@ int srl_lstm_forward(srl_lstm_t* L, const float* core, const uint8_t* done, cons
                      float* hT, float* cT, void* stream);
 int srl_lstm_backward(srl_lstm_t* L, const float* dout, const uint8_t* done, float* dcore, void* stream);
 const char* srl_lstm_last_error(void);
+/* Address and element count of one of the context's device rows (tests only; no CUDA call), named as srl_lstm_core_debug_buffer's.
+ * The backward covers the first (T1-1)*B rows, so "dgates" and "dx" have that many; "done" is unused (the caller passes its own). */
+int srl_lstm_debug_buffer(srl_lstm_t* L, const char* name, int layer, void** ptr, int64_t* count);
 
 /* ---- stand-alone LSTM core: the trainable AtariNet's use_lstm=True core under autograd ---------------------------------------
  * The same kernels as srl_lstm_*, on two caller-owned blocks as srl_encoder_*: `saved` is written by the forward and read by its
@@ -303,7 +306,18 @@ const char* srl_lstm_last_error(void);
  *           hT/cT f32 [2,B,H] (the state after row T1-1).
  * backward: dout f32 [T1,B,H] (every row, the last included), dhT/dcT f32 [2,B,H] (gradients of hT/cT; NULL = zero)
  *           -> grads8 (the 8 tensors' gradients, OVERWRITTEN), dcore f32 [T1,B,H], dh0/dc0 f32 [2,B,H] (gradients of h0/c0; NULL = not
- *           wanted, which skips their extra GEMM). */
+ *           wanted, which skips their extra GEMM).
+ * debug_buffer (tests only; host arithmetic, no CUDA call): address and element count of one row of the blocks of a call with the same
+ * T1, B, A.  Hp = H rounded up to 64, G = 4Hp, N1 = T1*B; per-layer rows take layer 0 or 1, every other row layer 0.
+ *   saved:   "xin0" bf16 [N1][Hp] (layer 0's input; layer 1's is hbf of layer 0), per layer "hm" bf16 [N1][Hp] (m_t . h_{t-1}),
+ *            "hbf" bf16 [N1][Hp] (h_t), "Wih"/"Whh" bf16 [4][Hp][Hp] (gate-major, zero padded), "WihT"/"WhhT" bf16 [Hp][G] (transposes),
+ *            "gates" f32 [N1][4][Hp] (activations i, f, g, o), "cseq" f32 [N1][Hp] (c_t); "c_init" f32 [2][B][Hp] (columns [H, Hp) are
+ *            never written), "done" u8 [N1].
+ *   scratch: "gx" f32 [N1][G], "r" f32 [B][G], per layer "hseq" f32 [N1][Hp], "dgates" bf16 [N1][G]; "dx" f32 [N1][Hp],
+ *            "dwpad" f32 [G][Hp], "dc"/"dhm" f32 [B][Hp], "bias_part" f32 [ceil(N1/64)][G].  After a backward, dgates of each layer and
+ *            (layer 0's input gradient, padded) dx hold its results; the rest are the last step's temporaries. */
+int srl_lstm_core_debug_buffer(int T1, int B, int A, void* saved, void* scratch, const char* name, int layer, void** ptr,
+                               int64_t* count);
 int srl_lstm_core_sizes(int T1, int B, int A, int64_t* saved_bytes, int64_t* scratch_bytes);
 int srl_lstm_core_forward(const float* core, const uint8_t* done, const float* h0, const float* c0, int A, int T1, int B,
                           const float* const* weights8, void* saved, void* scratch, float* out, float* hT, float* cT, void* stream);

@@ -66,6 +66,8 @@ _SIGS = {
     'srl_lstm_core_sizes': [_I, _I, _I, C.POINTER(_L), C.POINTER(_L)],
     'srl_lstm_core_forward': [_P, _P, _P, _P, _I, _I, _I, C.POINTER(_P), _P, _P, _P, _P, _P, _P],
     'srl_lstm_core_backward': [_P, _P, _P, _I, _I, _I, _P, _P, C.POINTER(_P), _P, _P, _P, _P],
+    'srl_lstm_core_debug_buffer': [_I, _I, _I, _P, _P, C.c_char_p, _I, C.POINTER(_P), C.POINTER(_L)],
+    'srl_lstm_debug_buffer': [_P, C.c_char_p, _I, C.POINTER(_P), C.POINTER(_L)],
     'srl_per_create': [_L, C.c_double, C.POINTER(_P)],
     'srl_per_destroy': [_P],
     'srl_per_add': [_P, _L, _P],

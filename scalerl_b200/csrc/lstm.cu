@@ -13,6 +13,7 @@
 // H = 513 + A is padded to Hp (multiple of 64); the gate dimension is laid out [4][Hp] so every GEMM has K = Hp or 4Hp.
 // All GEMM operands are bf16 (fp32 accumulate); cell state, gate activations and gradients are fp32.
 // The actor's single step (one row of B environments, no BPTT) has its own fused kernel further down (lstm_step_kernel).
+#include <cstring>
 #include <new>
 #include "tma_problems.cuh"
 #include "kernels.h"
@@ -457,6 +458,16 @@ static int lstm_rows(LstmBuffers& b, const LstmDims& d, WsRow* t) {
   t[n++] = ws_row("bias_part", (NB + LSTM_BIAS_CHUNK - 1) / LSTM_BIAS_CHUNK * G, &b.bias_part);
   return n;
 }
+// the layer-th row of a carved table called `name` (the per-layer rows appear once per layer, l = 0 first; every other row once)
+static int lstm_find_row(const WsRow* t, const char* name, int layer, void** ptr, int64_t* count, const char* what) {
+  int seen = 0;
+  for (int i = 0; i < LSTM_ROWS; ++i) {
+    if (strcmp(t[i].name, name) != 0) continue;
+    if (seen++ == layer) { *ptr = *t[i].hi; *count = t[i].count; return 0; }
+  }
+  if (!seen) return fail(SRL_EINVAL, "%s: unknown buffer '%s'", what, name);
+  return fail(SRL_EINVAL, "%s: '%s' exists for layer 0%s only, not layer=%d", what, name, seen > 1 ? " and 1" : "", layer);
+}
 
 struct LstmMaps {
   CUtensorMap xin[2], hm[2], hm64[2], xin64[2], Wih[2], Whh[2], WihT[2], WhhT[2], dg128[2], dg64[2];
@@ -607,6 +618,15 @@ extern "C" int srl_lstm_backward(srl_lstm_t* L, const float* dout, const uint8_t
   return lstm_backward_rows(L->d, L->b, L->m, L->g, done, dout, nullptr, nullptr, dcore, nullptr, nullptr, (cudaStream_t)stream);
 }
 
+extern "C" int srl_lstm_debug_buffer(srl_lstm_t* L, const char* name, int layer, void** ptr, int64_t* count) {
+  REQ(L && name && ptr && count, "lstm_debug_buffer: NULL argument");
+  LstmBuffers b = {};
+  WsRow t[LSTM_ROWS];
+  lstm_rows(b, L->d, t);
+  carve_rows(t, LSTM_ROWS, false, L->arena);          // the same table and arena as srl_lstm_create: the same addresses
+  return lstm_find_row(t, name, layer, ptr, count, "lstm_debug_buffer");
+}
+
 // ------------------------------------------------------------------------------------------------ stand-alone core on caller-owned blocks
 static int check_core_shape(int T1, int B, int A, const char* what) {
   REQ(T1 >= 1 && B >= 1 && (int64_t)T1 * B <= MAX_FRAMES, "%s: T1=%d B=%d: need T1 >= 1, B >= 1 and T1*B <= %d", what, T1, B, MAX_FRAMES);
@@ -633,6 +653,21 @@ static int check_core_call(int T1, int B, int A, const void* saved, const void* 
   if (rc) return rc;
   REQ(!misaligned(saved, 256) && !misaligned(scratch, 256), "%s: saved and scratch must be 256-byte aligned", what);
   return srl_lstm_core_sizes(T1, B, A, sb, kb);
+}
+
+// host arithmetic only (no CUDA call): the blocks are carved as core_call_setup carves them
+extern "C" int srl_lstm_core_debug_buffer(int T1, int B, int A, void* saved, void* scratch, const char* name, int layer, void** ptr,
+                                          int64_t* count) {
+  REQ(saved && scratch && name && ptr && count, "lstm_core_debug_buffer: NULL argument");
+  int64_t sb = 0, kb = 0;
+  const int rc = check_core_call(T1, B, A, saved, scratch, &sb, &kb, "lstm_core_debug_buffer");
+  if (rc) return rc;
+  LstmBuffers b = {};
+  WsRow t[LSTM_ROWS];
+  lstm_rows(b, lstm_dims(T1, B, 513 + A, (int64_t)T1 * B), t);
+  carve_rows(t, LSTM_SAVED_ROWS, false, static_cast<char*>(saved));
+  carve_rows(t + LSTM_SAVED_ROWS, LSTM_ROWS - LSTM_SAVED_ROWS, false, static_cast<char*>(scratch));
+  return lstm_find_row(t, name, layer, ptr, count, "lstm_core_debug_buffer");
 }
 
 // the blocks of one call -> the buffers and their tensor maps, encoded on the host for this call (legal under stream capture)

@@ -126,6 +126,58 @@ def test_backward_rejects_bad_arguments_before_any_cuda_call(lib):
     assert _rejects(_bwd(L, g=(C.c_void_p * 8)(*([_at(0)] + g[1:]))), L, 'overlaps dout')
 
 
+def _lookup(L, name, layer=0, T1=5, B=3, A=6, saved=_at(4), scratch=_at(5)):
+    p, n = C.c_void_p(), C.c_int64()
+    rc = L.srl_lstm_core_debug_buffer(T1, B, A, saved, scratch, name.encode() if name is not None else None, layer, C.byref(p), C.byref(n))
+    return rc, (p.value or 0), n.value
+
+
+def test_debug_buffer_rejects_bad_arguments_before_any_cuda_call(lib):
+    L = lib
+    assert _rejects(_lookup(L, 'gates', saved=None)[0], L, 'NULL') and _rejects(_lookup(L, None)[0], L, 'NULL')
+    p, n = C.c_void_p(), C.c_int64()
+    assert _rejects(L.srl_lstm_core_debug_buffer(5, 3, 6, _at(4), _at(5), b'gates', 0, None, C.byref(n)), L, 'NULL')
+    assert _rejects(L.srl_lstm_debug_buffer(None, b'gates', 0, C.byref(p), C.byref(n)), L, 'NULL')
+    for name in ('nope', 'gate', 'gates_lo', '', 'Hm'):
+        assert _rejects(_lookup(L, name)[0], L, 'unknown buffer'), name
+    for name, layer in (('gates', 2), ('gates', -1), ('hm', 7), ('xin0', 1), ('done', 1), ('dc', -1)):
+        assert _rejects(_lookup(L, name, layer)[0], L, f'layer={layer}'), (name, layer)
+    for T1, B, A in ((0, 3, 6), (5, 0, 6), (65537, 1, 6), (5, 3, 0), (5, 3, 32)):
+        assert _rejects(_lookup(L, 'gates', T1=T1, B=B, A=A)[0], L, 'lstm_core_debug_buffer'), (T1, B, A)
+    assert _rejects(_lookup(L, 'gates', saved=_at(4) + 32)[0], L, 'aligned')
+
+
+@pytest.mark.parametrize('T1,B,A', [(5, 3, 6), (1, 7, 6), (2, 130, 31), (9, 128, 1), (101, 16, 6)])
+def test_debug_buffer_rows_follow_the_table(lib, T1, B, A):
+    """every named row: its count from the shapes, 256-byte aligned, inside the block srl_lstm_core_sizes reports, no two rows overlapping,
+    and the saved / scratch split of the table"""
+    from tests import lstm_ref as R
+    L = lib
+    H = R.hidden(A)
+    Hp, N1 = R.padded(H), T1 * B
+    G = 4 * Hp
+    want = {'xin0': N1 * Hp, 'hm': N1 * Hp, 'hbf': N1 * Hp, 'Wih': G * Hp, 'WihT': G * Hp, 'Whh': G * Hp, 'WhhT': G * Hp, 'gates': N1 * G,
+            'cseq': N1 * Hp, 'c_init': 2 * B * Hp, 'done': N1, 'gx': N1 * G, 'r': B * G, 'hseq': N1 * Hp, 'dgates': N1 * G, 'dx': N1 * Hp,
+            'dwpad': G * Hp, 'dc': B * Hp, 'dhm': B * Hp, 'bias_part': (N1 + 63) // 64 * G}
+    assert set(want) == set(R.LAYER_ROWS) | set(R.SHARED_ROWS)
+    sb, kb = lstm_block_sizes(T1, B, A)
+    spans = []
+    for name in want:
+        for layer in ((0, 1) if name in R.LAYER_ROWS else (0,)):
+            rc, p, n = _lookup(L, name, layer, T1, B, A)
+            assert rc == 0, (name, layer, _err(L))
+            assert n == want[name], (name, n, want[name])
+            assert p % 256 == 0, name
+            base, size = (_at(4), sb) if p < _at(5) else (_at(5), kb)
+            end = p + n * R.row_dtype(name).itemsize
+            assert base <= p and end <= base + size, (name, layer)
+            saved = name in ('xin0', 'c_init', 'done') or (name in R.LAYER_ROWS and name not in ('hseq', 'dgates'))
+            assert (base == _at(4)) == saved, name
+            spans.append((p, end, name, layer))
+    spans.sort()
+    assert all(a[1] <= b[0] for a, b in zip(spans, spans[1:])), 'rows overlap'
+
+
 def test_errors_are_reported_by_srl_last_error(lib):
     """the LSTM core reports through the library's one message: srl_lstm_last_error returns what srl_last_error does"""
     L = lib
