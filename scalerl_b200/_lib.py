@@ -226,6 +226,17 @@ def apex_param_layout(A, dueling=False, num_atoms=0):
     return int(total), [int(x) for x in off][:n], [int(x) for x in cnt][:n]
 
 
+def apex_actor_create(A, num_envs, precision, seed, params, head) -> C.c_void_p:
+    """srl_apex_actor_create_ex / _cat for ``head`` (dueling, num_atoms, v_min, v_max) on the device buffer at ``params``"""
+    h = C.c_void_p()
+    if head.num_atoms:
+        check(lib().srl_apex_actor_create_cat(A, num_envs, precision, head.num_atoms, head.v_min, head.v_max, seed, params, C.byref(h)),
+              'srl_apex_actor_create_cat')
+    else:
+        check(lib().srl_apex_actor_create_ex(A, num_envs, precision, int(head.dueling), seed, params, C.byref(h)), 'srl_apex_actor_create_ex')
+    return h
+
+
 def param_layout(A, use_lstm=False):
     """(total floats, offsets, counts) of the flat parameter buffer; 12 AtariNet tensors (+ 8 nn.LSTM tensors with use_lstm)"""
     off = (_L * 20)()

@@ -27,7 +27,7 @@ import numpy as np
 import torch
 
 from ... import _lib
-from .learner import MAX_FRAMES, apex_param_shapes, check_categorical, default_q_state_dict, flat_views, load_views
+from .learner import MAX_FRAMES, QHead, default_q_state_dict, flat_views, load_views
 
 PRECISIONS = {'bf16': 0, 'fp32_split': 1}
 
@@ -48,6 +48,8 @@ class B200ApexActor:
     the learner's; ``priority_eps`` (> 0) is added to every priority the actor computes; ``dueling_dqn``, ``categorical_dqn`` (with
     ``v_min``, ``v_max``, ``num_atoms``): the learner's head.  Calls run on the current stream and share the actor's buffers: issue them
     from one stream."""
+    # the head settings as the constructor stores them; the class values are its defaults
+    dueling_dqn, categorical_dqn, v_min, v_max, num_atoms = False, False, 0.0, 200.0, 51
 
     def __init__(self, num_envs: int, num_actions: int, epsilons=None, seed: int = 0, precision: str = 'bf16', priority_eps: float = 1e-6,
                  device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None, dueling_dqn: bool = False,
@@ -59,41 +61,32 @@ class B200ApexActor:
             raise ValueError(f'seed must be an int in [0, 2**64), got {seed!r}')
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be 'bf16' or 'fp32_split', got {precision!r}")
-        if not isinstance(dueling_dqn, bool):
-            raise ValueError(f'dueling_dqn must be a bool, got {dueling_dqn!r}')
-        if not isinstance(categorical_dqn, bool):
-            raise ValueError(f'categorical_dqn must be a bool, got {categorical_dqn!r}')
-        check_categorical(num_atoms, v_min, v_max)
-        if categorical_dqn and dueling_dqn:
-            raise ValueError('categorical_dqn with dueling_dqn is not supported: choose one head')
+        head = QHead.of(dueling_dqn, categorical_dqn, num_atoms, v_min, v_max)
         priority_eps = float(priority_eps)
         if not (math.isfinite(priority_eps) and priority_eps > 0.0):
             raise ValueError(f'priority_eps must be finite and > 0 (a zero leaf makes the sampler\'s IS weight infinite), got {priority_eps}')
         self.num_envs, self.num_actions, self.seed, self.precision = int(num_envs), int(num_actions), int(seed), precision
         self.priority_eps, self.dueling_dqn, self.categorical_dqn = priority_eps, dueling_dqn, categorical_dqn
         self.v_min, self.v_max, self.num_atoms = float(v_min), float(v_max), int(num_atoms)
-        atoms = self.num_atoms if categorical_dqn else 0
         eps = self._epsilons(apex_epsilons(self.num_envs) if epsilons is None else epsilons)
         if not torch.cuda.is_available():
             raise RuntimeError('B200ApexActor needs a CUDA device: scalerl_b200 has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._L = _lib.lib()
-        self.shapes = apex_param_shapes(self.num_actions, dueling_dqn, atoms)
+        self.shapes = head.shapes(self.num_actions)
         with torch.cuda.device(self.device):
-            total, off, cnt = _lib.apex_param_layout(self.num_actions, dueling_dqn, atoms)
+            total, off, cnt = head.layout(self.num_actions)
             self.flat_params = torch.zeros(total, dtype=torch.float32, device=self.device)
             self.params = flat_views(self.flat_params, off, cnt, self.shapes)
             self.epsilons = eps.to(self.device)           # read by the act kernel when it runs
-            h = C.c_void_p()
-            if atoms:
-                _lib.check(self._L.srl_apex_actor_create_cat(self.num_actions, self.num_envs, PRECISIONS[precision], atoms, self.v_min, self.v_max,
-                                                             self.seed, self.flat_params.data_ptr(), C.byref(h)), 'srl_apex_actor_create_cat')
-            else:
-                _lib.check(self._L.srl_apex_actor_create_ex(self.num_actions, self.num_envs, PRECISIONS[precision], int(dueling_dqn), self.seed,
-                                                            self.flat_params.data_ptr(), C.byref(h)), 'srl_apex_actor_create_ex')
-            self._h = h
-        self.load_state_dict(default_q_state_dict(self.num_actions, self.seed, dueling_dqn, atoms) if init_state_dict is None else init_state_dict)
+            self._h = _lib.apex_actor_create(self.num_actions, self.num_envs, PRECISIONS[precision], self.seed, self.flat_params.data_ptr(), head)
+        sd = default_q_state_dict(self.num_actions, self.seed, head.dueling, head.num_atoms) if init_state_dict is None else init_state_dict
+        self.load_state_dict(sd)
         self.weights_version = 0
+
+    @property
+    def head(self) -> QHead:
+        return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max)
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
@@ -122,14 +115,8 @@ class B200ApexActor:
             raise ValueError(f'sync_from needs a B200ApexLearner, got {type(learner).__name__}')
         if learner.hp.num_actions != self.num_actions:
             raise ValueError(f'the learner has num_actions={learner.hp.num_actions}, the actor {self.num_actions}')
-        if learner.hp.dueling_dqn != self.dueling_dqn:
-            raise ValueError(f'the learner has dueling_dqn={learner.hp.dueling_dqn}, the actor {self.dueling_dqn}')
-        if learner.hp.categorical_dqn != self.categorical_dqn:
-            raise ValueError(f'the learner has categorical_dqn={learner.hp.categorical_dqn}, the actor {self.categorical_dqn}')
-        if self.categorical_dqn:
-            mine, theirs = (self.num_atoms, self.v_min, self.v_max), (learner.hp.num_atoms, float(learner.hp.v_min), float(learner.hp.v_max))
-            if mine != theirs:
-                raise ValueError(f'the learner has (num_atoms, v_min, v_max)={theirs}, the actor {mine}')
+        if learner.hp.head != self.head:
+            raise ValueError(f'the learner has {learner.hp.head}, the actor {self.head}')
         if learner.device != self.device:
             raise ValueError(f'the learner is on {learner.device}, the actor on {self.device}')
         self.flat_params.copy_(learner.flat_params)

@@ -150,13 +150,7 @@ class ApexHParams:
             raise ValueError(f'batch_size must be an int in [1, {MAX_FRAMES}], got {self.batch_size!r}')
         if not (isinstance(self.num_actions, int) and 1 <= self.num_actions <= 31):
             raise ValueError(f'num_actions must be an int in [1, 31], got {self.num_actions!r}')
-        if not isinstance(self.dueling_dqn, bool):
-            raise ValueError(f'dueling_dqn must be a bool, got {self.dueling_dqn!r}')
-        if not isinstance(self.categorical_dqn, bool):
-            raise ValueError(f'categorical_dqn must be a bool, got {self.categorical_dqn!r}')
-        check_categorical(self.num_atoms, self.v_min, self.v_max)
-        if self.categorical_dqn and self.dueling_dqn:
-            raise ValueError('categorical_dqn with dueling_dqn is not supported: choose one head')
+        self.head                            # ValueError on a bad head setting
         if not (math.isfinite(self.gamma) and self.gamma >= 0.0):
             raise ValueError(f'gamma must be finite and >= 0, got {self.gamma}')
         if not (math.isfinite(self.learning_rate) and self.learning_rate > 0.0):
@@ -175,6 +169,11 @@ class ApexHParams:
             raise ValueError(f'Adam betas must be in [0, 1), got ({self.adam_beta1}, {self.adam_beta2})')
         if not (math.isfinite(self.adam_eps) and self.adam_eps >= 0.0):
             raise ValueError(f'adam_eps must be finite and >= 0, got {self.adam_eps}')
+
+    @property
+    def head(self) -> 'QHead':
+        """the Q head these settings describe (ValueError on a bad one)"""
+        return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max)
 
     def to_c(self) -> _lib.SrlApexConfig:
         self.validate()
@@ -196,14 +195,46 @@ class ApexHParams:
         return self.num_atoms if self.categorical_dqn else 0
 
 
-def check_categorical(num_atoms, v_min, v_max) -> None:
-    """the categorical head's settings: num_atoms an int in [2, 64], v_min < v_max finite (also as fp32, as the kernels read them)"""
-    if isinstance(num_atoms, bool) or not isinstance(num_atoms, (int, np.integer)) or not 2 <= num_atoms <= 64:
-        raise ValueError(f'num_atoms must be an int in [2, 64], got {num_atoms!r}')
-    with np.errstate(over='ignore'):
-        lo, hi = np.float32(v_min), np.float32(v_max)
-    if not (np.isfinite(lo) and np.isfinite(hi) and lo < hi and np.isfinite(np.float32((float(hi) - float(lo)) / (num_atoms - 1)))):
-        raise ValueError(f'v_min and v_max must be finite fp32 values with v_min < v_max, got ({v_min}, {v_max})')
+@dataclass(frozen=True)
+class QHead:
+    """The Q head of the learner and its actors: q = Linear(512, A), the dueling head (``dueling``), or the categorical head on
+    ``num_atoms`` > 0 atoms of the support [v_min, v_max].  A scalar head keeps no support, so equal heads compare equal."""
+    dueling: bool = False
+    num_atoms: int = 0
+    v_min: float = 0.0
+    v_max: float = 0.0
+
+    @classmethod
+    def of(cls, dueling_dqn, categorical_dqn, num_atoms, v_min, v_max) -> 'QHead':
+        """the head of ApexHParams' / B200ApexActor's settings, checked (the support, as the kernels read it in fp32, even when
+        categorical_dqn is off)"""
+        if not isinstance(dueling_dqn, bool):
+            raise ValueError(f'dueling_dqn must be a bool, got {dueling_dqn!r}')
+        if not isinstance(categorical_dqn, bool):
+            raise ValueError(f'categorical_dqn must be a bool, got {categorical_dqn!r}')
+        if isinstance(num_atoms, bool) or not isinstance(num_atoms, (int, np.integer)) or not 2 <= num_atoms <= 64:
+            raise ValueError(f'num_atoms must be an int in [2, 64], got {num_atoms!r}')
+        with np.errstate(over='ignore'):
+            lo, hi = np.float32(v_min), np.float32(v_max)
+        if not (np.isfinite(lo) and np.isfinite(hi) and lo < hi and np.isfinite(np.float32((float(hi) - float(lo)) / (num_atoms - 1)))):
+            raise ValueError(f'v_min and v_max must be finite fp32 values with v_min < v_max, got ({v_min}, {v_max})')
+        if categorical_dqn and dueling_dqn:
+            raise ValueError('categorical_dqn with dueling_dqn is not supported: choose one head')
+        return cls(False, int(num_atoms), float(v_min), float(v_max)) if categorical_dqn else cls(dueling_dqn)
+
+    def __str__(self):
+        s = f'dueling_dqn={self.dueling}, categorical_dqn={self.num_atoms > 0}'
+        return s + f', (num_atoms, v_min, v_max)={(self.num_atoms, self.v_min, self.v_max)}' if self.num_atoms else s
+
+    def names(self):
+        return apex_param_names(self.dueling)
+
+    def shapes(self, num_actions: int):
+        return apex_param_shapes(num_actions, self.dueling, self.num_atoms)
+
+    def layout(self, num_actions: int):
+        """(total floats, offsets, counts) of the flat buffer"""
+        return _lib.apex_param_layout(num_actions, self.dueling, self.num_atoms)
 
 
 def flat_views(flat: torch.Tensor, off, cnt, shapes) -> 'OrderedDict[str, torch.Tensor]':
@@ -248,10 +279,11 @@ class B200ApexLearner(BaseAgent):
         self.hp = hp
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._L = _lib.lib()
-        self.names = apex_param_names(hp.dueling_dqn)
-        self.shapes = apex_param_shapes(hp.num_actions, hp.dueling_dqn, hp.atoms())
+        head = hp.head
+        self.names = head.names()
+        self.shapes = head.shapes(hp.num_actions)
         with torch.cuda.device(self.device):
-            total, self._off, self._cnt = _lib.apex_param_layout(hp.num_actions, hp.dueling_dqn, hp.atoms())
+            total, self._off, self._cnt = head.layout(hp.num_actions)
             z = lambda: torch.zeros(total, dtype=torch.float32, device=self.device)
             self.flat_params, self.flat_grads, self.exp_avg, self.exp_avg_sq, self.flat_target = z(), z(), z(), z(), z()
             self.params = self._views(self.flat_params)
@@ -264,7 +296,7 @@ class B200ApexLearner(BaseAgent):
                                                        C.byref(h)), 'srl_apex_learner_create')
             self._h = h
             self._stats = torch.zeros(4, device=self.device)      # {loss, gradient norm, clip coefficient, pad}
-        sd = default_q_state_dict(hp.num_actions, seed, hp.dueling_dqn, hp.atoms()) if init_state_dict is None else init_state_dict
+        sd = default_q_state_dict(hp.num_actions, seed, head.dueling, head.num_atoms) if init_state_dict is None else init_state_dict
         self.load_state_dict(sd)
         self.load_state_dict(sd, target=True)       # actor_target starts as a copy (dqn_agent.py:66-67)
         self.use_graph = use_graph

@@ -2,13 +2,14 @@
 // Restates the reference's
 //   scalerl/algorithms/apex/worker.py:14-30 (Actor: one eps per actor), :59-79 (compute_prior: |Q(s)[a] - (r + mask gamma^steps max Q(s'))|)
 //   scalerl/algorithms/apex/memory.py:43-64 (PrioritizedReplayBuffer.add: each transition enters with its actor's priority)
-// with one encoder forward (srl_encoder_forward) per frame set and the Q head of the learner (dqn_head.cuh), so that a priority computed
-// here has the bits of the learner's for the same weights.  fp32 on the CUDA cores: the Q head is 512 x A, no tensor-core work.
-//   apex_act_kernel       the Q row, its first argmax and the epsilon-greedy draw (one warp per env)
-//   apex_priority_kernel  q(s, a), the n-step target from max_a Q(s') and the priority (one warp per transition)
-// Both are templates on the head: plain q = Linear(512, A), or the dueling V + Adv - mean(Adv) (dqn_head.cuh's dueling_q).  The
-// categorical head (C51) runs the learner's logits GEMM (dqn_cat.cu) first; apex_cat_act_kernel and apex_cat_priority_kernel then
-// read the logits through dqn_cat.cuh's functions, the learner tail's.
+// with one encoder forward (srl_encoder_forward) per frame set and the Q head of the learner (dqn_head.cuh, dqn_cat.cuh), so that a
+// priority computed here has the bits of the learner's for the same weights.  fp32 on the CUDA cores: the Q head is 512 x A, no
+// tensor-core work.
+//   apex_act_kernel       the Q row, its first argmax and the epsilon-greedy draw (one warp per env), a template on the head kind
+//   apex_priority_kernel  q(s, a), the n-step target from max_a Q(s') and the priority (one warp per transition), plain or dueling
+//   apex_cat_priority_kernel  the same on the categorical head: the learner tail's cat_transition
+// The categorical head runs the learner's logits GEMM (dqn_cat.cu) first.  launch_apex_act and launch_apex_priorities are the one
+// place that picks the kernels of a head.
 #include <math.h>
 #include <string.h>
 #include <new>
@@ -55,32 +56,17 @@ SRL_DEVINL void advance_draws(unsigned long long* draws, unsigned long long d) {
 }
 
 // One warp per env, 4 per block.  draws[0]: the draw counter (u64), read by every block and advanced by the block that finishes
-// last (draws[1] low word: the ticket, re-armed by that block), so every env of one launch uses the same draw.
-// DUELING: W = [(A + 1)][512], b the value bias, ba the advantage biases.
-template <bool DUELING>
-__global__ void __launch_bounds__(128) apex_act_kernel(const float* __restrict__ core, const float* __restrict__ W, const float* __restrict__ b,
-                                                       int E, int A, const float* __restrict__ eps, uint2 key,
-                                                       unsigned long long* draws, int64_t* __restrict__ actions, const float* __restrict__ ba) {
+// last (draws[1] low word: the ticket, re-armed by that block), so every env of one launch uses the same draw.  rows: q_lane's (the
+// core rows, or the categorical head's logits).
+template <QKind KIND>
+__global__ void __launch_bounds__(128) apex_act_kernel(const QHead h, const float* __restrict__ rows, int E, const float* __restrict__ eps,
+                                                       uint2 key, unsigned long long* draws, int64_t* __restrict__ actions) {
   const int lane = threadIdx.x & 31, e = blockIdx.x * 4 + (threadIdx.x >> 5);
   const unsigned long long d = *reinterpret_cast<volatile unsigned long long*>(draws);
   if (e < E) {
     int greedy;
-    if constexpr (DUELING) q_row_max(dueling_q<false>(core + (size_t)e * ENC_CORE, W, b, ba, A, lane, nullptr), A, &greedy);
-    else q_max(core + (size_t)e * ENC_CORE, W, b, A, lane, &greedy);
-    if (lane == 0) actions[e] = eps_greedy(d, e, key, A, eps, greedy);
-  }
-  advance_draws(draws, d);
-}
-// the same on the categorical head's logits [E][A K]: greedy = the first argmax of the expected Q
-__global__ void __launch_bounds__(128) apex_cat_act_kernel(const float* __restrict__ logits, int E, int A, const CatSupport c,
-                                                           const float* __restrict__ eps, uint2 key, unsigned long long* draws,
-                                                           int64_t* __restrict__ actions) {
-  const int lane = threadIdx.x & 31, e = blockIdx.x * 4 + (threadIdx.x >> 5);
-  const unsigned long long d = *reinterpret_cast<volatile unsigned long long*>(draws);
-  if (e < E) {
-    int greedy;
-    q_row_max(cat_q_lane(logits + (size_t)e * A * c.K, A, c, lane), A, &greedy);
-    if (lane == 0) actions[e] = eps_greedy(d, e, key, A, eps, greedy);
+    q_row_max(q_lane<KIND>(h, rows, e, lane), h.A, &greedy);
+    if (lane == 0) actions[e] = eps_greedy(d, e, key, h.A, eps, greedy);
   }
   advance_draws(draws, d);
 }
@@ -88,53 +74,88 @@ __global__ void __launch_bounds__(128) apex_cat_act_kernel(const float* __restri
 // One warp per transition e in ring slot (ptr + e) mod M, 4 per block: q = Q(s)[a], y = R + gamma_n (1 - d) max_a Q(s'), the
 // learner tail's arithmetic (dqn_tail_kernel with the snapshot as online and target network, no double DQN)
 template <bool DUELING>
-__global__ void __launch_bounds__(128) apex_priority_kernel(const float* __restrict__ core_s, const float* __restrict__ core_n,
-                                                            const float* __restrict__ W, const float* __restrict__ b, int E, int A,
-                                                            const int64_t* __restrict__ action, const float* __restrict__ reward,
+__global__ void __launch_bounds__(128) apex_priority_kernel(const QHead h, const float* __restrict__ core_s, const float* __restrict__ core_n,
+                                                            int E, const int64_t* __restrict__ action, const float* __restrict__ reward,
                                                             const uint8_t* __restrict__ done, int64_t ptr, int64_t M, float gamma_n, float eps,
-                                                            double* __restrict__ prio, const float* __restrict__ ba) {
+                                                            double* __restrict__ prio) {
   const int lane = threadIdx.x & 31, e = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (e >= E) return;
   const int64_t slot = (ptr + e) % M;
-  const int act = ld_action(action + slot, A);
+  const int act = ld_action(action + slot, h.A);
   float q, nx;
   int a_star;
   if constexpr (DUELING) {
-    q = __shfl_sync(0xffffffffu, dueling_q<false>(core_s + (size_t)e * ENC_CORE, W, b, ba, A, lane, nullptr), act);
-    nx = q_row_max(dueling_q<false>(core_n + (size_t)e * ENC_CORE, W, b, ba, A, lane, nullptr), A, &a_star);
+    q = __shfl_sync(0xffffffffu, dueling_q<false>(core_s + (size_t)e * ENC_CORE, h.W, h.b, h.ba, h.A, lane, nullptr), act);
+    nx = q_row_max(dueling_q<false>(core_n + (size_t)e * ENC_CORE, h.W, h.b, h.ba, h.A, lane, nullptr), h.A, &a_star);
   } else {
-    q = q_dot(core_s + (size_t)e * ENC_CORE, W + (size_t)act * 512, lane) + __ldg(b + act);
-    nx = q_max(core_n + (size_t)e * ENC_CORE, W, b, A, lane, &a_star);
+    q = q_dot(core_s + (size_t)e * ENC_CORE, h.W + (size_t)act * 512, lane) + __ldg(h.b + act);
+    nx = q_max(core_n + (size_t)e * ENC_CORE, h.W, h.b, h.A, lane, &a_star);
   }
   const float y = td_target(__ldg(reward + slot), gamma_n, nx, done[slot] != 0);
   if (lane == 0) prio[e] = td_priority(__fsub_rn(q, y), eps);
 }
 // the categorical head: the learner tail's cat_transition with the snapshot's logits of s (logits_s) and s' (logits_n) as the online and
 // target network's, no double DQN -> max(KL(m || p(s)[a]), 0) + eps
-__global__ void __launch_bounds__(128) apex_cat_priority_kernel(const float* __restrict__ logits_s, const float* __restrict__ logits_n, int E,
-                                                                int A, const CatSupport c, const int64_t* __restrict__ action,
-                                                                const float* __restrict__ reward, const uint8_t* __restrict__ done, int64_t ptr,
-                                                                int64_t M, float gamma_n, float eps, double* __restrict__ prio) {
+__global__ void __launch_bounds__(128) apex_cat_priority_kernel(const QHead h, const float* __restrict__ logits_s, const float* __restrict__ logits_n,
+                                                                int E, const int64_t* __restrict__ action, const float* __restrict__ reward,
+                                                                const uint8_t* __restrict__ done, int64_t ptr, int64_t M, float gamma_n, float eps,
+                                                                double* __restrict__ prio) {
   __shared__ float sm[4][CAT_MAX_ATOMS];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, e = blockIdx.x * 4 + warp;
   if (e >= E) return;
   const int64_t slot = (ptr + e) % M;
-  const int act = ld_action(action + slot, A), R = A * c.K;
-  const CatLoss r = cat_transition(logits_s + (size_t)e * R + (size_t)act * c.K, nullptr, logits_n + (size_t)e * R, A, __ldg(reward + slot),
-                                   done[slot] ? 0.f : gamma_n, c, lane, sm[warp], 0.f, nullptr);
+  const int act = ld_action(action + slot, h.A);
+  const CatLoss r = cat_transition(logits_s + (size_t)e * h.R + (size_t)act * h.c.K, nullptr, logits_n + (size_t)e * h.R, h.A,
+                                   __ldg(reward + slot), done[slot] ? 0.f : gamma_n, h.c, lane, sm[warp], 0.f, nullptr);
   if (lane == 0) prio[e] = cat_priority(r.kl, eps);
+}
+
+// the act kernel of head h over the E core rows (the categorical head: through logits [E][A K])
+cudaError_t launch_apex_act(const QHead& h, const float* core, float* logits, int E, const float* eps, uint2 key, unsigned long long* draws,
+                            int64_t* actions, cudaStream_t st) {
+  const int blocks = (E + 3) / 4;
+  switch (h.kind) {
+    case Q_PLAIN: apex_act_kernel<Q_PLAIN><<<blocks, 128, 0, st>>>(h, core, E, eps, key, draws, actions); break;
+    case Q_DUELING: apex_act_kernel<Q_DUELING><<<blocks, 128, 0, st>>>(h, core, E, eps, key, draws, actions); break;
+    case Q_CATEGORICAL: {
+      const cudaError_t e = launch_cat_logits(core, h.W, h.b, E, h.R, logits, st);
+      if (e != cudaSuccess) return e;
+      apex_act_kernel<Q_CATEGORICAL><<<blocks, 128, 0, st>>>(h, logits, E, eps, key, draws, actions);
+      break;
+    }
+  }
+  return cudaGetLastError();
+}
+// the priority kernel of head h over the core rows of s (core) and s' (core + E rows); the categorical head: through logits [2E][A K]
+cudaError_t launch_apex_priorities(const QHead& h, const float* core, float* logits, int E, const int64_t* action, const float* reward,
+                                   const uint8_t* done, int64_t ptr, int64_t M, float gamma_n, float eps, double* prio, cudaStream_t st) {
+  const int blocks = (E + 3) / 4;
+  const float* core_n = core + (size_t)E * ENC_CORE;
+  switch (h.kind) {
+    case Q_PLAIN:
+      apex_priority_kernel<false><<<blocks, 128, 0, st>>>(h, core, core_n, E, action, reward, done, ptr, M, gamma_n, eps, prio);
+      break;
+    case Q_DUELING:
+      apex_priority_kernel<true><<<blocks, 128, 0, st>>>(h, core, core_n, E, action, reward, done, ptr, M, gamma_n, eps, prio);
+      break;
+    case Q_CATEGORICAL: {
+      const cudaError_t e = launch_cat_logits(core, h.W, h.b, 2 * E, h.R, logits, st);      // s and s' rows in one GEMM
+      if (e != cudaSuccess) return e;
+      apex_cat_priority_kernel<<<blocks, 128, 0, st>>>(h, logits, logits + (size_t)E * h.R, E, action, reward, done, ptr, M, gamma_n, eps, prio);
+      break;
+    }
+  }
+  return cudaGetLastError();
 }
 
 }  // namespace srl
 using namespace srl;
 
 struct srl_apex_actor {
-  int A, E;
+  int E;
   uint2 key;
   const float* w8[8];              // the encoder tensors of the snapshot
-  const float *Wq, *bq;            // plain: q.weight, q.bias; dueling: [value.weight; advantage.weight], value.bias
-  const float* bqa;                // dueling: advantage.bias (NULL: the plain head)
-  CatSupport cs;                   // the categorical head (cs.K > 0)
+  QHead head;                      // the snapshot's Q head
   float* logits;                   // categorical: [2E][A K], the logits of the core rows
   srl_encoder_t* enc;
   char *saved, *scratch;           // encoder blocks for E frames: the two forwards of an add run one after the other
@@ -157,7 +178,7 @@ int actor_rows(srl_apex_actor* X, int64_t saved, int64_t scratch, WsRow* t) {
   t[n++] = ws_row(nullptr, E, &X->zero_action);
   t[n++] = ws_row(nullptr, E, &X->prio);
   t[n++] = ws_row(nullptr, 2, &X->draws);
-  t[n++] = ws_row(nullptr, 2 * E * X->A * X->cs.K, &X->logits);
+  t[n++] = ws_row(nullptr, X->head.kind == Q_CATEGORICAL ? 2 * E * X->head.R : 0, &X->logits);
   return n;
 }
 constexpr int ACTOR_ROWS = 8;
@@ -188,28 +209,24 @@ extern "C" int srl_apex_actor_create_cat(int A, int num_envs, int precision, int
 static int actor_create(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max,
                                           uint64_t seed, const float* params, srl_apex_actor_t** out) {
   REQ(params && out, "apex_actor_create: NULL argument");
-  REQ(A >= 1 && A <= 31, "apex_actor_create: A=%d must be in [1,31]", A);
   REQ(num_envs >= 1 && num_envs <= MAX_FRAMES, "apex_actor_create: num_envs=%d must be in [1, %d]", num_envs, MAX_FRAMES);
   REQ(precision == 0 || precision == 1, "apex_actor_create: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", precision);
-  REQ(dueling == 0 || dueling == 1, "apex_actor_create: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", dueling);
-  int rc = check_cat_head("apex_actor_create", num_atoms, v_min, v_max, dueling);
+  QHead head;
+  int rc = make_q_head("apex_actor_create", A, dueling, num_atoms, v_min, v_max, &head);
   if (rc) return rc;
   REQ(!misaligned(params, 16), "apex_actor_create: params must be 16-byte aligned");
-  int64_t off[12];
-  if (num_atoms) srl_apex_param_layout_cat(A, num_atoms, off, nullptr);
-  else srl_apex_param_layout_ex(A, dueling, off, nullptr);
   int64_t sb = 0, kb = 0;
   rc = srl_encoder_sizes(num_envs, precision, &sb, &kb);
   if (rc) return rc;
   srl_apex_actor* X = new (std::nothrow) srl_apex_actor();
   REQ(X, "out of host memory");
   auto undo = [X](int code) { srl_apex_actor_destroy(X); return code; };
-  X->A = A; X->E = num_envs;
+  X->E = num_envs;
   X->key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  int64_t off[12];
+  apex_layout(head, off, nullptr);
   for (int i = 0; i < 8; ++i) X->w8[i] = params + off[i];
-  X->Wq = params + off[8]; X->bq = params + off[9];
-  X->bqa = dueling ? params + off[11] : nullptr;
-  if (num_atoms) X->cs = cat_support(num_atoms, v_min, v_max);
+  X->head = bind_q_head(head, params);
   rc = srl_encoder_create(precision, &X->enc);
   if (rc) return undo(rc);
   WsRow t[ACTOR_ROWS];
@@ -241,19 +258,15 @@ extern "C" int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const
   const cudaStream_t st = (cudaStream_t)stream;
   rc = actor_forward(X, obs, E, X->core, st);
   if (rc) return rc;
-  if (X->cs.K) {
-    CU(launch_cat_logits(X->core, X->Wq, X->bq, E, X->A * X->cs.K, X->logits, st), "cat_logits");
-    apex_cat_act_kernel<<<(E + 3) / 4, 128, 0, st>>>(X->logits, E, X->A, X->cs, epsilons, X->key, X->draws, actions);
-  } else if (X->bqa) apex_act_kernel<true><<<(E + 3) / 4, 128, 0, st>>>(X->core, X->Wq, X->bq, E, X->A, epsilons, X->key, X->draws, actions, X->bqa);
-  else apex_act_kernel<false><<<(E + 3) / 4, 128, 0, st>>>(X->core, X->Wq, X->bq, E, X->A, epsilons, X->key, X->draws, actions, nullptr);
-  CU(cudaGetLastError(), "apex_act_kernel");
+  CU(launch_apex_act(X->head, X->core, X->logits, E, epsilons, X->key, X->draws, actions, st), "apex_act");
   return 0;
 }
 
 extern "C" int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, int n, float* q_out, void* stream) {
   REQ(X && obs && q_out, "apex_actor_q_values: NULL pointer");
   REQ(n >= 1, "apex_actor_q_values: n=%d must be >= 1", n);
-  const Span s[2] = {{obs, n * ACTOR_OBS_BYTES, false, "obs"}, {q_out, (int64_t)n * X->A * 4, true, "q_out"}};
+  const int A = X->head.A;
+  const Span s[2] = {{obs, n * ACTOR_OBS_BYTES, false, "obs"}, {q_out, (int64_t)n * A * 4, true, "q_out"}};
   int rc = check_spans(s, 2, "apex_actor_q_values");
   if (rc) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
@@ -261,8 +274,7 @@ extern "C" int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, 
     const int f = n - f0 < X->E ? n - f0 : X->E;
     rc = actor_forward(X, obs + (size_t)f0 * ACTOR_OBS_BYTES, f, X->core, st);
     if (rc) return rc;
-    if (X->cs.K) CU(launch_cat_q_values(X->core, X->Wq, X->bq, f, X->A, X->cs, X->logits, q_out + (size_t)f0 * X->A, st), "cat_q_values");
-    else CU(launch_dqn_q_values(X->core, X->Wq, X->bq, X->bqa, f, X->A, q_out + (size_t)f0 * X->A, st), "dqn_q_values");
+    CU(launch_q_values(X->head, X->core, f, X->logits, q_out + (size_t)f0 * A, st), "q_values");
   }
   return 0;
 }
@@ -271,7 +283,7 @@ extern "C" int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name
   REQ(X && name && ptr && count, "apex_actor_debug_buffer: NULL argument");
   const int64_t rows = 2 * (int64_t)X->E;
   if (strcmp(name, "core") == 0) { *ptr = X->core; *count = rows * ENC_CORE; return 0; }
-  if (strcmp(name, "logits") == 0 && X->cs.K) { *ptr = X->logits; *count = rows * X->A * X->cs.K; return 0; }
+  if (strcmp(name, "logits") == 0 && X->head.kind == Q_CATEGORICAL) { *ptr = X->logits; *count = rows * X->head.R; return 0; }
   return fail(SRL_EINVAL, "apex_actor_debug_buffer: unknown buffer '%s'", name);
 }
 
@@ -281,22 +293,10 @@ int apex_actor_num_envs(const srl_apex_actor* X) { return X->E; }
 int apex_actor_priorities(srl_apex_actor* X, const uint8_t* s, const uint8_t* s_next, const int64_t* action, const float* reward,
                           const uint8_t* done, int64_t ptr, int64_t M, float gamma_n, float eps, const double** prio, cudaStream_t st) {
   const int E = X->E;
-  float* core_n = X->core + (size_t)E * ENC_CORE;
   int rc = actor_forward(X, s, E, X->core, st);
-  if (!rc) rc = actor_forward(X, s_next, E, core_n, st);
+  if (!rc) rc = actor_forward(X, s_next, E, X->core + (size_t)E * ENC_CORE, st);
   if (rc) return rc;
-  if (X->cs.K) {
-    const int R = X->A * X->cs.K;
-    CU(launch_cat_logits(X->core, X->Wq, X->bq, 2 * E, R, X->logits, st), "cat_logits");      // s and s' rows in one GEMM
-    apex_cat_priority_kernel<<<(E + 3) / 4, 128, 0, st>>>(X->logits, X->logits + (size_t)E * R, E, X->A, X->cs, action, reward, done, ptr, M,
-                                                          gamma_n, eps, X->prio);
-  } else if (X->bqa)
-    apex_priority_kernel<true><<<(E + 3) / 4, 128, 0, st>>>(X->core, core_n, X->Wq, X->bq, E, X->A, action, reward, done, ptr, M, gamma_n, eps,
-                                                             X->prio, X->bqa);
-  else
-    apex_priority_kernel<false><<<(E + 3) / 4, 128, 0, st>>>(X->core, core_n, X->Wq, X->bq, E, X->A, action, reward, done, ptr, M, gamma_n, eps,
-                                                              X->prio, nullptr);
-  CU(cudaGetLastError(), "apex_priority_kernel");
+  CU(launch_apex_priorities(X->head, X->core, X->logits, E, action, reward, done, ptr, M, gamma_n, eps, X->prio, st), "apex_priorities");
   *prio = X->prio;
   return 0;
 }

@@ -898,12 +898,15 @@ extern "C" int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int fr
 // dueling: {..., fc.b, value.w [1,512], value.b [1], advantage.w [A,512], advantage.b [A]}; in memory value.weight directly before
 // advantage.weight (one [(A + 1)][512] head block for the kernels) and value.bias before advantage.bias
 // categorical (atoms = K > 0): the plain order with q.weight [A K, 512] and q.bias [A K] (row a K + k: atom k of action a)
-static int64_t apex_layout(int A, int dueling, int atoms, int64_t* off, int64_t* cnt) {
-  const int64_t R = (int64_t)A * (atoms ? atoms : 1);
+// The layout depends on the head's kind and rows only.
+namespace srl {
+int64_t apex_layout(const QHead& h, int64_t* off, int64_t* cnt) {
+  const int64_t A = h.A, R = h.R;
   const int64_t plain[10] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, R * 512, R};
-  const int64_t duel[12] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, 512, 1, (int64_t)A * 512, A};
+  const int64_t duel[12] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, 512, 1, A * 512, A};
   const int plain_order[10] = {0, 1, 2, 3, 4, 5, 7, 8, 9, 6};
   const int duel_order[12] = {0, 1, 2, 3, 4, 5, 7, 8, 10, 9, 11, 6};
+  const bool dueling = h.kind == Q_DUELING;
   const int64_t* counts = dueling ? duel : plain;
   const int* order = dueling ? duel_order : plain_order;
   const int n = dueling ? 12 : 10;
@@ -916,32 +919,56 @@ static int64_t apex_layout(int A, int dueling, int atoms, int64_t* off, int64_t*
   }
   return o;
 }
-extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) { return apex_layout(A, 0, 0, offsets10, counts10); }
+
+int make_q_head(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, QHead* h) {
+  REQ(A >= 1 && A <= 31, "%s: A=%d must be in [1,31]", who, A);
+  REQ(dueling == 0 || dueling == 1, "%s: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", who, dueling);
+  REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "%s: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]", who,
+      num_atoms, CAT_MAX_ATOMS);
+  *h = QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling};
+  if (num_atoms == 0) return 0;
+  REQ(std::isfinite(v_min) && std::isfinite(v_max) && v_min < v_max, "%s: v_min=%g, v_max=%g must be finite with v_min < v_max", who,
+      (double)v_min, (double)v_max);
+  const CatSupport c = cat_support(num_atoms, v_min, v_max);
+  REQ(std::isfinite(c.dz) && c.dz > 0.f, "%s: the atom spacing (v_max - v_min) / (num_atoms - 1) = %g is not a positive finite float", who,
+      (double)c.dz);
+  REQ(dueling == 0, "%s: the categorical head (num_atoms=%d) with dueling=1 is not supported", who, num_atoms);
+  h->kind = Q_CATEGORICAL;
+  h->R = A * num_atoms;
+  h->c = c;
+  return 0;
+}
+
+QHead bind_q_head(QHead h, const float* params) {
+  int64_t off[12];
+  apex_layout(h, off, nullptr);
+  h.W = params + off[8];
+  h.b = params + off[9];
+  h.ba = h.kind == Q_DUELING ? params + off[11] : nullptr;
+  return h;
+}
+
+QHeadGrad bind_q_grad(const QHead& h, float* grads) {
+  int64_t off[12];
+  apex_layout(h, off, nullptr);
+  return {grads + off[8], grads + off[9], h.kind == Q_DUELING ? grads + off[11] : nullptr};
+}
+}  // namespace srl
+
+extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) {
+  return apex_layout(QHead{Q_PLAIN, A, A}, offsets10, counts10);
+}
 extern "C" int64_t srl_apex_param_layout_ex(int A, int dueling, int64_t* offsets12, int64_t* counts12) {
   REQ(A >= 1 && A <= 31, "apex_param_layout: A=%d must be in [1,31]", A);
   REQ(dueling == 0 || dueling == 1, "apex_param_layout: dueling=%d must be 0 or 1", dueling);
-  return apex_layout(A, dueling, 0, offsets12, counts12);
+  return apex_layout(QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling}, offsets12, counts12);
 }
 extern "C" int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offsets10, int64_t* counts10) {
   REQ(A >= 1 && A <= 31, "apex_param_layout: A=%d must be in [1,31]", A);
   REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "apex_param_layout: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]",
       num_atoms, CAT_MAX_ATOMS);
-  return apex_layout(A, 0, num_atoms, offsets10, counts10);
+  return apex_layout(QHead{num_atoms ? Q_CATEGORICAL : Q_PLAIN, A, A * (num_atoms ? num_atoms : 1)}, offsets10, counts10);
 }
-
-namespace srl {
-int check_cat_head(const char* who, int num_atoms, float v_min, float v_max, int dueling) {
-  REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "%s: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]", who,
-      num_atoms, CAT_MAX_ATOMS);
-  if (num_atoms == 0) return 0;
-  REQ(std::isfinite(v_min) && std::isfinite(v_max) && v_min < v_max, "%s: v_min=%g, v_max=%g must be finite with v_min < v_max", who,
-      (double)v_min, (double)v_max);
-  const float dz = cat_support(num_atoms, v_min, v_max).dz;
-  REQ(std::isfinite(dz) && dz > 0.f, "%s: the atom spacing (v_max - v_min) / (num_atoms - 1) = %g is not a positive finite float", who, (double)dz);
-  REQ(dueling == 0, "%s: the categorical head (num_atoms=%d) with dueling=1 is not supported", who, num_atoms);
-  return 0;
-}
-}  // namespace srl
 
 struct srl_apex_learner {
   srl_apex_config_t cfg;
@@ -949,8 +976,8 @@ struct srl_apex_learner {
   int64_t nparams;
   const float *w8[8], *t8[8];     // the encoder tensors of the online and target parameters
   float* g8[8];
-  float *Wq, *bq, *Wt, *bt, *gWq, *gbq;   // dueling: the [(A + 1)][512] head block and value.bias (of params / target / grads)
-  float *bqa, *bta, *gbqa;              // dueling: advantage.bias; NULL for the plain head
+  QHead on, tg;                   // the Q head of the online and target parameters
+  QHeadGrad g;                    // ... and its gradients
   srl_encoder_t *E, *Eq;          // the step's encoder context, and the q-value forwards' own (lanes, events)
   char *saved_s, *saved_n, *enc_scratch;   // encoder blocks: the forward over s (read by the backward), the forwards over s'
   char *saved_q, *scratch_q;      // the q-value forwards' blocks: they may run on another stream than the step
@@ -962,7 +989,6 @@ struct srl_apex_learner {
   // the categorical head (cfg.num_atoms = K > 0): logits [B][A K] over s, s' (online, double DQN only) and s' (target), their
   // gradient, the projected targets m [B][K], the cross-entropies [B] and the q-value chunk's logits
   float *logits_s, *logits_n, *logits_nt, *dlogits, *mproj, *ce, *logits_q;
-  CatSupport cs;
   char* arena;
 };
 
@@ -1012,10 +1038,10 @@ static int apex_rows(srl_apex_learner* L, const int64_t* b4, WsRow* t) {
 }
 constexpr int APEX_ROWS = 29;
 
-static int check_apex_cfg(const srl_apex_config_t* c) {
+// -> the unbound head of a valid config
+static int check_apex_cfg(const srl_apex_config_t* c, QHead* head) {
   REQ(c, "apex_learner: config is NULL");
   REQ(c->B >= 1 && c->B <= MAX_FRAMES, "apex_learner: B=%d must be in [1, %d]", c->B, MAX_FRAMES);
-  REQ(c->A >= 1 && c->A <= 31, "apex_learner: A=%d must be in [1,31]", c->A);
   REQ(c->precision == 0 || c->precision == 1, "apex_learner: precision must be 0 (bf16 operands) or 1 (fp32-accurate split operands)");
   REQ(c->double_dqn == 0 || c->double_dqn == 1, "apex_learner: double_dqn must be 0 or 1");
   REQ(std::isfinite(c->gamma) && c->gamma >= 0.f, "apex_learner: gamma=%g must be finite and >= 0", (double)c->gamma);
@@ -1024,19 +1050,19 @@ static int check_apex_cfg(const srl_apex_config_t* c) {
   REQ(c->adam_beta1 >= 0.f && c->adam_beta1 < 1.f && c->adam_beta2 >= 0.f && c->adam_beta2 < 1.f, "apex_learner: Adam betas must be in [0, 1)");
   REQ(std::isfinite(c->adam_eps) && c->adam_eps >= 0.f, "apex_learner: adam_eps=%g must be finite and >= 0", (double)c->adam_eps);
   REQ(std::isfinite(c->priority_eps) && c->priority_eps >= 0.f, "apex_learner: priority_eps=%g must be finite and >= 0", (double)c->priority_eps);
-  REQ(c->dueling == 0 || c->dueling == 1, "apex_learner: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", (int)c->dueling);
-  return check_cat_head("apex_learner", c->num_atoms, c->v_min, c->v_max, c->dueling);
+  return make_q_head("apex_learner", c->A, c->dueling, c->num_atoms, c->v_min, c->v_max, head);
 }
 
 extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* params, float* grads, float* exp_avg, float* exp_avg_sq,
                                        float* target_params, srl_apex_learner_t** out) {
-  int rc = check_apex_cfg(cfg);
+  QHead head;
+  int rc = check_apex_cfg(cfg, &head);
   if (rc) return rc;
   REQ(params && grads && exp_avg && exp_avg_sq && target_params && out, "apex_learner_create: NULL argument");
   REQ(!misaligned(params, 16) && !misaligned(grads, 16) && !misaligned(exp_avg, 16) && !misaligned(exp_avg_sq, 16) &&
       !misaligned(target_params, 16), "apex_learner_create: flat buffers must be 16-byte aligned");
   int64_t off[12];
-  const int64_t np = apex_layout(cfg->A, cfg->dueling, cfg->num_atoms, off, nullptr);
+  const int64_t np = apex_layout(head, off, nullptr);
   const Span s[5] = {{params, np * 4, true, "params"}, {grads, np * 4, true, "grads"}, {exp_avg, np * 4, true, "exp_avg"},
                      {exp_avg_sq, np * 4, true, "exp_avg_sq"}, {target_params, np * 4, true, "target_params"}};
   rc = check_spans(s, 5, "apex_learner_create");
@@ -1046,10 +1072,7 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   auto undo = [L](int code) { srl_apex_learner_destroy(L); return code; };
   L->cfg = *cfg; L->params = params; L->grads = grads; L->m = exp_avg; L->v = exp_avg_sq; L->target = target_params; L->nparams = np;
   for (int i = 0; i < 8; ++i) { L->w8[i] = params + off[i]; L->t8[i] = target_params + off[i]; L->g8[i] = grads + off[i]; }
-  L->Wq = params + off[8]; L->bq = params + off[9]; L->Wt = target_params + off[8]; L->bt = target_params + off[9];
-  L->gWq = grads + off[8]; L->gbq = grads + off[9];
-  if (cfg->dueling) { L->bqa = params + off[11]; L->bta = target_params + off[11]; L->gbqa = grads + off[11]; }
-  if (cfg->num_atoms) L->cs = cat_support(cfg->num_atoms, cfg->v_min, cfg->v_max);
+  L->on = bind_q_head(head, params); L->tg = bind_q_head(head, target_params); L->g = bind_q_grad(head, grads);
   rc = srl_encoder_create(cfg->precision, &L->E);
   if (!rc) rc = srl_encoder_create(cfg->precision, &L->Eq);
   if (rc) return undo(rc);
@@ -1091,30 +1114,11 @@ extern "C" int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, 
   if (!rc && c.double_dqn) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->w8, L->saved_n, L->enc_scratch, L->core_n, stream);
   if (!rc) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->t8, L->saved_n, L->enc_scratch, L->core_nt, stream);
   if (rc) return rc;
-  if (c.num_atoms) {       // the categorical head: the three logit sets, the projection / cross-entropy tail, the head gradients
-    const int R = c.A * c.num_atoms;
-    CU(launch_cat_logits(L->core_s, L->Wq, L->bq, B, R, L->logits_s, st), "cat_logits");
-    if (c.double_dqn) CU(launch_cat_logits(L->core_n, L->Wq, L->bq, B, R, L->logits_n, st), "cat_logits");
-    CU(launch_cat_logits(L->core_nt, L->Wt, L->bt, B, R, L->logits_nt, st), "cat_logits");
-    CatTail t;
-    t.logits_s = L->logits_s; t.logits_n = c.double_dqn ? L->logits_n : nullptr; t.logits_nt = L->logits_nt; t.W = L->Wq;
-    t.action = action; t.reward = reward; t.done = done; t.weight = weights;
-    t.B = B; t.A = c.A; t.c = L->cs; t.gamma = c.gamma; t.inv_B = 1.f / (float)B; t.priority_eps = c.priority_eps;
-    t.q = L->q; t.y = L->y; t.ce = L->ce; t.m = L->mproj; t.dlogits = L->dlogits; t.dcore = L->dcore; t.loss = L->loss;
-    t.scratch = L->tail_scratch; t.prio = L->prio;
-    CU(launch_cat_tail(t, st), "cat_tail");
-    CU(launch_cat_wgrad(L->dlogits, L->core_s, B, R, L->gWq, L->gbq, st), "cat_wgrad");
-  } else {
-    DqnTail t;
-    t.core_s = L->core_s; t.core_n = c.double_dqn ? L->core_n : nullptr; t.core_nt = L->core_nt;
-    t.Wq = L->Wq; t.bq = L->bq; t.Wt = L->Wt; t.bt = L->bt;
-    t.action = action; t.reward = reward; t.done = done; t.weight = weights;
-    t.B = B; t.A = c.A; t.gamma = c.gamma; t.two_over_B = 2.f / (float)B; t.priority_eps = c.priority_eps;
-    t.q = L->q; t.y = L->y; t.dq = L->dq; t.dcore = L->dcore; t.loss = L->loss; t.scratch = L->tail_scratch; t.prio = L->prio;
-    t.bqa = L->bqa; t.bta = L->bta; t.dueling = c.dueling;
-    CU(launch_dqn_tail(t, st), "dqn_tail");
-    CU(launch_dqn_wgrad(L->dq, action, L->core_s, B, c.A, L->head_part, L->gWq, L->gbq, L->gbqa, st), "dqn_wgrad");
-  }
+  const QTail t = {L->core_s, c.double_dqn ? L->core_n : nullptr, L->core_nt, action, reward, done, weights, B, c.gamma, c.priority_eps,
+                   L->q, L->y, L->dcore, L->loss, L->tail_scratch, L->prio, L->dq, L->head_part, L->logits_s, L->logits_n, L->logits_nt,
+                   L->mproj, L->ce, L->dlogits};
+  CU(launch_q_tail(L->on, L->tg, t, st), "q_tail");
+  CU(launch_q_wgrad(L->on, L->g, t, st), "q_wgrad");
   rc = srl_encoder_backward(L->E, L->dcore, B, 1, L->saved_s, L->enc_scratch, L->g8, stream);
   if (rc) return rc;
   const OptStep o = {1, L->params, L->grads, L->m, L->v, L->nparams, c.max_grad_norm, L->coef, L->opt_scratch, c.learning_rate,
@@ -1159,10 +1163,7 @@ extern "C" int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* o
     rc = srl_encoder_forward(L->Eq, obs + (size_t)f0 * 28224, L->zero_reward, L->zero_action, f, 1, L->w8, L->saved_q, L->scratch_q,
                              L->core_q, stream);
     if (rc) return rc;
-    if (L->cfg.num_atoms)
-      CU(launch_cat_q_values(L->core_q, L->Wq, L->bq, f, A, L->cs, L->logits_q, q_out + (size_t)f0 * A, (cudaStream_t)stream), "cat_q_values");
-    else
-      CU(launch_dqn_q_values(L->core_q, L->Wq, L->bq, L->bqa, f, A, q_out + (size_t)f0 * A, (cudaStream_t)stream), "dqn_q_values");
+    CU(launch_q_values(L->on, L->core_q, f, L->logits_q, q_out + (size_t)f0 * A, (cudaStream_t)stream), "q_values");
   }
   return 0;
 }

@@ -4,49 +4,51 @@
 //                             (apex/worker.py:148-157; dqn/dqn_agent.py:155-171)
 //   dqn_wgrad_kernel /        the Q head's weight and bias gradients: slab-group partials added in group order (the order of
 //   dqn_wgrad_reduce_kernel   heads.cu's head_wgrad kernels), so every run computes the same bits
-//   dqn_q_values_kernel       the forward-only Q head (predict / get_action)
+//   q_values_kernel           the forward-only Q head (predict / get_action)
 //   apex_soft_update_kernel   theta_t <- tau theta + (1 - tau) theta_t (dqn_agent.py:185-190, utils/model_utils.py:29-32)
 // The Q head arithmetic (q_dot, q_max, dueling_q, q_row_max, the target and the priority) is dqn_head.cuh's, shared with the Ape-X actor.
-// The tail, the head gradients and the Q values are templates on the head: DUELING = the dueling head V + Adv - mean(Adv) on the shared
-// fc output (Wang et al. 2016, eq. 9), whose A + 1 rows (the value row first) lie as one [(A + 1)][512] block; the plain instantiations
-// are the single-head kernels unchanged.
+// The tail and the head gradients are templates on the scalar heads: DUELING = the dueling head V + Adv - mean(Adv) on the shared fc
+// output (Wang et al. 2016, eq. 9), whose A + 1 rows (the value row first) lie as one [(A + 1)][512] block.  launch_q_tail,
+// launch_q_wgrad and launch_q_values are the one place that picks the kernels of a head; the categorical head's are dqn_cat.cu's.
 #include "common.cuh"
+#include "dqn_cat.cuh"
 #include "dqn_head.cuh"
 #include "kernels.h"
 
 namespace srl {
 
-// One warp per transition, 4 per block.  scratch: [0] the ticket, [4 + k] block k's partial of sum_n w_n (q_n - y_n)^2.
-// DUELING: the dueling head (dqn_head.cuh's dueling_q) in place of q = Linear(512, A); the target, loss and priority are the same.
+// One warp per transition, 4 per block: on, tg = the online and target heads.  scratch: [0] the ticket, [4 + k] block k's partial of
+// sum_n w_n (q_n - y_n)^2.  DUELING: the dueling head (dqn_head.cuh's dueling_q) in place of q = Linear(512, A); the target, loss and
+// priority are the same.
 template <bool DUELING>
-__global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
+__global__ void __launch_bounds__(128) dqn_tail_kernel(const QHead on, const QHead tg, const QTail t, float two_over_B) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = blockIdx.x * 4 + warp;
   float l = 0.f;
   if (n < t.B) {
-    const int act = ld_action(t.action + n, t.A);
+    const int act = ld_action(t.action + n, on.A);
     const float* hs = t.core_s + (size_t)n * ENC_CORE;
     float q, nx;
     float wsum[16];     // dueling: the advantage rows' column sums (lane + 32 i)
     if constexpr (!DUELING) {
-      q = q_dot(hs, t.Wq + (size_t)act * 512, lane) + __ldg(t.bq + act);
+      q = q_dot(hs, on.W + (size_t)act * 512, lane) + __ldg(on.b + act);
       const float* hn = t.core_nt + (size_t)n * ENC_CORE;
       int a_star;
       if (t.core_n) {     // double DQN: the online network picks a*, the target network values it (dqn_agent.py:155-160)
-        q_max(t.core_n + (size_t)n * ENC_CORE, t.Wq, t.bq, t.A, lane, &a_star);
-        nx = q_dot(hn, t.Wt + (size_t)a_star * 512, lane) + __ldg(t.bt + a_star);
+        q_max<2>(t.core_n + (size_t)n * ENC_CORE, on.W, on.b, on.A, lane, &a_star);
+        nx = q_dot(hn, tg.W + (size_t)a_star * 512, lane) + __ldg(tg.b + a_star);
       } else {            // max_a Q_target(s', a) (apex/worker.py:149, dqn_agent.py:162-163)
-        nx = q_max(hn, t.Wt, t.bt, t.A, lane, &a_star);
+        nx = q_max<2>(hn, tg.W, tg.b, on.A, lane, &a_star);
       }
     } else {            // the same statements on the dueling Q rows (lane a holds Q_a)
-      q = __shfl_sync(0xffffffffu, dueling_q<true>(hs, t.Wq, t.bq, t.bqa, t.A, lane, wsum), act);
-      const float qt = dueling_q<false>(t.core_nt + (size_t)n * ENC_CORE, t.Wt, t.bt, t.bta, t.A, lane, nullptr);
+      q = __shfl_sync(0xffffffffu, dueling_q<true>(hs, on.W, on.b, on.ba, on.A, lane, wsum), act);
+      const float qt = dueling_q<false>(t.core_nt + (size_t)n * ENC_CORE, tg.W, tg.b, tg.ba, on.A, lane, nullptr);
       int a_star;
       if (t.core_n) {
-        q_row_max(dueling_q<false>(t.core_n + (size_t)n * ENC_CORE, t.Wq, t.bq, t.bqa, t.A, lane, nullptr), t.A, &a_star);
+        q_row_max(dueling_q<false>(t.core_n + (size_t)n * ENC_CORE, on.W, on.b, on.ba, on.A, lane, nullptr), on.A, &a_star);
         nx = __shfl_sync(0xffffffffu, qt, a_star);
       } else {
-        nx = q_row_max(qt, t.A, &a_star);
+        nx = q_row_max(qt, on.A, &a_star);
       }
     }
     const float y = td_target(__ldg(t.reward + n), t.gamma, nx, t.done[n] != 0);
@@ -54,46 +56,27 @@ __global__ void __launch_bounds__(128) dqn_tail_kernel(const DqnTail t) {
     const float delta = __fsub_rn(q, y);
     l = __fmul_rn(w, __fmul_rn(delta, delta));
     // d loss / d q of mean(w (q - y)^2): the gradient flows through q only (y is detached)
-    const float dq = t.two_over_B * w * delta;
+    const float dq = two_over_B * w * delta;
     if (lane == 0) {
       t.q[n] = q; t.y[n] = y; t.dq[n] = dq;
       t.prio[n] = td_priority(delta, t.priority_eps);
     }
     if constexpr (!DUELING) {
-      const float* wa = t.Wq + (size_t)act * 512;
+      const float* wa = on.W + (size_t)act * 512;
       float* dc = t.dcore + (size_t)n * ENC_CORE;
       for (int j = lane; j < ENC_CORE; j += 32) dc[j] = j < 512 ? dq * __ldg(wa + j) : 0.f;
     } else {            // dL/dV = dq, dL/dAdv_a = dq (1[a = act] - 1/A): dL/dh = dq (w_v + W_adv[act] - mean_a W_adv[a])
-      const float* wa = t.Wq + (size_t)(act + 1) * 512;
+      const float* wa = on.W + (size_t)(act + 1) * 512;
       float* dc = t.dcore + (size_t)n * ENC_CORE;
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         const int j = lane + 32 * i;
-        dc[j] = dq * __fsub_rn(__fadd_rn(__ldg(t.Wq + j), __ldg(wa + j)), __fdiv_rn(wsum[i], (float)t.A));
+        dc[j] = dq * __fsub_rn(__fadd_rn(__ldg(on.W + j), __ldg(wa + j)), __fdiv_rn(wsum[i], (float)on.A));
       }
       if (lane < ENC_CORE - 512) dc[512 + lane] = 0.f;
     }
   }
-  // block partial: the warps' losses in warp order, then the ticket; the last block adds the partials in block order
-  __shared__ float red[4];
-  __shared__ bool is_last;
-  if (lane == 0) red[warp] = l;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    t.scratch[4 + blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
-    is_last = take_ticket(t.scratch);
-  }
-  __syncthreads();
-  if (is_last && warp == 0) {
-    __threadfence();
-    float s = 0.f;
-    for (unsigned k = lane; k < gridDim.x; k += 32) s += reinterpret_cast<volatile float*>(t.scratch)[4 + k];
-    s = warp_sum(s);
-    if (lane == 0) {
-      t.loss[0] = s / (float)t.B;
-      *reinterpret_cast<unsigned*>(t.scratch) = 0u;      // re-arm the ticket
-    }
-  }
+  tail_loss(l, t.B, t.scratch, t.loss);
 }
 
 // Q head weight/bias gradients: thread = one column j of h (j == 512 is the bias "ones" column), blockIdx.y = a group of consecutive
@@ -158,22 +141,13 @@ __global__ void __launch_bounds__(256) dqn_wgrad_reduce_kernel(const float* __re
   if (j < 512) gW[(size_t)a * 512 + j] = s; else if (!DUELING || a == 0) gb[a] = s; else gba[a - 1] = s;
 }
 
-// q_out[n][a] = Q(h[n])[a]: the tail's head arithmetic without the loss (one warp per frame).  Plain: h[n] . W[a] + b[a]; DUELING:
-// dueling_q with the value bias b and the advantage biases ba
-template <bool DUELING>
-__global__ void __launch_bounds__(128) dqn_q_values_kernel(const float* __restrict__ core, const float* __restrict__ W, const float* __restrict__ b,
-                                                           int N, int A, float* __restrict__ q_out, const float* __restrict__ ba) {
+// q_out[n][a] = Q(rows[n])[a] (q_lane: core rows, or the categorical head's logits), one warp per frame
+template <QKind KIND>
+__global__ void __launch_bounds__(128) q_values_kernel(const QHead h, const float* __restrict__ rows, int N, float* __restrict__ q_out) {
   const int lane = threadIdx.x & 31, n = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (n >= N) return;
-  if constexpr (DUELING) {
-    const float q = dueling_q<false>(core + (size_t)n * ENC_CORE, W, b, ba, A, lane, nullptr);
-    if (lane < A) q_out[(size_t)n * A + lane] = q;
-  } else {
-    for (int a = 0; a < A; ++a) {
-      const float v = q_dot(core + (size_t)n * ENC_CORE, W + (size_t)a * 512, lane) + __ldg(b + a);
-      if (lane == 0) q_out[(size_t)n * A + a] = v;
-    }
-  }
+  const float q = q_lane<KIND>(h, rows, n, lane);
+  if (lane < h.A) q_out[(size_t)n * h.A + lane] = q;
 }
 
 // theta_t = tau * theta + one_minus_tau * theta_t, each product and the sum rounded separately as torch computes it
@@ -183,28 +157,39 @@ __global__ void __launch_bounds__(256) apex_soft_update_kernel(const float* __re
     pt[i] = __fadd_rn(__fmul_rn(tau, p[i]), __fmul_rn(one_minus_tau, pt[i]));
 }
 
-cudaError_t launch_dqn_tail(const DqnTail& t, cudaStream_t st) {
-  if (t.dueling) dqn_tail_kernel<true><<<dqn_tail_blocks(t.B), 128, 0, st>>>(t);
-  else dqn_tail_kernel<false><<<dqn_tail_blocks(t.B), 128, 0, st>>>(t);
-  return cudaGetLastError();
-}
-cudaError_t launch_dqn_wgrad(const float* dq, const int64_t* action, const float* core, int N, int A, float* part, float* gW, float* gb,
-                             float* gba, cudaStream_t st) {
-  const int nslab = (N + DQN_SLAB - 1) / DQN_SLAB, spg = (nslab + HEAD_GROUPS - 1) / HEAD_GROUPS, groups = (nslab + spg - 1) / spg;
-  const dim3 grid((513 + 127) / 128, groups);
-  if (gba) {
-    dqn_wgrad_kernel<true><<<grid, 128, 0, st>>>(dq, action, core, N, A, spg, part);
-    dqn_wgrad_reduce_kernel<true><<<((A + 1) * 513 + 255) / 256, 256, 0, st>>>(part, groups, A, gW, gb, gba);
-  } else {
-    dqn_wgrad_kernel<false><<<grid, 128, 0, st>>>(dq, action, core, N, A, spg, part);
-    dqn_wgrad_reduce_kernel<false><<<(A * 513 + 255) / 256, 256, 0, st>>>(part, groups, A, gW, gb, nullptr);
+cudaError_t launch_q_tail(const QHead& on, const QHead& tg, const QTail& t, cudaStream_t st) {
+  switch (on.kind) {
+    case Q_PLAIN: dqn_tail_kernel<false><<<dqn_tail_blocks(t.B), 128, 0, st>>>(on, tg, t, 2.f / (float)t.B); break;
+    case Q_DUELING: dqn_tail_kernel<true><<<dqn_tail_blocks(t.B), 128, 0, st>>>(on, tg, t, 2.f / (float)t.B); break;
+    case Q_CATEGORICAL: return launch_cat_tail(on, tg, t, st);
   }
   return cudaGetLastError();
 }
-cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* b, const float* ba, int N, int A, float* q_out,
-                                cudaStream_t st) {
-  if (ba) dqn_q_values_kernel<true><<<(N + 3) / 4, 128, 0, st>>>(core, W, b, N, A, q_out, ba);
-  else dqn_q_values_kernel<false><<<(N + 3) / 4, 128, 0, st>>>(core, W, b, N, A, q_out, nullptr);
+cudaError_t launch_q_wgrad(const QHead& h, const QHeadGrad& g, const QTail& t, cudaStream_t st) {
+  if (h.kind == Q_CATEGORICAL) return launch_cat_wgrad(t.dlogits, t.core_s, t.B, h.R, g.gW, g.gb, st);
+  const int nslab = (t.B + DQN_SLAB - 1) / DQN_SLAB, spg = (nslab + HEAD_GROUPS - 1) / HEAD_GROUPS, groups = (nslab + spg - 1) / spg;
+  const dim3 grid((513 + 127) / 128, groups);
+  if (h.kind == Q_DUELING) {
+    dqn_wgrad_kernel<true><<<grid, 128, 0, st>>>(t.dq, t.action, t.core_s, t.B, h.A, spg, t.head_part);
+    dqn_wgrad_reduce_kernel<true><<<(h.R * 513 + 255) / 256, 256, 0, st>>>(t.head_part, groups, h.A, g.gW, g.gb, g.gba);
+  } else {
+    dqn_wgrad_kernel<false><<<grid, 128, 0, st>>>(t.dq, t.action, t.core_s, t.B, h.A, spg, t.head_part);
+    dqn_wgrad_reduce_kernel<false><<<(h.R * 513 + 255) / 256, 256, 0, st>>>(t.head_part, groups, h.A, g.gW, g.gb, nullptr);
+  }
+  return cudaGetLastError();
+}
+cudaError_t launch_q_values(const QHead& h, const float* core, int N, float* logits, float* q_out, cudaStream_t st) {
+  const int blocks = (N + 3) / 4;
+  switch (h.kind) {
+    case Q_PLAIN: q_values_kernel<Q_PLAIN><<<blocks, 128, 0, st>>>(h, core, N, q_out); break;
+    case Q_DUELING: q_values_kernel<Q_DUELING><<<blocks, 128, 0, st>>>(h, core, N, q_out); break;
+    case Q_CATEGORICAL: {
+      const cudaError_t e = launch_cat_logits(core, h.W, h.b, N, h.R, logits, st);
+      if (e != cudaSuccess) return e;
+      q_values_kernel<Q_CATEGORICAL><<<blocks, 128, 0, st>>>(h, logits, N, q_out);
+      break;
+    }
+  }
   return cudaGetLastError();
 }
 cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st) {

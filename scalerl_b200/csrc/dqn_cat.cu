@@ -7,7 +7,7 @@
 //   cat_tail_kernel         per transition: Q of the target (or, double DQN, the online) network at s', a*, the projection of
 //                           p_target(s')[a*], the cross-entropy, the KL priority, the loss through the ticket reduction, the dense
 //                           dlogits row and the dcore row of the encoder backward
-//   cat_q_values_kernel     the expected Q per action (predict / q_values)
+// dqn.cu's launchers call these for the categorical head (its q values: dqn.cu's q_values_kernel on the logits).
 // Every logit is one fmaf chain over j = 0 .. 511 from 0, then + bias rounded once; every other sum has a fixed order: eager, captured
 // and repeated runs compute the same bits, and no float atomics are used.
 #include "common.cuh"
@@ -91,20 +91,21 @@ __global__ void __launch_bounds__(256) cat_gemm_kernel(const CatGemm g) {
   }
 }
 
-// One warp per transition, 4 per block.  scratch: [0] the ticket, [4 + k] block k's partial of sum_n w_n ce_n (dqn_tail_kernel's).
-__global__ void __launch_bounds__(128) cat_tail_kernel(const CatTail t) {
+// One warp per transition, 4 per block: on = the online head.  scratch: [0] the ticket, [4 + k] block k's partial of sum_n w_n ce_n
+// (dqn_head.cuh's tail_loss).
+__global__ void __launch_bounds__(128) cat_tail_kernel(const QHead on, const QTail t, float inv_B) {
   __shared__ float sm[4][CAT_MAX_ATOMS], sd[4][CAT_MAX_ATOMS];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = blockIdx.x * 4 + warp;
   float l = 0.f;
   if (n < t.B) {
-    const int K = t.c.K, R = t.A * K;
-    const int act = ld_action(t.action + n, t.A);
+    const int K = on.c.K, R = on.R;
+    const int act = ld_action(t.action + n, on.A);
     const float w = t.weight ? __ldg(t.weight + n) : 1.f;
     float *m = sm[warp], *d = sd[warp];
-    const CatLoss r = cat_transition(t.logits_s + (size_t)n * R + (size_t)act * K, t.logits_n ? t.logits_n + (size_t)n * R : nullptr,
-                                     t.logits_nt + (size_t)n * R, t.A, __ldg(t.reward + n), t.done[n] ? 0.f : t.gamma, t.c, lane, m,
-                                     __fmul_rn(w, t.inv_B), d);
+    const CatLoss r = cat_transition(t.logits_s + (size_t)n * R + (size_t)act * K, t.core_n ? t.logits_n + (size_t)n * R : nullptr,
+                                     t.logits_nt + (size_t)n * R, on.A, __ldg(t.reward + n), t.done[n] ? 0.f : t.gamma, on.c, lane, m,
+                                     __fmul_rn(w, inv_B), d);
     if (lane == 0) {
       l = __fmul_rn(w, r.ce);
       t.q[n] = r.q; t.y[n] = r.y; t.ce[n] = r.ce;
@@ -122,7 +123,7 @@ __global__ void __launch_bounds__(128) cat_tail_kernel(const CatTail t) {
     for (int i = 0; i < 16; ++i) acc[i] = 0.f;
     for (int k = 0; k < K; ++k) {
       const float dk = d[k];
-      const float* wr = t.W + (size_t)(act * K + k) * 512;
+      const float* wr = on.W + (size_t)(act * K + k) * 512;
 #pragma unroll
       for (int i = 0; i < 16; ++i) acc[i] = fmaf(dk, __ldg(wr + lane + 32 * i), acc[i]);
     }
@@ -131,35 +132,7 @@ __global__ void __launch_bounds__(128) cat_tail_kernel(const CatTail t) {
     for (int i = 0; i < 16; ++i) dc[lane + 32 * i] = acc[i];
     if (lane < ENC_CORE - 512) dc[512 + lane] = 0.f;
   }
-  // block partial: the warps' losses in warp order, then the ticket; the last block adds the partials in block order
-  __shared__ float red[4];
-  __shared__ bool is_last;
-  if (lane == 0) red[warp] = l;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    t.scratch[4 + blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
-    is_last = take_ticket(t.scratch);
-  }
-  __syncthreads();
-  if (is_last && warp == 0) {
-    __threadfence();
-    float s = 0.f;
-    for (unsigned k = lane; k < gridDim.x; k += 32) s += reinterpret_cast<volatile float*>(t.scratch)[4 + k];
-    s = warp_sum(s);
-    if (lane == 0) {
-      t.loss[0] = s / (float)t.B;
-      *reinterpret_cast<unsigned*>(t.scratch) = 0u;      // re-arm the ticket
-    }
-  }
-}
-
-// q_out[n][a] = sum_k z_k p_k of frame n's logits, one warp per frame, one action per lane
-__global__ void __launch_bounds__(128) cat_q_values_kernel(const float* __restrict__ logits, int N, int A, const CatSupport c,
-                                                           float* __restrict__ q_out) {
-  const int lane = threadIdx.x & 31, n = blockIdx.x * 4 + (threadIdx.x >> 5);
-  if (n >= N) return;
-  const float q = cat_q_lane(logits + (size_t)n * A * c.K, A, c, lane);
-  if (lane < A) q_out[(size_t)n * A + lane] = q;
+  tail_loss(l, t.B, t.scratch, t.loss);
 }
 
 cudaError_t launch_cat_logits(const float* core, const float* W, const float* b, int N, int R, float* logits, cudaStream_t st) {
@@ -172,15 +145,13 @@ cudaError_t launch_cat_wgrad(const float* dlogits, const float* core, int N, int
   cat_gemm_kernel<true><<<dim3((513 + CG_BN - 1) / CG_BN, (R + CG_BM - 1) / CG_BM), 256, 0, st>>>(g);
   return cudaGetLastError();
 }
-cudaError_t launch_cat_tail(const CatTail& t, cudaStream_t st) {
-  cat_tail_kernel<<<dqn_tail_blocks(t.B), 128, 0, st>>>(t);
-  return cudaGetLastError();
-}
-cudaError_t launch_cat_q_values(const float* core, const float* W, const float* b, int N, int A, const CatSupport& c, float* logits,
-                                float* q_out, cudaStream_t st) {
-  const cudaError_t e = launch_cat_logits(core, W, b, N, A * c.K, logits, st);
+// the three logit sets (s and s' under the online head, s' under the target head), then the projection / cross-entropy tail
+cudaError_t launch_cat_tail(const QHead& on, const QHead& tg, const QTail& t, cudaStream_t st) {
+  cudaError_t e = launch_cat_logits(t.core_s, on.W, on.b, t.B, on.R, t.logits_s, st);
+  if (e == cudaSuccess && t.core_n) e = launch_cat_logits(t.core_n, on.W, on.b, t.B, on.R, t.logits_n, st);
+  if (e == cudaSuccess) e = launch_cat_logits(t.core_nt, tg.W, tg.b, t.B, tg.R, t.logits_nt, st);
   if (e != cudaSuccess) return e;
-  cat_q_values_kernel<<<(N + 3) / 4, 128, 0, st>>>(logits, N, A, c, q_out);
+  cat_tail_kernel<<<dqn_tail_blocks(t.B), 128, 0, st>>>(on, t, 1.f / (float)t.B);
   return cudaGetLastError();
 }
 

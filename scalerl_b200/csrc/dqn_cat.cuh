@@ -38,6 +38,24 @@ SRL_DEVINL float cat_q(const float* __restrict__ x, const CatSupport& c) {
 SRL_DEVINL float cat_q_lane(const float* __restrict__ row, int A, const CatSupport& c, int lane) {
   return lane < A ? cat_q(row + (size_t)lane * c.K, c) : 0.f;
 }
+// the Q row of frame n, one action per lane (lane a < A: Q_a), for every head: rows = the core rows [N][ENC_CORE] (scalar heads) or the
+// logits [N][A K] (categorical).  The plain head's dot products end in warp_sum, whose xor butterfly leaves the same sum on every lane,
+// so lane a holds the value q_max compares at a.
+template <QKind KIND>
+SRL_DEVINL float q_lane(const QHead& h, const float* rows, size_t n, int lane) {
+  if constexpr (KIND == Q_CATEGORICAL) {
+    return cat_q_lane(rows + n * h.R, h.A, h.c, lane);
+  } else if constexpr (KIND == Q_DUELING) {
+    return dueling_q<false>(rows + n * ENC_CORE, h.W, h.b, h.ba, h.A, lane, nullptr);
+  } else {
+    float mine = 0.f;
+    for (int a = 0; a < h.A; ++a) {
+      const float v = q_dot(rows + n * ENC_CORE, h.W + (size_t)a * 512, lane) + __ldg(h.b + a);
+      if (lane == a) mine = v;
+    }
+    return mine;
+  }
+}
 
 // Algorithm 1 of Bellemare et al. 2017 on one lane: m[0 .. K-1] <- the projection onto the support of the target distribution p' (the
 // softmax of x's K logits) moved to Tz_j = clamp(r + g z_j, v_min, v_max), g = gamma (1 - d).  b_j = (Tz_j - v_min) / dz, l = floor(b_j)

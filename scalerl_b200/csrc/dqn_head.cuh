@@ -14,10 +14,13 @@ SRL_DEVINL float q_dot(const float* __restrict__ h, const float* __restrict__ w,
   for (int i = 0; i < 16; ++i) s = fmaf(__ldg(h + lane + 32 * i), __ldg(w + lane + 32 * i), s);
   return warp_sum(s);
 }
-// max_a Q(h)[a] and its first argmax (torch.max(dim=1) returns the first maximal index)
+// max_a Q(h)[a] and its first argmax (torch.max(dim=1) returns the first maximal index).  UNROLL rows in flight: the learner's tail
+// takes 2, since its loop is bound by the weight rows' load latency
+template <int UNROLL = 1>
 SRL_DEVINL float q_max(const float* h, const float* W, const float* b, int A, int lane, int* arg) {
   float best = -INFINITY;
   int ib = 0;
+#pragma unroll UNROLL
   for (int a = 0; a < A; ++a) {
     const float v = q_dot(h, W + (size_t)a * 512, lane) + __ldg(b + a);
     if (v > best) { best = v; ib = a; }
@@ -70,5 +73,31 @@ SRL_DEVINL float td_target(float reward, float gamma, float next_q, bool done) {
 }
 // |q - y| + eps in double (apex/worker.py:152-154; + eps > 0 keeps the tree's assert), from delta = q - y
 SRL_DEVINL double td_priority(float delta, float eps) { return (double)fabsf(delta) + (double)eps; }
+
+// The learner tails' loss (one warp per transition, 4 per block; every thread of every block calls it with l = its warp's weighted loss
+// on lane 0): the block partial (l0 + l1) + (l2 + l3) goes to scratch[4 + block], then the ticket scratch[0]; the last block adds the
+// partials lane-strided in block order, then the warp sum, and writes loss[0] = sum / B and re-arms the ticket.
+SRL_DEVINL void tail_loss(float l, int B, float* scratch, float* loss) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __shared__ float red[4];
+  __shared__ bool is_last;
+  if (lane == 0) red[warp] = l;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    scratch[4 + blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
+    is_last = take_ticket(scratch);
+  }
+  __syncthreads();
+  if (is_last && warp == 0) {
+    __threadfence();
+    float s = 0.f;
+    for (unsigned k = lane; k < gridDim.x; k += 32) s += reinterpret_cast<volatile float*>(scratch)[4 + k];
+    s = warp_sum(s);
+    if (lane == 0) {
+      loss[0] = s / (float)B;
+      *reinterpret_cast<unsigned*>(scratch) = 0u;      // re-arm the ticket
+    }
+  }
+}
 
 }  // namespace srl

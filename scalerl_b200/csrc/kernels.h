@@ -216,39 +216,11 @@ cudaError_t launch_rmsprop(float* p, const float* g, float* v, int64_t n, const 
 cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, const float* coef, float lr, float b1, float b2, float eps,
                         int step, cudaStream_t st);
 
-// ---- dqn.cu: the Q-learning tail of the Ape-X learner step (srl_apex_learner_*)
+// ---- dqn.cu, dqn_cat.cu: the Q head of the Ape-X learner step and actors (srl_apex_*)
 // The encoder runs with a one-hot width of 1 for the Q network: its core rows are [h (512), clamp(reward), 1], ENC_CORE floats.
 constexpr int ENC_CORE = 514;
-// one batch of B transitions: core rows of the online forward over s, the online forward over s' (null: plain max, no double DQN) and
-// the target forward over s'; the Q heads [A][512] + [A]; the batch columns; outputs q, y, dq f32 [B], priorities f64 [B], dcore
-// [B][ENC_CORE] and loss f32 [1].  scratch: 4 + dqn_tail_blocks(B) floats, zero before the first launch (re-armed by the kernel).
-// dueling: W* = [(A + 1)][512] (value row, then the advantage rows), b* = the value bias [1], b*a = the advantage biases [A]
-// (dqn_head.cuh's dueling_q); the plain head leaves bqa / bta unused.
-struct DqnTail {
-  const float *core_s, *core_n, *core_nt;
-  const float *Wq, *bq, *Wt, *bt;
-  const int64_t* action; const float* reward; const uint8_t* done; const float* weight;
-  int B, A;
-  float gamma, two_over_B, priority_eps;
-  float *q, *y, *dq, *dcore, *loss, *scratch;
-  double* prio;
-  const float *bqa, *bta;
-  int dueling;
-};
-inline int dqn_tail_blocks(int B) { return (B + 3) / 4; }
-cudaError_t launch_dqn_tail(const DqnTail& t, cudaStream_t st);
-// the Q head gradients (stored) from dq and the actions over the core rows.  Plain head (gba NULL): gW [A][512], gb [A]; part:
-// HEAD_GROUPS * A * 513 floats.  Dueling head (gba set): gW [(A + 1)][512] (value row first), gb [1] the value bias, gba [A] the
-// advantage biases; part: HEAD_GROUPS * (A + 1) * 513 floats.
-cudaError_t launch_dqn_wgrad(const float* dq, const int64_t* action, const float* core, int N, int A, float* part, float* gW, float* gb,
-                             float* gba, cudaStream_t st);
-// q_out [N][A] = Q(h) of the plain head (ba NULL) or of the dueling head (W [(A + 1)][512], b the value bias, ba the advantage biases)
-cudaError_t launch_dqn_q_values(const float* core, const float* W, const float* b, const float* ba, int N, int A, float* q_out,
-                                cudaStream_t st);
-cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
-
-// ---- dqn_cat.cu: the categorical (C51) Q head, q = Linear(512, A K), K atoms on the support z_k = v_min + k dz (dqn_cat.cuh)
 constexpr int CAT_MAX_ATOMS = 64;
+// the categorical head's support z_k = v_min + k dz (dqn_cat.cuh)
 struct CatSupport {
   float v_min, v_max, dz;
   int K;
@@ -257,31 +229,66 @@ struct CatSupport {
 inline CatSupport cat_support(int K, float v_min, float v_max) {
   return {v_min, v_max, (float)(((double)v_max - (double)v_min) / (double)(K - 1)), K};
 }
-// api.cu: the checks of a head setting shared by the learner and the actor (num_atoms 0: a scalar head, nothing else is read).  0, or
-// SRL_EINVAL with "<who>: ..." as the message
-int check_cat_head(const char* who, int num_atoms, float v_min, float v_max, int dueling);
-// one batch of B transitions on the categorical head: the logits [B][A K] of the online network over s, of the online network over s'
-// (null: no double DQN) and of the target network over s'; the online head weights W [A K][512] (dcore); the batch columns; outputs q
-// (sum z p at the taken action), y (sum z m), ce f32 [B], m f32 [B][K], dlogits f32 [B][A K] (zero outside the taken action's K
-// rows), dcore f32 [B][ENC_CORE], priorities f64 [B] and loss f32 [1] = mean(w ce); scratch as DqnTail's
-struct CatTail {
-  const float *logits_s, *logits_n, *logits_nt, *W;
-  const int64_t* action; const float* reward; const uint8_t* done; const float* weight;
-  int B, A;
+enum QKind { Q_PLAIN, Q_DUELING, Q_CATEGORICAL };
+// One Q head on the 512 h columns of the core rows, bound onto a flat parameter buffer (apex_layout order):
+//   Q_PLAIN        q = Linear(512, A): W = q.weight [A][512], b = q.bias [A]
+//   Q_DUELING      V + Adv - mean(Adv) (dqn_head.cuh's dueling_q): W = [value.weight; advantage.weight] [(A + 1)][512] (the value row
+//                  first), b = value.bias [1], ba = advantage.bias [A]
+//   Q_CATEGORICAL  C51, q = Linear(512, A K) (dqn_cat.cuh): W = q.weight [A K][512], b = q.bias [A K] (row a K + k: atom k of action
+//                  a) on the support c
+// R = W's rows: A, A + 1 or A K.
+struct QHead {
+  QKind kind;
+  int A, R;
+  const float *W, *b, *ba;
   CatSupport c;
-  float gamma, inv_B, priority_eps;
-  float *q, *y, *ce, *m, *dlogits, *dcore, *loss, *scratch;
-  double* prio;
 };
-cudaError_t launch_cat_tail(const CatTail& t, cudaStream_t st);
+// the same tensors of a gradient buffer
+struct QHeadGrad {
+  float *gW, *gb, *gba;
+};
+// api.cu: the head a setting describes (num_atoms 0: a scalar head, whose support is not read), unbound.  0, or SRL_EINVAL with
+// "<who>: ..." as the message
+int make_q_head(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, QHead* h);
+// api.cu: the flat parameter layout of the Q network with head h (srl_apex_param_layout*'s): the offsets and counts (NULL: not wanted)
+// of its 10 (12: dueling) tensors -> the buffer's floats
+int64_t apex_layout(const QHead& h, int64_t* off, int64_t* cnt);
+// api.cu: h bound onto the flat parameter buffer `params` of its layout, and onto a gradient buffer of that layout
+QHead bind_q_head(QHead h, const float* params);
+QHeadGrad bind_q_grad(const QHead& h, float* grads);
+
+// One batch of B transitions: the core rows of the online forward over s, of the online forward over s' (NULL: no double DQN) and of
+// the target forward over s'; the batch columns; outputs q (Q(s, a); categorical: sum z p at the taken action), y (the target;
+// categorical: sum z m), priorities f64 [B], dcore [B][ENC_CORE] and loss [1] (mean(w (q - y)^2); categorical: mean(w ce)).
+// scratch: 4 + dqn_tail_blocks(B) floats, zero before the first launch (re-armed by the kernel).  The scalar heads write dq [B] and
+// reduce the head gradients through head_part (HEAD_GROUPS * R * 513 floats); the categorical head writes the logits [B][A K] of the
+// three forwards (logits_n: double DQN only), the projected targets m [B][K], ce [B] and dlogits [B][A K] (zero outside the taken
+// action's K rows).
+struct QTail {
+  const float *core_s, *core_n, *core_nt;
+  const int64_t* action; const float* reward; const uint8_t* done; const float* weight;
+  int B;
+  float gamma, priority_eps;
+  float *q, *y, *dcore, *loss, *scratch;
+  double* prio;
+  float *dq, *head_part;
+  float *logits_s, *logits_n, *logits_nt, *m, *ce, *dlogits;
+};
+inline int dqn_tail_blocks(int B) { return (B + 3) / 4; }
+// the tail of `on` (the online head) and `tg` (the target head); the categorical head runs its logits GEMMs first
+cudaError_t launch_q_tail(const QHead& on, const QHead& tg, const QTail& t, cudaStream_t st);
+// the head gradients (stored) of the tail t has run
+cudaError_t launch_q_wgrad(const QHead& h, const QHeadGrad& g, const QTail& t, cudaStream_t st);
+// q_out [N][A] = Q(h) over N core rows; the categorical head goes through logits [N][A K]
+cudaError_t launch_q_values(const QHead& h, const float* core, int N, float* logits, float* q_out, cudaStream_t st);
+cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
+// dqn_cat.cu: the categorical halves of the launchers above
 // logits [N][R] = h W^T + b over N core rows (stride ENC_CORE), W [R][512]: one fmaf chain per logit over j = 0 .. 511 from 0, then
 // + b rounded once, whatever the tiling
 cudaError_t launch_cat_logits(const float* core, const float* W, const float* b, int N, int R, float* logits, cudaStream_t st);
+cudaError_t launch_cat_tail(const QHead& on, const QHead& tg, const QTail& t, cudaStream_t st);
 // gW [R][512] = dlogits^T h, gb [R] = dlogits^T 1 over the N core rows (stored), each a fmaf chain over n = 0 .. N-1 in order
 cudaError_t launch_cat_wgrad(const float* dlogits, const float* core, int N, int R, float* gW, float* gb, cudaStream_t st);
-// q_out [N][A] = the expected Q of the categorical head over N core rows, through logits [N][A K]
-cudaError_t launch_cat_q_values(const float* core, const float* W, const float* b, int N, int A, const CatSupport& c, float* logits,
-                                float* q_out, cudaStream_t st);
 
 }  // namespace srl
 struct srl_per;
