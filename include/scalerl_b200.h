@@ -405,6 +405,8 @@ typedef struct srl_apex_config {
   int32_t dueling;           /* 0: q = Linear(512, A); 1: the dueling head Q = V + Adv - mean(Adv)             */
   int32_t num_atoms;         /* 0: a scalar Q head; K in [2, 64]: the categorical head (not with dueling = 1)  */
   float v_min, v_max;        /* the categorical support [v_min, v_max], finite, v_min < v_max (read when num_atoms > 0) */
+  int32_t noisy;             /* 0: plain layers; 1: noisy fc and head layers (srl_apex_param_layout_noisy)        */
+  uint64_t noise_seed;       /* the Philox key of the noise (read when noisy = 1)                                */
 } srl_apex_config_t;
 int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10);
 /* the layout of either head: dueling 0 -> 10 tensors (srl_apex_param_layout's), 1 -> 12; -1 with srl_last_error set for A outside
@@ -413,6 +415,14 @@ int64_t srl_apex_param_layout_ex(int A, int dueling, int64_t* offsets12, int64_t
 /* the 10-tensor layout with q.weight [A num_atoms, 512] and q.bias [A num_atoms] (num_atoms 0: srl_apex_param_layout's); -1 with
  * srl_last_error set for A outside [1, 31] or num_atoms outside {0} and [2, 64] */
 int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offsets10, int64_t* counts10);
+/* The layout of every head, with or without noisy networks (Fortunato et al. 2018, factorised Gaussian noise): noisy = 0 gives
+ * srl_apex_param_layout_ex / _cat's (dueling and num_atoms > 0 together are refused); noisy = 1 replaces fc and each head layer
+ * <l> by <l>.weight_mu, <l>.weight_sigma, <l>.bias_mu, <l>.bias_sigma in that order: {conv1..3 (6), fc (4), q (4)} = 14 tensors,
+ * or {conv1..3, fc, value (4), advantage (4)} = 18 with the dueling head.  Each noisy layer computes
+ *   y = (mu_w + sigma_w (.) eps_w) x + mu_b + sigma_b (.) eps_b,  eps_w = f(eps_out) f(eps_in)^T,  eps_b = f(eps_out),  f(x) = sgn(x) sqrt|x|
+ * In memory the biases come first, then the head weights (value.weight_mu directly before advantage.weight_mu, and the same for
+ * sigma), then fc.weight_mu and fc.weight_sigma; segments padded to 4 floats.  -> the buffer's floats, or -1 with srl_last_error set */
+int64_t srl_apex_param_layout_noisy(int A, int dueling, int num_atoms, int noisy, int64_t* offsets18, int64_t* counts18);
 /* params / grads / exp_avg / exp_avg_sq / target_params: caller-owned flat f32 device buffers of srl_apex_param_layout floats,
  * 16-byte aligned and disjoint.  The context owns the encoder's blocks (one saved block for the forward over s, one for the
  * forwards over s', their scratch) and the tail's buffers.  Synchronous. */
@@ -429,6 +439,10 @@ int srl_apex_learner_destroy(srl_apex_learner_t* L);
  *   support (Algorithm 1, j ascending);  ce = -sum_k m_k log p(s)[a, k];  loss = mean(w ce);  priority = max(KL(m || p(s)[a]), 0) +
  *   priority_eps (Hessel et al. 2018).  q holds sum_k z_k p(s)[a, k], y holds sum_k z_k m_k.
  *   clip_grad_norm_(max_grad_norm), torch.optim.Adam step with the step count kept on the device       (dqn_agent.py:172-182)
+ * With noisy = 1 update k (the device step count before the update) first draws the noise of both networks: standard normals from
+ * Philox4x32-10 keyed by noise_seed, counted by (k, network), Box-Muller.  The online network's one draw per layer serves Q(s) and the
+ * double-DQN choice at s'; the target network's draw is independent.  The step runs on the composed weights mu + sigma (.) eps; their
+ * gradients are the mu gradients, and the sigma gradients are dW (.) eps and db (.) f(eps_out), before the clip and Adam.
  * stats_out: f32 [3] device = {loss, gradient norm, clip coefficient} (may be NULL).  No host synchronisation; capturable. */
 int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, const int64_t* action, const float* reward, const uint8_t* next_obs,
                           const uint8_t* done, const float* weights, const int64_t* idxs, srl_per_t* per, float* stats_out, void* stream);
@@ -446,7 +460,12 @@ int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* obs, int n, 
  * h = columns < 512), "dcore" f32 [B,514], "q", "y" f32 [B], "priorities" f64 [B], "loss" f32 [1], "step" i32 [1] (device step count),
  * and the bf16 activations the forward over s saved, in the learner's layouts (srl_learner_debug_buffer): "a1", "a2", "a3".
  * The categorical head adds "logits", "logits_next" (double DQN only), "logits_next_target" and "dlogits" f32 [B,A*K], "m" f32 [B,K]
- * (the projected targets) and "ce" f32 [B] (the cross-entropies); its "y" is sum_k z_k m_k. */
+ * (the projected targets) and "ce" f32 [B] (the cross-entropies); its "y" is sum_k z_k m_k.
+ * Noisy networks add, per network <n> = "online" or "target", the last step's "normals_<n>" (the standard normals) and "noise_<n>"
+ * (f of them) f32 [NN] = [fc in 3136 | fc out 512 | head in 512 (dueling: value's, then advantage's) | head out R (dueling: value's 1,
+ * then advantage's A)], R = the head's rows (A, A K, or A + 1), and the composed weights "fc_weight_<n>" [512,3136], "fc_bias_<n>"
+ * [512], "head_weight_<n>" [R,512], "head_bias_<n>" ([R]; dueling: the value bias [1]) and "head_adv_bias_<n>" (dueling: [A]).
+ * srl_apex_learner_q_values reads the mean weights mu (NoisyLinear's eval mode). */
 int srl_apex_learner_debug_buffer(srl_apex_learner_t* L, const char* name, void** ptr, int64_t* count);
 
 /* ---- Ape-X actor: per-env epsilon-greedy acting and actor-computed initial priorities (apex/worker.py:59-79, apex/memory.py:43-64) --
@@ -465,6 +484,12 @@ int srl_apex_actor_create_ex(int A, int num_envs, int precision, int dueling, ui
  * priorities max(KL(m || p(s)[a]), 0) + priority_eps with the snapshot as online and target network (srl_apex_learner_step's bits) */
 int srl_apex_actor_create_cat(int A, int num_envs, int precision, int num_atoms, float v_min, float v_max, uint64_t seed, const float* params,
                               srl_apex_actor_t** out);
+/* the same for every head: dueling, num_atoms, v_min, v_max as srl_apex_config_t's, and noisy (0 or 1); params in
+ * srl_apex_param_layout_noisy(A, dueling, num_atoms, noisy) order.  A noisy actor keeps one noise draw (Philox keyed by seed, counted by
+ * a device noise counter, shared by all envs): create draws the first, every act draws a new one before its forward, and q_values and
+ * the prioritized add compose the kept draw with the snapshot as it is when they run. */
+int srl_apex_actor_create_noisy(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int noisy,
+                                uint64_t seed, const float* params, srl_apex_actor_t** out);
 int srl_apex_actor_destroy(srl_apex_actor_t* X);
 /* obs u8 [E,4,84,84], epsilons f32 [E] (device) -> actions i64 [E]: with probability epsilons[e] a uniform action, else the first
  * argmax of Q(obs[e]) (torch.argmax's pick).  The random numbers are Philox4x32-10 keyed by seed, counted by (draw, env); the launch
@@ -473,7 +498,9 @@ int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const float* eps
 /* Q(obs) with the snapshot for n >= 1 frames: obs u8 [n,4,84,84] -> q_out f32 [n,A] */
 int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, int n, float* q_out, void* stream);
 /* borrow the actor's buffers for tests: "core" f32 [2E,514] (rows 0..E-1: the last act or the states of the last prioritized add,
- * rows E..2E-1: its next states) and, categorical head only, "logits" f32 [2E,A*K] of the same rows */
+ * rows E..2E-1: its next states) and, categorical head only, "logits" f32 [2E,A*K] of the same rows.  A noisy actor adds its kept draw
+ * "normals" and "noise" and the weights its last call composed, "fc_weight", "fc_bias", "head_weight", "head_bias" and (dueling)
+ * "head_adv_bias", in the layouts of srl_apex_learner_debug_buffer's */
 int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name, void** ptr, int64_t* count);
 /* srl_replay_add, then, for the E transitions the call completes, their initial priorities computed by `actor` (built for the memory's
  * num_envs) instead of max_priority:  p = |Q(s)[a] - y| + priority_eps,  y = R + fp32(gamma^n_step) (1 - d) max_a Q(s')  with the

@@ -15,6 +15,9 @@ epsilon, from a parameter snapshot on the device (srl_apex_actor_*, csrc/apex_ac
 ``dueling_dqn=True`` gives the actor the dueling head of ``ApexHParams(dueling_dqn=True)``; it syncs from dueling learners only.
 ``categorical_dqn=True`` (with ``v_min``, ``v_max``, ``num_atoms``) gives it the categorical head of ``ApexHParams(categorical_dqn=True)``:
 it acts on the expected Q and prioritises by the learner's KL divergence, and syncs from learners with the same atoms and support only.
+``noisy_dqn=True`` gives it the noisy layers of ``ApexHParams(noisy_dqn=True)`` (with any head): every ``act`` draws new noise for the
+snapshot before its forward (one draw for all envs, from ``seed`` and a device counter, so a captured ``act`` draws anew on every
+replay) and keeps it; ``q_values`` and the prioritized add use the kept draw on the snapshot as it is.  Its default epsilons are 0.
 """
 from __future__ import annotations
 
@@ -46,14 +49,16 @@ class B200ApexActor:
     """``num_envs`` Ape-X actors on one GPU, acting on a snapshot of a ``B200ApexLearner``'s Q network (``AtariQNet`` names and
     shapes).  ``epsilons``: [num_envs] values in [0, 1] (None: ``apex_epsilons(num_envs)``); ``precision``: the encoder operands, as
     the learner's; ``priority_eps`` (> 0) is added to every priority the actor computes; ``dueling_dqn``, ``categorical_dqn`` (with
-    ``v_min``, ``v_max``, ``num_atoms``): the learner's head.  Calls run on the current stream and share the actor's buffers: issue them
-    from one stream."""
+    ``v_min``, ``v_max``, ``num_atoms``), ``noisy_dqn`` (with ``noisy_std``, the initial sigma0 of the default weights): the learner's head
+    (noisy: epsilons None means 0 for every env).  Calls run on the current stream and share the actor's buffers: issue them from one
+    stream."""
     # the head settings as the constructor stores them; the class values are its defaults
-    dueling_dqn, categorical_dqn, v_min, v_max, num_atoms = False, False, 0.0, 200.0, 51
+    dueling_dqn, categorical_dqn, v_min, v_max, num_atoms, noisy_dqn = False, False, 0.0, 200.0, 51, False
 
     def __init__(self, num_envs: int, num_actions: int, epsilons=None, seed: int = 0, precision: str = 'bf16', priority_eps: float = 1e-6,
                  device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None, dueling_dqn: bool = False,
-                 categorical_dqn: bool = False, v_min: float = 0.0, v_max: float = 200.0, num_atoms: int = 51):
+                 categorical_dqn: bool = False, v_min: float = 0.0, v_max: float = 200.0, num_atoms: int = 51, noisy_dqn: bool = False,
+                 noisy_std: float = 0.5):
         for name, v, hi in (('num_envs', num_envs, MAX_FRAMES), ('num_actions', num_actions, 31)):
             if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= hi:
                 raise ValueError(f'{name} must be an int in [1, {hi}], got {v!r}')
@@ -61,14 +66,19 @@ class B200ApexActor:
             raise ValueError(f'seed must be an int in [0, 2**64), got {seed!r}')
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be 'bf16' or 'fp32_split', got {precision!r}")
-        head = QHead.of(dueling_dqn, categorical_dqn, num_atoms, v_min, v_max)
+        head = QHead.of(dueling_dqn, categorical_dqn, num_atoms, v_min, v_max, noisy_dqn)
+        if isinstance(noisy_std, bool) or not isinstance(noisy_std, (int, float)) or not (math.isfinite(noisy_std) and noisy_std >= 0.0):
+            raise ValueError(f'noisy_std must be finite and >= 0, got {noisy_std!r}')
         priority_eps = float(priority_eps)
         if not (math.isfinite(priority_eps) and priority_eps > 0.0):
             raise ValueError(f'priority_eps must be finite and > 0 (a zero leaf makes the sampler\'s IS weight infinite), got {priority_eps}')
         self.num_envs, self.num_actions, self.seed, self.precision = int(num_envs), int(num_actions), int(seed), precision
         self.priority_eps, self.dueling_dqn, self.categorical_dqn = priority_eps, dueling_dqn, categorical_dqn
         self.v_min, self.v_max, self.num_atoms = float(v_min), float(v_max), int(num_atoms)
-        eps = self._epsilons(apex_epsilons(self.num_envs) if epsilons is None else epsilons)
+        self.noisy_dqn = noisy_dqn
+        if epsilons is None:
+            epsilons = np.zeros(self.num_envs) if noisy_dqn else apex_epsilons(self.num_envs)
+        eps = self._epsilons(epsilons)
         if not torch.cuda.is_available():
             raise RuntimeError('B200ApexActor needs a CUDA device: scalerl_b200 has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
@@ -80,13 +90,14 @@ class B200ApexActor:
             self.params = flat_views(self.flat_params, off, cnt, self.shapes)
             self.epsilons = eps.to(self.device)           # read by the act kernel when it runs
             self._h = _lib.apex_actor_create(self.num_actions, self.num_envs, PRECISIONS[precision], self.seed, self.flat_params.data_ptr(), head)
-        sd = default_q_state_dict(self.num_actions, self.seed, head.dueling, head.num_atoms) if init_state_dict is None else init_state_dict
+        sd = default_q_state_dict(self.num_actions, self.seed, head.dueling, head.num_atoms, head.noisy, noisy_std) \
+            if init_state_dict is None else init_state_dict
         self.load_state_dict(sd)
         self.weights_version = 0
 
     @property
     def head(self) -> QHead:
-        return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max)
+        return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max, self.noisy_dqn)
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
@@ -141,7 +152,7 @@ class B200ApexActor:
     @torch.no_grad()
     def act(self, obs) -> torch.Tensor:
         """obs uint8 [num_envs, 4, 84, 84] (a host array or tensor is copied on the current stream) -> int64 [num_envs] on the device:
-        per env, a uniform action with probability epsilons[e], else the first argmax of Q(obs[e])"""
+        per env, a uniform action with probability epsilons[e], else the first argmax of Q(obs[e]) (noisy: under a new noise draw)"""
         obs = self._obs(obs, self.num_envs)
         actions = torch.empty(self.num_envs, dtype=torch.int64, device=self.device)
         _lib.check(self._L.srl_apex_actor_act(self._h, obs.data_ptr(), self.epsilons.data_ptr(), actions.data_ptr(), self._stream()),

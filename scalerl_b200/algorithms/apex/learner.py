@@ -16,6 +16,11 @@ fc output (the paper's Atari network gives each stream an fc layer of its own), 
 a softmax over each action's ``num_atoms`` logits on the support ``z_k = v_min + k dz``, Q = sum_k z_k p_k for acting and the greedy
 target, and the cross-entropy against the projected target distribution as the loss.  Priorities are the KL divergence of the target
 from the online distribution (Hessel et al. 2018).  The state-dict names stay the plain head's ten.
+
+``ApexHParams(noisy_dqn=True)`` makes fc and every head layer a noisy layer (Fortunato et al. 2018, factorised Gaussian noise):
+``y = (mu_w + sigma_w * eps_w) x + mu_b + sigma_b * eps_b`` with ``eps_w = f(eps_out) f(eps_in)^T``, ``eps_b = f(eps_out)`` and
+``f(x) = sgn(x) sqrt|x|``.  Update k draws new noise for the online network (shared by Q(s) and the double-DQN choice at s') and an
+independent draw for the target network, both from (seed, k); ``q_values``, ``predict`` and ``get_action`` use the mean weights mu.
 """
 from __future__ import annotations
 
@@ -40,21 +45,85 @@ APEX_PARAM_NAMES = ('conv1.weight', 'conv1.bias', 'conv2.weight', 'conv2.bias', 
                     'fc.weight', 'fc.bias', 'q.weight', 'q.bias')
 # the same for the dueling head (srl_apex_param_layout_ex(A, 1) order)
 APEX_DUELING_PARAM_NAMES = APEX_PARAM_NAMES[:8] + ('value.weight', 'value.bias', 'advantage.weight', 'advantage.bias')
+NOISY_SUFFIXES = ('weight_mu', 'weight_sigma', 'bias_mu', 'bias_sigma')     # NoisyLinear's parameters, in registration order
+# the noisy networks (srl_apex_param_layout_noisy order): fc and each head layer as NoisyLinear
+APEX_NOISY_PARAM_NAMES = APEX_PARAM_NAMES[:6] + tuple(f'{l}.{s}' for l in ('fc', 'q') for s in NOISY_SUFFIXES)
+APEX_NOISY_DUELING_PARAM_NAMES = APEX_PARAM_NAMES[:6] + tuple(f'{l}.{s}' for l in ('fc', 'value', 'advantage') for s in NOISY_SUFFIXES)
 MAX_FRAMES = 65536           # frames of one encoder call (MAX_FRAMES in csrc/kernels.h)
 
 
-def apex_param_names(dueling: bool = False):
+def apex_param_names(dueling: bool = False, noisy: bool = False):
+    if noisy:
+        return APEX_NOISY_DUELING_PARAM_NAMES if dueling else APEX_NOISY_PARAM_NAMES
     return APEX_DUELING_PARAM_NAMES if dueling else APEX_PARAM_NAMES
 
 
-def apex_param_shapes(num_actions: int, dueling: bool = False, num_atoms: int = 0):
-    """the named shapes of the Q network's parameters; num_atoms > 0: the categorical head q = Linear(512, num_actions * num_atoms)"""
+def apex_param_shapes(num_actions: int, dueling: bool = False, num_atoms: int = 0, noisy: bool = False):
+    """the named shapes of the Q network's parameters; num_atoms > 0: the categorical head q = Linear(512, num_actions * num_atoms);
+    noisy: each of fc and the head layers as NoisyLinear's weight_mu, weight_sigma, bias_mu, bias_sigma"""
     R = num_actions * num_atoms if num_atoms else num_actions
-    head = [('value.weight', (1, 512)), ('value.bias', (1,)), ('advantage.weight', (num_actions, 512)), ('advantage.bias', (num_actions,))] \
-        if dueling else [('q.weight', (R, 512)), ('q.bias', (R,))]
-    return OrderedDict([
-        ('conv1.weight', (32, 4, 8, 8)), ('conv1.bias', (32,)), ('conv2.weight', (64, 32, 4, 4)), ('conv2.bias', (64,)),
-        ('conv3.weight', (64, 64, 3, 3)), ('conv3.bias', (64,)), ('fc.weight', (512, 3136)), ('fc.bias', (512,))] + head)
+    layers = [('fc', 512, 3136)] + ([('value', 1, 512), ('advantage', num_actions, 512)] if dueling else [('q', R, 512)])
+    conv = [('conv1.weight', (32, 4, 8, 8)), ('conv1.bias', (32,)), ('conv2.weight', (64, 32, 4, 4)), ('conv2.bias', (64,)),
+            ('conv3.weight', (64, 64, 3, 3)), ('conv3.bias', (64,))]
+    if noisy:
+        return OrderedDict(conv + [(f'{l}.{s}', (o, i) if s.startswith('weight') else (o,)) for l, o, i in layers for s in NOISY_SUFFIXES])
+    return OrderedDict(conv + [p for l, o, i in layers for p in ((f'{l}.weight', (o, i)), (f'{l}.bias', (o,)))])
+
+
+def scale_noise(x: torch.Tensor) -> torch.Tensor:
+    """f(x) = sgn(x) sqrt|x| of factorised Gaussian noise"""
+    return x.sign().mul(x.abs().sqrt())
+
+
+class NoisyLinear(nn.Module):
+    """The factorised Gaussian noisy layer of Fortunato et al. 2018: in train mode ``y = (weight_mu + weight_sigma * weight_epsilon) x
+    + bias_mu + bias_sigma * bias_epsilon`` with ``weight_epsilon = outer(eps_out, eps_in)`` and ``bias_epsilon = eps_out``, the f-scaled
+    noise vectors (non-persistent buffers, redrawn by ``reset_noise()`` or set by ``set_noise``); in eval mode ``y = weight_mu x +
+    bias_mu``.  Init (section 3.2): mu ~ U[-1/sqrt(p), 1/sqrt(p)], sigma = std_init / sqrt(p), p = in_features."""
+
+    def __init__(self, in_features: int, out_features: int, std_init: float = 0.5):
+        super().__init__()
+        self.in_features, self.out_features, self.std_init = int(in_features), int(out_features), float(std_init)
+        self.weight_mu = nn.Parameter(torch.empty(out_features, in_features))
+        self.weight_sigma = nn.Parameter(torch.empty(out_features, in_features))
+        self.bias_mu = nn.Parameter(torch.empty(out_features))
+        self.bias_sigma = nn.Parameter(torch.empty(out_features))
+        self.register_buffer('eps_in', torch.zeros(in_features), persistent=False)
+        self.register_buffer('eps_out', torch.zeros(out_features), persistent=False)
+        self.register_buffer('weight_epsilon', torch.zeros(out_features, in_features), persistent=False)
+        self.register_buffer('bias_epsilon', torch.zeros(out_features), persistent=False)
+        self.reset_parameters()
+        self.reset_noise()
+
+    def reset_parameters(self) -> None:
+        r = 1.0 / math.sqrt(self.in_features)
+        with torch.no_grad():
+            self.weight_mu.uniform_(-r, r)
+            self.weight_sigma.fill_(self.std_init / math.sqrt(self.in_features))
+            self.bias_mu.uniform_(-r, r)
+            self.bias_sigma.fill_(self.std_init / math.sqrt(self.in_features))
+
+    @torch.no_grad()
+    def set_noise(self, eps_in: torch.Tensor, eps_out: torch.Tensor) -> None:
+        """the f-scaled noise vectors [in_features] and [out_features]"""
+        self.eps_in.copy_(eps_in)
+        self.eps_out.copy_(eps_out)
+        self.weight_epsilon.copy_(torch.outer(self.eps_out, self.eps_in))
+        self.bias_epsilon.copy_(self.eps_out)
+
+    def reset_noise(self) -> None:
+        """new noise from torch's generator of the layer's device (capturable on a CUDA device)"""
+        dev = self.eps_in.device
+        self.set_noise(scale_noise(torch.randn(self.in_features, device=dev)), scale_noise(torch.randn(self.out_features, device=dev)))
+
+    def effective(self):
+        """(weight, bias) of the current mode"""
+        if not self.training:
+            return self.weight_mu, self.bias_mu
+        return self.weight_mu + self.weight_sigma * self.weight_epsilon, self.bias_mu + self.bias_sigma * self.bias_epsilon
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return F.linear(x, *self.effective())
 
 
 def categorical_support(num_atoms: int, v_min: float, v_max: float) -> torch.Tensor:
@@ -71,10 +140,12 @@ class AtariQNet(nn.Module):
     nn.Linear(512, num_actions)`` combined as Q = V + Adv - mean_a Adv (Wang et al. 2016, eq. 9), or, with ``categorical``, by
     ``q = nn.Linear(512, num_actions * num_atoms)`` whose row a * num_atoms + k is atom k of action a (C51): ``dist(obs)`` gives the
     softmax per action, ``forward`` its expectation on the support (a non-persistent buffer: the state-dict names are the plain ten).
-    Initialised by torch's default layer init, so ``torch.manual_seed(s)`` before construction fixes the weights."""
+    Initialised by torch's default layer init, so ``torch.manual_seed(s)`` before construction fixes the weights.  With ``noisy``, fc
+    and the head layers are ``NoisyLinear(..., noisy_std)`` (train mode: the noisy weights, eval mode: mu; ``reset_noise()`` redraws
+    every layer's noise)."""
 
     def __init__(self, num_actions: int, observation_shape=(4, 84, 84), dueling: bool = False, categorical: bool = False,
-                 num_atoms: int = 51, v_min: float = 0.0, v_max: float = 200.0):
+                 num_atoms: int = 51, v_min: float = 0.0, v_max: float = 200.0, noisy: bool = False, noisy_std: float = 0.5):
         super().__init__()
         if dueling and categorical:
             raise ValueError('the categorical head with the dueling head is not supported')
@@ -82,19 +153,30 @@ class AtariQNet(nn.Module):
         self.num_actions = int(num_actions)
         self.dueling = bool(dueling)
         self.categorical = bool(categorical)
+        self.noisy = bool(noisy)
         self.num_atoms = int(num_atoms) if self.categorical else 0
+        linear = (lambda i, o: NoisyLinear(i, o, noisy_std)) if self.noisy else nn.Linear
         self.conv1 = nn.Conv2d(self.observation_shape[0], 32, kernel_size=8, stride=4)
         self.conv2 = nn.Conv2d(32, 64, kernel_size=4, stride=2)
         self.conv3 = nn.Conv2d(64, 64, kernel_size=3, stride=1)
-        self.fc = nn.Linear(3136, 512)
+        self.fc = linear(3136, 512)
         if self.dueling:
-            self.value = nn.Linear(512, 1)
-            self.advantage = nn.Linear(512, self.num_actions)
+            self.value = linear(512, 1)
+            self.advantage = linear(512, self.num_actions)
         elif self.categorical:
-            self.q = nn.Linear(512, self.num_actions * self.num_atoms)
+            self.q = linear(512, self.num_actions * self.num_atoms)
             self.register_buffer('support', categorical_support(self.num_atoms, v_min, v_max), persistent=False)
         else:
-            self.q = nn.Linear(512, self.num_actions)
+            self.q = linear(512, self.num_actions)
+
+    def noisy_layers(self):
+        """the NoisyLinear layers in state-dict order (none without noise)"""
+        return [m for m in (self.fc, getattr(self, 'q', None), getattr(self, 'value', None), getattr(self, 'advantage', None))
+                if isinstance(m, NoisyLinear)]
+
+    def reset_noise(self) -> None:
+        for m in self.noisy_layers():
+            m.reset_noise()
 
     def _features(self, obs: torch.Tensor) -> torch.Tensor:
         x = obs.float() / 255.0
@@ -131,6 +213,8 @@ class ApexHParams:
     max_grad_norm: Optional[float] = None
     double_dqn: bool = False
     dueling_dqn: bool = False            # the dueling head V + Adv - mean(Adv) on the shared fc output instead of q = Linear(512, A)
+    noisy_dqn: bool = False              # fc and the head layers as factorised Gaussian noisy layers (Fortunato et al. 2018)
+    noisy_std: float = 0.5               # their initial sigma0: sigma = noisy_std / sqrt(in_features)
     categorical_dqn: bool = False        # the categorical (C51) head q = Linear(512, A num_atoms) on the support [v_min, v_max]
     v_min: float = 0.0
     v_max: float = 200.0
@@ -151,6 +235,8 @@ class ApexHParams:
         if not (isinstance(self.num_actions, int) and 1 <= self.num_actions <= 31):
             raise ValueError(f'num_actions must be an int in [1, 31], got {self.num_actions!r}')
         self.head                            # ValueError on a bad head setting
+        if isinstance(self.noisy_std, bool) or not isinstance(self.noisy_std, (int, float)) or not (math.isfinite(self.noisy_std) and self.noisy_std >= 0.0):
+            raise ValueError(f'noisy_std must be finite and >= 0, got {self.noisy_std!r}')
         if not (math.isfinite(self.gamma) and self.gamma >= 0.0):
             raise ValueError(f'gamma must be finite and >= 0, got {self.gamma}')
         if not (math.isfinite(self.learning_rate) and self.learning_rate > 0.0):
@@ -173,7 +259,7 @@ class ApexHParams:
     @property
     def head(self) -> 'QHead':
         """the Q head these settings describe (ValueError on a bad one)"""
-        return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max)
+        return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max, self.noisy_dqn)
 
     def to_c(self) -> _lib.SrlApexConfig:
         self.validate()
@@ -188,6 +274,7 @@ class ApexHParams:
         c.dueling = 1 if self.dueling_dqn else 0
         c.num_atoms = self.atoms()
         c.v_min, c.v_max = self.v_min, self.v_max
+        c.noisy = 1 if self.noisy_dqn else 0
         return c
 
     def atoms(self) -> int:
@@ -198,14 +285,16 @@ class ApexHParams:
 @dataclass(frozen=True)
 class QHead:
     """The Q head of the learner and its actors: q = Linear(512, A), the dueling head (``dueling``), or the categorical head on
-    ``num_atoms`` > 0 atoms of the support [v_min, v_max].  A scalar head keeps no support, so equal heads compare equal."""
+    ``num_atoms`` > 0 atoms of the support [v_min, v_max]; ``noisy``: fc and the head layers are noisy layers.  A scalar head keeps no
+    support, so equal heads compare equal."""
     dueling: bool = False
     num_atoms: int = 0
     v_min: float = 0.0
     v_max: float = 0.0
+    noisy: bool = False
 
     @classmethod
-    def of(cls, dueling_dqn, categorical_dqn, num_atoms, v_min, v_max) -> 'QHead':
+    def of(cls, dueling_dqn, categorical_dqn, num_atoms, v_min, v_max, noisy_dqn=False) -> 'QHead':
         """the head of ApexHParams' / B200ApexActor's settings, checked (the support, as the kernels read it in fp32, even when
         categorical_dqn is off)"""
         if not isinstance(dueling_dqn, bool):
@@ -218,23 +307,25 @@ class QHead:
             lo, hi = np.float32(v_min), np.float32(v_max)
         if not (np.isfinite(lo) and np.isfinite(hi) and lo < hi and np.isfinite(np.float32((float(hi) - float(lo)) / (num_atoms - 1)))):
             raise ValueError(f'v_min and v_max must be finite fp32 values with v_min < v_max, got ({v_min}, {v_max})')
+        if not isinstance(noisy_dqn, bool):
+            raise ValueError(f'noisy_dqn must be a bool, got {noisy_dqn!r}')
         if categorical_dqn and dueling_dqn:
             raise ValueError('categorical_dqn with dueling_dqn is not supported: choose one head')
-        return cls(False, int(num_atoms), float(v_min), float(v_max)) if categorical_dqn else cls(dueling_dqn)
+        return cls(False, int(num_atoms), float(v_min), float(v_max), noisy_dqn) if categorical_dqn else cls(dueling_dqn, noisy=noisy_dqn)
 
     def __str__(self):
-        s = f'dueling_dqn={self.dueling}, categorical_dqn={self.num_atoms > 0}'
+        s = f'dueling_dqn={self.dueling}, categorical_dqn={self.num_atoms > 0}, noisy_dqn={self.noisy}'
         return s + f', (num_atoms, v_min, v_max)={(self.num_atoms, self.v_min, self.v_max)}' if self.num_atoms else s
 
     def names(self):
-        return apex_param_names(self.dueling)
+        return apex_param_names(self.dueling, self.noisy)
 
     def shapes(self, num_actions: int):
-        return apex_param_shapes(num_actions, self.dueling, self.num_atoms)
+        return apex_param_shapes(num_actions, self.dueling, self.num_atoms, self.noisy)
 
     def layout(self, num_actions: int):
         """(total floats, offsets, counts) of the flat buffer"""
-        return _lib.apex_param_layout(num_actions, self.dueling, self.num_atoms)
+        return _lib.apex_param_layout(num_actions, self.dueling, self.num_atoms, self.noisy)
 
 
 def flat_views(flat: torch.Tensor, off, cnt, shapes) -> 'OrderedDict[str, torch.Tensor]':
@@ -252,12 +343,13 @@ def load_views(dst: Dict[str, torch.Tensor], sd: Dict[str, torch.Tensor]) -> Non
         v.copy_(sd[n].to(v.device, torch.float32))
 
 
-def default_q_state_dict(num_actions: int, seed: int = 0, dueling: bool = False, num_atoms: int = 0) -> 'OrderedDict[str, torch.Tensor]':
+def default_q_state_dict(num_actions: int, seed: int = 0, dueling: bool = False, num_atoms: int = 0, noisy: bool = False,
+                         noisy_std: float = 0.5) -> 'OrderedDict[str, torch.Tensor]':
     """AtariQNet's initial weights under ``torch.manual_seed(seed)``, drawn without disturbing the global RNG (num_atoms > 0: the
-    categorical head's)"""
+    categorical head's; noisy: the noisy network's with sigma0 = noisy_std)"""
     with torch.random.fork_rng(devices=[]):
         torch.manual_seed(seed)
-        net = AtariQNet(num_actions, dueling=dueling, categorical=num_atoms > 0, num_atoms=num_atoms or 51)
+        net = AtariQNet(num_actions, dueling=dueling, categorical=num_atoms > 0, num_atoms=num_atoms or 51, noisy=noisy, noisy_std=noisy_std)
     return OrderedDict((k, v.detach().clone()) for k, v in net.state_dict().items())
 
 
@@ -268,7 +360,8 @@ class B200ApexLearner(BaseAgent):
     is captured as a CUDA graph per set of input addresses (first call eager, second captures, later calls replay), so a caller that
     gathers into fixed buffers replays -- the sampled idxs and weights included: ``GpuPrioritizedSampler.sample`` returns new tensors,
     copy them into fixed ones (each new address set costs an eager step and a capture, and its graph is kept).  The target network follows DQNAgent's cadence: after update k (from 0), when
-    k % target_update_frequency == 0, target <- tau * online + (1 - tau) * target."""
+    k % target_update_frequency == 0, target <- tau * online + (1 - tau) * target.  With ``hp.noisy_dqn`` the noise of update k is
+    drawn from (``seed``, k): two learners with the same seed and step count draw the same noise."""
 
     def __init__(self, hp: ApexHParams, device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None, seed: int = 0,
                  use_graph: bool = True):
@@ -276,6 +369,7 @@ class B200ApexLearner(BaseAgent):
             raise RuntimeError('B200ApexLearner needs a CUDA device: scalerl_b200 has no CPU fallback')
         super().__init__(hp)
         cfg = hp.to_c()
+        cfg.noise_seed = int(seed) % 2 ** 64
         self.hp = hp
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._L = _lib.lib()
@@ -296,7 +390,7 @@ class B200ApexLearner(BaseAgent):
                                                        C.byref(h)), 'srl_apex_learner_create')
             self._h = h
             self._stats = torch.zeros(4, device=self.device)      # {loss, gradient norm, clip coefficient, pad}
-        sd = default_q_state_dict(hp.num_actions, seed, head.dueling, head.num_atoms) if init_state_dict is None else init_state_dict
+        sd = default_q_state_dict(hp.num_actions, seed, head.dueling, head.num_atoms, head.noisy, hp.noisy_std) if init_state_dict is None else init_state_dict
         self.load_state_dict(sd)
         self.load_state_dict(sd, target=True)       # actor_target starts as a copy (dqn_agent.py:66-67)
         self.use_graph = use_graph
@@ -333,8 +427,8 @@ class B200ApexLearner(BaseAgent):
         return {'exp_avg': self._views(self.exp_avg), 'exp_avg_sq': self._views(self.exp_avg_sq)}
 
     def optimizer_state_dict(self) -> dict:
-        """``torch.optim.Adam(AtariQNet(A, dueling=hp.dueling_dqn, categorical=hp.categorical_dqn, ...).parameters()).state_dict()``
-        layout"""
+        """``torch.optim.Adam(AtariQNet(A, dueling=hp.dueling_dqn, categorical=hp.categorical_dqn, noisy=hp.noisy_dqn,
+        ...).parameters()).state_dict()`` layout"""
         return to_torch_optimizer_state(self.hp, self._opt_tensors(), self._opt_steps, order=self.names)
 
     def load_optimizer_state_dict(self, sd: dict) -> None:
@@ -381,7 +475,8 @@ class B200ApexLearner(BaseAgent):
 
     @torch.no_grad()
     def q_values(self, obs) -> torch.Tensor:
-        """Q(obs) with the online network: uint8 [N, 4, 84, 84] (or one [4, 84, 84] frame stack) -> float32 [N, A].  Runs on its own
+        """Q(obs) with the online network (noisy: its mean weights mu): uint8 [N, 4, 84, 84] (or one [4, 84, 84] frame stack) ->
+        float32 [N, A].  Runs on its own
         encoder context and buffers, so actors may call it on another stream than learn(); it reads the parameters as they are when
         it runs."""
         obs = self._obs(obs)

@@ -24,18 +24,6 @@ namespace srl {
 
 constexpr int64_t ACTOR_OBS_BYTES = 4 * 84 * 84;
 
-// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011): four 32-bit words of counter c under key k
-SRL_DEVINL uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-    k.x += 0x9E3779B9u; k.y += 0xBB67AE85u;
-  }
-  return c;
-}
-
 // env e's action of draw d: with probability eps[e] a uniform action, else `greedy`
 SRL_DEVINL int64_t eps_greedy(unsigned long long d, int e, uint2 key, int A, const float* __restrict__ eps, int greedy) {
   const uint4 r = philox4x32_10(make_uint4((uint32_t)d, (uint32_t)(d >> 32), (uint32_t)e, 0u), key);
@@ -152,7 +140,7 @@ cudaError_t launch_apex_priorities(const QHead& h, const float* core, float* log
 using namespace srl;
 
 struct srl_apex_actor {
-  int E;
+  int E, precision;
   uint2 key;
   const float* w8[8];              // the encoder tensors of the snapshot
   QHead head;                      // the snapshot's Q head
@@ -164,6 +152,12 @@ struct srl_apex_actor {
   int64_t* zero_action;
   double* prio;                    // [E] the priorities of the last add
   unsigned long long* draws;       // [0] draw counter, [1] the act kernel's ticket
+  // noisy networks: the snapshot's mu / sigma tensors, the kept draw, its counter and the composed weights (w8[6..7] and head)
+  int noisy;
+  NoisyTensors nz;
+  float *normals, *noise;
+  unsigned long long* noise_draws;
+  NoisyWeights cw;
   char* arena;
 };
 
@@ -179,9 +173,30 @@ int actor_rows(srl_apex_actor* X, int64_t saved, int64_t scratch, WsRow* t) {
   t[n++] = ws_row(nullptr, E, &X->prio);
   t[n++] = ws_row(nullptr, 2, &X->draws);
   t[n++] = ws_row(nullptr, X->head.kind == Q_CATEGORICAL ? 2 * E * X->head.R : 0, &X->logits);
+  const int64_t on = X->noisy, R = X->head.R, dueling = X->head.kind == Q_DUELING, NN = on * noise_count(X->head);
+  t[n++] = ws_row("normals", NN, &X->normals);
+  t[n++] = ws_row("noise", NN, &X->noise);
+  t[n++] = ws_row(nullptr, on, &X->noise_draws);
+  t[n++] = ws_row("fc_weight", on * NOISE_FC_OUT * NOISE_FC_IN, &X->cw.fc_w);
+  t[n++] = ws_row("fc_bias", on * NOISE_FC_OUT, &X->cw.fc_b);
+  t[n++] = ws_row("head_weight", on * R * NOISE_HEAD_IN, &X->cw.h_w);
+  t[n++] = ws_row("head_bias", on * (dueling ? 1 : R), &X->cw.h_b);
+  t[n++] = ws_row("head_adv_bias", on * dueling * X->head.A, &X->cw.h_ba);
   return n;
 }
-constexpr int ACTOR_ROWS = 8;
+constexpr int ACTOR_ROWS = 16;
+
+// a noisy actor's weights for its next forwards: a new draw first when `draw` (act), then the composition of the kept draw with the
+// snapshot as it is now.  Nothing without noise.
+cudaError_t actor_noise(srl_apex_actor* X, bool draw, cudaStream_t st) {
+  if (!X->noisy) return cudaSuccess;
+  if (draw) {
+    const cudaError_t e = launch_noisy_draw(X->key, nullptr, X->noise_draws, 1, noise_count(X->head), &X->normals, &X->noise, st);
+    if (e != cudaSuccess) return e;
+  }
+  const float* noise = X->noise;
+  return launch_noisy_compose(&X->nz, &X->cw, &noise, 1, X->head, st);
+}
 
 // Q head rows of `frames` frames of obs into core (f <= E frames per call)
 int actor_forward(srl_apex_actor* X, const uint8_t* obs, int frames, float* core, cudaStream_t st) {
@@ -189,7 +204,7 @@ int actor_forward(srl_apex_actor* X, const uint8_t* obs, int frames, float* core
 }
 }  // namespace
 
-static int actor_create(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, uint64_t seed,
+static int actor_create(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int noisy, uint64_t seed,
                         const float* params, srl_apex_actor_t** out);
 
 extern "C" int srl_apex_actor_create(int A, int num_envs, int precision, uint64_t seed, const float* params, srl_apex_actor_t** out) {
@@ -198,21 +213,26 @@ extern "C" int srl_apex_actor_create(int A, int num_envs, int precision, uint64_
 
 extern "C" int srl_apex_actor_create_ex(int A, int num_envs, int precision, int dueling, uint64_t seed, const float* params,
                                         srl_apex_actor_t** out) {
-  return actor_create(A, num_envs, precision, dueling, 0, 0.f, 0.f, seed, params, out);
+  return actor_create(A, num_envs, precision, dueling, 0, 0.f, 0.f, 0, seed, params, out);
 }
 
 extern "C" int srl_apex_actor_create_cat(int A, int num_envs, int precision, int num_atoms, float v_min, float v_max, uint64_t seed,
                                          const float* params, srl_apex_actor_t** out) {
-  return actor_create(A, num_envs, precision, 0, num_atoms, v_min, v_max, seed, params, out);
+  return actor_create(A, num_envs, precision, 0, num_atoms, v_min, v_max, 0, seed, params, out);
 }
 
-static int actor_create(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max,
-                                          uint64_t seed, const float* params, srl_apex_actor_t** out) {
+extern "C" int srl_apex_actor_create_noisy(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int noisy,
+                                           uint64_t seed, const float* params, srl_apex_actor_t** out) {
+  return actor_create(A, num_envs, precision, dueling, num_atoms, v_min, v_max, noisy, seed, params, out);
+}
+
+static int actor_create(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int noisy,
+                        uint64_t seed, const float* params, srl_apex_actor_t** out) {
   REQ(params && out, "apex_actor_create: NULL argument");
   REQ(num_envs >= 1 && num_envs <= MAX_FRAMES, "apex_actor_create: num_envs=%d must be in [1, %d]", num_envs, MAX_FRAMES);
   REQ(precision == 0 || precision == 1, "apex_actor_create: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", precision);
   QHead head;
-  int rc = make_q_head("apex_actor_create", A, dueling, num_atoms, v_min, v_max, &head);
+  int rc = make_q_head("apex_actor_create", A, dueling, num_atoms, v_min, v_max, noisy, &head);
   if (rc) return rc;
   REQ(!misaligned(params, 16), "apex_actor_create: params must be 16-byte aligned");
   int64_t sb = 0, kb = 0;
@@ -222,11 +242,13 @@ static int actor_create(int A, int num_envs, int precision, int dueling, int num
   REQ(X, "out of host memory");
   auto undo = [X](int code) { srl_apex_actor_destroy(X); return code; };
   X->E = num_envs;
+  X->precision = precision;
   X->key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-  int64_t off[12];
-  apex_layout(head, off, nullptr);
-  for (int i = 0; i < 8; ++i) X->w8[i] = params + off[i];
-  X->head = bind_q_head(head, params);
+  const ApexNet snap = bind_apex(head, noisy, const_cast<float*>(params));
+  for (int i = 0; i < 8; ++i) X->w8[i] = snap.w8[i];
+  X->head = snap.q;
+  X->noisy = noisy;
+  X->nz = snap.nz;
   rc = srl_encoder_create(precision, &X->enc);
   if (rc) return undo(rc);
   WsRow t[ACTOR_ROWS];
@@ -234,9 +256,15 @@ static int actor_create(int A, int num_envs, int precision, int dueling, int num
   const int64_t total = rows_bytes(t, n, false);
   cudaError_t e = cudaMalloc(&X->arena, total);
   if (e != cudaSuccess) return undo(cuda_fail(e, "apex_actor_create: cudaMalloc"));
-  e = cudaMemset(X->arena, 0, total);          // the zero columns, the draw counter and the ticket
+  e = cudaMemset(X->arena, 0, total);          // the zero columns, the draw counters and the ticket
   if (e != cudaSuccess) return undo(cuda_fail(e, "apex_actor_create: cudaMemset"));
   carve_rows(t, n, false, X->arena);
+  if (noisy) {      // the first draw, kept until the first act; the forwards run on the composed weights
+    bind_composed(snap, X->cw, X->w8, &X->head);
+    e = launch_noisy_draw(X->key, nullptr, X->noise_draws, 1, noise_count(X->head), &X->normals, &X->noise, nullptr);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) return undo(cuda_fail(e, "apex_actor_create: first noise draw"));
+  }
   *out = X;
   return 0;
 }
@@ -256,6 +284,7 @@ extern "C" int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const
   int rc = check_spans(s, 3, "apex_actor_act");
   if (rc) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
+  CU(actor_noise(X, true, st), "apex_actor_act: noise");
   rc = actor_forward(X, obs, E, X->core, st);
   if (rc) return rc;
   CU(launch_apex_act(X->head, X->core, X->logits, E, epsilons, X->key, X->draws, actions, st), "apex_act");
@@ -270,6 +299,7 @@ extern "C" int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, 
   int rc = check_spans(s, 2, "apex_actor_q_values");
   if (rc) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
+  CU(actor_noise(X, false, st), "apex_actor_q_values: noise");
   for (int f0 = 0; f0 < n; f0 += X->E) {        // chunks of at most E frames: the blocks' size
     const int f = n - f0 < X->E ? n - f0 : X->E;
     rc = actor_forward(X, obs + (size_t)f0 * ACTOR_OBS_BYTES, f, X->core, st);
@@ -284,6 +314,15 @@ extern "C" int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name
   const int64_t rows = 2 * (int64_t)X->E;
   if (strcmp(name, "core") == 0) { *ptr = X->core; *count = rows * ENC_CORE; return 0; }
   if (strcmp(name, "logits") == 0 && X->head.kind == Q_CATEGORICAL) { *ptr = X->logits; *count = rows * X->head.R; return 0; }
+  int64_t sb = 0, kb = 0;
+  int rc = srl_encoder_sizes(X->E, X->precision, &sb, &kb);
+  if (rc) return rc;
+  srl_apex_actor shadow = *X;          // the table's rows re-derived on a copy: the same sizes give the same addresses
+  WsRow t[ACTOR_ROWS];
+  const int n = actor_rows(&shadow, sb, kb, t);
+  carve_rows(t, n, false, X->arena);
+  for (int i = 0; i < n; ++i)
+    if (t[i].name && strcmp(t[i].name, name) == 0 && t[i].count > 0) { *ptr = *t[i].hi; *count = t[i].count; return 0; }
   return fail(SRL_EINVAL, "apex_actor_debug_buffer: unknown buffer '%s'", name);
 }
 
@@ -293,6 +332,7 @@ int apex_actor_num_envs(const srl_apex_actor* X) { return X->E; }
 int apex_actor_priorities(srl_apex_actor* X, const uint8_t* s, const uint8_t* s_next, const int64_t* action, const float* reward,
                           const uint8_t* done, int64_t ptr, int64_t M, float gamma_n, float eps, const double** prio, cudaStream_t st) {
   const int E = X->E;
+  CU(actor_noise(X, false, st), "apex_actor_priorities: noise");
   int rc = actor_forward(X, s, E, X->core, st);
   if (!rc) rc = actor_forward(X, s_next, E, X->core + (size_t)E * ENC_CORE, st);
   if (rc) return rc;

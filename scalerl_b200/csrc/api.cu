@@ -920,9 +920,10 @@ int64_t apex_layout(const QHead& h, int64_t* off, int64_t* cnt) {
   return o;
 }
 
-int make_q_head(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, QHead* h) {
+int make_q_head(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int noisy, QHead* h) {
   REQ(A >= 1 && A <= 31, "%s: A=%d must be in [1,31]", who, A);
   REQ(dueling == 0 || dueling == 1, "%s: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", who, dueling);
+  REQ(noisy == 0 || noisy == 1, "%s: noisy=%d must be 0 (plain layers) or 1 (noisy fc and head layers)", who, noisy);
   REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "%s: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]", who,
       num_atoms, CAT_MAX_ATOMS);
   *h = QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling};
@@ -953,6 +954,58 @@ QHeadGrad bind_q_grad(const QHead& h, float* grads) {
   apex_layout(h, off, nullptr);
   return {grads + off[8], grads + off[9], h.kind == Q_DUELING ? grads + off[11] : nullptr};
 }
+
+// The noisy network: state_dict order {conv1..3 (6), fc.{weight_mu, weight_sigma, bias_mu, bias_sigma}, q.{...}} (14), or with the
+// dueling head {..., value.{weight_mu, weight_sigma, bias_mu, bias_sigma}, advantage.{...}} (18).  In memory the biases come first
+// (value.bias_mu before advantage.bias_mu, and so for sigma), then the head weights (the mu rows one [(A + 1)][512] block, the sigma
+// rows another), then fc.weight_mu and fc.weight_sigma; segments padded to 4 floats.
+int64_t apex_layout_noisy(const QHead& h, int64_t* off, int64_t* cnt) {
+  const int64_t A = h.A, R = h.R, F = 512 * 3136;
+  const int64_t plain[14] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, F, F, 512, 512, R * 512, R * 512, R, R};
+  const int64_t duel[18] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, F, F, 512, 512, 512, 512, 1, 1, A * 512, A * 512, A, A};
+  const int plain_order[14] = {0, 1, 2, 3, 4, 5, 8, 9, 12, 13, 10, 11, 6, 7};
+  const int duel_order[18] = {0, 1, 2, 3, 4, 5, 8, 9, 12, 16, 13, 17, 10, 14, 11, 15, 6, 7};
+  const bool dueling = h.kind == Q_DUELING;
+  const int64_t* counts = dueling ? duel : plain;
+  const int* order = dueling ? duel_order : plain_order;
+  const int n = dueling ? 18 : 14;
+  int64_t o = 0;
+  for (int k = 0; k < n; ++k) {
+    const int i = order[k];
+    if (off) off[i] = o;
+    if (cnt) cnt[i] = counts[i];
+    o += (counts[i] + 3) & ~int64_t(3);
+  }
+  return o;
+}
+
+ApexNet bind_apex(const QHead& h, int noisy, float* base) {
+  ApexNet n = {};
+  int64_t off[18];
+  if (!noisy) {
+    apex_layout(h, off, nullptr);
+    for (int i = 0; i < 8; ++i) n.w8[i] = base + off[i];
+    n.q = bind_q_head(h, base);
+    n.g = bind_q_grad(h, base);
+    return n;
+  }
+  apex_layout_noisy(h, off, nullptr);
+  const bool dueling = h.kind == Q_DUELING;
+  for (int i = 0; i < 6; ++i) n.w8[i] = base + off[i];
+  n.w8[6] = base + off[6];
+  n.w8[7] = base + off[8];
+  for (int s = 0; s < 2; ++s) {
+    n.nz.fc_w[s] = base + off[6 + s];
+    n.nz.fc_b[s] = base + off[8 + s];
+    n.nz.h_w[s] = base + off[10 + s];
+    n.nz.h_b[s] = base + off[12 + s];
+    n.nz.h_ba[s] = dueling ? base + off[16 + s] : nullptr;
+  }
+  n.q = h;
+  n.q.W = n.nz.h_w[0]; n.q.b = n.nz.h_b[0]; n.q.ba = n.nz.h_ba[0];
+  n.g = {n.nz.h_w[0], n.nz.h_b[0], n.nz.h_ba[0]};
+  return n;
+}
 }  // namespace srl
 
 extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) {
@@ -968,6 +1021,11 @@ extern "C" int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offs
   REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "apex_param_layout: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]",
       num_atoms, CAT_MAX_ATOMS);
   return apex_layout(QHead{num_atoms ? Q_CATEGORICAL : Q_PLAIN, A, A * (num_atoms ? num_atoms : 1)}, offsets10, counts10);
+}
+extern "C" int64_t srl_apex_param_layout_noisy(int A, int dueling, int num_atoms, int noisy, int64_t* offsets18, int64_t* counts18) {
+  QHead h;
+  if (make_q_head("apex_param_layout", A, dueling, num_atoms, 0.f, 1.f, noisy, &h)) return -1;
+  return noisy ? apex_layout_noisy(h, offsets18, counts18) : apex_layout(h, offsets18, counts18);
 }
 
 struct srl_apex_learner {
@@ -989,6 +1047,15 @@ struct srl_apex_learner {
   // the categorical head (cfg.num_atoms = K > 0): logits [B][A K] over s, s' (online, double DQN only) and s' (target), their
   // gradient, the projected targets m [B][K], the cross-entropies [B] and the q-value chunk's logits
   float *logits_s, *logits_n, *logits_nt, *dlogits, *mproj, *ce, *logits_q;
+  // noisy networks (cfg.noisy): the mu / sigma tensors of the online, target and gradient buffers, the step's normals and noise and
+  // the composed weights ([0] online, [1] target); the step runs the encoder and the head on sw8 / st8 and son / stg, which are the
+  // composed weights with noise and w8 / t8, on / tg without
+  NoisyTensors nz[2], nzg;
+  float *normals[2], *noise[2];
+  NoisyWeights cw[2];
+  const float *sw8[8], *st8[8];
+  QHead son, stg;
+  uint2 noise_key;
   char* arena;
 };
 
@@ -1034,9 +1101,25 @@ static int apex_rows(srl_apex_learner* L, const int64_t* b4, WsRow* t) {
   t[n++] = ws_row("m", B * K, &L->mproj);
   t[n++] = ws_row("ce", B * (K ? 1 : 0), &L->ce);
   t[n++] = ws_row(nullptr, QC * R, &L->logits_q);
+  // noisy networks: empty rows without noise
+  const int64_t dueling = L->cfg.dueling, HR = K ? R : A + dueling, on = L->cfg.noisy ? 1 : 0;
+  const int64_t NN = on * (NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (1 + dueling) + HR);
+  const char* names[2][7] = {{"normals_online", "noise_online", "fc_weight_online", "fc_bias_online", "head_weight_online",
+                              "head_bias_online", "head_adv_bias_online"},
+                             {"normals_target", "noise_target", "fc_weight_target", "fc_bias_target", "head_weight_target",
+                              "head_bias_target", "head_adv_bias_target"}};
+  for (int i = 0; i < 2; ++i) {
+    t[n++] = ws_row(names[i][0], NN, &L->normals[i]);
+    t[n++] = ws_row(names[i][1], NN, &L->noise[i]);
+    t[n++] = ws_row(names[i][2], on * NOISE_FC_OUT * NOISE_FC_IN, &L->cw[i].fc_w);
+    t[n++] = ws_row(names[i][3], on * NOISE_FC_OUT, &L->cw[i].fc_b);
+    t[n++] = ws_row(names[i][4], on * HR * NOISE_HEAD_IN, &L->cw[i].h_w);
+    t[n++] = ws_row(names[i][5], on * (dueling ? 1 : HR), &L->cw[i].h_b);
+    t[n++] = ws_row(names[i][6], on * dueling * A, &L->cw[i].h_ba);
+  }
   return n;
 }
-constexpr int APEX_ROWS = 29;
+constexpr int APEX_ROWS = 43;
 
 // -> the unbound head of a valid config
 static int check_apex_cfg(const srl_apex_config_t* c, QHead* head) {
@@ -1050,7 +1133,7 @@ static int check_apex_cfg(const srl_apex_config_t* c, QHead* head) {
   REQ(c->adam_beta1 >= 0.f && c->adam_beta1 < 1.f && c->adam_beta2 >= 0.f && c->adam_beta2 < 1.f, "apex_learner: Adam betas must be in [0, 1)");
   REQ(std::isfinite(c->adam_eps) && c->adam_eps >= 0.f, "apex_learner: adam_eps=%g must be finite and >= 0", (double)c->adam_eps);
   REQ(std::isfinite(c->priority_eps) && c->priority_eps >= 0.f, "apex_learner: priority_eps=%g must be finite and >= 0", (double)c->priority_eps);
-  return make_q_head("apex_learner", c->A, c->dueling, c->num_atoms, c->v_min, c->v_max, head);
+  return make_q_head("apex_learner", c->A, c->dueling, c->num_atoms, c->v_min, c->v_max, c->noisy, head);
 }
 
 extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* params, float* grads, float* exp_avg, float* exp_avg_sq,
@@ -1061,8 +1144,7 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   REQ(params && grads && exp_avg && exp_avg_sq && target_params && out, "apex_learner_create: NULL argument");
   REQ(!misaligned(params, 16) && !misaligned(grads, 16) && !misaligned(exp_avg, 16) && !misaligned(exp_avg_sq, 16) &&
       !misaligned(target_params, 16), "apex_learner_create: flat buffers must be 16-byte aligned");
-  int64_t off[12];
-  const int64_t np = apex_layout(head, off, nullptr);
+  const int64_t np = cfg->noisy ? apex_layout_noisy(head, nullptr, nullptr) : apex_layout(head, nullptr, nullptr);
   const Span s[5] = {{params, np * 4, true, "params"}, {grads, np * 4, true, "grads"}, {exp_avg, np * 4, true, "exp_avg"},
                      {exp_avg_sq, np * 4, true, "exp_avg_sq"}, {target_params, np * 4, true, "target_params"}};
   rc = check_spans(s, 5, "apex_learner_create");
@@ -1071,8 +1153,12 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   REQ(L, "out of host memory");
   auto undo = [L](int code) { srl_apex_learner_destroy(L); return code; };
   L->cfg = *cfg; L->params = params; L->grads = grads; L->m = exp_avg; L->v = exp_avg_sq; L->target = target_params; L->nparams = np;
-  for (int i = 0; i < 8; ++i) { L->w8[i] = params + off[i]; L->t8[i] = target_params + off[i]; L->g8[i] = grads + off[i]; }
-  L->on = bind_q_head(head, params); L->tg = bind_q_head(head, target_params); L->g = bind_q_grad(head, grads);
+  const ApexNet on = bind_apex(head, cfg->noisy, params), tg = bind_apex(head, cfg->noisy, target_params),
+               gr = bind_apex(head, cfg->noisy, grads);
+  for (int i = 0; i < 8; ++i) { L->w8[i] = on.w8[i]; L->t8[i] = tg.w8[i]; L->g8[i] = gr.w8[i]; }
+  L->on = on.q; L->tg = tg.q; L->g = gr.g;
+  L->nz[0] = on.nz; L->nz[1] = tg.nz; L->nzg = gr.nz;
+  L->noise_key = make_uint2((uint32_t)cfg->noise_seed, (uint32_t)(cfg->noise_seed >> 32));
   rc = srl_encoder_create(cfg->precision, &L->E);
   if (!rc) rc = srl_encoder_create(cfg->precision, &L->Eq);
   if (rc) return undo(rc);
@@ -1088,6 +1174,13 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   if (e == cudaSuccess) e = cudaMemset(grads, 0, np * 4);      // the padding between the segments enters the gradient norm
   if (e != cudaSuccess) return undo(cuda_fail(e, "apex_learner_create: cudaMemset"));
   carve_rows(t, n, false, L->arena);
+  if (cfg->noisy) {
+    bind_composed(on, L->cw[0], L->sw8, &L->son);
+    bind_composed(tg, L->cw[1], L->st8, &L->stg);
+  } else {
+    for (int i = 0; i < 8; ++i) { L->sw8[i] = L->w8[i]; L->st8[i] = L->t8[i]; }
+    L->son = L->on; L->stg = L->tg;
+  }
   *out = L;
   return 0;
 }
@@ -1108,19 +1201,26 @@ extern "C" int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, 
   const srl_apex_config_t& c = L->cfg;
   const int B = c.B;
   const cudaStream_t st = (cudaStream_t)stream;
+  if (c.noisy) {      // update k's noise (k = the device step count) for both networks, and their composed weights
+    CU(launch_noisy_draw(L->noise_key, L->dstep, nullptr, 2, noise_count(L->on), L->normals, L->noise, st), "noisy_draw");
+    const float* noise[2] = {L->noise[0], L->noise[1]};
+    CU(launch_noisy_compose(L->nz, L->cw, noise, 2, L->on, st), "noisy_compose");
+  }
   // the three forwards (the encoder checks obs / next_obs and the blocks); the target forward runs last so that its rows are the
   // ones left in saved_n
-  int rc = srl_encoder_forward(L->E, obs, reward, action, B, 1, L->w8, L->saved_s, L->enc_scratch, L->core_s, stream);
-  if (!rc && c.double_dqn) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->w8, L->saved_n, L->enc_scratch, L->core_n, stream);
-  if (!rc) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->t8, L->saved_n, L->enc_scratch, L->core_nt, stream);
+  int rc = srl_encoder_forward(L->E, obs, reward, action, B, 1, L->sw8, L->saved_s, L->enc_scratch, L->core_s, stream);
+  if (!rc && c.double_dqn) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->sw8, L->saved_n, L->enc_scratch, L->core_n, stream);
+  if (!rc) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->st8, L->saved_n, L->enc_scratch, L->core_nt, stream);
   if (rc) return rc;
   const QTail t = {L->core_s, c.double_dqn ? L->core_n : nullptr, L->core_nt, action, reward, done, weights, B, c.gamma, c.priority_eps,
                    L->q, L->y, L->dcore, L->loss, L->tail_scratch, L->prio, L->dq, L->head_part, L->logits_s, L->logits_n, L->logits_nt,
                    L->mproj, L->ce, L->dlogits};
-  CU(launch_q_tail(L->on, L->tg, t, st), "q_tail");
-  CU(launch_q_wgrad(L->on, L->g, t, st), "q_wgrad");
+  CU(launch_q_tail(L->son, L->stg, t, st), "q_tail");
+  CU(launch_q_wgrad(L->son, L->g, t, st), "q_wgrad");
+  // the gradients of the composed weights land in the mu segments
   rc = srl_encoder_backward(L->E, L->dcore, B, 1, L->saved_s, L->enc_scratch, L->g8, stream);
   if (rc) return rc;
+  if (c.noisy) CU(launch_noisy_sigma_grad(L->nzg, L->noise[0], L->on, st), "noisy_sigma_grad");
   const OptStep o = {1, L->params, L->grads, L->m, L->v, L->nparams, c.max_grad_norm, L->coef, L->opt_scratch, c.learning_rate,
                      c.adam_beta1, c.adam_beta2, c.adam_eps, 0, L->dstep, OptExtra{}};
   CU(launch_clip_optim(o, st), "clip+adam");

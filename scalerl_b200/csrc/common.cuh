@@ -223,6 +223,19 @@ SRL_DEVINL int ld_action(const int64_t* p, int A) {
   return a < 0 ? 0 : (a >= A ? A - 1 : (int)a);
 }
 
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011): four 32-bit words of counter c under key k.
+// The Ape-X actor's epsilon-greedy draws and the noisy networks' noise (noisy.cu) use it.
+SRL_DEVINL uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u; k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+
 SRL_DEVINL float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

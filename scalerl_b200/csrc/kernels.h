@@ -247,9 +247,9 @@ struct QHead {
 struct QHeadGrad {
   float *gW, *gb, *gba;
 };
-// api.cu: the head a setting describes (num_atoms 0: a scalar head, whose support is not read), unbound.  0, or SRL_EINVAL with
-// "<who>: ..." as the message
-int make_q_head(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, QHead* h);
+// api.cu: the head a setting describes (num_atoms 0: a scalar head, whose support is not read), unbound; noisy must be 0 or 1 (the
+// head's layers noisy or not: the head itself is the same).  0, or SRL_EINVAL with "<who>: ..." as the message
+int make_q_head(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int noisy, QHead* h);
 // api.cu: the flat parameter layout of the Q network with head h (srl_apex_param_layout*'s): the offsets and counts (NULL: not wanted)
 // of its 10 (12: dueling) tensors -> the buffer's floats
 int64_t apex_layout(const QHead& h, int64_t* off, int64_t* cnt);
@@ -282,6 +282,52 @@ cudaError_t launch_q_wgrad(const QHead& h, const QHeadGrad& g, const QTail& t, c
 // q_out [N][A] = Q(h) over N core rows; the categorical head goes through logits [N][A K]
 cudaError_t launch_q_values(const QHead& h, const float* core, int N, float* logits, float* q_out, cudaStream_t st);
 cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
+// ---- noisy.cu: noisy networks (Fortunato et al. 2018, factorised Gaussian noise) on the fc layer and the Q head
+// One network's noise vector f(x) = sgn(x) sqrt|x| of standard normals x, nn = noise_count(h) floats:
+//   [fc in 3136 | fc out 512 | head in 512 (dueling: the value layer's, then the advantage layer's) | head out R (dueling: value, then
+//   the A advantage rows)]; every segment but the last starts on a multiple of 4 floats.
+constexpr int NOISE_FC_IN = 3136, NOISE_FC_OUT = 512, NOISE_HEAD_IN = 512, NOISE_HEAD_IN_OFF = NOISE_FC_IN + NOISE_FC_OUT;
+inline int noise_count(const QHead& h) { return NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (h.kind == Q_DUELING ? 2 : 1) + h.R; }
+// the noisy layers' tensors on one flat buffer, [0] mu and [1] sigma (of the parameters, or of their gradients): the fc weight
+// [512][3136] and bias [512]; the head in QHead's layout: W [R][512], b and (dueling) ba
+struct NoisyTensors {
+  float *fc_w[2], *fc_b[2];
+  float *h_w[2], *h_b[2], *h_ba[2];
+};
+// the composed (effective) weights of one network in the same layouts
+struct NoisyWeights {
+  float *fc_w, *fc_b, *h_w, *h_b, *h_ba;
+};
+// the normals and noise of `nets` (1 or 2) networks; network i's go to normals[i] / noise[i] (nn floats each).  Philox4x32-10 under
+// `key`, counter (g, 'nois', c, c >> 32 | i << 31) for the normals 4g .. 4g + 3 (Box-Muller).  c = *step (the learner's Adam step
+// count, read only), or *draws (the actor's noise counter: nets = 1, advanced by one when the draw ends)
+cudaError_t launch_noisy_draw(uint2 key, const int* step, unsigned long long* draws, int nets, int nn, float* const* normals,
+                              float* const* noise, cudaStream_t st);
+// w[i] = p[i]'s mu + sigma (.) (f(eps_out) f(eps_in)^T) and mu_b + sigma_b (.) f(eps_out) under noise[i], for the `nets` networks of head h
+cudaError_t launch_noisy_compose(const NoisyTensors* p, const NoisyWeights* w, const float* const* noise, int nets, const QHead& h,
+                                 cudaStream_t st);
+// the sigma gradients g.x[1] = g.x[0] (.) eps of the online network's noise (the mu gradients are those of the composed weights)
+cudaError_t launch_noisy_sigma_grad(const NoisyTensors& g, const float* noise, const QHead& h, cudaStream_t st);
+// api.cu: the noisy Q network's layout (srl_apex_param_layout_noisy's): 14 tensors (18: dueling) -> the buffer's floats
+int64_t apex_layout_noisy(const QHead& h, int64_t* off, int64_t* cnt);
+// api.cu: one network of head h on a flat buffer of its layout (noisy: the noisy layout): the encoder's 8 tensors and the Q head
+// (noisy: fc's and the head's mu tensors), the head as a gradient binding, and (noisy) the noisy layers' mu / sigma pairs
+struct ApexNet {
+  float* w8[8];
+  QHead q;
+  QHeadGrad g;
+  NoisyTensors nz;
+};
+ApexNet bind_apex(const QHead& h, int noisy, float* base);
+// the network that runs on the composed weights w: net's conv tensors, w's fc and head (QHead's layout)
+inline void bind_composed(const ApexNet& net, const NoisyWeights& w, const float** w8, QHead* q) {
+  for (int i = 0; i < 6; ++i) w8[i] = net.w8[i];
+  w8[6] = w.fc_w;
+  w8[7] = w.fc_b;
+  *q = net.q;
+  q->W = w.h_w; q->b = w.h_b; q->ba = net.q.kind == Q_DUELING ? w.h_ba : nullptr;
+}
+
 // dqn_cat.cu: the categorical halves of the launchers above
 // logits [N][R] = h W^T + b over N core rows (stride ENC_CORE), W [R][512]: one fmaf chain per logit over j = 0 .. 511 from 0, then
 // + b rounded once, whatever the tiling

@@ -7,9 +7,12 @@ With --dueling the learner runs the dueling head (ApexHParams(dueling_dqn=True))
 and the torch statements use AtariQNet(A, dueling=True).  With --categorical it runs the categorical head (ApexHParams(categorical_dqn=True,
 num_atoms=--atoms, v_min=-10, v_max=10)) beside the plain one, the torch statements become C51's (projection, cross-entropy, KL
 priorities) on AtariQNet(A, categorical=True), and a last line gives the head kernels' times from torch.profiler at B = 512, A = 18
-with their FLOP rate against the fp32 data-sheet rate (67 TFLOP/s).
+with their FLOP rate against the fp32 data-sheet rate (67 TFLOP/s).  With --noisy it runs the noisy learner (ApexHParams(noisy_dqn=True))
+beside the plain one, the torch statements run on AtariQNet(A, noisy=True) with reset_noise() on the online and target network every
+step, and a last line gives the noise kernels' times from torch.profiler at B = 512, A = 18 with the bytes they move against the HBM3
+data-sheet bandwidth (3.35 TB/s).
 
-    python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18] [--dueling | --categorical [--atoms 51]]
+    python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18] [--dueling | --categorical [--atoms 51] | --noisy]
 """
 import argparse
 import json
@@ -57,9 +60,10 @@ class TorchStep:
     """the reference's statements on torch/cuDNN (the priorities stay on the device and go into the GPU sampler).  The object owns
     every tensor the step reads or writes, so a captured replay of it stays valid as long as the object lives."""
 
-    def __init__(self, B, A, exp, w, idxs, gamma=0.99, dueling=False, atoms=0):
-        sd = default_q_state_dict(A, dueling=dueling, num_atoms=atoms)
-        net = lambda: AtariQNet(A, dueling=dueling, categorical=atoms > 0, num_atoms=atoms or 51, v_min=V_MIN, v_max=V_MAX).cuda()
+    def __init__(self, B, A, exp, w, idxs, gamma=0.99, dueling=False, atoms=0, noisy=False):
+        sd = default_q_state_dict(A, dueling=dueling, num_atoms=atoms, noisy=noisy)
+        net = lambda: AtariQNet(A, dueling=dueling, categorical=atoms > 0, num_atoms=atoms or 51, v_min=V_MIN, v_max=V_MAX, noisy=noisy).cuda()
+        self.noisy = noisy
         self.model, self.target, self.A, self.K = net(), net(), A, atoms
         self.rows = torch.arange(B, device='cuda')
         self.model.load_state_dict(sd)
@@ -72,6 +76,9 @@ class TorchStep:
         self.prio = torch.empty(B, dtype=torch.float64, device='cuda')
 
     def __call__(self):
+        if self.noisy:                  # new noise for both networks every update
+            self.model.reset_noise()
+            self.target.reset_noise()
         if self.K:
             return self.c51()
         current_q_values = self.model(self.obs).gather(1, self.actions)                       # worker.py:148
@@ -142,6 +149,41 @@ def head_profile(atoms, B=512, A=18, steps=20):
             'head_share_of_step': total / step_us}
 
 
+def noisy_profile(B=512, A=18, steps=20):
+    """the noise kernels in one captured noisy learner step (torch.profiler over `steps` replays): mean µs per step, the bytes each
+    moves (from the shapes) and its share of the HBM3 data-sheet bandwidth"""
+    from torch.profiler import ProfilerActivity, profile
+    exp, w, idxs = batch(B, A)
+    L, S = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, noisy_dqn=True)), sampler()
+    step = lambda: L.learn(exp, weights=w, idxs=idxs, sampler=S, sync_stats=False)
+    for _ in range(3):
+        step()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            step()
+        torch.cuda.synchronize()
+    weights = 4 * (512 * 3136 + 512 + A * 512 + A)          # one fp32 copy of the noisy layers' weights and biases
+    nn = 3136 + 512 + 512 + A
+    nbytes = {'noisy_draw_kernel': 2 * 2 * nn * 4,        # two networks' normals and noise
+              'noisy_compose_kernel': 2 * (3 * weights + 2 * nn * 4),    # per network: mu, sigma read, W written
+              'noisy_sigma_grad_kernel': 2 * weights + nn * 4}          # dmu read, dsigma written
+    out, total = {}, 0.0
+    for e in prof.key_averages():
+        name = next((k for k in nbytes if k in e.key), None)
+        if name is None:
+            continue
+        us = e.device_time_total / steps
+        out[name] = {'us_per_step': us, 'bytes': nbytes[name], 'tb_per_s': nbytes[name] / us * 1e-6,
+                     'fraction_of_3_35_tb_per_s': nbytes[name] / us * 1e-6 / 3.35}
+        total += us
+    step_us = 1e6 / timed(step, 50)
+    L.release_graphs()
+    L.close()
+    return {'card': card(), 'B': B, 'A': A, 'noise_kernels': out, 'noise_us_per_step': total, 'step_us': step_us,
+            'noise_share_of_step': total / step_us}
+
+
 class Captured:
     """a CUDA graph of `step` (warmed up on a side stream first); holds `step`, whose tensors the graph reads and writes"""
 
@@ -178,9 +220,10 @@ def main():
     ap.add_argument('--dueling', action='store_true', help='add the dueling learner and run the torch statements on the dueling net')
     ap.add_argument('--categorical', action='store_true', help='add the categorical learner and run C51 in torch statements')
     ap.add_argument('--atoms', type=int, default=51)
+    ap.add_argument('--noisy', action='store_true', help='add the noisy learner and run the torch statements on the noisy net')
     a = ap.parse_args()
-    if a.dueling and a.categorical:
-        sys.exit('--dueling and --categorical are separate comparisons: pass one')
+    if a.dueling + a.categorical + a.noisy > 1:
+        sys.exit('--dueling, --categorical and --noisy are separate comparisons: pass one')
     atoms = a.atoms if a.categorical else 0
     if not torch.cuda.is_available():
         sys.exit('bench_apex.py measures on a CUDA device; none is present')
@@ -200,8 +243,12 @@ def main():
             SC = sampler()
             learners.append(LC)
             variants['b200_categorical_captured'] = lambda: LC.learn(exp, weights=w, idxs=idxs, sampler=SC, sync_stats=False)
-        variants['torch_eager'] = TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms)
-        variants['torch_captured'] = Captured(TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms))
+        if a.noisy:
+            LN, SN = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, noisy_dqn=True)), sampler()
+            learners.append(LN)
+            variants['b200_noisy_captured'] = lambda: LN.learn(exp, weights=w, idxs=idxs, sampler=SN, sync_stats=False)
+        variants['torch_eager'] = TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms, noisy=a.noisy)
+        variants['torch_captured'] = Captured(TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms, noisy=a.noisy))
         for fn in variants.values():           # warm-up: the learner's first call runs eagerly, the second captures
             for _ in range(3):
                 fn()
@@ -209,7 +256,7 @@ def main():
         for _ in range(a.rounds):
             for k, fn in variants.items():
                 rates[k].append(timed(fn, a.steps))
-        torch_net = 'dueling' if a.dueling else (f'categorical K={atoms}' if atoms else 'plain')
+        torch_net = 'dueling' if a.dueling else (f'categorical K={atoms}' if atoms else ('noisy' if a.noisy else 'plain'))
         out = {'card': name, 'B': B, 'A': A, 'precision': 'bf16', 'torch_net': torch_net, 'rounds': a.rounds,
                'steps_per_round': a.steps}
         for k, r in rates.items():
@@ -223,6 +270,8 @@ def main():
             x.close()
     if atoms:
         print(json.dumps(head_profile(atoms)), flush=True)
+    if a.noisy:
+        print(json.dumps(noisy_profile()), flush=True)
 
 
 if __name__ == '__main__':

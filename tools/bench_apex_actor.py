@@ -5,9 +5,10 @@ frames resident on the device (no env is stepped: the numbers price the GPU work
   (c) reference: the reference's statements on torch/cuDNN AtariQNet: per-env epsilon-greedy in torch, plain save_to_memory, then
                  compute_prior (apex/worker.py:59-79) on the transitions the add completed and update_priorities of their slots
 Rounds alternate between the legs; the median and range over rounds are printed with the card's name and power limit, one JSON line
-per workload.
+per workload.  With --noisy a noisy actor (B200ApexActor(..., noisy_dqn=True): a new noise draw and the composition of its weights on
+every act) runs leg (a) beside the plain actor, and the act calls alone are timed for both ('act', 'noisy_act').
 
-    python tools/bench_apex_actor.py [--rounds 5] [--steps 100] [--configs 64x6,64x18,256x6,256x18]
+    python tools/bench_apex_actor.py [--rounds 5] [--steps 100] [--configs 64x6,64x18,256x6,256x18] [--noisy]
 """
 import argparse
 import json
@@ -79,6 +80,7 @@ def main():
     ap.add_argument('--rounds', type=int, default=5)
     ap.add_argument('--steps', type=int, default=100)
     ap.add_argument('--configs', default='64x6,64x18,256x6,256x18')
+    ap.add_argument('--noisy', action='store_true', help='add the noisy actor and time act alone for both actors')
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('bench_apex_actor.py measures on a CUDA device; none is present')
@@ -99,6 +101,14 @@ def main():
             mem_b.save_to_memory(obs, L.get_action(obs, 0.1), rew, nobs, done, is_vectorised=True)
 
         legs = {'actor': actor, 'plain': plain, 'reference': lambda: ref(obs, nobs, rew, done)}
+        if a.noisy:
+            XN = B200ApexActor(E, A, priority_eps=PRIORITY_EPS, noisy_dqn=True)
+            mem_n = GpuPrioritizedReplayBuffer(MEMORY, E, n_step=N_STEP, gamma=GAMMA)
+
+            def noisy_actor():
+                mem_n.save_to_memory(obs, XN.act(obs), rew, nobs, done, is_vectorised=True, priorities_from=XN)
+
+            legs.update({'noisy_actor': noisy_actor, 'act': lambda: X.act(obs), 'noisy_act': lambda: XN.act(obs)})
         for fn in legs.values():
             for _ in range(5):
                 fn()
@@ -112,9 +122,11 @@ def main():
             r = sorted(r)
             out[k] = {'env_steps_per_s_median': r[len(r) // 2], 'env_steps_per_s_range': [r[0], r[-1]]}
         print(json.dumps(out), flush=True)
-        for m in (mem_a, mem_b, ref.mem):
+        for m in (mem_a, mem_b, ref.mem) + ((mem_n,) if a.noisy else ()):
             m.close()
         X.close()
+        if a.noisy:
+            XN.close()
         L.close()
         del ref
 
