@@ -390,8 +390,9 @@ int srl_replay_gather(srl_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* 
  * The dueling head's state_dict order is {conv1..3, fc, value.weight [1,512], value.bias [1], advantage.weight [A,512],
  * advantage.bias [A]} (int64[12], srl_apex_param_layout_ex); value.weight lies directly before advantage.weight.
  * The categorical head keeps the 10 plain names with q.weight [A K, 512] and q.bias [A K] (srl_apex_param_layout_cat).
- * In memory the small tensors come first and fc.weight last; segments are padded to 4 floats.  Params, grads, both Adam states
- * and the target copy share the layout. */
+ * Every head, with or without noise, has one layout rule (srl_apex_param_layout_noisy's): in memory, each segment padded to 4
+ * floats, come the conv tensors, fc's bias, the head weights and the head biases (noisy: the head biases first), then fc's weight,
+ * each group by (mu before sigma, layer).  Params, grads, both Adam states and the target copy share the layout. */
 typedef struct srl_apex_learner srl_apex_learner_t;
 typedef struct srl_apex_config {
   int32_t B;                 /* transitions per step, 1 <= B <= 65536                                        */
@@ -421,7 +422,7 @@ int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offsets10, int6
  * or {conv1..3, fc, value (4), advantage (4)} = 18 with the dueling head.  Each noisy layer computes
  *   y = (mu_w + sigma_w (.) eps_w) x + mu_b + sigma_b (.) eps_b,  eps_w = f(eps_out) f(eps_in)^T,  eps_b = f(eps_out),  f(x) = sgn(x) sqrt|x|
  * In memory the biases come first, then the head weights (value.weight_mu directly before advantage.weight_mu, and the same for
- * sigma), then fc.weight_mu and fc.weight_sigma; segments padded to 4 floats.  -> the buffer's floats, or -1 with srl_last_error set */
+ * sigma), then fc.weight_mu and fc.weight_sigma, as the rule above.  -> the buffer's floats, or -1 with srl_last_error set */
 int64_t srl_apex_param_layout_noisy(int A, int dueling, int num_atoms, int noisy, int64_t* offsets18, int64_t* counts18);
 /* params / grads / exp_avg / exp_avg_sq / target_params: caller-owned flat f32 device buffers of srl_apex_param_layout floats,
  * 16-byte aligned and disjoint.  The context owns the encoder's blocks (one saved block for the forward over s, one for the

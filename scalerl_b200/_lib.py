@@ -215,38 +215,23 @@ class SrlApexConfig(C.Structure):
 
 
 def apex_param_layout(A, dueling=False, num_atoms=0, noisy=False):
-    """(total floats, offsets, counts) of the Ape-X Q network's flat buffer in state_dict order: 10 tensors, or 12 with the dueling
-    head; num_atoms > 0: the categorical head's 10 (q.weight [A num_atoms, 512], q.bias [A num_atoms]); noisy: 14, or 18 with the
-    dueling head (srl_apex_param_layout_noisy)"""
+    """(total floats, offsets, counts) of the Ape-X Q network's flat buffer in state_dict order (srl_apex_param_layout_noisy): 10
+    tensors, or 12 with the dueling head; num_atoms > 0: the categorical head's 10 (q.weight [A num_atoms, 512], q.bias
+    [A num_atoms]); noisy: 14, or 18 with the dueling head"""
     off = (_L * 18)()
     cnt = (_L * 18)()
-    if noisy:
-        total = lib().srl_apex_param_layout_noisy(int(A), 1 if dueling else 0, int(num_atoms), 1, off, cnt)
-        if total < 0:
-            check(-1, 'srl_apex_param_layout_noisy')
-        n = 18 if dueling else 14
-        return int(total), [int(x) for x in off][:n], [int(x) for x in cnt][:n]
-    if num_atoms:
-        total = lib().srl_apex_param_layout_cat(int(A), int(num_atoms), off, cnt)
-    else:
-        total = lib().srl_apex_param_layout_ex(int(A), 1 if dueling else 0, off, cnt)
+    total = lib().srl_apex_param_layout_noisy(int(A), 1 if dueling else 0, int(num_atoms), 1 if noisy else 0, off, cnt)
     if total < 0:
-        check(-1, 'srl_apex_param_layout')
-    n = 12 if dueling else 10
+        check(-1, 'srl_apex_param_layout_noisy')
+    n = 6 + (3 if dueling else 2) * (4 if noisy else 2)
     return int(total), [int(x) for x in off][:n], [int(x) for x in cnt][:n]
 
 
 def apex_actor_create(A, num_envs, precision, seed, params, head) -> C.c_void_p:
-    """srl_apex_actor_create_ex / _cat / _noisy for ``head`` (dueling, num_atoms, v_min, v_max, noisy) on the device buffer at ``params``"""
+    """srl_apex_actor_create_noisy for ``head`` (dueling, num_atoms, v_min, v_max, noisy) on the device buffer at ``params``"""
     h = C.c_void_p()
-    if head.noisy:
-        check(lib().srl_apex_actor_create_noisy(A, num_envs, precision, int(head.dueling), head.num_atoms, head.v_min, head.v_max, 1, seed,
-                                                params, C.byref(h)), 'srl_apex_actor_create_noisy')
-    elif head.num_atoms:
-        check(lib().srl_apex_actor_create_cat(A, num_envs, precision, head.num_atoms, head.v_min, head.v_max, seed, params, C.byref(h)),
-              'srl_apex_actor_create_cat')
-    else:
-        check(lib().srl_apex_actor_create_ex(A, num_envs, precision, int(head.dueling), seed, params, C.byref(h)), 'srl_apex_actor_create_ex')
+    check(lib().srl_apex_actor_create_noisy(A, num_envs, precision, int(head.dueling), head.num_atoms, head.v_min, head.v_max, int(head.noisy),
+                                            seed, params, C.byref(h)), 'srl_apex_actor_create_noisy')
     return h
 
 

@@ -24,13 +24,14 @@ from __future__ import annotations
 import ctypes as C
 import math
 from collections import OrderedDict
+from functools import cached_property
 from typing import Dict, Optional
 
 import numpy as np
 import torch
 
 from ... import _lib
-from .learner import MAX_FRAMES, QHead, default_q_state_dict, flat_views, load_views
+from .learner import MAX_FRAMES, QHead, check_net_args, default_q_state_dict, flat_views, load_views
 
 PRECISIONS = {'bf16': 0, 'fp32_split': 1}
 
@@ -59,16 +60,14 @@ class B200ApexActor:
                  device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None, dueling_dqn: bool = False,
                  categorical_dqn: bool = False, v_min: float = 0.0, v_max: float = 200.0, num_atoms: int = 51, noisy_dqn: bool = False,
                  noisy_std: float = 0.5):
-        for name, v, hi in (('num_envs', num_envs, MAX_FRAMES), ('num_actions', num_actions, 31)):
-            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 1 <= v <= hi:
-                raise ValueError(f'{name} must be an int in [1, {hi}], got {v!r}')
+        if isinstance(num_envs, bool) or not isinstance(num_envs, (int, np.integer)) or not 1 <= num_envs <= MAX_FRAMES:
+            raise ValueError(f'num_envs must be an int in [1, {MAX_FRAMES}], got {num_envs!r}')
+        check_net_args(num_actions, noisy_std)
         if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 2 ** 64:
             raise ValueError(f'seed must be an int in [0, 2**64), got {seed!r}')
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be 'bf16' or 'fp32_split', got {precision!r}")
-        head = QHead.of(dueling_dqn, categorical_dqn, num_atoms, v_min, v_max, noisy_dqn)
-        if isinstance(noisy_std, bool) or not isinstance(noisy_std, (int, float)) or not (math.isfinite(noisy_std) and noisy_std >= 0.0):
-            raise ValueError(f'noisy_std must be finite and >= 0, got {noisy_std!r}')
+        self.head = head = QHead.of(dueling_dqn, categorical_dqn, num_atoms, v_min, v_max, noisy_dqn)
         priority_eps = float(priority_eps)
         if not (math.isfinite(priority_eps) and priority_eps > 0.0):
             raise ValueError(f'priority_eps must be finite and > 0 (a zero leaf makes the sampler\'s IS weight infinite), got {priority_eps}')
@@ -95,8 +94,9 @@ class B200ApexActor:
         self.load_state_dict(sd)
         self.weights_version = 0
 
-    @property
+    @cached_property
     def head(self) -> QHead:
+        """the Q head of the settings above (the constructor stores the one it built)"""
         return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max, self.noisy_dqn)
 
     def _stream(self):

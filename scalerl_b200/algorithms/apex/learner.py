@@ -40,34 +40,39 @@ from ... import _lib
 from ...learner import from_torch_optimizer_state, to_torch_optimizer_state
 from ..base import BaseAgent
 
-# state_dict order = AtariQNet.parameters() order = the integer keys of the Adam state (srl_apex_param_layout order)
-APEX_PARAM_NAMES = ('conv1.weight', 'conv1.bias', 'conv2.weight', 'conv2.bias', 'conv3.weight', 'conv3.bias',
-                    'fc.weight', 'fc.bias', 'q.weight', 'q.bias')
-# the same for the dueling head (srl_apex_param_layout_ex(A, 1) order)
-APEX_DUELING_PARAM_NAMES = APEX_PARAM_NAMES[:8] + ('value.weight', 'value.bias', 'advantage.weight', 'advantage.bias')
-NOISY_SUFFIXES = ('weight_mu', 'weight_sigma', 'bias_mu', 'bias_sigma')     # NoisyLinear's parameters, in registration order
-# the noisy networks (srl_apex_param_layout_noisy order): fc and each head layer as NoisyLinear
-APEX_NOISY_PARAM_NAMES = APEX_PARAM_NAMES[:6] + tuple(f'{l}.{s}' for l in ('fc', 'q') for s in NOISY_SUFFIXES)
-APEX_NOISY_DUELING_PARAM_NAMES = APEX_PARAM_NAMES[:6] + tuple(f'{l}.{s}' for l in ('fc', 'value', 'advantage') for s in NOISY_SUFFIXES)
 MAX_FRAMES = 65536           # frames of one encoder call (MAX_FRAMES in csrc/kernels.h)
-
-
-def apex_param_names(dueling: bool = False, noisy: bool = False):
-    if noisy:
-        return APEX_NOISY_DUELING_PARAM_NAMES if dueling else APEX_NOISY_PARAM_NAMES
-    return APEX_DUELING_PARAM_NAMES if dueling else APEX_PARAM_NAMES
+PLAIN_SUFFIXES = ('weight', 'bias')
+NOISY_SUFFIXES = ('weight_mu', 'weight_sigma', 'bias_mu', 'bias_sigma')     # NoisyLinear's parameters, in registration order
 
 
 def apex_param_shapes(num_actions: int, dueling: bool = False, num_atoms: int = 0, noisy: bool = False):
-    """the named shapes of the Q network's parameters; num_atoms > 0: the categorical head q = Linear(512, num_actions * num_atoms);
-    noisy: each of fc and the head layers as NoisyLinear's weight_mu, weight_sigma, bias_mu, bias_sigma"""
-    R = num_actions * num_atoms if num_atoms else num_actions
-    layers = [('fc', 512, 3136)] + ([('value', 1, 512), ('advantage', num_actions, 512)] if dueling else [('q', R, 512)])
-    conv = [('conv1.weight', (32, 4, 8, 8)), ('conv1.bias', (32,)), ('conv2.weight', (64, 32, 4, 4)), ('conv2.bias', (64,)),
-            ('conv3.weight', (64, 64, 3, 3)), ('conv3.bias', (64,))]
-    if noisy:
-        return OrderedDict(conv + [(f'{l}.{s}', (o, i) if s.startswith('weight') else (o,)) for l, o, i in layers for s in NOISY_SUFFIXES])
-    return OrderedDict(conv + [p for l, o, i in layers for p in ((f'{l}.weight', (o, i)), (f'{l}.bias', (o,)))])
+    """the named shapes of the Q network's parameters in state_dict order = AtariQNet.parameters() order = the integer keys of the
+    Adam state (srl_apex_param_layout_noisy order): conv1..3, fc, then q or value and advantage; num_atoms > 0: the categorical head
+    q = Linear(512, num_actions * num_atoms); noisy: fc and the head layers as NoisyLinear's weight_mu, weight_sigma, bias_mu,
+    bias_sigma"""
+    lin = NOISY_SUFFIXES if noisy else PLAIN_SUFFIXES
+    head = [('value', (1, 512)), ('advantage', (num_actions, 512))] if dueling else [('q', (num_actions * (num_atoms or 1), 512))]
+    layers = [('conv1', (32, 4, 8, 8), PLAIN_SUFFIXES), ('conv2', (64, 32, 4, 4), PLAIN_SUFFIXES), ('conv3', (64, 64, 3, 3), PLAIN_SUFFIXES),
+              ('fc', (512, 3136), lin)] + [(l, w, lin) for l, w in head]
+    return OrderedDict((f'{l}.{s}', w if s.startswith('weight') else w[:1]) for l, w, suffixes in layers for s in suffixes)
+
+
+def apex_param_names(dueling: bool = False, noisy: bool = False):
+    return tuple(apex_param_shapes(1, dueling, 0, noisy))
+
+
+APEX_PARAM_NAMES = apex_param_names()
+APEX_DUELING_PARAM_NAMES = apex_param_names(dueling=True)
+APEX_NOISY_PARAM_NAMES = apex_param_names(noisy=True)
+APEX_NOISY_DUELING_PARAM_NAMES = apex_param_names(dueling=True, noisy=True)
+
+
+def check_net_args(num_actions, noisy_std) -> None:
+    """ValueError unless num_actions is an int in [1, 31] and noisy_std (the noisy layers' sigma0) a finite number >= 0"""
+    if isinstance(num_actions, bool) or not isinstance(num_actions, (int, np.integer)) or not 1 <= num_actions <= 31:
+        raise ValueError(f'num_actions must be an int in [1, 31], got {num_actions!r}')
+    if isinstance(noisy_std, bool) or not isinstance(noisy_std, (int, float)) or not (math.isfinite(noisy_std) and noisy_std >= 0.0):
+        raise ValueError(f'noisy_std must be finite and >= 0, got {noisy_std!r}')
 
 
 def scale_noise(x: torch.Tensor) -> torch.Tensor:
@@ -232,11 +237,8 @@ class ApexHParams:
     def validate(self) -> None:
         if not (isinstance(self.batch_size, int) and 1 <= self.batch_size <= MAX_FRAMES):
             raise ValueError(f'batch_size must be an int in [1, {MAX_FRAMES}], got {self.batch_size!r}')
-        if not (isinstance(self.num_actions, int) and 1 <= self.num_actions <= 31):
-            raise ValueError(f'num_actions must be an int in [1, 31], got {self.num_actions!r}')
+        check_net_args(self.num_actions, self.noisy_std)
         self.head                            # ValueError on a bad head setting
-        if isinstance(self.noisy_std, bool) or not isinstance(self.noisy_std, (int, float)) or not (math.isfinite(self.noisy_std) and self.noisy_std >= 0.0):
-            raise ValueError(f'noisy_std must be finite and >= 0, got {self.noisy_std!r}')
         if not (math.isfinite(self.gamma) and self.gamma >= 0.0):
             raise ValueError(f'gamma must be finite and >= 0, got {self.gamma}')
         if not (math.isfinite(self.learning_rate) and self.learning_rate > 0.0):

@@ -142,8 +142,9 @@ using namespace srl;
 struct srl_apex_actor {
   int E, precision;
   uint2 key;
-  const float* w8[8];              // the encoder tensors of the snapshot
-  QHead head;                      // the snapshot's Q head
+  ApexNetDesc desc;
+  ApexNet snap;                    // the snapshot on its flat buffer (noisy: the mu tensors)
+  ApexNet run;                     // what the forwards run on: noisy, the kept draw's composed weights (apex_forward_net); else snap
   float* logits;                   // categorical: [2E][A K], the logits of the core rows
   srl_encoder_t* enc;
   char *saved, *scratch;           // encoder blocks for E frames: the two forwards of an add run one after the other
@@ -152,9 +153,7 @@ struct srl_apex_actor {
   int64_t* zero_action;
   double* prio;                    // [E] the priorities of the last add
   unsigned long long* draws;       // [0] draw counter, [1] the act kernel's ticket
-  // noisy networks: the snapshot's mu / sigma tensors, the kept draw, its counter and the composed weights (w8[6..7] and head)
-  int noisy;
-  NoisyTensors nz;
+  // noisy networks: the kept draw, its counter and the composed weights
   float *normals, *noise;
   unsigned long long* noise_draws;
   NoisyWeights cw;
@@ -172,16 +171,9 @@ int actor_rows(srl_apex_actor* X, int64_t saved, int64_t scratch, WsRow* t) {
   t[n++] = ws_row(nullptr, E, &X->zero_action);
   t[n++] = ws_row(nullptr, E, &X->prio);
   t[n++] = ws_row(nullptr, 2, &X->draws);
-  t[n++] = ws_row(nullptr, X->head.kind == Q_CATEGORICAL ? 2 * E * X->head.R : 0, &X->logits);
-  const int64_t on = X->noisy, R = X->head.R, dueling = X->head.kind == Q_DUELING, NN = on * noise_count(X->head);
-  t[n++] = ws_row("normals", NN, &X->normals);
-  t[n++] = ws_row("noise", NN, &X->noise);
-  t[n++] = ws_row(nullptr, on, &X->noise_draws);
-  t[n++] = ws_row("fc_weight", on * NOISE_FC_OUT * NOISE_FC_IN, &X->cw.fc_w);
-  t[n++] = ws_row("fc_bias", on * NOISE_FC_OUT, &X->cw.fc_b);
-  t[n++] = ws_row("head_weight", on * R * NOISE_HEAD_IN, &X->cw.h_w);
-  t[n++] = ws_row("head_bias", on * (dueling ? 1 : R), &X->cw.h_b);
-  t[n++] = ws_row("head_adv_bias", on * dueling * X->head.A, &X->cw.h_ba);
+  t[n++] = ws_row(nullptr, X->desc.head.kind == Q_CATEGORICAL ? 2 * E * X->desc.head.R : 0, &X->logits);
+  t[n++] = ws_row(nullptr, X->desc.noisy, &X->noise_draws);
+  n += noise_rows(X->desc, 0, &X->normals, &X->noise, &X->cw, t + n);
   return n;
 }
 constexpr int ACTOR_ROWS = 16;
@@ -189,50 +181,42 @@ constexpr int ACTOR_ROWS = 16;
 // a noisy actor's weights for its next forwards: a new draw first when `draw` (act), then the composition of the kept draw with the
 // snapshot as it is now.  Nothing without noise.
 cudaError_t actor_noise(srl_apex_actor* X, bool draw, cudaStream_t st) {
-  if (!X->noisy) return cudaSuccess;
+  if (!X->desc.noisy) return cudaSuccess;
   if (draw) {
-    const cudaError_t e = launch_noisy_draw(X->key, nullptr, X->noise_draws, 1, noise_count(X->head), &X->normals, &X->noise, st);
+    const cudaError_t e = launch_noisy_draw(X->key, nullptr, X->noise_draws, 1, noise_count(X->desc), &X->normals, &X->noise, st);
     if (e != cudaSuccess) return e;
   }
   const float* noise = X->noise;
-  return launch_noisy_compose(&X->nz, &X->cw, &noise, 1, X->head, st);
+  return launch_noisy_compose(&X->snap.nz, &X->cw, &noise, 1, X->desc.head, st);
 }
 
 // Q head rows of `frames` frames of obs into core (f <= E frames per call)
 int actor_forward(srl_apex_actor* X, const uint8_t* obs, int frames, float* core, cudaStream_t st) {
-  return srl_encoder_forward(X->enc, obs, X->zero_reward, X->zero_action, frames, 1, X->w8, X->saved, X->scratch, core, st);
+  return srl_encoder_forward(X->enc, obs, X->zero_reward, X->zero_action, frames, 1, X->run.w8, X->saved, X->scratch, core, st);
 }
 }  // namespace
 
-static int actor_create(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int noisy, uint64_t seed,
-                        const float* params, srl_apex_actor_t** out);
-
 extern "C" int srl_apex_actor_create(int A, int num_envs, int precision, uint64_t seed, const float* params, srl_apex_actor_t** out) {
-  return srl_apex_actor_create_ex(A, num_envs, precision, 0, seed, params, out);
+  return srl_apex_actor_create_noisy(A, num_envs, precision, 0, 0, 0.f, 0.f, 0, seed, params, out);
 }
 
 extern "C" int srl_apex_actor_create_ex(int A, int num_envs, int precision, int dueling, uint64_t seed, const float* params,
                                         srl_apex_actor_t** out) {
-  return actor_create(A, num_envs, precision, dueling, 0, 0.f, 0.f, 0, seed, params, out);
+  return srl_apex_actor_create_noisy(A, num_envs, precision, dueling, 0, 0.f, 0.f, 0, seed, params, out);
 }
 
 extern "C" int srl_apex_actor_create_cat(int A, int num_envs, int precision, int num_atoms, float v_min, float v_max, uint64_t seed,
                                          const float* params, srl_apex_actor_t** out) {
-  return actor_create(A, num_envs, precision, 0, num_atoms, v_min, v_max, 0, seed, params, out);
+  return srl_apex_actor_create_noisy(A, num_envs, precision, 0, num_atoms, v_min, v_max, 0, seed, params, out);
 }
 
 extern "C" int srl_apex_actor_create_noisy(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int noisy,
                                            uint64_t seed, const float* params, srl_apex_actor_t** out) {
-  return actor_create(A, num_envs, precision, dueling, num_atoms, v_min, v_max, noisy, seed, params, out);
-}
-
-static int actor_create(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int noisy,
-                        uint64_t seed, const float* params, srl_apex_actor_t** out) {
   REQ(params && out, "apex_actor_create: NULL argument");
   REQ(num_envs >= 1 && num_envs <= MAX_FRAMES, "apex_actor_create: num_envs=%d must be in [1, %d]", num_envs, MAX_FRAMES);
   REQ(precision == 0 || precision == 1, "apex_actor_create: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", precision);
-  QHead head;
-  int rc = make_q_head("apex_actor_create", A, dueling, num_atoms, v_min, v_max, noisy, &head);
+  ApexNetDesc d;
+  int rc = make_apex_desc("apex_actor_create", A, dueling, num_atoms, v_min, v_max, noisy, &d);
   if (rc) return rc;
   REQ(!misaligned(params, 16), "apex_actor_create: params must be 16-byte aligned");
   int64_t sb = 0, kb = 0;
@@ -244,11 +228,8 @@ static int actor_create(int A, int num_envs, int precision, int dueling, int num
   X->E = num_envs;
   X->precision = precision;
   X->key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-  const ApexNet snap = bind_apex(head, noisy, const_cast<float*>(params));
-  for (int i = 0; i < 8; ++i) X->w8[i] = snap.w8[i];
-  X->head = snap.q;
-  X->noisy = noisy;
-  X->nz = snap.nz;
+  X->desc = d;
+  X->snap = bind_apex(d, const_cast<float*>(params));
   rc = srl_encoder_create(precision, &X->enc);
   if (rc) return undo(rc);
   WsRow t[ACTOR_ROWS];
@@ -259,9 +240,9 @@ static int actor_create(int A, int num_envs, int precision, int dueling, int num
   e = cudaMemset(X->arena, 0, total);          // the zero columns, the draw counters and the ticket
   if (e != cudaSuccess) return undo(cuda_fail(e, "apex_actor_create: cudaMemset"));
   carve_rows(t, n, false, X->arena);
-  if (noisy) {      // the first draw, kept until the first act; the forwards run on the composed weights
-    bind_composed(snap, X->cw, X->w8, &X->head);
-    e = launch_noisy_draw(X->key, nullptr, X->noise_draws, 1, noise_count(X->head), &X->normals, &X->noise, nullptr);
+  X->run = apex_forward_net(d, X->snap, X->cw);
+  if (noisy) {      // the first draw, kept until the first act
+    e = launch_noisy_draw(X->key, nullptr, X->noise_draws, 1, noise_count(d), &X->normals, &X->noise, nullptr);
     if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
     if (e != cudaSuccess) return undo(cuda_fail(e, "apex_actor_create: first noise draw"));
   }
@@ -287,14 +268,14 @@ extern "C" int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const
   CU(actor_noise(X, true, st), "apex_actor_act: noise");
   rc = actor_forward(X, obs, E, X->core, st);
   if (rc) return rc;
-  CU(launch_apex_act(X->head, X->core, X->logits, E, epsilons, X->key, X->draws, actions, st), "apex_act");
+  CU(launch_apex_act(X->run.q, X->core, X->logits, E, epsilons, X->key, X->draws, actions, st), "apex_act");
   return 0;
 }
 
 extern "C" int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, int n, float* q_out, void* stream) {
   REQ(X && obs && q_out, "apex_actor_q_values: NULL pointer");
   REQ(n >= 1, "apex_actor_q_values: n=%d must be >= 1", n);
-  const int A = X->head.A;
+  const int A = X->desc.head.A;
   const Span s[2] = {{obs, n * ACTOR_OBS_BYTES, false, "obs"}, {q_out, (int64_t)n * A * 4, true, "q_out"}};
   int rc = check_spans(s, 2, "apex_actor_q_values");
   if (rc) return rc;
@@ -304,7 +285,7 @@ extern "C" int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, 
     const int f = n - f0 < X->E ? n - f0 : X->E;
     rc = actor_forward(X, obs + (size_t)f0 * ACTOR_OBS_BYTES, f, X->core, st);
     if (rc) return rc;
-    CU(launch_q_values(X->head, X->core, f, X->logits, q_out + (size_t)f0 * A, st), "q_values");
+    CU(launch_q_values(X->run.q, X->core, f, X->logits, q_out + (size_t)f0 * A, st), "q_values");
   }
   return 0;
 }
@@ -313,7 +294,7 @@ extern "C" int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name
   REQ(X && name && ptr && count, "apex_actor_debug_buffer: NULL argument");
   const int64_t rows = 2 * (int64_t)X->E;
   if (strcmp(name, "core") == 0) { *ptr = X->core; *count = rows * ENC_CORE; return 0; }
-  if (strcmp(name, "logits") == 0 && X->head.kind == Q_CATEGORICAL) { *ptr = X->logits; *count = rows * X->head.R; return 0; }
+  if (strcmp(name, "logits") == 0 && X->desc.head.kind == Q_CATEGORICAL) { *ptr = X->logits; *count = rows * X->desc.head.R; return 0; }
   int64_t sb = 0, kb = 0;
   int rc = srl_encoder_sizes(X->E, X->precision, &sb, &kb);
   if (rc) return rc;
@@ -336,7 +317,7 @@ int apex_actor_priorities(srl_apex_actor* X, const uint8_t* s, const uint8_t* s_
   int rc = actor_forward(X, s, E, X->core, st);
   if (!rc) rc = actor_forward(X, s_next, E, X->core + (size_t)E * ENC_CORE, st);
   if (rc) return rc;
-  CU(launch_apex_priorities(X->head, X->core, X->logits, E, action, reward, done, ptr, M, gamma_n, eps, X->prio, st), "apex_priorities");
+  CU(launch_apex_priorities(X->run.q, X->core, X->logits, E, action, reward, done, ptr, M, gamma_n, eps, X->prio, st), "apex_priorities");
   *prio = X->prio;
   return 0;
 }

@@ -894,39 +894,44 @@ extern "C" int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int fr
 // Ape-X learner step: three encoder forwards on the context's blocks, the Q-learning tail (dqn.cu), the encoder backward over s,
 // clip + Adam, and the priorities into the sampler's trees
 // ------------------------------------------------------------------------------------------------
-// state_dict order {conv1.w, conv1.b, conv2.w, conv2.b, conv3.w, conv3.b, fc.w, fc.b, q.w, q.b}; in memory fc.weight last.
-// dueling: {..., fc.b, value.w [1,512], value.b [1], advantage.w [A,512], advantage.b [A]}; in memory value.weight directly before
-// advantage.weight (one [(A + 1)][512] head block for the kernels) and value.bias before advantage.bias
-// categorical (atoms = K > 0): the plain order with q.weight [A K, 512] and q.bias [A K] (row a K + k: atom k of action a)
-// The layout depends on the head's kind and rows only.
+// The Q network's tensors in state_dict order: conv1..3 {weight, bias}, then fc and the head layers (q, or value [1, 512] and
+// advantage [A, 512]) as {weight, bias}, or noisy as {weight_mu, weight_sigma, bias_mu, bias_sigma}.  In memory (each segment padded
+// to 4 floats) they come in groups, each group by (mu / sigma, layer, weight / bias): the conv tensors; fc's biases; the head weights
+// and the head biases (plain: the weights first; noisy: the biases first); fc's weights.  So the dueling head's weight rows are one
+// [(A + 1)][512] block for the kernels (noisy: the mu rows one, the sigma rows another), the value row first.  The categorical head
+// (K atoms) is q with A K rows (row a K + k: atom k of action a).
 namespace srl {
-int64_t apex_layout(const QHead& h, int64_t* off, int64_t* cnt) {
-  const int64_t A = h.A, R = h.R;
-  const int64_t plain[10] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, R * 512, R};
-  const int64_t duel[12] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, 512 * 3136, 512, 512, 1, A * 512, A};
-  const int plain_order[10] = {0, 1, 2, 3, 4, 5, 7, 8, 9, 6};
-  const int duel_order[12] = {0, 1, 2, 3, 4, 5, 7, 8, 10, 9, 11, 6};
-  const bool dueling = h.kind == Q_DUELING;
-  const int64_t* counts = dueling ? duel : plain;
-  const int* order = dueling ? duel_order : plain_order;
-  const int n = dueling ? 12 : 10;
+int64_t apex_layout(const ApexNetDesc& d, int64_t* off, int64_t* cnt) {
+  const bool dueling = d.head.kind == Q_DUELING;
+  const int64_t layers[6][2] = {{32, 256}, {64, 512}, {64, 576}, {512, 3136}, {dueling ? 1 : d.head.R, 512}, {d.head.A, 512}};  // [out, in]
+  const int nl = dueling ? 6 : 5, S = d.noisy ? 2 : 1;
+  // the memory group of [conv, fc, head][weight, bias], without and with noise
+  static const int group[2][3][2] = {{{0, 0}, {4, 1}, {2, 3}}, {{0, 0}, {4, 1}, {3, 2}}};
   int64_t o = 0;
-  for (int k = 0; k < n; ++k) {
-    const int i = order[k];
-    if (off) off[i] = o;
-    if (cnt) cnt[i] = counts[i];
-    o += (counts[i] + 3) & ~int64_t(3);
-  }
+  for (int g = 0; g < 5; ++g)
+    for (int s = 0; s < S; ++s)
+      for (int l = 0, i = 0; l < nl; ++l) {
+        const int kind = l < 3 ? 0 : l == 3 ? 1 : 2, ns = kind ? S : 1;       // i: the layer's first tensor, ns: its mu / sigma
+        for (int p = 0; p < 2; ++p) {
+          if (group[d.noisy][kind][p] != g || s >= ns) continue;
+          const int t = i + p * ns + s;
+          const int64_t c = p ? layers[l][0] : layers[l][0] * layers[l][1];
+          if (off) off[t] = o;
+          if (cnt) cnt[t] = c;
+          o += (c + 3) & ~int64_t(3);
+        }
+        i += 2 * ns;
+      }
   return o;
 }
 
-int make_q_head(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int noisy, QHead* h) {
+int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int noisy, ApexNetDesc* d) {
   REQ(A >= 1 && A <= 31, "%s: A=%d must be in [1,31]", who, A);
   REQ(dueling == 0 || dueling == 1, "%s: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", who, dueling);
   REQ(noisy == 0 || noisy == 1, "%s: noisy=%d must be 0 (plain layers) or 1 (noisy fc and head layers)", who, noisy);
   REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "%s: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]", who,
       num_atoms, CAT_MAX_ATOMS);
-  *h = QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling};
+  *d = ApexNetDesc{QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling}, noisy};
   if (num_atoms == 0) return 0;
   REQ(std::isfinite(v_min) && std::isfinite(v_max) && v_min < v_max, "%s: v_min=%g, v_max=%g must be finite with v_min < v_max", who,
       (double)v_min, (double)v_max);
@@ -934,108 +939,89 @@ int make_q_head(const char* who, int A, int dueling, int num_atoms, float v_min,
   REQ(std::isfinite(c.dz) && c.dz > 0.f, "%s: the atom spacing (v_max - v_min) / (num_atoms - 1) = %g is not a positive finite float", who,
       (double)c.dz);
   REQ(dueling == 0, "%s: the categorical head (num_atoms=%d) with dueling=1 is not supported", who, num_atoms);
-  h->kind = Q_CATEGORICAL;
-  h->R = A * num_atoms;
-  h->c = c;
+  d->head.kind = Q_CATEGORICAL;
+  d->head.R = A * num_atoms;
+  d->head.c = c;
   return 0;
 }
 
-QHead bind_q_head(QHead h, const float* params) {
-  int64_t off[12];
-  apex_layout(h, off, nullptr);
-  h.W = params + off[8];
-  h.b = params + off[9];
-  h.ba = h.kind == Q_DUELING ? params + off[11] : nullptr;
-  return h;
-}
-
-QHeadGrad bind_q_grad(const QHead& h, float* grads) {
-  int64_t off[12];
-  apex_layout(h, off, nullptr);
-  return {grads + off[8], grads + off[9], h.kind == Q_DUELING ? grads + off[11] : nullptr};
-}
-
-// The noisy network: state_dict order {conv1..3 (6), fc.{weight_mu, weight_sigma, bias_mu, bias_sigma}, q.{...}} (14), or with the
-// dueling head {..., value.{weight_mu, weight_sigma, bias_mu, bias_sigma}, advantage.{...}} (18).  In memory the biases come first
-// (value.bias_mu before advantage.bias_mu, and so for sigma), then the head weights (the mu rows one [(A + 1)][512] block, the sigma
-// rows another), then fc.weight_mu and fc.weight_sigma; segments padded to 4 floats.
-int64_t apex_layout_noisy(const QHead& h, int64_t* off, int64_t* cnt) {
-  const int64_t A = h.A, R = h.R, F = 512 * 3136;
-  const int64_t plain[14] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, F, F, 512, 512, R * 512, R * 512, R, R};
-  const int64_t duel[18] = {32 * 256, 32, 64 * 512, 64, 64 * 576, 64, F, F, 512, 512, 512, 512, 1, 1, A * 512, A * 512, A, A};
-  const int plain_order[14] = {0, 1, 2, 3, 4, 5, 8, 9, 12, 13, 10, 11, 6, 7};
-  const int duel_order[18] = {0, 1, 2, 3, 4, 5, 8, 9, 12, 16, 13, 17, 10, 14, 11, 15, 6, 7};
-  const bool dueling = h.kind == Q_DUELING;
-  const int64_t* counts = dueling ? duel : plain;
-  const int* order = dueling ? duel_order : plain_order;
-  const int n = dueling ? 18 : 14;
-  int64_t o = 0;
-  for (int k = 0; k < n; ++k) {
-    const int i = order[k];
-    if (off) off[i] = o;
-    if (cnt) cnt[i] = counts[i];
-    o += (counts[i] + 3) & ~int64_t(3);
-  }
-  return o;
-}
-
-ApexNet bind_apex(const QHead& h, int noisy, float* base) {
-  ApexNet n = {};
+ApexNet bind_apex(const ApexNetDesc& d, float* base) {
   int64_t off[18];
-  if (!noisy) {
-    apex_layout(h, off, nullptr);
-    for (int i = 0; i < 8; ++i) n.w8[i] = base + off[i];
-    n.q = bind_q_head(h, base);
-    n.g = bind_q_grad(h, base);
-    return n;
+  apex_layout(d, off, nullptr);
+  auto at = [&](int t) { return base + off[t]; };
+  const bool dueling = d.head.kind == Q_DUELING;
+  const int S = d.noisy ? 2 : 1, F = 6, H = F + 2 * S, V = H + 2 * S;     // the first tensor of fc, the head, the advantage layer
+  ApexNet n = {};
+  for (int i = 0; i < 6; ++i) n.w8[i] = at(i);
+  n.w8[6] = at(F);
+  n.w8[7] = at(F + S);
+  n.q = d.head;
+  n.q.W = at(H); n.q.b = at(H + S); n.q.ba = dueling ? at(V + S) : nullptr;
+  n.g = {at(H), at(H + S), dueling ? at(V + S) : nullptr};
+  for (int s = 0; d.noisy && s < 2; ++s) {
+    n.nz.fc_w[s] = at(F + s);
+    n.nz.fc_b[s] = at(F + S + s);
+    n.nz.h_w[s] = at(H + s);
+    n.nz.h_b[s] = at(H + S + s);
+    n.nz.h_ba[s] = dueling ? at(V + S + s) : nullptr;
   }
-  apex_layout_noisy(h, off, nullptr);
-  const bool dueling = h.kind == Q_DUELING;
-  for (int i = 0; i < 6; ++i) n.w8[i] = base + off[i];
-  n.w8[6] = base + off[6];
-  n.w8[7] = base + off[8];
-  for (int s = 0; s < 2; ++s) {
-    n.nz.fc_w[s] = base + off[6 + s];
-    n.nz.fc_b[s] = base + off[8 + s];
-    n.nz.h_w[s] = base + off[10 + s];
-    n.nz.h_b[s] = base + off[12 + s];
-    n.nz.h_ba[s] = dueling ? base + off[16 + s] : nullptr;
-  }
-  n.q = h;
-  n.q.W = n.nz.h_w[0]; n.q.b = n.nz.h_b[0]; n.q.ba = n.nz.h_ba[0];
-  n.g = {n.nz.h_w[0], n.nz.h_b[0], n.nz.h_ba[0]};
   return n;
+}
+
+ApexNet apex_forward_net(const ApexNetDesc& d, const ApexNet& net, const NoisyWeights& w) {
+  if (!d.noisy) return net;
+  ApexNet r = net;
+  r.w8[6] = w.fc_w;
+  r.w8[7] = w.fc_b;
+  r.q.W = w.h_w; r.q.b = w.h_b; r.q.ba = d.head.kind == Q_DUELING ? w.h_ba : nullptr;
+  return r;
+}
+
+int noise_rows(const ApexNetDesc& d, int which, float** normals, float** noise, NoisyWeights* w, WsRow* t) {
+  static const char* const names[3][7] = {
+      {"normals", "noise", "fc_weight", "fc_bias", "head_weight", "head_bias", "head_adv_bias"},
+      {"normals_online", "noise_online", "fc_weight_online", "fc_bias_online", "head_weight_online", "head_bias_online", "head_adv_bias_online"},
+      {"normals_target", "noise_target", "fc_weight_target", "fc_bias_target", "head_weight_target", "head_bias_target", "head_adv_bias_target"}};
+  const char* const* nm = names[which];
+  const int64_t on = d.noisy, R = d.head.R, dueling = d.head.kind == Q_DUELING;
+  t[0] = ws_row(nm[0], noise_count(d), normals);
+  t[1] = ws_row(nm[1], noise_count(d), noise);
+  t[2] = ws_row(nm[2], on * NOISE_FC_OUT * NOISE_FC_IN, &w->fc_w);
+  t[3] = ws_row(nm[3], on * NOISE_FC_OUT, &w->fc_b);
+  t[4] = ws_row(nm[4], on * R * NOISE_HEAD_IN, &w->h_w);
+  t[5] = ws_row(nm[5], on * (dueling ? 1 : R), &w->h_b);
+  t[6] = ws_row(nm[6], on * dueling * d.head.A, &w->h_ba);
+  return 7;
 }
 }  // namespace srl
 
 extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) {
-  return apex_layout(QHead{Q_PLAIN, A, A}, offsets10, counts10);
+  return apex_layout(ApexNetDesc{QHead{Q_PLAIN, A, A}, 0}, offsets10, counts10);
 }
 extern "C" int64_t srl_apex_param_layout_ex(int A, int dueling, int64_t* offsets12, int64_t* counts12) {
   REQ(A >= 1 && A <= 31, "apex_param_layout: A=%d must be in [1,31]", A);
   REQ(dueling == 0 || dueling == 1, "apex_param_layout: dueling=%d must be 0 or 1", dueling);
-  return apex_layout(QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling}, offsets12, counts12);
+  return apex_layout(ApexNetDesc{QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling}, 0}, offsets12, counts12);
 }
 extern "C" int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offsets10, int64_t* counts10) {
   REQ(A >= 1 && A <= 31, "apex_param_layout: A=%d must be in [1,31]", A);
   REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "apex_param_layout: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]",
       num_atoms, CAT_MAX_ATOMS);
-  return apex_layout(QHead{num_atoms ? Q_CATEGORICAL : Q_PLAIN, A, A * (num_atoms ? num_atoms : 1)}, offsets10, counts10);
+  return apex_layout(ApexNetDesc{QHead{num_atoms ? Q_CATEGORICAL : Q_PLAIN, A, A * (num_atoms ? num_atoms : 1)}, 0}, offsets10, counts10);
 }
 extern "C" int64_t srl_apex_param_layout_noisy(int A, int dueling, int num_atoms, int noisy, int64_t* offsets18, int64_t* counts18) {
-  QHead h;
-  if (make_q_head("apex_param_layout", A, dueling, num_atoms, 0.f, 1.f, noisy, &h)) return -1;
-  return noisy ? apex_layout_noisy(h, offsets18, counts18) : apex_layout(h, offsets18, counts18);
+  ApexNetDesc d;
+  if (make_apex_desc("apex_param_layout", A, dueling, num_atoms, 0.f, 1.f, noisy, &d)) return -1;
+  return apex_layout(d, offsets18, counts18);
 }
 
 struct srl_apex_learner {
   srl_apex_config_t cfg;
   float *params, *grads, *m, *v, *target;
   int64_t nparams;
-  const float *w8[8], *t8[8];     // the encoder tensors of the online and target parameters
-  float* g8[8];
-  QHead on, tg;                   // the Q head of the online and target parameters
-  QHeadGrad g;                    // ... and its gradients
+  ApexNetDesc desc;
+  ApexNet net[3];                 // the online and target parameters and the gradients (noisy: the mu tensors)
+  ApexNet run[2];                 // what the step's online and target forwards run on (apex_forward_net)
   srl_encoder_t *E, *Eq;          // the step's encoder context, and the q-value forwards' own (lanes, events)
   char *saved_s, *saved_n, *enc_scratch;   // encoder blocks: the forward over s (read by the backward), the forwards over s'
   char *saved_q, *scratch_q;      // the q-value forwards' blocks: they may run on another stream than the step
@@ -1047,14 +1033,9 @@ struct srl_apex_learner {
   // the categorical head (cfg.num_atoms = K > 0): logits [B][A K] over s, s' (online, double DQN only) and s' (target), their
   // gradient, the projected targets m [B][K], the cross-entropies [B] and the q-value chunk's logits
   float *logits_s, *logits_n, *logits_nt, *dlogits, *mproj, *ce, *logits_q;
-  // noisy networks (cfg.noisy): the mu / sigma tensors of the online, target and gradient buffers, the step's normals and noise and
-  // the composed weights ([0] online, [1] target); the step runs the encoder and the head on sw8 / st8 and son / stg, which are the
-  // composed weights with noise and w8 / t8, on / tg without
-  NoisyTensors nz[2], nzg;
+  // noisy networks: the step's normals and noise and the composed weights ([0] online, [1] target)
   float *normals[2], *noise[2];
   NoisyWeights cw[2];
-  const float *sw8[8], *st8[8];
-  QHead son, stg;
   uint2 noise_key;
   char* arena;
 };
@@ -1101,28 +1082,13 @@ static int apex_rows(srl_apex_learner* L, const int64_t* b4, WsRow* t) {
   t[n++] = ws_row("m", B * K, &L->mproj);
   t[n++] = ws_row("ce", B * (K ? 1 : 0), &L->ce);
   t[n++] = ws_row(nullptr, QC * R, &L->logits_q);
-  // noisy networks: empty rows without noise
-  const int64_t dueling = L->cfg.dueling, HR = K ? R : A + dueling, on = L->cfg.noisy ? 1 : 0;
-  const int64_t NN = on * (NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (1 + dueling) + HR);
-  const char* names[2][7] = {{"normals_online", "noise_online", "fc_weight_online", "fc_bias_online", "head_weight_online",
-                              "head_bias_online", "head_adv_bias_online"},
-                             {"normals_target", "noise_target", "fc_weight_target", "fc_bias_target", "head_weight_target",
-                              "head_bias_target", "head_adv_bias_target"}};
-  for (int i = 0; i < 2; ++i) {
-    t[n++] = ws_row(names[i][0], NN, &L->normals[i]);
-    t[n++] = ws_row(names[i][1], NN, &L->noise[i]);
-    t[n++] = ws_row(names[i][2], on * NOISE_FC_OUT * NOISE_FC_IN, &L->cw[i].fc_w);
-    t[n++] = ws_row(names[i][3], on * NOISE_FC_OUT, &L->cw[i].fc_b);
-    t[n++] = ws_row(names[i][4], on * HR * NOISE_HEAD_IN, &L->cw[i].h_w);
-    t[n++] = ws_row(names[i][5], on * (dueling ? 1 : HR), &L->cw[i].h_b);
-    t[n++] = ws_row(names[i][6], on * dueling * A, &L->cw[i].h_ba);
-  }
+  for (int i = 0; i < 2; ++i) n += noise_rows(L->desc, 1 + i, &L->normals[i], &L->noise[i], &L->cw[i], t + n);
   return n;
 }
 constexpr int APEX_ROWS = 43;
 
-// -> the unbound head of a valid config
-static int check_apex_cfg(const srl_apex_config_t* c, QHead* head) {
+// -> the network of a valid config
+static int check_apex_cfg(const srl_apex_config_t* c, ApexNetDesc* d) {
   REQ(c, "apex_learner: config is NULL");
   REQ(c->B >= 1 && c->B <= MAX_FRAMES, "apex_learner: B=%d must be in [1, %d]", c->B, MAX_FRAMES);
   REQ(c->precision == 0 || c->precision == 1, "apex_learner: precision must be 0 (bf16 operands) or 1 (fp32-accurate split operands)");
@@ -1133,18 +1099,18 @@ static int check_apex_cfg(const srl_apex_config_t* c, QHead* head) {
   REQ(c->adam_beta1 >= 0.f && c->adam_beta1 < 1.f && c->adam_beta2 >= 0.f && c->adam_beta2 < 1.f, "apex_learner: Adam betas must be in [0, 1)");
   REQ(std::isfinite(c->adam_eps) && c->adam_eps >= 0.f, "apex_learner: adam_eps=%g must be finite and >= 0", (double)c->adam_eps);
   REQ(std::isfinite(c->priority_eps) && c->priority_eps >= 0.f, "apex_learner: priority_eps=%g must be finite and >= 0", (double)c->priority_eps);
-  return make_q_head("apex_learner", c->A, c->dueling, c->num_atoms, c->v_min, c->v_max, c->noisy, head);
+  return make_apex_desc("apex_learner", c->A, c->dueling, c->num_atoms, c->v_min, c->v_max, c->noisy, d);
 }
 
 extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* params, float* grads, float* exp_avg, float* exp_avg_sq,
                                        float* target_params, srl_apex_learner_t** out) {
-  QHead head;
-  int rc = check_apex_cfg(cfg, &head);
+  ApexNetDesc d;
+  int rc = check_apex_cfg(cfg, &d);
   if (rc) return rc;
   REQ(params && grads && exp_avg && exp_avg_sq && target_params && out, "apex_learner_create: NULL argument");
   REQ(!misaligned(params, 16) && !misaligned(grads, 16) && !misaligned(exp_avg, 16) && !misaligned(exp_avg_sq, 16) &&
       !misaligned(target_params, 16), "apex_learner_create: flat buffers must be 16-byte aligned");
-  const int64_t np = cfg->noisy ? apex_layout_noisy(head, nullptr, nullptr) : apex_layout(head, nullptr, nullptr);
+  const int64_t np = apex_layout(d, nullptr, nullptr);
   const Span s[5] = {{params, np * 4, true, "params"}, {grads, np * 4, true, "grads"}, {exp_avg, np * 4, true, "exp_avg"},
                      {exp_avg_sq, np * 4, true, "exp_avg_sq"}, {target_params, np * 4, true, "target_params"}};
   rc = check_spans(s, 5, "apex_learner_create");
@@ -1153,11 +1119,8 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   REQ(L, "out of host memory");
   auto undo = [L](int code) { srl_apex_learner_destroy(L); return code; };
   L->cfg = *cfg; L->params = params; L->grads = grads; L->m = exp_avg; L->v = exp_avg_sq; L->target = target_params; L->nparams = np;
-  const ApexNet on = bind_apex(head, cfg->noisy, params), tg = bind_apex(head, cfg->noisy, target_params),
-               gr = bind_apex(head, cfg->noisy, grads);
-  for (int i = 0; i < 8; ++i) { L->w8[i] = on.w8[i]; L->t8[i] = tg.w8[i]; L->g8[i] = gr.w8[i]; }
-  L->on = on.q; L->tg = tg.q; L->g = gr.g;
-  L->nz[0] = on.nz; L->nz[1] = tg.nz; L->nzg = gr.nz;
+  L->desc = d;
+  L->net[0] = bind_apex(d, params); L->net[1] = bind_apex(d, target_params); L->net[2] = bind_apex(d, grads);
   L->noise_key = make_uint2((uint32_t)cfg->noise_seed, (uint32_t)(cfg->noise_seed >> 32));
   rc = srl_encoder_create(cfg->precision, &L->E);
   if (!rc) rc = srl_encoder_create(cfg->precision, &L->Eq);
@@ -1174,13 +1137,7 @@ extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* para
   if (e == cudaSuccess) e = cudaMemset(grads, 0, np * 4);      // the padding between the segments enters the gradient norm
   if (e != cudaSuccess) return undo(cuda_fail(e, "apex_learner_create: cudaMemset"));
   carve_rows(t, n, false, L->arena);
-  if (cfg->noisy) {
-    bind_composed(on, L->cw[0], L->sw8, &L->son);
-    bind_composed(tg, L->cw[1], L->st8, &L->stg);
-  } else {
-    for (int i = 0; i < 8; ++i) { L->sw8[i] = L->w8[i]; L->st8[i] = L->t8[i]; }
-    L->son = L->on; L->stg = L->tg;
-  }
+  for (int i = 0; i < 2; ++i) L->run[i] = apex_forward_net(d, L->net[i], L->cw[i]);
   *out = L;
   return 0;
 }
@@ -1201,26 +1158,28 @@ extern "C" int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, 
   const srl_apex_config_t& c = L->cfg;
   const int B = c.B;
   const cudaStream_t st = (cudaStream_t)stream;
-  if (c.noisy) {      // update k's noise (k = the device step count) for both networks, and their composed weights
-    CU(launch_noisy_draw(L->noise_key, L->dstep, nullptr, 2, noise_count(L->on), L->normals, L->noise, st), "noisy_draw");
+  if (L->desc.noisy) {      // update k's noise (k = the device step count) for both networks, and their composed weights
+    CU(launch_noisy_draw(L->noise_key, L->dstep, nullptr, 2, noise_count(L->desc), L->normals, L->noise, st), "noisy_draw");
     const float* noise[2] = {L->noise[0], L->noise[1]};
-    CU(launch_noisy_compose(L->nz, L->cw, noise, 2, L->on, st), "noisy_compose");
+    const NoisyTensors nz[2] = {L->net[0].nz, L->net[1].nz};
+    CU(launch_noisy_compose(nz, L->cw, noise, 2, L->desc.head, st), "noisy_compose");
   }
   // the three forwards (the encoder checks obs / next_obs and the blocks); the target forward runs last so that its rows are the
   // ones left in saved_n
-  int rc = srl_encoder_forward(L->E, obs, reward, action, B, 1, L->sw8, L->saved_s, L->enc_scratch, L->core_s, stream);
-  if (!rc && c.double_dqn) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->sw8, L->saved_n, L->enc_scratch, L->core_n, stream);
-  if (!rc) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, L->st8, L->saved_n, L->enc_scratch, L->core_nt, stream);
+  const ApexNet &on = L->run[0], &tg = L->run[1];
+  int rc = srl_encoder_forward(L->E, obs, reward, action, B, 1, on.w8, L->saved_s, L->enc_scratch, L->core_s, stream);
+  if (!rc && c.double_dqn) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, on.w8, L->saved_n, L->enc_scratch, L->core_n, stream);
+  if (!rc) rc = srl_encoder_forward(L->E, next_obs, reward, action, B, 1, tg.w8, L->saved_n, L->enc_scratch, L->core_nt, stream);
   if (rc) return rc;
   const QTail t = {L->core_s, c.double_dqn ? L->core_n : nullptr, L->core_nt, action, reward, done, weights, B, c.gamma, c.priority_eps,
                    L->q, L->y, L->dcore, L->loss, L->tail_scratch, L->prio, L->dq, L->head_part, L->logits_s, L->logits_n, L->logits_nt,
                    L->mproj, L->ce, L->dlogits};
-  CU(launch_q_tail(L->son, L->stg, t, st), "q_tail");
-  CU(launch_q_wgrad(L->son, L->g, t, st), "q_wgrad");
+  CU(launch_q_tail(on.q, tg.q, t, st), "q_tail");
+  CU(launch_q_wgrad(on.q, L->net[2].g, t, st), "q_wgrad");
   // the gradients of the composed weights land in the mu segments
-  rc = srl_encoder_backward(L->E, L->dcore, B, 1, L->saved_s, L->enc_scratch, L->g8, stream);
+  rc = srl_encoder_backward(L->E, L->dcore, B, 1, L->saved_s, L->enc_scratch, L->net[2].w8, stream);
   if (rc) return rc;
-  if (c.noisy) CU(launch_noisy_sigma_grad(L->nzg, L->noise[0], L->on, st), "noisy_sigma_grad");
+  if (L->desc.noisy) CU(launch_noisy_sigma_grad(L->net[2].nz, L->noise[0], L->desc.head, st), "noisy_sigma_grad");
   const OptStep o = {1, L->params, L->grads, L->m, L->v, L->nparams, c.max_grad_norm, L->coef, L->opt_scratch, c.learning_rate,
                      c.adam_beta1, c.adam_beta2, c.adam_eps, 0, L->dstep, OptExtra{}};
   CU(launch_clip_optim(o, st), "clip+adam");
@@ -1260,10 +1219,10 @@ extern "C" int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* o
   if (rc) return rc;
   for (int f0 = 0; f0 < n; f0 += QC) {       // chunks through the q-value forwards' own context and blocks
     const int f = n - f0 < QC ? n - f0 : QC;
-    rc = srl_encoder_forward(L->Eq, obs + (size_t)f0 * 28224, L->zero_reward, L->zero_action, f, 1, L->w8, L->saved_q, L->scratch_q,
+    rc = srl_encoder_forward(L->Eq, obs + (size_t)f0 * 28224, L->zero_reward, L->zero_action, f, 1, L->net[0].w8, L->saved_q, L->scratch_q,
                              L->core_q, stream);
     if (rc) return rc;
-    CU(launch_q_values(L->on, L->core_q, f, L->logits_q, q_out + (size_t)f0 * A, (cudaStream_t)stream), "q_values");
+    CU(launch_q_values(L->net[0].q, L->core_q, f, L->logits_q, q_out + (size_t)f0 * A, (cudaStream_t)stream), "q_values");
   }
   return 0;
 }

@@ -247,15 +247,6 @@ struct QHead {
 struct QHeadGrad {
   float *gW, *gb, *gba;
 };
-// api.cu: the head a setting describes (num_atoms 0: a scalar head, whose support is not read), unbound; noisy must be 0 or 1 (the
-// head's layers noisy or not: the head itself is the same).  0, or SRL_EINVAL with "<who>: ..." as the message
-int make_q_head(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int noisy, QHead* h);
-// api.cu: the flat parameter layout of the Q network with head h (srl_apex_param_layout*'s): the offsets and counts (NULL: not wanted)
-// of its 10 (12: dueling) tensors -> the buffer's floats
-int64_t apex_layout(const QHead& h, int64_t* off, int64_t* cnt);
-// api.cu: h bound onto the flat parameter buffer `params` of its layout, and onto a gradient buffer of that layout
-QHead bind_q_head(QHead h, const float* params);
-QHeadGrad bind_q_grad(const QHead& h, float* grads);
 
 // One batch of B transitions: the core rows of the online forward over s, of the online forward over s' (NULL: no double DQN) and of
 // the target forward over s'; the batch columns; outputs q (Q(s, a); categorical: sum z p at the taken action), y (the target;
@@ -283,11 +274,10 @@ cudaError_t launch_q_wgrad(const QHead& h, const QHeadGrad& g, const QTail& t, c
 cudaError_t launch_q_values(const QHead& h, const float* core, int N, float* logits, float* q_out, cudaStream_t st);
 cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
 // ---- noisy.cu: noisy networks (Fortunato et al. 2018, factorised Gaussian noise) on the fc layer and the Q head
-// One network's noise vector f(x) = sgn(x) sqrt|x| of standard normals x, nn = noise_count(h) floats:
+// One network's noise vector f(x) = sgn(x) sqrt|x| of standard normals x, nn = noise_count floats:
 //   [fc in 3136 | fc out 512 | head in 512 (dueling: the value layer's, then the advantage layer's) | head out R (dueling: value, then
 //   the A advantage rows)]; every segment but the last starts on a multiple of 4 floats.
 constexpr int NOISE_FC_IN = 3136, NOISE_FC_OUT = 512, NOISE_HEAD_IN = 512, NOISE_HEAD_IN_OFF = NOISE_FC_IN + NOISE_FC_OUT;
-inline int noise_count(const QHead& h) { return NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (h.kind == Q_DUELING ? 2 : 1) + h.R; }
 // the noisy layers' tensors on one flat buffer, [0] mu and [1] sigma (of the parameters, or of their gradients): the fc weight
 // [512][3136] and bias [512]; the head in QHead's layout: W [R][512], b and (dueling) ba
 struct NoisyTensors {
@@ -308,25 +298,37 @@ cudaError_t launch_noisy_compose(const NoisyTensors* p, const NoisyWeights* w, c
                                  cudaStream_t st);
 // the sigma gradients g.x[1] = g.x[0] (.) eps of the online network's noise (the mu gradients are those of the composed weights)
 cudaError_t launch_noisy_sigma_grad(const NoisyTensors& g, const float* noise, const QHead& h, cudaStream_t st);
-// api.cu: the noisy Q network's layout (srl_apex_param_layout_noisy's): 14 tensors (18: dueling) -> the buffer's floats
-int64_t apex_layout_noisy(const QHead& h, int64_t* off, int64_t* cnt);
-// api.cu: one network of head h on a flat buffer of its layout (noisy: the noisy layout): the encoder's 8 tensors and the Q head
-// (noisy: fc's and the head's mu tensors), the head as a gradient binding, and (noisy) the noisy layers' mu / sigma pairs
+
+// The Ape-X Q network a setting describes: its head, unbound, and whether fc and the head layers are noisy (0 or 1)
+struct ApexNetDesc {
+  QHead head;
+  int noisy;
+};
+// api.cu: the network of a setting (num_atoms 0: a scalar head, whose support is not read).  0, or SRL_EINVAL with "<who>: ..." as
+// the message
+int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int noisy, ApexNetDesc* d);
+// the floats of one network's noise vector (0 without noise)
+inline int noise_count(const ApexNetDesc& d) {
+  return d.noisy ? NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (d.head.kind == Q_DUELING ? 2 : 1) + d.head.R : 0;
+}
+// api.cu: the flat parameter layout of network d (srl_apex_param_layout*'s): the offsets and counts (NULL: not wanted) of its
+// tensors in state_dict order (10, 12 dueling; noisy: 14, 18 dueling) -> the buffer's floats
+int64_t apex_layout(const ApexNetDesc& d, int64_t* off, int64_t* cnt);
+// One network of d on a flat buffer of its layout: the encoder's 8 tensors and the Q head (noisy: fc's and the head's mu tensors),
+// the head as a gradient binding, and (noisy) the noisy layers' mu / sigma pairs
 struct ApexNet {
   float* w8[8];
   QHead q;
   QHeadGrad g;
   NoisyTensors nz;
 };
-ApexNet bind_apex(const QHead& h, int noisy, float* base);
-// the network that runs on the composed weights w: net's conv tensors, w's fc and head (QHead's layout)
-inline void bind_composed(const ApexNet& net, const NoisyWeights& w, const float** w8, QHead* q) {
-  for (int i = 0; i < 6; ++i) w8[i] = net.w8[i];
-  w8[6] = w.fc_w;
-  w8[7] = w.fc_b;
-  *q = net.q;
-  q->W = w.h_w; q->b = w.h_b; q->ba = net.q.kind == Q_DUELING ? w.h_ba : nullptr;
-}
+// api.cu
+ApexNet bind_apex(const ApexNetDesc& d, float* base);
+// the network a forward of `net` runs on: noisy, net's conv tensors with fc and the head from the composed weights w; else net
+ApexNet apex_forward_net(const ApexNetDesc& d, const ApexNet& net, const NoisyWeights& w);
+// the rows of one network's normals, noise and composed weights (empty without noise), named with the suffix `which` (0: none,
+// 1: _online, 2: _target) -> the rows written
+int noise_rows(const ApexNetDesc& d, int which, float** normals, float** noise, NoisyWeights* w, WsRow* t);
 
 // dqn_cat.cu: the categorical halves of the launchers above
 // logits [N][R] = h W^T + b over N core rows (stride ENC_CORE), W [R][512]: one fmaf chain per logit over j = 0 .. 511 from 0, then
