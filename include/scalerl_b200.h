@@ -382,14 +382,17 @@ int srl_replay_gather(srl_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* 
  * advantage(h) = Linear(512, A), Q = V + Adv - mean_a Adv.  Both heads read the shared fc output (the paper's Atari network has two
  * separate 512-unit fc streams): the encoder is the same for both.  With `num_atoms` = K > 0 the head is categorical (C51,
  * Bellemare et al. 2017): q = Linear(512, A K), row a K + k atom k of action a, p(s)[a] = softmax over the action's K logits, Q(s, a) =
- * sum_k z_k p_k on the support z_k = v_min + k dz, dz = (v_max - v_min) / (K - 1) rounded once to fp32.
+ * sum_k z_k p_k on the support z_k = v_min + k dz, dz = (v_max - v_min) / (K - 1) rounded once to fp32.  With `num_quantiles` = N > 0
+ * the head is the quantile head (QR-DQN, Dabney et al. 2018): q = Linear(512, A N), row a N + i quantile i of action a at the midpoint
+ * tau^_i = (2 i + 1) / (2 N), Q(s, a) = (sum_i theta_{a,i}) / N.
  * srl_replay_* stores and folds n-step transitions (pass gamma^n for them, and srl_replay_per as `per`); srl_apex_actor_* acts and computes
  * their initial priorities.
  * Parameters in state_dict order {conv1.weight, conv1.bias, conv2.weight, conv2.bias, conv3.weight, conv3.bias, fc.weight, fc.bias,
  * q.weight [A,512], q.bias [A]}; srl_apex_param_layout returns the flat buffer's floats and each tensor's offset / count (int64[10]).
  * The dueling head's state_dict order is {conv1..3, fc, value.weight [1,512], value.bias [1], advantage.weight [A,512],
  * advantage.bias [A]} (int64[12], srl_apex_param_layout_ex); value.weight lies directly before advantage.weight.
- * The categorical head keeps the 10 plain names with q.weight [A K, 512] and q.bias [A K] (srl_apex_param_layout_cat).
+ * The categorical head keeps the 10 plain names with q.weight [A K, 512] and q.bias [A K] (srl_apex_param_layout_cat), and so does the
+ * quantile head with q.weight [A N, 512] and q.bias [A N] (srl_apex_param_layout_quantile).
  * Every head, with or without noise, has one layout rule (srl_apex_param_layout_noisy's): in memory, each segment padded to 4
  * floats, come the conv tensors, fc's bias, the head weights and the head biases (noisy: the head biases first), then fc's weight,
  * each group by (mu before sigma, layer).  Params, grads, both Adam states and the target copy share the layout. */
@@ -408,6 +411,8 @@ typedef struct srl_apex_config {
   float v_min, v_max;        /* the categorical support [v_min, v_max], finite, v_min < v_max (read when num_atoms > 0) */
   int32_t noisy;             /* 0: plain layers; 1: noisy fc and head layers (srl_apex_param_layout_noisy)        */
   uint64_t noise_seed;       /* the Philox key of the noise (read when noisy = 1)                                */
+  int32_t num_quantiles;     /* 0: no quantile head; N in [2, 256]: the quantile head (not with dueling = 1 or num_atoms > 0) */
+  float kappa;               /* the quantile Huber threshold, finite and > 0 (read when num_quantiles > 0; QR-DQN-1: 1)      */
 } srl_apex_config_t;
 int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10);
 /* the layout of either head: dueling 0 -> 10 tensors (srl_apex_param_layout's), 1 -> 12; -1 with srl_last_error set for A outside
@@ -424,6 +429,10 @@ int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offsets10, int6
  * In memory the biases come first, then the head weights (value.weight_mu directly before advantage.weight_mu, and the same for
  * sigma), then fc.weight_mu and fc.weight_sigma, as the rule above.  -> the buffer's floats, or -1 with srl_last_error set */
 int64_t srl_apex_param_layout_noisy(int A, int dueling, int num_atoms, int noisy, int64_t* offsets18, int64_t* counts18);
+/* The layout of every head: srl_apex_param_layout_noisy's with num_quantiles = N in [2, 256] for the quantile head (q.weight [A N, 512],
+ * q.bias [A N]; not with dueling = 1 or num_atoms > 0), 0 for the others.  -> the buffer's floats, or -1 with srl_last_error set */
+int64_t srl_apex_param_layout_quantile(int A, int dueling, int num_atoms, int num_quantiles, int noisy, int64_t* offsets18,
+                                       int64_t* counts18);
 /* params / grads / exp_avg / exp_avg_sq / target_params: caller-owned flat f32 device buffers of srl_apex_param_layout floats,
  * 16-byte aligned and disjoint.  The context owns the encoder's blocks (one saved block for the forward over s, one for the
  * forwards over s', their scratch) and the tail's buffers.  Synchronous. */
@@ -439,6 +448,10 @@ int srl_apex_learner_destroy(srl_apex_learner_t* L);
  *   a* as above on the expected Q;  m = the projection of p_t(s')[a*] moved to clamp(r + gamma (1 - d) z_j, v_min, v_max) onto the
  *   support (Algorithm 1, j ascending);  ce = -sum_k m_k log p(s)[a, k];  loss = mean(w ce);  priority = max(KL(m || p(s)[a]), 0) +
  *   priority_eps (Hessel et al. 2018).  q holds sum_k z_k p(s)[a, k], y holds sum_k z_k m_k.
+ * The quantile head (num_quantiles = N > 0) replaces it by the quantile Huber loss of Dabney et al. 2018 (eq. 10):
+ *   a* as above on Q = mean_i theta_i;  T_j = r + gamma theta_t(s')[a*, j] (T_j = r when d = 1 or gamma = 0: s' is not read);
+ *   u_ij = T_j - theta(s)[a, i];  rho_ij = |tau^_i - 1{u_ij < 0}| L_kappa(u_ij) / kappa, L_kappa the Huber loss;  loss_n = (1 / N)
+ *   sum_i sum_j rho_ij;  loss = mean(w loss_n);  priority = loss_n + priority_eps.  q holds Q(s, a), y holds mean_j T_j.
  *   clip_grad_norm_(max_grad_norm), torch.optim.Adam step with the step count kept on the device       (dqn_agent.py:172-182)
  * With noisy = 1 update k (the device step count before the update) first draws the noise of both networks: standard normals from
  * Philox4x32-10 keyed by noise_seed, counted by (k, network), Box-Muller.  The online network's one draw per layer serves Q(s) and the
@@ -461,7 +474,9 @@ int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* obs, int n, 
  * h = columns < 512), "dcore" f32 [B,514], "q", "y" f32 [B], "priorities" f64 [B], "loss" f32 [1], "step" i32 [1] (device step count),
  * and the bf16 activations the forward over s saved, in the learner's layouts (srl_learner_debug_buffer): "a1", "a2", "a3".
  * The categorical head adds "logits", "logits_next" (double DQN only), "logits_next_target" and "dlogits" f32 [B,A*K], "m" f32 [B,K]
- * (the projected targets) and "ce" f32 [B] (the cross-entropies); its "y" is sum_k z_k m_k.
+ * (the projected targets) and "ce" f32 [B] (the cross-entropies); its "y" is sum_k z_k m_k.  The quantile head adds "theta",
+ * "theta_next" (double DQN only), "theta_next_target" and "dtheta" f32 [B,A*N] (the quantiles and their gradient), "target_quantiles"
+ * f32 [B,N] and "qr_loss" f32 [B] (the per-transition losses).
  * Noisy networks add, per network <n> = "online" or "target", the last step's "normals_<n>" (the standard normals) and "noise_<n>"
  * (f of them) f32 [NN] = [fc in 3136 | fc out 512 | head in 512 (dueling: value's, then advantage's) | head out R (dueling: value's 1,
  * then advantage's A)], R = the head's rows (A, A K, or A + 1), and the composed weights "fc_weight_<n>" [512,3136], "fc_bias_<n>"
@@ -491,6 +506,12 @@ int srl_apex_actor_create_cat(int A, int num_envs, int precision, int num_atoms,
  * the prioritized add compose the kept draw with the snapshot as it is when they run. */
 int srl_apex_actor_create_noisy(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int noisy,
                                 uint64_t seed, const float* params, srl_apex_actor_t** out);
+/* the same with the quantile head: num_quantiles and kappa as srl_apex_config_t's (num_quantiles 0: srl_apex_actor_create_noisy's
+ * head); params in srl_apex_param_layout_quantile(A, dueling, num_atoms, num_quantiles, noisy) order.  Its Q values are the quantile
+ * means and its priorities the quantile Huber loss + priority_eps with the snapshot as online and target network
+ * (srl_apex_learner_step's bits) */
+int srl_apex_actor_create_quantile(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int num_quantiles,
+                                   float kappa, int noisy, uint64_t seed, const float* params, srl_apex_actor_t** out);
 int srl_apex_actor_destroy(srl_apex_actor_t* X);
 /* obs u8 [E,4,84,84], epsilons f32 [E] (device) -> actions i64 [E]: with probability epsilons[e] a uniform action, else the first
  * argmax of Q(obs[e]) (torch.argmax's pick).  The random numbers are Philox4x32-10 keyed by seed, counted by (draw, env); the launch
@@ -499,7 +520,8 @@ int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const float* eps
 /* Q(obs) with the snapshot for n >= 1 frames: obs u8 [n,4,84,84] -> q_out f32 [n,A] */
 int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, int n, float* q_out, void* stream);
 /* borrow the actor's buffers for tests: "core" f32 [2E,514] (rows 0..E-1: the last act or the states of the last prioritized add,
- * rows E..2E-1: its next states) and, categorical head only, "logits" f32 [2E,A*K] of the same rows.  A noisy actor adds its kept draw
+ * rows E..2E-1: its next states) and, categorical head only, "logits" f32 [2E,A*K] of the same rows (quantile head: "theta"
+ * f32 [2E,A*N]).  A noisy actor adds its kept draw
  * "normals" and "noise" and the weights its last call composed, "fc_weight", "fc_bias", "head_weight", "head_bias" and (dueling)
  * "head_adv_bias", in the layouts of srl_apex_learner_debug_buffer's */
 int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name, void** ptr, int64_t* count);

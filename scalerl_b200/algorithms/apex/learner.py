@@ -21,6 +21,11 @@ from the online distribution (Hessel et al. 2018).  The state-dict names stay th
 ``y = (mu_w + sigma_w * eps_w) x + mu_b + sigma_b * eps_b`` with ``eps_w = f(eps_out) f(eps_in)^T``, ``eps_b = f(eps_out)`` and
 ``f(x) = sgn(x) sqrt|x|``.  Update k draws new noise for the online network (shared by Q(s) and the double-DQN choice at s') and an
 independent draw for the target network, both from (seed, k); ``q_values``, ``predict`` and ``get_action`` use the mean weights mu.
+
+``ApexHParams(quantile_dqn=True)`` makes the head the quantile head of QR-DQN (Dabney et al. 2018): ``q = Linear(512, A *
+num_quantiles)``, row a N + i quantile i of action a at the midpoint tau_i = (2 i + 1) / (2 N), Q = the mean of an action's quantiles
+for acting and the greedy target, and the quantile Huber loss (threshold ``quantile_kappa``) against the target quantiles
+``r + gamma theta'(s')[a*]`` as the loss and the priority.  It needs no support; the state-dict names stay the plain head's ten.
 """
 from __future__ import annotations
 
@@ -45,13 +50,14 @@ PLAIN_SUFFIXES = ('weight', 'bias')
 NOISY_SUFFIXES = ('weight_mu', 'weight_sigma', 'bias_mu', 'bias_sigma')     # NoisyLinear's parameters, in registration order
 
 
-def apex_param_shapes(num_actions: int, dueling: bool = False, num_atoms: int = 0, noisy: bool = False):
+def apex_param_shapes(num_actions: int, dueling: bool = False, num_atoms: int = 0, noisy: bool = False, num_quantiles: int = 0):
     """the named shapes of the Q network's parameters in state_dict order = AtariQNet.parameters() order = the integer keys of the
-    Adam state (srl_apex_param_layout_noisy order): conv1..3, fc, then q or value and advantage; num_atoms > 0: the categorical head
-    q = Linear(512, num_actions * num_atoms); noisy: fc and the head layers as NoisyLinear's weight_mu, weight_sigma, bias_mu,
-    bias_sigma"""
+    Adam state (srl_apex_param_layout_quantile order): conv1..3, fc, then q or value and advantage; num_atoms > 0: the categorical head
+    q = Linear(512, num_actions * num_atoms); num_quantiles > 0: the quantile head q = Linear(512, num_actions * num_quantiles); noisy:
+    fc and the head layers as NoisyLinear's weight_mu, weight_sigma, bias_mu, bias_sigma"""
     lin = NOISY_SUFFIXES if noisy else PLAIN_SUFFIXES
-    head = [('value', (1, 512)), ('advantage', (num_actions, 512))] if dueling else [('q', (num_actions * (num_atoms or 1), 512))]
+    rows = num_actions * (num_atoms or num_quantiles or 1)
+    head = [('value', (1, 512)), ('advantage', (num_actions, 512))] if dueling else [('q', (rows, 512))]
     layers = [('conv1', (32, 4, 8, 8), PLAIN_SUFFIXES), ('conv2', (64, 32, 4, 4), PLAIN_SUFFIXES), ('conv3', (64, 64, 3, 3), PLAIN_SUFFIXES),
               ('fc', (512, 3136), lin)] + [(l, w, lin) for l, w in head]
     return OrderedDict((f'{l}.{s}', w if s.startswith('weight') else w[:1]) for l, w, suffixes in layers for s in suffixes)
@@ -139,6 +145,11 @@ def categorical_support(num_atoms: int, v_min: float, v_max: float) -> torch.Ten
     return torch.tensor(lo, dtype=torch.float32) + torch.arange(num_atoms, dtype=torch.float32) * dz
 
 
+def quantile_taus(num_quantiles: int) -> torch.Tensor:
+    """the quantile midpoints tau_i = (2 i + 1) / (2 N), i = 0 .. N - 1, each one fp32 division"""
+    return (2 * torch.arange(num_quantiles, dtype=torch.float32) + 1) / torch.tensor(2 * num_quantiles, dtype=torch.float32)
+
+
 class AtariQNet(nn.Module):
     """Nature DQN on 4 stacked 84x84 frames: AtariNet's conv1..3 and fc (scalerl/algorithms/utils/atari_model.py:30-47, 91-101)
     followed by ``q = nn.Linear(512, num_actions)``, or, with ``dueling``, by ``value = nn.Linear(512, 1)`` and ``advantage =
@@ -147,19 +158,26 @@ class AtariQNet(nn.Module):
     softmax per action, ``forward`` its expectation on the support (a non-persistent buffer: the state-dict names are the plain ten).
     Initialised by torch's default layer init, so ``torch.manual_seed(s)`` before construction fixes the weights.  With ``noisy``, fc
     and the head layers are ``NoisyLinear(..., noisy_std)`` (train mode: the noisy weights, eval mode: mu; ``reset_noise()`` redraws
-    every layer's noise)."""
+    every layer's noise).  With ``quantile``, ``q = nn.Linear(512, num_actions * num_quantiles)`` whose row a * num_quantiles + i is
+    quantile i of action a (QR-DQN): ``quantiles(obs)`` gives them, ``forward`` their mean (the midpoints ``taus`` are a non-persistent
+    buffer)."""
 
     def __init__(self, num_actions: int, observation_shape=(4, 84, 84), dueling: bool = False, categorical: bool = False,
-                 num_atoms: int = 51, v_min: float = 0.0, v_max: float = 200.0, noisy: bool = False, noisy_std: float = 0.5):
+                 num_atoms: int = 51, v_min: float = 0.0, v_max: float = 200.0, noisy: bool = False, noisy_std: float = 0.5,
+                 quantile: bool = False, num_quantiles: int = 200):
         super().__init__()
         if dueling and categorical:
             raise ValueError('the categorical head with the dueling head is not supported')
+        if quantile and (dueling or categorical):
+            raise ValueError('the quantile head with the dueling or the categorical head is not supported')
         self.observation_shape = tuple(observation_shape)
         self.num_actions = int(num_actions)
         self.dueling = bool(dueling)
         self.categorical = bool(categorical)
         self.noisy = bool(noisy)
         self.num_atoms = int(num_atoms) if self.categorical else 0
+        self.quantile = bool(quantile)
+        self.num_quantiles = int(num_quantiles) if self.quantile else 0
         linear = (lambda i, o: NoisyLinear(i, o, noisy_std)) if self.noisy else nn.Linear
         self.conv1 = nn.Conv2d(self.observation_shape[0], 32, kernel_size=8, stride=4)
         self.conv2 = nn.Conv2d(32, 64, kernel_size=4, stride=2)
@@ -171,6 +189,9 @@ class AtariQNet(nn.Module):
         elif self.categorical:
             self.q = linear(512, self.num_actions * self.num_atoms)
             self.register_buffer('support', categorical_support(self.num_atoms, v_min, v_max), persistent=False)
+        elif self.quantile:
+            self.q = linear(512, self.num_actions * self.num_quantiles)
+            self.register_buffer('taus', quantile_taus(self.num_quantiles), persistent=False)
         else:
             self.q = linear(512, self.num_actions)
 
@@ -196,10 +217,18 @@ class AtariQNet(nn.Module):
             raise ValueError('dist() needs the categorical head (AtariQNet(..., categorical=True))')
         return F.softmax(self.q(self._features(obs)).view(-1, self.num_actions, self.num_atoms), dim=2)
 
+    def quantiles(self, obs: torch.Tensor) -> torch.Tensor:
+        """quantile head: obs u8 [n, 4, 84, 84] -> the quantiles theta [n, A, num_quantiles]"""
+        if not self.quantile:
+            raise ValueError('quantiles() needs the quantile head (AtariQNet(..., quantile=True))')
+        return self.q(self._features(obs)).view(-1, self.num_actions, self.num_quantiles)
+
     def forward(self, obs: torch.Tensor) -> torch.Tensor:
         """obs u8 [N, 4, 84, 84] -> Q values [N, A]"""
         if self.categorical:
             return (self.dist(obs) * self.support).sum(2)
+        if self.quantile:
+            return self.quantiles(obs).mean(2)
         x = self._features(obs)
         if self.dueling:
             v, adv = self.value(x), self.advantage(x)
@@ -231,6 +260,9 @@ class ApexHParams:
     adam_beta1: float = 0.9
     adam_beta2: float = 0.999
     adam_eps: float = 1e-8
+    quantile_dqn: bool = False           # the quantile (QR-DQN) head q = Linear(512, A num_quantiles) and the quantile Huber loss
+    num_quantiles: int = 200             # N, the paper's Atari setting
+    quantile_kappa: float = 1.0          # the Huber threshold kappa > 0 (1: QR-DQN-1)
     optimizer: ClassVar[str] = 'adam'            # read by learner.py's optimizer-state converters
     lr_schedule: ClassVar[str] = 'constant'
 
@@ -261,7 +293,8 @@ class ApexHParams:
     @property
     def head(self) -> 'QHead':
         """the Q head these settings describe (ValueError on a bad one)"""
-        return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max, self.noisy_dqn)
+        return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max, self.noisy_dqn, self.quantile_dqn,
+                        self.num_quantiles, self.quantile_kappa)
 
     def to_c(self) -> _lib.SrlApexConfig:
         self.validate()
@@ -277,28 +310,38 @@ class ApexHParams:
         c.num_atoms = self.atoms()
         c.v_min, c.v_max = self.v_min, self.v_max
         c.noisy = 1 if self.noisy_dqn else 0
+        c.num_quantiles = self.quantiles()
+        c.kappa = self.quantile_kappa
         return c
 
     def atoms(self) -> int:
         """the categorical head's atom count, 0 for a scalar head"""
         return self.num_atoms if self.categorical_dqn else 0
 
+    def quantiles(self) -> int:
+        """the quantile head's quantile count, 0 for the other heads"""
+        return self.num_quantiles if self.quantile_dqn else 0
+
 
 @dataclass(frozen=True)
 class QHead:
-    """The Q head of the learner and its actors: q = Linear(512, A), the dueling head (``dueling``), or the categorical head on
-    ``num_atoms`` > 0 atoms of the support [v_min, v_max]; ``noisy``: fc and the head layers are noisy layers.  A scalar head keeps no
-    support, so equal heads compare equal."""
+    """The Q head of the learner and its actors: q = Linear(512, A), the dueling head (``dueling``), the categorical head on
+    ``num_atoms`` > 0 atoms of the support [v_min, v_max], or the quantile head on ``num_quantiles`` > 0 quantiles with the Huber
+    threshold ``kappa``; ``noisy``: fc and the head layers are noisy layers.  A head keeps no setting of another kind, so equal heads
+    compare equal."""
     dueling: bool = False
     num_atoms: int = 0
     v_min: float = 0.0
     v_max: float = 0.0
     noisy: bool = False
+    num_quantiles: int = 0
+    kappa: float = 0.0
 
     @classmethod
-    def of(cls, dueling_dqn, categorical_dqn, num_atoms, v_min, v_max, noisy_dqn=False) -> 'QHead':
-        """the head of ApexHParams' / B200ApexActor's settings, checked (the support, as the kernels read it in fp32, even when
-        categorical_dqn is off)"""
+    def of(cls, dueling_dqn, categorical_dqn, num_atoms, v_min, v_max, noisy_dqn=False, quantile_dqn=False, num_quantiles=200,
+           quantile_kappa=1.0) -> 'QHead':
+        """the head of ApexHParams' / B200ApexActor's settings, checked (the support and the quantile setting, as the kernels read
+        them in fp32, even when their head is off)"""
         if not isinstance(dueling_dqn, bool):
             raise ValueError(f'dueling_dqn must be a bool, got {dueling_dqn!r}')
         if not isinstance(categorical_dqn, bool):
@@ -313,21 +356,38 @@ class QHead:
             raise ValueError(f'noisy_dqn must be a bool, got {noisy_dqn!r}')
         if categorical_dqn and dueling_dqn:
             raise ValueError('categorical_dqn with dueling_dqn is not supported: choose one head')
+        if not isinstance(quantile_dqn, bool):
+            raise ValueError(f'quantile_dqn must be a bool, got {quantile_dqn!r}')
+        if isinstance(num_quantiles, bool) or not isinstance(num_quantiles, (int, np.integer)) or not 2 <= num_quantiles <= 256:
+            raise ValueError(f'num_quantiles must be an int in [2, 256], got {num_quantiles!r}')
+        with np.errstate(over='ignore'):
+            ok = not isinstance(quantile_kappa, bool) and isinstance(quantile_kappa, (int, float, np.floating)) and \
+                np.isfinite(np.float32(quantile_kappa)) and np.float32(quantile_kappa) > 0
+        if not ok:
+            raise ValueError(f'quantile_kappa must be a finite fp32 value > 0, got {quantile_kappa!r}')
+        if quantile_dqn and dueling_dqn:
+            raise ValueError('quantile_dqn with dueling_dqn is not supported: choose one head')
+        if quantile_dqn and categorical_dqn:
+            raise ValueError('quantile_dqn with categorical_dqn is not supported: choose one head')
+        if quantile_dqn:
+            return cls(noisy=noisy_dqn, num_quantiles=int(num_quantiles), kappa=float(quantile_kappa))
         return cls(False, int(num_atoms), float(v_min), float(v_max), noisy_dqn) if categorical_dqn else cls(dueling_dqn, noisy=noisy_dqn)
 
     def __str__(self):
         s = f'dueling_dqn={self.dueling}, categorical_dqn={self.num_atoms > 0}, noisy_dqn={self.noisy}'
+        if self.num_quantiles:
+            return s + f', quantile_dqn=True, (num_quantiles, quantile_kappa)={(self.num_quantiles, self.kappa)}'
         return s + f', (num_atoms, v_min, v_max)={(self.num_atoms, self.v_min, self.v_max)}' if self.num_atoms else s
 
     def names(self):
         return apex_param_names(self.dueling, self.noisy)
 
     def shapes(self, num_actions: int):
-        return apex_param_shapes(num_actions, self.dueling, self.num_atoms, self.noisy)
+        return apex_param_shapes(num_actions, self.dueling, self.num_atoms, self.noisy, self.num_quantiles)
 
     def layout(self, num_actions: int):
         """(total floats, offsets, counts) of the flat buffer"""
-        return _lib.apex_param_layout(num_actions, self.dueling, self.num_atoms, self.noisy)
+        return _lib.apex_param_layout(num_actions, self.dueling, self.num_atoms, self.noisy, self.num_quantiles)
 
 
 def flat_views(flat: torch.Tensor, off, cnt, shapes) -> 'OrderedDict[str, torch.Tensor]':
@@ -346,12 +406,13 @@ def load_views(dst: Dict[str, torch.Tensor], sd: Dict[str, torch.Tensor]) -> Non
 
 
 def default_q_state_dict(num_actions: int, seed: int = 0, dueling: bool = False, num_atoms: int = 0, noisy: bool = False,
-                         noisy_std: float = 0.5) -> 'OrderedDict[str, torch.Tensor]':
+                         noisy_std: float = 0.5, num_quantiles: int = 0) -> 'OrderedDict[str, torch.Tensor]':
     """AtariQNet's initial weights under ``torch.manual_seed(seed)``, drawn without disturbing the global RNG (num_atoms > 0: the
-    categorical head's; noisy: the noisy network's with sigma0 = noisy_std)"""
+    categorical head's; num_quantiles > 0: the quantile head's; noisy: the noisy network's with sigma0 = noisy_std)"""
     with torch.random.fork_rng(devices=[]):
         torch.manual_seed(seed)
-        net = AtariQNet(num_actions, dueling=dueling, categorical=num_atoms > 0, num_atoms=num_atoms or 51, noisy=noisy, noisy_std=noisy_std)
+        net = AtariQNet(num_actions, dueling=dueling, categorical=num_atoms > 0, num_atoms=num_atoms or 51, noisy=noisy, noisy_std=noisy_std,
+                        quantile=num_quantiles > 0, num_quantiles=num_quantiles or 200)
     return OrderedDict((k, v.detach().clone()) for k, v in net.state_dict().items())
 
 
@@ -392,7 +453,8 @@ class B200ApexLearner(BaseAgent):
                                                        C.byref(h)), 'srl_apex_learner_create')
             self._h = h
             self._stats = torch.zeros(4, device=self.device)      # {loss, gradient norm, clip coefficient, pad}
-        sd = default_q_state_dict(hp.num_actions, seed, head.dueling, head.num_atoms, head.noisy, hp.noisy_std) if init_state_dict is None else init_state_dict
+        sd = default_q_state_dict(hp.num_actions, seed, head.dueling, head.num_atoms, head.noisy, hp.noisy_std, head.num_quantiles) \
+            if init_state_dict is None else init_state_dict
         self.load_state_dict(sd)
         self.load_state_dict(sd, target=True)       # actor_target starts as a copy (dqn_agent.py:66-67)
         self.use_graph = use_graph
@@ -430,7 +492,7 @@ class B200ApexLearner(BaseAgent):
 
     def optimizer_state_dict(self) -> dict:
         """``torch.optim.Adam(AtariQNet(A, dueling=hp.dueling_dqn, categorical=hp.categorical_dqn, noisy=hp.noisy_dqn,
-        ...).parameters()).state_dict()`` layout"""
+        quantile=hp.quantile_dqn, ...).parameters()).state_dict()`` layout"""
         return to_torch_optimizer_state(self.hp, self._opt_tensors(), self._opt_steps, order=self.names)
 
     def load_optimizer_state_dict(self, sd: dict) -> None:
@@ -559,7 +621,7 @@ class B200ApexLearner(BaseAgent):
     def learn(self, experiences, weights: Optional[torch.Tensor] = None, idxs: Optional[torch.Tensor] = None, sampler=None,
               sync_stats: bool = True, use_graph: Optional[bool] = None) -> Dict[str, float]:
         """one update (apex/worker.py:134-161; dqn_agent.py:136-190) -> {'loss': float}, or {} with nothing synchronised.  The
-        categorical head's loss is mean(w * cross-entropy)."""
+        categorical head's loss is mean(w * cross-entropy), the quantile head's mean(w * quantile Huber loss)."""
         obs, action, reward, next_obs, done = self._inputs(experiences, weights, idxs, sampler)
         args = (obs, action, reward, next_obs, done, weights, idxs, sampler)
         key = tuple(a.data_ptr() if isinstance(a, torch.Tensor) else (a._h.value if a is not None else None) for a in args)
@@ -623,7 +685,8 @@ class B200ApexLearner(BaseAgent):
 
     def debug_buffer(self, name: str) -> torch.Tensor:
         """copy of one of the step's device buffers (tests only; names: srl_apex_learner_debug_buffer; the categorical head's
-        logits, dlogits and m come flat, [B * A * num_atoms] and [B * num_atoms])"""
+        logits, dlogits and m come flat, [B * A * num_atoms] and [B * num_atoms], and so do the quantile head's theta, dtheta and
+        target_quantiles)"""
         p, n = C.c_void_p(), C.c_int64()
         _lib.check(self._L.srl_apex_learner_debug_buffer(self._h, name.encode(), C.byref(p), C.byref(n)), 'debug_buffer')
         dt = {'priorities': torch.float64, 'step': torch.int32, 'a1': torch.bfloat16, 'a2': torch.bfloat16, 'a3': torch.bfloat16}.get(name, torch.float32)

@@ -2,13 +2,14 @@
 // Restates the reference's
 //   scalerl/algorithms/apex/worker.py:14-30 (Actor: one eps per actor), :59-79 (compute_prior: |Q(s)[a] - (r + mask gamma^steps max Q(s'))|)
 //   scalerl/algorithms/apex/memory.py:43-64 (PrioritizedReplayBuffer.add: each transition enters with its actor's priority)
-// with one encoder forward (srl_encoder_forward) per frame set and the Q head of the learner (dqn_head.cuh, dqn_cat.cuh), so that a
+// with one encoder forward (srl_encoder_forward) per frame set and the Q head of the learner (dqn_head.cuh, dqn_cat.cuh, dqn_qr.cuh), so that a
 // priority computed here has the bits of the learner's for the same weights.  fp32 on the CUDA cores: the Q head is 512 x A, no
 // tensor-core work.
 //   apex_act_kernel       the Q row, its first argmax and the epsilon-greedy draw (one warp per env), a template on the head kind
 //   apex_priority_kernel  q(s, a), the n-step target from max_a Q(s') and the priority (one warp per transition), plain or dueling
 //   apex_cat_priority_kernel  the same on the categorical head: the learner tail's cat_transition
-// The categorical head runs the learner's logits GEMM (dqn_cat.cu) first.  launch_apex_act and launch_apex_priorities are the one
+//   apex_qr_priority_kernel   the same on the quantile head: the learner tail's qr_transition
+// The categorical and quantile heads run the learner's logits GEMM (dqn_cat.cu) first.  launch_apex_act and launch_apex_priorities are the one
 // place that picks the kernels of a head.
 #include <math.h>
 #include <string.h>
@@ -98,7 +99,23 @@ __global__ void __launch_bounds__(128) apex_cat_priority_kernel(const QHead h, c
   if (lane == 0) prio[e] = cat_priority(r.kl, eps);
 }
 
-// the act kernel of head h over the E core rows (the categorical head: through logits [E][A K])
+// the quantile head: the learner tail's qr_transition with the snapshot's quantiles of s (theta_s) and s' (theta_n) as the online and
+// target network's, no double DQN -> the quantile Huber loss + eps
+__global__ void __launch_bounds__(128) apex_qr_priority_kernel(const QHead h, const float* __restrict__ theta_s, const float* __restrict__ theta_n,
+                                                               int E, const int64_t* __restrict__ action, const float* __restrict__ reward,
+                                                               const uint8_t* __restrict__ done, int64_t ptr, int64_t M, float gamma_n, float eps,
+                                                               double* __restrict__ prio) {
+  __shared__ float st[4][QR_MAX_QUANTILES];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, e = blockIdx.x * 4 + warp;
+  if (e >= E) return;
+  const int64_t slot = (ptr + e) % M;
+  const int act = ld_action(action + slot, h.A);
+  const QrLoss r = qr_transition<false>(theta_s + (size_t)e * h.R + (size_t)act * h.qr.N, nullptr, theta_n + (size_t)e * h.R, h.A, h.qr.N,
+                                        __ldg(reward + slot), done[slot] ? 0.f : gamma_n, h.qr.kappa, lane, st[warp], 0.f, nullptr);
+  if (lane == 0) prio[e] = qr_priority(r.loss, eps);
+}
+
+// the act kernel of head h over the E core rows (the categorical and quantile heads: through logits [E][R])
 cudaError_t launch_apex_act(const QHead& h, const float* core, float* logits, int E, const float* eps, uint2 key, unsigned long long* draws,
                             int64_t* actions, cudaStream_t st) {
   const int blocks = (E + 3) / 4;
@@ -111,10 +128,17 @@ cudaError_t launch_apex_act(const QHead& h, const float* core, float* logits, in
       apex_act_kernel<Q_CATEGORICAL><<<blocks, 128, 0, st>>>(h, logits, E, eps, key, draws, actions);
       break;
     }
+    case Q_QUANTILE: {
+      const cudaError_t e = launch_cat_logits(core, h.W, h.b, E, h.R, logits, st);
+      if (e != cudaSuccess) return e;
+      apex_act_kernel<Q_QUANTILE><<<blocks, 128, 0, st>>>(h, logits, E, eps, key, draws, actions);
+      break;
+    }
   }
   return cudaGetLastError();
 }
-// the priority kernel of head h over the core rows of s (core) and s' (core + E rows); the categorical head: through logits [2E][A K]
+// the priority kernel of head h over the core rows of s (core) and s' (core + E rows); the categorical and quantile heads: through
+// logits [2E][R]
 cudaError_t launch_apex_priorities(const QHead& h, const float* core, float* logits, int E, const int64_t* action, const float* reward,
                                    const uint8_t* done, int64_t ptr, int64_t M, float gamma_n, float eps, double* prio, cudaStream_t st) {
   const int blocks = (E + 3) / 4;
@@ -132,6 +156,12 @@ cudaError_t launch_apex_priorities(const QHead& h, const float* core, float* log
       apex_cat_priority_kernel<<<blocks, 128, 0, st>>>(h, logits, logits + (size_t)E * h.R, E, action, reward, done, ptr, M, gamma_n, eps, prio);
       break;
     }
+    case Q_QUANTILE: {
+      const cudaError_t e = launch_cat_logits(core, h.W, h.b, 2 * E, h.R, logits, st);      // s and s' rows in one GEMM
+      if (e != cudaSuccess) return e;
+      apex_qr_priority_kernel<<<blocks, 128, 0, st>>>(h, logits, logits + (size_t)E * h.R, E, action, reward, done, ptr, M, gamma_n, eps, prio);
+      break;
+    }
   }
   return cudaGetLastError();
 }
@@ -145,7 +175,7 @@ struct srl_apex_actor {
   ApexNetDesc desc;
   ApexNet snap;                    // the snapshot on its flat buffer (noisy: the mu tensors)
   ApexNet run;                     // what the forwards run on: noisy, the kept draw's composed weights (apex_forward_net); else snap
-  float* logits;                   // categorical: [2E][A K], the logits of the core rows
+  float* logits;                   // categorical / quantile: [2E][R], the logits (quantiles) of the core rows
   srl_encoder_t* enc;
   char *saved, *scratch;           // encoder blocks for E frames: the two forwards of an add run one after the other
   float* core;                     // [2E][ENC_CORE]: the forward over s (and act's), then the one over s'
@@ -171,7 +201,7 @@ int actor_rows(srl_apex_actor* X, int64_t saved, int64_t scratch, WsRow* t) {
   t[n++] = ws_row(nullptr, E, &X->zero_action);
   t[n++] = ws_row(nullptr, E, &X->prio);
   t[n++] = ws_row(nullptr, 2, &X->draws);
-  t[n++] = ws_row(nullptr, X->desc.head.kind == Q_CATEGORICAL ? 2 * E * X->desc.head.R : 0, &X->logits);
+  t[n++] = ws_row(nullptr, head_has_logits(X->desc.head) ? 2 * E * X->desc.head.R : 0, &X->logits);
   t[n++] = ws_row(nullptr, X->desc.noisy, &X->noise_draws);
   n += noise_rows(X->desc, 0, &X->normals, &X->noise, &X->cw, t + n);
   return n;
@@ -197,26 +227,32 @@ int actor_forward(srl_apex_actor* X, const uint8_t* obs, int frames, float* core
 }  // namespace
 
 extern "C" int srl_apex_actor_create(int A, int num_envs, int precision, uint64_t seed, const float* params, srl_apex_actor_t** out) {
-  return srl_apex_actor_create_noisy(A, num_envs, precision, 0, 0, 0.f, 0.f, 0, seed, params, out);
+  return srl_apex_actor_create_quantile(A, num_envs, precision, 0, 0, 0.f, 0.f, 0, 0.f, 0, seed, params, out);
 }
 
 extern "C" int srl_apex_actor_create_ex(int A, int num_envs, int precision, int dueling, uint64_t seed, const float* params,
                                         srl_apex_actor_t** out) {
-  return srl_apex_actor_create_noisy(A, num_envs, precision, dueling, 0, 0.f, 0.f, 0, seed, params, out);
+  return srl_apex_actor_create_quantile(A, num_envs, precision, dueling, 0, 0.f, 0.f, 0, 0.f, 0, seed, params, out);
 }
 
 extern "C" int srl_apex_actor_create_cat(int A, int num_envs, int precision, int num_atoms, float v_min, float v_max, uint64_t seed,
                                          const float* params, srl_apex_actor_t** out) {
-  return srl_apex_actor_create_noisy(A, num_envs, precision, 0, num_atoms, v_min, v_max, 0, seed, params, out);
+  return srl_apex_actor_create_quantile(A, num_envs, precision, 0, num_atoms, v_min, v_max, 0, 0.f, 0, seed, params, out);
 }
 
 extern "C" int srl_apex_actor_create_noisy(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int noisy,
                                            uint64_t seed, const float* params, srl_apex_actor_t** out) {
+  return srl_apex_actor_create_quantile(A, num_envs, precision, dueling, num_atoms, v_min, v_max, 0, 0.f, noisy, seed, params, out);
+}
+
+extern "C" int srl_apex_actor_create_quantile(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max,
+                                              int num_quantiles, float kappa, int noisy, uint64_t seed, const float* params,
+                                              srl_apex_actor_t** out) {
   REQ(params && out, "apex_actor_create: NULL argument");
   REQ(num_envs >= 1 && num_envs <= MAX_FRAMES, "apex_actor_create: num_envs=%d must be in [1, %d]", num_envs, MAX_FRAMES);
   REQ(precision == 0 || precision == 1, "apex_actor_create: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", precision);
   ApexNetDesc d;
-  int rc = make_apex_desc("apex_actor_create", A, dueling, num_atoms, v_min, v_max, noisy, &d);
+  int rc = make_apex_desc("apex_actor_create", A, dueling, num_atoms, v_min, v_max, num_quantiles, kappa, noisy, &d);
   if (rc) return rc;
   REQ(!misaligned(params, 16), "apex_actor_create: params must be 16-byte aligned");
   int64_t sb = 0, kb = 0;
@@ -294,7 +330,9 @@ extern "C" int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name
   REQ(X && name && ptr && count, "apex_actor_debug_buffer: NULL argument");
   const int64_t rows = 2 * (int64_t)X->E;
   if (strcmp(name, "core") == 0) { *ptr = X->core; *count = rows * ENC_CORE; return 0; }
-  if (strcmp(name, "logits") == 0 && X->desc.head.kind == Q_CATEGORICAL) { *ptr = X->logits; *count = rows * X->desc.head.R; return 0; }
+  if (strcmp(name, X->desc.head.kind == Q_QUANTILE ? "theta" : "logits") == 0 && head_has_logits(X->desc.head)) {
+    *ptr = X->logits; *count = rows * X->desc.head.R; return 0;
+  }
   int64_t sb = 0, kb = 0;
   int rc = srl_encoder_sizes(X->E, X->precision, &sb, &kb);
   if (rc) return rc;

@@ -899,7 +899,8 @@ extern "C" int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int fr
 // to 4 floats) they come in groups, each group by (mu / sigma, layer, weight / bias): the conv tensors; fc's biases; the head weights
 // and the head biases (plain: the weights first; noisy: the biases first); fc's weights.  So the dueling head's weight rows are one
 // [(A + 1)][512] block for the kernels (noisy: the mu rows one, the sigma rows another), the value row first.  The categorical head
-// (K atoms) is q with A K rows (row a K + k: atom k of action a).
+// (K atoms) is q with A K rows (row a K + k: atom k of action a), the quantile head (N quantiles) q with A N rows (row a N + i:
+// quantile i of action a).
 namespace srl {
 int64_t apex_layout(const ApexNetDesc& d, int64_t* off, int64_t* cnt) {
   const bool dueling = d.head.kind == Q_DUELING;
@@ -925,13 +926,26 @@ int64_t apex_layout(const ApexNetDesc& d, int64_t* off, int64_t* cnt) {
   return o;
 }
 
-int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int noisy, ApexNetDesc* d) {
+int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int num_quantiles, float kappa, int noisy,
+                   ApexNetDesc* d) {
   REQ(A >= 1 && A <= 31, "%s: A=%d must be in [1,31]", who, A);
   REQ(dueling == 0 || dueling == 1, "%s: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", who, dueling);
   REQ(noisy == 0 || noisy == 1, "%s: noisy=%d must be 0 (plain layers) or 1 (noisy fc and head layers)", who, noisy);
   REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "%s: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]", who,
       num_atoms, CAT_MAX_ATOMS);
+  REQ(num_quantiles == 0 || (num_quantiles >= 2 && num_quantiles <= QR_MAX_QUANTILES),
+      "%s: num_quantiles=%d must be 0 (no quantile head) or in [2, %d]", who, num_quantiles, QR_MAX_QUANTILES);
   *d = ApexNetDesc{QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling}, noisy};
+  if (num_quantiles) {
+    REQ(std::isfinite(kappa) && kappa > 0.f, "%s: kappa=%g must be finite and > 0 (the quantile Huber threshold)", who, (double)kappa);
+    REQ(dueling == 0, "%s: the quantile head (num_quantiles=%d) with dueling=1 is not supported", who, num_quantiles);
+    REQ(num_atoms == 0, "%s: the quantile head (num_quantiles=%d) with the categorical head (num_atoms=%d) is not supported", who,
+        num_quantiles, num_atoms);
+    d->head.kind = Q_QUANTILE;
+    d->head.R = A * num_quantiles;
+    d->head.qr = QrSetting{num_quantiles, kappa};
+    return 0;
+  }
   if (num_atoms == 0) return 0;
   REQ(std::isfinite(v_min) && std::isfinite(v_max) && v_min < v_max, "%s: v_min=%g, v_max=%g must be finite with v_min < v_max", who,
       (double)v_min, (double)v_max);
@@ -1010,8 +1024,12 @@ extern "C" int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offs
   return apex_layout(ApexNetDesc{QHead{num_atoms ? Q_CATEGORICAL : Q_PLAIN, A, A * (num_atoms ? num_atoms : 1)}, 0}, offsets10, counts10);
 }
 extern "C" int64_t srl_apex_param_layout_noisy(int A, int dueling, int num_atoms, int noisy, int64_t* offsets18, int64_t* counts18) {
-  ApexNetDesc d;
-  if (make_apex_desc("apex_param_layout", A, dueling, num_atoms, 0.f, 1.f, noisy, &d)) return -1;
+  return srl_apex_param_layout_quantile(A, dueling, num_atoms, 0, noisy, offsets18, counts18);
+}
+extern "C" int64_t srl_apex_param_layout_quantile(int A, int dueling, int num_atoms, int num_quantiles, int noisy, int64_t* offsets18,
+                                                  int64_t* counts18) {
+  ApexNetDesc d;      // the support and kappa do not shape the layout
+  if (make_apex_desc("apex_param_layout", A, dueling, num_atoms, 0.f, 1.f, num_quantiles, 1.f, noisy, &d)) return -1;
   return apex_layout(d, offsets18, counts18);
 }
 
@@ -1031,7 +1049,8 @@ struct srl_apex_learner {
   int64_t* zero_action;
   int* dstep;
   // the categorical head (cfg.num_atoms = K > 0): logits [B][A K] over s, s' (online, double DQN only) and s' (target), their
-  // gradient, the projected targets m [B][K], the cross-entropies [B] and the q-value chunk's logits
+  // gradient, the projected targets m [B][K], the cross-entropies [B] and the q-value chunk's logits.  The quantile head
+  // (cfg.num_quantiles = N > 0) keeps its quantiles [B][A N], dtheta, the target quantiles [B][N] and the losses [B] in the same rows.
   float *logits_s, *logits_n, *logits_nt, *dlogits, *mproj, *ce, *logits_q;
   // noisy networks: the step's normals and noise and the composed weights ([0] online, [1] target)
   float *normals[2], *noise[2];
@@ -1069,18 +1088,21 @@ static int apex_rows(srl_apex_learner* L, const int64_t* b4, WsRow* t) {
   t[n++] = ws_row("step", 4, &L->dstep);
   t[n++] = ws_row(nullptr, B, &L->dq);
   t[n++] = ws_row(nullptr, 4 + dqn_tail_blocks((int)B), &L->tail_scratch);
-  const int64_t K = L->cfg.num_atoms, R = A * K;     // K = 0: the scalar heads, whose rows below are empty
+  // K: the atoms or quantiles per action (0: the scalar heads, whose rows below are empty); the quantile head's rows have names of their own
+  const QHead& h = L->desc.head;
+  const bool qr = h.kind == Q_QUANTILE;
+  const int64_t K = h.kind == Q_CATEGORICAL ? h.c.K : qr ? h.qr.N : 0, R = A * K;
   t[n++] = ws_row(nullptr, K ? 0 : HEAD_GROUPS * (A + L->cfg.dueling) * 513, &L->head_part);
   t[n++] = ws_row(nullptr, 4, &L->coef);
   t[n++] = ws_row(nullptr, 2048, &L->opt_scratch);
   t[n++] = ws_row(nullptr, QC, &L->zero_reward);     // the reward / action columns of the q-value forwards (the Q head reads h only)
   t[n++] = ws_row(nullptr, QC, &L->zero_action);
-  t[n++] = ws_row("logits", B * R, &L->logits_s);
-  t[n++] = ws_row("logits_next", L->cfg.double_dqn ? B * R : 0, &L->logits_n);
-  t[n++] = ws_row("logits_next_target", B * R, &L->logits_nt);
-  t[n++] = ws_row("dlogits", B * R, &L->dlogits);
-  t[n++] = ws_row("m", B * K, &L->mproj);
-  t[n++] = ws_row("ce", B * (K ? 1 : 0), &L->ce);
+  t[n++] = ws_row(qr ? "theta" : "logits", B * R, &L->logits_s);
+  t[n++] = ws_row(qr ? "theta_next" : "logits_next", L->cfg.double_dqn ? B * R : 0, &L->logits_n);
+  t[n++] = ws_row(qr ? "theta_next_target" : "logits_next_target", B * R, &L->logits_nt);
+  t[n++] = ws_row(qr ? "dtheta" : "dlogits", B * R, &L->dlogits);
+  t[n++] = ws_row(qr ? "target_quantiles" : "m", B * K, &L->mproj);
+  t[n++] = ws_row(qr ? "qr_loss" : "ce", B * (K ? 1 : 0), &L->ce);
   t[n++] = ws_row(nullptr, QC * R, &L->logits_q);
   for (int i = 0; i < 2; ++i) n += noise_rows(L->desc, 1 + i, &L->normals[i], &L->noise[i], &L->cw[i], t + n);
   return n;
@@ -1099,7 +1121,7 @@ static int check_apex_cfg(const srl_apex_config_t* c, ApexNetDesc* d) {
   REQ(c->adam_beta1 >= 0.f && c->adam_beta1 < 1.f && c->adam_beta2 >= 0.f && c->adam_beta2 < 1.f, "apex_learner: Adam betas must be in [0, 1)");
   REQ(std::isfinite(c->adam_eps) && c->adam_eps >= 0.f, "apex_learner: adam_eps=%g must be finite and >= 0", (double)c->adam_eps);
   REQ(std::isfinite(c->priority_eps) && c->priority_eps >= 0.f, "apex_learner: priority_eps=%g must be finite and >= 0", (double)c->priority_eps);
-  return make_apex_desc("apex_learner", c->A, c->dueling, c->num_atoms, c->v_min, c->v_max, c->noisy, d);
+  return make_apex_desc("apex_learner", c->A, c->dueling, c->num_atoms, c->v_min, c->v_max, c->num_quantiles, c->kappa, c->noisy, d);
 }
 
 extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* params, float* grads, float* exp_avg, float* exp_avg_sq,

@@ -9,7 +9,8 @@
 // The Q head arithmetic (q_dot, q_max, dueling_q, q_row_max, the target and the priority) is dqn_head.cuh's, shared with the Ape-X actor.
 // The tail and the head gradients are templates on the scalar heads: DUELING = the dueling head V + Adv - mean(Adv) on the shared fc
 // output (Wang et al. 2016, eq. 9), whose A + 1 rows (the value row first) lie as one [(A + 1)][512] block.  launch_q_tail,
-// launch_q_wgrad and launch_q_values are the one place that picks the kernels of a head; the categorical head's are dqn_cat.cu's.
+// launch_q_wgrad and launch_q_values are the one place that picks the kernels of a head; the categorical head's are dqn_cat.cu's, the
+// quantile head's dqn_qr.cu's tail on dqn_cat.cu's GEMMs.
 #include "common.cuh"
 #include "dqn_cat.cuh"
 #include "dqn_head.cuh"
@@ -141,7 +142,7 @@ __global__ void __launch_bounds__(256) dqn_wgrad_reduce_kernel(const float* __re
   if (j < 512) gW[(size_t)a * 512 + j] = s; else if (!DUELING || a == 0) gb[a] = s; else gba[a - 1] = s;
 }
 
-// q_out[n][a] = Q(rows[n])[a] (q_lane: core rows, or the categorical head's logits), one warp per frame
+// q_out[n][a] = Q(rows[n])[a] (q_lane: core rows, or the categorical / quantile head's logits), one warp per frame
 template <QKind KIND>
 __global__ void __launch_bounds__(128) q_values_kernel(const QHead h, const float* __restrict__ rows, int N, float* __restrict__ q_out) {
   const int lane = threadIdx.x & 31, n = blockIdx.x * 4 + (threadIdx.x >> 5);
@@ -162,11 +163,12 @@ cudaError_t launch_q_tail(const QHead& on, const QHead& tg, const QTail& t, cuda
     case Q_PLAIN: dqn_tail_kernel<false><<<dqn_tail_blocks(t.B), 128, 0, st>>>(on, tg, t, 2.f / (float)t.B); break;
     case Q_DUELING: dqn_tail_kernel<true><<<dqn_tail_blocks(t.B), 128, 0, st>>>(on, tg, t, 2.f / (float)t.B); break;
     case Q_CATEGORICAL: return launch_cat_tail(on, tg, t, st);
+    case Q_QUANTILE: return launch_qr_tail(on, tg, t, st);
   }
   return cudaGetLastError();
 }
 cudaError_t launch_q_wgrad(const QHead& h, const QHeadGrad& g, const QTail& t, cudaStream_t st) {
-  if (h.kind == Q_CATEGORICAL) return launch_cat_wgrad(t.dlogits, t.core_s, t.B, h.R, g.gW, g.gb, st);
+  if (head_has_logits(h)) return launch_cat_wgrad(t.dlogits, t.core_s, t.B, h.R, g.gW, g.gb, st);
   const int nslab = (t.B + DQN_SLAB - 1) / DQN_SLAB, spg = (nslab + HEAD_GROUPS - 1) / HEAD_GROUPS, groups = (nslab + spg - 1) / spg;
   const dim3 grid((513 + 127) / 128, groups);
   if (h.kind == Q_DUELING) {
@@ -187,6 +189,12 @@ cudaError_t launch_q_values(const QHead& h, const float* core, int N, float* log
       const cudaError_t e = launch_cat_logits(core, h.W, h.b, N, h.R, logits, st);
       if (e != cudaSuccess) return e;
       q_values_kernel<Q_CATEGORICAL><<<blocks, 128, 0, st>>>(h, logits, N, q_out);
+      break;
+    }
+    case Q_QUANTILE: {
+      const cudaError_t e = launch_cat_logits(core, h.W, h.b, N, h.R, logits, st);
+      if (e != cudaSuccess) return e;
+      q_values_kernel<Q_QUANTILE><<<blocks, 128, 0, st>>>(h, logits, N, q_out);
       break;
     }
   }

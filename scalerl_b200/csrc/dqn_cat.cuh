@@ -7,6 +7,7 @@
 #pragma once
 #include "common.cuh"
 #include "dqn_head.cuh"
+#include "dqn_qr.cuh"
 #include "kernels.h"
 
 namespace srl {
@@ -39,12 +40,14 @@ SRL_DEVINL float cat_q_lane(const float* __restrict__ row, int A, const CatSuppo
   return lane < A ? cat_q(row + (size_t)lane * c.K, c) : 0.f;
 }
 // the Q row of frame n, one action per lane (lane a < A: Q_a), for every head: rows = the core rows [N][ENC_CORE] (scalar heads) or the
-// logits [N][A K] (categorical).  The plain head's dot products end in warp_sum, whose xor butterfly leaves the same sum on every lane,
-// so lane a holds the value q_max compares at a.
+// logits [N][R] (categorical, quantile: dqn_qr.cuh).  The plain head's dot products end in warp_sum, whose xor butterfly leaves the
+// same sum on every lane, so lane a holds the value q_max compares at a.
 template <QKind KIND>
 SRL_DEVINL float q_lane(const QHead& h, const float* rows, size_t n, int lane) {
   if constexpr (KIND == Q_CATEGORICAL) {
     return cat_q_lane(rows + n * h.R, h.A, h.c, lane);
+  } else if constexpr (KIND == Q_QUANTILE) {
+    return qr_q_lane(rows + n * h.R, h.A, h.qr.N, lane);
   } else if constexpr (KIND == Q_DUELING) {
     return dueling_q<false>(rows + n * ENC_CORE, h.W, h.b, h.ba, h.A, lane, nullptr);
   } else {

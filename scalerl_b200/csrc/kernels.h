@@ -216,10 +216,11 @@ cudaError_t launch_rmsprop(float* p, const float* g, float* v, int64_t n, const 
 cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, const float* coef, float lr, float b1, float b2, float eps,
                         int step, cudaStream_t st);
 
-// ---- dqn.cu, dqn_cat.cu: the Q head of the Ape-X learner step and actors (srl_apex_*)
+// ---- dqn.cu, dqn_cat.cu, dqn_qr.cu: the Q head of the Ape-X learner step and actors (srl_apex_*)
 // The encoder runs with a one-hot width of 1 for the Q network: its core rows are [h (512), clamp(reward), 1], ENC_CORE floats.
 constexpr int ENC_CORE = 514;
 constexpr int CAT_MAX_ATOMS = 64;
+constexpr int QR_MAX_QUANTILES = 256;
 // the categorical head's support z_k = v_min + k dz (dqn_cat.cuh)
 struct CatSupport {
   float v_min, v_max, dz;
@@ -229,20 +230,30 @@ struct CatSupport {
 inline CatSupport cat_support(int K, float v_min, float v_max) {
   return {v_min, v_max, (float)(((double)v_max - (double)v_min) / (double)(K - 1)), K};
 }
-enum QKind { Q_PLAIN, Q_DUELING, Q_CATEGORICAL };
+// the quantile head's N quantiles per action and its Huber threshold kappa > 0 (dqn_qr.cuh)
+struct QrSetting {
+  int N;
+  float kappa;
+};
+enum QKind { Q_PLAIN, Q_DUELING, Q_CATEGORICAL, Q_QUANTILE };
 // One Q head on the 512 h columns of the core rows, bound onto a flat parameter buffer (apex_layout order):
 //   Q_PLAIN        q = Linear(512, A): W = q.weight [A][512], b = q.bias [A]
 //   Q_DUELING      V + Adv - mean(Adv) (dqn_head.cuh's dueling_q): W = [value.weight; advantage.weight] [(A + 1)][512] (the value row
 //                  first), b = value.bias [1], ba = advantage.bias [A]
 //   Q_CATEGORICAL  C51, q = Linear(512, A K) (dqn_cat.cuh): W = q.weight [A K][512], b = q.bias [A K] (row a K + k: atom k of action
 //                  a) on the support c
-// R = W's rows: A, A + 1 or A K.
+//   Q_QUANTILE     QR-DQN, q = Linear(512, A N) (dqn_qr.cuh): W = q.weight [A N][512], b = q.bias [A N] (row a N + i: quantile i of
+//                  action a), with the setting qr
+// R = W's rows: A, A + 1, A K or A N.
 struct QHead {
   QKind kind;
   int A, R;
   const float *W, *b, *ba;
   CatSupport c;
+  QrSetting qr;
 };
+// the categorical and quantile heads run a GEMM to their rows [N][R] (logits, quantiles) before anything else of theirs
+inline bool head_has_logits(const QHead& h) { return h.kind == Q_CATEGORICAL || h.kind == Q_QUANTILE; }
 // the same tensors of a gradient buffer
 struct QHeadGrad {
   float *gW, *gb, *gba;
@@ -250,11 +261,13 @@ struct QHeadGrad {
 
 // One batch of B transitions: the core rows of the online forward over s, of the online forward over s' (NULL: no double DQN) and of
 // the target forward over s'; the batch columns; outputs q (Q(s, a); categorical: sum z p at the taken action), y (the target;
-// categorical: sum z m), priorities f64 [B], dcore [B][ENC_CORE] and loss [1] (mean(w (q - y)^2); categorical: mean(w ce)).
+// categorical: sum z m; quantile: the mean of the target quantiles), priorities f64 [B], dcore [B][ENC_CORE] and loss [1] (mean(w
+// (q - y)^2); categorical: mean(w ce); quantile: mean(w loss)).
 // scratch: 4 + dqn_tail_blocks(B) floats, zero before the first launch (re-armed by the kernel).  The scalar heads write dq [B] and
 // reduce the head gradients through head_part (HEAD_GROUPS * R * 513 floats); the categorical head writes the logits [B][A K] of the
 // three forwards (logits_n: double DQN only), the projected targets m [B][K], ce [B] and dlogits [B][A K] (zero outside the taken
-// action's K rows).
+// action's K rows).  The quantile head writes the same slots: its quantiles theta [B][A N] in the logits, the target quantiles
+// [B][N] in m, the per-transition loss [B] in ce and dtheta [B][A N] in dlogits.
 struct QTail {
   const float *core_s, *core_n, *core_nt;
   const int64_t* action; const float* reward; const uint8_t* done; const float* weight;
@@ -266,11 +279,11 @@ struct QTail {
   float *logits_s, *logits_n, *logits_nt, *m, *ce, *dlogits;
 };
 inline int dqn_tail_blocks(int B) { return (B + 3) / 4; }
-// the tail of `on` (the online head) and `tg` (the target head); the categorical head runs its logits GEMMs first
+// the tail of `on` (the online head) and `tg` (the target head); the categorical and quantile heads run their logits GEMMs first
 cudaError_t launch_q_tail(const QHead& on, const QHead& tg, const QTail& t, cudaStream_t st);
 // the head gradients (stored) of the tail t has run
 cudaError_t launch_q_wgrad(const QHead& h, const QHeadGrad& g, const QTail& t, cudaStream_t st);
-// q_out [N][A] = Q(h) over N core rows; the categorical head goes through logits [N][A K]
+// q_out [N][A] = Q(h) over N core rows; the categorical and quantile heads go through logits [N][R]
 cudaError_t launch_q_values(const QHead& h, const float* core, int N, float* logits, float* q_out, cudaStream_t st);
 cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
 // ---- noisy.cu: noisy networks (Fortunato et al. 2018, factorised Gaussian noise) on the fc layer and the Q head
@@ -304,9 +317,10 @@ struct ApexNetDesc {
   QHead head;
   int noisy;
 };
-// api.cu: the network of a setting (num_atoms 0: a scalar head, whose support is not read).  0, or SRL_EINVAL with "<who>: ..." as
-// the message
-int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int noisy, ApexNetDesc* d);
+// api.cu: the network of a setting (num_atoms 0: no categorical head, whose support is not read; num_quantiles 0: no quantile
+// head, whose kappa is not read).  0, or SRL_EINVAL with "<who>: ..." as the message
+int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int num_quantiles, float kappa, int noisy,
+                   ApexNetDesc* d);
 // the floats of one network's noise vector (0 without noise)
 inline int noise_count(const ApexNetDesc& d) {
   return d.noisy ? NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (d.head.kind == Q_DUELING ? 2 : 1) + d.head.R : 0;
@@ -337,6 +351,8 @@ cudaError_t launch_cat_logits(const float* core, const float* W, const float* b,
 cudaError_t launch_cat_tail(const QHead& on, const QHead& tg, const QTail& t, cudaStream_t st);
 // gW [R][512] = dlogits^T h, gb [R] = dlogits^T 1 over the N core rows (stored), each a fmaf chain over n = 0 .. N-1 in order
 cudaError_t launch_cat_wgrad(const float* dlogits, const float* core, int N, int R, float* gW, float* gb, cudaStream_t st);
+// dqn_qr.cu: the quantile head's tail (its quantiles, head gradients and q values run dqn_cat.cu's GEMMs)
+cudaError_t launch_qr_tail(const QHead& on, const QHead& tg, const QTail& t, cudaStream_t st);
 
 }  // namespace srl
 struct srl_per;

@@ -7,12 +7,15 @@ With --dueling the learner runs the dueling head (ApexHParams(dueling_dqn=True))
 and the torch statements use AtariQNet(A, dueling=True).  With --categorical it runs the categorical head (ApexHParams(categorical_dqn=True,
 num_atoms=--atoms, v_min=-10, v_max=10)) beside the plain one, the torch statements become C51's (projection, cross-entropy, KL
 priorities) on AtariQNet(A, categorical=True), and a last line gives the head kernels' times from torch.profiler at B = 512, A = 18
-with their FLOP rate against the fp32 data-sheet rate (67 TFLOP/s).  With --noisy it runs the noisy learner (ApexHParams(noisy_dqn=True))
-beside the plain one, the torch statements run on AtariQNet(A, noisy=True) with reset_noise() on the online and target network every
+with their FLOP rate against the fp32 data-sheet rate (67 TFLOP/s).  With --quantile it runs the quantile learners
+(ApexHParams(quantile_dqn=True, num_quantiles=N) for each N of --quantiles) and the categorical one at K = --atoms beside the plain one
+(the torch statements stay the plain network's), and a last line per N gives the quantile head's kernel times at B = 512, A = 18.
+With --noisy it runs the noisy learner (ApexHParams(noisy_dqn=True)) beside the plain one, the torch statements run on AtariQNet(A, noisy=True) with reset_noise() on the online and target network every
 step, and a last line gives the noise kernels' times from torch.profiler at B = 512, A = 18 with the bytes they move against the HBM3
 data-sheet bandwidth (3.35 TB/s).
 
-    python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18] [--dueling | --categorical [--atoms 51] | --noisy]
+    python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18] [--dueling | --categorical [--atoms 51] | --noisy |
+        --quantile [--quantiles 51,200]]
 """
 import argparse
 import json
@@ -149,6 +152,42 @@ def head_profile(atoms, B=512, A=18, steps=20):
             'head_share_of_step': total / step_us}
 
 
+def quantile_profile(N, B=512, A=18, steps=20):
+    """the quantile head's kernels in one captured learner step (torch.profiler over `steps` replays): mean µs per step, the GEMMs'
+    FLOP rate against the fp32 data-sheet rate and the tail's quantile pairs per second"""
+    from torch.profiler import ProfilerActivity, profile
+    exp, w, idxs = batch(B, A)
+    L, S = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, quantile_dqn=True, num_quantiles=N)), sampler()
+    step = lambda: L.learn(exp, weights=w, idxs=idxs, sampler=S, sync_stats=False)
+    for _ in range(3):
+        step()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            step()
+        torch.cuda.synchronize()
+    R = A * N
+    flops = {'cat_gemm_kernel<false>': 2.0 * B * R * 512 * 2, 'cat_gemm_kernel<true>': 2.0 * B * R * 513}    # two quantile sets: s, s' target
+    out, total = {}, 0.0
+    for e in prof.key_averages():
+        if 'cat_gemm' not in e.key and 'qr_tail' not in e.key:
+            continue
+        us = e.device_time_total / steps
+        name = 'qr_tail_kernel' if 'qr_tail' in e.key else ('cat_gemm_kernel<true>' if 'Lb1' in e.key or '<true>' in e.key else 'cat_gemm_kernel<false>')
+        out[name] = {'us_per_step': us}
+        if name in flops:
+            out[name]['tflops'] = flops[name] / us * 1e-6
+            out[name]['fraction_of_67_tflops'] = flops[name] / us * 1e-6 / 67.0
+        else:
+            out[name]['quantile_pairs_per_s'] = B * N * N / us * 1e6
+        total += us
+    step_us = 1e6 / timed(step, 50)
+    L.release_graphs()
+    L.close()
+    return {'card': card(), 'B': B, 'A': A, 'N': N, 'head_kernels': out, 'head_us_per_step': total, 'step_us': step_us,
+            'head_share_of_step': total / step_us}
+
+
 def noisy_profile(B=512, A=18, steps=20):
     """the noise kernels in one captured noisy learner step (torch.profiler over `steps` replays): mean µs per step, the bytes each
     moves (from the shapes) and its share of the HBM3 data-sheet bandwidth"""
@@ -221,10 +260,13 @@ def main():
     ap.add_argument('--categorical', action='store_true', help='add the categorical learner and run C51 in torch statements')
     ap.add_argument('--atoms', type=int, default=51)
     ap.add_argument('--noisy', action='store_true', help='add the noisy learner and run the torch statements on the noisy net')
+    ap.add_argument('--quantile', action='store_true', help='add the quantile learners and the categorical one at --atoms beside them')
+    ap.add_argument('--quantiles', default='51,200', help='the quantile learners\' num_quantiles (--quantile)')
     a = ap.parse_args()
-    if a.dueling + a.categorical + a.noisy > 1:
-        sys.exit('--dueling, --categorical and --noisy are separate comparisons: pass one')
+    if a.dueling + a.categorical + a.noisy + a.quantile > 1:
+        sys.exit('--dueling, --categorical, --noisy and --quantile are separate comparisons: pass one')
     atoms = a.atoms if a.categorical else 0
+    quantiles = [int(x) for x in a.quantiles.split(',')] if a.quantile else []
     if not torch.cuda.is_available():
         sys.exit('bench_apex.py measures on a CUDA device; none is present')
     name = card()
@@ -247,6 +289,16 @@ def main():
             LN, SN = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, noisy_dqn=True)), sampler()
             learners.append(LN)
             variants['b200_noisy_captured'] = lambda: LN.learn(exp, weights=w, idxs=idxs, sampler=SN, sync_stats=False)
+        if quantiles:
+            LC = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, categorical_dqn=True, num_atoms=a.atoms, v_min=V_MIN, v_max=V_MAX))
+            learners.append(LC)
+            variants[f'b200_categorical_K{a.atoms}_captured'] = (lambda L_, S_: lambda: L_.learn(exp, weights=w, idxs=idxs, sampler=S_,
+                                                                                               sync_stats=False))(LC, sampler())
+        for N in quantiles:
+            LQ = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, quantile_dqn=True, num_quantiles=N))
+            learners.append(LQ)
+            variants[f'b200_quantile_N{N}_captured'] = (lambda L_, S_: lambda: L_.learn(exp, weights=w, idxs=idxs, sampler=S_,
+                                                                                       sync_stats=False))(LQ, sampler())
         variants['torch_eager'] = TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms, noisy=a.noisy)
         variants['torch_captured'] = Captured(TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms, noisy=a.noisy))
         for fn in variants.values():           # warm-up: the learner's first call runs eagerly, the second captures
@@ -272,6 +324,8 @@ def main():
         print(json.dumps(head_profile(atoms)), flush=True)
     if a.noisy:
         print(json.dumps(noisy_profile()), flush=True)
+    for N in quantiles:
+        print(json.dumps(quantile_profile(N)), flush=True)
 
 
 if __name__ == '__main__':

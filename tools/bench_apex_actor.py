@@ -6,9 +6,11 @@ frames resident on the device (no env is stepped: the numbers price the GPU work
                  compute_prior (apex/worker.py:59-79) on the transitions the add completed and update_priorities of their slots
 Rounds alternate between the legs; the median and range over rounds are printed with the card's name and power limit, one JSON line
 per workload.  With --noisy a noisy actor (B200ApexActor(..., noisy_dqn=True): a new noise draw and the composition of its weights on
-every act) runs leg (a) beside the plain actor, and the act calls alone are timed for both ('act', 'noisy_act').
+every act) runs leg (a) beside the plain actor, and the act calls alone are timed for both ('act', 'noisy_act').  With --quantile a
+quantile actor (B200ApexActor(..., quantile_dqn=True, num_quantiles=--quantiles): the quantile GEMM, the quantile means and the quantile
+Huber priorities) runs leg (a) the same way ('quantile_actor', 'act', 'quantile_act').
 
-    python tools/bench_apex_actor.py [--rounds 5] [--steps 100] [--configs 64x6,64x18,256x6,256x18] [--noisy]
+    python tools/bench_apex_actor.py [--rounds 5] [--steps 100] [--configs 64x6,64x18,256x6,256x18] [--noisy | --quantile [--quantiles 200]]
 """
 import argparse
 import json
@@ -81,7 +83,11 @@ def main():
     ap.add_argument('--steps', type=int, default=100)
     ap.add_argument('--configs', default='64x6,64x18,256x6,256x18')
     ap.add_argument('--noisy', action='store_true', help='add the noisy actor and time act alone for both actors')
+    ap.add_argument('--quantile', action='store_true', help='add the quantile actor and time act alone for both actors')
+    ap.add_argument('--quantiles', type=int, default=200)
     a = ap.parse_args()
+    if a.noisy and a.quantile:
+        sys.exit('--noisy and --quantile are separate comparisons: pass one')
     if not torch.cuda.is_available():
         sys.exit('bench_apex_actor.py measures on a CUDA device; none is present')
     name = card()
@@ -109,6 +115,14 @@ def main():
                 mem_n.save_to_memory(obs, XN.act(obs), rew, nobs, done, is_vectorised=True, priorities_from=XN)
 
             legs.update({'noisy_actor': noisy_actor, 'act': lambda: X.act(obs), 'noisy_act': lambda: XN.act(obs)})
+        if a.quantile:
+            XN = B200ApexActor(E, A, priority_eps=PRIORITY_EPS, quantile_dqn=True, num_quantiles=a.quantiles)
+            mem_n = GpuPrioritizedReplayBuffer(MEMORY, E, n_step=N_STEP, gamma=GAMMA)
+
+            def quantile_actor():
+                mem_n.save_to_memory(obs, XN.act(obs), rew, nobs, done, is_vectorised=True, priorities_from=XN)
+
+            legs.update({'quantile_actor': quantile_actor, 'act': lambda: X.act(obs), 'quantile_act': lambda: XN.act(obs)})
         for fn in legs.values():
             for _ in range(5):
                 fn()
@@ -116,16 +130,16 @@ def main():
         for _ in range(a.rounds):
             for k, fn in legs.items():
                 rates[k].append(timed(fn, a.steps) * E)
-        out = {'card': name, 'E': E, 'A': A, 'n_step': N_STEP, 'memory_size': MEMORY, 'precision': 'bf16', 'rounds': a.rounds,
+        out = {'card': name, 'E': E, 'A': A, **({'num_quantiles': a.quantiles} if a.quantile else {}), 'n_step': N_STEP, 'memory_size': MEMORY, 'precision': 'bf16', 'rounds': a.rounds,
                'vector_steps_per_round': a.steps}
         for k, r in rates.items():
             r = sorted(r)
             out[k] = {'env_steps_per_s_median': r[len(r) // 2], 'env_steps_per_s_range': [r[0], r[-1]]}
         print(json.dumps(out), flush=True)
-        for m in (mem_a, mem_b, ref.mem) + ((mem_n,) if a.noisy else ()):
+        for m in (mem_a, mem_b, ref.mem) + ((mem_n,) if a.noisy or a.quantile else ()):
             m.close()
         X.close()
-        if a.noisy:
+        if a.noisy or a.quantile:
             XN.close()
         L.close()
         del ref
