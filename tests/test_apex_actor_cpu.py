@@ -7,11 +7,11 @@ import pytest
 import torch
 
 from oracle import apex_oracle as O
-from tests import apex_actor_ref as AR
 from scalerl_b200 import _lib
 from scalerl_b200 import build as srl_build
 from scalerl_b200.algorithms.apex import AtariQNet, B200ApexActor, apex_epsilons
 from scalerl_b200.data.replay_memory import GpuPrioritizedReplayBuffer
+from tests.apex_cases import frames, unbuilt
 
 
 @pytest.fixture(scope='module')
@@ -46,9 +46,7 @@ def test_constructor_errors_without_gpu(kw, match):
 
 def _unbuilt_actor(num_envs=4, num_actions=6):
     """an actor with only its host attributes: the checks before any device work"""
-    a = B200ApexActor.__new__(B200ApexActor)
-    a.num_envs, a.num_actions, a.device, a._h, a.priority_eps = num_envs, num_actions, torch.device('cuda', 0), None, 1e-6
-    return a
+    return unbuilt(B200ApexActor, num_envs=num_envs, num_actions=num_actions, device=torch.device('cuda', 0), _h=None, priority_eps=1e-6)
 
 
 @pytest.mark.parametrize('eps', [[0.1] * 3, [0.1] * 5, [0.1, 0.1, -0.1, 0.1], [0.1, 2.0, 0.1, 0.1]])
@@ -70,9 +68,7 @@ def test_sync_from_needs_a_learner():
 
 
 def _unbuilt_memory(num_envs):
-    m = GpuPrioritizedReplayBuffer.__new__(GpuPrioritizedReplayBuffer)
-    m.num_envs, m.device, m._h = num_envs, torch.device('cuda', 0), None
-    return m
+    return unbuilt(GpuPrioritizedReplayBuffer, num_envs=num_envs, device=torch.device('cuda', 0), _h=None)
 
 
 @pytest.mark.parametrize('actor,match', [(object(), 'B200ApexActor'), (_unbuilt_actor(num_envs=3), 'num_envs'), ('dev', 'cuda:1')])
@@ -113,23 +109,19 @@ def _sd(A, seed=0):
     return AtariQNet(A).state_dict()
 
 
-def _frames(N, seed):
-    return torch.randint(0, 256, (N, 4, 84, 84), dtype=torch.uint8, generator=torch.Generator().manual_seed(seed))
-
-
 def test_initial_priorities_hand_computed():
     A, N = 5, 6
     sd = _sd(A)
-    s, ns = _frames(N, 1), _frames(N, 2)
+    s, ns = frames(N, 1), frames(N, 2)
     a = torch.tensor([0, 1, 2, 3, 4, 2])
     R = torch.tensor([0.5, -1.0, 2.0, 0.0, 0.25, 3.0])
     q = O.RefQNet(A, sd)(s).detach()
     qa = q[torch.arange(N), a]
     # all done: y = R, whatever gamma and s'
-    p = AR.initial_priorities(sd, s, a, R, ns, torch.ones(N, dtype=torch.bool), 0.97, 1e-6)
+    p = O.initial_priorities(sd, s, a, R, ns, torch.ones(N, dtype=torch.bool), 0.97, 1e-6)
     assert p.dtype == torch.float64 and torch.equal(p, (qa - R).abs().double() + 1e-6)
     # gamma = 0: y = R
-    p0 = AR.initial_priorities(sd, s, a, R, ns, torch.zeros(N, dtype=torch.bool), 0.0, 0.0)
+    p0 = O.initial_priorities(sd, s, a, R, ns, torch.zeros(N, dtype=torch.bool), 0.0, 0.0)
     assert torch.equal(p0, (qa - R).abs().double())
     # a Q head with a unique argmax at s': q.bias[3] dominates, so max_a Q(s') = Q(s')[3] and y = R + gamma_n Q(s')[3] where not done
     sd2 = {k: v.clone() for k, v in sd.items()}
@@ -139,6 +131,6 @@ def test_initial_priorities_hand_computed():
     d = torch.tensor([0, 1, 0, 0, 1, 0], dtype=torch.bool)
     q2 = O.RefQNet(A, sd2)(s).detach()[torch.arange(N), a]
     y = R + (1 - d.float()) * 0.5 * qn[:, 3]
-    p2 = AR.initial_priorities(sd2, s, a, R, ns, d, 0.5, 1e-3)
+    p2 = O.initial_priorities(sd2, s, a, R, ns, d, 0.5, 1e-3)
     assert torch.equal(p2, (q2 - y).abs().double() + 1e-3)
     assert torch.equal(p2[d], (q2 - R).abs().double()[d] + 1e-3)

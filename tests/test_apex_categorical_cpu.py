@@ -11,11 +11,12 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import apex_categorical_ref as R
+from oracle import apex_oracle as O
 from scalerl_b200 import _lib
 from scalerl_b200 import build as srl_build
 from scalerl_b200.algorithms.apex import (APEX_PARAM_NAMES, ApexHParams, AtariQNet, B200ApexActor, B200ApexLearner, apex_param_shapes,
                                           categorical_support, default_q_state_dict)
+from tests.apex_cases import frames, unbuilt
 
 
 @pytest.fixture(scope='module')
@@ -91,9 +92,9 @@ def test_categorical_forward_is_the_formula(A, K, lo, hi):
     assert got_p.shape == (7, A, K) and got_q.shape == (7, A)
     assert float((got_p - want_p).abs().max()) <= 1e-6
     assert float((got_q - want_q).abs().max()) <= 1e-5 * max(abs(lo), abs(hi))
-    assert torch.equal(categorical_support(K, lo, hi), R.support(K, lo, hi)[0])
+    assert torch.equal(categorical_support(K, lo, hi), O.support(K, lo, hi)[0])
     # the oracle's network computes the same logits from the same state dict
-    assert torch.equal(R.CatRefQNet(A, K, net.state_dict()).logits(obs), net.q(net._features(obs)).view(7, A, K))
+    assert torch.equal(O.RefQNet(A, net.state_dict(), O.Head('categorical', num_atoms=K, v_min=lo, v_max=hi))(obs), net.q(net._features(obs)).view(7, A, K))
 
 
 @pytest.mark.parametrize('K', [2, 51, 64])
@@ -149,20 +150,13 @@ def test_categorical_c_argument_errors(lib):
     assert b'NULL' in lib.srl_last_error()
 
 
-def _unbuilt(cls, **attrs):
-    o = cls.__new__(cls)
-    for k, v in attrs.items():
-        setattr(o, k, v)
-    return o
-
-
 @pytest.mark.parametrize('learner,msg', [(dict(categorical_dqn=False), 'categorical_dqn'), (dict(num_atoms=64), 'num_atoms'),
                                          (dict(v_min=-10.0), 'v_min'), (dict(v_max=10.0), 'v_max')])
 def test_sync_from_needs_the_same_head(learner, msg):
     hp = dict(num_actions=6, categorical_dqn=True, v_min=0.0, v_max=200.0, num_atoms=51)
     hp.update(learner)
-    L = _unbuilt(B200ApexLearner, hp=ApexHParams(**hp), device=torch.device('cuda', 0))
-    X = _unbuilt(B200ApexActor, num_envs=4, num_actions=6, dueling_dqn=False, categorical_dqn=True, num_atoms=51, v_min=0.0, v_max=200.0,
+    L = unbuilt(B200ApexLearner, hp=ApexHParams(**hp), device=torch.device('cuda', 0))
+    X = unbuilt(B200ApexActor, num_envs=4, num_actions=6, dueling_dqn=False, categorical_dqn=True, num_atoms=51, v_min=0.0, v_max=200.0,
                  device=torch.device('cuda', 0), _h=None)
     with pytest.raises(ValueError, match=msg):
         X.sync_from(L)
@@ -181,11 +175,11 @@ def test_projection_preserves_mass_and_equals_the_fp64_loop(K, lo, hi, gamma):
     g = torch.Generator().manual_seed(1)
     r = 4 * torch.randn(N, generator=g) * (hi - lo) / 20
     d = torch.rand(N, generator=g) < 0.3
-    z, dz = R.support(K, lo, hi)
-    m = R.project(p, r, d, gamma, z, dz, lo, hi)
+    z, dz = O.support(K, lo, hi)
+    m = O.project(p, r, d, gamma, z, dz, lo, hi)
     assert bool((m >= 0).all())
     torch.testing.assert_close(m.sum(1), torch.ones(N), rtol=0, atol=2e-6)
-    m64 = R.project_fp64_loop(p.double().numpy(), r.double().numpy(), d.numpy(), float(np.float32(gamma)), lo, hi)
+    m64 = O.project_fp64_loop(p.double().numpy(), r.double().numpy(), d.numpy(), float(np.float32(gamma)), lo, hi)
     assert np.allclose(m64.sum(1), 1.0, atol=1e-12)
     # b_j <= K - 1 carries fp32 rounding of a few ulp of 64 (about 4e-6 each), which moves that much mass between neighbours
     assert float(np.abs(m.double().numpy() - m64).max()) <= 1e-5
@@ -193,26 +187,26 @@ def test_projection_preserves_mass_and_equals_the_fp64_loop(K, lo, hi, gamma):
 
 @pytest.mark.parametrize('K,lo,hi', [(51, -10.0, 10.0), (11, 0.0, 200.0)])
 def test_projection_closed_forms(K, lo, hi):
-    z, dz = R.support(K, lo, hi)
+    z, dz = O.support(K, lo, hi)
     p = _dist(5, K, 3)
     # done (or gamma = 0): Tz = r for every j; a reward on atom i puts all the mass there
     i = K // 3
-    m = R.project(p, torch.full((5,), float(z[i])), torch.ones(5, dtype=torch.bool), 0.99, z, dz, lo, hi)
+    m = O.project(p, torch.full((5,), float(z[i])), torch.ones(5, dtype=torch.bool), 0.99, z, dz, lo, hi)
     want = torch.zeros(5, K)
     want[:, i] = 1.0
     torch.testing.assert_close(m, want, rtol=0, atol=2e-6)
-    torch.testing.assert_close(R.project(p, torch.full((5,), float(z[i])), torch.zeros(5, dtype=torch.bool), 0.0, z, dz, lo, hi), want,
+    torch.testing.assert_close(O.project(p, torch.full((5,), float(z[i])), torch.zeros(5, dtype=torch.bool), 0.0, z, dz, lo, hi), want,
                                rtol=0, atol=2e-6)
     # a reward a quarter of the way from atom i to atom i + 1 splits 3 : 1
     r = float(z[i]) + 0.25 * float(dz)
-    m = R.project(p, torch.full((5,), r), torch.ones(5, dtype=torch.bool), 0.99, z, dz, lo, hi)
+    m = O.project(p, torch.full((5,), r), torch.ones(5, dtype=torch.bool), 0.99, z, dz, lo, hi)
     torch.testing.assert_close(m[:, i], torch.full((5,), 0.75), rtol=0, atol=2e-5)
     torch.testing.assert_close(m[:, i + 1], torch.full((5,), 0.25), rtol=0, atol=2e-5)
     assert float(m.sum(1).sub(1).abs().max()) <= 2e-6
     # Tz beyond the support clamps to the end atoms
     big = 10 * (hi - lo)
     for r, k in ((big, K - 1), (-big, 0)):
-        m = R.project(p, torch.full((5,), r), torch.zeros(5, dtype=torch.bool), 0.5, z, dz, lo, hi)
+        m = O.project(p, torch.full((5,), r), torch.zeros(5, dtype=torch.bool), 0.5, z, dz, lo, hi)
         want = torch.zeros(5, K)
         want[:, k] = 1.0
         torch.testing.assert_close(m, want, rtol=0, atol=2e-6)
@@ -221,16 +215,12 @@ def test_projection_closed_forms(K, lo, hi):
 def test_kl_is_nonnegative_and_zero_at_m_equals_p():
     p = _dist(32, 51, 9)
     logp = p.log()
-    assert float(R.kl(p, logp).abs().max()) <= 1e-6
+    assert float(O.kl(p, logp).abs().max()) <= 1e-6
     m = _dist(32, 51, 10)
     m[:, :5] = 0                                   # 0 log 0 = 0
     m = m / m.sum(1, keepdim=True)
-    k = R.kl(m, F.log_softmax(torch.randn(32, 51, generator=torch.Generator().manual_seed(2)), dim=1))
+    k = O.kl(m, F.log_softmax(torch.randn(32, 51, generator=torch.Generator().manual_seed(2)), dim=1))
     assert bool(torch.isfinite(k).all()) and float(k.min()) >= 0.0
-
-
-def _frames(N, seed):
-    return torch.randint(0, 256, (N, 4, 84, 84), dtype=torch.uint8, generator=torch.Generator().manual_seed(seed))
 
 
 @pytest.mark.parametrize('double', [False, True])
@@ -239,10 +229,11 @@ def test_written_logit_gradient_is_autogradss(double):
     on, tg = default_q_state_dict(A, 0, num_atoms=K), default_q_state_dict(A, 1, num_atoms=K)
     g = torch.Generator().manual_seed(2)
     a, r, d, w = torch.randint(0, A, (B,), generator=g), 3 * torch.randn(B, generator=g), torch.rand(B, generator=g) < 0.3, torch.rand(B, generator=g) + 0.1
-    obs = _frames(B, 3)
-    out = R.learn_step(on, tg, obs, a, r, _frames(B, 4), d, K, lo, hi, weights=w, gamma=0.9, double_dqn=double)
+    obs = frames(B, 3)
+    out = O.learn_step(on, tg, obs, a, r, frames(B, 4), d, weights=w, gamma=0.9, double_dqn=double,
+                       head=O.Head('categorical', num_atoms=K, v_min=lo, v_max=hi))
     with torch.no_grad():
-        logits = R.CatRefQNet(A, K, on).logits(obs)
+        logits = O.RefQNet(A, on, O.Head('categorical', num_atoms=K, v_min=lo, v_max=hi))(obs)
         p = F.softmax(logits, dim=2)[torch.arange(B), a]
     want = torch.zeros(B, A * K)
     dl = (w / B)[:, None] * (p * out['m'].sum(1, keepdim=True) - out['m'])       # (w / B) (p_k sum m - m_k) on the taken action
@@ -258,10 +249,11 @@ def test_written_logit_gradient_is_autogradss(double):
 def test_initial_priorities_are_the_learners_kl():
     A, K, N, lo, hi = 4, 21, 5, 0.0, 200.0
     sd = default_q_state_dict(A, 2, num_atoms=K)
-    s, ns = _frames(N, 1), _frames(N, 2)
+    head = O.Head('categorical', num_atoms=K, v_min=lo, v_max=hi)
+    s, ns = frames(N, 1), frames(N, 2)
     a = torch.tensor([0, 1, 2, 3, 1])
     Rw = torch.tensor([0.5, -1.0, 2.0, 0.0, 0.25])
     d = torch.tensor([0, 1, 0, 0, 1], dtype=torch.bool)
-    p = R.initial_priorities(sd, s, a, Rw, ns, d, 0.5, 1e-3, K, lo, hi)
-    out = R.learn_step(sd, sd, s, a, Rw, ns, d, K, lo, hi, gamma=0.5)
+    p = O.initial_priorities(sd, s, a, Rw, ns, d, 0.5, 1e-3, head=head)
+    out = O.learn_step(sd, sd, s, a, Rw, ns, d, gamma=0.5, head=head)
     assert torch.equal(p, out['kl'].clamp(min=0).double() + 1e-3)

@@ -7,11 +7,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import apex_dueling_ref as D
+from oracle import apex_oracle as O
 from scalerl_b200 import _lib
 from scalerl_b200 import build as srl_build
 from scalerl_b200.algorithms.apex import (APEX_DUELING_PARAM_NAMES, APEX_PARAM_NAMES, ApexHParams, AtariQNet, B200ApexActor,
                                           B200ApexLearner, apex_param_shapes, default_q_state_dict)
+from tests.apex_cases import frames, unbuilt
+
+DUELING = O.Head('dueling')
 
 
 @pytest.fixture(scope='module')
@@ -67,7 +70,7 @@ def test_dueling_forward_is_the_formula(A):
     if A == 1:                                  # one action: Q = V
         assert torch.allclose(got, v, rtol=1e-6, atol=1e-6)
     # the oracle's network computes the same Q from the same state dict
-    ref = D.DuelingRefQNet(A, net.state_dict())
+    ref = O.RefQNet(A, net.state_dict(), DUELING)
     assert torch.equal(ref(obs), net(obs))
 
 
@@ -117,36 +120,25 @@ def test_dueling_c_argument_errors(lib):
     assert b'dueling=2' in lib.srl_last_error()
 
 
-def _unbuilt(cls, **attrs):
-    o = cls.__new__(cls)
-    for k, v in attrs.items():
-        setattr(o, k, v)
-    return o
-
-
 @pytest.mark.parametrize('learner_dueling', [False, True])
 def test_sync_from_needs_the_same_head(learner_dueling):
-    L = _unbuilt(B200ApexLearner, hp=ApexHParams(num_actions=6, dueling_dqn=learner_dueling), device=torch.device('cuda', 0))
-    X = _unbuilt(B200ApexActor, num_envs=4, num_actions=6, dueling_dqn=not learner_dueling, device=torch.device('cuda', 0), _h=None)
+    L = unbuilt(B200ApexLearner, hp=ApexHParams(num_actions=6, dueling_dqn=learner_dueling), device=torch.device('cuda', 0))
+    X = unbuilt(B200ApexActor, num_envs=4, num_actions=6, dueling_dqn=not learner_dueling, device=torch.device('cuda', 0), _h=None)
     with pytest.raises(ValueError, match='dueling_dqn'):
         X.sync_from(L)
-
-
-def _frames(N, seed):
-    return torch.randint(0, 256, (N, 4, 84, 84), dtype=torch.uint8, generator=torch.Generator().manual_seed(seed))
 
 
 def _case(A, B, seed=0):
     on, tg = default_q_state_dict(A, seed, dueling=True), default_q_state_dict(A, seed + 1, dueling=True)
     g = torch.Generator().manual_seed(seed + 2)
-    return on, tg, (_frames(B, seed + 3), torch.randint(0, A, (B,), generator=g), torch.randn(B, generator=g), _frames(B, seed + 4),
+    return on, tg, (frames(B, seed + 3), torch.randint(0, A, (B,), generator=g), torch.randn(B, generator=g), frames(B, seed + 4),
                     torch.rand(B, generator=g) < 0.3), torch.rand(B, generator=g) + 0.1
 
 
 @pytest.mark.parametrize('A', [1, 6])
 def test_oracle_advantage_gradients_sum_to_zero(A):
     on, tg, batch, w = _case(A, 8)
-    out = D.learn_step(on, tg, *batch, weights=w, double_dqn=True)
+    out = O.learn_step(on, tg, *batch, weights=w, double_dqn=True, head=DUELING)
     gW, gb = out['grads']['advantage.weight'], out['grads']['advantage.bias']
     assert tuple(out['grads']) == APEX_DUELING_PARAM_NAMES
     if A == 1:                                  # Adv - mean(Adv) is 0 for one action: no gradient reaches the advantage stream
@@ -167,7 +159,7 @@ def test_oracle_targets_use_the_dueling_q(double):
     tg['advantage.bias'][1] += 1.0              # the target network prefers action 1, the online network does not
 
     def q_rows(sd, x):                          # the formula, on the oracle's own features
-        net = D.DuelingRefQNet(A, sd)
+        net = O.RefQNet(A, sd, DUELING)
         with torch.no_grad():
             h = net.features(x)
             v = h @ sd['value.weight'].T + sd['value.bias']
@@ -178,7 +170,7 @@ def test_oracle_targets_use_the_dueling_q(double):
     astar = (qn_o if double else qn_t).argmax(1)
     want_y = r + (1 - d.float()) * gamma * qn_t.gather(1, astar[:, None]).squeeze(1)
     want_q = q_rows(on, obs).gather(1, a[:, None]).squeeze(1)
-    out = D.learn_step(on, tg, obs, a, r, nobs, d, weights=w, gamma=gamma, double_dqn=double)
+    out = O.learn_step(on, tg, obs, a, r, nobs, d, weights=w, gamma=gamma, double_dqn=double, head=DUELING)
     torch.testing.assert_close(out['y'], want_y, rtol=1e-6, atol=1e-6)
     torch.testing.assert_close(out['q'], want_q, rtol=1e-6, atol=1e-6)
     # the two rules pick different actions somewhere, so the test tells them apart
@@ -188,13 +180,13 @@ def test_oracle_targets_use_the_dueling_q(double):
 def test_initial_priorities_on_the_dueling_net():
     A, N = 4, 5
     sd = default_q_state_dict(A, 2, dueling=True)
-    s, ns = _frames(N, 1), _frames(N, 2)
+    s, ns = frames(N, 1), frames(N, 2)
     a = torch.tensor([0, 1, 2, 3, 1])
     R = torch.tensor([0.5, -1.0, 2.0, 0.0, 0.25])
     d = torch.tensor([0, 1, 0, 0, 1], dtype=torch.bool)
-    net = D.DuelingRefQNet(A, sd)
+    net = O.RefQNet(A, sd, DUELING)
     with torch.no_grad():
         q = net(s)[torch.arange(N), a]
         y = R + (1 - d.float()) * 0.5 * net(ns).max(1)[0]
-    p = D.initial_priorities(sd, s, a, R, ns, d, 0.5, 1e-3)
+    p = O.initial_priorities(sd, s, a, R, ns, d, 0.5, 1e-3, head=DUELING)
     assert torch.equal(p, (q - y).abs().double() + 1e-3)

@@ -9,12 +9,13 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import apex_noisy_ref as NR
+from oracle import apex_oracle as O
 from scalerl_b200 import _lib
 from scalerl_b200 import build as srl_build
 from scalerl_b200.algorithms.apex import (APEX_NOISY_DUELING_PARAM_NAMES, APEX_NOISY_PARAM_NAMES, APEX_PARAM_NAMES, ApexHParams, AtariQNet,
                                           B200ApexActor, B200ApexLearner, NoisyLinear, apex_param_shapes, default_q_state_dict)
 from scalerl_b200.algorithms.apex.learner import QHead, scale_noise
+from tests.apex_cases import frames, unbuilt
 
 HEADS = {'plain': dict(), 'dueling': dict(dueling=True), 'categorical': dict(categorical=True, num_atoms=5)}
 
@@ -211,25 +212,14 @@ def test_noisy_c_argument_errors(lib):
     assert b'noisy=2' in lib.srl_last_error()
 
 
-def _unbuilt(cls, **attrs):
-    o = cls.__new__(cls)
-    for k, v in attrs.items():
-        setattr(o, k, v)
-    return o
-
-
 @pytest.mark.parametrize('learner,actor', [(dict(noisy_dqn=True), dict(noisy_dqn=False)), (dict(noisy_dqn=False), dict(noisy_dqn=True)),
                                            (dict(noisy_dqn=True), dict(noisy_dqn=True, dueling_dqn=True)),
                                            (dict(noisy_dqn=True, categorical_dqn=True), dict(noisy_dqn=True))])
 def test_sync_from_needs_the_same_noisy_head(learner, actor):
-    L = _unbuilt(B200ApexLearner, hp=ApexHParams(num_actions=6, **learner), device=torch.device('cuda', 0))
-    X = _unbuilt(B200ApexActor, num_envs=4, num_actions=6, device=torch.device('cuda', 0), _h=None, **actor)
+    L = unbuilt(B200ApexLearner, hp=ApexHParams(num_actions=6, **learner), device=torch.device('cuda', 0))
+    X = unbuilt(B200ApexActor, num_envs=4, num_actions=6, device=torch.device('cuda', 0), _h=None, **actor)
     with pytest.raises(ValueError, match='noisy_dqn'):
         X.sync_from(L)
-
-
-def _frames(N, seed):
-    return torch.randint(0, 256, (N, 4, 84, 84), dtype=torch.uint8, generator=torch.Generator().manual_seed(seed))
 
 
 @pytest.mark.parametrize('head', list(HEADS))
@@ -243,18 +233,19 @@ def test_oracle_sigma_gradient_is_dW_times_eps(head):
     g = torch.Generator().manual_seed(2)
     nn_ = 3648 + 512 * (1 + dueling) + R
     n_on, n_tg = scale_noise(torch.randn(nn_, generator=g)), scale_noise(torch.randn(nn_, generator=g))
-    batch = (_frames(B, 3), torch.randint(0, A, (B,), generator=g), torch.randn(B, generator=g), _frames(B, 4), torch.rand(B, generator=g) < 0.3)
-    out = NR.learn_step(on, tg, n_on, n_tg, *batch, dueling=dueling, num_atoms=K, v_min=-10.0, v_max=10.0, double_dqn=True)
-    assert tuple(out['grads']) == NR.names(dueling)
+    batch = (frames(B, 3), torch.randint(0, A, (B,), generator=g), torch.randn(B, generator=g), frames(B, 4), torch.rand(B, generator=g) < 0.3)
+    oh = O.Head('dueling' if dueling else 'categorical' if K else 'plain', noisy=True, num_atoms=K, v_min=-10.0, v_max=10.0)
+    out = O.learn_step(on, tg, *batch, double_dqn=True, head=oh, noise_online=n_on, noise_target=n_tg)
+    assert tuple(out['grads']) == O.names(dueling)
     # the gradient of the composed weight W is the mu gradient; sigma's is dW * eps (autograd's own rounding: bit for bit)
-    for name, (ei, eo) in NR.split_noise(n_on, A, dueling, K).items():
+    for name, (ei, eo) in O.split_noise(n_on, A, dueling, K).items():
         gW, gb = out['grads'][f'{name}.weight_mu'], out['grads'][f'{name}.bias_mu']
         assert torch.equal(out['grads'][f'{name}.weight_sigma'], gW * torch.outer(eo, ei)), name
         assert torch.equal(out['grads'][f'{name}.bias_sigma'], gb * eo), name
         assert float(gW.abs().max()) > 0 or (name == 'advantage' and A == 1)
     # the oracle's composed weights are composed() in torch's order
-    net = NR.NoisyRefQNet(A, dueling, K, on, NR.split_noise(n_on, A, dueling, K))
-    for name, (W, b) in NR.composed(on, n_on, A, dueling, K).items():
+    net = O.RefQNet(A, on, oh, n_on)
+    for name, (W, b) in O.composed(on, n_on, A, dueling, K).items():
         w2, b2 = getattr(net, name).weights()
         assert torch.equal(W, w2) and torch.equal(b, b2)
 

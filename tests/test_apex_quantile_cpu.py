@@ -12,12 +12,13 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests import apex_quantile_ref as R
+from oracle import apex_oracle as O
 from scalerl_b200 import _lib
 from scalerl_b200 import build as srl_build
 from scalerl_b200.algorithms.apex import (APEX_NOISY_PARAM_NAMES, APEX_PARAM_NAMES, ApexHParams, AtariQNet, B200ApexActor, B200ApexLearner,
                                           apex_param_shapes, default_q_state_dict, quantile_taus)
 from scalerl_b200.algorithms.apex.learner import QHead
+from tests.apex_cases import frames, unbuilt
 
 
 @pytest.fixture(scope='module')
@@ -71,7 +72,7 @@ def test_quantile_net_names_shapes_and_flat_layout(A, N, noisy, lib):
     assert {n: tuple(p.shape) for n, p in net.named_parameters()} == dict(shapes)
     w = 'q.weight_mu' if noisy else 'q.weight'
     assert shapes[w] == (A * N, 512)
-    assert torch.equal(net.taus, quantile_taus(N)) and torch.equal(net.taus, R.taus(N))
+    assert torch.equal(net.taus, quantile_taus(N)) and torch.equal(net.taus, O.taus(N))
     sd = default_q_state_dict(A, 3, noisy=noisy, num_quantiles=N)
     assert tuple(sd) == names and tuple(sd[w].shape) == (A * N, 512)
     # the encoder's initial weights are the plain network's (the head is drawn last)
@@ -114,7 +115,7 @@ def test_quantile_forward_is_the_formula(A, N):
     assert float((got_t - theta).abs().max()) <= 1e-5 * max(1.0, float(theta.abs().max()))
     assert float((got_q - want_q).abs().max()) <= 1e-5 * max(1.0, float(theta.abs().max()))
     # the oracle's network computes the same quantiles from the same state dict
-    assert torch.equal(R.QrRefQNet(A, N, net.state_dict()).theta(obs), net.quantiles(obs))
+    assert torch.equal(O.RefQNet(A, net.state_dict(), O.Head('quantile', num_quantiles=N))(obs), net.quantiles(obs))
     with pytest.raises(ValueError, match='quantile'):
         AtariQNet(A).quantiles(obs)
 
@@ -171,34 +172,23 @@ def test_quantile_c_argument_errors(lib):
     assert b'NULL' in lib.srl_last_error()
 
 
-def _unbuilt(cls, **attrs):
-    o = cls.__new__(cls)
-    for k, v in attrs.items():
-        setattr(o, k, v)
-    return o
-
-
 @pytest.mark.parametrize('learner,msg', [(dict(quantile_dqn=False), 'quantile_dqn'), (dict(num_quantiles=51), 'num_quantiles'),
                                          (dict(quantile_kappa=0.5), 'quantile_kappa'), (dict(noisy_dqn=True), 'noisy_dqn')])
 def test_sync_from_needs_the_same_head(learner, msg):
     hp = dict(num_actions=6, quantile_dqn=True, num_quantiles=200, quantile_kappa=1.0)
     hp.update(learner)
-    L = _unbuilt(B200ApexLearner, hp=ApexHParams(**hp), device=torch.device('cuda', 0))
-    X = _unbuilt(B200ApexActor, num_envs=4, num_actions=6, quantile_dqn=True, num_quantiles=200, quantile_kappa=1.0,
+    L = unbuilt(B200ApexLearner, hp=ApexHParams(**hp), device=torch.device('cuda', 0))
+    X = unbuilt(B200ApexActor, num_envs=4, num_actions=6, quantile_dqn=True, num_quantiles=200, quantile_kappa=1.0,
                  device=torch.device('cuda', 0), _h=None)
     with pytest.raises(ValueError, match=msg):
         X.sync_from(L)
     # and the other way round: a quantile learner, a plain actor
-    X = _unbuilt(B200ApexActor, num_envs=4, num_actions=6, device=torch.device('cuda', 0), _h=None)
+    X = unbuilt(B200ApexActor, num_envs=4, num_actions=6, device=torch.device('cuda', 0), _h=None)
     with pytest.raises(ValueError, match='quantile_dqn'):
-        X.sync_from(_unbuilt(B200ApexLearner, hp=ApexHParams(num_actions=6, quantile_dqn=True), device=torch.device('cuda', 0)))
+        X.sync_from(unbuilt(B200ApexLearner, hp=ApexHParams(num_actions=6, quantile_dqn=True), device=torch.device('cuda', 0)))
 
 
 # ---------------------------------------------------------------------------------------------------------------- the oracle
-def _frames(N, seed):
-    return torch.randint(0, 256, (N, 4, 84, 84), dtype=torch.uint8, generator=torch.Generator().manual_seed(seed))
-
-
 @pytest.mark.parametrize('kappa', [1.0, 0.5])
 @pytest.mark.parametrize('double', [False, True])
 def test_written_dtheta_is_fp64_autograd(double, kappa):
@@ -206,12 +196,12 @@ def test_written_dtheta_is_fp64_autograd(double, kappa):
     on, tg = default_q_state_dict(A, 0, num_quantiles=N), default_q_state_dict(A, 1, num_quantiles=N)
     g = torch.Generator().manual_seed(2)
     a, r, d, w = torch.randint(0, A, (B,), generator=g), torch.randn(B, generator=g), torch.rand(B, generator=g) < 0.3, torch.rand(B, generator=g) + 0.1
-    obs = _frames(B, 3)
-    out = R.learn_step(on, tg, obs, a, r, _frames(B, 4), d, N, kappa, weights=w, gamma=0.9, double_dqn=double)
+    obs = frames(B, 3)
+    out = O.learn_step(on, tg, obs, a, r, frames(B, 4), d, weights=w, gamma=0.9, double_dqn=double, head=O.Head('quantile', num_quantiles=N, kappa=kappa))
     # fp64 autograd of mean(w loss) with respect to theta, from the oracle's own theta and targets
     theta = out['theta'].double().requires_grad_(True)
     ta = theta[torch.arange(B), a]
-    loss = (w.double() * R.quantile_loss(ta, out['T'].double(), kappa)).mean()
+    loss = (w.double() * O.quantile_loss(ta, out['T'].double(), kappa)).mean()
     loss.backward()
     want = theta.grad.reshape(B, A * N)
     torch.testing.assert_close(out['dtheta'].double(), want, rtol=1e-5, atol=1e-9)
@@ -231,25 +221,25 @@ def test_quantile_loss_closed_forms(kappa):
     g = torch.Generator().manual_seed(4)
     N = 17
     th, T = 2 * torch.randn(32, N, generator=g, dtype=torch.float64), 2 * torch.randn(32, N, generator=g, dtype=torch.float64)
-    assert bool((R.quantile_loss(th, T, kappa) >= 0).all())
+    assert bool((O.quantile_loss(th, T, kappa) >= 0).all())
     # every theta_i equal to every T_j: u = 0 everywhere, no loss and no gradient
     c = torch.randn(32, 1, generator=g, dtype=torch.float64).expand(32, N)
-    assert float(R.quantile_loss(c, c, kappa).abs().max()) == 0.0
-    assert float(R.dtheta_written(c, c, kappa, torch.ones(32, dtype=torch.float64)).abs().max()) == 0.0
+    assert float(O.quantile_loss(c, c, kappa).abs().max()) == 0.0
+    assert float(O.dtheta_written(c, c, kappa, torch.ones(32, dtype=torch.float64)).abs().max()) == 0.0
     # inside |u| <= kappa: rho = |tau - 1{u < 0}| u^2 / (2 kappa)
     small = th[:, :1] + (kappa / 3) * torch.rand(32, N, generator=g, dtype=torch.float64)
     u = small[:, None, :] - th[:, :1, None].expand(32, N, 1)
-    tau = R.taus(N, torch.float64)[None, :, None]
-    rho = R.rho(th[:, :1].expand(32, N), small, kappa)
+    tau = O.taus(N, torch.float64)[None, :, None]
+    rho = O.rho(th[:, :1].expand(32, N), small, kappa)
     assert bool((u.abs() <= kappa).all())
     torch.testing.assert_close(rho, (tau - (u < 0).double()).abs() * u * u / (2 * kappa), rtol=1e-12, atol=0)
     # outside: rho = |tau - 1{u < 0}| (|u| - kappa / 2)
     far = th[:, :1] + 3 * kappa + torch.rand(32, N, generator=g, dtype=torch.float64)
-    rho = R.rho(th[:, :1].expand(32, N), far, kappa)
+    rho = O.rho(th[:, :1].expand(32, N), far, kappa)
     uf = far[:, None, :] - th[:, :1, None].expand(32, N, 1)
     torch.testing.assert_close(rho, tau * (uf.abs() - kappa / 2), rtol=1e-12, atol=1e-12)
     # tau_i is the midpoint of the i-th of N equal probability bins
-    assert torch.equal(R.taus(4), torch.tensor([0.125, 0.375, 0.625, 0.875]))
+    assert torch.equal(O.taus(4), torch.tensor([0.125, 0.375, 0.625, 0.875]))
 
 
 def test_done_target_is_the_reward_whatever_s_prime_holds():
@@ -258,7 +248,7 @@ def test_done_target_is_the_reward_whatever_s_prime_holds():
     bad[1, 2, 3] = math.nan
     r = torch.arange(n, dtype=torch.float32) - 2.5
     done = torch.ones(n, dtype=torch.bool)
-    T = R.targets(bad, r, done, 0.99, theta_next_online=bad)
+    T = O.targets(bad, r, done, 0.99, theta_next_online=bad)
     assert torch.equal(T, r[:, None].expand(n, N))
     # not done: r + gamma theta'(s')[a*], a* the first argmax of the quantile means (ties: the first index)
     g = torch.Generator().manual_seed(1)
@@ -266,19 +256,20 @@ def test_done_target_is_the_reward_whatever_s_prime_holds():
     tn[:, 2] = tn[:, 0]
     tn[:, 0] += 5.0
     tn[:, 2] += 5.0
-    T = R.targets(tn, r, torch.zeros(n, dtype=torch.bool), 0.99)
+    T = O.targets(tn, r, torch.zeros(n, dtype=torch.bool), 0.99)
     torch.testing.assert_close(T, r[:, None] + torch.tensor(np.float32(0.99)) * tn[:, 0], rtol=0, atol=0)
 
 
 def test_initial_priorities_are_the_learners_loss():
     A, N, n = 4, 21, 5
     sd = default_q_state_dict(A, 2, num_quantiles=N)
-    s, ns = _frames(n, 1), _frames(n, 2)
+    head = O.Head('quantile', num_quantiles=N, kappa=0.5)
+    s, ns = frames(n, 1), frames(n, 2)
     a = torch.tensor([0, 1, 2, 3, 1])
     Rw = torch.tensor([0.5, -1.0, 2.0, 0.0, 0.25])
     d = torch.tensor([0, 1, 0, 0, 1], dtype=torch.bool)
-    p = R.initial_priorities(sd, s, a, Rw, ns, d, 0.5, 1e-3, N, 0.5)
-    out = R.learn_step(sd, sd, s, a, Rw, ns, d, N, 0.5, gamma=0.5)
+    p = O.initial_priorities(sd, s, a, Rw, ns, d, 0.5, 1e-3, head=head)
+    out = O.learn_step(sd, sd, s, a, Rw, ns, d, gamma=0.5, head=head)
     assert torch.equal(p, out['loss_n'].double() + 1e-3)
 
 

@@ -1,48 +1,31 @@
-"""The Ape-X actor on the H100 (B200ApexActor / srl_apex_actor_*, srl_replay_add_prioritized):
+"""The Ape-X actor on the H100 (B200ApexActor / srl_apex_actor_*, srl_replay_add_prioritized); 1 and 5 are the checks every head
+shares (tests/apex_cases.py), here with the plain head:
   1. after sync_from(learner) the actor's Q values equal the learner's bit for bit; with every epsilon 0, act is their first argmax;
   2. epsilon = 1 gives uniform actions, and the apex_epsilons schedule gives each env group its non-greedy rate eps (A - 1) / A;
   3. seeded, eager and captured acting draw the same sequence; each replay draws anew and follows set_epsilons;
-  4. fp32-accurate actor: the inserted leaves against compute_prior's p^alpha (tests/apex_actor_ref.py), the trees against PerOracle, the ring against the plain add;
+  4. fp32-accurate actor: the inserted leaves against compute_prior's p^alpha (oracle/apex_oracle.initial_priorities), the trees against
+     PerOracle, the ring against the plain add;
   5. bf16 actor and learner on the same weights: the actor's priorities are the learner's, bit for bit;
   6. a NaN in the snapshot gives finite trees, leaves at max_priority^alpha and E invalid updates;
   7. a 200-step act -> env -> prioritized add -> learn_from loop stays finite and two seeded runs are bit-identical.
 The measured errors are written to $SRL_RESULTS_DIR/apex_actor.json when SRL_RESULTS_DIR is set."""
-import json
 import math
-import os
 
 import numpy as np
 import pytest
 import torch
 
-from tests import apex_actor_ref as AR
+from oracle import apex_oracle as O
 from oracle import replay_oracle as RO
 from oracle.per_oracle import PerOracle
 from scalerl_b200.algorithms.apex import ApexHParams, B200ApexActor, B200ApexLearner, apex_epsilons, default_q_state_dict
 from scalerl_b200.data.replay_memory import GpuPrioritizedReplayBuffer
+from tests import apex_cases as cases
+from tests.apex_cases import frames, nmax, record
 
 pytestmark = pytest.mark.gpu
 NPIX = 4 * 84 * 84
-
-
-def _record(name, obj):
-    d = os.environ.get('SRL_RESULTS_DIR')
-    if not d:
-        return
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, 'apex_actor.json')
-    cur = json.load(open(p)) if os.path.exists(p) else {}
-    cur[name] = obj
-    json.dump(cur, open(p, 'w'), indent=1)
-
-
-def frames(n, seed):
-    return torch.randint(0, 256, (n, 4, 84, 84), dtype=torch.uint8, generator=torch.Generator().manual_seed(seed)).cuda()
-
-
-def nmax(a, b):
-    a, b = torch.as_tensor(a).double().cpu(), torch.as_tensor(b).double().cpu()
-    return float((a - b).abs().max() / max(float(b.abs().max()), 1e-300))
+PLAIN = cases.HEADS['plain']
 
 
 def _dominant(sd, a, by=50.0):
@@ -55,36 +38,20 @@ def _dominant(sd, a, by=50.0):
 # ---------------------------------------------------------------------------------------------------------------- 1
 @pytest.mark.parametrize('E', [1, 13, 256, 1500])
 def test_q_values_equal_the_learners_and_greedy_act(E):
-    A = 6
-    L = B200ApexLearner(ApexHParams(batch_size=32, num_actions=A), seed=3)
-    X = B200ApexActor(E, A, epsilons=np.zeros(E), seed=1)
-    X.sync_from(L)
-    assert X.weights_version == 1
-    obs = frames(E, E)
-    q = X.q_values(obs)
-    assert torch.equal(q, L.q_values(obs))
-    assert torch.equal(X.act(obs), torch.argmax(q, dim=1))
-    # ties: actions 1 and 4 have the same head row and the largest bias: the first index wins, as in torch.argmax
-    sd = L.state_dict()
-    sd['q.weight'][4] = sd['q.weight'][1]
-    sd['q.bias'][1] = sd['q.bias'][4] = 30.0
-    X.load_state_dict(sd)
-    q = X.q_values(obs)
-    assert torch.equal(q[:, 1], q[:, 4]) and bool((torch.argmax(q, dim=1) == 1).all())
-    assert bool((X.act(obs) == 1).all())
+    cases.check_actor_q_values_and_greedy_act(PLAIN, E)
 
 
 # ---------------------------------------------------------------------------------------------------------------- 2
 def test_epsilon_one_is_uniform():
     E, A, T = 1500, 6, 20
     X = B200ApexActor(E, A, epsilons=np.ones(E), seed=7)
-    obs = frames(E, 2)
+    obs = frames(E, 2, 'cuda')
     counts = torch.zeros(A, dtype=torch.int64)
     for _ in range(T):
         counts += torch.bincount(X.act(obs).cpu(), minlength=A)
     n, p = E * T, 1.0 / A
     sigma = math.sqrt(n * p * (1 - p))
-    _record('uniform_counts', counts.tolist())
+    record('apex_actor.json', 'uniform_counts', counts.tolist())
     assert counts.sum() == n and float((counts - n * p).abs().max()) <= 5 * sigma, counts
 
 
@@ -92,7 +59,7 @@ def test_apex_schedule_rates():
     E, A, T, groups = 256, 6, 300, 8
     eps = apex_epsilons(E)
     X = B200ApexActor(E, A, seed=11, init_state_dict=_dominant(default_q_state_dict(A, 0), 2))
-    obs = frames(E, 3)
+    obs = frames(E, 3, 'cuda')
     assert bool((torch.argmax(X.q_values(obs), 1) == 2).all())
     off = torch.zeros(E, dtype=torch.int64)
     for _ in range(T):
@@ -102,14 +69,14 @@ def test_apex_schedule_rates():
     for g in np.array_split(np.arange(E), groups):
         want, sigma = T * p[g].sum(), math.sqrt(T * (p[g] * (1 - p[g])).sum())
         dev.append((float(off[g].sum()) - want) / sigma)
-    _record('schedule_group_deviation_sigma', dev)
+    record('apex_actor.json', 'schedule_group_deviation_sigma', dev)
     assert max(abs(d) for d in dev) <= 5, dev
 
 
 # ---------------------------------------------------------------------------------------------------------------- 3
 def test_seeded_eager_and_captured_acting():
     E, A = 256, 6
-    obs = frames(E, 4)
+    obs = frames(E, 4, 'cuda')
     a1, a2 = B200ApexActor(E, A, epsilons=np.full(E, 0.5), seed=5), B200ApexActor(E, A, epsilons=np.full(E, 0.5), seed=5)
     eager = [a1.act(obs) for _ in range(6)]
     assert all(torch.equal(x, a2.act(obs)) for x in eager[:1])          # same seed, same draw
@@ -160,7 +127,7 @@ def test_fp32_actor_against_oracle(M, E, n, steps, alpha):
         rows = [ro.slots[i] for i in slots]
         s = torch.from_numpy(np.stack([st[r[0]] for r in rows]))
         ns = torch.from_numpy(np.stack([nst[r[3]] for r in rows]))
-        want = AR.initial_priorities(sd, s, torch.tensor([r[1] for r in rows]), torch.tensor([r[2] for r in rows]), ns,
+        want = O.initial_priorities(sd, s, torch.tensor([r[1] for r in rows]), torch.tensor([r[2] for r in rows]), ns,
                                     torch.tensor([bool(r[4]) for r in rows]), float(np.float32(gamma ** n)), 1e-6)
         sum_t, min_t, mp = mem.sampler.trees()
         cap = mem.sampler.capacity
@@ -177,7 +144,7 @@ def test_fp32_actor_against_oracle(M, E, n, steps, alpha):
         assert mp == po.max_priority if alpha == 1.0 else mp == pytest.approx(po.max_priority, rel=1e-5)
         assert len(mem) == po.size
     assert mem.sampler._L.srl_per_invalid_updates(mem.sampler._h, mem.sampler._stream()) == 0
-    _record(f'fp32_split_M{M}_E{E}_n{n}_alpha{alpha}', {'leaf_nmax': worst})
+    record('apex_actor.json', f'fp32_split_M{M}_E{E}_n{n}_alpha{alpha}', {'leaf_nmax': worst})
     assert worst <= 1e-5, worst
     idx = torch.arange(M)
     for x, y in zip(mem.gather(idx), plain.gather(idx)):
@@ -186,30 +153,7 @@ def test_fp32_actor_against_oracle(M, E, n, steps, alpha):
 
 # ---------------------------------------------------------------------------------------------------------------- 5
 def test_bf16_priorities_are_the_learners():
-    E, A, n, gamma = 32, 6, 3, 0.99
-    L = B200ApexLearner(ApexHParams(batch_size=E, num_actions=A, gamma=gamma ** n, double_dqn=False, priority_eps=1e-6), seed=2)
-    X = B200ApexActor(E, A, priority_eps=1e-6)
-    X.sync_from(L)
-    mem = GpuPrioritizedReplayBuffer(256, E, alpha=1.0, n_step=n, gamma=gamma)     # alpha = 1: the leaves are the priorities
-    g = torch.Generator().manual_seed(6)
-    compared = 0
-    for t in range(5):
-        args = (torch.randint(0, 256, (E, 4, 84, 84), dtype=torch.uint8, generator=g).cuda(), torch.randint(0, A, (E,), generator=g).cuda(),
-                torch.randn(E, generator=g).cuda(), torch.randint(0, 256, (E, 4, 84, 84), dtype=torch.uint8, generator=g).cuda(),
-                (torch.rand(E, generator=g) < 0.3).cuda())
-        ptr = (t - n + 1) * E % 256
-        mem.save_to_memory(*args, is_vectorised=True, priorities_from=X)
-        if t + 1 < n:
-            continue
-        idxs = (torch.arange(E) + ptr) % 256
-        cap = mem.sampler.capacity
-        leaves = mem.sampler.trees()[0][cap + idxs.cuda()]
-        L.learn(mem.gather(idxs), use_graph=False)
-        assert torch.equal(L.debug_buffer('priorities'), leaves), t
-        X.sync_from(L)                  # the next add's weights are the learner's after this step (target == online until refreshed)
-        L.update_target(1.0)
-        compared += 1
-    assert compared == 3
+    cases.check_bf16_actor_priorities(PLAIN)
 
 
 # ---------------------------------------------------------------------------------------------------------------- 6
@@ -217,7 +161,7 @@ def test_nan_snapshot_keeps_the_trees_finite():
     E, A, alpha = 8, 6, 0.6
     X = B200ApexActor(E, A)
     mem = GpuPrioritizedReplayBuffer(32, E, alpha=alpha)
-    obs = frames(E, 9)
+    obs = frames(E, 9, 'cuda')
     z = torch.zeros(E, device='cuda')
     mem.save_to_memory(obs, torch.zeros(E, dtype=torch.int64, device='cuda'), z, obs, z.bool(), is_vectorised=True, priorities_from=X)
     before = mem.sampler._L.srl_per_invalid_updates(mem.sampler._h, mem.sampler._stream())
@@ -257,7 +201,7 @@ class ToyVecEnv:
         return next_obs, reward, done, self.obs()
 
 
-def _loop(seed, steps=200):
+def _env_loop(seed, steps=200):
     torch.manual_seed(seed)
     E, A, n = 16, 4, 3
     L = B200ApexLearner(ApexHParams(batch_size=32, num_actions=A, gamma=0.99 ** n, target_update_frequency=20), seed=seed)
@@ -280,11 +224,11 @@ def _loop(seed, steps=200):
 
 
 def test_one_gpu_apex_loop_is_finite_and_deterministic():
-    L1, m1, l1 = _loop(21)
-    L2, m2, l2 = _loop(21)
+    L1, m1, l1 = _env_loop(21)
+    L2, m2, l2 = _env_loop(21)
     assert len(l1) > 150 and len(L1._graphs) == 1 and all(math.isfinite(x) for x in l1)
     assert bool(torch.isfinite(L1.flat_params).all()) and bool(torch.isfinite(m1.sampler.trees()[0]).all())
     assert l1 == l2 and torch.equal(L1.flat_params, L2.flat_params)
     assert torch.equal(m1.sampler.trees()[0], m2.sampler.trees()[0]) and torch.equal(m1.sampler.trees()[1], m2.sampler.trees()[1])
     assert m1.sampler._L.srl_per_invalid_updates(m1.sampler._h, m1.sampler._stream()) == 0
-    _record('loop_200', {'updates': len(l1), 'first_loss': l1[0], 'last_loss': l1[-1]})
+    record('apex_actor.json', 'loop_200', {'updates': len(l1), 'first_loss': l1[0], 'last_loss': l1[-1]})
