@@ -27,7 +27,7 @@ int srl_version(void);
 /* ---- V-trace -------------------------------------------------------------------------------------------
  * replaces vtrace.from_importance_weights (scalerl/algorithms/impala/vtrace.py:78-172).
  * log_rhos, discounts, rewards, values: f32 [T,B] row-major; bootstrap_value f32 [B]; outputs f32 [T,B].
- * clip thresholds < 0 mean None (no clipping), as the Python API's clip_*=None.
+ * clip thresholds < 0 mean None (no clipping), as the Python API's clip_*=None; a NaN threshold is refused (SRL_EINVAL).
  * variant: 0 = column-sequential (float4 over B when B%4==0), 1 = warp-shuffle affine scan over T. */
 int srl_vtrace_from_importance_weights(const float* log_rhos, const float* discounts, const float* rewards,
                                        const float* values, const float* bootstrap_value, int T, int B,
@@ -92,7 +92,7 @@ typedef struct srl_config {
                               * hi*hi + hi*lo + lo*hi into the fp32 accumulator (16 significant operand bits, tighter than
                               * kind::tf32's 11) -- the whole-step parity mode SURVEY.md §7.9 asks for; ~3x the MMAs */
   float discounting, baseline_cost, entropy_cost;
-  float clip_rho_threshold, clip_pg_rho_threshold;   /* < 0: None */
+  float clip_rho_threshold, clip_pg_rho_threshold;   /* < 0: None; NaN: refused */
   float max_grad_norm;       /* clip_grad_norm_ threshold (rl_args.py:108)       */
   float learning_rate, alpha, epsilon;               /* RMSprop (rl_args.py:112-117) */
   float adam_beta1, adam_beta2, adam_eps;

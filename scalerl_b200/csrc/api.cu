@@ -20,6 +20,7 @@ extern "C" int srl_vtrace_from_importance_weights(const float* log_rhos, const f
                                                   const float* values, const float* bootstrap_value, int T, int B,
                                                   float clip_rho, float clip_pg, float* vs, float* pg, int variant, void* stream) {
   REQ(T >= 0 && B >= 0, "vtrace: negative shape T=%d B=%d", T, B);
+  REQ(!std::isnan(clip_rho) && !std::isnan(clip_pg), "vtrace: a clip threshold is NaN (< 0 means None)");
   if (T == 0 || B == 0) return 0;
   REQ(log_rhos && discounts && rewards && values && bootstrap_value && vs && pg, "vtrace: NULL pointer");
   CU(launch_vtrace_iw(log_rhos, discounts, rewards, values, bootstrap_value, T, B, clip_rho, clip_pg, vs, pg, variant,
@@ -32,6 +33,7 @@ extern "C" int srl_vtrace_from_logits(const float* bl, const float* tl, const in
                                       float clip_rho, float clip_pg, float* vs, float* pg, float* log_rhos, float* balp, float* talp,
                                       void* stream) {
   REQ(T >= 0 && B >= 0 && A >= 1, "vtrace_from_logits: bad shape T=%d B=%d A=%d", T, B, A);
+  REQ(!std::isnan(clip_rho) && !std::isnan(clip_pg), "vtrace_from_logits: a clip threshold is NaN (< 0 means None)");
   if (T == 0 || B == 0) return 0;
   REQ(bl && tl && actions && discounts && rewards && values && bootstrap_value && vs && pg, "vtrace_from_logits: NULL pointer");
   CU(launch_vtrace_logits(bl, tl, actions, discounts, rewards, values, bootstrap_value, T, B, A, clip_rho, clip_pg, vs, pg, log_rhos,
@@ -56,6 +58,7 @@ extern "C" int srl_impala_loss_and_head_grads(const float* bl, const float* tl, 
                                               float entropy_cost, float* vs, float* pg, float* dlogits, float* dbaseline, float* losses,
                                               float* scratch, void* stream) {
   REQ(T >= 1 && B >= 1 && A >= 1, "impala_loss: bad shape T=%d B=%d A=%d", T, B, A);
+  REQ(!std::isnan(clip_rho) && !std::isnan(clip_pg), "impala_loss: a clip threshold is NaN (< 0 means None)");
   REQ(bl && tl && baseline && action && reward && done && dlogits && dbaseline && losses && scratch, "impala_loss: NULL pointer");
   srl_config_t c = {};
   c.T = T; c.B = B; c.A = A; c.discounting = discounting; c.reward_clip_abs_one = reward_clip_abs_one;
@@ -211,6 +214,7 @@ static int check_cfg(const srl_config_t* c) {
   REQ(c->use_lstm == 0 || c->use_lstm == 1, "config: use_lstm must be 0 or 1");
   REQ(c->precision == 0 || c->precision == 1, "config: precision must be 0 (bf16 operands) or 1 (fp32-accurate split operands)");
   REQ(!(c->precision == 1 && c->use_lstm), "config: the fp32-accurate operand mode covers the non-LSTM learner only");
+  REQ(!std::isnan(c->clip_rho_threshold) && !std::isnan(c->clip_pg_rho_threshold), "config: a clip threshold is NaN (< 0 means None)");
   return 0;
 }
 

@@ -161,7 +161,7 @@ class ImpalaHParams:
     total_frames: Optional[int] = None   # frame budget of the 'linear' schedule (ImpalaArguments.total_steps)
 
     def validate(self) -> None:
-        """the optimizer settings the fused kernels support; anything else raises ValueError"""
+        """the optimizer settings the fused kernels support and the clip thresholds; anything else raises ValueError"""
         if self.optimizer not in ('rmsprop', 'adam'):
             raise ValueError("optimizer must be 'rmsprop' or 'adam'")
         if not self.momentum >= 0.0:
@@ -174,6 +174,10 @@ class ImpalaHParams:
             raise ValueError(f'min_learning_rate must be >= 0, got {self.min_learning_rate}')
         if self.lr_schedule == 'linear' and not (self.total_frames is not None and self.total_frames > 0):
             raise ValueError("lr_schedule='linear' needs total_frames > 0 (the frame budget the lr decays over)")
+        for name in ('clip_rho_threshold', 'clip_pg_rho_threshold'):
+            v = getattr(self, name)
+            if v is not None and not float(v) >= 0.0:
+                raise ValueError(f'{name} must be >= 0 or None (no clipping), got {v}')
 
     def to_c(self) -> _lib.SrlConfig:
         if self.reward_clipping not in ('abs_one', 'none'):

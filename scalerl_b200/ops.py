@@ -30,7 +30,14 @@ def _f32(t, name):
 
 
 def _clip(v):
-    return -1.0 if v is None else float(v)
+    """a clip threshold for the C ABI: None (no clipping) is -1; a number must be >= 0 (a negative or NaN one is refused, not read as
+    None)"""
+    if v is None:
+        return -1.0
+    v = float(v)
+    if not v >= 0.0:
+        raise ValueError(f'clip thresholds must be >= 0 or None, got {v}')
+    return v
 
 
 @torch.no_grad()
