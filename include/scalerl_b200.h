@@ -201,7 +201,8 @@ int srl_learner_forward_backward_begin(srl_learner_t* L, const uint8_t* obs, con
                                        float* losses, float* vs, float* pg_advantages, void* stream);
 int srl_learner_backward_finish(srl_learner_t* L, const uint8_t* obs, void* stream);
 
-/* clip_grad_norm_(max_grad_norm) over `grads` (after the caller's all-reduce, if any) + optimizer step.
+/* clip_grad_norm_(max_grad_norm) over `grads` (after the caller's all-reduce, if any) + optimizer step.  A NaN gradient makes the
+ * norm and the clip coefficient NaN and poisons every weight, as clip_grad_norm_ + step does (max_grad_norm < 0: no clip, coefficient 1).
  * grad_norm_out: f32 [2] = {total L2 norm, clip coefficient} (may be NULL); f32 [3] = {..., lr of the step} once
  * srl_learner_set_lr_schedule has been called.  The bf16 operand copies of the weights
  * are re-derived at the start of the next srl_learner_forward* call. */
@@ -223,7 +224,7 @@ int srl_learner_apply_gradients_dp(srl_learner_t* L, const srl_dp_peers_t* peers
 
 /* Weight-publish snapshot (impala_atari.py:348, actor_model.load_state_dict(learner_model.state_dict())): copies the flat fp32
  * parameters to `dst` (same layout, srl_param_layout elements) on `stream` -- unless losses[3] (the step's total loss, device
- * f32[4]; may be NULL = unconditional) is NaN/Inf, in which case `dst` keeps the last good weights.  The caller then copies
+ * f32[4]; may be NULL = unconditional) is NaN/Inf, in which case `dst` keeps the last good weights (every finite loss copies).  The caller then copies
  * `dst` to the actors' host memory asynchronously while the next step already updates the live parameters. */
 int srl_learner_snapshot_params(srl_learner_t* L, float* dst, const float* losses, void* stream);
 
@@ -544,7 +545,10 @@ int srl_unpack_slots(const uint8_t* staging, int64_t slot_bytes, const int64_t* 
                      void* stream);
 
 /* ---- stand-alone optimizer ops (flat f32 buffers of n elements) ------------------------------------------
- * srl_grad_norm_clip_coef: coef[0] = ||g||_2, coef[1] = min(1, max_norm/(||g||+1e-6)); scratch f32[>=1028]. */
+ * srl_grad_norm_clip_coef: coef[0] = ||g||_2, coef[1] = min(1, max_norm/(||g||+1e-6)); scratch f32[>=1028].  max_norm < 0 or +inf:
+ * no clip (coefficient 1).  A NaN norm gives a NaN coefficient, as torch.nn.utils.clip_grad_norm_ does, so one NaN gradient poisons
+ * every clipped gradient; an Inf one gives the coefficient 0.  The fused steps (srl_learner_apply_gradients[_dp],
+ * srl_apex_learner_step) clip the same way. */
 int srl_grad_norm_clip_coef(const float* grads, int64_t n, float max_norm, float* coef, float* scratch, void* stream);
 int srl_rmsprop_step(float* params, const float* grads, float* square_avg, int64_t n, const float* coef,
                      float lr, float alpha, float eps, void* stream);

@@ -16,6 +16,16 @@ int srl_test_shifted_operand(const void* A, const void* B, float* D, int shift, 
 int srl_test_poison_smem(void* stream);
 /* programmatic-dependent-launch self test; every out[0..nblk) must read 1 (flag, out: device int buffers) */
 int srl_test_pdl(int* flag, int* out, int nblk, unsigned delay_ns, void* stream);
+/* one fused clip + optimizer step (the cooperative kernel srl_learner_apply_gradients and srl_apex_learner_step run) on flat f32
+ * device buffers of any n >= 1.  optimizer 0 = RMSprop: s0 = square_avg, a = alpha (b, s1 unused); 1 = Adam: s0 = exp_avg,
+ * s1 = exp_avg_sq, a, b = beta1, beta2.  coef f32[3] receives {norm, clip coefficient, lr of the step (but for constant-lr RMSprop
+ * without momentum)}; scratch f32[>= 596] the block partials.  The step count is *dstep + 1 (dstep NULL: step >= 1), stored back to
+ * *dstep.  schedule 0 = constant lr, 1 = linear (lr_end >= 0, frames_per_step > 0, total_frames > 0); momentum_buf (RMSprop only,
+ * NULL: none) with momentum >= 0.  p, g, s0, s1, momentum_buf 16-byte aligned.  blocks (may be NULL) receives the grid launched,
+ * variant (may be NULL) the parameters of the clip_optim_kernel<OPT, SCHED, MOM> template launched: 4 OPT + 2 SCHED + MOM. */
+int srl_test_clip_optim(int optimizer, float* p, float* g, float* s0, float* s1, int64_t n, float max_norm, float* coef, float* scratch,
+                        float lr, float a, float b, float eps, int step, int* dstep, int schedule, float lr_end, double frames_per_step,
+                        double total_frames, float* momentum_buf, float momentum, int* blocks, int* variant, void* stream);
 #ifdef __cplusplus
 }
 #endif

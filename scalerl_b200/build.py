@@ -13,6 +13,7 @@ OUT = os.path.join(HERE, 'libscalerl_b200.so')
 OUT_HOOKS = os.path.join(HERE, 'libscalerl_b200_testhooks.so')
 SOURCES = ['api.cu', 'encoder.cu', 'vtrace.cu', 'heads.cu', 'optim.cu', 'lstm.cu', 'per.cu', 'dqn.cu', 'dqn_cat.cu', 'dqn_qr.cu', 'replay.cu', 'apex_actor.cu', 'noisy.cu']
 HOOK_SOURCES = ['testhooks.cu', 'test_shift.cu']
+HOOK_LINKS = ['optim.cu']          # product objects the hooks library links too (compiled once, for both libraries)
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xptxas', '-v', '--expt-relaxed-constexpr'] + \
              [f'-D{d}' for d in os.environ.get('SRL_DEFINES', '').split(',') if d]       # e.g. SRL_DEFINES=SRL_KSTAMP (diagnostics build)
@@ -58,7 +59,7 @@ def build(force=False, verbose=False):
             raise RuntimeError(f'nvcc failed on {src}:\n{r.stdout}\n{r.stderr}')
     with open(os.path.join(objdir, 'ptxas.log'), 'w') as f:
         f.write('\n'.join(log))
-    for out, srcs in ((OUT, SOURCES), (OUT_HOOKS, HOOK_SOURCES)):
+    for out, srcs in ((OUT, SOURCES), (OUT_HOOKS, HOOK_SOURCES + HOOK_LINKS)):
         cmd = [nvcc, '-shared', '-o', out] + [o for s_, o, _ in results if s_ in srcs] + ['-lcudart']
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

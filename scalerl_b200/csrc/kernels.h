@@ -206,7 +206,8 @@ struct OptStep {
   int* dstep;
   OptExtra x;
 };
-cudaError_t launch_clip_optim(const OptStep& o, cudaStream_t st);
+// blocks (may be null) receives the grid size launched, variant (may be null) the template's parameters 4 OPT + 2 SCHED + MOM
+cudaError_t launch_clip_optim(const OptStep& o, cudaStream_t st, int* blocks = nullptr, int* variant = nullptr);
 struct DpPeers { float* g[8]; float* rs[8]; unsigned* ctl[8]; int rank, world; float* mc_g; };      // peer-mapped gradient buffers / control blocks; mc_g: NVLS multicast address of the gradient buffers (or null)
 cudaError_t launch_dp_clip_optim(const OptStep& o, const DpPeers& P, cudaStream_t st);
 cudaError_t launch_snapshot_if_finite(float* dst, const float* src, int64_t n, const float* losses, cudaStream_t st);

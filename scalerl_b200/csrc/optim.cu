@@ -38,8 +38,14 @@ SRL_DEVINL double sum_partials(const float* scratch, unsigned count) {
   for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
   return t;
 }
-// torch.nn.utils.clip_grad_norm_: the gradients are scaled by min(1, max_norm / (||g|| + 1e-6)); max_norm < 0 does not clip
-SRL_DEVINL float clip_coef(float norm, float max_norm) { return max_norm >= 0.f ? fminf(max_norm / (norm + 1e-6f), 1.0f) : 1.0f; }
+// torch.nn.utils.clip_grad_norm_: the gradients are scaled by min(1, max_norm / (||g|| + 1e-6)); max_norm < 0 and max_norm = +inf
+// do not clip (coefficient exactly 1).  A NaN norm gives a NaN coefficient, as torch's clamp(max=1) does, so a NaN anywhere in the
+// gradients poisons every weight (fminf would return the non-NaN operand, 1, and step every other weight as if nothing happened).
+SRL_DEVINL float clip_coef(float norm, float max_norm) {
+  if (!(max_norm >= 0.f) || isinf(max_norm)) return 1.0f;
+  const float c = max_norm / (norm + 1e-6f);
+  return c < 1.0f || isnan(c) ? c : 1.0f;
+}
 
 // one element of torch.optim.RMSprop(centered=False) on the clipped gradient gk: v = a v + (1-a) gk^2, then
 // MOM: m = mu m + gk / (sqrt(v) + eps), p -= lr m;  else: p -= lr gk / (sqrt(v) + eps).
@@ -515,7 +521,7 @@ __global__ void __launch_bounds__(256) snapshot_if_finite_kernel(float4* __restr
                                                                  const float* __restrict__ losses) {
   if (losses) {
     const float t = losses[3];
-    if (!(fabsf(t) <= 3.0e38f)) return;          // NaN or Inf: keep the previous snapshot
+    if (!isfinite(t)) return;                    // NaN or Inf: keep the previous snapshot
   }
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) dst[i] = __ldg(src + i);
 }
@@ -555,9 +561,10 @@ static cudaError_t coop_blocks(int64_t n, int* blocks_out) {
   return cudaSuccess;
 }
 template <auto KERNEL>
-static cudaError_t launch_coop(int64_t n, void** args, cudaStream_t st) {
+static cudaError_t launch_coop(int64_t n, void** args, cudaStream_t st, int* blocks_out = nullptr) {
   int blocks = 0;
   SRL_TRY(coop_blocks<KERNEL>(n, &blocks));
+  if (blocks_out) *blocks_out = blocks;
   return cudaLaunchCooperativeKernel((const void*)KERNEL, dim3(blocks), dim3(512), args, 0, st);
 }
 // calls f(OPT, SCHED, MOM), as std::integral_constants, for the variant of the step: RMSprop with or without momentum, or Adam,
@@ -574,10 +581,13 @@ static cudaError_t with_variant(int optimizer, const OptExtra& x, F f) {
   return lin ? f(Rms(), Lin(), std::false_type()) : f(Rms(), Const(), std::false_type());
 }
 
-cudaError_t launch_clip_optim(const OptStep& o, cudaStream_t st) {
+cudaError_t launch_clip_optim(const OptStep& o, cudaStream_t st, int* blocks, int* variant) {
   OptStep a = o;        // addressable copies of the kernel arguments
   void* args[] = {&a.p, &a.g, &a.s0, &a.s1, &a.n, &a.max_norm, &a.coef, &a.scratch, &a.lr, &a.a, &a.b, &a.eps, &a.step, &a.dstep, &a.x};
-  return with_variant(o.optimizer, o.x, [&](auto O, auto S, auto M) { return launch_coop<clip_optim_kernel<O, S, M>>(o.n, args, st); });
+  return with_variant(o.optimizer, o.x, [&](auto O, auto S, auto M) {
+    if (variant) *variant = 4 * decltype(O)::value + 2 * decltype(S)::value + (decltype(M)::value ? 1 : 0);
+    return launch_coop<clip_optim_kernel<O, S, M>>(o.n, args, st, blocks);
+  });
 }
 cudaError_t launch_dp_clip_optim(const OptStep& o, const DpPeers& P, cudaStream_t st) {
   OptStep a = o;
