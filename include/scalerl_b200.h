@@ -385,7 +385,12 @@ int srl_replay_gather(srl_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* 
  * Bellemare et al. 2017): q = Linear(512, A K), row a K + k atom k of action a, p(s)[a] = softmax over the action's K logits, Q(s, a) =
  * sum_k z_k p_k on the support z_k = v_min + k dz, dz = (v_max - v_min) / (K - 1) rounded once to fp32.  With `num_quantiles` = N > 0
  * the head is the quantile head (QR-DQN, Dabney et al. 2018): q = Linear(512, A N), row a N + i quantile i of action a at the midpoint
- * tau^_i = (2 i + 1) / (2 N), Q(s, a) = (sum_i theta_{a,i}) / N.
+ * tau^_i = (2 i + 1) / (2 N), Q(s, a) = (sum_i theta_{a,i}) / N.  With `dist_dueling` = 1 either of these heads is Rainbow's dueling
+ * head per atom or quantile (Hessel et al. 2018), W = K or N rows per action: v = value(h) = Linear(512, W), adv = advantage(h) =
+ * Linear(512, A W), rows[a W + k] = (v[k] + adv[a W + k]) - (1/A) sum_a' adv[a' W + k], the advantage mean summed over a' in order and
+ * divided once.  The step composes W_eff and b_eff of these rows from value and advantage (online and target, from the parameters as they
+ * are when it runs), runs the categorical or quantile update on them unchanged, and splits the rows' gradients back into g_v[k] =
+ * sum_a g[a W + k] and g_adv[a W + k] = g[a W + k] - (1/A) sum_a' g[a' W + k].
  * srl_replay_* stores and folds n-step transitions (pass gamma^n for them, and srl_replay_per as `per`); srl_apex_actor_* acts and computes
  * their initial priorities.
  * Parameters in state_dict order {conv1.weight, conv1.bias, conv2.weight, conv2.bias, conv3.weight, conv3.bias, fc.weight, fc.bias,
@@ -393,7 +398,8 @@ int srl_replay_gather(srl_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* 
  * The dueling head's state_dict order is {conv1..3, fc, value.weight [1,512], value.bias [1], advantage.weight [A,512],
  * advantage.bias [A]} (int64[12], srl_apex_param_layout_ex); value.weight lies directly before advantage.weight.
  * The categorical head keeps the 10 plain names with q.weight [A K, 512] and q.bias [A K] (srl_apex_param_layout_cat), and so does the
- * quantile head with q.weight [A N, 512] and q.bias [A N] (srl_apex_param_layout_quantile).
+ * quantile head with q.weight [A N, 512] and q.bias [A N] (srl_apex_param_layout_quantile).  The distributional dueling head has the
+ * dueling head's 12 names with value [W, 512], [W] and advantage [A W, 512], [A W] (srl_apex_param_layout_dist_dueling).
  * Every head, with or without noise, has one layout rule (srl_apex_param_layout_noisy's): in memory, each segment padded to 4
  * floats, come the conv tensors, fc's bias, the head weights and the head biases (noisy: the head biases first), then fc's weight,
  * each group by (mu before sigma, layer).  Params, grads, both Adam states and the target copy share the layout. */
@@ -414,6 +420,7 @@ typedef struct srl_apex_config {
   uint64_t noise_seed;       /* the Philox key of the noise (read when noisy = 1)                                */
   int32_t num_quantiles;     /* 0: no quantile head; N in [2, 256]: the quantile head (not with dueling = 1 or num_atoms > 0) */
   float kappa;               /* the quantile Huber threshold, finite and > 0 (read when num_quantiles > 0; QR-DQN-1: 1)      */
+  int32_t dist_dueling;      /* 0; 1: the categorical or quantile head as dueling rows (not with dueling = 1)             */
 } srl_apex_config_t;
 int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10);
 /* the layout of either head: dueling 0 -> 10 tensors (srl_apex_param_layout's), 1 -> 12; -1 with srl_last_error set for A outside
@@ -434,6 +441,12 @@ int64_t srl_apex_param_layout_noisy(int A, int dueling, int num_atoms, int noisy
  * q.bias [A N]; not with dueling = 1 or num_atoms > 0), 0 for the others.  -> the buffer's floats, or -1 with srl_last_error set */
 int64_t srl_apex_param_layout_quantile(int A, int dueling, int num_atoms, int num_quantiles, int noisy, int64_t* offsets18,
                                        int64_t* counts18);
+/* The layout of every head: srl_apex_param_layout_quantile's with dist_dueling = 1 for the distributional dueling head (num_atoms > 0
+ * or num_quantiles > 0, not dueling = 1): value [W, 512] and advantage [A W, 512] with their biases in the dueling head's places, so
+ * value.weight lies directly before advantage.weight (noisy: the mu rows, and the sigma rows).  -> the buffer's floats, or -1 with
+ * srl_last_error set */
+int64_t srl_apex_param_layout_dist_dueling(int A, int dueling, int num_atoms, int num_quantiles, int dist_dueling, int noisy,
+                                           int64_t* offsets18, int64_t* counts18);
 /* params / grads / exp_avg / exp_avg_sq / target_params: caller-owned flat f32 device buffers of srl_apex_param_layout floats,
  * 16-byte aligned and disjoint.  The context owns the encoder's blocks (one saved block for the forward over s, one for the
  * forwards over s', their scratch) and the tail's buffers.  Synchronous. */
@@ -477,7 +490,9 @@ int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* obs, int n, 
  * The categorical head adds "logits", "logits_next" (double DQN only), "logits_next_target" and "dlogits" f32 [B,A*K], "m" f32 [B,K]
  * (the projected targets) and "ce" f32 [B] (the cross-entropies); its "y" is sum_k z_k m_k.  The quantile head adds "theta",
  * "theta_next" (double DQN only), "theta_next_target" and "dtheta" f32 [B,A*N] (the quantiles and their gradient), "target_quantiles"
- * f32 [B,N] and "qr_loss" f32 [B] (the per-transition losses).
+ * f32 [B,N] and "qr_loss" f32 [B] (the per-transition losses).  The distributional dueling head adds the rows the step composed,
+ * "rows_weight_online" / "rows_weight_target" f32 [A*W,512] and "rows_bias_online" / "rows_bias_target" f32 [A*W], and their
+ * gradients "rows_weight_grad" f32 [A*W,512] and "rows_bias_grad" f32 [A*W] (W = K or N).
  * Noisy networks add, per network <n> = "online" or "target", the last step's "normals_<n>" (the standard normals) and "noise_<n>"
  * (f of them) f32 [NN] = [fc in 3136 | fc out 512 | head in 512 (dueling: value's, then advantage's) | head out R (dueling: value's 1,
  * then advantage's A)], R = the head's rows (A, A K, or A + 1), and the composed weights "fc_weight_<n>" [512,3136], "fc_bias_<n>"
@@ -513,6 +528,12 @@ int srl_apex_actor_create_noisy(int A, int num_envs, int precision, int dueling,
  * (srl_apex_learner_step's bits) */
 int srl_apex_actor_create_quantile(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max, int num_quantiles,
                                    float kappa, int noisy, uint64_t seed, const float* params, srl_apex_actor_t** out);
+/* the same with dist_dueling as srl_apex_config_t's (0: srl_apex_actor_create_quantile's head); params in
+ * srl_apex_param_layout_dist_dueling(A, dueling, num_atoms, num_quantiles, dist_dueling, noisy) order.  Every act, q_values and
+ * prioritized add composes the head rows from the snapshot as it is then (after the noise, when noisy), as srl_apex_learner_step does */
+int srl_apex_actor_create_dist_dueling(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max,
+                                       int num_quantiles, float kappa, int dist_dueling, int noisy, uint64_t seed, const float* params,
+                                       srl_apex_actor_t** out);
 int srl_apex_actor_destroy(srl_apex_actor_t* X);
 /* obs u8 [E,4,84,84], epsilons f32 [E] (device) -> actions i64 [E]: with probability epsilons[e] a uniform action, else the first
  * argmax of Q(obs[e]) (torch.argmax's pick).  The random numbers are Philox4x32-10 keyed by seed, counted by (draw, env); the launch
@@ -524,7 +545,8 @@ int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, int n, floa
  * rows E..2E-1: its next states) and, categorical head only, "logits" f32 [2E,A*K] of the same rows (quantile head: "theta"
  * f32 [2E,A*N]).  A noisy actor adds its kept draw
  * "normals" and "noise" and the weights its last call composed, "fc_weight", "fc_bias", "head_weight", "head_bias" and (dueling)
- * "head_adv_bias", in the layouts of srl_apex_learner_debug_buffer's */
+ * "head_adv_bias", in the layouts of srl_apex_learner_debug_buffer's.  The distributional dueling head adds the rows its last call
+ * composed, "rows_weight" f32 [A*W,512] and "rows_bias" f32 [A*W] */
 int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name, void** ptr, int64_t* count);
 /* srl_replay_add, then, for the E transitions the call completes, their initial priorities computed by `actor` (built for the memory's
  * num_envs) instead of max_priority:  p = |Q(s)[a] - y| + priority_eps,  y = R + fp32(gamma^n_step) (1 - d) max_a Q(s')  with the

@@ -107,6 +107,7 @@ _SIGS = {
     'srl_apex_actor_create_cat': [_I, _I, _I, _I, _F, _F, C.c_uint64, _P, C.POINTER(_P)],
     'srl_apex_actor_create_noisy': [_I, _I, _I, _I, _I, _F, _F, _I, C.c_uint64, _P, C.POINTER(_P)],
     'srl_apex_actor_create_quantile': [_I, _I, _I, _I, _I, _F, _F, _I, _F, _I, C.c_uint64, _P, C.POINTER(_P)],
+    'srl_apex_actor_create_dist_dueling': [_I, _I, _I, _I, _I, _F, _F, _I, _F, _I, _I, C.c_uint64, _P, C.POINTER(_P)],
     'srl_apex_actor_debug_buffer': [_P, C.c_char_p, C.POINTER(_P), C.POINTER(_L)],
     'srl_apex_actor_destroy': [_P],
     'srl_apex_actor_act': [_P] * 5,
@@ -142,7 +143,7 @@ def hooks():
     return _hooks
 
 
-EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout', 'srl_apex_param_layout_ex', 'srl_apex_param_layout_cat', 'srl_apex_param_layout_noisy', 'srl_apex_param_layout_quantile', 'srl_replay_size', 'srl_replay_per'])
+EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout', 'srl_apex_param_layout_ex', 'srl_apex_param_layout_cat', 'srl_apex_param_layout_noisy', 'srl_apex_param_layout_quantile', 'srl_apex_param_layout_dist_dueling', 'srl_replay_size', 'srl_replay_per'])
 
 
 def lib():
@@ -189,6 +190,8 @@ def lib():
         L.srl_apex_param_layout_noisy.argtypes = [_I, _I, _I, _I, C.POINTER(_L), C.POINTER(_L)]
         L.srl_apex_param_layout_quantile.restype = C.c_int64
         L.srl_apex_param_layout_quantile.argtypes = [_I, _I, _I, _I, _I, C.POINTER(_L), C.POINTER(_L)]
+        L.srl_apex_param_layout_dist_dueling.restype = C.c_int64
+        L.srl_apex_param_layout_dist_dueling.argtypes = [_I, _I, _I, _I, _I, _I, C.POINTER(_L), C.POINTER(_L)]
         L.srl_learner_workspace_bytes.restype = C.c_int64
         L.srl_learner_workspace_bytes.argtypes = [_P]
         _lib = L
@@ -216,30 +219,33 @@ class SrlApexConfig(C.Structure):
                 ('gamma', C.c_float), ('max_grad_norm', C.c_float), ('learning_rate', C.c_float), ('adam_beta1', C.c_float),
                 ('adam_beta2', C.c_float), ('adam_eps', C.c_float), ('priority_eps', C.c_float), ('dueling', C.c_int32),
                 ('num_atoms', C.c_int32), ('v_min', C.c_float), ('v_max', C.c_float), ('noisy', C.c_int32), ('noise_seed', C.c_uint64),
-                ('num_quantiles', C.c_int32), ('kappa', C.c_float)]
+                ('num_quantiles', C.c_int32), ('kappa', C.c_float), ('dist_dueling', C.c_int32)]
 
 
-def apex_param_layout(A, dueling=False, num_atoms=0, noisy=False, num_quantiles=0):
-    """(total floats, offsets, counts) of the Ape-X Q network's flat buffer in state_dict order (srl_apex_param_layout_quantile): 10
-    tensors, or 12 with the dueling head; num_atoms > 0: the categorical head's 10 (q.weight [A num_atoms, 512], q.bias
-    [A num_atoms]); num_quantiles > 0: the quantile head's 10 (q.weight [A num_quantiles, 512], q.bias [A num_quantiles]); noisy: 14,
-    or 18 with the dueling head"""
+def apex_param_layout(A, dueling=False, num_atoms=0, noisy=False, num_quantiles=0, dist_dueling=False):
+    """(total floats, offsets, counts) of the Ape-X Q network's flat buffer in state_dict order (srl_apex_param_layout_dist_dueling):
+    10 tensors, or 12 with the dueling head; num_atoms > 0: the categorical head's 10 (q.weight [A num_atoms, 512], q.bias
+    [A num_atoms]); num_quantiles > 0: the quantile head's 10 (q.weight [A num_quantiles, 512], q.bias [A num_quantiles]);
+    dist_dueling: either head's 12 as value [W, 512] and advantage [A W, 512] (W = num_atoms or num_quantiles); noisy: 14, or 18 with
+    value and advantage"""
     off = (_L * 18)()
     cnt = (_L * 18)()
-    total = lib().srl_apex_param_layout_quantile(int(A), 1 if dueling else 0, int(num_atoms), int(num_quantiles), 1 if noisy else 0, off, cnt)
+    total = lib().srl_apex_param_layout_dist_dueling(int(A), 1 if dueling else 0, int(num_atoms), int(num_quantiles), 1 if dist_dueling else 0,
+                                                     1 if noisy else 0, off, cnt)
     if total < 0:
-        check(-1, 'srl_apex_param_layout_quantile')
-    n = 6 + (3 if dueling else 2) * (4 if noisy else 2)
+        check(-1, 'srl_apex_param_layout_dist_dueling')
+    n = 6 + (3 if dueling or dist_dueling else 2) * (4 if noisy else 2)
     return int(total), [int(x) for x in off][:n], [int(x) for x in cnt][:n]
 
 
 def apex_actor_create(A, num_envs, precision, seed, params, head) -> C.c_void_p:
-    """srl_apex_actor_create_quantile for ``head`` (dueling, num_atoms, v_min, v_max, num_quantiles, kappa, noisy) on the device
-    buffer at ``params``"""
+    """srl_apex_actor_create_dist_dueling for ``head`` (dueling, num_atoms, v_min, v_max, num_quantiles, kappa, dist_dueling, noisy)
+    on the device buffer at ``params``"""
     h = C.c_void_p()
-    check(lib().srl_apex_actor_create_quantile(A, num_envs, precision, int(head.dueling), head.num_atoms, head.v_min, head.v_max,
-                                               head.num_quantiles, head.kappa, int(head.noisy), seed, params, C.byref(h)),
-          'srl_apex_actor_create_quantile')
+    check(lib().srl_apex_actor_create_dist_dueling(A, num_envs, precision, int(head.dueling), head.num_atoms, head.v_min, head.v_max,
+                                                   head.num_quantiles, head.kappa, int(head.dist_dueling), int(head.noisy), seed, params,
+                                                   C.byref(h)),
+          'srl_apex_actor_create_dist_dueling')
     return h
 
 

@@ -20,6 +20,9 @@ snapshot before its forward (one draw for all envs, from ``seed`` and a device c
 replay) and keeps it; ``q_values`` and the prioritized add use the kept draw on the snapshot as it is.  Its default epsilons are 0.
 ``quantile_dqn=True`` (with ``num_quantiles``, ``quantile_kappa``) gives it the quantile head of ``ApexHParams(quantile_dqn=True)``: it
 acts on the quantile means and prioritises by the learner's quantile Huber loss, and syncs from learners with the same setting only.
+``distributional_dueling=True`` (with ``categorical_dqn`` or ``quantile_dqn``) gives it the dueling rows of
+``ApexHParams(distributional_dueling=True)``: every call composes the snapshot's value and advantage layers into the head rows as the
+learner does, so its rows, Q values, actions and priorities are the learner's bits.
 """
 from __future__ import annotations
 
@@ -53,16 +56,19 @@ class B200ApexActor:
     shapes).  ``epsilons``: [num_envs] values in [0, 1] (None: ``apex_epsilons(num_envs)``); ``precision``: the encoder operands, as
     the learner's; ``priority_eps`` (> 0) is added to every priority the actor computes; ``dueling_dqn``, ``categorical_dqn`` (with
     ``v_min``, ``v_max``, ``num_atoms``), ``noisy_dqn`` (with ``noisy_std``, the initial sigma0 of the default weights), ``quantile_dqn``
-    (with ``num_quantiles``, ``quantile_kappa``): the learner's head (noisy: epsilons None means 0 for every env).  Calls run on the current stream and share the actor's buffers: issue them from one
+    (with ``num_quantiles``, ``quantile_kappa``), ``distributional_dueling``: the learner's head (noisy: epsilons None means 0 for every
+    env).  Calls run on the current stream and share the actor's buffers: issue them from one
     stream."""
     # the head settings as the constructor stores them; the class values are its defaults
     dueling_dqn, categorical_dqn, v_min, v_max, num_atoms, noisy_dqn = False, False, 0.0, 200.0, 51, False
     quantile_dqn, num_quantiles, quantile_kappa = False, 200, 1.0
+    distributional_dueling = False
 
     def __init__(self, num_envs: int, num_actions: int, epsilons=None, seed: int = 0, precision: str = 'bf16', priority_eps: float = 1e-6,
                  device=None, init_state_dict: Optional[Dict[str, torch.Tensor]] = None, dueling_dqn: bool = False,
                  categorical_dqn: bool = False, v_min: float = 0.0, v_max: float = 200.0, num_atoms: int = 51, noisy_dqn: bool = False,
-                 noisy_std: float = 0.5, quantile_dqn: bool = False, num_quantiles: int = 200, quantile_kappa: float = 1.0):
+                 noisy_std: float = 0.5, quantile_dqn: bool = False, num_quantiles: int = 200, quantile_kappa: float = 1.0,
+                 distributional_dueling: bool = False):
         if isinstance(num_envs, bool) or not isinstance(num_envs, (int, np.integer)) or not 1 <= num_envs <= MAX_FRAMES:
             raise ValueError(f'num_envs must be an int in [1, {MAX_FRAMES}], got {num_envs!r}')
         check_net_args(num_actions, noisy_std)
@@ -71,7 +77,7 @@ class B200ApexActor:
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be 'bf16' or 'fp32_split', got {precision!r}")
         self.head = head = QHead.of(dueling_dqn, categorical_dqn, num_atoms, v_min, v_max, noisy_dqn, quantile_dqn, num_quantiles,
-                                    quantile_kappa)
+                                    quantile_kappa, distributional_dueling)
         priority_eps = float(priority_eps)
         if not (math.isfinite(priority_eps) and priority_eps > 0.0):
             raise ValueError(f'priority_eps must be finite and > 0 (a zero leaf makes the sampler\'s IS weight infinite), got {priority_eps}')
@@ -80,6 +86,7 @@ class B200ApexActor:
         self.v_min, self.v_max, self.num_atoms = float(v_min), float(v_max), int(num_atoms)
         self.noisy_dqn = noisy_dqn
         self.quantile_dqn, self.num_quantiles, self.quantile_kappa = quantile_dqn, int(num_quantiles), float(quantile_kappa)
+        self.distributional_dueling = distributional_dueling
         if epsilons is None:
             epsilons = np.zeros(self.num_envs) if noisy_dqn else apex_epsilons(self.num_envs)
         eps = self._epsilons(epsilons)
@@ -94,8 +101,8 @@ class B200ApexActor:
             self.params = flat_views(self.flat_params, off, cnt, self.shapes)
             self.epsilons = eps.to(self.device)           # read by the act kernel when it runs
             self._h = _lib.apex_actor_create(self.num_actions, self.num_envs, PRECISIONS[precision], self.seed, self.flat_params.data_ptr(), head)
-        sd = default_q_state_dict(self.num_actions, self.seed, head.dueling, head.num_atoms, head.noisy, noisy_std, head.num_quantiles) \
-            if init_state_dict is None else init_state_dict
+        sd = default_q_state_dict(self.num_actions, self.seed, head.dueling, head.num_atoms, head.noisy, noisy_std, head.num_quantiles,
+                                  head.dist_dueling) if init_state_dict is None else init_state_dict
         self.load_state_dict(sd)
         self.weights_version = 0
 
@@ -103,7 +110,7 @@ class B200ApexActor:
     def head(self) -> QHead:
         """the Q head of the settings above (the constructor stores the one it built)"""
         return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max, self.noisy_dqn, self.quantile_dqn,
-                        self.num_quantiles, self.quantile_kappa)
+                        self.num_quantiles, self.quantile_kappa, self.distributional_dueling)
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream

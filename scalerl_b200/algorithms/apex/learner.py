@@ -26,6 +26,11 @@ independent draw for the target network, both from (seed, k); ``q_values``, ``pr
 num_quantiles)``, row a N + i quantile i of action a at the midpoint tau_i = (2 i + 1) / (2 N), Q = the mean of an action's quantiles
 for acting and the greedy target, and the quantile Huber loss (threshold ``quantile_kappa``) against the target quantiles
 ``r + gamma theta'(s')[a*]`` as the loss and the priority.  It needs no support; the state-dict names stay the plain head's ten.
+
+``ApexHParams(distributional_dueling=True)``, with ``categorical_dqn`` or ``quantile_dqn``, gives that head the dueling architecture per
+atom or quantile, as in Rainbow (Hessel et al. 2018): ``value = Linear(512, W)`` and ``advantage = Linear(512, A * W)`` (W = num_atoms
+or num_quantiles) on the shared fc output, combined into the head rows ``v.view(-1, 1, W) + adv.view(-1, A, W) - adv.view(-1, A,
+W).mean(1, keepdim=True)``, which the C51 or QR update then reads as before.  The state-dict names are the dueling head's.
 """
 from __future__ import annotations
 
@@ -50,14 +55,20 @@ PLAIN_SUFFIXES = ('weight', 'bias')
 NOISY_SUFFIXES = ('weight_mu', 'weight_sigma', 'bias_mu', 'bias_sigma')     # NoisyLinear's parameters, in registration order
 
 
-def apex_param_shapes(num_actions: int, dueling: bool = False, num_atoms: int = 0, noisy: bool = False, num_quantiles: int = 0):
+def apex_param_shapes(num_actions: int, dueling: bool = False, num_atoms: int = 0, noisy: bool = False, num_quantiles: int = 0,
+                      dist_dueling: bool = False):
     """the named shapes of the Q network's parameters in state_dict order = AtariQNet.parameters() order = the integer keys of the
-    Adam state (srl_apex_param_layout_quantile order): conv1..3, fc, then q or value and advantage; num_atoms > 0: the categorical head
-    q = Linear(512, num_actions * num_atoms); num_quantiles > 0: the quantile head q = Linear(512, num_actions * num_quantiles); noisy:
-    fc and the head layers as NoisyLinear's weight_mu, weight_sigma, bias_mu, bias_sigma"""
+    Adam state (srl_apex_param_layout_dist_dueling order): conv1..3, fc, then q or value and advantage; num_atoms > 0: the categorical
+    head q = Linear(512, num_actions * num_atoms); num_quantiles > 0: the quantile head q = Linear(512, num_actions * num_quantiles);
+    dist_dueling: that head as value = Linear(512, W) and advantage = Linear(512, num_actions * W), W = num_atoms or num_quantiles;
+    noisy: fc and the head layers as NoisyLinear's weight_mu, weight_sigma, bias_mu, bias_sigma"""
     lin = NOISY_SUFFIXES if noisy else PLAIN_SUFFIXES
-    rows = num_actions * (num_atoms or num_quantiles or 1)
-    head = [('value', (1, 512)), ('advantage', (num_actions, 512))] if dueling else [('q', (rows, 512))]
+    width = num_atoms or num_quantiles or 1
+    rows = num_actions * width
+    if dist_dueling:
+        head = [('value', (width, 512)), ('advantage', (rows, 512))]
+    else:
+        head = [('value', (1, 512)), ('advantage', (num_actions, 512))] if dueling else [('q', (rows, 512))]
     layers = [('conv1', (32, 4, 8, 8), PLAIN_SUFFIXES), ('conv2', (64, 32, 4, 4), PLAIN_SUFFIXES), ('conv3', (64, 64, 3, 3), PLAIN_SUFFIXES),
               ('fc', (512, 3136), lin)] + [(l, w, lin) for l, w in head]
     return OrderedDict((f'{l}.{s}', w if s.startswith('weight') else w[:1]) for l, w, suffixes in layers for s in suffixes)
@@ -160,16 +171,20 @@ class AtariQNet(nn.Module):
     and the head layers are ``NoisyLinear(..., noisy_std)`` (train mode: the noisy weights, eval mode: mu; ``reset_noise()`` redraws
     every layer's noise).  With ``quantile``, ``q = nn.Linear(512, num_actions * num_quantiles)`` whose row a * num_quantiles + i is
     quantile i of action a (QR-DQN): ``quantiles(obs)`` gives them, ``forward`` their mean (the midpoints ``taus`` are a non-persistent
-    buffer)."""
+    buffer).  With ``distributional_dueling`` (and ``categorical`` or ``quantile``) the head rows are Rainbow's dueling ones per atom or
+    quantile: ``value = nn.Linear(512, W)`` and ``advantage = nn.Linear(512, num_actions * W)`` combined as ``v.view(-1, 1, W) +
+    adv.view(-1, A, W) - adv.view(-1, A, W).mean(1, keepdim=True)``, W = num_atoms or num_quantiles."""
 
     def __init__(self, num_actions: int, observation_shape=(4, 84, 84), dueling: bool = False, categorical: bool = False,
                  num_atoms: int = 51, v_min: float = 0.0, v_max: float = 200.0, noisy: bool = False, noisy_std: float = 0.5,
-                 quantile: bool = False, num_quantiles: int = 200):
+                 quantile: bool = False, num_quantiles: int = 200, distributional_dueling: bool = False):
         super().__init__()
         if dueling and categorical:
             raise ValueError('the categorical head with the dueling head is not supported')
         if quantile and (dueling or categorical):
             raise ValueError('the quantile head with the dueling or the categorical head is not supported')
+        if distributional_dueling and not (categorical or quantile):
+            raise ValueError('distributional_dueling needs the categorical or the quantile head')
         self.observation_shape = tuple(observation_shape)
         self.num_actions = int(num_actions)
         self.dueling = bool(dueling)
@@ -178,6 +193,8 @@ class AtariQNet(nn.Module):
         self.num_atoms = int(num_atoms) if self.categorical else 0
         self.quantile = bool(quantile)
         self.num_quantiles = int(num_quantiles) if self.quantile else 0
+        self.distributional_dueling = bool(distributional_dueling)
+        width = self.num_atoms or self.num_quantiles
         linear = (lambda i, o: NoisyLinear(i, o, noisy_std)) if self.noisy else nn.Linear
         self.conv1 = nn.Conv2d(self.observation_shape[0], 32, kernel_size=8, stride=4)
         self.conv2 = nn.Conv2d(32, 64, kernel_size=4, stride=2)
@@ -186,14 +203,17 @@ class AtariQNet(nn.Module):
         if self.dueling:
             self.value = linear(512, 1)
             self.advantage = linear(512, self.num_actions)
-        elif self.categorical:
-            self.q = linear(512, self.num_actions * self.num_atoms)
-            self.register_buffer('support', categorical_support(self.num_atoms, v_min, v_max), persistent=False)
-        elif self.quantile:
-            self.q = linear(512, self.num_actions * self.num_quantiles)
-            self.register_buffer('taus', quantile_taus(self.num_quantiles), persistent=False)
+        elif self.distributional_dueling:
+            self.value = linear(512, width)
+            self.advantage = linear(512, self.num_actions * width)
+        elif self.categorical or self.quantile:
+            self.q = linear(512, self.num_actions * width)
         else:
             self.q = linear(512, self.num_actions)
+        if self.categorical:
+            self.register_buffer('support', categorical_support(self.num_atoms, v_min, v_max), persistent=False)
+        if self.quantile:
+            self.register_buffer('taus', quantile_taus(self.num_quantiles), persistent=False)
 
     def noisy_layers(self):
         """the NoisyLinear layers in state-dict order (none without noise)"""
@@ -211,17 +231,26 @@ class AtariQNet(nn.Module):
         x = F.relu(self.conv3(x))
         return F.relu(self.fc(x.reshape(x.shape[0], -1)))
 
+    def _rows(self, obs: torch.Tensor) -> torch.Tensor:
+        """a distributional head's rows [n, A, W] (logits or quantiles)"""
+        x = self._features(obs)
+        W = self.num_atoms or self.num_quantiles
+        if self.distributional_dueling:
+            v, adv = self.value(x).view(-1, 1, W), self.advantage(x).view(-1, self.num_actions, W)
+            return v + adv - adv.mean(1, keepdim=True)
+        return self.q(x).view(-1, self.num_actions, W)
+
     def dist(self, obs: torch.Tensor) -> torch.Tensor:
         """categorical head: obs u8 [N, 4, 84, 84] -> the atom probabilities p [N, A, num_atoms]"""
         if not self.categorical:
             raise ValueError('dist() needs the categorical head (AtariQNet(..., categorical=True))')
-        return F.softmax(self.q(self._features(obs)).view(-1, self.num_actions, self.num_atoms), dim=2)
+        return F.softmax(self._rows(obs), dim=2)
 
     def quantiles(self, obs: torch.Tensor) -> torch.Tensor:
         """quantile head: obs u8 [n, 4, 84, 84] -> the quantiles theta [n, A, num_quantiles]"""
         if not self.quantile:
             raise ValueError('quantiles() needs the quantile head (AtariQNet(..., quantile=True))')
-        return self.q(self._features(obs)).view(-1, self.num_actions, self.num_quantiles)
+        return self._rows(obs)
 
     def forward(self, obs: torch.Tensor) -> torch.Tensor:
         """obs u8 [N, 4, 84, 84] -> Q values [N, A]"""
@@ -263,6 +292,7 @@ class ApexHParams:
     quantile_dqn: bool = False           # the quantile (QR-DQN) head q = Linear(512, A num_quantiles) and the quantile Huber loss
     num_quantiles: int = 200             # N, the paper's Atari setting
     quantile_kappa: float = 1.0          # the Huber threshold kappa > 0 (1: QR-DQN-1)
+    distributional_dueling: bool = False  # Rainbow's dueling head per atom / quantile (with categorical_dqn or quantile_dqn)
     optimizer: ClassVar[str] = 'adam'            # read by learner.py's optimizer-state converters
     lr_schedule: ClassVar[str] = 'constant'
 
@@ -294,7 +324,7 @@ class ApexHParams:
     def head(self) -> 'QHead':
         """the Q head these settings describe (ValueError on a bad one)"""
         return QHead.of(self.dueling_dqn, self.categorical_dqn, self.num_atoms, self.v_min, self.v_max, self.noisy_dqn, self.quantile_dqn,
-                        self.num_quantiles, self.quantile_kappa)
+                        self.num_quantiles, self.quantile_kappa, self.distributional_dueling)
 
     def to_c(self) -> _lib.SrlApexConfig:
         self.validate()
@@ -312,6 +342,7 @@ class ApexHParams:
         c.noisy = 1 if self.noisy_dqn else 0
         c.num_quantiles = self.quantiles()
         c.kappa = self.quantile_kappa
+        c.dist_dueling = 1 if self.distributional_dueling else 0
         return c
 
     def atoms(self) -> int:
@@ -327,8 +358,8 @@ class ApexHParams:
 class QHead:
     """The Q head of the learner and its actors: q = Linear(512, A), the dueling head (``dueling``), the categorical head on
     ``num_atoms`` > 0 atoms of the support [v_min, v_max], or the quantile head on ``num_quantiles`` > 0 quantiles with the Huber
-    threshold ``kappa``; ``noisy``: fc and the head layers are noisy layers.  A head keeps no setting of another kind, so equal heads
-    compare equal."""
+    threshold ``kappa``; ``noisy``: fc and the head layers are noisy layers; ``dist_dueling``: the categorical or quantile head as
+    Rainbow's dueling rows.  A head keeps no setting of another kind, so equal heads compare equal."""
     dueling: bool = False
     num_atoms: int = 0
     v_min: float = 0.0
@@ -336,10 +367,11 @@ class QHead:
     noisy: bool = False
     num_quantiles: int = 0
     kappa: float = 0.0
+    dist_dueling: bool = False
 
     @classmethod
     def of(cls, dueling_dqn, categorical_dqn, num_atoms, v_min, v_max, noisy_dqn=False, quantile_dqn=False, num_quantiles=200,
-           quantile_kappa=1.0) -> 'QHead':
+           quantile_kappa=1.0, distributional_dueling=False) -> 'QHead':
         """the head of ApexHParams' / B200ApexActor's settings, checked (the support and the quantile setting, as the kernels read
         them in fp32, even when their head is off)"""
         if not isinstance(dueling_dqn, bool):
@@ -369,25 +401,35 @@ class QHead:
             raise ValueError('quantile_dqn with dueling_dqn is not supported: choose one head')
         if quantile_dqn and categorical_dqn:
             raise ValueError('quantile_dqn with categorical_dqn is not supported: choose one head')
+        if not isinstance(distributional_dueling, bool):
+            raise ValueError(f'distributional_dueling must be a bool, got {distributional_dueling!r}')
+        if distributional_dueling and dueling_dqn:
+            raise ValueError('distributional_dueling with dueling_dqn is not supported: dueling_dqn is the scalar dueling head')
+        if distributional_dueling and not (categorical_dqn or quantile_dqn):
+            raise ValueError('distributional_dueling needs categorical_dqn or quantile_dqn')
         if quantile_dqn:
-            return cls(noisy=noisy_dqn, num_quantiles=int(num_quantiles), kappa=float(quantile_kappa))
-        return cls(False, int(num_atoms), float(v_min), float(v_max), noisy_dqn) if categorical_dqn else cls(dueling_dqn, noisy=noisy_dqn)
+            return cls(noisy=noisy_dqn, num_quantiles=int(num_quantiles), kappa=float(quantile_kappa), dist_dueling=distributional_dueling)
+        if categorical_dqn:
+            return cls(False, int(num_atoms), float(v_min), float(v_max), noisy_dqn, dist_dueling=distributional_dueling)
+        return cls(dueling_dqn, noisy=noisy_dqn)
 
     def __str__(self):
         s = f'dueling_dqn={self.dueling}, categorical_dqn={self.num_atoms > 0}, noisy_dqn={self.noisy}'
         if self.num_quantiles:
-            return s + f', quantile_dqn=True, (num_quantiles, quantile_kappa)={(self.num_quantiles, self.kappa)}'
-        return s + f', (num_atoms, v_min, v_max)={(self.num_atoms, self.v_min, self.v_max)}' if self.num_atoms else s
+            s += f', quantile_dqn=True, (num_quantiles, quantile_kappa)={(self.num_quantiles, self.kappa)}'
+        elif self.num_atoms:
+            s += f', (num_atoms, v_min, v_max)={(self.num_atoms, self.v_min, self.v_max)}'
+        return s + ', distributional_dueling=True' if self.dist_dueling else s
 
     def names(self):
-        return apex_param_names(self.dueling, self.noisy)
+        return apex_param_names(self.dueling or self.dist_dueling, self.noisy)
 
     def shapes(self, num_actions: int):
-        return apex_param_shapes(num_actions, self.dueling, self.num_atoms, self.noisy, self.num_quantiles)
+        return apex_param_shapes(num_actions, self.dueling, self.num_atoms, self.noisy, self.num_quantiles, self.dist_dueling)
 
     def layout(self, num_actions: int):
         """(total floats, offsets, counts) of the flat buffer"""
-        return _lib.apex_param_layout(num_actions, self.dueling, self.num_atoms, self.noisy, self.num_quantiles)
+        return _lib.apex_param_layout(num_actions, self.dueling, self.num_atoms, self.noisy, self.num_quantiles, self.dist_dueling)
 
 
 def flat_views(flat: torch.Tensor, off, cnt, shapes) -> 'OrderedDict[str, torch.Tensor]':
@@ -406,13 +448,14 @@ def load_views(dst: Dict[str, torch.Tensor], sd: Dict[str, torch.Tensor]) -> Non
 
 
 def default_q_state_dict(num_actions: int, seed: int = 0, dueling: bool = False, num_atoms: int = 0, noisy: bool = False,
-                         noisy_std: float = 0.5, num_quantiles: int = 0) -> 'OrderedDict[str, torch.Tensor]':
+                         noisy_std: float = 0.5, num_quantiles: int = 0, dist_dueling: bool = False) -> 'OrderedDict[str, torch.Tensor]':
     """AtariQNet's initial weights under ``torch.manual_seed(seed)``, drawn without disturbing the global RNG (num_atoms > 0: the
-    categorical head's; num_quantiles > 0: the quantile head's; noisy: the noisy network's with sigma0 = noisy_std)"""
+    categorical head's; num_quantiles > 0: the quantile head's; dist_dueling: either as dueling rows; noisy: the noisy network's with
+    sigma0 = noisy_std)"""
     with torch.random.fork_rng(devices=[]):
         torch.manual_seed(seed)
         net = AtariQNet(num_actions, dueling=dueling, categorical=num_atoms > 0, num_atoms=num_atoms or 51, noisy=noisy, noisy_std=noisy_std,
-                        quantile=num_quantiles > 0, num_quantiles=num_quantiles or 200)
+                        quantile=num_quantiles > 0, num_quantiles=num_quantiles or 200, distributional_dueling=dist_dueling)
     return OrderedDict((k, v.detach().clone()) for k, v in net.state_dict().items())
 
 
@@ -453,8 +496,8 @@ class B200ApexLearner(BaseAgent):
                                                        C.byref(h)), 'srl_apex_learner_create')
             self._h = h
             self._stats = torch.zeros(4, device=self.device)      # {loss, gradient norm, clip coefficient, pad}
-        sd = default_q_state_dict(hp.num_actions, seed, head.dueling, head.num_atoms, head.noisy, hp.noisy_std, head.num_quantiles) \
-            if init_state_dict is None else init_state_dict
+        sd = default_q_state_dict(hp.num_actions, seed, head.dueling, head.num_atoms, head.noisy, hp.noisy_std, head.num_quantiles,
+                                  head.dist_dueling) if init_state_dict is None else init_state_dict
         self.load_state_dict(sd)
         self.load_state_dict(sd, target=True)       # actor_target starts as a copy (dqn_agent.py:66-67)
         self.use_graph = use_graph
@@ -492,7 +535,7 @@ class B200ApexLearner(BaseAgent):
 
     def optimizer_state_dict(self) -> dict:
         """``torch.optim.Adam(AtariQNet(A, dueling=hp.dueling_dqn, categorical=hp.categorical_dqn, noisy=hp.noisy_dqn,
-        quantile=hp.quantile_dqn, ...).parameters()).state_dict()`` layout"""
+        quantile=hp.quantile_dqn, distributional_dueling=hp.distributional_dueling, ...).parameters()).state_dict()`` layout"""
         return to_torch_optimizer_state(self.hp, self._opt_tensors(), self._opt_steps, order=self.names)
 
     def load_optimizer_state_dict(self, sd: dict) -> None:

@@ -10,7 +10,8 @@
 //   apex_cat_priority_kernel  the same on the categorical head: the learner tail's cat_transition
 //   apex_qr_priority_kernel   the same on the quantile head: the learner tail's qr_transition
 // The categorical and quantile heads run the learner's logits GEMM (dqn_cat.cu) first.  launch_apex_act and launch_apex_priorities are the one
-// place that picks the kernels of a head.
+// place that picks the kernels of a head.  The distributional dueling head composes its rows from the snapshot first (dueling_rows.cu), as
+// the learner does, and then is the categorical or quantile head on them.
 #include <math.h>
 #include <string.h>
 #include <new>
@@ -187,6 +188,7 @@ struct srl_apex_actor {
   float *normals, *noise;
   unsigned long long* noise_draws;
   NoisyWeights cw;
+  HeadRows rows;                   // the distributional dueling head: the rows the last call composed
   char* arena;
 };
 
@@ -204,20 +206,29 @@ int actor_rows(srl_apex_actor* X, int64_t saved, int64_t scratch, WsRow* t) {
   t[n++] = ws_row(nullptr, head_has_logits(X->desc.head) ? 2 * E * X->desc.head.R : 0, &X->logits);
   t[n++] = ws_row(nullptr, X->desc.noisy, &X->noise_draws);
   n += noise_rows(X->desc, 0, &X->normals, &X->noise, &X->cw, t + n);
+  const int64_t DR = dist_dueling(X->desc) ? X->desc.head.R : 0;
+  t[n++] = ws_row("rows_weight", DR * 512, &X->rows.W);
+  t[n++] = ws_row("rows_bias", DR, &X->rows.b);
   return n;
 }
-constexpr int ACTOR_ROWS = 16;
+constexpr int ACTOR_ROWS = 18;
 
-// a noisy actor's weights for its next forwards: a new draw first when `draw` (act), then the composition of the kept draw with the
-// snapshot as it is now.  Nothing without noise.
-cudaError_t actor_noise(srl_apex_actor* X, bool draw, cudaStream_t st) {
-  if (!X->desc.noisy) return cudaSuccess;
-  if (draw) {
-    const cudaError_t e = launch_noisy_draw(X->key, nullptr, X->noise_draws, 1, noise_count(X->desc), &X->normals, &X->noise, st);
+// the head of the actor's next forwards, from the snapshot as it is now: a noisy actor draws new noise first when `draw` (act) and
+// composes the kept draw with the snapshot; the distributional dueling head composes its rows from those weights -> *h
+cudaError_t actor_head(srl_apex_actor* X, bool draw, cudaStream_t st, QHead* h) {
+  *h = X->run.q;
+  if (X->desc.noisy) {
+    if (draw) {
+      const cudaError_t e = launch_noisy_draw(X->key, nullptr, X->noise_draws, 1, noise_count(X->desc), &X->normals, &X->noise, st);
+      if (e != cudaSuccess) return e;
+    }
+    const float* noise = X->noise;
+    const cudaError_t e = launch_noisy_compose(&X->snap.nz, &X->cw, &noise, 1, X->desc, st);
     if (e != cudaSuccess) return e;
   }
-  const float* noise = X->noise;
-  return launch_noisy_compose(&X->snap.nz, &X->cw, &noise, 1, X->desc.head, st);
+  if (!dist_dueling(X->desc)) return cudaSuccess;
+  *h = on_rows(*h, X->rows);
+  return launch_dist_dueling_compose(&X->run.q, &X->rows, 1, X->desc.vrows, st);
 }
 
 // Q head rows of `frames` frames of obs into core (f <= E frames per call)
@@ -248,11 +259,18 @@ extern "C" int srl_apex_actor_create_noisy(int A, int num_envs, int precision, i
 extern "C" int srl_apex_actor_create_quantile(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max,
                                               int num_quantiles, float kappa, int noisy, uint64_t seed, const float* params,
                                               srl_apex_actor_t** out) {
+  return srl_apex_actor_create_dist_dueling(A, num_envs, precision, dueling, num_atoms, v_min, v_max, num_quantiles, kappa, 0, noisy, seed,
+                                            params, out);
+}
+
+extern "C" int srl_apex_actor_create_dist_dueling(int A, int num_envs, int precision, int dueling, int num_atoms, float v_min, float v_max,
+                                                  int num_quantiles, float kappa, int dist_dueling, int noisy, uint64_t seed,
+                                                  const float* params, srl_apex_actor_t** out) {
   REQ(params && out, "apex_actor_create: NULL argument");
   REQ(num_envs >= 1 && num_envs <= MAX_FRAMES, "apex_actor_create: num_envs=%d must be in [1, %d]", num_envs, MAX_FRAMES);
   REQ(precision == 0 || precision == 1, "apex_actor_create: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)", precision);
   ApexNetDesc d;
-  int rc = make_apex_desc("apex_actor_create", A, dueling, num_atoms, v_min, v_max, num_quantiles, kappa, noisy, &d);
+  int rc = make_apex_desc("apex_actor_create", A, dueling, num_atoms, v_min, v_max, num_quantiles, kappa, dist_dueling, noisy, &d);
   if (rc) return rc;
   REQ(!misaligned(params, 16), "apex_actor_create: params must be 16-byte aligned");
   int64_t sb = 0, kb = 0;
@@ -301,10 +319,11 @@ extern "C" int srl_apex_actor_act(srl_apex_actor_t* X, const uint8_t* obs, const
   int rc = check_spans(s, 3, "apex_actor_act");
   if (rc) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
-  CU(actor_noise(X, true, st), "apex_actor_act: noise");
+  QHead h;
+  CU(actor_head(X, true, st, &h), "apex_actor_act: head");
   rc = actor_forward(X, obs, E, X->core, st);
   if (rc) return rc;
-  CU(launch_apex_act(X->run.q, X->core, X->logits, E, epsilons, X->key, X->draws, actions, st), "apex_act");
+  CU(launch_apex_act(h, X->core, X->logits, E, epsilons, X->key, X->draws, actions, st), "apex_act");
   return 0;
 }
 
@@ -316,12 +335,13 @@ extern "C" int srl_apex_actor_q_values(srl_apex_actor_t* X, const uint8_t* obs, 
   int rc = check_spans(s, 2, "apex_actor_q_values");
   if (rc) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
-  CU(actor_noise(X, false, st), "apex_actor_q_values: noise");
+  QHead h;
+  CU(actor_head(X, false, st, &h), "apex_actor_q_values: head");
   for (int f0 = 0; f0 < n; f0 += X->E) {        // chunks of at most E frames: the blocks' size
     const int f = n - f0 < X->E ? n - f0 : X->E;
     rc = actor_forward(X, obs + (size_t)f0 * ACTOR_OBS_BYTES, f, X->core, st);
     if (rc) return rc;
-    CU(launch_q_values(X->run.q, X->core, f, X->logits, q_out + (size_t)f0 * A, st), "q_values");
+    CU(launch_q_values(h, X->core, f, X->logits, q_out + (size_t)f0 * A, st), "q_values");
   }
   return 0;
 }
@@ -351,11 +371,12 @@ int apex_actor_num_envs(const srl_apex_actor* X) { return X->E; }
 int apex_actor_priorities(srl_apex_actor* X, const uint8_t* s, const uint8_t* s_next, const int64_t* action, const float* reward,
                           const uint8_t* done, int64_t ptr, int64_t M, float gamma_n, float eps, const double** prio, cudaStream_t st) {
   const int E = X->E;
-  CU(actor_noise(X, false, st), "apex_actor_priorities: noise");
+  QHead h;
+  CU(actor_head(X, false, st, &h), "apex_actor_priorities: head");
   int rc = actor_forward(X, s, E, X->core, st);
   if (!rc) rc = actor_forward(X, s_next, E, X->core + (size_t)E * ENC_CORE, st);
   if (rc) return rc;
-  CU(launch_apex_priorities(X->run.q, X->core, X->logits, E, action, reward, done, ptr, M, gamma_n, eps, X->prio, st), "apex_priorities");
+  CU(launch_apex_priorities(h, X->core, X->logits, E, action, reward, done, ptr, M, gamma_n, eps, X->prio, st), "apex_priorities");
   *prio = X->prio;
   return 0;
 }

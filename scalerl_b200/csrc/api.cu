@@ -904,12 +904,13 @@ extern "C" int srl_encoder_backward(srl_encoder_t* E, const float* dcore, int fr
 // and the head biases (plain: the weights first; noisy: the biases first); fc's weights.  So the dueling head's weight rows are one
 // [(A + 1)][512] block for the kernels (noisy: the mu rows one, the sigma rows another), the value row first.  The categorical head
 // (K atoms) is q with A K rows (row a K + k: atom k of action a), the quantile head (N quantiles) q with A N rows (row a N + i:
-// quantile i of action a).
+// quantile i of action a).  The distributional dueling head (W = K or N rows per action) has value [W, 512] and advantage [A W, 512]
+// in the dueling head's places: one [(W + A W)][512] weight block, the value rows first.
 namespace srl {
 int64_t apex_layout(const ApexNetDesc& d, int64_t* off, int64_t* cnt) {
-  const bool dueling = d.head.kind == Q_DUELING;
-  const int64_t layers[6][2] = {{32, 256}, {64, 512}, {64, 576}, {512, 3136}, {dueling ? 1 : d.head.R, 512}, {d.head.A, 512}};  // [out, in]
-  const int nl = dueling ? 6 : 5, S = d.noisy ? 2 : 1;
+  const int64_t V = d.vrows, R = adv_rows(d);
+  const int64_t layers[6][2] = {{32, 256}, {64, 512}, {64, 576}, {512, 3136}, {V ? V : R, 512}, {R, 512}};  // [out, in]
+  const int nl = V ? 6 : 5, S = d.noisy ? 2 : 1;
   // the memory group of [conv, fc, head][weight, bias], without and with noise
   static const int group[2][3][2] = {{{0, 0}, {4, 1}, {2, 3}}, {{0, 0}, {4, 1}, {3, 2}}};
   int64_t o = 0;
@@ -930,16 +931,22 @@ int64_t apex_layout(const ApexNetDesc& d, int64_t* off, int64_t* cnt) {
   return o;
 }
 
-int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int num_quantiles, float kappa, int noisy,
-                   ApexNetDesc* d) {
+int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int num_quantiles, float kappa,
+                   int dist_dueling, int noisy, ApexNetDesc* d) {
   REQ(A >= 1 && A <= 31, "%s: A=%d must be in [1,31]", who, A);
   REQ(dueling == 0 || dueling == 1, "%s: dueling=%d must be 0 (q = Linear(512, A)) or 1 (dueling head)", who, dueling);
   REQ(noisy == 0 || noisy == 1, "%s: noisy=%d must be 0 (plain layers) or 1 (noisy fc and head layers)", who, noisy);
+  REQ(dist_dueling == 0 || dist_dueling == 1, "%s: dist_dueling=%d must be 0 or 1 (the distributional dueling head)", who, dist_dueling);
+  if (dist_dueling) {
+    REQ(dueling == 0, "%s: dist_dueling=1 with dueling=1 is not supported (dueling is the scalar dueling head)", who);
+    REQ(num_atoms > 0 || num_quantiles > 0, "%s: dist_dueling=1 needs the categorical head (num_atoms > 0) or the quantile head "
+        "(num_quantiles > 0)", who);
+  }
   REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "%s: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]", who,
       num_atoms, CAT_MAX_ATOMS);
   REQ(num_quantiles == 0 || (num_quantiles >= 2 && num_quantiles <= QR_MAX_QUANTILES),
       "%s: num_quantiles=%d must be 0 (no quantile head) or in [2, %d]", who, num_quantiles, QR_MAX_QUANTILES);
-  *d = ApexNetDesc{QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling}, noisy};
+  *d = ApexNetDesc{QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling}, noisy, dueling};
   if (num_quantiles) {
     REQ(std::isfinite(kappa) && kappa > 0.f, "%s: kappa=%g must be finite and > 0 (the quantile Huber threshold)", who, (double)kappa);
     REQ(dueling == 0, "%s: the quantile head (num_quantiles=%d) with dueling=1 is not supported", who, num_quantiles);
@@ -948,6 +955,7 @@ int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_m
     d->head.kind = Q_QUANTILE;
     d->head.R = A * num_quantiles;
     d->head.qr = QrSetting{num_quantiles, kappa};
+    d->vrows = dist_dueling ? num_quantiles : 0;
     return 0;
   }
   if (num_atoms == 0) return 0;
@@ -960,6 +968,7 @@ int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_m
   d->head.kind = Q_CATEGORICAL;
   d->head.R = A * num_atoms;
   d->head.c = c;
+  d->vrows = dist_dueling ? num_atoms : 0;
   return 0;
 }
 
@@ -967,7 +976,7 @@ ApexNet bind_apex(const ApexNetDesc& d, float* base) {
   int64_t off[18];
   apex_layout(d, off, nullptr);
   auto at = [&](int t) { return base + off[t]; };
-  const bool dueling = d.head.kind == Q_DUELING;
+  const bool dueling = d.vrows > 0;         // a value layer before the advantage layer
   const int S = d.noisy ? 2 : 1, F = 6, H = F + 2 * S, V = H + 2 * S;     // the first tensor of fc, the head, the advantage layer
   ApexNet n = {};
   for (int i = 0; i < 6; ++i) n.w8[i] = at(i);
@@ -991,7 +1000,7 @@ ApexNet apex_forward_net(const ApexNetDesc& d, const ApexNet& net, const NoisyWe
   ApexNet r = net;
   r.w8[6] = w.fc_w;
   r.w8[7] = w.fc_b;
-  r.q.W = w.h_w; r.q.b = w.h_b; r.q.ba = d.head.kind == Q_DUELING ? w.h_ba : nullptr;
+  r.q.W = w.h_w; r.q.b = w.h_b; r.q.ba = d.vrows ? w.h_ba : nullptr;
   return r;
 }
 
@@ -1001,39 +1010,43 @@ int noise_rows(const ApexNetDesc& d, int which, float** normals, float** noise, 
       {"normals_online", "noise_online", "fc_weight_online", "fc_bias_online", "head_weight_online", "head_bias_online", "head_adv_bias_online"},
       {"normals_target", "noise_target", "fc_weight_target", "fc_bias_target", "head_weight_target", "head_bias_target", "head_adv_bias_target"}};
   const char* const* nm = names[which];
-  const int64_t on = d.noisy, R = d.head.R, dueling = d.head.kind == Q_DUELING;
+  const int64_t on = d.noisy, V = d.vrows, R = adv_rows(d);
   t[0] = ws_row(nm[0], noise_count(d), normals);
   t[1] = ws_row(nm[1], noise_count(d), noise);
   t[2] = ws_row(nm[2], on * NOISE_FC_OUT * NOISE_FC_IN, &w->fc_w);
   t[3] = ws_row(nm[3], on * NOISE_FC_OUT, &w->fc_b);
-  t[4] = ws_row(nm[4], on * R * NOISE_HEAD_IN, &w->h_w);
-  t[5] = ws_row(nm[5], on * (dueling ? 1 : R), &w->h_b);
-  t[6] = ws_row(nm[6], on * dueling * d.head.A, &w->h_ba);
+  t[4] = ws_row(nm[4], on * (V + R) * NOISE_HEAD_IN, &w->h_w);
+  t[5] = ws_row(nm[5], on * (V ? V : R), &w->h_b);
+  t[6] = ws_row(nm[6], on * (V ? R : 0), &w->h_ba);
   return 7;
 }
 }  // namespace srl
 
 extern "C" int64_t srl_apex_param_layout(int A, int64_t* offsets10, int64_t* counts10) {
-  return apex_layout(ApexNetDesc{QHead{Q_PLAIN, A, A}, 0}, offsets10, counts10);
+  return apex_layout(ApexNetDesc{QHead{Q_PLAIN, A, A}, 0, 0}, offsets10, counts10);
 }
 extern "C" int64_t srl_apex_param_layout_ex(int A, int dueling, int64_t* offsets12, int64_t* counts12) {
   REQ(A >= 1 && A <= 31, "apex_param_layout: A=%d must be in [1,31]", A);
   REQ(dueling == 0 || dueling == 1, "apex_param_layout: dueling=%d must be 0 or 1", dueling);
-  return apex_layout(ApexNetDesc{QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling}, 0}, offsets12, counts12);
+  return apex_layout(ApexNetDesc{QHead{dueling ? Q_DUELING : Q_PLAIN, A, A + dueling}, 0, dueling}, offsets12, counts12);
 }
 extern "C" int64_t srl_apex_param_layout_cat(int A, int num_atoms, int64_t* offsets10, int64_t* counts10) {
   REQ(A >= 1 && A <= 31, "apex_param_layout: A=%d must be in [1,31]", A);
   REQ(num_atoms == 0 || (num_atoms >= 2 && num_atoms <= CAT_MAX_ATOMS), "apex_param_layout: num_atoms=%d must be 0 (a scalar Q head) or in [2, %d]",
       num_atoms, CAT_MAX_ATOMS);
-  return apex_layout(ApexNetDesc{QHead{num_atoms ? Q_CATEGORICAL : Q_PLAIN, A, A * (num_atoms ? num_atoms : 1)}, 0}, offsets10, counts10);
+  return apex_layout(ApexNetDesc{QHead{num_atoms ? Q_CATEGORICAL : Q_PLAIN, A, A * (num_atoms ? num_atoms : 1)}, 0, 0}, offsets10, counts10);
 }
 extern "C" int64_t srl_apex_param_layout_noisy(int A, int dueling, int num_atoms, int noisy, int64_t* offsets18, int64_t* counts18) {
   return srl_apex_param_layout_quantile(A, dueling, num_atoms, 0, noisy, offsets18, counts18);
 }
 extern "C" int64_t srl_apex_param_layout_quantile(int A, int dueling, int num_atoms, int num_quantiles, int noisy, int64_t* offsets18,
                                                   int64_t* counts18) {
+  return srl_apex_param_layout_dist_dueling(A, dueling, num_atoms, num_quantiles, 0, noisy, offsets18, counts18);
+}
+extern "C" int64_t srl_apex_param_layout_dist_dueling(int A, int dueling, int num_atoms, int num_quantiles, int dist_dueling, int noisy,
+                                                      int64_t* offsets18, int64_t* counts18) {
   ApexNetDesc d;      // the support and kappa do not shape the layout
-  if (make_apex_desc("apex_param_layout", A, dueling, num_atoms, 0.f, 1.f, num_quantiles, 1.f, noisy, &d)) return -1;
+  if (make_apex_desc("apex_param_layout", A, dueling, num_atoms, 0.f, 1.f, num_quantiles, 1.f, dist_dueling, noisy, &d)) return -1;
   return apex_layout(d, offsets18, counts18);
 }
 
@@ -1060,6 +1073,9 @@ struct srl_apex_learner {
   float *normals[2], *noise[2];
   NoisyWeights cw[2];
   uint2 noise_key;
+  // the distributional dueling head: the rows the kernels read, composed for the step's online and target forwards ([0], [1]), their
+  // gradients ([2]) and the q-value forwards' own
+  HeadRows rows[3], rows_q;
   char* arena;
 };
 
@@ -1109,9 +1125,18 @@ static int apex_rows(srl_apex_learner* L, const int64_t* b4, WsRow* t) {
   t[n++] = ws_row(qr ? "qr_loss" : "ce", B * (K ? 1 : 0), &L->ce);
   t[n++] = ws_row(nullptr, QC * R, &L->logits_q);
   for (int i = 0; i < 2; ++i) n += noise_rows(L->desc, 1 + i, &L->normals[i], &L->noise[i], &L->cw[i], t + n);
+  const int64_t DR = dist_dueling(L->desc) ? R : 0;
+  static const char* const rows_names[3][2] = {{"rows_weight_online", "rows_bias_online"}, {"rows_weight_target", "rows_bias_target"},
+                                               {"rows_weight_grad", "rows_bias_grad"}};
+  for (int i = 0; i < 3; ++i) {
+    t[n++] = ws_row(rows_names[i][0], DR * 512, &L->rows[i].W);
+    t[n++] = ws_row(rows_names[i][1], DR, &L->rows[i].b);
+  }
+  t[n++] = ws_row(nullptr, DR * 512, &L->rows_q.W);
+  t[n++] = ws_row(nullptr, DR, &L->rows_q.b);
   return n;
 }
-constexpr int APEX_ROWS = 43;
+constexpr int APEX_ROWS = 51;
 
 // -> the network of a valid config
 static int check_apex_cfg(const srl_apex_config_t* c, ApexNetDesc* d) {
@@ -1125,7 +1150,8 @@ static int check_apex_cfg(const srl_apex_config_t* c, ApexNetDesc* d) {
   REQ(c->adam_beta1 >= 0.f && c->adam_beta1 < 1.f && c->adam_beta2 >= 0.f && c->adam_beta2 < 1.f, "apex_learner: Adam betas must be in [0, 1)");
   REQ(std::isfinite(c->adam_eps) && c->adam_eps >= 0.f, "apex_learner: adam_eps=%g must be finite and >= 0", (double)c->adam_eps);
   REQ(std::isfinite(c->priority_eps) && c->priority_eps >= 0.f, "apex_learner: priority_eps=%g must be finite and >= 0", (double)c->priority_eps);
-  return make_apex_desc("apex_learner", c->A, c->dueling, c->num_atoms, c->v_min, c->v_max, c->num_quantiles, c->kappa, c->noisy, d);
+  return make_apex_desc("apex_learner", c->A, c->dueling, c->num_atoms, c->v_min, c->v_max, c->num_quantiles, c->kappa, c->dist_dueling,
+                        c->noisy, d);
 }
 
 extern "C" int srl_apex_learner_create(const srl_apex_config_t* cfg, float* params, float* grads, float* exp_avg, float* exp_avg_sq,
@@ -1188,7 +1214,19 @@ extern "C" int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, 
     CU(launch_noisy_draw(L->noise_key, L->dstep, nullptr, 2, noise_count(L->desc), L->normals, L->noise, st), "noisy_draw");
     const float* noise[2] = {L->noise[0], L->noise[1]};
     const NoisyTensors nz[2] = {L->net[0].nz, L->net[1].nz};
-    CU(launch_noisy_compose(nz, L->cw, noise, 2, L->desc.head, st), "noisy_compose");
+    CU(launch_noisy_compose(nz, L->cw, noise, 2, L->desc, st), "noisy_compose");
+  }
+  // the heads the tail reads and the gradients q_wgrad writes: the distributional dueling head's composed rows (the target's from
+  // target_params as they are now, so an update of them between replays is seen) and their gradients
+  QHead head_on = L->run[0].q, head_tg = L->run[1].q;
+  QHeadGrad head_g = L->net[2].g;
+  const bool dd = dist_dueling(L->desc);
+  if (dd) {
+    const QHead p[2] = {head_on, head_tg};
+    CU(launch_dist_dueling_compose(p, L->rows, 2, L->desc.vrows, st), "dist_dueling_compose");
+    head_on = on_rows(head_on, L->rows[0]);
+    head_tg = on_rows(head_tg, L->rows[1]);
+    head_g = QHeadGrad{L->rows[2].W, L->rows[2].b, nullptr};
   }
   // the three forwards (the encoder checks obs / next_obs and the blocks); the target forward runs last so that its rows are the
   // ones left in saved_n
@@ -1200,12 +1238,13 @@ extern "C" int srl_apex_learner_step(srl_apex_learner_t* L, const uint8_t* obs, 
   const QTail t = {L->core_s, c.double_dqn ? L->core_n : nullptr, L->core_nt, action, reward, done, weights, B, c.gamma, c.priority_eps,
                    L->q, L->y, L->dcore, L->loss, L->tail_scratch, L->prio, L->dq, L->head_part, L->logits_s, L->logits_n, L->logits_nt,
                    L->mproj, L->ce, L->dlogits};
-  CU(launch_q_tail(on.q, tg.q, t, st), "q_tail");
-  CU(launch_q_wgrad(on.q, L->net[2].g, t, st), "q_wgrad");
+  CU(launch_q_tail(head_on, head_tg, t, st), "q_tail");
+  CU(launch_q_wgrad(head_on, head_g, t, st), "q_wgrad");
+  if (dd) CU(launch_dist_dueling_grad(L->rows[2], L->net[2].g, c.A, L->desc.vrows, st), "dist_dueling_grad");
   // the gradients of the composed weights land in the mu segments
   rc = srl_encoder_backward(L->E, L->dcore, B, 1, L->saved_s, L->enc_scratch, L->net[2].w8, stream);
   if (rc) return rc;
-  if (L->desc.noisy) CU(launch_noisy_sigma_grad(L->net[2].nz, L->noise[0], L->desc.head, st), "noisy_sigma_grad");
+  if (L->desc.noisy) CU(launch_noisy_sigma_grad(L->net[2].nz, L->noise[0], L->desc, st), "noisy_sigma_grad");
   const OptStep o = {1, L->params, L->grads, L->m, L->v, L->nparams, c.max_grad_norm, L->coef, L->opt_scratch, c.learning_rate,
                      c.adam_beta1, c.adam_beta2, c.adam_eps, 0, L->dstep, OptExtra{}};
   CU(launch_clip_optim(o, st), "clip+adam");
@@ -1243,12 +1282,17 @@ extern "C" int srl_apex_learner_q_values(srl_apex_learner_t* L, const uint8_t* o
   const Span s[2] = {{obs, (int64_t)n * 28224, false, "obs"}, {q_out, (int64_t)n * A * 4, true, "q_out"}};
   int rc = check_spans(s, 2, "apex_learner_q_values");
   if (rc) return rc;
+  QHead head = L->net[0].q;
+  if (dist_dueling(L->desc)) {                // composed into the q-value forwards' own rows: the step's may be in use on another stream
+    CU(launch_dist_dueling_compose(&head, &L->rows_q, 1, L->desc.vrows, (cudaStream_t)stream), "dist_dueling_compose");
+    head = on_rows(head, L->rows_q);
+  }
   for (int f0 = 0; f0 < n; f0 += QC) {       // chunks through the q-value forwards' own context and blocks
     const int f = n - f0 < QC ? n - f0 : QC;
     rc = srl_encoder_forward(L->Eq, obs + (size_t)f0 * 28224, L->zero_reward, L->zero_action, f, 1, L->net[0].w8, L->saved_q, L->scratch_q,
                              L->core_q, stream);
     if (rc) return rc;
-    CU(launch_q_values(L->net[0].q, L->core_q, f, L->logits_q, q_out + (size_t)f0 * A, (cudaStream_t)stream), "q_values");
+    CU(launch_q_values(head, L->core_q, f, L->logits_q, q_out + (size_t)f0 * A, (cudaStream_t)stream), "q_values");
   }
   return 0;
 }

@@ -245,7 +245,8 @@ enum QKind { Q_PLAIN, Q_DUELING, Q_CATEGORICAL, Q_QUANTILE };
 //                  a) on the support c
 //   Q_QUANTILE     QR-DQN, q = Linear(512, A N) (dqn_qr.cuh): W = q.weight [A N][512], b = q.bias [A N] (row a N + i: quantile i of
 //                  action a), with the setting qr
-// R = W's rows: A, A + 1, A K or A N.
+// R = W's rows: A, A + 1, A K or A N.  The distributional dueling head (ApexNetDesc.vrows) is a Q_CATEGORICAL or Q_QUANTILE head on
+// the composed rows of its value and advantage layers (dueling_rows.cu).
 struct QHead {
   QKind kind;
   int A, R;
@@ -289,11 +290,11 @@ cudaError_t launch_q_values(const QHead& h, const float* core, int N, float* log
 cudaError_t launch_apex_soft_update(const float* p, float* pt, int64_t n, float tau, float one_minus_tau, cudaStream_t st);
 // ---- noisy.cu: noisy networks (Fortunato et al. 2018, factorised Gaussian noise) on the fc layer and the Q head
 // One network's noise vector f(x) = sgn(x) sqrt|x| of standard normals x, nn = noise_count floats:
-//   [fc in 3136 | fc out 512 | head in 512 (dueling: the value layer's, then the advantage layer's) | head out R (dueling: value, then
-//   the A advantage rows)]; every segment but the last starts on a multiple of 4 floats.
+//   [fc in 3136 | fc out 512 | head in 512 (value and advantage layers: the value layer's, then the advantage layer's) | head out
+//   (the head's parameter rows: the value rows, then the advantage rows)]; every segment but the last starts on a multiple of 4 floats.
 constexpr int NOISE_FC_IN = 3136, NOISE_FC_OUT = 512, NOISE_HEAD_IN = 512, NOISE_HEAD_IN_OFF = NOISE_FC_IN + NOISE_FC_OUT;
 // the noisy layers' tensors on one flat buffer, [0] mu and [1] sigma (of the parameters, or of their gradients): the fc weight
-// [512][3136] and bias [512]; the head in QHead's layout: W [R][512], b and (dueling) ba
+// [512][3136] and bias [512]; the head's parameter rows: W [rows][512], b and (value and advantage layers) ba
 struct NoisyTensors {
   float *fc_w[2], *fc_b[2];
   float *h_w[2], *h_b[2], *h_ba[2];
@@ -307,24 +308,36 @@ struct NoisyWeights {
 // count, read only), or *draws (the actor's noise counter: nets = 1, advanced by one when the draw ends)
 cudaError_t launch_noisy_draw(uint2 key, const int* step, unsigned long long* draws, int nets, int nn, float* const* normals,
                               float* const* noise, cudaStream_t st);
-// w[i] = p[i]'s mu + sigma (.) (f(eps_out) f(eps_in)^T) and mu_b + sigma_b (.) f(eps_out) under noise[i], for the `nets` networks of head h
-cudaError_t launch_noisy_compose(const NoisyTensors* p, const NoisyWeights* w, const float* const* noise, int nets, const QHead& h,
+struct ApexNetDesc;
+// w[i] = p[i]'s mu + sigma (.) (f(eps_out) f(eps_in)^T) and mu_b + sigma_b (.) f(eps_out) under noise[i], for the `nets` networks of d
+cudaError_t launch_noisy_compose(const NoisyTensors* p, const NoisyWeights* w, const float* const* noise, int nets, const ApexNetDesc& d,
                                  cudaStream_t st);
 // the sigma gradients g.x[1] = g.x[0] (.) eps of the online network's noise (the mu gradients are those of the composed weights)
-cudaError_t launch_noisy_sigma_grad(const NoisyTensors& g, const float* noise, const QHead& h, cudaStream_t st);
+cudaError_t launch_noisy_sigma_grad(const NoisyTensors& g, const float* noise, const ApexNetDesc& d, cudaStream_t st);
 
-// The Ape-X Q network a setting describes: its head, unbound, and whether fc and the head layers are noisy (0 or 1)
+// The Ape-X Q network a setting describes: its head as the kernels read it, unbound, whether fc and the head layers are noisy (0 or 1),
+// and the head's value rows, the one place that decides the head's parameter rows: 0 (one layer, q), 1 (the scalar dueling head,
+// whose kernels read value and advantage themselves) or W = K or N (the distributional dueling head: value [W][512] and advantage
+// [A W][512], composed into the A W rows the head's kernels read)
 struct ApexNetDesc {
   QHead head;
   int noisy;
+  int vrows;
 };
+// the rows of the advantage layer (of q without a value layer)
+inline int adv_rows(const ApexNetDesc& d) { return d.head.kind == Q_DUELING ? d.head.A : d.head.R; }
+// the head's parameter rows: the value rows, then the advantage rows
+inline int param_rows(const ApexNetDesc& d) { return d.vrows + adv_rows(d); }
+// the distributional dueling head: the kernels read composed rows, not the parameters
+inline bool dist_dueling(const ApexNetDesc& d) { return d.vrows > 0 && d.head.kind != Q_DUELING; }
 // api.cu: the network of a setting (num_atoms 0: no categorical head, whose support is not read; num_quantiles 0: no quantile
-// head, whose kappa is not read).  0, or SRL_EINVAL with "<who>: ..." as the message
-int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int num_quantiles, float kappa, int noisy,
-                   ApexNetDesc* d);
+// head, whose kappa is not read; dist_dueling 1: that head as value and advantage layers).  0, or SRL_EINVAL with "<who>: ..." as the
+// message
+int make_apex_desc(const char* who, int A, int dueling, int num_atoms, float v_min, float v_max, int num_quantiles, float kappa,
+                   int dist_dueling, int noisy, ApexNetDesc* d);
 // the floats of one network's noise vector (0 without noise)
 inline int noise_count(const ApexNetDesc& d) {
-  return d.noisy ? NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (d.head.kind == Q_DUELING ? 2 : 1) + d.head.R : 0;
+  return d.noisy ? NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (d.vrows ? 2 : 1) + param_rows(d) : 0;
 }
 // api.cu: the flat parameter layout of network d (srl_apex_param_layout*'s): the offsets and counts (NULL: not wanted) of its
 // tensors in state_dict order (10, 12 dueling; noisy: 14, 18 dueling) -> the buffer's floats
@@ -341,6 +354,17 @@ struct ApexNet {
 ApexNet bind_apex(const ApexNetDesc& d, float* base);
 // the network a forward of `net` runs on: noisy, net's conv tensors with fc and the head from the composed weights w; else net
 ApexNet apex_forward_net(const ApexNetDesc& d, const ApexNet& net, const NoisyWeights& w);
+// ---- dueling_rows.cu: the distributional dueling head's rows W_eff [R][512], b_eff [R] (R = A W), or their gradients
+struct HeadRows {
+  float *W, *b;
+};
+// the head h reads on rows r
+inline QHead on_rows(QHead h, const HeadRows& r) { h.W = r.W; h.b = r.b; h.ba = nullptr; return h; }
+// rows[i] = (v + adv) - mean_a adv of p[i] (bound as the scalar dueling head: W = [value.weight; advantage.weight], b = value.bias,
+// ba = advantage.bias) for the `nets` networks, V = W rows per action
+cudaError_t launch_dist_dueling_compose(const QHead* p, const HeadRows* rows, int nets, int V, cudaStream_t st);
+// the value and advantage gradients (out: the parameter-side binding, stored) of the rows' gradients g
+cudaError_t launch_dist_dueling_grad(const HeadRows& g, const QHeadGrad& out, int A, int V, cudaStream_t st);
 // the rows of one network's normals, noise and composed weights (empty without noise), named with the suffix `which` (0: none,
 // 1: _online, 2: _target) -> the rows written
 int noise_rows(const ApexNetDesc& d, int which, float** normals, float** noise, NoisyWeights* w, WsRow* t);

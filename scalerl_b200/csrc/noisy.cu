@@ -15,24 +15,24 @@ namespace {
 
 constexpr uint32_t NOISE_TAG = 0x6E6F6973u;        // 'nois': keeps the noise counters apart from the actor's epsilon-greedy ones
 
-// row r of one network's noisy layers: fc rows 0 .. 511, then the head's R rows
+// row r of one network's noisy layers: fc rows 0 .. 511, then the head's parameter rows (V value rows first, when V > 0)
 struct NoisyRow {
   const float* fi;          // f(eps_in) of the row's layer
   float fo;                 // f(eps_out) of the row
   int n4;                   // float4s per row
   int64_t w;                // the row's first element in its weight tensor
-  int bias;                 // 0: fc bias, 1: head b, 2: head ba (dueling advantage biases)
+  int bias;                 // 0: fc bias, 1: head b, 2: head ba (the advantage biases)
   int b;                    // the row's index in that bias
 };
-SRL_DEVINL NoisyRow noisy_row(int r, int R, int dueling, const float* nz) {
+SRL_DEVINL NoisyRow noisy_row(int r, int V, const float* nz) {
   NoisyRow q;
   if (r < NOISE_FC_OUT) {
     q.fi = nz; q.fo = nz[NOISE_FC_IN + r]; q.n4 = NOISE_FC_IN / 4; q.w = (int64_t)r * NOISE_FC_IN; q.bias = 0; q.b = r;
   } else {
-    const int h = r - NOISE_FC_OUT, adv = dueling && h > 0;
+    const int h = r - NOISE_FC_OUT, two = V > 0, adv = two && h >= V;
     q.fi = nz + NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * adv;
-    q.fo = nz[NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (1 + dueling) + h];
-    q.n4 = NOISE_HEAD_IN / 4; q.w = (int64_t)h * NOISE_HEAD_IN; q.bias = adv ? 2 : 1; q.b = adv ? h - 1 : h;
+    q.fo = nz[NOISE_HEAD_IN_OFF + NOISE_HEAD_IN * (1 + two) + h];
+    q.n4 = NOISE_HEAD_IN / 4; q.w = (int64_t)h * NOISE_HEAD_IN; q.bias = adv ? 2 : 1; q.b = adv ? h - V : h;
   }
   return q;
 }
@@ -91,13 +91,13 @@ struct NoisyCompose {
   NoisyTensors p[2];
   NoisyWeights w[2];
   const float* noise[2];
-  int R, dueling;
+  int V;
 };
 // one block per (row, network): W row = mu + sigma eps over float4s, and the row's bias
 __global__ void __launch_bounds__(256) noisy_compose_kernel(const __grid_constant__ NoisyCompose a) {
   const int net = blockIdx.y;
   const NoisyTensors& p = a.p[net];
-  const NoisyRow q = noisy_row(blockIdx.x, a.R, a.dueling, a.noise[net]);
+  const NoisyRow q = noisy_row(blockIdx.x, a.V, a.noise[net]);
   const bool fc = q.bias == 0;
   const float4* __restrict__ mu = reinterpret_cast<const float4*>(noisy_w(p, 0, fc) + q.w);
   const float4* __restrict__ sg = reinterpret_cast<const float4*>(noisy_w(p, 1, fc) + q.w);
@@ -117,11 +117,11 @@ __global__ void __launch_bounds__(256) noisy_compose_kernel(const __grid_constan
 struct NoisySigmaGrad {
   NoisyTensors g;
   const float* noise;
-  int R, dueling;
+  int V;
 };
 // one block per row of the online network: dsigma = dmu (.) eps for the row's weights and its bias
 __global__ void __launch_bounds__(256) noisy_sigma_grad_kernel(const __grid_constant__ NoisySigmaGrad a) {
-  const NoisyRow q = noisy_row(blockIdx.x, a.R, a.dueling, a.noise);
+  const NoisyRow q = noisy_row(blockIdx.x, a.V, a.noise);
   const bool fc = q.bias == 0;
   const float4* __restrict__ gm = reinterpret_cast<const float4*>(noisy_w(a.g, 0, fc) + q.w);
   const float4* __restrict__ fi = reinterpret_cast<const float4*>(q.fi);
@@ -142,19 +142,18 @@ cudaError_t launch_noisy_draw(uint2 key, const int* step, unsigned long long* dr
   return cudaGetLastError();
 }
 
-cudaError_t launch_noisy_compose(const NoisyTensors* p, const NoisyWeights* w, const float* const* noise, int nets, const QHead& h,
+cudaError_t launch_noisy_compose(const NoisyTensors* p, const NoisyWeights* w, const float* const* noise, int nets, const ApexNetDesc& d,
                                  cudaStream_t st) {
   NoisyCompose a = {};
   for (int i = 0; i < nets; ++i) { a.p[i] = p[i]; a.w[i] = w[i]; a.noise[i] = noise[i]; }
-  a.R = h.R;
-  a.dueling = h.kind == Q_DUELING;
-  noisy_compose_kernel<<<dim3(NOISE_FC_OUT + h.R, nets), 256, 0, st>>>(a);
+  a.V = d.vrows;
+  noisy_compose_kernel<<<dim3(NOISE_FC_OUT + param_rows(d), nets), 256, 0, st>>>(a);
   return cudaGetLastError();
 }
 
-cudaError_t launch_noisy_sigma_grad(const NoisyTensors& g, const float* noise, const QHead& h, cudaStream_t st) {
-  const NoisySigmaGrad a = {g, noise, h.R, h.kind == Q_DUELING};
-  noisy_sigma_grad_kernel<<<NOISE_FC_OUT + h.R, 256, 0, st>>>(a);
+cudaError_t launch_noisy_sigma_grad(const NoisyTensors& g, const float* noise, const ApexNetDesc& d, cudaStream_t st) {
+  const NoisySigmaGrad a = {g, noise, d.vrows};
+  noisy_sigma_grad_kernel<<<NOISE_FC_OUT + param_rows(d), 256, 0, st>>>(a);
   return cudaGetLastError();
 }
 

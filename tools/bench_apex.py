@@ -13,9 +13,13 @@ with their FLOP rate against the fp32 data-sheet rate (67 TFLOP/s).  With --quan
 With --noisy it runs the noisy learner (ApexHParams(noisy_dqn=True)) beside the plain one, the torch statements run on AtariQNet(A, noisy=True) with reset_noise() on the online and target network every
 step, and a last line gives the noise kernels' times from torch.profiler at B = 512, A = 18 with the bytes they move against the HBM3
 data-sheet bandwidth (3.35 TB/s).
+With --dist-dueling it runs the categorical learner at K = --atoms and the quantile learners at each N of --quantiles, each beside
+itself with the distributional dueling rows (ApexHParams(distributional_dueling=True)), alternated in the same rounds (the torch
+statements stay the plain network's), and a last line per head gives the compose and decompose kernels' times from torch.profiler
+with the bytes they move against the HBM3 data-sheet bandwidth, at B = 512, A = 18 and at the largest head, A = 31, K = 64.
 
     python tools/bench_apex.py [--rounds 5] [--steps 50] [--configs 32x6,32x18,512x6,512x18] [--dueling | --categorical [--atoms 51] | --noisy |
-        --quantile [--quantiles 51,200]]
+        --quantile [--quantiles 51,200] | --dist-dueling [--atoms 51] [--quantiles 51,200]]
 """
 import argparse
 import json
@@ -223,6 +227,40 @@ def noisy_profile(B=512, A=18, steps=20):
             'noise_share_of_step': total / step_us}
 
 
+def dist_dueling_profile(kind, W, B=512, A=18, steps=20):
+    """the distributional dueling head's compose and decompose kernels in one captured learner step (torch.profiler over `steps`
+    replays): mean µs per step, the bytes each moves (from the shapes) and its share of the HBM3 data-sheet bandwidth"""
+    from torch.profiler import ProfilerActivity, profile
+    exp, w, idxs = batch(B, A)
+    head = dict(categorical_dqn=True, num_atoms=W, v_min=V_MIN, v_max=V_MAX) if kind == 'categorical' else dict(quantile_dqn=True, num_quantiles=W)
+    L, S = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, distributional_dueling=True, **head)), sampler()
+    step = lambda: L.learn(exp, weights=w, idxs=idxs, sampler=S, sync_stats=False)
+    for _ in range(3):
+        step()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            step()
+        torch.cuda.synchronize()
+    params, rows = 4 * (W + A * W) * 513, 4 * A * W * 513       # value and advantage weights and biases; the composed rows
+    nbytes = {'dist_dueling_compose_kernel': 2 * (params + rows),    # online and target: value and advantage read, rows written
+              'dist_dueling_grad_kernel': rows + params}             # the rows' gradient read, the value and advantage gradients written
+    out, total = {}, 0.0
+    for e in prof.key_averages():
+        name = next((k for k in nbytes if k in e.key), None)
+        if name is None:
+            continue
+        us = e.device_time_total / steps
+        out[name] = {'us_per_step': us, 'bytes': nbytes[name], 'tb_per_s': nbytes[name] / us * 1e-6,
+                     'fraction_of_3_35_tb_per_s': nbytes[name] / us * 1e-6 / 3.35}
+        total += us
+    step_us = 1e6 / timed(step, 50)
+    L.release_graphs()
+    L.close()
+    return {'card': card(), 'B': B, 'A': A, 'head': kind, 'W': W, 'dueling_row_kernels': out, 'dueling_rows_us_per_step': total,
+            'step_us': step_us, 'dueling_rows_share_of_step': total / step_us}
+
+
 class Captured:
     """a CUDA graph of `step` (warmed up on a side stream first); holds `step`, whose tensors the graph reads and writes"""
 
@@ -261,12 +299,18 @@ def main():
     ap.add_argument('--atoms', type=int, default=51)
     ap.add_argument('--noisy', action='store_true', help='add the noisy learner and run the torch statements on the noisy net')
     ap.add_argument('--quantile', action='store_true', help='add the quantile learners and the categorical one at --atoms beside them')
-    ap.add_argument('--quantiles', default='51,200', help='the quantile learners\' num_quantiles (--quantile)')
+    ap.add_argument('--quantiles', default='51,200', help='the quantile learners\' num_quantiles (--quantile, --dist-dueling)')
+    ap.add_argument('--dist-dueling', action='store_true', help='the categorical and quantile learners with and without the distributional '
+                    'dueling rows')
     a = ap.parse_args()
-    if a.dueling + a.categorical + a.noisy + a.quantile > 1:
-        sys.exit('--dueling, --categorical, --noisy and --quantile are separate comparisons: pass one')
+    if a.dueling + a.categorical + a.noisy + a.quantile + a.dist_dueling > 1:
+        sys.exit('--dueling, --categorical, --noisy, --quantile and --dist-dueling are separate comparisons: pass one')
     atoms = a.atoms if a.categorical else 0
     quantiles = [int(x) for x in a.quantiles.split(',')] if a.quantile else []
+    dd_heads = []           # --dist-dueling: (name, ApexHParams head keywords) of each head, run without and with the dueling rows
+    if a.dist_dueling:
+        dd_heads = [(f'categorical_K{a.atoms}', dict(categorical_dqn=True, num_atoms=a.atoms, v_min=V_MIN, v_max=V_MAX))] + \
+            [(f'quantile_N{N}', dict(quantile_dqn=True, num_quantiles=int(N))) for N in a.quantiles.split(',')]
     if not torch.cuda.is_available():
         sys.exit('bench_apex.py measures on a CUDA device; none is present')
     name = card()
@@ -299,6 +343,12 @@ def main():
             learners.append(LQ)
             variants[f'b200_quantile_N{N}_captured'] = (lambda L_, S_: lambda: L_.learn(exp, weights=w, idxs=idxs, sampler=S_,
                                                                                        sync_stats=False))(LQ, sampler())
+        for hname, kw in dd_heads:
+            for dd in (False, True):
+                LH = B200ApexLearner(ApexHParams(batch_size=B, num_actions=A, distributional_dueling=dd, **kw))
+                learners.append(LH)
+                variants[f'b200_{hname}{"_dist_dueling" if dd else ""}_captured'] = \
+                    (lambda L_, S_: lambda: L_.learn(exp, weights=w, idxs=idxs, sampler=S_, sync_stats=False))(LH, sampler())
         variants['torch_eager'] = TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms, noisy=a.noisy)
         variants['torch_captured'] = Captured(TorchStep(B, A, exp, w, idxs, dueling=a.dueling, atoms=atoms, noisy=a.noisy))
         for fn in variants.values():           # warm-up: the learner's first call runs eagerly, the second captures
@@ -326,6 +376,10 @@ def main():
         print(json.dumps(noisy_profile()), flush=True)
     for N in quantiles:
         print(json.dumps(quantile_profile(N)), flush=True)
+    if a.dist_dueling:
+        for kind, W in [('categorical', a.atoms)] + [('quantile', int(N)) for N in a.quantiles.split(',')]:
+            print(json.dumps(dist_dueling_profile(kind, W)), flush=True)
+        print(json.dumps(dist_dueling_profile('categorical', 64, A=31)), flush=True)
 
 
 if __name__ == '__main__':
