@@ -75,7 +75,6 @@ struct RConv2Fwd {   // 4x4 s2 over a1: tap j = (kh, kww): plane kh&1, shift (kh
   static constexpr int KID = 12;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
   static constexpr int BN = 64, NT = 8, NWIN = 2, WROWS = 128 + 11, STAGES = 3, SPLIT_STAGES = 1;
-  static constexpr int TILE_ROWB = 0;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP in1; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP in1_lo; SRL_TMAP w_lo; const float* bias; bf16* out; bf16* out_lo; int NF; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.in1); tma_prefetch_desc(&p.w); }
@@ -87,6 +86,22 @@ struct RConv2Fwd {   // 4x4 s2 over a1: tap j = (kh, kww): plane kh&1, shift (kh
     tma_load_2d(dst + win_bytes, lo ? &p.in1_lo : &p.in1, bar, 0, t * 128);
   }
   SRL_DEVINL static void prefetch16(const Params&, int, int, int, uint4 (&)[2]) {}
+  // bf16 mode: the tile's 128 positions x 64 channels are staged in shared memory and leave as 16-byte pieces, eight per position,
+  // consecutive lanes on consecutive pieces: a warp stores four whole a2 rows, consecutive along a valid run of 9 positions, where a
+  // row per thread touched 32 rows per store.  The 18 KB image fits the row hand-off's buffer: shared memory and ring depth are unchanged
+  static constexpr int TILE_ROWB = 144;
+  SRL_DEVINL static void prefetch_tile(const Params&, int, int, uint4 (&)[BN / 16][2]) {}
+  SRL_DEVINL static void epilogue_tile(const Params& p, int t, int wt, const float (&acc)[2][BN / 2], uint8_t* img, int bar,
+                                       const uint4 (&)[BN / 16][2]) {
+    wg_acc_stage_bf16<BN, TILE_ROWB>(acc, img, wt, bar, [&](int c, float v) { return fmaxf(v + __ldg(p.bias + c), 0.f); });
+#pragma unroll
+    for (int s = 0; s < 8; ++s) {
+      const int e = s * 128 + wt, q = e >> 3, k = e & 7;
+      const int Q = t * 128 + q, n = Q / 100, r = Q - n * 100, oh = r / 10, ow = r - oh * 10;
+      if (n >= p.NF || oh >= 9 || ow >= 9) continue;
+      *reinterpret_cast<uint4*>(p.out + ((size_t)n * 81 + oh * 9 + ow) * 64 + k * 8) = *reinterpret_cast<const uint4*>(img + q * TILE_ROWB + k * 16);
+    }
+  }
   template <int SPLIT>
   SRL_DEVINL static void epilogue16(const Params& p, int t, int row, int c0, float (&v)[16], const uint4 (&)[2]) {
     const int Q = t * 128 + row, n = Q / 100, r = Q - n * 100, oh = r / 10, ow = r - oh * 10;
@@ -101,7 +116,6 @@ struct RConv3Fwd {   // 3x3 s1 over a2: tap (kh,kw) -> shift kh*9 + kw
   static constexpr int KID = 13;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
   static constexpr int BN = 64, NT = 9, NWIN = 1, WROWS = 128 + 20, STAGES = 4, SPLIT_STAGES = 2;
-  static constexpr int TILE_ROWB = 0;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP w_lo; const float* bias; bf16* out; bf16* out_lo; int NF; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.w); }
@@ -110,6 +124,20 @@ struct RConv3Fwd {   // 3x3 s1 over a2: tap (kh,kw) -> shift kh*9 + kw
   SRL_DEVINL static constexpr int tap_shift(int j) { return (j / 3) * 9 + j % 3; }
   SRL_DEVINL static void load_windows(const Params& p, int t, uint8_t* dst, int, uint64_t* bar, bool lo) { tma_load_2d(dst, lo ? &p.in0_lo : &p.in0, bar, 0, t * 128); }
   SRL_DEVINL static void prefetch16(const Params&, int, int, int, uint4 (&)[2]) {}
+  // bf16 mode: staged tile as in RConv2Fwd; a warp stores four whole a3 rows, consecutive along a valid run of 7 positions
+  static constexpr int TILE_ROWB = 144;
+  SRL_DEVINL static void prefetch_tile(const Params&, int, int, uint4 (&)[BN / 16][2]) {}
+  SRL_DEVINL static void epilogue_tile(const Params& p, int t, int wt, const float (&acc)[2][BN / 2], uint8_t* img, int bar,
+                                       const uint4 (&)[BN / 16][2]) {
+    wg_acc_stage_bf16<BN, TILE_ROWB>(acc, img, wt, bar, [&](int c, float v) { return fmaxf(v + __ldg(p.bias + c), 0.f); });
+#pragma unroll
+    for (int s = 0; s < 8; ++s) {
+      const int e = s * 128 + wt, q = e >> 3, k = e & 7;
+      const int Q = t * 128 + q, n = Q / 81, r = Q - n * 81, oh = r / 9, ow = r - oh * 9;
+      if (n >= p.NF || oh >= 7 || ow >= 7) continue;
+      *reinterpret_cast<uint4*>(p.out + ((size_t)n * 49 + oh * 7 + ow) * 64 + k * 8) = *reinterpret_cast<const uint4*>(img + q * TILE_ROWB + k * 16);
+    }
+  }
   template <int SPLIT>
   SRL_DEVINL static void epilogue16(const Params& p, int t, int row, int c0, float (&v)[16], const uint4 (&)[2]) {
     const int Q = t * 128 + row, n = Q / 81, r = Q - n * 81, oh = r / 9, ow = r - oh * 9;
@@ -125,7 +153,6 @@ struct RConv3Dgrad {   // da2[ih,iw] = sum_{kh,kw} da3g[(ih-kh),(iw-kw)] W3[:, :
   static constexpr int KID = 14;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
   static constexpr int BN = 64, NT = 9, NWIN = 1, WROWS = 128 + 20, STAGES = 4, SPLIT_STAGES = 2;
-  static constexpr int TILE_ROWB = 0;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP w_lo; const bf16* act; bf16* dx; bf16* dx_lo; int NB; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.w); }
@@ -136,6 +163,31 @@ struct RConv3Dgrad {   // da2[ih,iw] = sum_{kh,kw} da3g[(ih-kh),(iw-kw)] W3[:, :
   SRL_DEVINL static void prefetch16(const Params& p, int t, int row, int c0, uint4 (&m)[2]) {
     const int Q = t * 128 + row;
     if (Q < p.NB * 81) ld_mask16(p.act + (size_t)Q * 64 + c0, m);                  // a2 lives on the same 9x9 grid
+  }
+  // bf16 mode: the tile (128 positions x 64 channels) is staged in shared memory and leaves as 16-byte pieces e = s * 128 + wt
+  // (position q = e >> 3, piece k = e & 7): the tile's mask is one contiguous 16 KB run of a2 and each position's 128 bytes are one
+  // da2g row, so a warp loads 512 contiguous bytes of mask and stores four whole da2g rows where a row per thread touched 32 rows per
+  // instruction.  Masking the rounded value gives the bits of rounding the masked one.
+  static constexpr int TILE_ROWB = 144;
+  SRL_DEVINL static void prefetch_tile(const Params& p, int t, int wt, uint4 (&m)[BN / 16][2]) {
+#pragma unroll
+    for (int s = 0; s < 8; ++s) {
+      const int e = s * 128 + wt, Q = t * 128 + (e >> 3);
+      if (Q < p.NB * 81) m[s >> 1][s & 1] = ldg16(p.act + (size_t)Q * 64 + (e & 7) * 8);
+    }
+  }
+  SRL_DEVINL static void epilogue_tile(const Params& p, int t, int wt, const float (&acc)[2][BN / 2], uint8_t* img, int bar,
+                                       const uint4 (&m)[BN / 16][2]) {
+    wg_acc_stage_bf16<BN, TILE_ROWB>(acc, img, wt, bar, [](int, float v) { return v; });
+#pragma unroll
+    for (int s = 0; s < 8; ++s) {
+      const int e = s * 128 + wt, q = e >> 3, k = e & 7;
+      const int Q = t * 128 + q, n = Q / 81, r = Q - n * 81, ih = r / 9, iw = r - ih * 9;
+      if (n >= p.NB) continue;
+      const uint4 x = *reinterpret_cast<const uint4*>(img + q * TILE_ROWB + k * 16), mk = m[s >> 1][s & 1];
+      *reinterpret_cast<uint4*>(p.dx + ((size_t)n * 100 + ih * 10 + iw) * 64 + k * 8) =
+          make_uint4(relu_mask_bf16x2(x.x, mk.x), relu_mask_bf16x2(x.y, mk.y), relu_mask_bf16x2(x.z, mk.z), relu_mask_bf16x2(x.w, mk.w));
+    }
   }
   template <int SPLIT>
   SRL_DEVINL static void epilogue16(const Params& p, int t, int row, int c0, float (&v)[16], const uint4 (&m)[2]) {

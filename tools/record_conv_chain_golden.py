@@ -22,16 +22,17 @@ GRADS = ('conv1.weight', 'conv1.bias', 'conv2.weight', 'conv2.bias', 'conv3.weig
 OUT = os.path.join(ROOT, 'tests', 'golden', 'conv_chain_digests.json')
 
 
-def step_digests(T, B, A):
-    """{array name: sha256 of its raw bytes} after one default learner step on seeded parameters and batch"""
+def step_digests(T, B, A, buffers=('a1', 'da1'), grads=GRADS):
+    """{array name: sha256 of its raw bytes} of the named workspace buffers and parameter gradients after one default learner
+    step on seeded parameters and batch"""
     from oracle import impala_oracle as O
     from scalerl_b200.learner import B200ImpalaLearner, ImpalaHParams
     L = B200ImpalaLearner(ImpalaHParams(rollout_length=T, batch_size=B, num_actions=A), init_state_dict=O.init_params(A, seed=0),
                           process_group=False)
     L.learn({k: v.cuda() for k, v in O.synthetic_batch(T, B, A, seed=1, done_p=0.02).items()})
     torch.cuda.synchronize()
-    arrays = {'a1': L.debug_buffer('a1'), 'da1': L.debug_buffer('da1')}
-    arrays.update((n, L.grads[n]) for n in GRADS)
+    arrays = {n: L.debug_buffer(n) for n in buffers}
+    arrays.update((n, L.grads[n]) for n in grads)
     return {n: hashlib.sha256(t.detach().contiguous().view(torch.uint8).cpu().numpy().tobytes()).hexdigest() for n, t in arrays.items()}
 
 
