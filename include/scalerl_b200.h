@@ -375,6 +375,36 @@ int srl_replay_sample(srl_replay_t* R, const double* uniforms, int batch, const 
 int srl_replay_gather(srl_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* state, int64_t* action, float* reward, uint8_t* next_state,
                       uint8_t* done, void* stream);
 
+/* ---- frame replay memory: srl_replay_* with each 84x84 frame stored once -------------------------------------------------------
+ * The transitions, fold, trees, sampling and outputs of srl_replay_*, bit for bit for the same adds, with the frame stacks kept as
+ * handles into a FIFO pool of frame_capacity u8 [84,84] frames (frame of 64-bit sequence number s at s mod frame_capacity).  An add
+ * compares each env's 8 incoming frames (state 0..3, next_state 0..3) byte for byte with the env's earlier frames of the call and with
+ * its previous next_state frames, reuses the sequence number of an equal one and numbers the rest in env order; an Atari stream that
+ * continues an episode adds one frame per env step.  Frames it overwrites retire every ring slot that references them: a retired slot
+ * has sum-tree leaf 0 and min-tree leaf +inf (never sampled, outside p_min), leaves the gather's output rows as they were, is skipped by
+ * srl_per_update_priorities without counting as invalid, and lives again when an add writes its slot.  It only saves memory when the
+ * stacks of the stream share frames.  Every call is stream-ordered. */
+typedef struct srl_frame_replay srl_frame_replay_t;
+/* srl_replay_create's arguments and limits, and frame_capacity in [8 num_envs (n_step + 1), 2^32] frames (the lower bound keeps the
+ * staging window's frames from being overwritten; memory_size + memory_size / 8 + 8 num_envs (n_step + 4) retires nothing while
+ * episodes average 32 steps or more).  Allocates frame_capacity * 7,056 B plus 94 B per slot and the window.  Synchronous. */
+int srl_frame_replay_create(int64_t memory_size, int num_envs, int n_step, double gamma, double alpha, int64_t frame_capacity,
+                            srl_frame_replay_t** out);
+int srl_frame_replay_destroy(srl_frame_replay_t* R);
+int64_t srl_frame_replay_size(const srl_frame_replay_t* R);   /* slots written, retired ones included (len of the reference's memory) */
+srl_per_t* srl_frame_replay_per(srl_frame_replay_t* R);        /* its trees, with the retired mask attached */
+/* srl_replay_add: state / next_state u8 [E,4,84,84] (device or host memory, copied on `stream`), action i64, reward f32, done u8 [E] */
+int srl_frame_replay_add(srl_frame_replay_t* R, const uint8_t* state, const int64_t* action, const float* reward, const uint8_t* next_state,
+                         const uint8_t* done, void* stream);
+/* srl_replay_sample and srl_replay_gather, each stack rebuilt from its 4 frames; a retired slot leaves its rows as they were */
+int srl_frame_replay_sample(srl_frame_replay_t* R, const double* uniforms, int batch, const double* beta_dev, uint8_t* state, int64_t* action,
+                            float* reward, uint8_t* next_state, uint8_t* done, int64_t* idxs, float* weights, void* stream);
+int srl_frame_replay_gather(srl_frame_replay_t* R, const int64_t* idxs, int64_t n, uint8_t* state, int64_t* action, float* reward,
+                            uint8_t* next_state, uint8_t* done, void* stream);
+/* frames written to the pool since creation, and slots retired since creation; each synchronises `stream`; -1 on error */
+int64_t srl_frame_replay_frames_allocated(srl_frame_replay_t* R, void* stream);
+int64_t srl_frame_replay_retired(srl_frame_replay_t* R, void* stream);
+
 /* ---- Ape-X learner step: a prioritized (double) DQN update on the encoder (BASELINE.json configs[3]) --------------------------
  * replaces the learner statements of the reference's Ape-X Learner.train (scalerl/algorithms/apex/worker.py:134-161) and, with
  * double DQN, clipping and the target cadence, DQNAgent.learn (scalerl/algorithms/dqn/dqn_agent.py:136-190).  The Q network is
@@ -556,6 +586,9 @@ int srl_apex_actor_debug_buffer(srl_apex_actor_t* X, const char* name, void** pt
  * > 0.  While the window fills nothing runs beyond the copy. */
 int srl_replay_add_prioritized(srl_replay_t* R, srl_apex_actor_t* actor, const uint8_t* state, const int64_t* action, const float* reward,
                                const uint8_t* next_state, const uint8_t* done, float priority_eps, void* stream);
+/* srl_replay_add_prioritized on the frame replay memory: s is the oldest staged step's states, rebuilt from their frames when n_step > 1 */
+int srl_frame_replay_add_prioritized(srl_frame_replay_t* R, srl_apex_actor_t* actor, const uint8_t* state, const int64_t* action,
+                                     const float* reward, const uint8_t* next_state, const uint8_t* done, float priority_eps, void* stream);
 
 /* ---- trajectory ring -> time-major batch (the stacking step of ImpalaTrainer.get_batch, impala_atari.py:248-251) -----------
  * staging: B trajectory slots on the DEVICE, each one contiguous record of slot_bytes holding every key of create_buffers

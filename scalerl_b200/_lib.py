@@ -113,6 +113,12 @@ _SIGS = {
     'srl_apex_actor_act': [_P] * 5,
     'srl_apex_actor_q_values': [_P, _P, _I, _P, _P],
     'srl_replay_add_prioritized': [_P] * 7 + [_F, _P],
+    'srl_frame_replay_create': [_L, _I, _I, C.c_double, C.c_double, _L, C.POINTER(_P)],
+    'srl_frame_replay_destroy': [_P],
+    'srl_frame_replay_add': [_P] * 7,
+    'srl_frame_replay_add_prioritized': [_P] * 7 + [_F, _P],
+    'srl_frame_replay_sample': [_P, _P, _I] + [_P] * 9,
+    'srl_frame_replay_gather': [_P, _P, _L] + [_P] * 6,
 }
 # libscalerl_b200_testhooks.so (include/scalerl_b200_testhooks.h): unit-test entry points, loaded by tests only
 _HOOK_SIGS = {
@@ -143,7 +149,7 @@ def hooks():
     return _hooks
 
 
-EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout', 'srl_apex_param_layout_ex', 'srl_apex_param_layout_cat', 'srl_apex_param_layout_noisy', 'srl_apex_param_layout_quantile', 'srl_apex_param_layout_dist_dueling', 'srl_replay_size', 'srl_replay_per'])
+EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout', 'srl_apex_param_layout_ex', 'srl_apex_param_layout_cat', 'srl_apex_param_layout_noisy', 'srl_apex_param_layout_quantile', 'srl_apex_param_layout_dist_dueling', 'srl_replay_size', 'srl_replay_per', 'srl_frame_replay_size', 'srl_frame_replay_per', 'srl_frame_replay_frames_allocated', 'srl_frame_replay_retired'])
 
 
 def lib():
@@ -172,6 +178,13 @@ def lib():
         L.srl_replay_size.argtypes = [_P]
         L.srl_replay_per.restype = _P
         L.srl_replay_per.argtypes = [_P]
+        L.srl_frame_replay_size.restype = C.c_int64
+        L.srl_frame_replay_size.argtypes = [_P]
+        L.srl_frame_replay_per.restype = _P
+        L.srl_frame_replay_per.argtypes = [_P]
+        for nm in ('srl_frame_replay_frames_allocated', 'srl_frame_replay_retired'):
+            getattr(L, nm).restype = C.c_int64
+            getattr(L, nm).argtypes = [_P, _P]
         L.srl_learner_get_step.restype = C.c_int64
         L.srl_learner_get_step.argtypes = [_P, _P]
         L.srl_per_invalid_updates.restype = C.c_int64

@@ -673,16 +673,16 @@ class B200ApexLearner(BaseAgent):
 
     @torch.no_grad()
     def learn_from(self, memory, beta: float = 0.4, sync_stats: bool = True, use_graph: Optional[bool] = None) -> Dict[str, float]:
-        """one update on a batch of ``batch_size`` transitions sampled from ``memory`` (a GpuPrioritizedReplayBuffer on this
-        learner's device), all on the device: uniforms drawn by ``torch.rand`` (the default CUDA generator) into a fixed buffer, the
+        """one update on a batch of ``batch_size`` transitions sampled from ``memory`` (a GpuPrioritizedReplayBuffer or a
+        GpuFrameReplayBuffer on this learner's device), all on the device: uniforms drawn by ``torch.rand`` (the default CUDA generator) into a fixed buffer, the
         prioritized sample and the gather into learner-owned fixed buffers, the step, and the new priorities written into
         ``memory``'s trees.  It is captured as one graph per memory (first call eager, second captures, later calls replay); the
         sampler reads the stored count and ``beta`` from the device, so a replay sees every add made since and a new ``beta`` costs
         one fill, not a recapture.  ``hp.gamma`` is used as given: for n-step memories pass ``gamma ** n_step``.  The target cadence
         and the step counters are learn()'s.  -> {'loss': float}, or {} with nothing synchronised."""
-        from ...data.replay_memory import GpuPrioritizedReplayBuffer
-        if not isinstance(memory, GpuPrioritizedReplayBuffer):
-            raise ValueError(f'memory must be a GpuPrioritizedReplayBuffer, got {type(memory).__name__}')
+        from ...data.replay_memory import GpuFrameReplayBuffer, GpuPrioritizedReplayBuffer
+        if not isinstance(memory, (GpuPrioritizedReplayBuffer, GpuFrameReplayBuffer)):
+            raise ValueError(f'memory must be a GpuPrioritizedReplayBuffer or a GpuFrameReplayBuffer, got {type(memory).__name__}')
         if memory.device != self.device:
             raise ValueError(f'memory is on {memory.device}, the learner on {self.device}')
         if len(memory) < 2:

@@ -388,6 +388,12 @@ int64_t per_tree_ptr(const srl_per* P);          // the leaf the next add writes
 // n new leaves at tree_ptr.. = priorities[i]^alpha (f64 [n], device), max_priority updated, the count advanced as by srl_per_add; a
 // non-finite priority is stored as max_priority^alpha and counted by srl_per_invalid_updates.  0, or an error code with the message set
 int per_add_prioritized(srl_per* P, const double* priorities, int64_t n, cudaStream_t st);
+// the per-leaf retired mask (u8 [memory_size] on the device, zeroed, owned by the caller; frame_replay.cu).  With it, srl_per_update_priorities
+// skips retired leaves without counting them, every add makes the leaves it writes live again, and the sample's descent skips subtrees
+// of sum 0.  Without it (a NULL mask, the default) every kernel computes what it computed before retirement existed.
+void per_attach_retired(srl_per* P, uint8_t* retired);
+// leaves[0 .. *n_dev) (device count, read when the kernel runs) retire: sum 0, min +inf, marked in the mask.  Needs the mask attached.
+int per_retire(srl_per* P, const int64_t* leaves, const unsigned long long* n_dev, cudaStream_t st);
 // ---- apex_actor.cu: what the prioritized add (replay.cu) uses of an Ape-X actor
 int apex_actor_num_envs(const srl_apex_actor* X);
 // the actor's initial priorities of E transitions that sit in ring slots (ptr + e) mod M: s = state rows, s' = next_state rows (u8

@@ -22,9 +22,12 @@ __device__ __forceinline__ int64_t* per_count_slot(double* scal) { return reinte
 //   mode 1: leaves ptr.. (mod memory_size) = max_priority^alpha, stored count = min(count + n, memory_size)
 //   mode 2: leaves ptr.. (mod memory_size) = priority^alpha from prios, max_priority updated, the count as mode 1.  A non-finite priority
 //           is counted in scal[1] and stored as mode 1 would store it (max_priority^alpha as the launch found it)
+// retired (optional, [memory_size]): the leaves per_retire_kernel took out of sampling.  Mode 0 skips a retired leaf without counting it
+// (its priority may be written after it retired); modes 1 and 2 make the leaves they write live again.
 __global__ void __launch_bounds__(1024) per_update_kernel(double* __restrict__ sum, double* __restrict__ mn, int64_t cap, int levels,
                                                           const int64_t* __restrict__ idxs, const double* __restrict__ prios, int n,
-                                                          double alpha, double* __restrict__ scal, int mode, int64_t ptr, int64_t memory_size) {
+                                                          double alpha, double* __restrict__ scal, int mode, int64_t ptr, int64_t memory_size,
+                                                          uint8_t* __restrict__ retired) {
   __shared__ int64_t sidx[1024];
   __shared__ double smax[32];
   const int t = threadIdx.x;
@@ -38,6 +41,7 @@ __global__ void __launch_bounds__(1024) per_update_kernel(double* __restrict__ s
       // the reference asserts priority > 0 and 0 <= idx < len(self) (replay_buffer.py:346-351): an invalid entry is
       // skipped here (never an out-of-bounds write) and counted in scal[1]; the Python wrapper raises on it
       if (!(leaf >= 0 && leaf < count) || !(pr > 0.0)) { valid = false; leaf = -1; atomicAdd(reinterpret_cast<unsigned long long*>(scal + 1), 1ull); }
+      else if (retired && retired[leaf]) { valid = false; leaf = -1; }
     } else {
       leaf = (ptr + t) % memory_size;
       if (mode == 2) pr = prios[t];
@@ -55,7 +59,10 @@ __global__ void __launch_bounds__(1024) per_update_kernel(double* __restrict__ s
   if (winner && mode == 0)
     for (int u = t + 1; u < n; ++u)
       if (sidx[u] == leaf) { winner = false; break; }
-  if (winner) { sum[cap + leaf] = v; mn[cap + leaf] = v; }
+  if (winner) {
+    sum[cap + leaf] = v; mn[cap + leaf] = v;
+    if (retired && mode != 0) retired[leaf] = 0;
+  }
   if (mode != 1) {       // max_priority = max(max_priority, priorities...)
     double m = valid ? pr : 0.0;
     for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -91,10 +98,12 @@ __device__ double prefix_sum_ref_order(const double* __restrict__ sum, int64_t c
   return r;
 }
 
-// beta_dev (optional): beta read from the device when the kernel runs, so a replayed graph sees every change; else `beta`
+// beta_dev (optional): beta read from the device when the kernel runs, so a replayed graph sees every change; else `beta`.
+// skip_empty (trees with retired leaves): the descent never enters a subtree of sum 0, so it ends on a leaf of positive priority even
+// where rounding puts the prefix at or past the mass it came from (a retired leaf, 0, would otherwise be the rightmost choice).
 __global__ void per_sample_kernel(const double* __restrict__ sum, const double* __restrict__ mn, int64_t cap, const double* __restrict__ u,
                                   int batch, const double* __restrict__ scal, double beta, const double* __restrict__ beta_dev,
-                                  int64_t* __restrict__ idxs, double* __restrict__ w64, float* __restrict__ w32) {
+                                  int64_t* __restrict__ idxs, double* __restrict__ w64, float* __restrict__ w32, bool skip_empty) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= batch) return;
   const int64_t n = *reinterpret_cast<const int64_t*>(scal + 2);
@@ -107,7 +116,7 @@ __global__ void per_sample_kernel(const double* __restrict__ sum, const double* 
   while (idx < cap) {                                            // find_prefixsum_idx
     const int64_t left = 2 * idx;
     const double lv = sum[left];
-    if (lv > prefix) idx = left;
+    if (lv > prefix || (skip_empty && sum[left + 1] == 0.0)) idx = left;
     else { prefix -= lv; idx = left + 1; }
   }
   idx -= cap;
@@ -118,6 +127,28 @@ __global__ void per_sample_kernel(const double* __restrict__ sum, const double* 
   const double wt = pow((sum[cap + idx] / total) * (double)n, -beta) / max_weight;
   if (w64) w64[i] = wt;
   if (w32) w32[i] = (float)wt;
+}
+
+// leaves[0 .. *n_dev) leave sampling: sum 0, min +inf (so they enter neither p_total nor p_min), marked in `retired`; their
+// ancestors are recomputed level by level, 1024 leaves at a time, as per_update_kernel does.  One block.
+__global__ void __launch_bounds__(1024) per_retire_kernel(double* __restrict__ sum, double* __restrict__ mn, int64_t cap, int levels,
+                                                          const int64_t* __restrict__ leaves, const unsigned long long* __restrict__ n_dev,
+                                                          uint8_t* __restrict__ retired) {
+  const int64_t n = (int64_t)*n_dev;
+  for (int64_t o = 0; o < n; o += 1024) {
+    const bool valid = o + threadIdx.x < n;
+    const int64_t leaf = valid ? leaves[o + threadIdx.x] : 0;
+    if (valid) { sum[cap + leaf] = 0.0; mn[cap + leaf] = INFINITY; retired[leaf] = 1; }
+    __syncthreads();
+    for (int d = 1; d <= levels; ++d) {
+      if (valid) {
+        const int64_t node = (cap + leaf) >> d;
+        sum[node] = sum[2 * node] + sum[2 * node + 1];
+        mn[node] = fmin(mn[2 * node], mn[2 * node + 1]);
+      }
+      __syncthreads();
+    }
+  }
 }
 
 __global__ void per_fill_kernel(double* __restrict__ sum, double* __restrict__ mn, int64_t n2, double* scal) {
@@ -134,6 +165,7 @@ struct srl_per {
   int levels;
   double alpha;
   double *sum, *mn, *scal;
+  uint8_t* retired;                // per-leaf retired mask (per_attach_retired), NULL for a plain sampler
 };
 extern "C" const char* srl_per_last_error(void) { return srl_last_error(); }
 
@@ -165,7 +197,7 @@ cudaError_t per_insert(srl_per* P, const double* prios, int64_t n, cudaStream_t 
     const int64_t c = n - o < 1024 ? n - o : 1024;
     const int cc = (int)(c < P->memory_size ? c : P->memory_size);
     per_update_kernel<<<1, 1024, 0, st>>>(P->sum, P->mn, P->capacity, P->levels, nullptr, prios ? prios + o : nullptr, cc, P->alpha, P->scal,
-                                          prios ? 2 : 1, P->tree_ptr, P->memory_size);
+                                          prios ? 2 : 1, P->tree_ptr, P->memory_size, P->retired);
     P->tree_ptr = (P->tree_ptr + cc) % P->memory_size;
     P->size = P->size + cc < P->memory_size ? P->size + cc : P->memory_size;
     o += cc;
@@ -186,7 +218,7 @@ extern "C" int srl_per_update_priorities(srl_per_t* P, const int64_t* idxs, cons
   for (int64_t o = 0; o < n; o += 1024) {
     const int c = (int)(n - o < 1024 ? n - o : 1024);
     per_update_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(P->sum, P->mn, P->capacity, P->levels, idxs + o, priorities + o, c, P->alpha, P->scal, 0,
-                                                            0, P->memory_size);  // mode 0 bounds idx by the device count (idx < len(self))
+                                                            0, P->memory_size, P->retired);  // mode 0 bounds idx by the device count (idx < len(self))
   }
   CU(cudaGetLastError(), "per_update_priorities");
   return 0;
@@ -202,6 +234,12 @@ extern "C" int64_t srl_per_invalid_updates(srl_per_t* P, void* stream) {
 }
 namespace srl {
 int64_t per_tree_ptr(const srl_per* P) { return P->tree_ptr; }
+void per_attach_retired(srl_per* P, uint8_t* retired) { P->retired = retired; }
+int per_retire(srl_per* P, const int64_t* leaves, const unsigned long long* n_dev, cudaStream_t st) {
+  per_retire_kernel<<<1, 1024, 0, st>>>(P->sum, P->mn, P->capacity, P->levels, leaves, n_dev, P->retired);
+  CU(cudaGetLastError(), "per_retire");
+  return 0;
+}
 int per_add_prioritized(srl_per* P, const double* priorities, int64_t n, cudaStream_t st) {
   CU(per_insert(P, priorities, n, st), "per_add_prioritized");
   return 0;
@@ -211,7 +249,7 @@ int per_sample(srl_per* P, const double* uniforms, int batch, double beta, const
   REQ(P && uniforms && idxs && batch >= 1, "per_sample: bad argument");
   REQ(P->size >= 2, "per_sample: need at least 2 stored transitions");
   per_sample_kernel<<<(batch + 127) / 128, 128, 0, st>>>(P->sum, P->mn, P->capacity, uniforms, batch, P->scal, beta, beta_dev, idxs, weights64,
-                                                         weights32);
+                                                         weights32, P->retired != nullptr);
   CU(cudaGetLastError(), "per_sample");
   return 0;
 }

@@ -8,19 +8,14 @@
 #include "common.cuh"
 #include "errors.h"
 #include "kernels.h"
+#include "replay.cuh"
 #include "../../include/scalerl_b200.h"
 
 namespace srl {
 
-constexpr int64_t OBS_BYTES = 4 * 84 * 84;                 // one u8 frame stack: 28,224 B
-constexpr int OBS_VEC = (int)(OBS_BYTES / 16);             // 1,764 16-byte vectors
-constexpr int ROW_PAIR_VEC = 2 * OBS_VEC;                  // state + next_state of one transition
-constexpr int REPLAY_MAX_NSTEP = 32;
 constexpr int FOLD_THREADS = 256;
 constexpr int GATHER_THREADS = 256, GATHER_VPT = 2;        // 16-byte vectors per thread, all loaded before any is stored
 constexpr int GATHER_CHUNKS = (ROW_PAIR_VEC + GATHER_THREADS * GATHER_VPT - 1) / (GATHER_THREADS * GATHER_VPT);   // CTAs per transition
-
-struct GammaPowers { float g[REPLAY_MAX_NSTEP]; };         // g[k] = fp32(double(gamma) ** k)
 
 // The transition fields: the ring ([M] rows) and the staging window ([n_step][E] rows; vector step t sits in window slot t mod n_step).
 struct ReplayRows {
@@ -36,15 +31,9 @@ struct ReplayRows {
 __global__ void __launch_bounds__(FOLD_THREADS) replay_fold_kernel(ReplayRows win, ReplayRows ring, int E, int n_step, int oldest,
                                                                    GammaPowers gp, int64_t ptr, int64_t M) {
   const int e = blockIdx.x;
-  int stop = oldest;
-  uint8_t d = win.done[(int64_t)oldest * E + e];
-  float r = win.reward[(int64_t)oldest * E + e];
-  for (int k = 1; k < n_step && !d; ++k) {
-    const int s = (oldest + k) % n_step;
-    r = __fadd_rn(r, __fmul_rn(win.reward[(int64_t)s * E + e], gp.g[k]));
-    d = win.done[(int64_t)s * E + e];
-    stop = s;
-  }
+  float r;
+  uint8_t d;
+  const int stop = fold_reward_done(win.reward, win.done, E, e, n_step, oldest, gp, &r, &d);
   const int64_t slot = (ptr + e) % M;
   const int i = blockIdx.y * FOLD_THREADS + threadIdx.x;
   if (i < OBS_VEC) ring.state[slot * OBS_VEC + i] = win.state[((int64_t)oldest * E + e) * OBS_VEC + i];

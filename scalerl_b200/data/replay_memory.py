@@ -17,6 +17,9 @@ Deviations from the reference:
   * the ring index is the tree index at every fill level.  The reference's deque index stops matching its tree index once the
     memory is full (replay_buffer.py:41-44 vs :319-323); oracle/replay_oracle.py documents the mapping.
 Everything runs on the current stream and is stream-ordered; adds are host calls and may come between replays of a graph that samples.
+
+GpuFrameReplayBuffer (srl_frame_replay_*, csrc/frame_replay.cu) keeps the same transitions, trees and outputs with each 84x84 frame
+stored once, in a FIFO pool of ``frame_capacity`` frames that the ring's slots reference by handle.
 """
 import ctypes as C
 import math
@@ -38,7 +41,11 @@ def _int_in(name, v, lo, hi):
     return int(v)
 
 
-class GpuPrioritizedReplayBuffer:
+class _GpuReplay:
+    """what the two device memories share: the argument checks, the field checks of ``save_to_memory``, the beta handling, sampling,
+    gathering and the trees.  ``_abi`` names the C-ABI family (srl_replay, srl_frame_replay) whose entry points take the same arguments."""
+    _abi = None
+
     def __init__(self, memory_size: int, num_envs: int, alpha: float = 0.6, n_step: int = 1, gamma: float = 0.99, device=None):
         self.memory_size = _int_in('memory_size', memory_size, 2, 1 << 30)
         self.num_envs = _int_in('num_envs', num_envs, 1, min(MAX_ENVS, self.memory_size))
@@ -48,24 +55,35 @@ class GpuPrioritizedReplayBuffer:
             raise ValueError(f'gamma must be finite, got {gamma}')
         if not math.isfinite(self.alpha):
             raise ValueError(f'alpha must be finite, got {alpha}')
+        self._check_extra()
         if not torch.cuda.is_available():
-            raise RuntimeError('GpuPrioritizedReplayBuffer needs a CUDA device (no CPU fallback)')
+            raise RuntimeError(f'{type(self).__name__} needs a CUDA device (no CPU fallback)')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._L = _lib.lib()
         h = C.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(self._L.srl_replay_create(self.memory_size, self.num_envs, self.n_step, self.gamma, self.alpha, C.byref(h)),
-                       'srl_replay_create')
+            _lib.check(self._fn('create')(self.memory_size, self.num_envs, self.n_step, self.gamma, self.alpha, *self._create_extra(), C.byref(h)),
+                       f'{self._abi}_create')
             self._h = h
-            self.sampler = GpuPrioritizedSampler._view(C.c_void_p(self._L.srl_replay_per(h)), self.memory_size, self.alpha, self.device)
+            self.sampler = GpuPrioritizedSampler._view(C.c_void_p(self._fn('per')(h)), self.memory_size, self.alpha, self.device)
             self._beta = torch.zeros(1, dtype=torch.float64, device=self.device)     # read by the sample kernel when it runs
         self._beta_value = None
+
+    def _check_extra(self):
+        """checks of the subclass's own constructor arguments (before any device work)"""
+
+    def _create_extra(self):
+        """the subclass's own arguments of <abi>_create, after alpha"""
+        return ()
+
+    def _fn(self, name):
+        return getattr(self._L, f'{self._abi}_{name}')
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
 
     def __len__(self):
-        return int(self._L.srl_replay_size(self._h))
+        return int(self._fn('size')(self._h))
 
     def size(self):
         return len(self)
@@ -112,12 +130,12 @@ class GpuPrioritizedReplayBuffer:
         s, a, r, ns, d = ((t.view(torch.uint8) if t.dtype == torch.bool else t).to(self.device, dt).contiguous() for t, dt in (s, a, r, ns, d))
         with torch.cuda.device(self.device):
             if priorities_from is None:
-                _lib.check(self._L.srl_replay_add(self._h, s.data_ptr(), a.data_ptr(), r.data_ptr(), ns.data_ptr(), d.data_ptr(), self._stream()),
-                           'srl_replay_add')
+                _lib.check(self._fn('add')(self._h, s.data_ptr(), a.data_ptr(), r.data_ptr(), ns.data_ptr(), d.data_ptr(), self._stream()),
+                           f'{self._abi}_add')
             else:
-                _lib.check(self._L.srl_replay_add_prioritized(self._h, priorities_from._h, s.data_ptr(), a.data_ptr(), r.data_ptr(), ns.data_ptr(),
-                                                              d.data_ptr(), priorities_from.priority_eps, self._stream()),
-                           'srl_replay_add_prioritized')
+                _lib.check(self._fn('add_prioritized')(self._h, priorities_from._h, s.data_ptr(), a.data_ptr(), r.data_ptr(), ns.data_ptr(),
+                                                       d.data_ptr(), priorities_from.priority_eps, self._stream()),
+                           f'{self._abi}_add_prioritized')
 
     # ------------------------------------------------------------------ sampling
     def _set_beta(self, beta: float) -> None:
@@ -130,10 +148,10 @@ class GpuPrioritizedReplayBuffer:
             self._beta_value = beta
 
     def _sample_into(self, uniforms, state, action, reward, next_state, done, idxs, weights) -> None:
-        """srl_replay_sample into caller-owned device buffers (no checks beyond the library's; nothing synchronised)"""
-        _lib.check(self._L.srl_replay_sample(self._h, uniforms.data_ptr(), uniforms.numel(), self._beta.data_ptr(), state.data_ptr(),
-                                             action.data_ptr(), reward.data_ptr(), next_state.data_ptr(), done.data_ptr(), idxs.data_ptr(),
-                                             weights.data_ptr(), self._stream()), 'srl_replay_sample')
+        """<abi>_sample into caller-owned device buffers (no checks beyond the library's; nothing synchronised)"""
+        _lib.check(self._fn('sample')(self._h, uniforms.data_ptr(), uniforms.numel(), self._beta.data_ptr(), state.data_ptr(),
+                                      action.data_ptr(), reward.data_ptr(), next_state.data_ptr(), done.data_ptr(), idxs.data_ptr(),
+                                      weights.data_ptr(), self._stream()), f'{self._abi}_sample')
 
     def _outputs(self, n):
         z = lambda *shape, dtype: torch.empty(*shape, dtype=dtype, device=self.device)
@@ -162,8 +180,8 @@ class GpuPrioritizedReplayBuffer:
         """(state, action, reward, next_state, done) of ring slots ``idxs`` (int64 [n]), new device tensors"""
         idxs = torch.as_tensor(idxs).to(self.device, torch.int64).contiguous().reshape(-1)
         out = self._outputs(idxs.numel())
-        _lib.check(self._L.srl_replay_gather(self._h, idxs.data_ptr(), idxs.numel(), *(t.data_ptr() for t in out), self._stream()),
-                   'srl_replay_gather')
+        _lib.check(self._fn('gather')(self._h, idxs.data_ptr(), idxs.numel(), *(t.data_ptr() for t in out), self._stream()),
+                   f'{self._abi}_gather')
         return out
 
     def update_priorities(self, idxs, priorities, validate: bool = True) -> None:
@@ -173,7 +191,7 @@ class GpuPrioritizedReplayBuffer:
     def close(self):
         if getattr(self, '_h', None) is not None:
             self.sampler.close()
-            self._L.srl_replay_destroy(self._h)
+            self._fn('destroy')(self._h)
             self._h = None
 
     def __del__(self):
@@ -181,3 +199,52 @@ class GpuPrioritizedReplayBuffer:
             self.close()
         except Exception:
             pass
+
+
+class GpuPrioritizedReplayBuffer(_GpuReplay):
+    """the reference's PrioritizedReplayBuffer on the device, each transition stored as two 4x84x84 u8 stacks (56,461 B).  It makes no
+    assumption about how the stacks of a stream relate, so it is the memory for streams whose stacks share no frames."""
+    _abi = 'srl_replay'
+
+
+class GpuFrameReplayBuffer(_GpuReplay):
+    """GpuPrioritizedReplayBuffer's transitions, trees, methods and outputs (the same bytes for the same adds) with each 84x84 frame
+    stored once.  It only saves memory when the stacks of the stream share frames, as Atari frame stacks do: a continuing episode then
+    adds one 7,056-byte frame per env step.
+
+    ``frame_capacity``: 84x84 frames in the pool, at least ``8 * num_envs * (n_step + 1)`` (so the staging window's frames are never
+    overwritten); default ``memory_size + memory_size // 8 + 8 * num_envs * (n_step + 4)``, which retires nothing while episodes average
+    at least 32 steps.  When new frames overwrite one that a stored transition references, that transition retires first: its priority
+    becomes 0 (never sampled, outside the weights' p_min), ``gather`` leaves its output rows as they were, and ``update_priorities``
+    skips it without raising.  An add that writes its slot makes it live again; ``len`` counts it throughout."""
+    _abi = 'srl_frame_replay'
+
+    def __init__(self, memory_size: int, num_envs: int, alpha: float = 0.6, n_step: int = 1, gamma: float = 0.99, frame_capacity=None,
+                 device=None):
+        self._frame_capacity_arg = frame_capacity
+        super().__init__(memory_size, num_envs, alpha=alpha, n_step=n_step, gamma=gamma, device=device)
+
+    def _check_extra(self):
+        E, n, M = self.num_envs, self.n_step, self.memory_size
+        fc = self._frame_capacity_arg
+        lo = 8 * E * (n + 1)
+        self.frame_capacity = M + M // 8 + 8 * E * (n + 4) if fc is None else _int_in('frame_capacity', fc, lo, 1 << 32)
+
+    def _create_extra(self):
+        return (self.frame_capacity,)
+
+    def frames_allocated(self) -> int:
+        """frames written to the pool since creation.  Synchronises the device (the count is known there)."""
+        with torch.cuda.device(self.device):
+            return self._counter('frames_allocated')
+
+    def retired(self) -> int:
+        """transitions retired since creation (each time one retires).  Synchronises the device (the count is known there)."""
+        with torch.cuda.device(self.device):
+            return self._counter('retired')
+
+    def _counter(self, name):
+        v = int(self._fn(name)(self._h, self._stream()))
+        if v < 0:
+            raise RuntimeError(f'{self._abi}_{name}: reading the device counter failed')
+        return v
