@@ -19,7 +19,10 @@
 //
 // A Problem P supplies: BN, A_MN, B_MN, STAGES, KROWS (MN-major only), ZERO_INIT, Params (holds the CUtensorMaps),
 //   num_kblocks(p,tm,ty), issue(p,tm,ty,kb,sA,sB,bar), init_smem(p,tm,ty,stage_base,tid) [ZERO_INIT only, once per stage],
-//   epilogue16(p,tm,ty,row,c0,v).
+//   epilogue16(p,tm,ty,row,c0,v), TILE_ROWB.
+//   TILE_ROWB: 0, or (bf16 mode) the row pitch in bytes of an fp32 image of the whole 128 x BN output tile that the kernel stages
+//   in the stage ring once the last k-block has retired; epilogue_tile(p,tm,ty,t,image,pre) then copies it out in whole, coalesced
+//   output rows with all 256 consumer threads t, and prefetch_tile(p,tm,ty,t,pre) requests its global operands instead of prefetch16.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -68,10 +71,28 @@ struct TmaCfg {
   static_assert(SMEM_BYTES <= 232448, "shared memory budget (227 KB)");
   static_assert(NB == 32 || NB == 64 || NB == 128, "MMA N per warpgroup");
   static constexpr int MMAS = P::A_MN ? KROWS / 16 : 4;
+  // the output tile leaves through an fp32 image in the stage ring (bf16 mode of the problems that define one), or row by row
+  static constexpr bool TILE_EPI = P::TILE_ROWB > 0 && !SPLIT;
+  static_assert(!TILE_EPI || (P::TILE_ROWB >= 4 * P::BN && P::TILE_ROWB % 16 == 0 && 128 * P::TILE_ROWB <= STAGES * STAGE_BYTES),
+                "the tile image holds 128 rows of BN fp32 in 16-byte aligned rows inside the stage ring");
   static_assert(A_BYTES % 1024 == 0 && B_BYTES % 1024 == 0, "operand tiles must keep 1024 B alignment (SWIZZLE_128B atoms)");
   static_assert(P::A_MN == P::B_MN, "mixed majors are not used");
   static_assert(KROWS % 16 == 0, "contraction rows per stage must be a multiple of MMA K = 16");
 };
+
+// fp32 image of a warpgroup's 128 x N accumulator (wgmma fragment layout) in shared memory: row r at img + r * ROWB bytes, column c
+// at byte 4c.  With ROWB = 8N + 32 (the tile's BN = 2N = 64 or 256) a half-warp's float2 stores (4 rows x 8 words) hit 32 banks.
+template <int N, int ROWB>
+SRL_DEVINL void wg_acc_stage_f32(const float (&d)[2][N / 2], uint8_t* img, int wt) {
+  const int w = wt >> 5, l = wt & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < N / 2; i += 2) {
+      const int row = 64 * h + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3);
+      *reinterpret_cast<float2*>(img + row * ROWB + col * 4) = make_float2(d[h][i], d[h][i + 1]);
+    }
+}
 
 template <class P, int SPLIT>
 SRL_DEVINL void igt_epilogue(const typename P::Params& p, int tm, int ty, int row, int c0, float (&v)[16]) {
@@ -131,8 +152,11 @@ __global__ void __launch_bounds__(IGT_THREADS) igemm_tma_kernel(const __grid_con
     const int g = warp >> 2, wt = tid & 127;
     constexpr int NB = C::NB;
     // global operands of the epilogue (ReLU mask) are requested before the mainloop: their latency overlaps the MMAs
+    // (tile epilogue: the same NB / 8 pieces of 16 bytes per thread hold the tile's bf16 mask, 128 rows x BN, over all 256 threads)
     uint4 pre[P::PREFETCH ? NB / 16 : 1][2];
-    if constexpr (P::PREFETCH) {
+    if constexpr (C::TILE_EPI) {
+      if constexpr (P::PREFETCH) P::prefetch_tile(p, tm, ty, tid, pre);
+    } else if constexpr (P::PREFETCH) {
 #pragma unroll
       for (int c = 0; c < NB / 16; ++c) P::prefetch16(p, tm, ty, wt, g * NB + c * 16, pre[c]);
     }
@@ -175,13 +199,22 @@ __global__ void __launch_bounds__(IGT_THREADS) igemm_tma_kernel(const __grid_con
     }
     wg_wait_all();
     wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
-    float* my_img = img + g * (WG_IMG_BYTES / 4);
+    if constexpr (C::TILE_EPI) {
+      // one tile per CTA: once both warpgroups' last wgmma retired, every TMA write has landed and no MMA reads the ring (nor its
+      // zero-filled B rows) any more, so the image overwrites it
+      named_bar(1, 256);
+      wg_acc_stage_f32<NB, P::TILE_ROWB>(acc, smem + g * NB * 4, wt);
+      named_bar(1, 256);
+      P::epilogue_tile(p, tm, ty, tid, smem, pre);
+    } else {
+      float* my_img = img + g * (WG_IMG_BYTES / 4);
 #pragma unroll
-    for (int c = 0; c < NB / 16; ++c) {
-      float v[16];
-      wg_acc_row16<NB>(acc, c, my_img, wt, 2 + g, v);
-      if constexpr (P::PREFETCH) igt_epilogue<P, SPLIT>(p, tm, ty, wt, g * NB + c * 16, v, pre[c]);
-      else igt_epilogue<P, SPLIT>(p, tm, ty, wt, g * NB + c * 16, v);
+      for (int c = 0; c < NB / 16; ++c) {
+        float v[16];
+        wg_acc_row16<NB>(acc, c, my_img, wt, 2 + g, v);
+        if constexpr (P::PREFETCH) igt_epilogue<P, SPLIT>(p, tm, ty, wt, g * NB + c * 16, v, pre[c]);
+        else igt_epilogue<P, SPLIT>(p, tm, ty, wt, g * NB + c * 16, v);
+      }
     }
   }
 }

@@ -28,6 +28,7 @@ struct LGemmK {
   static constexpr bool PREFETCH = false;      // C[c_row0 + m][n] = sum_k A[a_row0 + m][k] * B[n][k];  grid = (ceil(M/128), Npad/64)
   static constexpr int BN = 64, STAGES = 4, KROWS = 64;
   static constexpr bool A_MN = false, B_MN = false, ZERO_INIT = false;
+  static constexpr int TILE_ROWB = 0;          // row hand-off
   struct Params { SRL_TMAP a; SRL_TMAP b; float* C; int M, nkb, ldc, a_row0, c_row0; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.a); tma_prefetch_desc(&p.b); }
   SRL_DEVINL static int num_kblocks(const Params& p, int, int) { return p.nkb; }
@@ -49,6 +50,7 @@ struct LGemmMN {
   static constexpr bool PREFETCH = false;     // C[i][j] = sum_r A[r][i] * B[r][j]  (rows r = samples, MN-major operands); grid = (Ipad/128, Jpad/64)
   static constexpr int BN = 64, STAGES = 4, KROWS = 64;
   static constexpr bool A_MN = true, B_MN = true, ZERO_INIT = false;
+  static constexpr int TILE_ROWB = 0;         // row hand-off
   struct Params { SRL_TMAP a; SRL_TMAP b; float* C; int R, ldc; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.a); tma_prefetch_desc(&p.b); }
   SRL_DEVINL static int num_kblocks(const Params& p, int, int) { return (p.R + 63) >> 6; }

@@ -42,6 +42,17 @@ struct TFcFwd {
 #pragma unroll
     for (int j = 0; j < 4; ++j) o[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
   }
+  // bf16 mode: the 128 x 64 fp32 tile leaves as 16-byte pieces e = s * 256 + t (row q = e >> 4, piece k = e & 15): a warp stores
+  // two whole 256-byte row pieces of hpart, where a row per thread touched 32 rows 2 KB apart per store
+  static constexpr int TILE_ROWB = 4 * BN + 32;
+  SRL_DEVINL static void epilogue_tile(const Params& p, int tm, int ty, int t, const uint8_t* img, const uint4 (&)[1][2]) {
+    float* out = p.out + (size_t)(ty % SPLITS) * p.M * 512 + (ty / SPLITS) * 64;
+#pragma unroll
+    for (int s = 0; s < 8; ++s) {
+      const int e = s * 256 + t, q = e >> 4, k = e & 15, m = tm * 128 + q;
+      if (m < p.M) *reinterpret_cast<float4*>(out + (size_t)m * 512 + k * 4) = *reinterpret_cast<const float4*>(img + q * TILE_ROWB + k * 16);
+    }
+  }
 };
 
 struct TFcDgrad {
@@ -87,6 +98,30 @@ struct TFcDgrad {
       store_bf16x16(p.da3_lo + o, r);
     }
   }
+  // bf16 mode: the tile (128 frames x 64 channels of one pixel) leaves as 16-byte pieces e = s * 256 + t (frame q = e >> 3, channels
+  // 8k.. with k = e & 7): a warp loads four whole 128-byte mask rows of a3 and stores four whole da3 pixel rows, where a row per
+  // thread touched 32 frames 10,368 bytes apart per store.  Masking the rounded value gives the bits of rounding the masked one.
+  static constexpr int TILE_ROWB = 4 * BN + 32;
+  SRL_DEVINL static void prefetch_tile(const Params& p, int tm, int ty, int t, uint4 (&mk)[2][2]) {
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int e = s * 256 + t, m = tm * 128 + (e >> 3);
+      if (m < p.M) mk[s >> 1][s & 1] = ldg16(p.a3 + (size_t)m * 3136 + ty * 64 + (e & 7) * 8);
+    }
+  }
+  SRL_DEVINL static void epilogue_tile(const Params& p, int tm, int ty, int t, const uint8_t* img, const uint4 (&mk)[2][2]) {
+    bf16* out = p.da3 + ((ty / 7) * 9 + ty % 7) * 64;
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int e = s * 256 + t, q = e >> 3, k = e & 7, m = tm * 128 + q;
+      if (m >= p.M) continue;
+      const float4 a = *reinterpret_cast<const float4*>(img + q * TILE_ROWB + k * 32), b = *reinterpret_cast<const float4*>(img + q * TILE_ROWB + k * 32 + 16);
+      const uint4 w = mk[s >> 1][s & 1];
+      *reinterpret_cast<uint4*>(out + (size_t)m * 81 * 64 + k * 8) =
+          make_uint4(relu_mask_bf16x2(pack_bf16x2(a.x, a.y), w.x), relu_mask_bf16x2(pack_bf16x2(a.z, a.w), w.y),
+                     relu_mask_bf16x2(pack_bf16x2(b.x, b.y), w.z), relu_mask_bf16x2(pack_bf16x2(b.z, b.w), w.w));
+    }
+  }
 };
 
 SRL_DEVINL void fill_ones(uint8_t* dst, int bytes, int tid) {   // bf16 1.0 = 0x3F80
@@ -98,7 +133,7 @@ SRL_DEVINL void fill_ones(uint8_t* dst, int bytes, int tid) {   // bf16 1.0 = 0x
 struct TFcWgrad {
   static constexpr int KID = 33;        // diagnostics timeline id
   static constexpr bool PREFETCH = false;   // grid = (1, 4*50): ty = hw*4 + jt, hw == 49 is the ones slice (B = ones -> dbfc); stage = 64 frames
-  static constexpr int BN = 64, STAGES = 4, KROWS = 64;
+  static constexpr int BN = 64, STAGES = 4, KROWS = 64, TILE_ROWB = 0;
   static constexpr bool A_MN = true, B_MN = true, ZERO_INIT = true;
   struct Params { SRL_TMAP dhm; SRL_TMAP a3m; SRL_TMAP dhm_lo; SRL_TMAP a3m_lo; float* dw; float* db; int M; };
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.dhm); tma_prefetch_desc(&p.a3m); }
@@ -175,6 +210,24 @@ struct TFcWgradN {
       }
     } else if (c0 == 0) {
       p.db[j] = v[0];
+    }
+  }
+  // bf16 mode: the 128 x 256 fp32 tile (128 KB, in the stage ring) leaves as 16-byte pieces, consecutive threads on consecutive pieces
+  // of a dW row: a warp stores 512 contiguous bytes, where a row per thread touched 32 rows 12,544 bytes apart per store.  The last
+  // column tile holds 64 valid columns (16 pieces per row); the bias slice stores column 0 as db.
+  static constexpr int TILE_ROWB = 4 * BN + 32;
+  SRL_DEVINL static void epilogue_tile(const Params& p, int, int ty, int t, const uint8_t* img, const uint4 (&)[1][2]) {
+    const int j0 = (ty & 3) * 128, ct = ty >> 2;
+    if (ct == NCT) {
+      if (t < 128) p.db[j0 + t] = *reinterpret_cast<const float*>(img + t * TILE_ROWB);
+      return;
+    }
+    float* dw = p.dw + (size_t)j0 * 3136 + ct * 256;
+    const int lg = ct == NCT - 1 ? 4 : 6;                         // log2 of the valid 16-byte pieces per row
+#pragma unroll 8
+    for (int e = t; e < 128 << lg; e += 256) {
+      const int q = e >> lg, k = e & ((1 << lg) - 1);
+      *reinterpret_cast<float4*>(dw + (size_t)q * 3136 + k * 4) = *reinterpret_cast<const float4*>(img + q * TILE_ROWB + k * 16);
     }
   }
 };
