@@ -16,6 +16,11 @@ int srl_test_shifted_operand(const void* A, const void* B, float* D, int shift, 
 int srl_test_poison_smem(void* stream);
 /* programmatic-dependent-launch self test; every out[0..nblk) must read 1 (flag, out: device int buffers) */
 int srl_test_pdl(int* flag, int* out, int nblk, unsigned delay_ns, void* stream);
+/* where srl_encoder_forward / srl_encoder_backward put a named row of their saved and scratch blocks (both as srl_encoder_sizes sized
+ * them for `frames` and `precision`): the same carving of the same table (kernels.h encoder_rows).  name: xs, a1, a2, a3, h, wpack,
+ * dh, da3, da2, da1, wgrad_part or a3t.  *hi receives the row's address, *lo its low twin's (NULL in the bf16 mode and for rows
+ * without one), *count its elements. */
+int srl_test_encoder_row(int frames, int precision, const char* name, void* saved, void* scratch, void** hi, void** lo, int64_t* count);
 /* one fused clip + optimizer step (the cooperative kernel srl_learner_apply_gradients and srl_apex_learner_step run) on flat f32
  * device buffers of any n >= 1.  optimizer 0 = RMSprop: s0 = square_avg, a = alpha (b, s1 unused); 1 = Adam: s0 = exp_avg,
  * s1 = exp_avg_sq, a, b = beta1, beta2.  coef f32[3] receives {norm, clip coefficient, lr of the step (but for constant-lr RMSprop

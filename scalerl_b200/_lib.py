@@ -126,6 +126,7 @@ _HOOK_SIGS = {
     'srl_test_poison_smem': [_P],
     'srl_test_pdl': [_P, _P, _I, C.c_uint, _P],
     'srl_test_clip_optim': [_I, _P, _P, _P, _P, _L, _F, _P, _P, _F, _F, _F, _F, _I, _P, _I, _F, C.c_double, C.c_double, _P, _F, _P, _P, _P],
+    'srl_test_encoder_row': [_I, _I, C.c_char_p, _P, _P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_L)],
 }
 HOOK_EXPORTS = sorted(list(_HOOK_SIGS) + ['srl_test_last_error'])
 HOOKS_PATH = os.path.join(_HERE, 'libscalerl_b200_testhooks.so')

@@ -222,28 +222,7 @@ static int check_cfg(const srl_config_t* c) {
 // creation (the zeros of the da*g grids are the padding of the transposed convolutions).  In the fp32-accurate operand mode a row
 // with a low twin is followed by the twin, which srl_learner_debug_buffer calls "<name>_lo".  Rows without a name are internal.
 constexpr int WS_MAX_ROWS = 32;
-// The encoder's rows, for NF forward and NB backward frames.  The first ENC_SAVED_ROWS are what a backward reads of its forward: the
-// activations and the packed weights the forward ran with.  The rest live for one call: the fc layer's split-K partials (forward),
-// the gradient operands and the wgrad partials (backward).  da3, da2 and da1 are adjacent, low twins included: one memset clears them.
-constexpr int ENC_SAVED_ROWS = 6, ENC_ROWS = 13;
-static int encoder_rows(EncoderBuffers& b, int64_t NF, int64_t NB, WsRow* t) {
-  OperandTensors &hi = b.hi, &lo = b.lo;
-  int n = 0;
-  t[n++] = ws_row("xs", NF * 441 * 64, &b.xs);
-  t[n++] = ws_row("a1", NF * 400 * 32, &hi.a1, &lo.a1);
-  t[n++] = ws_row("a2", NF * 81 * 64, &hi.a2, &lo.a2);
-  t[n++] = ws_row("a3", NF * 49 * 64, &hi.a3, &lo.a3);
-  t[n++] = ws_row("h", NF * 512, &b.h);
-  t[n++] = ws_row("wpack", WPack::TOTAL, &hi.wpack, &lo.wpack);
-  t[n++] = ws_row(nullptr, FC_SPLITS * NF * 512, &b.hpart);
-  t[n++] = ws_row("dh", NB * 512, &hi.dh, &lo.dh);
-  t[n++] = ws_row("da3", NB * 81 * 64, &hi.da3, &lo.da3);      // da3g (9x9 grid)
-  t[n++] = ws_row("da2", NB * 100 * 64, &hi.da2, &lo.da2);     // da2g (10x10 grid)
-  t[n++] = ws_row("da1", NB * 441 * 32, &hi.da1, &lo.da1);     // da1g (21x21 grid, 32 channels)
-  t[n++] = ws_row("wgrad_part", WSP_TOTAL, &b.wgrad_part);
-  t[n++] = ws_row("a3t", NF * 49 * 64, &b.a3t);
-  return n;
-}
+// (the encoder's rows: encoder_rows, kernels.h)
 static int workspace_table(srl_learner* L, WsRow* t) {
   const srl_config_t& c = L->cfg;
   const int64_t NF = (int64_t)(c.T + 1) * c.B, NB = (int64_t)c.T * c.B, A = c.A, H = 513 + A;

@@ -438,6 +438,30 @@ struct EncoderBuffers {   // row layouts: see res_problems.cuh
   float* wgrad_part;                    // per-CTA partials of the conv wgrad kernels (WSP_TOTAL floats)
   int NF;                               // frames the forward buffers were sized for (plane stride of a1)
 };
+// The encoder's rows, for NF forward and NB backward frames.  The first ENC_SAVED_ROWS are what a backward reads of its forward: the
+// activations and the packed weights the forward ran with.  The rest live for one call: the fc layer's split-K partials (forward),
+// the gradient operands and the wgrad partials (backward).  da3, da2 and da1 are adjacent, low twins included: one memset clears them.
+// The learner's workspace (api.cu), the stand-alone encoder's two blocks (api.cu) and the test hook that names a row of those blocks
+// (testhooks.cu) all carve this one table.
+constexpr int ENC_SAVED_ROWS = 6, ENC_ROWS = 13;
+inline int encoder_rows(EncoderBuffers& b, int64_t NF, int64_t NB, WsRow* t) {
+  OperandTensors &hi = b.hi, &lo = b.lo;
+  int n = 0;
+  t[n++] = ws_row("xs", NF * 441 * 64, &b.xs);
+  t[n++] = ws_row("a1", NF * 400 * 32, &hi.a1, &lo.a1);
+  t[n++] = ws_row("a2", NF * 81 * 64, &hi.a2, &lo.a2);
+  t[n++] = ws_row("a3", NF * 49 * 64, &hi.a3, &lo.a3);
+  t[n++] = ws_row("h", NF * 512, &b.h);
+  t[n++] = ws_row("wpack", WPack::TOTAL, &hi.wpack, &lo.wpack);
+  t[n++] = ws_row(nullptr, FC_SPLITS * NF * 512, &b.hpart);
+  t[n++] = ws_row("dh", NB * 512, &hi.dh, &lo.dh);
+  t[n++] = ws_row("da3", NB * 81 * 64, &hi.da3, &lo.da3);      // da3g (9x9 grid)
+  t[n++] = ws_row("da2", NB * 100 * 64, &hi.da2, &lo.da2);     // da2g (10x10 grid)
+  t[n++] = ws_row("da1", NB * 441 * 32, &hi.da1, &lo.da1);     // da1g (21x21 grid, 32 channels)
+  t[n++] = ws_row("wgrad_part", WSP_TOTAL, &b.wgrad_part);
+  t[n++] = ws_row("a3t", NF * 49 * 64, &b.a3t);
+  return n;
+}
 // tensor maps of the TMA kernels (built once per learner context: every operand buffer is fixed).
 // Activations are [rows][64] bf16; "w" = window box (128 + max tap shift rows), "b" = 128-row box.
 struct OperandMaps {      // the maps over one OperandTensors set

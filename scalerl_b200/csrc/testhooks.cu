@@ -5,6 +5,7 @@
 // depend on stale shared memory), and the fused clip + optimizer step of optim.cu at any size (the learners only run it
 // on their own parameter counts).
 #include <stdlib.h>
+#include <string.h>
 #include "../../include/scalerl_b200_testhooks.h"
 #include "errors.h"
 #include "kernels.h"
@@ -34,6 +35,25 @@ extern "C" int srl_test_pdl(int* flag, int* out, int nblk, unsigned delay_ns, vo
 }
 extern "C" int srl_test_poison_smem(void* stream) {
   CU(test_poison_smem((cudaStream_t)stream), "test_poison_smem");
+  return 0;
+}
+
+extern "C" int srl_test_encoder_row(int frames, int precision, const char* name, void* saved, void* scratch, void** hi, void** lo,
+                                    int64_t* count) {
+  REQ(name && saved && scratch && hi && lo && count, "test_encoder_row: NULL argument");
+  REQ(frames >= 1 && frames <= MAX_FRAMES, "test_encoder_row: frames=%d must be in [1, %d]", frames, MAX_FRAMES);
+  REQ(precision == 0 || precision == 1, "test_encoder_row: precision=%d must be 0 (bf16 operands) or 1 (fp32-accurate split operands)",
+      precision);
+  EncoderBuffers b = {};
+  WsRow t[ENC_ROWS];
+  encoder_rows(b, frames, frames, t);
+  int i = 0;
+  while (i < ENC_ROWS && !(t[i].name && strcmp(t[i].name, name) == 0)) ++i;
+  REQ(i < ENC_ROWS, "test_encoder_row: unknown row '%s'", name);
+  CU(carve_blocks(t, ENC_ROWS, ENC_SAVED_ROWS, precision == 1, saved, scratch), "test_encoder_row");
+  *hi = *t[i].hi;
+  *lo = precision == 1 && t[i].lo ? *t[i].lo : nullptr;
+  *count = t[i].count;
   return 0;
 }
 

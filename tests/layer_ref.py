@@ -198,8 +198,9 @@ def ordered_bits(x_bf16):
     return torch.where(i < 0, -(i & 0x7FFF), i)
 
 
-def compare_stored(got_hi, got_lo, ref, pre=None, terms=None):
-    """A bf16-stored output (got_lo: the split mode's low twin) against the fp64 result `ref`.
+def compare_stored(got_hi, got_lo, ref, pre=None, terms=None, rms_ref=None, rms_pre=None):
+    """A bf16-stored output (got_lo: the split mode's low twin) against the fp64 result `ref`.  rms_ref / rms_pre: the rms of the
+    whole tensor when `ref` / `pre` is one slice of it (a tensor compared slice by slice); by default the slice's own.
 
     `pre` (ReLU outputs): the fp64 pre-activation; where the GPU's mask disagrees with it the unit must be a tie,
     |pre| < TIE * rms(pre), and it is left out of the value comparison.
@@ -214,11 +215,11 @@ def compare_stored(got_hi, got_lo, ref, pre=None, terms=None):
     if pre is not None:
         pre = pre.to(F64).reshape(-1)
         flip = (got > 0) != (pre > 0)
-        rms_z = float(pre.pow(2).mean().sqrt()) if pre.numel() else 0.0
+        rms_z = rms_pre if rms_pre is not None else float(pre.pow(2).mean().sqrt()) if pre.numel() else 0.0
         st['mask_flips'] = int(flip.sum())
         st['worst_flip_margin'] = float(pre[flip].abs().max() / max(rms_z, 1e-300)) if bool(flip.any()) else 0.0
         keep = ~flip
-    rms = float(ref.pow(2).mean().sqrt()) if ref.numel() else 0.0
+    rms = rms_ref if rms_ref is not None else float(ref.pow(2).mean().sqrt()) if ref.numel() else 0.0
     err = (got - ref).abs()
     acc = torch.full_like(ref, TIE * rms)
     if terms is not None:

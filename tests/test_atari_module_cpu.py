@@ -121,6 +121,27 @@ def test_entry_points_reject_bad_arguments_before_any_cuda_call(lib):
         assert L.srl_encoder_destroy(h) == 0
 
 
+def test_encoder_row_hook_argument_errors(lib):
+    """srl_test_encoder_row (the test hook that names a row of the encoder's blocks) rejects what srl_encoder_sizes rejects, NULL
+    arguments and unknown rows before any CUDA call"""
+    H = _lib.hooks()
+    err = lambda: H.srl_test_last_error().decode()
+    hi, lo, n = C.c_void_p(), C.c_void_p(), C.c_int64()
+    saved, scratch = 1 << 40, (1 << 40) + (1 << 36)
+    row = lambda frames=8, prec=0, name=b'a1', s=saved, k=scratch, out=(C.byref(hi), C.byref(lo), C.byref(n)): \
+        H.srl_test_encoder_row(frames, prec, name, s, k, *out)
+    for frames in (0, -1, 65537):
+        assert row(frames=frames) == -1 and f'frames={frames}' in err()
+    assert row(prec=2) == -1 and 'precision=2' in err()
+    assert row(name=None) == -1 and 'NULL' in err()
+    assert row(s=None) == -1 and 'NULL' in err()
+    assert row(k=None) == -1 and 'NULL' in err()
+    assert row(out=(None, C.byref(lo), C.byref(n))) == -1 and 'NULL' in err()
+    assert row(out=(C.byref(hi), C.byref(lo), None)) == -1 and 'NULL' in err()
+    for bad in (b'hpart', b'', b'a1_lo', b'da0', b'logits'):
+        assert row(name=bad) == -1 and 'unknown row' in err(), bad
+
+
 def test_every_output_against_every_other_argument(lib):
     """each output of srl_encoder_forward / _backward placed on each other argument is rejected before any CUDA call"""
     L = lib

@@ -40,16 +40,34 @@ def test_bf16_tail_against_fp64_and_encoder_backward(B, A, double):
     cases.check_bf16_tail_and_encoder_backward(PLAIN, B, A, double)
 
 
+@pytest.mark.parametrize('B', [4097, 65536])
+def test_bf16_tail_and_encoder_backward_large_batch(B):
+    """above B = 512: the tail's block count, the head weight-gradient slabs and the three forwards at a ragged batch and at
+    MAX_FRAMES"""
+    cases.check_bf16_tail_and_encoder_backward(PLAIN, B, 6, True)
+
+
 # ---------------------------------------------------------------------------------------------------------------- 3
 def test_priorities_reach_the_trees():
-    B, A, mem = 48, 6, 64
+    B, mem = 48, 64
+    _check_priorities(B, mem, ((2, 7), (0, B - 1)))          # repeated indices: the last occurrence wins
+
+
+def test_priorities_reach_the_trees_across_launches():
+    """srl_per_update_priorities writes 1024 pairs per launch: at B = 2500 (three launches) a repeated index keeps its LAST
+    occurrence across launches too"""
+    _check_priorities(2500, 3000, ((5, 1024), (1023, 1024), (1023, 2048), (100, 1500), (1030, 2100), (0, 2499), (2, 7)))
+
+
+def _check_priorities(B, mem, repeats):
+    A = 6
     on, tg = nets(PLAIN, A)
     step_batch, w = batch(B, A, seed=11, device='cuda')
     S = GpuPrioritizedSampler(mem, alpha=0.6)
     S.add(mem)
     idxs = torch.randint(0, mem, (B,), generator=torch.Generator().manual_seed(5))
-    idxs[7] = idxs[2]
-    idxs[B - 1] = idxs[0]                     # repeated indices: the last occurrence wins
+    for first, later in repeats:
+        idxs[later] = idxs[first]
     L = learner(PLAIN, B, A, on, tg, priority_eps=1e-6)
     L.learn(step_batch, weights=w, idxs=idxs.cuda(), sampler=S, use_graph=False)
     prio = L.debug_buffer('priorities').cpu().numpy()
