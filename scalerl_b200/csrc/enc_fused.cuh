@@ -66,10 +66,6 @@ SRL_DEVINL void mbar_wait_relaxed(uint64_t* bar, uint32_t parity) {
     if (++spins > SRL_SPIN_LIMIT) __trap();
   }
 }
-SRL_DEVINL void bulk_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
 
 __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncFusedParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -160,7 +156,7 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
     }
   } else if (warp >= 8) {
     // ------------------------------------------------------------------------------------------------ converters (256 threads)
-    // thread = (16-byte chunk gp = (c, dy pair), row slot rb); rows rb, rb + 32, ... of the 150-row tile: two u32 (2 x 4 dx bytes) -> 8 bf16
+    // thread = (16-byte chunk gp = (c, dy pair), row slot rb); rows rb, rb + 32, ... of the 150-row tile (S2dWindow)
     const int t = tid - 256, gp = t & 7, rb = t >> 3;
     const int src_g = (gp >> 1) * 7056 + (gp & 1) * 168;           // (c, dy0 = 2 (gp & 1)) offset inside the u8 frame
     for (int it = 0; it < nmine; ++it) {
@@ -171,35 +167,12 @@ __global__ void __launch_bounds__(FF_THREADS, 1) enc_fused_fwd_kernel(const EncF
       for (int j = 0; j < 4; ++j) {
         const int n = 4 * it + j, s = n % FF_XS;
         // all ten source words of the thread's five rows first (the compiler cannot hoist shared loads above the shared stores below)
-        uint32_t w0[5], w1[5];
-        int Qs[5];
-        {
-          int Q = j * 128 + rb, Y = Q / 21, X = Q - Y * 21;
-#pragma unroll
-          for (int k = 0; k < 5; ++k) {
-            Qs[k] = Q;
-            if (rb + 32 * k < 150 && Q < 441) {
-              w0[k] = *reinterpret_cast<const uint32_t*>(u8 + Y * 336 + 4 * X);
-              w1[k] = *reinterpret_cast<const uint32_t*>(u8 + Y * 336 + 84 + 4 * X);
-            }
-            Q += 32; X += 11; Y += 1;                     // 32 = 21 + 11
-            if (X >= 21) { X -= 21; Y += 1; }
-          }
-        }
+        S2dWindow<32> win;
+        win.load(u8, rb, j * 128, 441);
         mbar_wait(&x_empty[s], ((n / FF_XS) & 1) ^ 1);    // on the critical cycle (MMA commit -> refill): tight poll
-        uint8_t* x = sX + s * FF_X_BYTES;
-#pragma unroll
-        for (int k = 0; k < 5; ++k) {
-          const int row = rb + 32 * k;
-          if (row < 150) {
-            uint4 v = make_uint4(0u, 0u, 0u, 0u);
-            if (Qs[k] < 441) {
-              v = u8x8_to_bf16x8(w0[k], w1[k]);
-              if (row < 128) *reinterpret_cast<uint4*>(xs_f + (size_t)Qs[k] * 64) = v;     // conv1 wgrad's operand
-            }
-            *reinterpret_cast<uint4*>(x + swz128(row, gp)) = v;
-          }
-        }
+        win.store(sX + s * FF_X_BYTES, gp, rb, [&](int row, uint4 v) {
+          if (row < 128) *reinterpret_cast<uint4*>(xs_f + (size_t)(j * 128 + row) * 64) = v;     // conv1 wgrad's operand
+        });
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) mbar_arrive(&x_full[s]);

@@ -260,6 +260,7 @@ cudaError_t build_tma_maps(const EncoderBuffers& b, int NF, int NB, TmaMaps* M, 
   return mk.failed ? cudaErrorInvalidValue : cudaSuccess;
 }
 
+// frames = 0: only the weight-copy blocks (conv1 converts the frames itself: RConv1Fwd::FromFrames)
 static cudaError_t launch_s2d(const uint8_t* obs, int frames, bf16* xs, cudaStream_t st, const float* w1, bf16* w1k, bf16* w1k_lo) {
   constexpr int WB = (32 * 256 + 351) / 352;      // extra blocks that write conv1's weight copy
   SRL_TRY(launch_chain(obs_s2d_kernel, dim3(frames + WB), dim3(352), 0, st, obs, xs, frames, w1, w1k, w1k_lo));
@@ -380,9 +381,18 @@ cudaError_t encoder_forward(const uint8_t* obs, int frames, const ParamPtrs& p, 
     S.b(PS_ENC_FUSED); SRL_TRY(enc_fused_fwd_launch(q, kPersistentCtas, st)); S.e(PS_ENC_FUSED);
     SRL_TRY(S.join(LANE_PACK));      // conv3 / fc read the packed weights
   } else {
-  S.b(PS_S2D); SRL_TRY(launch_s2d(obs, frames, buf.xs, st, p.w1, buf.hi.wpack + WPack::W1K, sp ? buf.lo.wpack + WPack::W1K : nullptr)); S.e(PS_S2D);
+  // bf16 mode with 16-byte aligned frames (the bulk copies' alignment): conv1 converts its windows from the frames and writes xs itself,
+  // and the frame-conversion kernel only writes conv1's weight copy.  The fp32-accurate mode and 4-byte aligned frames convert the
+  // frames to xs first and feed conv1 from xs.
+  const bool u8_feed = !sp && (reinterpret_cast<uintptr_t>(obs) & 15) == 0;
+  S.b(PS_S2D);
+  SRL_TRY(launch_s2d(obs, u8_feed ? 0 : frames, buf.xs, st, p.w1, buf.hi.wpack + WPack::W1K, sp ? buf.lo.wpack + WPack::W1K : nullptr));
+  S.e(PS_S2D);
   { RConv1Fwd::Params q{maps.xs_w, maps.hi.w1k, maps.lo.w1k, p.b1, buf.hi.a1, buf.lo.a1, frames, buf.NF};
-    S.b(PS_CONV1_FWD); SRL_TRY(res_fwd_launch<RConv1Fwd>(q, cdiv(frames * 441, 128), kPersistentCtas, st, sp)); S.e(PS_CONV1_FWD); }
+    S.b(PS_CONV1_FWD);
+    if (u8_feed) SRL_TRY((res_fwd_launch_t<RConv1Fwd::FromFrames, 0>(RConv1Fwd::FromFrames::Params{q, obs, buf.xs}, cdiv(frames * 441, 128), kPersistentCtas, st)));
+    else SRL_TRY(res_fwd_launch<RConv1Fwd>(q, cdiv(frames * 441, 128), kPersistentCtas, st, sp));
+    S.e(PS_CONV1_FWD); }
   SRL_TRY(S.join(LANE_PACK));      // conv1's weight copy comes from the frame-conversion kernel; conv2 is the first reader of the re-packed copies
   { RConv2Fwd::Params q{maps.hi.a1p0_w, maps.hi.a1p1_w, maps.hi.w2k, maps.lo.a1p0_w, maps.lo.a1p1_w, maps.lo.w2k, p.b2, buf.hi.a2, buf.lo.a2, frames};
     S.b(PS_CONV2_FWD); SRL_TRY(res_fwd_launch<RConv2Fwd>(q, cdiv(frames * 100, 128), kPersistentCtas, st, sp)); S.e(PS_CONV2_FWD); }

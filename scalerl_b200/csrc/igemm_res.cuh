@@ -25,11 +25,13 @@
 //                       one chunk's MMAs in flight while they issue the next.
 #pragma once
 #include "igemm_tma.cuh"
+#include "encoder_problems.cuh"
 
 namespace srl {
 
 constexpr int RES_THREADS = 384;      // res_fwd_kernel: two consumer warpgroups + the producer warpgroup
-// register budgets (per thread, setmaxnreg) of res_fwd_kernel: one warp of each warpgroup per sub-partition, 40 + 2 x 232 <= 512
+// register budgets (per thread, setmaxnreg) of res_fwd_kernel: one warp of each warpgroup per sub-partition, 40 + 2 x 232 <= 3 x 168
+// (the launch allocation, which the budgets only redistribute)
 constexpr int RES_PRODUCER_REGS = 40, RES_CONSUMER_REGS = 232;
 constexpr int RES_MAX_TAPS = 10;
 
@@ -74,6 +76,14 @@ struct ResFwdCfg {
   static constexpr int WIN_BYTES = ((P::WROWS * 128 + 1023) / 1024) * 1024;
   static constexpr int IN_HI_BYTES = P::NWIN * WIN_BYTES;
   static constexpr int IN_BYTES = IN_HI_BYTES * (1 + ALO);
+  // U8: the producer warpgroup converts each window from u8 frame rows staged beside it (U8_BYTES per stage, RConv1Fwd::FromFrames); the
+  // converters' registers come from the consumers
+  static constexpr bool U8 = P::U8_BYTES > 0;
+  static constexpr int U8_BYTES = P::U8_BYTES;
+  static_assert(!U8 || (!SPLIT && P::NWIN == 1), "u8-fed windows: bf16 mode, one window");
+  static constexpr int PRODUCER_REGS = U8 ? 72 : RES_PRODUCER_REGS, CONSUMER_REGS = U8 ? 216 : RES_CONSUMER_REGS;
+  // setmaxnreg moves registers inside the CTA's launch allocation (168 per thread): the consumers can only claim what the producer gave back
+  static_assert(PRODUCER_REGS + 2 * CONSUMER_REGS <= 3 * (65536 / RES_THREADS & ~7), "register budgets within the launch allocation");
   static constexpr int W_HI_BYTES = P::NT * P::BN * 128;
   static constexpr int W_BYTES = W_HI_BYTES * (1 + SPLIT);
   // the output tile leaves through a bf16 image in shared memory (bf16 mode of the problems that define one), or row by row
@@ -84,13 +94,39 @@ struct ResFwdCfg {
   static constexpr int IMG_BYTES = TILE_EPI ? TILE_IMG_BYTES : IMG1 ? WG_IMG_BYTES / 2 : WG_IMG_BYTES;
   // the two consumer warpgroups take alternate tiles: with an even depth every stage (and every phase of its barrier) belongs to one
   // warpgroup, so a warpgroup never waits for phase k of a stage whose phase k-1 (the other warpgroup's tile) may still be filling
-  static constexpr int FIT = fit_stages(SPLIT ? P::SPLIT_STAGES : P::STAGES, W_BYTES + 2 * IMG_BYTES + 1024 + 256, IN_BYTES);
+  static constexpr int FIT = fit_stages(SPLIT ? P::SPLIT_STAGES : P::STAGES, W_BYTES + 2 * IMG_BYTES + 1024 + 256, IN_BYTES + U8_BYTES);
   static constexpr int STAGES = FIT > 1 ? FIT & ~1 : 1;
-  static constexpr int SMEM_BYTES = W_BYTES + STAGES * IN_BYTES + 2 * IMG_BYTES + 1024 + 256;
+  static constexpr int SMEM_BYTES = W_BYTES + STAGES * (IN_BYTES + U8_BYTES) + 2 * IMG_BYTES + 1024 + 256;
   static_assert(SMEM_BYTES <= 232448, "shared memory budget (227 KB)");
   static_assert(W_BYTES % 1024 == 0, "weight block alignment");
   static_assert(P::BN == 32 || P::BN == 64 || P::BN == 128, "MMA N");
 };
+
+// Converter warps 9-11 of a u8-fed res_fwd_kernel (C::U8): tile it's window, from the source rows staged in u8 stage it % STAGES,
+// into input stage it % STAGES, and its rows 0..127 that lie inside the frames to xs (a warp's store is 4 whole, consecutive xs rows)
+template <class P, class C>
+SRL_DEVINL void res_u8_converters(const typename P::Params& p, uint8_t* sIn, uint8_t* sU8, uint64_t* in_full, uint64_t* in_empty,
+                                  uint64_t* u8_full, uint64_t* u8_empty, int tid) {
+  constexpr int STAGES = C::STAGES;
+  static_assert(P::CONV_SLOTS == 12, "warps 9-11");
+  const int ct = tid - 288, gp = ct & 7, rb = ct >> 3;
+  const int ntiles = P::num_tiles(p), qend = p.NF * 441;
+  const int plane = (gp >> 1) * P::U8_PLANE + (gp & 1) * 168;       // chunk gp's channel plane c and source row dy = 2 (gp & 1)
+  int it = 0;
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
+    const int s = it % STAGES, q0 = t * 128, r0 = q0 / 21;
+    const uint32_t ph = (it / STAGES) & 1;
+    S2dWindow<P::CONV_SLOTS> w;
+    mbar_wait(&u8_full[s], ph);
+    w.load(sU8 + s * C::U8_BYTES + plane, rb, q0 - r0 * 21, qend - r0 * 21);
+    mbar_wait(&in_empty[s], ph ^ 1);
+    bf16* xs = p.xs + (size_t)q0 * 64 + gp * 8;
+    w.store(sIn + s * C::IN_BYTES, gp, rb, [&](int row, uint4 v) { if (row < 128) *reinterpret_cast<uint4*>(xs + (size_t)row * 64) = v; });
+    fence_proxy_async_smem();                        // the window's generic stores -> the MMAs' reads
+    __syncwarp();
+    if ((tid & 31) == 0) { mbar_arrive(&u8_empty[s]); mbar_arrive(&in_full[s]); }    // the stores consumed every staged word read
+  }
+}
 
 template <class P, int SPLIT>
 __global__ void __launch_bounds__(RES_THREADS, 1) res_fwd_kernel(const __grid_constant__ typename P::Params p) {
@@ -101,15 +137,20 @@ __global__ void __launch_bounds__(RES_THREADS, 1) res_fwd_kernel(const __grid_co
   uint8_t* sW = smem;
   uint8_t* sIn = smem + C::W_BYTES;
   float* img = reinterpret_cast<float*>(sIn + STAGES * C::IN_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sIn + STAGES * C::IN_BYTES + 2 * C::IMG_BYTES);
+  uint8_t* sU8 = sIn + STAGES * C::IN_BYTES + 2 * C::IMG_BYTES;           // U8 only
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sU8 + STAGES * C::U8_BYTES);
   uint64_t* in_full = bars;
   uint64_t* in_empty = bars + STAGES;
   uint64_t* w_full = bars + 2 * STAGES;
+  uint64_t* u8_full = bars + 2 * STAGES + 1;         // U8 only
+  uint64_t* u8_empty = bars + 3 * STAGES + 1;
   const int tid = threadIdx.x, warp = tid >> 5;
   const int ntiles = P::num_tiles(p);
 
   if (warp == 8 && (tid & 31) == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&in_full[s], 1); mbar_init(&in_empty[s], 4); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&in_full[s], C::U8 ? 3 : 1); mbar_init(&in_empty[s], 4); }
+    if constexpr (C::U8)
+      for (int s = 0; s < STAGES; ++s) { mbar_init(&u8_full[s], 1); mbar_init(&u8_empty[s], 3); }
     mbar_init(w_full, 1);
     mbar_fence_init();
     P::prefetch(p);
@@ -117,8 +158,10 @@ __global__ void __launch_bounds__(RES_THREADS, 1) res_fwd_kernel(const __grid_co
   __syncthreads();
 
   if (warp >= 8) {
-    reg_release<RES_PRODUCER_REGS>();
-    if (warp != 8) return;                 // warps 9-11 only give their registers back
+    reg_release<C::PRODUCER_REGS>();
+    if constexpr (C::U8) {
+      if (warp != 8) { res_u8_converters<P, C>(p, sIn, sU8, in_full, in_empty, u8_full, u8_empty, tid); return; }
+    } else if (warp != 8) return;          // warps 9-11 only give their registers back
     const uint32_t leader = elect_one_sync();      // converged warp, one elected issuing lane: no vote loop around every TMA instruction
     // the packed weights were complete before the first kernel of the chain started: their load overlaps the previous
     // kernel's tail; the activations are only touched after pdl_wait().  (W_AFTER_WAIT: the weights come from the stream predecessor.)
@@ -137,16 +180,21 @@ __global__ void __launch_bounds__(RES_THREADS, 1) res_fwd_kernel(const __grid_co
     int it = 0;
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
       const int s = it % STAGES;
-      mbar_wait(&in_empty[s], ((it / STAGES) & 1) ^ 1);
-      if (leader) {
-        mbar_arrive_expect_tx(&in_full[s], P::NWIN * P::WROWS * 128 * (1 + C::ALO));
-        P::load_windows(p, t, sIn + s * C::IN_BYTES, C::WIN_BYTES, &in_full[s], false);
-        if constexpr (C::ALO) P::load_windows(p, t, sIn + s * C::IN_BYTES + C::IN_HI_BYTES, C::WIN_BYTES, &in_full[s], true);
+      if constexpr (C::U8) {        // the frame rows of the window: up to STAGES tiles ahead of the converters
+        mbar_wait(&u8_empty[s], ((it / STAGES) & 1) ^ 1);
+        if (leader) P::load_u8(p, t, sU8 + s * C::U8_BYTES, &u8_full[s]);
+      } else {
+        mbar_wait(&in_empty[s], ((it / STAGES) & 1) ^ 1);
+        if (leader) {
+          mbar_arrive_expect_tx(&in_full[s], P::NWIN * P::WROWS * 128 * (1 + C::ALO));
+          P::load_windows(p, t, sIn + s * C::IN_BYTES, C::WIN_BYTES, &in_full[s], false);
+          if constexpr (C::ALO) P::load_windows(p, t, sIn + s * C::IN_BYTES + C::IN_HI_BYTES, C::WIN_BYTES, &in_full[s], true);
+        }
       }
       __syncwarp();
     }
   } else {
-    reg_claim<RES_CONSUMER_REGS>();
+    reg_claim<C::CONSUMER_REGS>();
     pdl_wait(P::KID);
     // consumer warpgroup g takes this CTA's tiles it = g, g + 2, ...: its epilogue overlaps the other warpgroup's MMAs.  With a
     // single input stage warpgroup 0 takes every tile: tile it + 2 would be awaited on the same barrier with the parity of the

@@ -37,6 +37,8 @@ struct RConv1Fwd {   // 2x2 s1 over xs (== 8x8 s4 over the frame): taps (kh2,kw2
   // pack_weights_kernel: conv1 then depends only on its stream predecessor and never waits for the re-pack (encoder_forward joins the
   // re-pack stream only before conv2); the weight tiles are therefore loaded AFTER griddepcontrol.wait
   static constexpr bool W_AFTER_WAIT = true;
+  static constexpr int U8_BYTES = 0;        // the windows come from TMA loads of xs (FromFrames: converted from the frames)
+  struct FromFrames;                        // the same GEMM fed straight from the u8 frames
   SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.in0); tma_prefetch_desc(&p.w); }
   SRL_DEVINL static int num_tiles(const Params& p) { return (p.NF * 441 + 127) >> 7; }
   SRL_DEVINL static constexpr int tap_win(int) { return 0; }
@@ -71,9 +73,34 @@ struct RConv1Fwd {   // 2x2 s1 over xs (== 8x8 s4 over the frame): taps (kh2,kw2
   }
 };
 
+// conv1's forward fed straight from the u8 frames (bf16 mode, 16-byte aligned frames).  The producer warpgroup builds each window in
+// shared memory: warp 8 brings in the source rows it covers (one bulk copy per frame and channel plane), warps 9-11 convert them into
+// the SWIZZLE_128B window a TMA load of xs would give (S2dWindow) and write its rows 0..127 -- the tile's own positions -- to xs, conv1
+// wgrad's operand, instead of reading xs back.  The MMAs and the epilogue are RConv1Fwd's on the same operand bytes.
+struct RConv1Fwd::FromFrames : RConv1Fwd {
+  static constexpr int SPAN = 9;                    // rows of the 21x21 grid (or of two frames' grids) a 150-row window touches, at most
+  static constexpr int U8_PLANE = SPAN * 336;       // one channel plane of the staged source rows: a grid row is 4 source rows of 84 B
+  static constexpr int U8_BYTES = 4 * U8_PLANE;     // per ring stage
+  static constexpr int CONV_SLOTS = 12;             // converter threads (warps 9-11) / 8 chunks per row
+  struct Params : RConv1Fwd::Params { const uint8_t* obs; bf16* xs; };
+  SRL_DEVINL static void prefetch(const Params& p) { tma_prefetch_desc(&p.w); }
+  // grid rows r0 .. r1 of tile t's window (positions t * 128 .. t * 128 + 149, clipped to the frames), plane c at dst + c * U8_PLANE
+  SRL_DEVINL static void load_u8(const Params& p, int t, uint8_t* dst, uint64_t* bar) {
+    const int q0 = t * 128, q1 = min(q0 + WROWS, p.NF * 441) - 1, r0 = q0 / 21, r1 = q1 / 21;
+    mbar_arrive_expect_tx(bar, (r1 - r0 + 1) * 4 * 336);
+    for (int ra = r0; ra <= r1;) {                  // a window straddles at most two frames
+      const int n = ra / 21, rz = min(r1, n * 21 + 20);
+      const uint8_t* src = p.obs + (size_t)n * 28224 + (ra - n * 21) * 336;
+      for (int c = 0; c < 4; ++c) bulk_load_1d(dst + c * U8_PLANE + (ra - r0) * 336, src + c * 7056, (rz - ra + 1) * 336, bar);
+      ra = rz + 1;
+    }
+  }
+};
+
 struct RConv2Fwd {   // 4x4 s2 over a1: tap j = (kh, kww): plane kh&1, shift (kh>>1)*10 + kww, K-block = (kh, kw in {2kww, 2kww+1}, c)
   static constexpr int KID = 12;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
+  static constexpr int U8_BYTES = 0;        // the windows come from TMA loads
   static constexpr int BN = 64, NT = 8, NWIN = 2, WROWS = 128 + 11, STAGES = 3, SPLIT_STAGES = 1;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP in1; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP in1_lo; SRL_TMAP w_lo; const float* bias; bf16* out; bf16* out_lo; int NF; };
@@ -115,6 +142,7 @@ struct RConv2Fwd {   // 4x4 s2 over a1: tap j = (kh, kww): plane kh&1, shift (kh
 struct RConv3Fwd {   // 3x3 s1 over a2: tap (kh,kw) -> shift kh*9 + kw
   static constexpr int KID = 13;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
+  static constexpr int U8_BYTES = 0;        // the windows come from TMA loads
   static constexpr int BN = 64, NT = 9, NWIN = 1, WROWS = 128 + 20, STAGES = 4, SPLIT_STAGES = 2;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP w_lo; const float* bias; bf16* out; bf16* out_lo; int NF; };
@@ -152,6 +180,7 @@ struct RConv3Fwd {   // 3x3 s1 over a2: tap (kh,kw) -> shift kh*9 + kw
 struct RConv3Dgrad {   // da2[ih,iw] = sum_{kh,kw} da3g[(ih-kh),(iw-kw)] W3[:, :, kh, kw]: shifts -(kh*9+kw); window starts 20 rows early
   static constexpr int KID = 14;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
+  static constexpr int U8_BYTES = 0;        // the windows come from TMA loads
   static constexpr int BN = 64, NT = 9, NWIN = 1, WROWS = 128 + 20, STAGES = 4, SPLIT_STAGES = 2;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP w_lo; const bf16* act; bf16* dx; bf16* dx_lo; int NB; };
@@ -201,6 +230,7 @@ struct RConv3Dgrad {   // da2[ih,iw] = sum_{kh,kw} da3g[(ih-kh),(iw-kw)] W3[:, :
 struct RConv2Dgrad {   // the 4 stride-parity classes share A (da2g at (i'-kh', j'-kw')): one N = 4 x 32 GEMM; shifts -(kh'*10 + kw')
   static constexpr int KID = 15;        // diagnostics timeline id
   static constexpr bool W_AFTER_WAIT = false;
+  static constexpr int U8_BYTES = 0;        // the windows come from TMA loads
   static constexpr int BN = 128, NT = 4, NWIN = 1, WROWS = 128 + 11, STAGES = 3, SPLIT_STAGES = 2;
   static constexpr bool A_LO = true;
   struct Params { SRL_TMAP in0; SRL_TMAP w; SRL_TMAP in0_lo; SRL_TMAP w_lo; const bf16* act; bf16* dx; bf16* dx_lo; int NB; int NF; };
