@@ -8,9 +8,7 @@ file its measured errors go to under $SRL_RESULTS_DIR.  A row's head setting (K 
 default; a test varies it with ``row.but(...)``."""
 import ctypes as C
 import dataclasses
-import json
 import math
-import os
 from typing import Optional
 
 import numpy as np
@@ -25,6 +23,7 @@ from scalerl_b200.algorithms.apex import ApexHParams, AtariQNet, B200ApexActor, 
 from scalerl_b200.data.per_sampler import GpuPrioritizedSampler
 from scalerl_b200.data.replay_memory import GpuPrioritizedReplayBuffer
 from tests import layer_ref as R
+from tests.exact import record
 
 F64 = torch.float64
 
@@ -61,18 +60,6 @@ def scaled(a, b, scale):
     """max |a - b| over the largest term size of the sums a and b are"""
     a, b = a.detach().cpu().to(F64), b.detach().cpu().to(F64)
     return float((a - b).abs().max() / max(float(scale.abs().max()), 1e-300))
-
-
-def record(results_file, name, obj):
-    """store obj under name in $SRL_RESULTS_DIR/results_file, when SRL_RESULTS_DIR is set"""
-    d = os.environ.get('SRL_RESULTS_DIR')
-    if not d:
-        return
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, results_file)
-    cur = json.load(open(p)) if os.path.exists(p) else {}
-    cur[name] = obj
-    json.dump(cur, open(p, 'w'), indent=1)
 
 
 def unbuilt(cls, **attrs):

@@ -27,12 +27,15 @@ Discrete choices.  a* is an argmax.  pick() returns the fp64 first argmax, the r
 bounds (the tie set): the caller accepts such a row under either action and counts it (<= MAX_TIE_FRAC).  Exact fp64 ties (equal
 rows, tests/apex_cases.py's _tie_*) are not in the tie set: they resolve to the first index, as in the kernels.
 """
+import functools
 import math
 
 import torch
 
+from tests import exact as E
+from tests.exact import U
+
 F64 = torch.float64
-U = 2.0 ** -24
 ETA = 2.0 ** -126
 SENS = 20.0
 MAX_TIE_FRAC = 1e-3
@@ -75,19 +78,10 @@ def t64(x, device=None):
     return x.to(device or x.device, F64)
 
 
-def ratio(got, ref, S, c):
-    """max |got - ref| / (c (U S + ETA)); a NaN on one side only is infinite"""
-    got, ref, S = t64(got), t64(ref).to(got.device), t64(S).to(got.device)
-    diff = (got - ref).abs()
-    q = torch.where(diff == 0, torch.zeros_like(diff), diff / (c * (U * S + ETA)))
-    q = torch.where(got.isnan() != ref.isnan(), torch.full_like(q, math.inf), q)
-    q = torch.where(got.isnan() & ref.isnan(), torch.zeros_like(q), q)
-    return float(q.max()) if q.numel() else 0.0
-
-
-def sensitivity(pert, ref, S, c):
-    """how far a mistake moves the reference, in bounds"""
-    return ratio(pert, ref, S, c)
+# max |got - ref| / (c (U S + ETA)) on the tensors' device, and how far a mistake moves the reference in those units; an output NaN
+# on both sides agrees
+ratio = functools.partial(E.ratio, eta=ETA, nan_equal=True)
+sensitivity = functools.partial(E.sensitivity, eta=ETA, nan_equal=True)
 
 
 def n_loss(B):

@@ -182,6 +182,9 @@ def abs_terms(f, a, b):
 
 # ------------------------------------------------------------------------------------------------ comparisons
 ACC_REL = 2.0 ** -18      # fp32 accumulation error allowance per unit of sum |terms|
+MISMATCH = 5e-3           # the largest fraction of a bf16-stored output that may be one ulp from the rounding of the fp64 result
+
+
 def rel_l2(a, b):
     a, b = a.to(F64), b.to(F64)
     return float((a - b).norm() / max(float(b.norm()), 1e-300))
@@ -244,7 +247,7 @@ def stored_ok(st, split_mode):
         return False
     if split_mode:
         return st['bad'] == 0
-    return st['max_ulp'] <= 1 and st['mismatch_frac'] <= 5e-3
+    return st['max_ulp'] <= 1 and st['mismatch_frac'] <= MISMATCH
 
 
 # ------------------------------------------------------------------------------------------------ wgrad partition (igemm_res.cuh)
@@ -278,6 +281,10 @@ def wgrad_partition(positions, target_ctas):
     return {'chunks': nch, 'chunks_per_cta': cpc, 'grid': grid, 'last_cta_chunks': nch - (grid - 1) * cpc}
 
 
+def sm_count():
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
 def cta_counts(sm_count, env):
     """encoder.cu persistent_ctas / bwd_ctas / side_wgrad_ctas from the SRL_* overrides in `env`"""
     def _int(k):
@@ -302,6 +309,15 @@ def wgrad_partitions(NB, ctas, split_mode):
         d['ring'] = wgrad_ring_depth(name, split_mode)
         out[name] = d
     return out
+
+
+def mid_chunk_frames(NB, G, part):
+    """frames and position mask [n1-n0, 1, G, G] of the first chunk of the middle CTA of a wgrad launch"""
+    q0 = (part['grid'] // 2) * part['chunks_per_cta'] * 128
+    n0, n1 = q0 // (G * G), min(NB, (q0 + 127) // (G * G) + 1)
+    m = torch.zeros((n1 - n0) * G * G, dtype=F64)
+    m[q0 - n0 * G * G:q0 - n0 * G * G + 128] = 1
+    return n0, n1, m.view(n1 - n0, 1, G, G)
 
 
 def regimes(part):

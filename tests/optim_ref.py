@@ -14,9 +14,13 @@ it.  A clipped gradient (or exp_avg) in fp32's subnormal range is only accurate 
 scales it, S carries ETA / U / (sqrt(v) + eps).  sqrtf and the division are correctly rounded (no fast-math).  The norm's sum of squares uses S = n_chain * sum g^2, n_chain the
 longest chain of roundings in the kernel's summation order (n_chain_norm).
 """
+import functools
+
 import numpy as np
 
-U = 2.0 ** -24
+from tests import exact as E
+from tests.exact import U
+
 ETA = 2.0 ** -149           # fp32's smallest subnormal: a rounding in the subnormal range is off by at most half of it, absolutely
 SENS = 20.0
 
@@ -204,20 +208,10 @@ def adam(p, g, m, v, c, lr, b1, b2, eps, t, m_k=None, v_k=None, lr_prev=None, mi
 
 
 # ------------------------------------------------------------------------------------------------ comparisons
-def ratio(got, ref, S, c):
-    """max |got - ref| / (c (U S + ETA)) (0 where both agree exactly; inf where only one is NaN)"""
-    got, ref, S = f64(got), f64(ref), f64(S)
-    with np.errstate(invalid='ignore'):
-        diff = np.abs(got - ref)
-        b = c * (U * S + ETA)
-        q = np.where(diff == 0, 0.0, diff / b)
-    q = np.where(np.isnan(got) != np.isnan(ref), np.inf, np.where(np.isnan(got) & np.isnan(ref), 0.0, q))
-    return float(q.max()) if q.size else 0.0
-
-
-def sensitivity(pert, ref, S, c):
-    """how far a mistake moves the reference, in bounds: max |pert - ref| / (c (U S + ETA))"""
-    return ratio(pert, ref, S, c)
+# max |got - ref| / (c (U S + ETA)), and how far a mistake moves the reference in those units; an output NaN on both sides agrees (a
+# NaN gradient poisons the kernel's weights and the reference's alike)
+ratio = functools.partial(E.ratio, eta=ETA, nan_equal=True)
+sensitivity = functools.partial(E.sensitivity, eta=ETA, nan_equal=True)
 
 
 def loose(v, S, c):

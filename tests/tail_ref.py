@@ -14,9 +14,13 @@ logf within 1 ulp (CUDA C Programming Guide, Mathematical Functions); the projec
 
 MISTAKES are plausible kernel errors; each must move the reference of its witness case by at least SENS x the bound on some element.
 """
+import functools
+
 import numpy as np
 
-U = 2.0 ** -24
+from tests import exact as E
+from tests.exact import U
+
 ETA = 2.0 ** -126           # fp32's smallest normal: a result that underflows keeps only an absolute accuracy, c * ETA is added to each bound
 SENS = 20.0
 
@@ -259,20 +263,10 @@ TAIL_MISTAKES = {'vs': ('cbar_rho', 'clips_swapped', 'boot_zero', 'chunk_carry',
 
 
 # ------------------------------------------------------------------------------------------------ comparisons
-def ratio(got, ref, S, c):
-    """max |got - ref| / (c (U S + ETA)) (0 where both agree exactly)"""
-    got, ref, S = f64(got), f64(ref), f64(S)
-    diff = np.abs(got - ref)
-    b = c * (U * S + ETA)
-    with np.errstate(divide='ignore', invalid='ignore'):
-        q = np.where(diff == 0, 0.0, diff / b)
-    q = np.where(np.isnan(got) != np.isnan(ref), np.inf, q)
-    return float(q.max()) if q.size else 0.0
-
-
-def sensitivity(pert, ref, S, c):
-    """how far a mistake moves the reference, in bounds: max |pert - ref| / (c (U S + ETA))"""
-    return ratio(pert, ref, S, c)
+# max |got - ref| / (c (U S + ETA)), and how far a mistake moves the reference in those units; an output NaN on both sides is NaN, so
+# its check fails
+ratio = functools.partial(E.ratio, eta=ETA, nan_equal=False)
+sensitivity = functools.partial(E.sensitivity, eta=ETA, nan_equal=False)
 
 
 # ------------------------------------------------------------------------------------------------ shared case table and inputs

@@ -69,7 +69,7 @@ def test_gpu_actor_weight_refresh_paths():
 def test_gpu_actor_throughput_is_recorded():
     """actor steps per second at N = 256 environments per call (host tensors in and out, as the actor loop uses it)"""
     from scalerl_b200.algorithms.impala.gpu_actor import B200ActorModel
-    from tests.test_gpu_fullsize import _record
+    from tests.exact import record
     N, A = 256, 6
     gpu = B200ActorModel(N, A)
     env = _env_batch(N, A, 3)
@@ -80,6 +80,6 @@ def test_gpu_actor_throughput_is_recorded():
     for _ in range(n):
         gpu(env, ())
     dt = time.perf_counter() - t0
-    _record('gpu_actor_N256', {'calls_per_sec': n / dt, 'env_steps_per_sec': n * N / dt, 'ms_per_call': dt / n * 1e3})
+    record('parity_fullsize.json', 'gpu_actor_N256', {'calls_per_sec': n / dt, 'env_steps_per_sec': n * N / dt, 'ms_per_call': dt / n * 1e3})
     assert n * N / dt > 2e4
     gpu.close()

@@ -98,7 +98,7 @@ def test_step_matches_fp64_on_its_own_operands(N):
 def test_actor_steps_match_the_learner_rollout(T, B):
     """the behaviour logits of T+1 actor steps and the learner's target logits of the same rollout (the pair V-trace compares)"""
     from scalerl_b200.learner import B200ImpalaLearner, ImpalaHParams
-    from tests.test_gpu_fullsize import _record
+    from tests.exact import record
     sd = _cpu_actor(4).state_dict()
     x = _inputs(T + 1, B, 7, done_p=0.1)
     x['done'][0, :4] = True                       # done at row 0
@@ -114,7 +114,7 @@ def test_actor_steps_match_the_learner_rollout(T, B):
         lg.append(a); bs.append(b)
     err = {'logits': nerr(torch.cat(lg).cpu(), ref['policy_logits'].cpu()), 'baseline': nerr(torch.cat(bs).cpu(), ref['baseline'].cpu()),
            'hT': nerr(state[0].cpu(), hT.cpu()), 'cT': nerr(state[1].cpu(), cT.cpu())}
-    _record(f'actor_lstm_vs_learner_T{T}_B{B}', err)
+    record('parity_fullsize.json', f'actor_lstm_vs_learner_T{T}_B{B}', err)
     assert all(v <= 1e-3 for v in err.values()), err
     gpu.close(); L.close()
 
@@ -249,7 +249,7 @@ def test_trainer_batched_actor_loop(tmp_path):
 
 def test_lstm_actor_throughput_is_recorded():
     """actor steps per second at N = 256 environments per call, host tensors in and out (the state stays on the device)"""
-    from tests.test_gpu_fullsize import _record
+    from tests.exact import record
     N = 256
     gpu = _actor(N)
     env = _inputs(1, N, 3, done_p=0.05)
@@ -261,5 +261,5 @@ def test_lstm_actor_throughput_is_recorded():
     for _ in range(n):
         _, state = gpu(env, state)
     dt = time.perf_counter() - t0
-    _record('gpu_actor_lstm_N256', {'calls_per_sec': n / dt, 'env_steps_per_sec': n * N / dt, 'ms_per_call': dt / n * 1e3})
+    record('parity_fullsize.json', 'gpu_actor_lstm_N256', {'calls_per_sec': n / dt, 'env_steps_per_sec': n * N / dt, 'ms_per_call': dt / n * 1e3})
     gpu.close()

@@ -21,7 +21,8 @@ from oracle.per_oracle import PerOracle
 from scalerl_b200.algorithms.apex import ApexHParams, B200ApexActor, B200ApexLearner, apex_epsilons, default_q_state_dict
 from scalerl_b200.data.replay_memory import GpuPrioritizedReplayBuffer
 from tests import apex_cases as cases
-from tests.apex_cases import frames, nmax, record
+from tests.apex_cases import frames, nmax
+from tests.exact import record
 
 pytestmark = pytest.mark.gpu
 NPIX = 4 * 84 * 84

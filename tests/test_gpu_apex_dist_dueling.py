@@ -24,7 +24,8 @@ import torch
 from scalerl_b200.algorithms.apex import ApexHParams, AtariQNet, B200ApexActor, B200ApexLearner, default_q_state_dict
 from tests import apex_cases as cases
 from tests import apex_dist_dueling_ref as R
-from tests.apex_cases import batch, learner, nmax, record, rel_l2
+from tests.apex_cases import batch, learner, nmax, rel_l2
+from tests.exact import record
 
 pytestmark = pytest.mark.gpu
 

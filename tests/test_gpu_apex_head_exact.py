@@ -15,9 +15,7 @@ GpuPrioritizedReplayBuffer.save_to_memory(..., priorities_from=actor).
 The worst err / bound of every check, its margin and the strongest sensitivity go to $SRL_RESULTS_DIR/apex_head_exact.json (per case,
 and a summary per check)."""
 import ctypes as C
-import json
 import math
-import os
 
 import numpy as np
 import pytest
@@ -28,6 +26,7 @@ from scalerl_b200.algorithms.apex import default_q_state_dict
 from scalerl_b200.data.replay_memory import GpuPrioritizedReplayBuffer
 from tests import apex_cases as AC
 from tests import apex_head_ref as R
+from tests import exact
 
 pytestmark = pytest.mark.gpu
 
@@ -112,78 +111,22 @@ CASES = [
 ]
 
 
-# ------------------------------------------------------------------------------------------------ results
-def _record(name, obj):
-    d = os.environ.get('SRL_RESULTS_DIR')
-    if not d:
-        return
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, RESULTS)
-    cur = json.load(open(p)) if os.path.exists(p) else {}
-    cur[name] = obj
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
+_summary = exact.summary(RESULTS)
 
 
-@pytest.fixture(scope='module', autouse=True)
-def _summary():
-    """after the module: per check, the worst err / bound over every case, its margin, and the strongest sensitivity"""
-    yield
-    d = os.environ.get('SRL_RESULTS_DIR')
-    p = os.path.join(d, RESULTS) if d else None
-    if not p or not os.path.exists(p):
-        return
-    cur = json.load(open(p))
-    table = {}
-    for case, res in cur.items():
-        if case == 'summary':
-            continue
-        for name, e in res.items():
-            if not isinstance(e, dict):
-                continue
-            t = table.setdefault(name, {})
-            for k, v in e.items():
-                if isinstance(v, (int, float)):
-                    t[k] = v if k not in t else (min if k == 'margin' else max)(t[k], v)
-    cur['summary'] = table
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
+def _ties(Ck, name, tie, B):
+    """the a* tie rows (pick()'s tie set) are at most MAX_TIE_FRAC of the batch"""
+    n = int(tie.sum())
+    Ck.res[name] = {'tie_rows': n, 'tie_frac': n / B}
+    if n > max(1, R.MAX_TIE_FRAC * B):
+        Ck.fails.append(f'{name}: {n} tie rows of {B}')
 
 
-class Checker:
-    def __init__(self):
-        self.res, self.fails, self.sens = {}, [], {}
-
-    def bound(self, name, got, ref, S, c, mistakes=None):
-        """got within c U S of ref; mistakes: {mistake: its reference}, whose move in bounds is recorded"""
-        q = R.ratio(got, ref, S, c)
-        e = {'err_over_bound': q, 'margin': 1.0 / q if q > 0 else float('inf')}
-        for m, pert in (mistakes or {}).items():
-            s = R.sensitivity(pert, ref, S, c)
-            self.sens[m] = max(self.sens.get(m, 0.0), s)
-            e[f'sens_{m}'] = min(s, 1e30)
-        self.res[name] = e
-        if not q <= 1.0:
-            self.fails.append(f'{name}: {q:.3f} x the bound')
-
-    def zero(self, name, got):
-        """every element is +0.0 (bits 0)"""
-        n = int((got.contiguous().view(torch.int32) != 0).sum())
-        self.res[name] = {'nonzero': n}
-        if n:
-            self.fails.append(f'{name}: {n} elements are not +0')
-
-    def ties(self, name, tie, B):
-        n = int(tie.sum())
-        self.res[name] = {'tie_rows': n, 'tie_frac': n / B}
-        if n > max(1, R.MAX_TIE_FRAC * B):
-            self.fails.append(f'{name}: {n} tie rows of {B}')
-
-    def done(self, case, witness=()):
-        for m in witness:
-            if not self.sens.get(m, 0.0) >= R.SENS:
-                self.fails.append(f'{m} ({R.MISTAKES[m]}) moves {case} by only {self.sens.get(m, 0.0):.1f} x the bound')
-        self.res['sensitivity'] = {m: min(v, 1e30) for m, v in self.sens.items()}
-        _record(case, self.res)
-        assert not self.fails, '\n'.join(self.fails)
+def _done(Ck, case, witness=()):
+    """the mistakes of `witness` each move some check of the case by >= SENS x its bound; record the case's strongest sensitivities"""
+    Ck.require(case, Ck.sens, witness)
+    Ck.res['sensitivity'] = {m: min(v, 1e30) for m, v in Ck.sens.items()}
+    Ck.done(case)
 
 
 def _nan_fill(L, names):
@@ -270,7 +213,7 @@ def _check_step(cid, head, dd, L, B, A, kw, bt, w, gamma, double, eps, witness, 
     core = lambda n: dbg(n).view(B, 514)
     h, hnt = core('core')[:, :512], core('core_next_target')[:, :512]
     hn = core('core_next')[:, :512] if double else None
-    Ck = Checker()
+    Ck = exact.Checker(RESULTS, R)
     dcore = core('dcore')
     Ck.zero('dcore_pad', dcore[:, 512:])
     g32 = float(np.float32(gamma))
@@ -286,7 +229,7 @@ def _check_step(cid, head, dd, L, B, A, kw, bt, w, gamma, double, eps, witness, 
             Ck.fails.append(f'exact ties: the fp64 a* is not the first index on {n} rows')
     peak = torch.cuda.max_memory_allocated() / 2 ** 30
     Ck.res['memory'] = {'learner_gib': arena, 'reference_peak_gib': peak, 'total_gib': arena + peak}
-    Ck.done(cid, witness)
+    _done(Ck, cid, witness)
 
 
 def _scalar_nets(head, L, sd, net):
@@ -309,28 +252,28 @@ def _scalar(Ck, head, L, pre, pre_t, h, hn, hnt, act, rew, done, w, g32, double,
     mist = {}
     if kind == 'dueling':
         mist['dueling_mean_A_minus_1'] = R.take(R.scalar_q(kind, h, on, 'dueling_mean_A_minus_1')[0], act) if A > 1 else R.take(Q, act)
-    Ck.bound('q', dbg_(L, 'q'), R.take(Q, act), R.take(SQ, act), R.CHECK_C['q'], mist)
+    Ck.bound('q', dbg_(L, 'q'), R.take(Q, act), R.take(SQ, act), R.CHECK_C['q'], mistakes=mist)
     nx1, S1, nx2, S2, tie, a1 = R.scalar_targets(kind, hn, hnt, on, tg, double)
     y1, Sy1 = R.td_target(rew, done, g32, nx1, S1)
     y2, Sy2 = R.td_target(rew, done, g32, nx2, S2)
     ydev = dbg_(L, 'y')
     pick2 = tie & (_choose([y1, y2], ydev) == 1)
     y, Sy = torch.where(pick2, y2, y1), torch.where(pick2, Sy2, Sy1)
-    Ck.ties('a_star_ties', tie, B)
+    _ties(Ck, 'a_star_ties', tie, B)
     mist = {}
     if double:
         nxm, Sm, *_ = R.scalar_targets(kind, hn, hnt, on, tg, double, 'double_target_astar')
         mist['double_target_astar'] = R.td_target(rew, done, g32, nxm, Sm)[0]
-    Ck.bound('y', ydev, y, Sy, R.CHECK_C['y'], mist)
+    Ck.bound('y', ydev, y, Sy, R.CHECK_C['y'], mistakes=mist)
     fq = R.from_qy(dbg_(L, 'q'), ydev, w, B, eps)
     Ck.bound('priority', L.debug_buffer('priorities'), fq['prio'][0], fq['prio'][1], R.CHECK_C['priority'])
     dc, Sdc = R.scalar_dcore(kind, fq['dq'], act, on)
     mist = {m: R.scalar_dcore(kind, fq['dq'], act, on, m)[0] for m in ('dueling_mean_A_minus_1', 'dueling_dcore_no_mean')
             if kind == 'dueling' and A > 1}
-    Ck.bound('dcore_scalar', dcore[:, :512], dc, Sdc, R.CHECK_C['dcore_scalar'], mist)
+    Ck.bound('dcore_scalar', dcore[:, :512], dc, Sdc, R.CHECK_C['dcore_scalar'], mistakes=mist)
     lo, Sl = R.loss_ref(fq['l'], B)
     Ck.bound('loss', L.debug_buffer('loss')[:1], lo.view(1), Sl.view(1), R.CHECK_C['loss'],
-             {'loss_last_block': R.loss_ref(fq['l'], B, 'loss_last_block')[0].view(1)})
+             mistakes={'loss_last_block': R.loss_ref(fq['l'], B, 'loss_last_block')[0].view(1)})
     if head.noisy:
         return a1
     g, Sg = R.scalar_wgrad(kind, fq['dq'], act, h, A, B)
@@ -342,7 +285,7 @@ def _scalar(Ck, head, L, pre, pre_t, h, hn, hnt, act, rew, done, w, g32, double,
                          torch.cat([L.grads['advantage.weight'], L.grads['advantage.bias'][:, None]], 1)])
     else:
         dev = torch.cat([L.grads['q.weight'], L.grads['q.bias'][:, None]], 1)
-    Ck.bound('head_grad', dev, g, Sg, R.CHECK_C['head_grad'], mist)
+    Ck.bound('head_grad', dev, g, Sg, R.CHECK_C['head_grad'], mistakes=mist)
     return a1
 
 
@@ -377,13 +320,14 @@ def _distributional(Ck, head, dd, L, pre, pre_t, h, hn, hnt, act, rew, done, w, 
     for n, hh, W_, b_ in gemm:
         x, S = R.gemm_rows(hh, W_, b_)
         dev[n] = L.debug_buffer(n).view(B, R_)
-        Ck.bound(n, dev[n], x, S, R.CHECK_C['theta' if qr else 'logits'], {'gemm_row0_unstored': R.gemm_rows(hh, W_, b_, 'gemm_row0_unstored')[0]})
+        Ck.bound(n, dev[n], x, S, R.CHECK_C['theta' if qr else 'logits'],
+                 mistakes={'gemm_row0_unstored': R.gemm_rows(hh, W_, b_, 'gemm_row0_unstored')[0]})
     xs_all = dev[names[0]].to(F64).view(B, A, Kw)
     xt = dev[names[2]].to(F64).view(B, A, Kw)
     xsel = dev[names[1]].to(F64).view(B, A, Kw) if double else xt
     Qsel, Ssel = R.qr_q(xsel) if qr else R.cat_q(xsel, AC.O.support(Kw, head.v_min, head.v_max)[0])
     a1, a2, tie = R.pick(Qsel, Ssel)
-    Ck.ties('a_star_ties', tie, B)
+    _ties(Ck, 'a_star_ties', tie, B)
     g = g32 * (1 - done.to(F64))
     xs = xs_all[rows, act]
     wv = torch.ones(B, dtype=F64, device='cuda') if w is None else w.to(F64)
@@ -396,10 +340,10 @@ def _distributional(Ck, head, dd, L, pre, pre_t, h, hn, hnt, act, rew, done, w, 
         if double:
             am = R.pick(*R.qr_q(xt))[0]
             mist['double_target_astar'] = R.qr_targets(xt, am, rew, g)[0]
-        Ck.bound('target_quantiles', Tdev, torch.where(c2, T2, T1), torch.where(c2, ST2, ST1), R.CHECK_C['target_quantiles'], mist)
+        Ck.bound('target_quantiles', Tdev, torch.where(c2, T2, T1), torch.where(c2, ST2, ST1), R.CHECK_C['target_quantiles'], mistakes=mist)
         ln, Sln, d, Sd = R.qr_loss(xs, Tdev, head.kappa, wv, B)
         lt, _, dt, _ = R.qr_loss(xs, Tdev, head.kappa, wv, B, 'tau_i_over_N')
-        Ck.bound('qr_loss', L.debug_buffer('qr_loss'), ln, Sln, R.CHECK_C['qr_loss'], {'tau_i_over_N': lt})
+        Ck.bound('qr_loss', L.debug_buffer('qr_loss'), ln, Sln, R.CHECK_C['qr_loss'], mistakes={'tau_i_over_N': lt})
         Ck.bound('priority', L.debug_buffer('priorities'), ln + eps, Sln, R.CHECK_C['qr_loss'])
         q, Sq = R.qr_q(xs)
         Ck.bound('q', L.debug_buffer('q'), q, Sq, R.CHECK_C['q'])
@@ -422,7 +366,7 @@ def _distributional(Ck, head, dd, L, pre, pre_t, h, hn, hnt, act, rew, done, w, 
             am = R.pick(*R.cat_q(xt, z32))[0]
             pm, _, Spm, _ = R.softmax_rows(xt[rows, am])
             mist['double_target_astar'] = R.project(pm, Spm, rew, g, z32, float(dz32), lo, hi)[0]
-        Ck.bound('m', mdev, m_ref, Sm, R.CHECK_C['m'], mist)
+        Ck.bound('m', mdev, m_ref, Sm, R.CHECK_C['m'], mistakes=mist)
         t = R.cat_tail(xs, mdev, z32, wv, B)
         Ck.bound('ce', L.debug_buffer('ce'), *t['ce'], R.CHECK_C['ce'])
         Ck.bound('priority', L.debug_buffer('priorities'), t['kl'][0].clamp(min=0) + eps, t['kl'][1], R.CHECK_C['kl'])
@@ -439,7 +383,7 @@ def _distributional(Ck, head, dd, L, pre, pre_t, h, hn, hnt, act, rew, done, w, 
     Ck.bound('dcore', dcore[:, :512], dc, Sdc, R.CHECK_C['dcore'])
     lo_, Sl = R.loss_ref(lterm, B)
     Ck.bound('loss', L.debug_buffer('loss')[:1], lo_.view(1), Sl.view(1), R.CHECK_C['loss'],
-             {'loss_last_block': R.loss_ref(lterm, B, 'loss_last_block')[0].view(1)})
+             mistakes={'loss_last_block': R.loss_ref(lterm, B, 'loss_last_block')[0].view(1)})
     if head.noisy:
         return a1
     dlf = dl_dev.view(B, R_)
@@ -449,7 +393,7 @@ def _distributional(Ck, head, dd, L, pre, pre_t, h, hn, hnt, act, rew, done, w, 
         gdev = torch.cat([L.debug_buffer('rows_weight_grad').view(R_, 512), L.debug_buffer('rows_bias_grad')[:, None]], 1)
     else:
         gdev = torch.cat([L.grads['q.weight'], L.grads['q.bias'][:, None]], 1)
-    Ck.bound('head_grad', gdev, gW, SgW, R.CHECK_C['head_grad'], mist)
+    Ck.bound('head_grad', gdev, gW, SgW, R.CHECK_C['head_grad'], mistakes=mist)
     Ck.res['head_grad']['rel_l2'] = AC.rel_l2(gdev, gW)
     if dd:
         gv, Sv, ga, Sa = R.dd_grad(gdev[:, :512], gdev[:, 512], A, Kw)
@@ -457,7 +401,7 @@ def _distributional(Ck, head, dd, L, pre, pre_t, h, hn, hnt, act, rew, done, w, 
               if A > 1 or m == 'dd_grad_mean_axis'}
         Ck.bound('dd_grad_value', torch.cat([L.grads['value.weight'], L.grads['value.bias'][:, None]], 1), gv, Sv, R.CHECK_C['rows_sum'])
         Ck.bound('dd_grad_advantage', torch.cat([L.grads['advantage.weight'], L.grads['advantage.bias'][:, None]], 1), ga, Sa,
-                 R.CHECK_C['rows'], mv)
+                 R.CHECK_C['rows'], mistakes=mv)
     return a1
 
 
@@ -522,7 +466,7 @@ def test_actor_q_values_exact(hname, A):
     NaN first, against fp64 on the actor's own core rows (the scalar heads) or logits / quantiles"""
     n = 37
     head, dd, X, sd = _actor(hname, n, A)
-    Ck = Checker()
+    Ck = exact.Checker(RESULTS, R)
     try:
         obs = AC.frames(n, A, 'cuda')
         q = torch.full((n, A), math.nan, device='cuda')
@@ -535,10 +479,10 @@ def test_actor_q_values_exact(hname, A):
         else:
             x = _actor_rows(Ck, head, X, net, core, n)
             Q, S = R.qr_q(x) if head.kind == 'quantile' else R.cat_q(x, AC.O.support(head.width, head.v_min, head.v_max)[0])
-        Ck.bound('q_values', q, Q, S, R.CHECK_C['q'], {'q_values_last_lane': R.q_values_mistake(Q, 'q_values_last_lane')})
+        Ck.bound('q_values', q, Q, S, R.CHECK_C['q'], mistakes={'q_values_last_lane': R.q_values_mistake(Q, 'q_values_last_lane')})
     finally:
         X.close()
-    Ck.done(f'q_values_{hname}_A{A}', ('q_values_last_lane',))
+    _done(Ck, f'q_values_{hname}_A{A}', ('q_values_last_lane',))
 
 
 @pytest.mark.parametrize('hname', ACTOR_HEADS)
@@ -549,7 +493,7 @@ def test_actor_priorities_exact(hname, E):
     A, n, gamma, eps = 5, 3, 0.99, 1e-6
     head, dd, X, sd = _actor(hname, E, A, priority_eps=eps)
     eps = float(np.float32(eps))            # the kernels add the fp32 eps in double
-    Ck = Checker()
+    Ck = exact.Checker(RESULTS, R)
     try:
         M = E + E // 2 + 1
         mem = GpuPrioritizedReplayBuffer(M, E, alpha=1.0, n_step=n, gamma=gamma)
@@ -609,8 +553,8 @@ def test_actor_priorities_exact(hname, E):
                     Ss.append(t['kl'][1] + 2 * (Sm * ((lm - lp).abs() + 1)).sum(1))
             c2 = tie & (_choose(cand, leaves.to(F64)) == 1)
             ref, S = torch.where(c2, cand[1], cand[0]), torch.where(c2, Ss[1], Ss[0])
-        Ck.ties('a_star_ties', tie, E)
+        _ties(Ck, 'a_star_ties', tie, E)
         Ck.bound('actor_priority', leaves, ref, S, R.CHECK_C['priority'])
     finally:
         X.close()
-    Ck.done(f'actor_{hname}_E{E}')
+    _done(Ck, f'actor_{hname}_E{E}')

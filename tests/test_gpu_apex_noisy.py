@@ -21,7 +21,8 @@ from oracle import apex_oracle as O
 from scalerl_b200.algorithms.apex import ApexHParams, B200ApexActor, B200ApexLearner
 from scalerl_b200.data.replay_memory import GpuPrioritizedReplayBuffer
 from tests import apex_cases as cases
-from tests.apex_cases import HEADS as ROWS, batch, device_composed, frames, learner, nets, record
+from tests.apex_cases import HEADS as ROWS, batch, device_composed, frames, learner, nets
+from tests.exact import record
 
 pytestmark = pytest.mark.gpu
 HEADS = {h: ROWS[f'noisy_{h}'] for h in ('plain', 'dueling', 'categorical')}

@@ -24,7 +24,6 @@ weight gradients and their S are summed over the blocks in fp64.  Every frame is
 back to the host.  The per-tensor rms that compare_stored's tie rule uses is that of the whole tensor (a first pass over the blocks).
 Measured errors, err / bound, partitions, peak device memory and wall time go to $SRL_RESULTS_DIR/encoder_exact.json."""
 import ctypes as C
-import json
 import os
 import time
 
@@ -34,13 +33,13 @@ import torch
 from oracle.impala_oracle import init_params
 from scalerl_b200 import _lib
 from tests import layer_ref as R
-from tests.test_gpu_layer_exact import NTOL, RTOL, SENS, Checker, _mid_chunk_frames, _sm_count
+from tests.exact import NTOL, RTOL, SENS, U, Checker, record
 
 pytestmark = pytest.mark.gpu
 F64 = torch.float64
 FRAME_BLOCK = 1024
 LARGE = 1024                 # from here on the sensitivity share is 1/16 of the wgrad CTAs (fc: of the frames)
-U = 2.0 ** -24
+RESULTS = 'encoder_exact.json'
 ENC_NAMES = ('conv1.weight', 'conv1.bias', 'conv2.weight', 'conv2.bias', 'conv3.weight', 'conv3.bias', 'fc.weight', 'fc.bias')
 
 # each frame count sits on an edge of the kernels (A = 6)
@@ -66,17 +65,6 @@ COUNTS = {
 }
 A_SWEEP_FRAMES = 129
 ACTIONS = (1, 6, 18, 31)     # A changes only the core width 513 + A
-
-
-def _record(name, obj):
-    d = os.environ.get('SRL_RESULTS_DIR')
-    if not d:
-        return
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, 'encoder_exact.json')
-    cur = json.load(open(p)) if os.path.exists(p) else {}
-    cur[name] = obj
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
 
 
 def _hooks():
@@ -219,10 +207,10 @@ def run_case(F, A, split, seed=0):
 
 
 def check(F, A, split, obs, reward, action, dcore, core_out, grads, params, rows):
-    ck = Checker()
+    ck = Checker(RESULTS)
     W = {k: tuple(None if t is None else t.cuda() for t in v) for k, v in R.weights(params, split).items()}
     bias = {k: params[k].cuda() for k in ('conv1.bias', 'conv2.bias', 'conv3.bias', 'fc.bias')}
-    ctas = R.cta_counts(_sm_count(), os.environ)
+    ctas = R.cta_counts(R.sm_count(), os.environ)
     parts = R.wgrad_partitions(F, ctas, split)
     get = lambda n: rows[n][0]
     lo = lambda n: rows[n][1] if split else None
@@ -413,10 +401,10 @@ def _run_and_check(F, A, split):
     need = _need_bytes(F, split, A)
     free, total = torch.cuda.mem_get_info()
     if need > free:
-        _record(f'F{F}_A{A}_{"split" if split else "bf16"}', {'skipped': True, 'need_bytes': need, 'free_bytes': free})
+        record(RESULTS, f'F{F}_A{A}_{"split" if split else "bf16"}', {'skipped': True, 'need_bytes': need, 'free_bytes': free})
         pytest.skip(f'needs about {need / 2**30:.1f} GiB of device memory, {free / 2**30:.1f} GiB free')
     ck, rec = run_case(F, A, split)
-    _record(f'F{F}_A{A}_{"split" if split else "bf16"}', rec)
+    record(RESULTS, f'F{F}_A{A}_{"split" if split else "bf16"}', rec)
     print(f'F={F} A={A} split={split}: peak {rec["peak_device_bytes"] / 2**30:.2f} GiB, {rec["wall_s"]:.1f} s, '
           + ', '.join(f'{k} {v["err_over_bound"]:.3g}' for k, v in rec['grads'].items()))
     assert not ck.fails, '\n'.join(ck.fails)
@@ -437,19 +425,19 @@ def test_encoder_exact_core_width(A, precision):
 
 def test_frame_counts_reach_every_partition_regime():
     """the frame-count table drives srl_encoder_backward's three wgrad launches through all four partition regimes"""
-    ctas = R.cta_counts(_sm_count(), os.environ)
+    ctas = R.cta_counts(R.sm_count(), os.environ)
     seen, table = set(), []
     for F in COUNTS:
         for split in (False, True):
             for name, p in R.wgrad_partitions(F, ctas, split).items():
                 table.append({'frames': F, 'split': split, 'layer': name, **p})
                 seen.update(k for k, v in R.regimes(p).items() if v)
-    _record('partition_regimes', {'ctas': ctas, 'table': table, 'reached': sorted(seen)})
+    record(RESULTS, 'partition_regimes', {'ctas': ctas, 'table': table, 'reached': sorted(seen)})
     # below LARGE the sensitivity share is test_gpu_layer_exact's: the first chunk of the middle CTA
     for F in (f for f in COUNTS if f < LARGE):
         for name, G in (('conv3', 9), ('conv2', 10), ('conv1', 21)):
             p = R.wgrad_partitions(F, ctas, False)[name]
-            n0, n1, m = _mid_chunk_frames(F, G, p)
+            n0, n1, m = R.mid_chunk_frames(F, G, p)
             q0, q1 = _share_range(F, p, G)
             assert torch.equal(_share_mask(n0, n1, G, q0, q1).cpu(), m), (F, name)
     assert seen == {'one_chunk_per_cta', 'within_ring', 'ring_wraps_twice', 'last_cta_single_chunk'}, sorted(seen)

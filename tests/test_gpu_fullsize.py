@@ -7,7 +7,6 @@ OPERANDS, not of the kernels: the oracle's own bf16 emulation is as far from its
 "shrinks with the batch" claim was measured here and is false: 0.076 / 0.044 / 0.094 at B = 2 / 8 / 32).  Parity against the
 fp32 reference proper is the job of the fp32-accurate operand mode (tests/test_gpu_precision.py, <= 2e-3).
 The measured errors are written to $SRL_RESULTS_DIR/parity_fullsize.json when SRL_RESULTS_DIR is set."""
-import json
 import os
 
 import numpy as np
@@ -15,21 +14,12 @@ import pytest
 import torch
 
 from oracle import impala_oracle as O
+from tests.exact import record
 from tests.helpers import assert_close, rel_l2
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _record(name, obj):
-    d = os.environ.get('SRL_RESULTS_DIR')
-    if not d:
-        return
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, 'parity_fullsize.json')
-    cur = json.load(open(p)) if os.path.exists(p) else {}
-    cur[name] = obj
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
+RESULTS = 'parity_fullsize.json'
 
 
 def _learner(T, B, A, seed, **kw):
@@ -64,7 +54,7 @@ def test_learn_step_at_baseline_sizes(T, B, A):
            'vs_vs_bf16': rel_l2(L._vs.cpu(), ref_bf['vs']), 'vs_vs_fp32': rel_l2(L._vs.cpu(), ref_32['vs']),
            'total_loss': [stats['total_loss'], ref_bf['total_loss'], ref_32['total_loss']],
            'grad_norm': [stats['grad_norm'], ref_bf['grad_norm'], ref_32['grad_norm']]}
-    _record(f'learn_T{T}_B{B}_A{A}', rec)
+    record(RESULTS, f'learn_T{T}_B{B}_A{A}', rec)
     assert rec['logits_vs_bf16'] < TOL_OUT_BF16 and rec['logits_vs_fp32'] < TOL_OUT_FP32, rec
     assert rec['vs_vs_bf16'] < TOL_OUT_BF16 and rec['vs_vs_fp32'] < TOL_OUT_FP32, rec
     for k in ('pg_loss', 'baseline_loss', 'entropy_loss', 'total_loss'):
@@ -101,7 +91,7 @@ def test_bf16_gap_is_operand_rounding_only():
         for k in O.PARAM_ORDER:
             assert kern[k] <= 1.3 * emul[k] + 2e-3, (B, k, kern[k], emul[k])
         L.close()
-    _record('bf16_gap_kernel_vs_emulation_T20', rec)
+    record(RESULTS, 'bf16_gap_kernel_vs_emulation_T20', rec)
 
 
 def test_lstm_learn_step_T100():
@@ -118,7 +108,7 @@ def test_lstm_learn_step_T100():
     allg = {**ref['grads'], **ref['lstm_grads']}
     errs = {k: rel_l2(L.grads[k].cpu(), v) for k, v in allg.items()}
     rec = {'grad_vs_fp32_oracle': errs, 'vs': rel_l2(L._vs.cpu(), ref['vs']), 'total_loss': [stats['total_loss'], ref['total_loss']]}
-    _record(f'lstm_learn_T{T}_B{B}', rec)
+    record(RESULTS, f'lstm_learn_T{T}_B{B}', rec)
     assert abs(stats['total_loss'] - ref['total_loss']) <= 1e-2 * max(1.0, abs(ref['total_loss'])), rec['total_loss']
     assert rec['vs'] < 1e-2
     for k, e in errs.items():       # encoder tensors: bf16 operand bound (no LSTM emulation oracle); LSTM / head tensors far tighter

@@ -25,13 +25,13 @@ import sys
 import pytest
 import torch
 
+from tests import exact as E
 from tests import layer_ref as R
 from tests.layer_exact_worker import digest, run_step
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-RTOL, NTOL, SENS = 2e-5, 1e-4, 20
+RESULTS = 'layer_exact.json'
 
 # each shape sits on an edge of the kernels
 SHAPES = {
@@ -53,66 +53,11 @@ MODES = {
 }
 
 
-def _record(name, obj):
-    d = os.environ.get('SRL_RESULTS_DIR')
-    if not d:
-        return
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, 'layer_exact.json')
-    cur = json.load(open(p)) if os.path.exists(p) else {}
-    cur[name] = obj
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
-
-
-def _sm_count():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
-class Checker:
-    def __init__(self):
-        self.res, self.fails = {}, []
-
-    def fp32(self, name, got, ref, sens=None):
-        e = {'rel_l2': R.rel_l2(got.reshape(ref.shape), ref), 'nerr': R.nerr(got.reshape(ref.shape), ref)}
-        if sens is not None:
-            e['sensitivity'] = sens
-            if sens < SENS * RTOL:
-                self.fails.append(f'{name}: one left-out chunk moves the reference by {sens:.2e} < {SENS} x {RTOL:.0e}')
-        self.res[name] = e
-        if not (e['rel_l2'] <= RTOL and e['nerr'] <= NTOL):
-            self.fails.append(f'{name}: {e}')
-
-    def stored(self, name, hi, lo, ref, pre=None, split=False, terms=None):
-        st = R.compare_stored(hi, lo, ref, pre, terms)
-        self.res[name] = st
-        if not R.stored_ok(st, split):
-            self.fails.append(f'{name}: {st}')
-
-    def zero_pad(self, name, pad):
-        n = int((pad.contiguous().view(torch.int16) != 0).sum())
-        self.res[name + '_padding_nonzero'] = n
-        if n:
-            self.fails.append(f'{name}: {n} padding elements are not +0.0')
-
-
-def _sens(part, ref):
-    return float(part.norm() / max(float(ref.norm()), 1e-300))
-
-
-def _mid_chunk_frames(NB, G, part):
-    """frames and position mask [n1-n0, 1, G, G] of the first chunk of the middle CTA of a wgrad launch"""
-    q0 = (part['grid'] // 2) * part['chunks_per_cta'] * 128
-    n0, n1 = q0 // (G * G), min(NB, (q0 + 127) // (G * G) + 1)
-    m = torch.zeros((n1 - n0) * G * G, dtype=R.F64)
-    m[q0 - n0 * G * G:q0 - n0 * G * G + 128] = 1
-    return n0, n1, m.view(n1 - n0, 1, G, G)
-
-
 def check_layers(T, B, A, bufs, grads, params, batch, split, ctas):
     """all per-layer comparisons of one step; returns (Checker, fp64 reference gradients)"""
     NF, NB = (T + 1) * B, T * B
     W = R.weights(params, split)
-    C = Checker()
+    C = E.Checker(RESULTS)
     lo = lambda n: bufs[n + '_lo'] if split else None
     sl = lambda p, a, b: (p[0][a:b], None if p[1] is None else p[1][a:b])
     frames = batch['obs'].reshape(NF, 4, 84, 84)
@@ -135,7 +80,7 @@ def check_layers(T, B, A, bufs, grads, params, batch, split, ctas):
     zh = R.fc_fwd(a3p, W['fc.weight'], params['fc.bias'])
     idx = torch.arange(64) * 49 + 24                                    # one 64-channel k-block (pixel hw = 24)
     kblk = R.sp(lambda a, w: a.reshape(NF, -1)[:, idx] @ w[:, idx].t(), a3p, W['fc.weight'])
-    C.fp32('h', bufs['h'], zh.clamp_min(0), _sens((zh - kblk).clamp_min(0) - zh.clamp_min(0), zh.clamp_min(0)))
+    C.fp32('h', bufs['h'], zh.clamp_min(0), E.left_out((zh - kblk).clamp_min(0) - zh.clamp_min(0), zh.clamp_min(0)))
     h = bufs['h'].reshape(NF, 512).to(R.F64)
     lg, bs = R.heads_fwd(R.core(h, reward, action, A), params)
     C.fp32('logits', bufs['logits'], lg)
@@ -150,7 +95,7 @@ def check_layers(T, B, A, bufs, grads, params, batch, split, ctas):
     s0 = ((nslab + spg - 1) // spg // 2) * spg                           # first slab of the middle slab group
     part = R.head_grads(dl[16 * s0:16 * s0 + 16], dv[16 * s0:16 * s0 + 16], c_nb[16 * s0:16 * s0 + 16])
     for k in ref:
-        C.fp32(k, grads[k], ref[k], _sens(part[k], ref[k]))
+        C.fp32(k, grads[k], ref[k], E.left_out(part[k], ref[k]))
     # ---- fc
     dhp = R.pair(bufs['dh'].reshape(NB, 512), None if not split else lo('dh').reshape(NB, 512))
     mask3 = (a3[0][:NB] > 0).to(R.F64)
@@ -159,8 +104,8 @@ def check_layers(T, B, A, bufs, grads, params, batch, split, ctas):
     kb = ((NB + 63) // 64 // 2) * 64                                     # middle 64-frame k-block
     ke = min(NB, kb + 64)
     pWf, pbf, _ = R.fc_bwd(sl(dhp, kb, ke), sl(a3p, kb, ke), W['fc.weight'], mask3[kb:ke])
-    C.fp32('fc.weight', grads['fc.weight'], dWf, _sens(pWf, dWf))
-    C.fp32('fc.bias', grads['fc.bias'], dbf, _sens(pbf, dbf))
+    C.fp32('fc.weight', grads['fc.weight'], dWf, E.left_out(pWf, dWf))
+    C.fp32('fc.bias', grads['fc.bias'], dbf, E.left_out(pbf, dbf))
     ref.update({'fc.weight': dWf, 'fc.bias': dbf})
     # ---- conv3 / conv2 / conv1: dgrad on the grid, wgrad + bias from the GPU's own dY
     layers = (('conv3', 'da3', 9, 7, 64, a2p, a2, 1, 1.0), ('conv2', 'da2', 10, 9, 64, a1p, a1, 2, 1.0),
@@ -169,20 +114,20 @@ def check_layers(T, B, A, bufs, grads, params, batch, split, ctas):
     parts = R.wgrad_partitions(NB, ctas, split)
     for name, dname, G, V, Cch, xp, xs, stride, scale in layers:
         dy_hi, pad = R.grid_to_nchw(bufs[dname], NB, G, V, Cch)
-        C.zero_pad(dname, pad)
+        C.zero(f'{dname}_padding', pad)
         dy_lo = None
         if split:
             dy_lo, pad_lo = R.grid_to_nchw(lo(dname), NB, G, V, Cch)
-            C.zero_pad(dname + '_lo', pad_lo)
+            C.zero(f'{dname}_lo_padding', pad_lo)
         C.stored(dname, dy_hi, dy_lo, dref, split=split, terms=dterms)
         dyp = R.pair(dy_hi, dy_lo)
         mask = None if xs is None else (xs[0][:NB] > 0).to(R.F64)
         dW, db, dx = R.conv_bwd(sl(xp, 0, NB), dyp, W[f'{name}.weight'], stride, mask, scale)
-        n0, n1, m = _mid_chunk_frames(NB, G, parts[name])
+        n0, n1, m = R.mid_chunk_frames(NB, G, parts[name])
         m = m[:, :, :V, :V]
         pW, pb, _ = R.conv_bwd(sl(xp, n0, n1), (dyp[0][n0:n1] * m, None if dy_lo is None else dyp[1][n0:n1] * m), W[f'{name}.weight'], stride, None, scale)
-        C.fp32(f'{name}.weight', grads[f'{name}.weight'], dW, _sens(pW, dW))
-        C.fp32(f'{name}.bias', grads[f'{name}.bias'], db, _sens(pb, db))
+        C.fp32(f'{name}.weight', grads[f'{name}.weight'], dW, E.left_out(pW, dW))
+        C.fp32(f'{name}.bias', grads[f'{name}.bias'], db, E.left_out(pb, db))
         ref.update({f'{name}.weight': dW, f'{name}.bias': db})
         dref = dx
         if mask is not None:
@@ -197,18 +142,16 @@ def test_layers_exact(T, B, A, mode, monkeypatch):
     precision, column, fused, replay, poison = MODES[mode]
     monkeypatch.setenv('SRL_NO_COLUMN_FUSION', '0' if column else '1')      # read when the learner is created
     bufs, grads, batch, params = run_step(T, B, A, precision, fused=fused, replay=replay, poison=poison)
-    C, _ = check_layers(T, B, A, bufs, grads, params, batch, precision == 'fp32_split', R.cta_counts(_sm_count(), os.environ))
-    _record(f'T{T}_B{B}_A{A}_{mode}', C.res)
-    assert not C.fails, '\n'.join(C.fails)
+    C, _ = check_layers(T, B, A, bufs, grads, params, batch, precision == 'fp32_split', R.cta_counts(R.sm_count(), os.environ))
+    C.done(f'T{T}_B{B}_A{A}_{mode}')
 
 
 def test_layers_exact_after_poisoned_shared_memory():
     """every SM's shared memory filled with NaN patterns before each of three replayed steps (ragged shape): same checks"""
     T, B, A = 7, 19, 18
     bufs, grads, batch, params = run_step(T, B, A, 'bf16', replay=True, poison=True)
-    C, _ = check_layers(T, B, A, bufs, grads, params, batch, False, R.cta_counts(_sm_count(), os.environ))
-    _record(f'T{T}_B{B}_A{A}_bf16_poisoned', C.res)
-    assert not C.fails, '\n'.join(C.fails)
+    C, _ = check_layers(T, B, A, bufs, grads, params, batch, False, R.cta_counts(R.sm_count(), os.environ))
+    C.done(f'T{T}_B{B}_A{A}_bf16_poisoned')
 
 
 # ------------------------------------------------------------------------------------------------ partition sweep
@@ -234,7 +177,7 @@ def test_partition_sweep(tmp_path):
     the weight gradients may change -- activations and dY bit-identical, gradients within the fp32 bounds of the fp64 reference;
     with SRL_PDL=0 (no programmatic dependent launch) everything bit-identical to the same partition with it"""
     T, B, A = 20, 32, 6
-    NB, sm = T * B, _sm_count()
+    NB, sm = T * B, R.sm_count()
     base = {}
     for precision in ('bf16', 'fp32_split'):
         bufs, grads, batch, params = run_step(T, B, A, precision)
@@ -267,7 +210,7 @@ def test_partition_sweep(tmp_path):
                 # the tensor cores' fp32 accumulation error grows linearly with the chunks one CTA sums into its registers
                 # (measured, fp32-split conv2: rel-L2 3.6e-6 at 8 chunks per CTA, 2.2e-5 at 63): the bounds scale beyond 16
                 grow = max(1.0, parts[k.split('.')[0]]['chunks_per_cta'] / 16) if k.split('.')[0] in parts else 1.0
-                assert e <= RTOL * grow and n <= NTOL * grow, (env_over, precision, k, e, n, grow)
+                assert e <= E.RTOL * grow and n <= E.NTOL * grow, (env_over, precision, k, e, n, grow)
             for name, p in parts.items():
                 table.append({'T': T, 'B': B, 'env': key, 'split': precision == 'fp32_split', 'layer': name, **p})
     # PDL off == PDL on, bit for bit, in the same partition
@@ -285,5 +228,5 @@ def test_partition_sweep(tmp_path):
                 assert torch.equal(a['grads'][k], b['grads'][k]), (pdl_off, precision, k, 'SRL_PDL=0 changed the bits')
     for row in table:
         seen.update(k for k, v in R.regimes(row).items() if v)
-    _record('partition_sweep_T20_B32', {'runs': rec, 'partition_table': table, 'regimes_reached': sorted(seen)})
+    E.record(RESULTS, 'partition_sweep_T20_B32', {'runs': rec, 'partition_table': table, 'regimes_reached': sorted(seen)})
     assert seen == {'one_chunk_per_cta', 'within_ring', 'ring_wraps_twice', 'last_cta_single_chunk'}, sorted(seen)

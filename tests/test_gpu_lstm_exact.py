@@ -19,8 +19,6 @@ Measured on an H100 80GB HBM3 at 700 W: the fp32 results within 2.3e-6 rel-L2 (d
 least 8.8x under the bound; the smallest sensitivity 1.8e-2 (gates), 45x the 20x requirement; dgates at most 1 ulp, 0.060 % of elements.
 Measured errors, sensitivities and the margin under every bound go to $SRL_RESULTS_DIR/lstm_exact.json when SRL_RESULTS_DIR is set."""
 import ctypes as C
-import json
-import os
 
 import pytest
 import torch
@@ -29,12 +27,11 @@ from oracle import impala_oracle as O
 from scalerl_b200 import _lib
 from scalerl_b200.algorithms.utils.atari_model import lstm_block_sizes
 from scalerl_b200.lstm import LSTM_PARAM_NAMES, B200LstmCore
-from tests import layer_ref as LR
+from tests import exact as E
 from tests import lstm_ref as R
 
 pytestmark = pytest.mark.gpu
 
-RTOL, NTOL, SENS, MISMATCH = 2e-5, 1e-4, 20, 5e-3
 F64, BF16 = torch.float64, torch.bfloat16
 RESULTS = 'lstm_exact.json'
 
@@ -58,94 +55,7 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-# ------------------------------------------------------------------------------------------------ results
-def _record(name, obj):
-    d = os.environ.get('SRL_RESULTS_DIR')
-    if not d:
-        return
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, RESULTS)
-    cur = json.load(open(p)) if os.path.exists(p) else {}
-    cur[name] = obj
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _summary():
-    """after the module: per check kind, the worst measured value over every case and its margin under the bound"""
-    yield
-    d = os.environ.get('SRL_RESULTS_DIR')
-    p = os.path.join(d, RESULTS) if d else None
-    if not p or not os.path.exists(p):
-        return
-    cur = json.load(open(p))
-    table = {}
-    for case, res in cur.items():
-        if case == 'summary':
-            continue
-        for name, e in res.items():
-            kind = name.rstrip('01')
-            t = table.setdefault(kind, {})
-            for k, v in e.items():
-                if not isinstance(v, (int, float)):
-                    continue
-                worst = min if k in ('sensitivity',) or k.endswith('margin') else max
-                t[k] = v if k not in t else worst(t[k], v)
-    cur['summary'] = table
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
-
-
-def _margin(bound, err):
-    return bound / err if err > 0 else float('inf')
-
-
-class Checker:
-    def __init__(self):
-        self.res, self.fails = {}, []
-
-    def fp32(self, name, got, ref, sens=None):
-        got = got.reshape(ref.shape)
-        e = {'rel_l2': LR.rel_l2(got, ref), 'nerr': LR.nerr(got, ref)}
-        e['rel_l2_margin'], e['nerr_margin'] = _margin(RTOL, e['rel_l2']), _margin(NTOL, e['nerr'])
-        if sens is not None:
-            e['sensitivity'] = sens
-            e['sensitivity_margin'] = sens / (SENS * RTOL)
-            if sens < SENS * RTOL:
-                self.fails.append(f'{name}: one left-out unit of work moves the reference by {sens:.2e} < {SENS} x {RTOL:.0e}')
-        self.res[name] = e
-        if not (e['rel_l2'] <= RTOL and e['nerr'] <= NTOL):
-            self.fails.append(f'{name}: {e}')
-
-    def stored(self, name, got, ref, terms):
-        st = LR.compare_stored(got, None, ref, terms=terms)
-        st['mismatch_margin'] = _margin(MISMATCH, st['mismatch_frac'])
-        self.res[name] = st
-        if not LR.stored_ok(st, False):
-            self.fails.append(f'{name}: {st}')
-
-    def exact(self, name, got, want):
-        got, want = got.contiguous(), want.contiguous()
-        if got.shape != want.shape or got.dtype != want.dtype:
-            self.fails.append(f'{name}: {tuple(got.shape)} {got.dtype} vs {tuple(want.shape)} {want.dtype}')
-            return
-        n = int((_bits(got) != _bits(want)).sum())
-        self.res[name] = {'bits_differ': n, 'n': got.numel()}
-        if n:
-            self.fails.append(f'{name}: {n} of {got.numel()} elements differ in their bits')
-
-    def zero(self, name, x):
-        n = int((_bits(x.contiguous()) != 0).sum())
-        self.res[name + '_not_pos_zero'] = {'count': n, 'n': x.numel()}
-        if n:
-            self.fails.append(f'{name}: {n} elements are not +0.0')
-
-
-def _bits(x):
-    return x.view({1: torch.uint8, 2: torch.int16, 4: torch.int32}[x.element_size()])
-
-
-def _sens(part, ref):
-    return float(part.norm() / max(float(ref.norm()), 1e-300))
+_summary = E.summary(RESULTS, kind=lambda name: name.rstrip('01'))      # per check kind: the two layers together
 
 
 # ------------------------------------------------------------------------------------------------ inputs and runs
@@ -294,7 +204,7 @@ def check_forward(Ck, T1, B, A, x, r):
         k0, k1 = R.mid_block(Hp)
         part = xin[:, k0:k1].to(F64) @ Wih[:, k0:k1].t()         # one 64-wide k-block of the input projection
         gates = fw['gates'][l].view(N1, G)
-        Ck.fp32(f'gates{l}', R.unpad_gates(gates, H), R.unpad_gates(ref, H), _sens(R.activate(pre - part, H) - ref, ref))
+        Ck.fp32(f'gates{l}', R.unpad_gates(gates, H), R.unpad_gates(ref, H), E.left_out(R.activate(pre - part, H) - ref, ref))
         Ck.zero(f'gates_padding{l}', R.gate_padding(gates, H))
         gates = gates.view(T1, B, G)
         cseq, hseq = fw['cseq'][l].view(T1, B, Hp), fw['hseq'][l].view(T1, B, Hp)
@@ -328,7 +238,7 @@ def check_backward(Ck, T1, B, A, x, r):
         Wih, Whh = fw['Wih'][l].view(G, Hp).to(F64), fw['Whh'][l].view(G, Hp).to(F64)
         seed = lambda v: None if v is None else R.pad_cols(v[l], Hp)
         ref = R.bptt_layer(gates, cseq, c_init, m, dh_out, Whh, steps, seed(x['dhT']), seed(x['dcT']), dgates_next=dg, dh_out_terms=dh_terms)
-        Ck.stored(f'dgates{l}', R.unpad_gates(dg, H), R.unpad_gates(ref['dgates'], H), R.unpad_gates(ref['terms'], H))
+        Ck.stored(f'dgates{l}', R.unpad_gates(dg, H), None, R.unpad_gates(ref['dgates'], H), terms=R.unpad_gates(ref['terms'], H))
         Ck.zero(f'dgates_padding{l}', R.gate_padding(dg, H))
         # weight and bias gradients over rows [0, NB) (the learner's bootstrap row T1-1 must not reach them)
         dgr = dg.reshape(NB, G)
@@ -338,9 +248,9 @@ def check_backward(Ck, T1, B, A, x, r):
         k0, k1 = R.mid_block(NB)
         pWih, pWhh, pdb = R.weight_grads(dgr, xin, hm, k0, k1)
         g = lambda n: r['grads'][f'rnn_layer.{n}_l{l}']
-        Ck.fp32(f'dWih{l}', g('weight_ih'), R.unpad_weight(dWih, H), _sens(pWih, dWih))
-        Ck.fp32(f'dWhh{l}', g('weight_hh'), R.unpad_weight(dWhh, H), _sens(pWhh, dWhh))
-        Ck.fp32(f'db{l}', g('bias_ih'), R.unpad_gates(db, H), _sens(pdb, db))
+        Ck.fp32(f'dWih{l}', g('weight_ih'), R.unpad_weight(dWih, H), E.left_out(pWih, dWih))
+        Ck.fp32(f'dWhh{l}', g('weight_hh'), R.unpad_weight(dWhh, H), E.left_out(pWhh, dWhh))
+        Ck.fp32(f'db{l}', g('bias_ih'), R.unpad_gates(db, H), E.left_out(pdb, db))
         Ck.exact(f'db_hh_equals_db_ih{l}', g('bias_hh'), g('bias_ih'))
         if r['dh0'] is not None:
             Ck.fp32(f'dh0_{l}', r['dh0'][l], ref['dh0'][:, :H])
@@ -353,15 +263,14 @@ def check_backward(Ck, T1, B, A, x, r):
         else:
             k0, k1 = R.mid_block(G)
             part = dgr[:, k0:k1].to(F64) @ Wih[k0:k1]                # one 64-wide k-block of K = 4Hp
-            Ck.fp32('dcore', r['dcore'][:steps], dx[..., :H], _sens(part, dx.reshape(NB, Hp)))
+            Ck.fp32('dcore', r['dcore'][:steps], dx[..., :H], E.left_out(part, dx.reshape(NB, Hp)))
 
 
 def _check(name, T1, B, A, x, r):
-    Ck = Checker()
+    Ck = E.Checker(RESULTS)
     check_forward(Ck, T1, B, A, x, r)
     check_backward(Ck, T1, B, A, x, r)
-    _record(name, Ck.res)
-    assert not Ck.fails, '\n'.join(Ck.fails)
+    Ck.done(name)
 
 
 # ------------------------------------------------------------------------------------------------ tests

@@ -23,7 +23,6 @@ process, later profiler sessions there returned no kernel records on the H100, a
 The worst err / bound of every check, its margin and its weakest sensitivity go to $SRL_RESULTS_DIR/optim_exact.json (per case, and a
 summary per check)."""
 import ctypes as C
-import json
 import math
 import os
 
@@ -32,6 +31,7 @@ import pytest
 import torch
 
 from scalerl_b200 import _lib
+from tests import exact as E
 from tests import optim_ref as R
 
 pytestmark = pytest.mark.gpu
@@ -49,77 +49,7 @@ def _variant_code(opt, mom, sched):
     return 4 * int(opt == 'adam') + 2 * int(sched == 'linear') + int(mom)
 
 
-# ------------------------------------------------------------------------------------------------ results
-def _record(name, obj):
-    d = os.environ.get('SRL_RESULTS_DIR')
-    if not d:
-        return
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, RESULTS)
-    cur = json.load(open(p)) if os.path.exists(p) else {}
-    cur[name] = obj
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _summary():
-    """after the module: per check, the worst err / bound over every case, its margin, and the weakest sensitivity (the smallest,
-    over the cases where some mistake moves the check, of the strongest mistake's)"""
-    yield
-    d = os.environ.get('SRL_RESULTS_DIR')
-    p = os.path.join(d, RESULTS) if d else None
-    if not p or not os.path.exists(p):
-        return
-    cur = json.load(open(p))
-    table = {}
-    for case, res in cur.items():
-        if case == 'summary':
-            continue
-        for name, e in res.items():
-            t = table.setdefault(name.split('@')[0], {})
-            for k, v in e.items():
-                if not isinstance(v, (int, float)) or (k == 'sensitivity' and not v > 0):     # max_norm 0: no mistake can move it
-                    continue
-                worst = min if k in ('margin', 'sensitivity') else max
-                t[k] = v if k not in t else worst(t[k], v)
-    cur['summary'] = table
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
-
-
-class Checker:
-    def __init__(self):
-        self.res, self.fails = {}, []
-
-    def bound(self, name, got, ref, S, c, sens=None):
-        q = R.ratio(got, ref, S, c)
-        e = {'err_over_bound': q, 'margin': 1.0 / q if q > 0 else float('inf')}
-        if sens:                            # the mistake this check shows best, and by how much
-            e['sensitivity'] = max(sens.values())
-            e['mistake'] = max(sens, key=sens.get)
-        self.res[name] = e
-        if not q <= 1.0:
-            self.fails.append(f'{name}: {q:.3f} x the bound')
-
-    def exact(self, name, got, want):
-        got, want = np.asarray(got, np.float32).reshape(-1), np.asarray(want, np.float32).reshape(-1)
-        n = int((got.view(np.int32) != want.view(np.int32)).sum()) if got.shape == want.shape else -1
-        self.res[name] = {'bits_differ': n, 'n': int(want.size)}
-        if n:
-            self.fails.append(f'{name}: {n} of {want.size} elements differ in their bits (got {got[:4]}, want {want[:4]})')
-
-    def equal(self, name, got, want):
-        self.res[name] = {'got': got, 'want': want}
-        if got != want:
-            self.fails.append(f'{name}: {got} != {want}')
-
-    def require(self, name, sens, mistakes):
-        for m in mistakes:
-            if not sens.get(m, 0.0) >= R.SENS:
-                self.fails.append(f'{name}: {m} ({R.MISTAKES[m]}) moves it by only {sens.get(m, 0.0):.1f} x the bound')
-
-    def done(self, case):
-        _record(case, self.res)
-        assert not self.fails, '\n'.join(self.fails[:20])
+_summary = E.summary(RESULTS, kind=lambda name: name.split('@')[0])        # per check, over its steps and calls
 
 
 def _dev(x):
@@ -274,7 +204,7 @@ def test_fused_step_exact(variant, label):
     k = GRID.index(label)
     mn1, mn3 = R.max_norm_of(MAX_NORMS[k % 5], g), R.max_norm_of(MAX_NORMS[(k + 2) % 5], g)
     b = Bufs(g, st, opt, mom)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     got_blocks = hook(opt, mom, sched, b, mn1)
     # step 1 from a fresh state: the mistakes every case that steps its small gradients must show (eps inside the root, the old v of a
     # fresh state); the cases of n < 64 hold marked elements only, and max_norm 0 steps nothing
@@ -300,7 +230,7 @@ def test_standalone_ops_exact(label):
     blocks = max(1, min(-(-(n // 4) // 256), 592))
     g = R.grads(rng, n, blocks)
     gd = _dev(g)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     scratch = torch.zeros(1028, device='cuda')
     coef = torch.empty(2, device='cuda')
     mn = R.max_norm_of('clip', g)
@@ -371,7 +301,7 @@ def test_non_finite_gradient(variant, bad, max_norm):
     b.dstep.fill_(2)
     blocks = hook(opt, mom, sched, b, max_norm)
     coef = _host(b.coef)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     c = R.clip_coef32(np.float32(coef[0]), max_norm)
     Ck.exact('coef', coef[1], c)
     if math.isnan(bad) and max_norm == 40.0:
@@ -465,7 +395,7 @@ def impala_case(name):
     hp = ImpalaHParams(rollout_length=T, batch_size=B, num_actions=A, use_lstm=c['use_lstm'], optimizer=opt, momentum=c['momentum'],
                        learning_rate=R.HP[opt]['lr'], **kw)
     L = B200ImpalaLearner(hp, process_group=False, seed=3)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     try:
         if c['start']:
             L._set_opt_step(c['start'])
@@ -523,7 +453,7 @@ def test_apex_learner_step_is_the_hook(head):
     B, A = 8, 4
     on, tg = AC.nets(h, A, seed=1)
     clip = 10.0 if len(head) % 2 else None
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     (obs, act, rew, nobs, done), w = AC.batch(B, A, seed=4)
     xs = tuple(t.cuda() for t in (obs, act, h.scale_reward(rew), nobs, done))
     L = AC.learner(h, B, A, on, tg, seed=1, max_grad_norm=clip)

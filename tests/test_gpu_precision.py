@@ -20,8 +20,8 @@ import torch
 from oracle import impala_oracle as O
 from tests import layer_ref as R
 from tests.conftest import GOLDEN
+from tests.exact import record
 from tests.helpers import assert_close, rel_l2, strided_sample
-from tests.test_gpu_fullsize import _record
 
 pytestmark = pytest.mark.gpu
 
@@ -77,7 +77,7 @@ def test_split_mode_vs_reference_goldens(name, fusion, monkeypatch):
         errs['grad_' + k] = rel_l2(strided_sample(L.grads[k].reshape(-1).cpu()), g['s0_gradsamp_' + k])
     flips, units, worst = _mask_flips(L, params, batch, T, B)
     errs.update(relu_mask_flips=flips, relu_units=units, worst_flipped_margin=worst)
-    _record(f'split_golden_{name}_{fusion}', errs)
+    record('parity_fullsize.json', f'split_golden_{name}_{fusion}', errs)
     assert errs['logits'] < 1e-5 and errs['baseline'] < 1e-5 and errs['vs'] < 1e-5, errs
     assert abs(stats['total_loss'] - g['s0_losses'][3]) <= 1e-5 * max(1.0, abs(g['s0_losses'][3]))
     assert flips <= 2 + units * 2e-5 and worst < 1e-4, (flips, units, worst)       # only genuine ties may flip
@@ -102,7 +102,7 @@ def test_split_mode_vs_fp32_oracle(T, B, A):
     errs['vs'] = rel_l2(L._vs.cpu(), ref['vs'])
     flips, units, worst = _mask_flips(L, params, batch, T, B)
     errs.update(relu_mask_flips=flips, relu_units=units, worst_flipped_margin=worst)
-    _record(f'split_vs_fp32_T{T}_B{B}_A{A}', errs)
+    record('parity_fullsize.json', f'split_vs_fp32_T{T}_B{B}_A{A}', errs)
     assert errs['logits'] < 1e-5 and errs['vs'] < 1e-5, errs
     assert flips <= 2 + units * 2e-5 and worst < 1e-4, (flips, units, worst)
     tol = 2e-3 if (T, B) == (20, 32) else _grad_tol(flips)          # BASELINE size: the round-1 verdict's bound, ties included

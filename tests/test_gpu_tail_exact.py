@@ -17,14 +17,12 @@ the GPU itself read, at every dispatch edge of the V-trace kernels, the fused lo
 
 The worst err / bound of every check, its margin and its sensitivity go to $SRL_RESULTS_DIR/tail_exact.json when SRL_RESULTS_DIR is
 set (per case, and a summary per check)."""
-import json
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import impala_oracle as O
+from tests import exact as E
 from tests import tail_ref as R
 
 pytestmark = pytest.mark.gpu
@@ -35,74 +33,7 @@ KERNELS = {'scan': 'vtrace_iw_scan_kernel', 'seq4': 'vtrace_iw_seq_kernel<4>', '
            'column8': 'column_step_kernel<4,8>', 'column32': 'column_step_kernel<4,32>'}
 MAX_EXCLUDED = 1e-3
 
-
-# ------------------------------------------------------------------------------------------------ results
-def _record(name, obj):
-    d = os.environ.get('SRL_RESULTS_DIR')
-    if not d:
-        return
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, RESULTS)
-    cur = json.load(open(p)) if os.path.exists(p) else {}
-    cur[name] = obj
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
-
-
-@pytest.fixture(scope='module', autouse=True)
-def _summary():
-    """after the module: per check, the worst err / bound over every case, its margin, and the strongest sensitivity (its witness)"""
-    yield
-    d = os.environ.get('SRL_RESULTS_DIR')
-    p = os.path.join(d, RESULTS) if d else None
-    if not p or not os.path.exists(p):
-        return
-    cur = json.load(open(p))
-    table = {}
-    for case, res in cur.items():
-        if case == 'summary':
-            continue
-        for name, e in res.items():
-            t = table.setdefault(name, {})
-            for k, v in e.items():
-                if not isinstance(v, (int, float)):
-                    continue
-                worst = min if k == 'margin' else max
-                t[k] = v if k not in t else worst(t[k], v)
-    cur['summary'] = table
-    json.dump(cur, open(p, 'w'), indent=1, sort_keys=True)
-
-
-class Checker:
-    def __init__(self):
-        self.res, self.fails = {}, []
-
-    def bound(self, name, got, ref, S, c, sens=None):
-        q = R.ratio(got, ref, S, c)
-        e = {'err_over_bound': q, 'margin': 1.0 / q if q > 0 else float('inf')}
-        if sens is not None:
-            e['sensitivity'] = sens
-        self.res[name] = e
-        if not q <= 1.0:
-            self.fails.append(f'{name}: {q:.3f} x the bound')
-
-    def exact(self, name, got, want):
-        got, want = got.contiguous(), want.contiguous()
-        n = int((got.view(torch.int32) != want.view(torch.int32)).sum()) if got.shape == want.shape else -1
-        self.res[name] = {'bits_differ': n, 'n': want.numel()}
-        if n:
-            self.fails.append(f'{name}: {n} of {want.numel()} elements differ in their bits')
-
-    def count(self, name, **kv):
-        self.res[name] = kv
-
-    def witness(self, case, mistakes, sens):
-        for m in mistakes:
-            if not sens.get(m, 0.0) >= R.SENS:
-                self.fails.append(f'{m} ({R.MISTAKES[m]}) moves {case} by only {sens.get(m, 0.0):.1f} x the bound')
-
-    def done(self, case):
-        _record(case, self.res)
-        assert not self.fails, '\n'.join(self.fails)
+_summary = E.summary(RESULTS)
 
 
 def _ran(fn, kernel, tries=3):
@@ -159,9 +90,9 @@ def test_from_importance_weights_exact(name):
     x = R.iw_inputs(name)
     d = [_dev(a, offset) for a in x]
     out = _ran(lambda: ops.from_importance_weights(*d, cr, cp, variant=variant), kernel)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     sens = _vtrace_checks(Ck, *x, cr, cp, _host(out.vs), _host(out.pg_advantages))
-    Ck.witness(name, witnesses, sens)
+    Ck.require(name, sens, witnesses)
     if variant == 1 and T > 128:
         seq = ops.from_importance_weights(*d, cr, cp, variant=0)
         Ck.exact('vs_equals_variant0', out.vs, seq.vs)
@@ -182,7 +113,7 @@ def test_from_logits_exact(name):
     tr, br = R.rows(tl), R.rows(bl)
     talp, balp = R.gather(tr['lp'], a), R.gather(br['lp'], a)
     s_t, s_b = R.gather(tr['s_lp'], a), R.gather(br['s_lp'], a)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     nb = (a + 1) % A                                                          # the neighbouring action read by mistake
     sens = lambda pert, ref, S, c: R.sensitivity(pert, ref, S, c) if A > 1 else None
     Ck.bound('talp', _host(out.target_action_log_probs), talp, s_t, R.CHECK_C['logp'], sens(R.gather(tr['lp'], nb), talp, s_t, R.CHECK_C['logp']))
@@ -213,7 +144,7 @@ def _tail_checks(Ck, case, inputs, hp, kernel, out, witnesses):
     Ck.bound('vs', vs, *own['vs'], R.CHECK_C['vs'], per_check('vs'))
     for k in got:
         Ck.bound(k, got[k], *ref[k], R.CHECK_C[R.TAIL_CHECK_C[k]], per_check(k))
-    Ck.witness(case, witnesses, {m: max(s.values()) for m, s in sens.items()})
+    Ck.require(case, {m: max(s.values()) for m, s in sens.items()}, witnesses)
 
 
 def _tail_call(inputs, hp):
@@ -229,7 +160,7 @@ def _tail_call(inputs, hp):
 def test_impala_tail_exact(name):
     inputs, hp, kernel = R.tail_case(name)
     out = _ran(lambda: _tail_call(inputs, hp), kernel)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     _tail_checks(Ck, name, inputs, hp, kernel, out, R.TAIL_CASES[name][7])
     Ck.done(f'tail_{name}')
 
@@ -258,7 +189,7 @@ def test_learner_tail_exact(T, B, A):
         L.close()
     inputs = tuple(_host(t) for t in (batch['policy_logits'], logits, baseline, batch['action'], batch['reward'], batch['done']))
     alone = _tail_call(inputs, hp)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     for k in ('vs', 'pg_advantages', 'dlogits', 'dbaseline'):
         Ck.exact(f'{k}_equals_standalone', mine[k], alone[k])
     _tail_checks(Ck, f'learner {T}x{B}x{A}', inputs, hp, 'column' if kernel.startswith('column') else kernel, mine, ())
@@ -271,7 +202,7 @@ def test_learner_tail_exact(T, B, A):
 def test_policy_rows_exact(N, A):
     from scalerl_b200 import ops
     rng = np.random.RandomState(N + A)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     for regime in R.LOGIT_REGIMES:
         x = R.logit_rows(rng, (N, A), regime)
         act = rng.randint(0, A, size=N).astype(np.int64)
@@ -319,7 +250,7 @@ def test_reduce_sum_exact(n):
     from scalerl_b200 import ops
     x = (np.random.RandomState(n % 1000).randn(n) + 1).astype(np.float32)
     xd = _dev(x)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     for square, scale in ((False, 1.0), (True, 0.5), (False, -0.25)):
         got = ops.reduce_sum(xd, square=square, scale=scale)
         val, S = R.reduce_sum(x, square, scale)
@@ -347,7 +278,7 @@ def _sample(xd, ud):
 def test_sample_actions_exact(A):
     N = 100003
     rng = np.random.RandomState(A)
-    Ck = Checker()
+    Ck = E.Checker(RESULTS, R)
     for regime in R.LOGIT_REGIMES:
         x = R.logit_rows(rng, (N, A), regime)
         u = rng.rand(N).astype(np.float32)
