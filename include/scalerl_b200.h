@@ -590,6 +590,70 @@ int srl_replay_add_prioritized(srl_replay_t* R, srl_apex_actor_t* actor, const u
 int srl_frame_replay_add_prioritized(srl_frame_replay_t* R, srl_apex_actor_t* actor, const uint8_t* state, const int64_t* action,
                                      const float* reward, const uint8_t* next_state, const uint8_t* done, float priority_eps, void* stream);
 
+/* ---- R2D2 learner step: a recurrent Q network trained on stored-state sequences (Kapturowski et al. 2019) -----------------------
+ * The Q network is AtariNet(use_lstm=True)'s encoder and 2-layer LSTM core (srl_encoder_*, srl_lstm_core_*: the row [relu(fc(x)) (512),
+ * clamp(r_{t-1}, -1, 1), one_hot(a_{t-1}) (A)], H = 513 + A, the state multiplied by (1 - done_t) before step t) followed by a Q head on
+ * the core output: q = Linear(H, A), or with `dueling` value = Linear(H, 1), advantage = Linear(H, A), Q = V + Adv - mean_a Adv (Wang et
+ * al. 2016, eq. 9; the mean summed in action order).  bf16 encoder and LSTM operands (the LSTM core has no split mode).
+ * Parameters in state_dict order {conv1.weight, conv1.bias, ..., fc.bias, rnn_layer.weight_ih_l0, weight_hh_l0, bias_ih_l0, bias_hh_l0,
+ * *_l1, q.weight [A,H], q.bias [A]} (18 tensors), or with the dueling head {..., value.weight [1,H], value.bias [1], advantage.weight
+ * [A,H], advantage.bias [A]} (20); in memory in that order, each segment padded to 4 floats (16-byte aligned).  Params, grads, both
+ * Adam states and the target copy share the layout.  -> the buffer's floats, or -1 with srl_last_error set (A outside [1, 31],
+ * dueling outside {0, 1}). */
+int64_t srl_r2d2_param_layout(int A, int dueling, int64_t* offsets20, int64_t* counts20);
+typedef struct srl_r2d2_learner srl_r2d2_learner_t;
+typedef struct srl_r2d2_config {
+  int32_t B;                 /* sequences per step                                                                      */
+  int32_t A;                 /* actions, [1, 31]                                                                        */
+  int32_t burn_in;           /* rows run without gradient before the trained rows, >= 0 (R2D2 section 3: 40)           */
+  int32_t T;                 /* trained rows per sequence, >= 1 (80)                                                    */
+  int32_t n_step;            /* n of the n-step return, >= 1 (5); (burn_in + T + n_step) * B <= 65536                    */
+  float gamma;               /* discount per step, [0, 1] (0.997); the kernel forms gamma^k itself                      */
+  int32_t dueling;           /* 0: q = Linear(H, A); 1: the dueling head                                                */
+  int32_t value_rescaling;   /* 1: h(x) = sign(x)(sqrt(|x| + 1) - 1) + eps x on the targets (Pohlen et al. 2018); 0: identity */
+  float rescale_eps;         /* eps of h, finite and > 0 when value_rescaling (1e-3)                                    */
+  float priority_eta;        /* eta of the sequence priority, [0, 1] (0.9)                                              */
+  float priority_eps;        /* added to every priority, finite and >= 0                                                */
+  float max_grad_norm;       /* clip_grad_norm_ threshold, > 0; +inf: no clip                                           */
+  float learning_rate, adam_beta1, adam_beta2, adam_eps;   /* torch.optim.Adam (1e-4, 0.9, 0.999, 1e-3)                 */
+} srl_r2d2_config_t;
+/* params / grads / exp_avg / exp_avg_sq / target_params: caller-owned flat f32 device buffers of srl_r2d2_param_layout floats, 16-byte
+ * aligned and disjoint.  The context owns the encoder and LSTM blocks of the step and of the q-value forwards.  Synchronous. */
+int srl_r2d2_learner_create(const srl_r2d2_config_t* cfg, float* params, float* grads, float* exp_avg, float* exp_avg_sq,
+                            float* target_params, srl_r2d2_learner_t** out);
+int srl_r2d2_learner_destroy(srl_r2d2_learner_t* L);
+/* One learner step on B stored sequences of L = burn_in + T + n_step rows, time-major: frame u8 [L,B,4,84,84], last_action i64 [L,B],
+ * reward f32 [L,B], done u8/bool [L,B]; h0 / c0 f32 [2,B,H] the stored recurrent state before row 0; weights f32 [B] (NULL = 1); idxs
+ * i64 [B] with per (both NULL, or both set).  Row t holds s_t, the action a_{t-1} and reward r_t that led to it, and done_t (the step
+ * into row t ended an episode); the transition of row t is (s_t, a_t = last_action[t+1], reward[t+1], done[t+1]).
+ *   burn-in (section 3): rows [0, burn_in) through the online network from (h0, c0), no gradient; the trained rows [burn_in, burn_in + T)
+ *     continue from that state; the target network runs all L rows from (h0, c0); the n bootstrap rows get no gradient
+ *   a* = first argmax_a Q_online(s_{t+n});  m = the first k in 1..n with done[t+k] (or none)
+ *   y_t = h(sum_{k=1}^{min(n,m)} gamma^{k-1} reward[t+k] + [no m] gamma^n h^-1(Q_target(s_{t+n}, a*)))   (section 2, the n-step
+ *     double-Q target with value rescaling; evaluated in double, rounded once to fp32)
+ *   delta_t = Q_online(s_t, a_t) - y_t;  loss = (1 / (B T)) sum_b w_b sum_t delta_t^2
+ *   priority_b = eta max_t |delta_t| + (1 - eta) mean_t |delta_t| + priority_eps (section 2) -> the sampler's trees (last idx wins)
+ *   clip_grad_norm_(max_grad_norm) and a torch.optim.Adam step with the step count kept on the device.
+ * stats_out: f32 [3] device = {loss, gradient norm, clip coefficient} (may be NULL).  No host synchronisation; capturable. */
+int srl_r2d2_learner_step(srl_r2d2_learner_t* L, const uint8_t* frame, const int64_t* last_action, const float* reward, const uint8_t* done,
+                          const float* h0, const float* c0, const float* weights, const int64_t* idxs, srl_per_t* per, float* stats_out,
+                          void* stream);
+/* Q values of the online network over T1 rows of N columns from the state (h0, c0): frame u8 [T1,N,4,84,84], last_action i64 [T1,N],
+ * reward f32 [T1,N], done u8 [T1,N], h0 / c0 f32 [2,N,H] -> q_out f32 [T1,N,A], hT / cT f32 [2,N,H] the state after row T1 - 1 (may
+ * not overlap h0 / c0).  T1 = 1 is one acting step.  N in [1, min(L B, 2048)].  Runs on its own encoder context and blocks, so it may
+ * run on another stream than the step; calls of it on two streams at once share those blocks and must be ordered. */
+int srl_r2d2_learner_q_values(srl_r2d2_learner_t* L, const uint8_t* frame, const int64_t* last_action, const float* reward, const uint8_t* done,
+                              int T1, int N, const float* h0, const float* c0, float* q_out, float* hT, float* cT, void* stream);
+/* target_params = tau * params + (1 - tau) * target_params (srl_apex_learner_update_target's arithmetic); tau in [0, 1] */
+int srl_r2d2_learner_update_target(srl_r2d2_learner_t* L, float tau, void* stream);
+/* Adam's step count for a resumed run: writes the device counter; synchronises `stream` */
+int srl_r2d2_learner_set_step(srl_r2d2_learner_t* L, int64_t step, void* stream);
+/* borrow the step's buffers for tests: "core" f32 [L*B,H] (the last encoder forward's rows: the target's), "out_online" f32
+ * [(T+n)*B,H] (the LSTM output of rows burn_in..L-1), "out_target" f32 [L*B,H], "h_burn_in" / "c_burn_in" f32 [2,B,H] (burn_in > 0),
+ * "q_online" f32 [(T+n)*B,A], "q_target" f32 [T*B,A] (rows burn_in+n..L-1), "dq" f32 [T*B,A], "dout" / "dcore" f32 [(T+n)*B,H] (the
+ * head's and the LSTM core's input gradients), "q_taken", "y", "delta" f32 [T*B], "priorities" f64 [B], "loss" f32 [1], "step" i32 [1] */
+int srl_r2d2_learner_debug_buffer(srl_r2d2_learner_t* L, const char* name, void** ptr, int64_t* count);
+
 /* ---- trajectory ring -> time-major batch (the stacking step of ImpalaTrainer.get_batch, impala_atari.py:248-251) -----------
  * staging: B trajectory slots on the DEVICE, each one contiguous record of slot_bytes holding every key of create_buffers
  * (impala_atari.py:135-147) for T+1 steps; offsets6_host (HOST array) = byte offsets of {obs u8[T+1,4,84,84], reward f32[T+1],

@@ -119,6 +119,13 @@ _SIGS = {
     'srl_frame_replay_add_prioritized': [_P] * 7 + [_F, _P],
     'srl_frame_replay_sample': [_P, _P, _I] + [_P] * 9,
     'srl_frame_replay_gather': [_P, _P, _L] + [_P] * 6,
+    'srl_r2d2_learner_create': [C.c_void_p, _P, _P, _P, _P, _P, C.POINTER(_P)],
+    'srl_r2d2_learner_destroy': [_P],
+    'srl_r2d2_learner_step': [_P] * 12,
+    'srl_r2d2_learner_q_values': [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P],
+    'srl_r2d2_learner_update_target': [_P, _F, _P],
+    'srl_r2d2_learner_set_step': [_P, _L, _P],
+    'srl_r2d2_learner_debug_buffer': [_P, C.c_char_p, C.POINTER(_P), C.POINTER(_L)],
 }
 # libscalerl_b200_testhooks.so (include/scalerl_b200_testhooks.h): unit-test entry points, loaded by tests only
 _HOOK_SIGS = {
@@ -150,7 +157,7 @@ def hooks():
     return _hooks
 
 
-EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout', 'srl_apex_param_layout_ex', 'srl_apex_param_layout_cat', 'srl_apex_param_layout_noisy', 'srl_apex_param_layout_quantile', 'srl_apex_param_layout_dist_dueling', 'srl_replay_size', 'srl_replay_per', 'srl_frame_replay_size', 'srl_frame_replay_per', 'srl_frame_replay_frames_allocated', 'srl_frame_replay_retired'])
+EXPORTS = sorted(list(_SIGS) + ['srl_last_error', 'srl_param_layout', 'srl_param_layout_ex', 'srl_learner_workspace_bytes', 'srl_profile_slot_name', 'srl_lstm_last_error', 'srl_per_last_error', 'srl_per_size', 'srl_per_capacity', 'srl_per_invalid_updates', 'srl_learner_get_step', 'srl_apex_param_layout', 'srl_apex_param_layout_ex', 'srl_apex_param_layout_cat', 'srl_apex_param_layout_noisy', 'srl_apex_param_layout_quantile', 'srl_apex_param_layout_dist_dueling', 'srl_replay_size', 'srl_replay_per', 'srl_frame_replay_size', 'srl_frame_replay_per', 'srl_frame_replay_frames_allocated', 'srl_frame_replay_retired', 'srl_r2d2_param_layout'])
 
 
 def lib():
@@ -206,6 +213,8 @@ def lib():
         L.srl_apex_param_layout_quantile.argtypes = [_I, _I, _I, _I, _I, C.POINTER(_L), C.POINTER(_L)]
         L.srl_apex_param_layout_dist_dueling.restype = C.c_int64
         L.srl_apex_param_layout_dist_dueling.argtypes = [_I, _I, _I, _I, _I, _I, C.POINTER(_L), C.POINTER(_L)]
+        L.srl_r2d2_param_layout.restype = C.c_int64
+        L.srl_r2d2_param_layout.argtypes = [_I, _I, C.POINTER(_L), C.POINTER(_L)]
         L.srl_learner_workspace_bytes.restype = C.c_int64
         L.srl_learner_workspace_bytes.argtypes = [_P]
         _lib = L
@@ -261,6 +270,26 @@ def apex_actor_create(A, num_envs, precision, seed, params, head) -> C.c_void_p:
                                                    C.byref(h)),
           'srl_apex_actor_create_dist_dueling')
     return h
+
+
+class SrlR2d2Config(C.Structure):
+    """mirror of srl_r2d2_config_t"""
+    _fields_ = [('B', C.c_int32), ('A', C.c_int32), ('burn_in', C.c_int32), ('T', C.c_int32), ('n_step', C.c_int32), ('gamma', C.c_float),
+                ('dueling', C.c_int32), ('value_rescaling', C.c_int32), ('rescale_eps', C.c_float), ('priority_eta', C.c_float),
+                ('priority_eps', C.c_float), ('max_grad_norm', C.c_float), ('learning_rate', C.c_float), ('adam_beta1', C.c_float),
+                ('adam_beta2', C.c_float), ('adam_eps', C.c_float)]
+
+
+def r2d2_param_layout(A, dueling=False):
+    """(total floats, offsets, counts) of the R2D2 Q network's flat buffer in state_dict order (srl_r2d2_param_layout): 18 tensors, or
+    20 with the dueling head"""
+    off = (_L * 20)()
+    cnt = (_L * 20)()
+    total = lib().srl_r2d2_param_layout(int(A), 1 if dueling else 0, off, cnt)
+    if total < 0:
+        check(-1, 'srl_r2d2_param_layout')
+    n = 20 if dueling else 18
+    return int(total), [int(x) for x in off][:n], [int(x) for x in cnt][:n]
 
 
 def param_layout(A, use_lstm=False):

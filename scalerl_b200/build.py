@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OUT = os.path.join(HERE, 'libscalerl_b200.so')
 OUT_HOOKS = os.path.join(HERE, 'libscalerl_b200_testhooks.so')
-SOURCES = ['api.cu', 'encoder.cu', 'vtrace.cu', 'heads.cu', 'optim.cu', 'lstm.cu', 'per.cu', 'dqn.cu', 'dqn_cat.cu', 'dqn_qr.cu', 'replay.cu', 'frame_replay.cu', 'apex_actor.cu', 'noisy.cu', 'dueling_rows.cu']
+SOURCES = ['api.cu', 'encoder.cu', 'vtrace.cu', 'heads.cu', 'optim.cu', 'lstm.cu', 'per.cu', 'dqn.cu', 'dqn_cat.cu', 'dqn_qr.cu', 'replay.cu', 'frame_replay.cu', 'apex_actor.cu', 'noisy.cu', 'dueling_rows.cu', 'r2d2.cu']
 HOOK_SOURCES = ['testhooks.cu', 'test_shift.cu']
 HOOK_LINKS = ['optim.cu']          # product objects the hooks library links too (compiled once, for both libraries)
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
